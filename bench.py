@@ -81,7 +81,7 @@ def metric_name(name):
 def workload_config(name, batch, world):
     return {"workload": CONFIGS[name]["workload"], "dialogs_per_gpu": batch, "global_batch_dialogs": batch * world,
             "parallelism": "dp%d" % world,
-            "l2": "per-step working set (LSTM gates/activations, GBs) >> 126 MB L2; 4 rotating input batches"}
+            "l2": "per-step working set (LSTM gates/activations, GBs) >> 50 MB L2; 4 rotating input batches"}
 
 
 def load_synthetic():
@@ -96,13 +96,14 @@ def measured_peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
-        return {"bf16_sustained": d.get("bf16_tflops_sustained", 1449.3), "bf16_burst": d.get("bf16_tflops", 1693.7),
-                "hbm": d.get("hbm_gbs", 6579.6), "src": "measured"}
-    return {"bf16_sustained": 1400.0, "bf16_burst": 1590.0, "hbm": 6650.0, "src": "fallback"}
+        return {"bf16_sustained": d.get("bf16_tflops_sustained", 989.0), "bf16_burst": d.get("bf16_tflops", 989.0),
+                "hbm": d.get("hbm_gbs", 3350.0), "src": "MEASURED_PEAKS.json"}
+    # NVIDIA H100 SXM data sheet (dense BF16, HBM3, 700 W card): a ceiling, not a measured rate
+    return {"bf16_sustained": 989.0, "bf16_burst": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md).  The sampler runs from
+    """nvidia-smi clocks / throttle reasons DURING the timed region.  The sampler runs from
     before the warm-up; only samples whose nvidia-smi timestamp falls inside the marked window are kept."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -347,11 +348,13 @@ def run_ours(args, rank, local, world):
             self.i += 1
             return self.b[self.i % len(self.b)]
 
+    last = {}                                         # what the most recent step handed back to its caller
+
     def one_step(loader):
         if train:
-            model.trainIteration(loader)
+            last["loss"] = model.trainIteration(loader)
         else:
-            eng.retrieve(loader.getTrainBatch(p), use_gt=True)
+            last["ranks"] = eng.retrieve(loader.getTrainBatch(p), use_gt=True)
 
     def timed(loader, steps, profile):
         barrier(world)
@@ -385,6 +388,8 @@ def run_ours(args, rank, local, world):
             if rank == 0 and Bs == cfg["sweep"][0]:
                 sampler.mark_begin()
             ms, _, launches = timed(dl, args.steps, 0)
+            if args.dump_outputs and rank == 0:
+                dump_outputs(args.dump_outputs, {"ranks_b%d" % Bs: last["ranks"]})
             ms_h, wall_h, _ = timed(hl, args.steps, 0)
             ms = max_over_ranks(ms, world)
             ms_h = max_over_ranks(max(ms_h, wall_h), world)
@@ -429,6 +434,9 @@ def run_ours(args, rank, local, world):
     ms_dev, wall_dev, launches = timed(dev_loader, args.steps, 0 if args.ncu_range else 2)
     if args.ncu_range:
         eng.profiler_range(False)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"loss": np.array([last["loss"]]), "parameters": eng.get_parameters(),
+                                         "gradients": eng.get_gradients()})
     stats_shared = {k: eng.kernel_stats(k) for k in LSTM_STEP_KEYS}
     ms_e2e, wall_e2e, _ = timed(host_loader, args.steps, 0)
     # Roofline pass: in the timed region above the option-LSTM kernels share the GPU with the encoder's concurrent
@@ -482,8 +490,8 @@ def run_ours(args, rank, local, world):
 
     peaks = measured_peaks()
     f16 = args.math == "f16"
-    # kind::f16 runs at the bf16 rate the driver measured with cuBLAS; TF32 operands at half of it (no TF32 peak was
-    # measured by the driver; tools/measure_tf32_peak.py measures this repo's own 8192^3 TF32 kernel for comparison)
+    # f16 wgmma runs at the bf16 rate; TF32 operands at half of it (tools/measure_tf32_peak.py measures this repo's own
+    # 8192^3 TF32 kernel for comparison)
     peak = peaks["bf16_sustained"] if f16 else peaks["bf16_sustained"] / 2.0
     roofline = None
     n_l = sum(stats[k]["launches"] for k in LSTM_STEP_KEYS)
@@ -496,9 +504,9 @@ def run_ours(args, rank, local, world):
                    "TFLOP/s": stats[k]["flops"] / max(stats[k]["ms"] * 1e-3, 1e-12) / 1e12,
                    "algorithmic_GB/s": stats[k]["bytes"] / max(stats[k]["ms"] * 1e-3, 1e-12) / 1e9} for k in LSTM_STEP_KEYS}
         hbm_gbs = by / max(t_ms * 1e-3, 1e-12) / 1e9
-        kernel_desc = ("k_lstm16<fwd|bwd>: option-LSTM step, fp16 operands (recurrent gate GEMM on tcgen05 kind::f16, CTA pairs, "
-                       "fp32 TMEM accumulators + SeqLSTM pointwise epilogue)" if f16 else
-                       "k_tc_gemm<256,LSTM_FWD|LSTM_BWD,2>: option-LSTM step (recurrent gate GEMM on tcgen05 kind::tf32 + SeqLSTM "
+        kernel_desc = ("k_lstm16<fwd|bwd>: option-LSTM step, fp16 operands (recurrent gate GEMM on f16 wgmma, 128x128 tiles, "
+                       "fp32 accumulators + SeqLSTM pointwise epilogue)" if f16 else
+                       "k_tc_gemm<128,LSTM_FWD|LSTM_BWD>: option-LSTM step (recurrent gate GEMM on tf32 wgmma + SeqLSTM "
                        "pointwise epilogue)") + ", %d launches per training step" % (n_l // args.steps)
         # SURVEY.md §8(d) convention (algorithmic FLOP: the forward step is credited with the D = embedSize x-projection
         # 2*R*4H*(H+D) although it executes as a table gather) — reported NEXT TO the executed figure, never instead of it
@@ -508,7 +516,7 @@ def run_ours(args, rank, local, world):
         tensor = {"achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                   "flops_counted": "executed tensor-core FLOP only (2*R*4H*H per launch): the gathered x-projection and the K=0 first/"
                                    "last steps are not credited",
-                  "peak_source": "%s bf16_tflops_sustained%s" % (peaks["src"], "" if f16 else " / 2 (TF32 operands)"),
+                  "peak_source": "%s, BF16 dense rate%s" % (peaks["src"], "" if f16 else " / 2 (TF32 operands)"),
                   "executed_flop_per_launch": fl / max(n_l, 1),
                   "achieved_survey_convention": conv, "frac_survey_convention": conv / peak,
                   "achieved_in_overlapped_step": (sum(stats_shared[k]["flops"] for k in LSTM_STEP_KEYS) /
@@ -517,23 +525,16 @@ def run_ours(args, rank, local, world):
                "bytes_counted": "algorithmic HBM bytes per launch (DESIGN.md §9): forward fp16 gates out + fp32 c in/out + fp16 h in/out = "
                                 "10 KB per option row (the fp16 projection-table gather is L2-resident, not counted); backward fp16 gates "
                                 "in + fp16 da in/out + fp32 c_{t-1}, c_t in + fp32 dc in/out = 20 KB per row",
-               "peak_source": "%s hbm_gbs (MEASURED_PEAKS.json)" % peaks["src"], "algorithmic_bytes_per_launch": by / max(n_l, 1)}
-        # VD_MATH_F16: the class sits nearer the HBM roof than the tensor roof (ncu: backward step DRAM 61 % / tensor 31 %, forward
-        # 40 % / 34 %), so HBM is the binding roofline; the TF32 kernels are nearer their (assumed) tensor roof.  Both are always given.
+               "peak_source": "%s, HBM bandwidth" % peaks["src"], "algorithmic_bytes_per_launch": by / max(n_l, 1)}
+        # VD_MATH_F16: the class is bound by bytes (fp16 operands halve the tensor work per byte), so HBM is the binding roofline;
+        # the TF32 kernels are nearer their tensor roof.  Both are always given.
         head = hbm if f16 else tensor
         roofline = {"bound": "hbm" if f16 else "tensor", "kernel": kernel_desc,
                     "achieved": head["achieved"], "peak": head["peak"], "unit": head["unit"], "frac": head["frac"],
                     "launches": n_l, "avg_launch_ms": t_ms / max(n_l, 1), "share_of_step": t_ms / max(ms_iso, 1e-9),
                     "per_direction": per, "hbm": hbm, "tensor": tensor,
                     "measured_in": "a second pass of the same %d steps with the option stream serialised behind the encoder "
-                                   "(%.3f ms/step), CUDA events around every launch of this kernel class on its stream" % (args.steps, ms_iso / args.steps),
-                    "traffic": None}
-        tpath = os.path.join(ROOT, "profiles", "r02_traffic.json")   # dram bytes per launch from the committed ncu --set full capture
-        if os.path.exists(tpath):
-            t = json.load(open(tpath)).get(args.math)
-            if t:
-                roofline["traffic"] = t["dram_bytes_per_launch_avg"]
-                roofline["traffic_source"] = t["source"]
+                                   "(%.3f ms/step), CUDA events around every launch of this kernel class on its stream" % (args.steps, ms_iso / args.steps)}
     line = {"metric": metric_name(args.config), "value": value, "unit": "QA-rounds/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_dev / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None,
@@ -553,6 +554,23 @@ def run_ours(args, rank, local, world):
     if world == 1 and not args.no_cpu:
         line["cpu_baseline"] = cpu_baseline(args)
     print(json.dumps(line), flush=True)
+
+
+DUMP_SAMPLE = 2_000_000                               # elements kept of a larger output (with their indices)
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes what the timed path computed in its last step as <out_dir>/<name>.npy (float32 values, float64 indices).  An
+    output of more than DUMP_SAMPLE elements is replaced by a fixed, seeded sample of them plus `<name>_index`, so that two
+    builds run with the same arguments can be compared output for output within 64 MB."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a, dtype=np.float32).ravel()
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def cpu_baseline(args):
@@ -632,6 +650,9 @@ def main():
     ap.add_argument("--no-resident", action="store_true", help=argparse.SUPPRESS)      # accepted for old command lines
     ap.add_argument("--corpus-dialogs", type=int, default=256, help="dialogs in the synthetic resident corpus per rank")
     ap.add_argument("--ncu-range", action="store_true", help="bracket the timed steps with cudaProfilerStart/Stop")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="after the timed steps, write what the last one returned (loss, parameters, gradients; ranks for C5) "
+                         "as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * visdial_b200 — C ABI of the B200-native Visual Dialog encoder/decoder engine.
+ * visdial_b200 — C ABI of the H100-native Visual Dialog encoder/decoder engine.
  *
  * This is the drop-in boundary for the reference's per-batch hot path.  Every entry point cites
  * the reference interface it replaces (paths relative to /root/reference).  Host languages bind it
@@ -111,7 +111,7 @@ int vd_set_training(vd_engine* e, int32_t training);   /* wrapper:training()/:ev
 /* Dropout masks are a pure function philox4x32-10(seed; site, iteration, element index)
  * (DESIGN.md §5) so that the oracle can be given identical masks. */
 int vd_set_dropout_seed(vd_engine* e, uint64_t seed, uint64_t iteration);
-#define VD_MATH_TF32 0        /* dense contractions on tcgen05 tensor cores, TF32 operands, fp32 accumulate */
+#define VD_MATH_TF32 0        /* dense contractions on wgmma tensor cores, TF32 operands, fp32 accumulate */
 #define VD_MATH_FP32 1        /* same contractions on CUDA cores in fp32 (verification mode) */
 #define VD_MATH_F16 2         /* TF32 mode + the many-row option LSTM (disc.lua:4-20) with fp16 operands and fp16 saved state
                                  (h, gates, da, x-projection table), fp32 accumulation, fp32 cell state and gradients */
@@ -210,7 +210,7 @@ int vd_gemm_tn(vd_engine* e, int32_t M, int32_t N, int32_t K, const float* A, in
 int vd_gemm_atb(vd_engine* e, int32_t M, int32_t N, int64_t K, const float* A, int64_t lda, const float* B, int64_t ldb,
                 float* C, int64_t ldc);
 /* test hook of the VD_MATH_F16 weight-gradient primitive: A (K x M) and B (K x N) fp32 DEVICE buffers are rounded to
- * fp16, then C[m,n] += inv_scale * sum_k A[k,m] B[k,n] on tcgen05 kind::f16 (both operands MN-major). */
+ * fp16, then C[m,n] += inv_scale * sum_k A[k,m] B[k,n] on f16 wgmma (both operands MN-major). */
 int vd_gemm_atb16(vd_engine* e, int32_t M, int32_t N, int64_t K, const float* A, int64_t lda, const float* B, int64_t ldb,
                   float* C, int64_t ldc, float inv_scale);
 /* cudaProfilerStart / cudaProfilerStop (ncu --profile-from-start off) */

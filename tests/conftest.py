@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with `-m gpu` on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with `-m gpu` on a GPU machine)")
 
 
 @pytest.fixture(scope="session", autouse=True)
@@ -45,7 +45,7 @@ def pytest_collection_modifyitems(config, items):
         return
     if _cuda_device_count() > 0:
         return
-    skip = pytest.mark.skip(reason="no CUDA device (gpu-marked tests run with `-m gpu` on the B200 box)")
+    skip = pytest.mark.skip(reason="no CUDA device (gpu-marked tests run with `-m gpu` on an H100)")
     for it in items:
         if "gpu" in it.keywords:
             it.add_marker(skip)

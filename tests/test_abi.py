@@ -1,6 +1,6 @@
 """CPU-side checks of the drop-in boundary: the C-ABI library loads, exports every symbol the header
 declares, the host-only layout entry points work without a GPU, and the product fails loudly (no CPU
-fallback) when there is no B200."""
+fallback) when there is no H100."""
 import ctypes as C
 import os
 import re
@@ -113,7 +113,7 @@ def test_bad_arguments_return_error_codes():
 
 
 def test_fails_loudly_without_a_gpu():
-    """No CPU fallback: creating an engine on a box without a B200 is an error, not a silent CPU path."""
+    """No CPU fallback: creating an engine on a box without an H100 is an error, not a silent CPU path."""
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present")

@@ -1,4 +1,4 @@
-"""Tensor-core (tcgen05 / TF32) path against fp64 numpy and against the oracle.
+"""Tensor-core (wgmma / TF32) path against fp64 numpy and against the oracle.
 
 Stated tolerance for TF32 operands (10-bit mantissa, unit round-off 2^-11, fp32 accumulate): a K-term
 contraction of O(1) terms: the tensor core TRUNCATES fp32 operands to TF32 (relative error < 2^-10 per operand),
@@ -138,7 +138,7 @@ def _rel(a, b):
 @pytest.mark.parametrize("enc,dec", [("mn-att-ques-im-hist", "disc"), ("lf-ques", "gen"), ("hrea-ques-im-hist", "gen"),
                                      ("lf-ques-im-hist", "disc")])
 def test_tf32_graph_matches_oracle_mid_size(enc, dec):
-    """H=128 so that the fused tcgen05 LSTM kernels (H % 128 == 0) are the ones that run."""
+    """H=128 so that the fused wgmma LSTM kernels (H % 128 == 0) are the ones that run."""
     p = small_params(enc, dec, rnnHiddenSize=128, embedSize=64, vocabSize=200, numOptions=10, commonEmbeddingSize=64,
                      imgFeatureSize=64 if "att" in enc else 256, imgSpatialSize=4, imgEmbedSize=32)
     flat = init_parameters(p, seed=3)
@@ -208,11 +208,12 @@ def test_tf32_headline_shapes_and_rank_exactness():
 
 
 def test_tf32_cta_pair_kernels_match_oracle():
-    """B=4 dialogs -> 4000 option sequences: enough 128x256 tiles for the persistent cta_group::2 (CTA-pair) kernels
-    of the option LSTM to be the ones that run, forward and backward."""
+    """B=5 dialogs -> 5000 option sequences: enough 128-row tiles (forward 40 x 16, backward 40 x 4 = 160 >= 132 SMs) for
+    the SM-filling TF32 step kernels of the option LSTM (k_tc_gemm<128, LSTM_FWD / LSTM_BWD>) to be the ones that run,
+    forward and backward.  (The name is historical: these tiles used to run on CTA pairs.)"""
     p = full_params("mn-att-ques-im-hist", "disc")
     flat = init_parameters(p, seed=3)
-    nb = make_batch(p, 4, seed=9)
+    nb = make_batch(p, 5, seed=9)
     eng = Engine(p)
     eng.set_math_mode(VD_MATH_TF32)
     eng.set_parameters(flat)

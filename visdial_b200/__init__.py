@@ -1,4 +1,4 @@
-"""visdial_b200 — B200-native engine for the per-batch hot path of batra-mlp-lab/visdial.
+"""visdial_b200 — H100-native engine for the per-batch hot path of batra-mlp-lab/visdial.
 
 Host-side mirror (Python, because no Lua runtime exists in this image) of the reference's plugin
 surface: `encoders/<name>` + `decoders/<name>` modules loaded by name (model.lua:19-26), the `Model`

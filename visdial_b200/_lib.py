@@ -1,6 +1,6 @@
 """ctypes binding of include/visdial_b200.h — the same declarations the LuaJIT shim cdef's
 (lua/visdial_ffi.lua, INTEGRATION.md).  There is no CPU fallback: a missing library or a missing
-B200 is an error the caller sees."""
+H100 is an error the caller sees."""
 from __future__ import annotations
 
 import ctypes as C

@@ -377,7 +377,7 @@ int vd_flush_l2(vd_engine* h) {
   VD_TRY({
     Engine* e = ENG(h);
     if (!e->flush_buf) {
-      e->flush_n = (int64_t)(192u << 20) / 4;      // 192 MiB > 126 MB L2
+      e->flush_n = (int64_t)(192u << 20) / 4;      // 192 MiB > 50 MB L2
       VD_CUDA_CHECK(cudaMalloc((void**)&e->flush_buf, (size_t)e->flush_n * 4));
     }
     vd::fill_l2_flush(e->cx, e->flush_buf, e->flush_n);

@@ -1,4 +1,4 @@
-// Shared definitions for the visdial_b200 engine (sm_100a only).
+// Shared definitions for the visdial_b200 engine (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -99,7 +99,7 @@ struct LaunchCtx {
   cudaStream_t stream = nullptr;
   int64_t launches = 0;
   int profiling = 0;          // 0 off, 1 every class, 2 only the roofline class (big lstm_step / lstm_step_bwd launches)
-  int sm_count = 148;
+  int sm_count = 132;
   int sm_budget = 0;          // > 0: persistent / single-wave kernels size their grids to this many SMs (the rest stay free
                               // for a concurrent higher-priority stream); 0 = all of them
   int sms() const { return sm_budget > 0 ? sm_budget : sm_count; }

@@ -2,10 +2,9 @@
 // encoders/mn-att-ques-im-hist.lua:27-45, hrea-ques-im-hist.lua:36,76, lf-*.lua): ONE launch runs both stacked layers over
 // all T time steps, forward (k_enc_pair_fwd) or BPTT (k_enc_pair_bwd), instead of 3 launches per time step.
 //
-// Why (profiles/r01_ncu_full_encoder_small_steps.md, r02_launches_f16_v1.md): the per-step kernels are latency-bound — 360
-// launches, 8.3 ms of serialised device time per training step for < 1 % of the FLOPs, each launch re-streaming the 4 MB
+// Why: the per-step kernels are latency-bound — 3 launches per time step for < 1 % of the FLOPs, each re-streaming the 4 MB
 // recurrent weight through L2.  Here the weight is STATIONARY: every CTA keeps a 128 KB fp16 slice of it (32 hidden units)
-// in shared memory for the whole sequence, and per step only a (128-row x K) fp16 panel moves (TMA, 6-stage ring).  Three
+// in shared memory for the whole sequence, and per step only a (128-row x K) fp16 panel moves (TMA, 5-stage ring).  Three
 // CTA roles per 128-row block, H/32 CTAs each, so that NO role contracts more than one panel per step:
 //
 //   forward   L1  cell of layer 1:   gates = xproj1[t] (batched GEMM, up front) + h1_{t-1} Wh1^T      -> h1_t      K = H
@@ -18,16 +17,13 @@
 //   k_enc_pair_bwd<true>: CTA (gate, 128-unit slice) contracts K = H against N = 128 and the four gate CTAs of a slice sum their
 //   partials in a zeroed fp32 dh[t] with red.add before each runs the pointwise of 32 units — see the comment at the kernel.)
 //
-// (Measured with the phase trace below, round 2: with the layer-2 cell contracting [h1_t | h2_{t-1}] itself, and the layer-1
-// BPTT cell [da2_t | da1_{t+1}], the two-panel role set the step time: 21.9k clk forward, 45.6k clk BPTT, of which the
-// operand stream — 64 KB in flight per SM against ~2.5k clk of L2 latency — was 12k / 37k.)
-//
-// tcgen05 kind::f16, M = 128 rows, N = 4 gates x 32 (forward) / 32 (BPTT), fp32 accumulators in TMEM; the pointwise half
-// runs in the epilogue warps (thread = row, 256-bit global accesses) with the cell state / its gradient held in REGISTERS
-// across the sequence.  Time steps are chained through global-memory flags: a CTA publishes "step t of my slice is stored"
-// (fence + atomicAdd), the TMA producer (and, for the parked partials, the epilogue threads) of a consumer CTA spin on the
-// count of the row block (ld.acquire) — no cluster / grid barrier.  A stuck wait traps.  All CTAs must be co-resident
-// (3 H/32 x row-block groups <= SM count, one CTA per SM): enc_pair_shape_ok.
+// f16 wgmma, two consumer warpgroups of 64 rows each, N = 4 gates x 32 (forward) / 32 or 128 (BPTT), fp32 accumulators in
+// registers that leave through a 32-column shared-memory chunk; the pointwise half runs in the same warps (two threads per row,
+// 16 hidden units each) with the cell state / its gradient held in REGISTERS across the sequence.  Time steps are chained
+// through global-memory flags: a CTA publishes "step t of my slice is stored" (barrier + release atomic), the TMA producer (and,
+// for the parked partials, the epilogue threads) of a consumer CTA spin on the count of the row block (ld.acquire) — no cluster
+// / grid barrier.  A stuck wait traps.  All CTAs must be co-resident (3 H/32 x row-block groups <= SM count, one CTA per SM):
+// enc_pair_shape_ok.
 //
 // Numerics: fp16 operands (h, da, weights) with fp32 accumulation = the VD_MATH_F16 class (10-bit mantissa like TF32); cell
 // state, gate pre-activations, saved activations and all gradients fp32.
@@ -40,30 +36,20 @@
 namespace vd {
 namespace tc {
 
-constexpr int EP_THREADS = 192;          // warp 0 = TMA producer, warp 1 = MMA issuer, warps 2-5 = epilogue (thread = row)
-constexpr int EP_STAGES = 6;
+constexpr int EP_THREADS = 288;          // warps 0-7 = two consumer warpgroups (64 rows each), warp 8 = TMA producer
+constexpr int EP_STAGES = 5;
 constexpr int EP_STAGE_BYTES = 128 * 64 * 2;      // 128 rows x 64 halves
 constexpr int EP_W_BYTES_MAX = 131072;            // weight slice: fwd 128 x H, BPTT 32 x 4H halves = 256*H bytes (H <= 512)
-constexpr int EP_SMEM = EP_W_BYTES_MAX + EP_STAGES * EP_STAGE_BYTES + 1024 + 256;
+constexpr int EP_ACC_BYTES = 32 * ACC_LD * 4;     // one 32-column chunk of the accumulator on its way to the epilogue
+constexpr int EP_SMEM = EP_W_BYTES_MAX + EP_STAGES * EP_STAGE_BYTES + EP_ACC_BYTES + 1024 + 256;
 constexpr int EP_HS = 32;                         // hidden units per CTA slice
 static_assert(EP_SMEM <= 227 * 1024, "persistent encoder LSTM: shared memory budget");
 
-__host__ __device__ constexpr uint32_t ep_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void ep_umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
 __device__ __forceinline__ uint32_t ep_pack2(float a, float b) {
   uint32_t r;
   asm("{\n .reg .f16 lo, hi;\n cvt.rn.satfinite.f16.f32 lo, %1;\n cvt.rn.satfinite.f16.f32 hi, %2;\n mov.b32 %0, {lo, hi};\n}"
       : "=r"(r) : "f"(a), "f"(b));
   return r;
-}
-__device__ __forceinline__ uint4 ep_pack8(const float* v) {
-  return make_uint4(ep_pack2(v[0], v[1]), ep_pack2(v[2], v[3]), ep_pack2(v[4], v[5]), ep_pack2(v[6], v[7]));
 }
 // spin until *flag >= want (published with fence + atomicAdd by the producers of that step); traps instead of hanging
 __device__ __forceinline__ void wait_flag_generic(const int* flag, int want) {
@@ -80,49 +66,34 @@ __device__ __forceinline__ void wait_flag(const int* flag, int want) {
   wait_flag_generic(flag, want);
   asm volatile("fence.proxy.async;" ::: "memory");       // the TMA (async proxy) reads what generic-proxy stores published
 }
-// thread = row: each thread touches its own 32-byte piece of a row.  One 256-bit access per piece (sm_100: LDG/STG.256) — the
-// epilogues are bound by LSU wavefronts (one per distinct line per instruction), not by bytes
-__device__ __forceinline__ void ld8g(const float* p, float* d) {
-  asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(d[0]), "=f"(d[1]), "=f"(d[2]), "=f"(d[3]), "=f"(d[4]), "=f"(d[5]), "=f"(d[6]), "=f"(d[7]) : "l"(p) : "memory");
-}
-__device__ __forceinline__ void st8g(float* p, const float* v) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
-}
-
-// one 128-byte line of a row per call (4 consecutive 256-bit accesses of the same thread: the LSU merges them far better than the same
-// bytes issued as 32-byte pieces of four different lines — measured: 140 vs 370 clk per store instruction and warp)
-__device__ __forceinline__ void ld32g(const float* p, float* d) { ld8g(p, d); ld8g(p + 8, d + 8); ld8g(p + 16, d + 16); ld8g(p + 24, d + 24); }
-__device__ __forceinline__ void st32g(float* p, const float* v) { st8g(p, v); st8g(p + 8, v + 8); st8g(p + 16, v + 16); st8g(p + 24, v + 24); }
-__device__ __forceinline__ void st32h(__half* p, const float* v) {            // 32 halves = 64 bytes
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"l"(p), "r"(ep_pack2(v[0], v[1])), "r"(ep_pack2(v[2], v[3])), "r"(ep_pack2(v[4], v[5])), "r"(ep_pack2(v[6], v[7])),
-                 "r"(ep_pack2(v[8], v[9])), "r"(ep_pack2(v[10], v[11])), "r"(ep_pack2(v[12], v[13])), "r"(ep_pack2(v[14], v[15])) : "memory");
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"l"(p + 16), "r"(ep_pack2(v[16], v[17])), "r"(ep_pack2(v[18], v[19])), "r"(ep_pack2(v[20], v[21])), "r"(ep_pack2(v[22], v[23])),
-                 "r"(ep_pack2(v[24], v[25])), "r"(ep_pack2(v[26], v[27])), "r"(ep_pack2(v[28], v[29])), "r"(ep_pack2(v[30], v[31])) : "memory");
-}
-__device__ __forceinline__ void zero32(float* d) {
+// two threads per row, 16 hidden units each: every access of a thread is a whole 64-byte half line of its row (four 16-byte
+// accesses of the same thread, which the LSU merges far better than pieces of different lines)
+constexpr int EP_HW = 16;                         // hidden units per epilogue thread
+__device__ __forceinline__ void ld16g(const float* p, float* d) {
 #pragma unroll
-  for (int e = 0; e < 32; ++e) d[e] = 0.f;
+  for (int i = 0; i < 4; ++i) {
+    const float4 v = *reinterpret_cast<const float4*>(p + 4 * i);
+    d[4 * i] = v.x; d[4 * i + 1] = v.y; d[4 * i + 2] = v.z; d[4 * i + 3] = v.w;
+  }
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  tmem_ld8(taddr, v); tmem_ld8(taddr + 8, v + 8); tmem_ld8(taddr + 16, v + 16); tmem_ld8(taddr + 24, v + 24);
+__device__ __forceinline__ void st16g(float* p, const float* v) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) reinterpret_cast<float4*>(p)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-                 "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])) : "memory");
+__device__ __forceinline__ void st16h(__half* p, const float* v) {            // 16 halves = 32 bytes
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+    reinterpret_cast<uint4*>(p)[i] = make_uint4(ep_pack2(v[8 * i], v[8 * i + 1]), ep_pack2(v[8 * i + 2], v[8 * i + 3]),
+                                                ep_pack2(v[8 * i + 4], v[8 * i + 5]), ep_pack2(v[8 * i + 6], v[8 * i + 7]));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-  tmem_st8(taddr, v); tmem_st8(taddr + 8, v + 8); tmem_st8(taddr + 16, v + 16); tmem_st8(taddr + 24, v + 24);
+__device__ __forceinline__ void zero16(float* d) {
+#pragma unroll
+  for (int e = 0; e < EP_HW; ++e) d[e] = 0.f;
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// Optional phase trace (VD_ENC_TRACE=1, debugging only): per (CTA, step) stamps — clock64 at {0: flag seen, 1: panel issued, 2: accumulator
-// free, 3: last operand chunk landed + MMAs issued, 4: accumulator ready, 5: epilogue math + stores issued, 6: published} and globaltimer at
-// {7: published, 8: flag seen}.  A null pointer (the normal case) costs one predicated branch per stamp.
+// Optional phase trace (VD_ENC_TRACE=1, debugging only): per (CTA, step) stamps — clock64 at {0: flag seen, 1: panel issued, 2: MMAs
+// started, 3: MMAs issued, 4: accumulator ready, 5: epilogue math + stores issued, 6: published} and globaltimer at {7: published, 8: flag
+// seen}.  A null pointer (the normal case) costs one predicated branch per stamp.
 constexpr int EP_TRACE_SLOTS = 10;
 __device__ __forceinline__ void ep_stamp(unsigned long long* trace, int T, int t, int slot, bool wall = false) {
   if (trace) {
@@ -148,64 +119,85 @@ struct EncFwdParams {
 
 // carve-up shared by both kernels
 struct EpSmem {
-  uint8_t* wsm; uint8_t* stages; uint64_t* full; uint64_t* empty; uint64_t* tfull; uint64_t* tempty; uint64_t* wbar; uint64_t* seen; uint32_t* tmem_slot;
+  uint8_t* wsm; uint8_t* stages; float* acc; uint64_t* full; uint64_t* empty; uint64_t* wbar;
   __device__ explicit EpSmem(uint8_t* raw) {
     uint8_t* smem = (uint8_t*)(((uintptr_t)raw + 1023) & ~(uintptr_t)1023);
     wsm = smem;                                               // resident weight slice: k-block tiles of [N rows][128 B]
     stages = smem + EP_W_BYTES_MAX;
-    full = (uint64_t*)(stages + EP_STAGES * EP_STAGE_BYTES);
+    acc = (float*)(stages + EP_STAGES * EP_STAGE_BYTES);
+    full = (uint64_t*)(stages + EP_STAGES * EP_STAGE_BYTES + EP_ACC_BYTES);
     empty = full + EP_STAGES;
-    tfull = empty + EP_STAGES;
-    tempty = tfull + 1;
-    wbar = tempty + 1;
-    seen = wbar + 1;                                          // producer -> epilogue: "the flag of the next step has been seen"
-    tmem_slot = (uint32_t*)(seen + 1);
+    wbar = empty + EP_STAGES;
   }
   __device__ void init_barriers() {
-    for (int s = 0; s < EP_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tfull, 1); mbar_init(tempty, 4); mbar_init(wbar, 1); mbar_init(seen, 1);
+    for (int s = 0; s < EP_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    mbar_init(wbar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
 };
 
-// MMA issuer of one step: KB k-blocks of the streamed panel against the resident slice, accumulator <- (not accumulate) on the first
-// k-block order of a CTA: rotated by `koff`, so that the CTAs streaming the same panel at the same moment (the H/32 slices of a role, and the
-// projection role beside the cell that shares its panel) ask L2 for different lines instead of queueing on the same ones
+// k-block order of a CTA: rotated by `koff`, so that the CTAs streaming the same panel at the same moment (the H/32 slices of a role, and
+// the projection role beside the cell that shares its panel) ask L2 for different lines instead of queueing on the same ones
 __device__ __forceinline__ int ep_koff(int role, int slice, int nS, int KB) {
   const int stride = KB >= 2 * nS ? KB / (2 * nS) : 1;
   return ((2 * slice + (role == EP_PROJ ? 1 : 0)) * stride) % KB;
 }
-__device__ __forceinline__ void ep_mma_step(const EpSmem& sm, uint32_t tmem_base, uint32_t idesc, int KB, int koff, int n_rows, int lane, int& s,
-                                            uint32_t& ph, unsigned long long* trace, int T, int t) {
-  uint32_t first = 1;
+template <int N> __device__ __forceinline__ void ep_wgmma(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (N == 128) wgmma_f16_n128(d, a, b, acc);
+  else { static_assert(N == 32, "accumulator width"); wgmma_f16_n32(d, a, b, acc); }
+}
+// contraction of one step by a consumer warpgroup: KB k-blocks of the streamed panel (its 64 rows) against the resident slice
+template <int N>
+__device__ __forceinline__ void ep_mma_step(const EpSmem& sm, float (&d)[N / 2], int wg, int KB, int koff, int& s, uint32_t& ph,
+                                            unsigned long long* trace, int T, int t) {
+  if (threadIdx.x == 0) ep_stamp(trace, T, t, 2);
+  int prev = -1;
   for (int kb = 0; kb < KB; ++kb) {
     mbar_wait(&sm.full[s], ph);
-    tc_fence_after();
-    if (lane == 0) {
-      int kr = kb + koff; if (kr >= KB) kr -= KB;
-      const uint32_t sa = smem_u32(sm.stages + s * EP_STAGE_BYTES);
-      const uint32_t sb = smem_u32(sm.wsm + kr * n_rows * 128);
-      const uint64_t adesc = make_desc(sa, 16, 1024), bdesc = make_desc(sb, 16, 1024);
+    int kr = kb + koff; if (kr >= KB) kr -= KB;
+    const uint32_t sa = smem_u32(sm.stages + s * EP_STAGE_BYTES) + wg * 64 * 128;
+    const uint32_t sb = smem_u32(sm.wsm + kr * N * 128);
+    const uint64_t adesc = make_desc(sa, 16, 1024), bdesc = make_desc(sb, 16, 1024);
+    wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        ep_umma_f16(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, first ? 0u : 1u);
-        first = 0;
-      }
-      umma_commit(&sm.empty[s]);
-      if (kb == KB - 1) { umma_commit(sm.tfull); ep_stamp(trace, T, t, 3); }
-    }
-    __syncwarp();
-    first = 0;
+    for (int k = 0; k < 4; ++k) ep_wgmma<N>(d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&sm.empty[prev]);
+    prev = s;
     if (++s == EP_STAGES) { s = 0; ph ^= 1; }
   }
+  wgmma_wait<0>();
+  wgmma_hold(d);
+  if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&sm.empty[prev]);
+  if (threadIdx.x == 0) { ep_stamp(trace, T, t, 3); ep_stamp(trace, T, t, 4); }
+}
+// accumulator columns [32 C, 32 C + 32) of this warpgroup's 64 rows -> the shared chunk (rows 64 wg ..); the warps of the warpgroup
+// then read their half row from it.  C is a compile-time constant at every call.
+template <int NR>
+__device__ __forceinline__ void ep_chunk(float* acc, const float (&d)[NR], int wg, int C) {
+  bar_named(2 + wg, 128);                          // the previous chunk has been read
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int r = wg * 64 + 16 * w + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * C + jj;
+    float* p = acc + (c + 8 * jj) * ACC_LD + r;
+    p[0] = d[4 * j]; p[ACC_LD] = d[4 * j + 1]; p[8] = d[4 * j + 2]; p[ACC_LD + 8] = d[4 * j + 3];
+  }
+  bar_named(2 + wg, 128);
+}
+__device__ __forceinline__ void ep_ld16(const float* arow, float* v) {
+#pragma unroll
+  for (int e = 0; e < EP_HW; ++e) v[e] = arow[e * ACC_LD];
 }
 
-// publish step t of this slice: barrier of the epilogue warps, then ONE gpu-scope release (cumulative over what the barrier made
+// publish step t of this slice: barrier of the consumer warps, then ONE gpu-scope release (cumulative over what the barrier made
 // visible to the signalling thread) that counts the slice in — the grid-sync idiom of cooperative groups
 __device__ __forceinline__ void ep_publish(int* flag, unsigned long long* trace, int T, int t) {
-  if (threadIdx.x == 64) ep_stamp(trace, T, t, 5);
-  asm volatile("bar.sync 1, 128;" ::: "memory");
-  if (threadIdx.x == 64) {
+  if (threadIdx.x == 0) ep_stamp(trace, T, t, 5);
+  bar_named(1, 256);
+  if (threadIdx.x == 0) {
     asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(flag) : "memory");
     ep_stamp(trace, T, t, 6); ep_stamp(trace, T, t, 7, true);
   }
@@ -229,13 +221,9 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
   int* flagL2 = p.flags + 2 * (size_t)p.RB * T;
 
   if (threadIdx.x == 0) sm.init_barriers();
-  if (warp == 1) tmem_alloc(sm.tmem_slot, 256);        // [0,128) accumulator, [128,256) staging of the activated gates (cell roles)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *sm.tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       // ---- weights, once: tile kb = 4 gate boxes of HS rows x 64 halves.  W1 = Wh1 [4H, H]; W2 = [Wx2 | Wh2] [4H, 2H]
       const CUtensorMap* tw = role == EP_CELL1 ? &tmW1 : &tmW2;
@@ -255,7 +243,6 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
             tm = role == EP_CELL1 ? &tmH1 : &tmH2; ts = t - 1;
           }
           ep_stamp(p.trace, T, t, 8, true); ep_stamp(p.trace, T, t, 0);
-          if (role != EP_PROJ) mbar_arrive(sm.seen);
           for (int kb = 0; kb < KB; ++kb) {
             int kr = kb + koff; if (kr >= KB) kr -= KB;
             mbar_wait(&sm.empty[s], ph ^ 1);
@@ -267,142 +254,112 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ---- MMA issuer: same (row block, step, k-block) order as the producer
-    const uint32_t idesc = ep_idesc_f16(128, N);
+  } else if (warp < 8) {
+    // ---- consumers: warpgroup wg contracts rows [64 wg, 64 wg + 64) of the block; its first two warps run the epilogue, thread = row
+    const int wg = warp >> 2;
+    const int hh = (warp >> 1) & 1;                          // which 16 of the slice's 32 hidden units
+    const int rloc = wg * 64 + (warp & 1) * 32 + lane;
+    const float* arow = sm.acc + hh * EP_HW * ACC_LD + rloc;
+    const int u0 = slice * HS + hh * EP_HW;
     mbar_wait(sm.wbar, 0);
-    tc_fence_after();
-    int s = 0; uint32_t ph = 0; uint32_t nuse = 0;
-    for (int rb = group; rb < p.RB; rb += p.groups) {
-      for (int t = 0; t < T; ++t) {
-        if (role != EP_PROJ && t == 0) continue;
-        mbar_wait(sm.tempty, (nuse & 1) ^ 1);                // the epilogue has drained the accumulator of the previous step
-        tc_fence_after();
-        ++nuse;
-        if (lane == 0) ep_stamp(p.trace, T, t, 2);
-        ep_mma_step(sm, tmem_base, idesc, KB, koff, N, lane, s, ph, p.trace, T, t);
-      }
-    }
-  } else {
-    // ---- epilogue: thread = row of the 128-row block
-    const int q = warp & 3;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    const int j0 = slice * HS;
-    uint32_t nuse = 0, nseen = 0;
+    int s = 0; uint32_t ph = 0;
     if (role == EP_PROJ) {
       // gates2[t] <- h1_t Wx2^T + b2 for the 4 x 32 gate columns of this slice (the layer-2 cell of the same slice adds its recurrent half)
       for (int rb = group; rb < p.RB; rb += p.groups) {
-        const int64_t row = (int64_t)rb * 128 + q * 32 + lane;
+        const int64_t row = (int64_t)rb * 128 + rloc;
         const bool row_ok = row < p.R;
         for (int t = 0; t < T; ++t) {
           const int64_t tr = (int64_t)t * p.R + row;
-          mbar_wait(sm.tfull, nuse & 1); tc_fence_after(); ++nuse;
-          if (threadIdx.x == 64) ep_stamp(p.trace, T, t, 4);
+          float d[N / 2];
+          ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
 #pragma unroll
           for (int g = 0; g < 4; ++g) {                        // one gate = one 128-byte line of the row per pass
-            float a[HS], bb[HS];
-            tmem_ld32(taddr + g * HS, a);
-            ld32g(p.bias2 + g * H + j0, bb);
-            tmem_ld_wait();
+            ep_chunk(sm.acc, d, wg, g);
+            if (row_ok) {
+              float a[EP_HW], bb[EP_HW];
+              ep_ld16(arow, a);
+              ld16g(p.bias2 + g * H + u0, bb);
 #pragma unroll
-            for (int e = 0; e < HS; ++e) a[e] += bb[e];
-            if (row_ok) st32g(p.gates2 + tr * 4 * H + g * H + j0, a);
+              for (int e = 0; e < EP_HW; ++e) a[e] += bb[e];
+              st16g(p.gates2 + tr * 4 * H + g * H + u0, a);
+            }
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(sm.tempty);
           ep_publish(flagX + (size_t)rb * T + t, p.trace, T, t);
         }
       }
     } else {
       // LSTM cell, state c in registers across the sequence.  One gate at a time over all 32 units of the slice (order i, g, f, o), so
-      // that every global access of a thread is a whole 128-byte line; the activated gates wait in TMEM (staging columns) until h_t is
-      // out and published — only the 64 bytes of h16 per row are stored ahead of the flag, the 768 bytes of saved state after it,
-      // while the consumers are already streaming the panel
+      // that every global access of a thread is a whole 128-byte line; the activated gates overwrite the x rows in place
       const bool l1 = role == EP_CELL1;
       float* gates = l1 ? p.gates1 : p.gates2;
       float* cst = l1 ? p.c1 : p.c2;
       float* hst = l1 ? p.h1 : p.h2;
       __half* h16 = l1 ? p.h1_16 : p.h2_16;
       int* flag = l1 ? flagL1 : flagL2;
-      const uint32_t tstage = taddr + 128;
       for (int rb = group; rb < p.RB; rb += p.groups) {
-        const int64_t row = (int64_t)rb * 128 + q * 32 + lane;
+        const int64_t row = (int64_t)rb * 128 + rloc;
         const bool row_ok = row < p.R;
-        float c[HS];
-        zero32(c);
+        float c[EP_HW];
+        zero16(c);
         for (int t = 0; t < T; ++t) {
           const bool has_acc = t > 0;
           const int64_t tr = (int64_t)t * p.R + row;
           const float keep = (row_ok && p.mask && p.mask[tr] == 0) ? 0.f : 1.f;
           // additive term of the pre-activation: the x-half (+ bias) rows — layer 1: batched GEMM before the kernel; layer 2: parked in
-          // gates2[t] by the projection CTAs of this step (acquire their count first).  Gate i's line is requested before the accumulator
-          // is awaited, every other gate's line one pass ahead of its use.
-          if (!l1) wait_flag_generic(flagX + (size_t)rb * T + t, p.nS);
-          float* xrow = gates + tr * 4 * H + j0;
-          float x[HS], a[HS], ig[HS];
-          // the four x lines go to the TMEM staging columns while the contraction of this step is still running: the passes below then
-          // read both summands from TMEM (~100 clk) instead of stalling on L2 (~1.5k clk) once per gate
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            if (row_ok) ld32g(xrow + g * H, x); else zero32(x);
-            tmem_st32(tstage + g * HS, x);
-          }
-          tmem_st_wait();
+          // gates2[t] by the projection CTAs of this step (acquire their count first)
+          if (!l1 && row_ok) wait_flag_generic(flagX + (size_t)rb * T + t, p.nS);
+          float* xrow = gates + tr * 4 * H + u0;
           if (l1 && row_ok && t + 1 < T) {                     // next step's x-projection rows: pull them into L2 now
 #pragma unroll
             for (int g = 0; g < 4; ++g) asm volatile("prefetch.global.L2 [%0];" ::"l"(xrow + (int64_t)p.R * 4 * H + g * H) : "memory");
           }
-          if (has_acc) { mbar_wait(sm.tfull, nuse & 1); tc_fence_after(); ++nuse; }
-          if (threadIdx.x == 64) ep_stamp(p.trace, T, t, 4);
+          float d[N / 2];
+          if (has_acc) ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
+          float x[EP_HW], a[EP_HW], ig[EP_HW];
           // ---- i
-          if (has_acc) tmem_ld32(taddr + 0 * HS, a); else zero32(a);
-          tmem_ld32(tstage + 0 * HS, x); tmem_ld_wait();
+          if (has_acc) ep_chunk(sm.acc, d, wg, 0);
+          if (row_ok) {
+            if (has_acc) ep_ld16(arow, a); else zero16(a);
+            ld16g(xrow + 0 * H, x);
 #pragma unroll
-          for (int e = 0; e < HS; ++e) { a[e] = fsigmoid(a[e] + x[e]) * keep; ig[e] = a[e]; }
-          tmem_st32(tstage + 0 * HS, a);
+            for (int e = 0; e < EP_HW; ++e) { a[e] = fsigmoid(a[e] + x[e]) * keep; ig[e] = a[e]; }
+            st16g(xrow + 0 * H, a);
+          }
           // ---- g
-          if (has_acc) tmem_ld32(taddr + 3 * HS, a); else zero32(a);
-          tmem_ld32(tstage + 3 * HS, x); tmem_ld_wait();
+          if (has_acc) ep_chunk(sm.acc, d, wg, 3);
+          if (row_ok) {
+            if (has_acc) ep_ld16(arow, a); else zero16(a);
+            ld16g(xrow + 3 * H, x);
 #pragma unroll
-          for (int e = 0; e < HS; ++e) { a[e] = ftanh(a[e] + x[e]) * keep; ig[e] *= a[e]; }
-          tmem_st32(tstage + 3 * HS, a);
+            for (int e = 0; e < EP_HW; ++e) { a[e] = ftanh(a[e] + x[e]) * keep; ig[e] *= a[e]; }
+            st16g(xrow + 3 * H, a);
+          }
           // ---- f  (maskzero: keep = 0 resets the state of an all-zero input row)
-          if (has_acc) tmem_ld32(taddr + 1 * HS, a); else zero32(a);
-          tmem_ld32(tstage + 1 * HS, x); tmem_ld_wait();
+          if (has_acc) ep_chunk(sm.acc, d, wg, 1);
+          if (row_ok) {
+            if (has_acc) ep_ld16(arow, a); else zero16(a);
+            ld16g(xrow + 1 * H, x);
 #pragma unroll
-          for (int e = 0; e < HS; ++e) { a[e] = fsigmoid(a[e] + x[e]) * keep; c[e] = (a[e] * c[e] + ig[e]) * keep; }
-          tmem_st32(tstage + 1 * HS, a);
+            for (int e = 0; e < EP_HW; ++e) { a[e] = fsigmoid(a[e] + x[e]) * keep; c[e] = (a[e] * c[e] + ig[e]) * keep; }
+            st16g(xrow + 1 * H, a);
+          }
           // ---- o, h
-          if (has_acc) tmem_ld32(taddr + 2 * HS, a); else zero32(a);
-          tmem_ld32(tstage + 2 * HS, x); tmem_ld_wait();
-          if (has_acc) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(sm.tempty);             // the accumulator is drained: the next step's MMAs may start
-          }
+          if (has_acc) ep_chunk(sm.acc, d, wg, 2);
+          if (row_ok) {
+            if (has_acc) ep_ld16(arow, a); else zero16(a);
+            ld16g(xrow + 2 * H, x);
 #pragma unroll
-          for (int e = 0; e < HS; ++e) { a[e] = fsigmoid(a[e] + x[e]) * keep; ig[e] = a[e] * ftanh(c[e]) * keep; }     // ig <- h_t
-          tmem_st32(tstage + 2 * HS, a);
-          if (row_ok) st32h(h16 + tr * H + j0, ig);             // what the next step's TMA reads: the only store ahead of the flag
+            for (int e = 0; e < EP_HW; ++e) { a[e] = fsigmoid(a[e] + x[e]) * keep; ig[e] = a[e] * ftanh(c[e]) * keep; }     // ig <- h_t
+            st16g(xrow + 2 * H, a);
+            st16h(h16 + tr * H + u0, ig);                      // what the next step's TMA reads
+          }
           ep_publish(flag + (size_t)rb * T + t, p.trace, T, t);
-          // ---- after the flag: saved state for the backward pass (activated gates from the staging columns, c_t, h_t) — held back until
-          // this CTA's producer has seen the next step's flag, so that its polling loads do not queue behind these 768 bytes per row
-          if (t + 1 < T) { mbar_wait(sm.seen, nseen & 1); ++nseen; }
-          tmem_st_wait();
-          if (row_ok) { st32g(cst + tr * H + j0, c); st32g(hst + tr * H + j0, ig); }
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            tmem_ld32(tstage + g * HS, a); tmem_ld_wait();
-            if (row_ok) st32g(xrow + g * H, a);
-          }
+          // after the flag: saved state for the backward pass
+          if (row_ok) { st16g(cst + tr * H + u0, c); st16g(hst + tr * H + u0, ig); }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 256); }
 }
 
 
@@ -423,9 +380,9 @@ struct EncBwdParams {
 };
 
 // GS = gate split (H % 128 == 0): a CTA contracts ONE gate's quarter of the da panel (K = H) against a 128-unit slice of the weight
-// (same 128 KB): 32 tcgen05.mma of N = 128 per step instead of 128 of N = 32 — the step is bound by the instruction count
-// (profiles/r02_enc_trace.md) — and a quarter of the panel bytes.  The four gate CTAs of a unit slice add their partials into dh (red.add),
-// count themselves in, and each then runs the pointwise for 32 of the slice's 128 units once the count is complete.
+// (same 128 KB): N = 128 per instruction instead of N = 32 and a quarter of the panel bytes.  The four gate CTAs of a unit slice add
+// their partials into dh (red.add), count themselves in, and each then runs the pointwise for 32 of the slice's 128 units once the
+// count is complete.
 template <bool GS>
 __global__ void __launch_bounds__(EP_THREADS, 1)
 k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__ CUtensorMap tmA2,
@@ -451,13 +408,9 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
   int* cntB = cntT + (size_t)p.RB * T * nU;
 
   if (threadIdx.x == 0) sm.init_barriers();
-  if (warp == 1) tmem_alloc(sm.tmem_slot, GS ? 512 : 256);   // [0,N) accumulator, then seven 32-column staging slots (cell roles)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *sm.tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       // W2 = Wh2 as [H, 4H]; W1 = [Wx2 | Wh1] as [H, 8H]
       const CUtensorMap* tw = role == EP_CELL1 ? &tmW2 : &tmW1;
@@ -476,7 +429,6 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
             tm = role == EP_CELL1 ? &tmA2 : &tmA1; ts = t + 1;
           }
           ep_stamp(p.trace, T, t, 8, true); ep_stamp(p.trace, T, t, 0);
-          if (role != EP_PROJ) mbar_arrive(sm.seen);
           for (int kb = 0; kb < KB; ++kb) {
             int kr = kb + koff; if (kr >= KB) kr -= KB;
             mbar_wait(&sm.empty[s], ph ^ 1);
@@ -488,82 +440,54 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = ep_idesc_f16(128, N);
+  } else if (warp < 8) {
+    const int wg = warp >> 2;
+    const int hh = (warp >> 1) & 1;                          // which 16 of the slice's 32 hidden units
+    const int rloc = wg * 64 + (warp & 1) * 32 + lane;
+    const float* arow = sm.acc + hh * EP_HW * ACC_LD + rloc;
+    const int u0 = j0 + hh * EP_HW;
     mbar_wait(sm.wbar, 0);
-    tc_fence_after();
-    int s = 0; uint32_t ph = 0; uint32_t nuse = 0;
-    for (int rb = group; rb < p.RB; rb += p.groups) {
-      for (int t = T - 1; t >= 0; --t) {
-        if (role != EP_PROJ && t == T - 1) continue;
-        mbar_wait(sm.tempty, (nuse & 1) ^ 1);
-        tc_fence_after();
-        ++nuse;
-        if (lane == 0) ep_stamp(p.trace, T, t, 2);
-        ep_mma_step(sm, tmem_base, idesc, KB, koff, N, lane, s, ph, p.trace, T, t);
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t nuse = 0, nseen = 0;
+    int s = 0; uint32_t ph = 0;
     // GS: add this CTA's (128 rows x 128 units) partial product into dh[t] and count it in for the unit slice
-    auto add_partial = [&](float* dhbuf, int* cnt, int rb, int t, int64_t tr, bool row_ok) {
+    auto add_partial = [&](const float (&d)[N / 2], float* dhbuf, int* cnt, int rb, int t, int64_t tr, bool row_ok) {
 #pragma unroll
-      for (int sb = 0; sb < 4; ++sb) {
-        float a[32];
-        tmem_ld32(taddr + sb * 32, a); tmem_ld_wait();
+      for (int sb = 0; sb < N / 32; ++sb) {
+        ep_chunk(sm.acc, d, wg, sb);
         if (row_ok) {
-          float* dst = dhbuf + tr * H + us * 128 + sb * 32;
+          float a[EP_HW];
+          ep_ld16(arow, a);
+          float* dst = dhbuf + tr * H + us * 128 + sb * 32 + hh * EP_HW;
 #pragma unroll
-          for (int e = 0; e < 32; e += 4) red_add_v4(dst + e, a[e], a[e + 1], a[e + 2], a[e + 3]);
+          for (int e = 0; e < EP_HW; e += 4) red_add_v4(dst + e, a[e], a[e + 1], a[e + 2], a[e + 3]);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sm.tempty);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (threadIdx.x == 64) asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(cnt + ((size_t)rb * T + t) * nU + us) : "memory");
+      bar_named(1, 256);
+      if (threadIdx.x == 0) asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(cnt + ((size_t)rb * T + t) * nU + us) : "memory");
     };
-    if (role == EP_PROJ && GS) {
-      // partial of dh1_t = da2_t Wx2 (this gate's quarter, this unit slice), summed into dh1[t]
+    if (role == EP_PROJ) {
+      // GS: partial of dh1_t = da2_t Wx2 (this gate's quarter, this unit slice), summed into dh1[t];  otherwise the partial of
+      // dh1_t = da2_t Wx2, parked in the first H columns of da1[t] (the B cell of the same slice reads it, then overwrites)
       for (int rb = group; rb < p.RB; rb += p.groups) {
-        const int64_t row = (int64_t)rb * 128 + q * 32 + lane;
-        const bool row_ok = row < p.R;
-        for (int t = T - 1; t >= 0; --t) {
-          mbar_wait(sm.tfull, nuse & 1); tc_fence_after(); ++nuse;
-          if (threadIdx.x == 64) ep_stamp(p.trace, T, t, 4);
-          if (threadIdx.x == 64) ep_stamp(p.trace, T, t, 5);
-          add_partial(p.dh1, cntB, rb, t, (int64_t)t * p.R + row, row_ok);
-          if (threadIdx.x == 64) { ep_stamp(p.trace, T, t, 6); ep_stamp(p.trace, T, t, 7, true); }
-        }
-      }
-    } else if (role == EP_PROJ) {
-      // partial of dh1_t = da2_t Wx2, parked in the first H columns of da1[t] (the B cell of the same slice reads it, then overwrites)
-      for (int rb = group; rb < p.RB; rb += p.groups) {
-        const int64_t row = (int64_t)rb * 128 + q * 32 + lane;
+        const int64_t row = (int64_t)rb * 128 + rloc;
         const bool row_ok = row < p.R;
         for (int t = T - 1; t >= 0; --t) {
           const int64_t tr = (int64_t)t * p.R + row;
-          mbar_wait(sm.tfull, nuse & 1); tc_fence_after(); ++nuse;
-          if (threadIdx.x == 64) ep_stamp(p.trace, T, t, 4);
-#pragma unroll
-          for (int sub = 0; sub < HS / 8; ++sub) {
-            float a[8];
-            tmem_ld8(taddr + sub * 8, a);
-            tmem_ld_wait();
-            if (row_ok) st8g(p.da1 + tr * 4 * H + j0 + sub * 8, a);
+          float d[N / 2];
+          ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
+          if constexpr (GS) {
+            if (threadIdx.x == 0) ep_stamp(p.trace, T, t, 5);
+            add_partial(d, p.dh1, cntB, rb, t, tr, row_ok);
+            if (threadIdx.x == 0) { ep_stamp(p.trace, T, t, 6); ep_stamp(p.trace, T, t, 7, true); }
+          } else {
+            ep_chunk(sm.acc, d, wg, 0);
+            if (row_ok) { float a[EP_HW]; ep_ld16(arow, a); st16g(p.da1 + tr * 4 * H + u0, a); }
+            ep_publish(flagX + (size_t)rb * T + t, p.trace, T, t);
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(sm.tempty);
-          ep_publish(flagX + (size_t)rb * T + t, p.trace, T, t);
         }
       }
     } else {
       // SeqLSTM backward pointwise, dc in registers across the sequence; whole 128-byte lines per thread and access (three passes: o, then
-      // i and g, then f), the fp16 da_t (the operand of the steps that follow) stored ahead of the flag, the fp32 da_t (read after the
-      // kernel by the weight / input gradients) parked in TMEM and stored after it
+      // i and g, then f), da_t stored as fp16 (the operand of the steps that follow) and fp32 (read after the kernel)
       const bool top = role == EP_CELL1;
       const float* gates = top ? p.gates2 : p.gates1;
       const float* cst = top ? p.c2 : p.c1;
@@ -572,111 +496,79 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
       const float* dh_last = top ? p.dh_last2 : p.dh_last1;
       const float* dc_last = top ? p.dc_last2 : p.dc_last1;
       int* flag = top ? flagT : flagB;
-      const uint32_t tstage = taddr + N;
       float* dhbuf = top ? p.dh2 : p.dh1;
       int* cnt = top ? cntT : cntB;
       for (int rb = group; rb < p.RB; rb += p.groups) {
-        const int64_t row = (int64_t)rb * 128 + q * 32 + lane;
+        const int64_t row = (int64_t)rb * 128 + rloc;
         const bool row_ok = row < p.R;
-        float dc[HS];
-        zero32(dc);
+        float dc[EP_HW];
+        zero16(dc);
         for (int t = T - 1; t >= 0; --t) {
           const bool has_acc = t < T - 1;
           const int64_t tr = (int64_t)t * p.R + row;
           const float keep = (row_ok && p.mask && p.mask[tr] == 0) ? 0.f : 1.f;
-          const float* grow = gates + tr * 4 * H + j0;
-          float* darow = da + tr * 4 * H + j0;
-          __half* da16row = da16 + tr * 4 * H + j0;
-          float va[HS], vb[HS], dh[HS];
-          // everything the pointwise reads besides the contraction (saved gates, c_t, c_{t-1}, the parked partial) goes to the TMEM staging
-          // columns while the contraction of this step is still running; da_t overwrites the gate columns in place
-          // staging map: S0 = o -> da_o, S1 = c_t, S2 = i -> da_i, S3 = g -> da_g, S4 = f -> da_f, S5 = c_{t-1}, S6 = partial
-          if (!GS && !top) wait_flag_generic(flagX + (size_t)rb * T + t, p.nS);     // the parked partial of this step is in place
-          {
-            const float* src[7] = {grow + 2 * H, cst + tr * H + j0, grow, grow + 3 * H, grow + 1 * H,
-                                   t > 0 ? cst + (tr - p.R) * H + j0 : nullptr, (top || GS) ? nullptr : darow};
-#pragma unroll
-            for (int k = 0; k < 7; ++k) {
-              if (k == 6 && (top || GS)) continue;
-              if (row_ok && src[k]) ld32g(src[k], va); else zero32(va);
-              tmem_st32(tstage + k * HS, va);
-            }
-          }
-          tmem_st_wait();
-          if (has_acc) { mbar_wait(sm.tfull, nuse & 1); tc_fence_after(); ++nuse; }
-          if (threadIdx.x == 64) ep_stamp(p.trace, T, t, 4);
+          const float* grow = gates + tr * 4 * H + u0;
+          float* darow = da + tr * 4 * H + u0;
+          __half* da16row = da16 + tr * 4 * H + u0;
+          float va[EP_HW], vb[EP_HW], dh[EP_HW];
+          float d[N / 2];
+          if (has_acc) ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
           if constexpr (GS) {
             // my partial into dh[t]; then the complete sum of my 32 units once every contributor of the unit slice has counted in:
             // layer 2: its 4 gate CTAs; layer 1: 4 projection CTAs (every step) + its own 4 gate CTAs (all steps but the last)
-            if (has_acc) add_partial(dhbuf, cnt, rb, t, tr, row_ok);
+            if (has_acc) add_partial(d, dhbuf, cnt, rb, t, tr, row_ok);
             const int want = top ? 4 : (has_acc ? 8 : 4);
-            if (top && !has_acc) zero32(dh);
+            if (!row_ok || (top && !has_acc)) zero16(dh);
             else {
               wait_flag_generic(cnt + ((size_t)rb * T + t) * nU + us, want);
-              if (row_ok) ld32g(dhbuf + tr * H + j0, dh); else zero32(dh);
+              ld16g(dhbuf + tr * H + u0, dh);
             }
-            tmem_ld32(tstage + 0 * HS, va); tmem_ld32(tstage + 1 * HS, vb); tmem_ld_wait();
           } else {
-            if (has_acc) tmem_ld32(taddr, dh); else zero32(dh);
-            tmem_ld32(tstage + 0 * HS, va); tmem_ld32(tstage + 1 * HS, vb); tmem_ld_wait();
-            if (has_acc) {
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(sm.tempty);
+            if (has_acc) ep_chunk(sm.acc, d, wg, 0);
+            if (has_acc && row_ok) ep_ld16(arow, dh); else zero16(dh);
+            if (!top && row_ok) {                              // the parked partial of this step
+              wait_flag_generic(flagX + (size_t)rb * T + t, p.nS);
+              ld16g(darow, va);
+#pragma unroll
+              for (int e = 0; e < EP_HW; ++e) dh[e] += va[e];
             }
-            if (!top) { float pp[HS]; tmem_ld32(tstage + 6 * HS, pp); tmem_ld_wait();
-#pragma unroll
-              for (int e = 0; e < HS; ++e) dh[e] += pp[e]; }
           }
-          if (t == T - 1 && row_ok) {
-            if (dh_last) { float pp[HS]; ld32g(dh_last + row * H + j0, pp);
+          if (row_ok) {
+            if (t == T - 1) {
+              if (dh_last) { ld16g(dh_last + row * H + u0, va);
 #pragma unroll
-              for (int e = 0; e < HS; ++e) dh[e] += pp[e]; }
-            if (dc_last) ld32g(dc_last + row * H + j0, dc);
+                for (int e = 0; e < EP_HW; ++e) dh[e] += va[e]; }
+              if (dc_last) ld16g(dc_last + row * H + u0, dc);
+            }
+            // ---- o:  da_o = dh tanh(c) o (1-o);  d = dc + dh o (1 - tanh(c)^2)
+            ld16g(grow + 2 * H, va); ld16g(cst + tr * H + u0, vb);
+#pragma unroll
+            for (int e = 0; e < EP_HW; ++e) {
+              const float tcv = ftanh(vb[e]), go = va[e], dhe = dh[e] * keep;
+              dc[e] = (dc[e] + dhe * go * (1.f - tcv * tcv)) * keep;           // dc <- d
+              dh[e] = dhe * tcv * go * (1.f - go);
+            }
+            st16h(da16row + 2 * H, dh); st16g(darow + 2 * H, dh);
+            // ---- i, g:  da_i = d g i (1-i);  da_g = d i (1-g^2)
+            ld16g(grow, va); ld16g(grow + 3 * H, vb);
+#pragma unroll
+            for (int e = 0; e < EP_HW; ++e) dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]);
+            st16h(da16row, dh); st16g(darow, dh);
+#pragma unroll
+            for (int e = 0; e < EP_HW; ++e) dh[e] = dc[e] * va[e] * (1.f - vb[e] * vb[e]);
+            st16h(da16row + 3 * H, dh); st16g(darow + 3 * H, dh);
+            // ---- f:  da_f = d c_{t-1} f (1-f);  dc_{t-1} = d f
+            ld16g(grow + 1 * H, va);
+            if (t > 0) ld16g(cst + (tr - p.R) * H + u0, vb); else zero16(vb);
+#pragma unroll
+            for (int e = 0; e < EP_HW; ++e) { dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]); dc[e] *= va[e]; }
+            st16h(da16row + 1 * H, dh); st16g(darow + 1 * H, dh);
           }
-          // ---- o:  da_o = dh tanh(c) o (1-o);  d = dc + dh o (1 - tanh(c)^2)
-#pragma unroll
-          for (int e = 0; e < HS; ++e) {
-            const float tcv = ftanh(vb[e]), go = va[e], dhe = dh[e] * keep;
-            dc[e] = (dc[e] + dhe * go * (1.f - tcv * tcv)) * keep;           // dc <- d
-            dh[e] = dhe * tcv * go * (1.f - go);
-          }
-          tmem_st32(tstage + 0 * HS, dh);
-          if (row_ok) st32h(da16row + 2 * H, dh);
-          // ---- i, g:  da_i = d g i (1-i);  da_g = d i (1-g^2)
-          tmem_ld32(tstage + 2 * HS, va); tmem_ld32(tstage + 3 * HS, vb); tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < HS; ++e) dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]);
-          tmem_st32(tstage + 2 * HS, dh);
-          if (row_ok) st32h(da16row, dh);
-#pragma unroll
-          for (int e = 0; e < HS; ++e) dh[e] = dc[e] * va[e] * (1.f - vb[e] * vb[e]);
-          tmem_st32(tstage + 3 * HS, dh);
-          if (row_ok) st32h(da16row + 3 * H, dh);
-          // ---- f:  da_f = d c_{t-1} f (1-f);  dc_{t-1} = d f
-          tmem_ld32(tstage + 4 * HS, va); tmem_ld32(tstage + 5 * HS, vb); tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < HS; ++e) { dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]); dc[e] *= va[e]; }
-          tmem_st32(tstage + 4 * HS, dh);
-          if (row_ok) st32h(da16row + 1 * H, dh);
           ep_publish(flag + (size_t)rb * T + t, p.trace, T, t);
-          // ---- after the flag: fp32 da_t from the staging columns, once this CTA's producer has seen the next step's flag
-          if (t > 0) { mbar_wait(sm.seen, nseen & 1); ++nseen; }
-          tmem_st_wait();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const int sg = k == 0 ? 0 : k + 1;                               // staging slot S0, S2, S3, S4
-            const int gate = k == 0 ? 2 : (k == 1 ? 0 : (k == 2 ? 3 : 1));   // = gate o, i, g, f
-            tmem_ld32(tstage + sg * HS, dh); tmem_ld_wait();
-            if (row_ok) st32g(darow + gate * H, dh);
-          }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, GS ? 512 : 256); }
 }
 
 // ------------------------------------------------------------------------------------------------ host

@@ -155,7 +155,7 @@ Engine::Engine(const vd_params* p) {
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cudaDeviceProp prop;
   VD_CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg.gpuid));
-  VD_REQUIRE(prop.major == 10, VD_E_CUDA, "visdial_b200 is built for sm_100a (B200) only");
+  VD_REQUIRE(prop.major == 9 && prop.minor == 0, VD_E_CUDA, "visdial_b200 is built for sm_90a (H100) only");
   cx.sm_count = prop.multiProcessorCount;
   // the encoder's chains of small dependent kernels get the highest priority, the option LSTM's SM-filling launches
   // the lowest: a freed SM goes to the latency-bound chain first
@@ -362,7 +362,7 @@ void Engine::lstm_forward_begin(LstmRun& r, bool save) {
   // Tensor-core path: the x-projection of an embedding-gathered input becomes a (V+1, 4H) projection table
   // computed once per forward (E Wx^T: the 300-wide half of every step's contraction collapses into a
   // gather in the step epilogue); a dense input keeps the batched x-projection.  Each step is then ONE fused
-  // kernel: recurrent tcgen05 GEMM + SeqLSTM pointwise epilogue.
+  // kernel: recurrent wgmma GEMM + SeqLSTM pointwise epilogue.
   r.tc = tcmode() && H % 64 == 0;
   r.ptable = nullptr;
   // VD_MATH_F16: a many-row LSTM over embedding-gathered tokens (the option LSTM) keeps h, the activated gates, da and
@@ -633,7 +633,7 @@ void Engine::lstm_backward_step(LstmRun& r, int t) {
   }
   LaunchCtx::Scope sc(&cx, (last && r.bw_tc) ? "lstm_step_bwd_last" : (R >= 4096 ? "lstm_step_bwd" : "lstm_step_bwd_small"), last ? 0.0 : 2.0 * R * G * H, 4.0 * R * (2.0 * G + 5.0 * H));
   if (r.bw_tc) {
-    // one fused kernel per step: dh_rec = da_{t+1} Wh on tcgen05, backward pointwise in the epilogue
+    // one fused kernel per step: dh_rec = da_{t+1} Wh on wgmma, backward pointwise in the epilogue
     if (last) {         // no recurrent gradient yet: pointwise only (dh_last rides in the recurrent slot)
       lstm_pointwise_bwd(cx, r.gates + (int64_t)t * R * G, cp, r.c + (int64_t)t * R * H, r.bw_dh_last, ext, nullptr, r.dc_carry, mk,
                          da_t, R, H);

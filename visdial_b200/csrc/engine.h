@@ -67,7 +67,7 @@ struct LstmRun {
   bool saved = false;
   float* demb_out = nullptr;         // projected-space embedding gradient goes here (overwritten) instead of dW(wordEmbed) +=
   // forward run state (lstm_forward_begin / _step)
-  bool tc = false;                   // fused tcgen05 step kernels
+  bool tc = false;                   // fused wgmma step kernels
   bool step_xproj = false;           // dense input projected per step (layer-2 of a pipelined pair) instead of batched
   bool xproj_external = false;       // ... and that per-step projection is issued by the caller (on its own stream)
   const float* ptable = nullptr;     // (V+1, 4H) projection table for embedding-gathered inputs
@@ -110,7 +110,7 @@ struct Engine {
   int training = 1;
   uint64_t drop_seed = 1234, drop_iter = 0;
   int math_mode = VD_MATH_TF32;
-  bool tcmode() const { return math_mode != VD_MATH_FP32; }   // TF32 and F16 both run the dense contractions on tcgen05
+  bool tcmode() const { return math_mode != VD_MATH_FP32; }   // TF32 and F16 both run the dense contractions on wgmma
   Arena arena;
   GrowBuf stage[9];
   // The image features are 80 % of a host batch (12.8 MB of pool5 at B = 32) and are not needed until the attention stage:

@@ -1,5 +1,5 @@
 // fp32 CUDA-core GEMMs: the VD_MATH_FP32 verification path, and the fallback for contraction
-// shapes the tcgen05 kernels do not take (tiny M / N).  Same contract as the tensor-core kernels
+// shapes the wgmma kernels do not take (tiny M / N).  Same contract as the tensor-core kernels
 // in gemm_tc.cu.
 //
 //   gemm_tn : C[m,n] = act(beta*C[m,n] + bias[n] + sum_k A[row(m),k] * B[n,k])

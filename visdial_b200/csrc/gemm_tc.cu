@@ -1,8 +1,8 @@
-// Dense contractions on the 5th-gen tensor cores: tcgen05.mma kind::tf32 (fp32 operands in shared memory,
-// TF32 multiply, fp32 accumulate in TMEM), operands staged by TMA (128B-swizzled tiles), one persistent CTA
-// per SM, warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM allocator), warps 2-9 =
-// epilogue (TMEM -> registers -> fused pointwise -> global).  Double-buffered TMEM accumulators let the
-// epilogue of tile i overlap the main loop of tile i+1.
+// Dense contractions on the Hopper tensor cores: wgmma kind tf32 (fp32 operands in shared memory, TF32 multiply,
+// fp32 accumulate in registers), operands staged by TMA (128B-swizzled tiles) through an mbarrier ring, one
+// persistent CTA per SM, warp-specialised: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, each
+// contracting a 64-row half of the 128-row tile; the accumulators then go through shared memory so that the fused
+// pointwise epilogue runs "thread = row" (consumer warp w: rows 32 (w % 4) .., column half w / 4).
 //
 //   MODE_GENERIC : C = act(beta*C + bias + A B^T)                          (nn.Linear and friends)
 //   MODE_LSTM_FWD: gates = A_h Wh^T (+ x-projection) -> SeqLSTM pointwise   (one launch per time step)
@@ -16,11 +16,11 @@
 namespace vd {
 namespace tc {
 
-constexpr int BM = 128;          // rows per tile (UMMA M)
+constexpr int BM = 128;          // rows per tile (two 64-row wgmma slabs)
 constexpr int BK = 32;           // fp32 elements per k-block = one 128-byte swizzle row
-constexpr int UMMA_K = 8;        // tf32: 32 bytes per instruction
-constexpr int EPI_WARPS = 8;     // 2 warps per TMEM lane quarter, each takes half of the tile's columns
-// threads per CTA = 64 (TMA producer warp + MMA issuer warp) + 32 * epilogue warps (template parameter EW)
+constexpr int MMA_K = 8;         // tf32: 32 bytes per instruction
+constexpr int EPI_WARPS = 8;     // the consumer warps: 2 per 32-row quarter, each takes half of the tile's columns
+constexpr int GEMM_THREADS = 128 + 32 * EPI_WARPS;
 
 enum { MODE_GENERIC = 0, MODE_LSTM_FWD = 1, MODE_LSTM_BWD = 2, MODE_LSE = 3, MODE_DLOGIT = 4 };
 // MODE_LSE    : vocabulary projection whose (rows, V) logits never leave the chip: per row and column slice only the running
@@ -63,34 +63,31 @@ __device__ __forceinline__ void st8_cs(float* p, const float* v) {
   __stcs(reinterpret_cast<float4*>(p) + 1, make_float4(v[4], v[5], v[6], v[7]));
 }
 
-// Epilogue staging (CTA-pair LSTM kernels): per epilogue warp, ARR arrays of [32 rows][16 floats].  The 16-byte
-// chunks of a row are XOR-swizzled by (row>>1)&3 so that both access patterns are bank-conflict free: "thread =
-// row" (the TMEM side) and "4 lanes = one row's 64 bytes" (the global side, coalesced 64-byte runs instead of one
-// 16-byte piece of 32 different lines per instruction, which is what saturated L1TEX before).
+// Epilogue staging of the generic / d-logit modes: per consumer warp one array of [32 rows][16 floats].  The 16-byte
+// chunks of a row are XOR-swizzled by (row>>1)&3 so that both access patterns are bank-conflict free: "thread = row" and
+// "4 lanes = one row's 64 bytes" (coalesced 64-byte runs on the global side).  C leaves by TMA tensor stores.
 constexpr int STG_ARR_BYTES = 32 * 16 * 4;
-template <int BN, int MODE, int CG, int EW = EPI_WARPS> struct StageCfg {
-  static constexpr bool ON = MODE == MODE_GENERIC || MODE == MODE_DLOGIT || (CG == 2 && (BN == 256 || (BN == 128 && MODE == MODE_LSTM_BWD)));
-  static constexpr int ARR = !ON ? 0 : ((MODE == MODE_GENERIC || MODE == MODE_DLOGIT) ? 1 : MODE == MODE_LSTM_FWD ? 6 : 7);
-  static constexpr int BYTES = EW * ARR * STG_ARR_BYTES;
+template <int MODE> struct StageCfg {
+  static constexpr bool ON = MODE == MODE_GENERIC || MODE == MODE_DLOGIT;
+  static constexpr int ARR = ON ? 1 : 0;
+  static constexpr int BYTES = EPI_WARPS * ARR * STG_ARR_BYTES;
 };
-template <int BN, int CG = 1, int STG_BYTES = 0, int MAXST = 16> struct SmemLayout {
-  static constexpr int A_BYTES = BM * BK * 4;        // 16 KB (this CTA's 128 rows)
-  static constexpr int B_BYTES = (BN / CG) * BK * 4; // a CTA pair splits the B tile
+template <int BN, int STG_BYTES = 0> struct SmemLayout {
+  static constexpr int A_BYTES = BM * BK * 4;        // 16 KB
+  static constexpr int B_BYTES = BN * BK * 4;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int WANT = (B_BYTES == 32768) ? 4 : (B_BYTES == 16384) ? 6 : (B_BYTES == 8192) ? 8 : 10;   // small tiles are latency-bound: deeper
-  static constexpr int FIT = (232448 - 1024 - 256 - STG_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES0 = WANT < FIT ? WANT : FIT;
-  static constexpr int STAGES = STAGES0 < MAXST ? STAGES0 : MAXST;   // MAXST = 4: the half-size CTAs that share an SM
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
+  static constexpr int ACC_BYTES = BN * ACC_LD * 4;  // the accumulator tile on its way to the epilogue
+  static constexpr int WANT = (B_BYTES == 16384) ? 6 : (B_BYTES == 8192) ? 8 : 10;   // small tiles are latency-bound: deeper
+  static constexpr int FIT = (232448 - 1024 - 256 - STG_BYTES - ACC_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = WANT < FIT ? WANT : FIT;
+  static constexpr int TOTAL = STAGES * STAGE_BYTES + STG_BYTES + ACC_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 __device__ __forceinline__ float4* stg_at(float* stg, int arr, int row, int q) {
   return reinterpret_cast<float4*>(stg + (arr * 32 + row) * 16 + ((q ^ ((row >> 1) & 3)) << 2));
 }
-// global -> staging: `mine` = this lane's row base (16 floats) or nullptr (zeros); coalesced 4 lanes per row.
-// cp.async (LDGSTS): no register staging, so every array of a group is in flight at once and the global latency is
-// paid once per group instead of once per array; the caller ends the group with stg_load_wait().
+// global -> staging: `mine` = this lane's row base (16 floats) or nullptr (zeros); coalesced 4 lanes per row, cp.async;
+// the caller ends the group with stg_load_wait().
 __device__ __forceinline__ void stg_load(float* stg, int arr, const float* mine, int lane) {
 #pragma unroll
   for (int ps = 0; ps < 4; ++ps) {
@@ -101,24 +98,10 @@ __device__ __forceinline__ void stg_load(float* stg, int arr, const float* mine,
     else *dst = make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
-// staging -> global through the TMA (one bulk tensor store per array instead of 4 passes of shuffles + LDS + STG per
-// lane): the staging arrays are laid out exactly like a SWIZZLE_64B box of 32 rows x 16 floats.
-struct EpiMaps { CUtensorMap g4, c, h; };      // [R,4H] gates / da;  [R,H] c_out / dc_carry;  [R,H] h_out
+struct EpiMaps { CUtensorMap g4; };      // C as 64B-swizzled boxes of 32 rows x 16 floats
 __device__ __forceinline__ void stg_load_wait() {
   asm volatile("cp.async.wait_all;" ::: "memory");
   __syncwarp();
-}
-template <bool STREAM>
-__device__ __forceinline__ void stg_store(float* stg, int arr, float* mine, int lane) {
-#pragma unroll
-  for (int ps = 0; ps < 4; ++ps) {
-    const int row = ps * 8 + (lane >> 2), q = lane & 3;
-    float* dst = const_cast<float*>(shfl_ptr(mine, row));
-    if (dst) {
-      const float4 v = *stg_at(stg, arr, row, q);
-      if (STREAM) __stcs(reinterpret_cast<float4*>(dst) + q, v); else reinterpret_cast<float4*>(dst)[q] = v;
-    }
-  }
 }
 __device__ __forceinline__ void stg_get8(float* stg, int arr, int row, int sub, float* d) {
   const float4 a = *stg_at(stg, arr, row, sub * 2), b = *stg_at(stg, arr, row, sub * 2 + 1);
@@ -129,144 +112,101 @@ __device__ __forceinline__ void stg_put8(float* stg, int arr, int row, int sub, 
   *stg_at(stg, arr, row, sub * 2 + 1) = make_float4(v[4], v[5], v[6], v[7]);
 }
 
+template <int BN> __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (BN == 128) wgmma_tf32_n128(d, a, b, acc);
+  else if constexpr (BN == 64) wgmma_tf32_n64(d, a, b, acc);
+  else { static_assert(BN == 32, "tile width"); wgmma_tf32_n32(d, a, b, acc); }
+}
+
 // ------------------------------------------------------------------------------------------------
-// EW = epilogue warps.  8 (320 threads, one CTA per SM) for the SM-filling kernels; 4 (192 threads, 4 pipeline stages,
-// TWO CTAs per SM) for the few-row encoder kernels: those are latency-bound, so a CTA that owns a whole SM mostly
-// waits — and, run beside the option stream, what they cost is SM time, not FLOPs.
-template <int BN, int MODE, int CG, int EW = EPI_WARPS>
-__global__ void __launch_bounds__(64 + 32 * EW, EW == 4 ? 2 : 1)
+template <int BN, int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
           const __grid_constant__ EpiMaps em, const Params p) {
-  using SC = StageCfg<BN, MODE, CG, EW>;
-  using L = SmemLayout<BN, CG, SC::BYTES, (EW == 4 ? 4 : 16)>;
-  constexpr int NH = EW / 4;                         // epilogue warps per TMEM lane quarter = column slices per tile
+  using SC = StageCfg<MODE>;
+  using L = SmemLayout<BN, SC::BYTES>;
+  constexpr int NH = EPI_WARPS / 4;                  // consumer warps per 32-row quarter = column slices per tile
   constexpr int STAGES = L::STAGES;
-  constexpr int TM = BM * CG;                        // rows per tile: 128, or 256 for a CTA pair
-  const uint32_t rank = CG == 2 ? cluster_ctarank() : 0;
-  const bool leader = rank == 0;
-  const int cta = CG == 2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;       // tile-loop index of this CTA (pair)
-  const int ncta = CG == 2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   float* stg_all = (float*)(smem + STAGES * L::STAGE_BYTES);
-  uint64_t* full = (uint64_t*)(smem + STAGES * L::STAGE_BYTES + SC::BYTES);
+  float* acc = (float*)(smem + STAGES * L::STAGE_BYTES + SC::BYTES);
+  uint64_t* full = (uint64_t*)(smem + STAGES * L::STAGE_BYTES + SC::BYTES + L::ACC_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_m = (p.M + TM - 1) / TM;
+  const int num_m = (p.M + BM - 1) / BM;
   const int num_n = (p.N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_kb = (p.K + BK - 1) / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], EW * CG); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (CG == 2) cluster_sync_all();                  // peer barriers exist before anyone signals them
-  if (warp == 1) { if (CG == 2) tmem_alloc_cg2(tmem_slot, L::TMEM_COLS); else tmem_alloc(tmem_slot, L::TMEM_COLS); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer (every CTA stages its own rows of A and its share of B) =====
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
+      // ===== TMA producer =====
       int s = 0; uint32_t ph = 0;
-      for (int tile = cta; tile < num_tiles; tile += ncta) {
-        const int m0 = (tile / num_n) * TM + (int)rank * BM;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM;
         const int nt = tile % num_n;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[s], ph ^ 1);
           uint8_t* sa = smem + s * L::STAGE_BYTES;
           uint8_t* sb = sa + L::A_BYTES;
-          if (CG == 1) {
-            mbar_expect_tx(&full[s], L::STAGE_BYTES);
-            tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
-            if (MODE == MODE_LSTM_FWD) {
-              // interleave the 4 gate blocks of this hidden-unit slice: tile columns = [i | f | o | g]
-              constexpr int HB = BN / 4;
+          mbar_expect_tx(&full[s], L::STAGE_BYTES);
+          tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
+          if (MODE == MODE_LSTM_FWD) {
+            // interleave the 4 gate blocks of this hidden-unit slice: tile columns = [i | f | o | g]
+            constexpr int HB = BN / 4;
 #pragma unroll
-              for (int g = 0; g < 4; ++g) tma_load_2d(sb + g * HB * BK * 4, &tmB, &full[s], kb * BK, g * p.H + nt * HB);
-            } else {
-              tma_load_2d(sb, &tmB, &full[s], kb * BK, nt * BN);
-            }
+            for (int g = 0; g < 4; ++g) tma_load_2d(sb + g * HB * BK * 4, &tmB, &full[s], kb * BK, g * p.H + nt * HB);
           } else {
-            // all transactions of the pair complete on the LEADER's full barrier
-            const uint32_t bar = mapa_u32(smem_u32(&full[s]), 0);
-            if (leader) mbar_expect_tx(&full[s], 2 * L::STAGE_BYTES);
-            tma_load_2d_cg2(sa, &tmA, bar, kb * BK, m0);
-            if (MODE == MODE_LSTM_FWD) {
-              constexpr int HB = BN / 4;              // leader stages gate blocks [i | f], peer [o | g]
-#pragma unroll
-              for (int g = 0; g < 2; ++g)
-                tma_load_2d_cg2(sb + g * HB * BK * 4, &tmB, bar, kb * BK, ((int)rank * 2 + g) * p.H + nt * HB);
-            } else {
-              tma_load_2d_cg2(sb, &tmB, bar, kb * BK, nt * BN + (int)rank * (BN / 2));
-            }
+            tma_load_2d(sb, &tmB, &full[s], kb * BK, nt * BN);
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1 && !leader) {
-    // peer CTA of a pair: its MMA warp only takes part in TMEM alloc / dealloc
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    constexpr uint32_t idesc = make_idesc(TM, BN, 0, 0);
+  } else {
+    // ===== consumers: warpgroup wg contracts rows [64 wg, 64 wg + 64) of the tile, then all 8 warps run the epilogue =====
+    const int cw = warp - 4, wg = cw >> 2;
+    const int q = cw & 3;
+    const int half = cw >> 2;
+    const float* arow = acc + q * 32 + lane;
     int s = 0; uint32_t ph = 0;
-    int it = 0;
-    for (int tile = cta; tile < num_tiles; tile += ncta, ++it) {
-      const int buf = it & 1;
-      const uint32_t bph = (it >> 1) & 1;
-      mbar_wait(&tempty[buf], bph ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * BN;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m0 = (tile / num_n) * BM;
+      const int nt = tile % num_n;
+      float d[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[s], ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-          const uint32_t sb = sa + L::A_BYTES;
-          const uint64_t adesc = make_desc(sa, 16, 1024);
-          const uint64_t bdesc = make_desc(sb, 16, 1024);
+        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
+        const uint64_t adesc = make_desc(sa + wg * 64 * 128, 16, 1024), bdesc = make_desc(sa + L::A_BYTES, 16, 1024);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            const uint64_t ad = adesc + (uint64_t)(k * UMMA_K * 4 >> 4), bd = bdesc + (uint64_t)(k * UMMA_K * 4 >> 4);
-            if (CG == 2) umma_tf32_cg2(d_tmem, ad, bd, idesc, (kb | k) ? 1u : 0u);
-            else umma_tf32(d_tmem, ad, bd, idesc, (kb | k) ? 1u : 0u);
-          }
-          if (CG == 2) { umma_commit_cg2(&empty[s]); if (kb == num_kb - 1) umma_commit_cg2(&tfull[buf]); }
-          else { umma_commit(&empty[s]); if (kb == num_kb - 1) umma_commit(&tfull[buf]); }
-        }
-        __syncwarp();
+        for (int k = 0; k < BK / MMA_K; ++k)
+          wgmma_tf32<BN>(d, adesc + (uint64_t)(k * MMA_K * 4 >> 4), bdesc + (uint64_t)(k * MMA_K * 4 >> 4), (kb | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();                              // the previous k-block's MMAs are done with their stage
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-      if (num_kb == 0 && lane == 0) {                 // K == 0: nothing to wait for, release the epilogue(s)
-        mbar_arrive(&tfull[buf]);
-        if (CG == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&tfull[buf]), 1));
-      }
-      __syncwarp();
-    }
-  } else {
-    // ===== epilogue: warps 2..9; TMEM lane quarter = warp % 4, column half = (warp - 2) / 4 =====
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int it = 0;
-    for (int tile = cta; tile < num_tiles; tile += ncta, ++it) {
-      const int buf = it & 1;
-      const uint32_t bph = (it >> 1) & 1;
-      const int m0 = (tile / num_n) * TM + (int)rank * BM;
-      const int nt = tile % num_n;
-      mbar_wait(&tfull[buf], bph);
-      tc_fence_after();
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      bar_named(1, 32 * EPI_WARPS);                    // the previous tile's epilogue is done with the accumulator tile
+      acc_store(acc, d, wg * 64);
+      bar_named(1, 32 * EPI_WARPS);
       const int64_t row = (int64_t)m0 + q * 32 + lane;
       const bool row_ok = row < p.M;
-      const uint32_t taddr = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16);
 
       if (MODE == MODE_LSE) {
         // online softmax statistics of this warp's column slice of the tile: nothing but (max, sum exp, target logit) leaves
@@ -278,8 +218,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 8) {
           if (n0 + c >= p.N) break;                 // warp-uniform
           float v[8];
-          tmem_ld8(taddr + c, v);
-          tmem_ld_wait();
+          acc_ld8(arow, c, v);
           float mx = -INFINITY;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
@@ -306,7 +245,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         // 16 output columns at a time through the warp's staging array; C leaves (and, for beta != 0, enters)
         // as 64-byte-swizzled boxes: TMA tensor store / cp.async load.  Rows >= M and columns >= N are clipped.
         const int n0 = nt * BN;
-        float* stg = stg_all + (warp - 2) * (SC::ARR * 32 * 16);
+        float* stg = stg_all + cw * (SC::ARR * 32 * 16);
 #pragma unroll 1
         for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 16) {
           if (n0 + c >= p.N) break;                 // warp-uniform
@@ -329,9 +268,8 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 #pragma unroll
           for (int sub = 0; sub < 2; ++sub) {
             float v[8], old[8];
-            tmem_ld8(taddr + c + sub * 8, v);
-            tmem_ld_wait();
-            if (p.beta != 0.f) stg_get8(stg, 0, lane, sub, old);
+            acc_ld8(arow, c + sub * 8, v);
+              if (p.beta != 0.f) stg_get8(stg, 0, lane, sub, old);
             if (MODE == MODE_DLOGIT) {
               // d loss / d logit of the sum criterion: softmax - onehot on kept rows (input token != pad, target != pad)
               const int tg = row_ok ? p.tgt[row] : 0;
@@ -366,73 +304,11 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         const bool masked = row_ok && p.mask_ids && p.mask_ids[row] == 0;
         const float* prow = (row_ok && p.ptable) ? p.ptable + (int64_t)p.tok[row] * 4 * H : nullptr;
         float* grow = p.gates ? p.gates + row * 4 * H : nullptr;
-        if constexpr (SC::ON) {
-          // staged epilogue: 16 hidden units at a time through the warp's swizzled staging tile
-          float* stg = stg_all + (warp - 2) * (SC::ARR * 32 * 16);
-#pragma unroll 1
-          for (int c = half * (HB / NH); c < (half + 1) * (HB / NH); c += 16) {
-            const int j = j0 + c;
-            if (lane == 0) bulk_wait_read0();    // the previous group's TMA stores have finished reading the staging tile
-            __syncwarp();
-            // phase 1: coalesced global -> staging (x-projection rows of the 4 gates, previous cell)
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const float* src = nullptr;
-              if (row_ok) src = p.has_xproj ? grow + g * H + j : (prow ? prow + g * H + j : nullptr);
-              stg_load(stg, g, src, lane);
-            }
-            stg_load(stg, 4, (row_ok && p.c_prev) ? p.c_prev + row * H + j : nullptr, lane);
-            stg_load_wait();
-            // phase 2: thread = row; TMEM accumulators + staged inputs -> gates, c, h back into the staging tile
-#pragma unroll
-            for (int sub = 0; sub < 2; ++sub) {
-              float a[4][8], cn[8], hn[8], cp[8];
-#pragma unroll
-              for (int g = 0; g < 4; ++g) tmem_ld8(taddr + g * HB + c + sub * 8, a[g]);
-              tmem_ld_wait();
-              stg_get8(stg, 4, lane, sub, cp);
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                float x[8];
-                stg_get8(stg, g, lane, sub, x);
-                if (p.bias) add8(p.bias + g * H + j + sub * 8, x);     // null when folded into the x-projection
-#pragma unroll
-                for (int e = 0; e < 8; ++e) a[g][e] += x[e];
-              }
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const float gi = fsigmoid(a[0][e]), gf = fsigmoid(a[1][e]), go = fsigmoid(a[2][e]), gg = ftanh(a[3][e]);
-                const float c_ = gf * cp[e] + gi * gg;
-                const float keep = masked ? 0.f : 1.f;
-                a[0][e] = gi * keep; a[1][e] = gf * keep; a[2][e] = go * keep; a[3][e] = gg * keep;
-                cn[e] = c_ * keep; hn[e] = go * ftanh(c_) * keep;
-              }
-#pragma unroll
-              for (int g = 0; g < 4; ++g) stg_put8(stg, g, lane, sub, a[g]);
-              stg_put8(stg, 4, lane, sub, cn);
-              stg_put8(stg, 5, lane, sub, hn);
-            }
-            // phase 3: staging -> global by TMA tensor stores (rows beyond R are clipped by the tensor map)
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              const int r0 = m0 + q * 32;
-              if (p.gates) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) tma_store_2d(&em.g4, stg + g * 512, g * H + j, r0);
-              }
-              tma_store_2d(&em.c, stg + 4 * 512, j, r0);
-              tma_store_2d(&em.h, stg + 5 * 512, j, r0);
-              bulk_commit();
-            }
-            __syncwarp();
-          }
-        } else {
 #pragma unroll 1
         for (int c = half * (HB / NH); c < (half + 1) * (HB / NH); c += 8) {
           const int j = j0 + c;
           float a[4][8], x[4][8], cp[8];
-          // issue the global loads first so that they overlap the TMEM read
+          // issue the global loads first so that they overlap the accumulator read
           if (row_ok && !masked) {
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
@@ -451,8 +327,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
           }
 #pragma unroll
-          for (int g = 0; g < 4; ++g) tmem_ld8(taddr + g * HB + c, a[g]);
-          tmem_ld_wait();
+          for (int g = 0; g < 4; ++g) acc_ld8(arow, g * HB + c, a[g]);
           if (row_ok) {
             float cn[8], hn[8];
             if (masked) {
@@ -478,69 +353,9 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           }
           __syncwarp();
         }
-        }   // !SC::ON
       } else {   // MODE_LSTM_BWD: accumulator = dh_rec for hidden units [nt*BN, nt*BN + BN)
         const int H = p.H, j0 = nt * BN;
         const bool masked = row_ok && p.mask_ids && p.mask_ids[row] == 0;
-        if constexpr (SC::ON) {
-          float* stg = stg_all + (warp - 2) * (SC::ARR * 32 * 16);
-#pragma unroll 1
-          for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 16) {
-            const int j = j0 + c;
-            if (lane == 0) bulk_wait_read0();
-            __syncwarp();
-            // phase 1: saved gates (4), c_prev, c_t, dc carry -> staging, coalesced
-#pragma unroll
-            for (int g = 0; g < 4; ++g) stg_load(stg, g, row_ok ? p.gsave + row * 4 * H + g * H + j : nullptr, lane);
-            stg_load(stg, 4, (row_ok && p.c_prev) ? p.c_prev + row * H + j : nullptr, lane);
-            stg_load(stg, 5, row_ok ? p.c_cur + row * H + j : nullptr, lane);
-            stg_load(stg, 6, row_ok ? p.dc_carry + row * H + j : nullptr, lane);
-            stg_load_wait();
-#pragma unroll
-            for (int sub = 0; sub < 2; ++sub) {
-              float dh[8], g[4][8], cp[8], cc[8], dc[8], out[4][8], dcn[8];
-              tmem_ld8(taddr + c + sub * 8, dh);
-              tmem_ld_wait();
-#pragma unroll
-              for (int gg = 0; gg < 4; ++gg) stg_get8(stg, gg, lane, sub, g[gg]);
-              stg_get8(stg, 4, lane, sub, cp);
-              stg_get8(stg, 5, lane, sub, cc);
-              stg_get8(stg, 6, lane, sub, dc);
-              if (p.dh_ext && row_ok) {          // only the last time step has an external gradient here
-                float ex[8];
-                ld8(p.dh_ext + row * H + j + sub * 8, ex);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) dh[e] += ex[e];
-              }
-              const float keep = masked ? 0.f : 1.f;
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
-                const float tcv = ftanh(cc[e]);
-                const float d = (dc[e] + dh[e] * go * (1.f - tcv * tcv)) * keep;
-                const float dhe = dh[e] * keep;
-                out[0][e] = d * gg_ * gi * (1.f - gi);
-                out[1][e] = d * cp[e] * gf * (1.f - gf);
-                out[2][e] = dhe * tcv * go * (1.f - go);
-                out[3][e] = d * gi * (1.f - gg_ * gg_);
-                dcn[e] = d * gf;
-              }
-#pragma unroll
-              for (int gg = 0; gg < 4; ++gg) stg_put8(stg, gg, lane, sub, out[gg]);
-              stg_put8(stg, 6, lane, sub, dcn);
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              const int r0 = m0 + q * 32;
-#pragma unroll
-              for (int gg = 0; gg < 4; ++gg) tma_store_2d(&em.g4, stg + gg * 512, gg * H + j, r0);
-              tma_store_2d(&em.c, stg + 6 * 512, j, r0);
-              bulk_commit();
-            }
-            __syncwarp();
-          }
-        } else {
 #pragma unroll 1
         for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 8) {
           const int j = j0 + c;
@@ -561,8 +376,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
               for (int e = 0; e < 8; ++e) ex[e] = 0.f;
             }
           }
-          tmem_ld8(taddr + c, dh);
-          tmem_ld_wait();
+          acc_ld8(arow, c, dh);
           if (row_ok) {
             float out[4][8], dcn[8];
             if (masked) {
@@ -588,139 +402,109 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           }
           __syncwarp();
         }
-        }   // !SC::ON
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                                // the accumulator buffer may be overwritten by the (leader's) MMAs
-        if (CG == 2 && !leader) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[buf]), 0));
-        else mbar_arrive(&tempty[buf]);
       }
     }
     if (SC::ON && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
   }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();   // nobody tears down while the peer still signals / reads
-  if (warp == 1) {
-    tc_fence_after();
-    if (CG == 2) tmem_dealloc_cg2(tmem_base, L::TMEM_COLS); else tmem_dealloc(tmem_base, L::TMEM_COLS);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
-// Weight gradients: C[M,N] += sum_k A[k,m] B[k,n].  Both operands are "MN-major" (the contraction index k is
-// the row index of the activations in HBM): a TMA box of 32 columns x KB rows lands in shared memory as KB rows
-// of 128 bytes; with the 128B_ATOM_32B swizzle this is the canonical MN-major SWIZZLE_128B_BASE32B UMMA layout, the
-// only MN-major layout tf32 operands may use (4 k-rows per 512-byte atom, SBO = 512; one K=8 MMA consumes two
-// atoms; 32-column groups are LBO bytes apart).  One (tile, K-split) per CTA; the fp32 partial sums are reduced
-// into C with vector red.global.add.
-constexpr int ATB_KB = 32;       // k-rows per pipeline stage (4 MMAs)
-constexpr int ATB_BN = 256;
-constexpr int ATB_THREADS = 192;
-struct AtbParams { int M, N; int64_t K, k_per_split; float* C; int64_t ldc; };
-struct AtbSmem {
-  static constexpr int A_BYTES = BM * ATB_KB * 4;         // 4 boxes of [32 rows x 128 B]
-  static constexpr int B_BYTES = ATB_BN * ATB_KB * 4;     // 8 boxes
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = 4;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
-};
+// Weight gradients: C[M,N] += sum_k A[k,m] B[k,n].  Both operands are "MN-major" (the contraction index k is the row
+// index of the activations in HBM), and wgmma takes tf32 operands K-major only: the two consumer warpgroups load each
+// k-block (32 rows of A and B) from global memory and transpose it into the K-major 128B-swizzled layout while storing
+// it (double-buffered: the next k-block's loads fly while the current one's MMAs run).  One (tile, K-split) per CTA; the
+// fp32 partial sums are reduced into C with red.global.add.
+constexpr int ATB_KB = 32;       // k-rows per k-block (4 MMAs)
+constexpr int ATB_BN = 128;
+constexpr int ATB_THREADS = 256;
+constexpr int ATB_OP_BYTES = 128 * ATB_KB * 4;            // one operand tile: 128 rows of 128 B
+constexpr int ATB_SMEM = 2 * 2 * ATB_OP_BYTES + 1024;
+struct AtbParams { int M, N; int64_t K, k_per_split; const float* A; int64_t lda; const float* B; int64_t ldb; float* C; int64_t ldc; };
+
+// thread's share of a k-block of one operand: 32 k-rows x 128 columns = 1024 chunks of (4 consecutive k, one column), 4 per
+// thread; a warp reads 32 consecutive columns of a k-row per load (coalesced), zero outside the operand
+__device__ __forceinline__ void atb_load(float4 (&r)[4], const float* X, int64_t ldx, int ncols, int c0, int64_t k0, int64_t kend) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int idx = (int)threadIdx.x + ATB_THREADS * i;
+    const int c = c0 + (idx & 127);
+    const int64_t k = k0 + (idx >> 7) * 4;
+    float v[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) v[e] = (c < ncols && k + e < kend) ? __ldg(X + (k + e) * ldx + c) : 0.f;
+    r[i] = make_float4(v[0], v[1], v[2], v[3]);
+  }
+}
+// chunk (k/4, col) of the K-major tile: row `col` of 128 bytes, 16-byte chunk k/4 swizzled with col % 8 — one vector store;
+// the 8 lanes of a store phase hold 8 consecutive columns, i.e. 8 different chunks: no bank conflict
+__device__ __forceinline__ void atb_store(uint8_t* tile, const float4 (&r)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int idx = (int)threadIdx.x + ATB_THREADS * i;
+    const int col = idx & 127, kq = idx >> 7;
+    *reinterpret_cast<float4*>(tile + col * 128 + ((kq ^ (col & 7)) << 4)) = r[i];
+  }
+}
 
 __global__ void __launch_bounds__(ATB_THREADS, 1)
-k_tc_atb(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const AtbParams p) {
-  using L = AtbSmem;
-  constexpr int STAGES = L::STAGES;
+k_tc_atb(const AtbParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = (uint64_t*)(smem + STAGES * L::STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(tfull + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int num_n = (p.N + ATB_BN - 1) / ATB_BN;
   const int m0 = (blockIdx.x / num_n) * BM, n0 = (blockIdx.x % num_n) * ATB_BN;
   const int64_t kbeg = (int64_t)blockIdx.y * p.k_per_split;
   const int64_t kend = min(p.K, kbeg + p.k_per_split);
   const int num_kb = (int)((kend - kbeg + ATB_KB - 1) / ATB_KB);
+  if (num_kb <= 0) return;
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tfull, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, ATB_BN);
-  tc_fence_before();
+  float d[ATB_BN / 2];
+#pragma unroll
+  for (int i = 0; i < ATB_BN / 2; ++i) d[i] = 0.f;
+  float4 ra[4], rb[4];
+  atb_load(ra, p.A, p.lda, p.M, m0, kbeg, kend);
+  atb_load(rb, p.B, p.ldb, p.N, n0, kbeg, kend);
+  atb_store(smem, ra);
+  atb_store(smem + ATB_OP_BYTES, rb);
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int s = 0; uint32_t ph = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* sa = smem + s * L::STAGE_BYTES;
-        uint8_t* sb = sa + L::A_BYTES;
-        mbar_expect_tx(&full[s], L::STAGE_BYTES);
-        const int krow = (int)(kbeg + (int64_t)kb * ATB_KB);
-        // k_per_split is a multiple of ATB_KB, so only the global K tail (zero-filled by TMA) can be partial
+  for (int kb = 0; kb < num_kb; ++kb) {
+    uint8_t* cur = smem + (kb & 1) * 2 * ATB_OP_BYTES;
+    const uint32_t sa = smem_u32(cur);
+    const uint64_t adesc = make_desc(sa + wg * 64 * 128, 16, 1024), bdesc = make_desc(sa + ATB_OP_BYTES, 16, 1024);
+    wgmma_fence();
 #pragma unroll
-        for (int g = 0; g < BM / 32; ++g) tma_load_2d(sa + g * ATB_KB * 128, &tmA, &full[s], m0 + g * 32, krow);
-#pragma unroll
-        for (int g = 0; g < ATB_BN / 32; ++g) tma_load_2d(sb + g * ATB_KB * 128, &tmB, &full[s], n0 + g * 32, krow);
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
+    for (int k = 0; k < ATB_KB / MMA_K; ++k)
+      wgmma_tf32_n128(d, adesc + (uint64_t)(k * MMA_K * 4 >> 4), bdesc + (uint64_t)(k * MMA_K * 4 >> 4), (kb | k) ? 1u : 0u);
+    wgmma_commit();
+    if (kb + 1 < num_kb) {
+      const int64_t k0 = kbeg + (int64_t)(kb + 1) * ATB_KB;
+      atb_load(ra, p.A, p.lda, p.M, m0, k0, kend);
+      atb_load(rb, p.B, p.ldb, p.N, n0, k0, kend);
+      uint8_t* nxt = smem + ((kb + 1) & 1) * 2 * ATB_OP_BYTES;   // its last readers (k-block kb - 1) have completed
+      atb_store(nxt, ra);
+      atb_store(nxt + ATB_OP_BYTES, rb);
+      fence_proxy_async_smem();
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc(BM, ATB_BN, 1, 1);
-    int s = 0; uint32_t ph = 0;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full[s], ph);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-        const uint32_t sb = sa + L::A_BYTES;
+    wgmma_wait<0>();
+    wgmma_hold(d);
+    __syncthreads();
+  }
+  // fragment -> red.add into C
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int r0 = m0 + wg * 64 + 16 * w + (lane >> 2), c0 = n0 + 2 * (lane & 3);
 #pragma unroll
-        for (int k = 0; k < ATB_KB / UMMA_K; ++k) {
-          const uint64_t adesc = make_desc(sa + k * 1024, ATB_KB * 128, 512, 1);
-          const uint64_t bdesc = make_desc(sb + k * 1024, ATB_KB * 128, 512, 1);
-          umma_tf32(tmem_base, adesc, bdesc, idesc, (kb | k) ? 1u : 0u);
-        }
-        umma_commit(&empty[s]);
-        if (kb == num_kb - 1) umma_commit(tfull);
-      }
-      __syncwarp();
-      if (++s == STAGES) { s = 0; ph ^= 1; }
-    }
-  } else if (num_kb > 0) {
-    const int q = warp & 3;
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    const int m = m0 + q * 32 + lane;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c = 0; c < ATB_BN; c += 8) {
-      if (n0 + c >= p.N) break;
-      float v[8];
-      tmem_ld8(taddr + c, v);
-      tmem_ld_wait();
+  for (int j = 0; j < ATB_BN / 8; ++j) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = r0 + 8 * h, n = c0 + 8 * j;
       if (m < p.M) {
-        float* crow = p.C + (int64_t)m * p.ldc + n0 + c;
-        if (n0 + c + 8 <= p.N && ((p.ldc & 3) == 0)) {
-          red_add_v4(crow, v[0], v[1], v[2], v[3]);
-          red_add_v4(crow + 4, v[4], v[5], v[6], v[7]);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (n0 + c + j < p.N) atomicAdd(crow + j, v[j]);
-        }
+        float* crow = p.C + (int64_t)m * p.ldc + n;
+        if (n < p.N) atomicAdd(crow, d[4 * j + 2 * h]);
+        if (n + 1 < p.N) atomicAdd(crow + 1, d[4 * j + 2 * h + 1]);
       }
-      __syncwarp();
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, ATB_BN); }
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -760,64 +544,25 @@ static CUtensorMap make_tmap(const float* base, int64_t rows, int64_t cols, int6
 
 static bool tma_ok(const float* p, int64_t ld) { return ((uintptr_t)p % 16 == 0) && (ld % 4 == 0); }
 
-template <int BN, int MODE, int CG = 1, int EW = EPI_WARPS>
+template <int BN, int MODE>
 static void launch(LaunchCtx& cx, const CUtensorMap& tA, const CUtensorMap& tB, const Params& p, int num_tiles,
                    const EpiMaps* epi = nullptr) {
-  using L = SmemLayout<BN, CG, StageCfg<BN, MODE, CG, EW>::BYTES, (EW == 4 ? 4 : 16)>;
-  constexpr int THREADS = 64 + 32 * EW;
+  using L = SmemLayout<BN, StageCfg<MODE>::BYTES>;
   static EpiMaps none = {};
   const EpiMaps& em = epi ? *epi : none;
   static bool attr_set = false;
   if (!attr_set) {
-    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_gemm<BN, MODE, CG, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
-    if (EW == 4)      // two of these CTAs per SM: ask for the full shared-memory carve-out
-      VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_gemm<BN, MODE, CG, EW>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                         cudaSharedmemCarveoutMaxShared));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_gemm<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     attr_set = true;
   }
-  // Persistent grid, balanced waves: with pmax CTAs (pairs) available the tiles need ceil(tiles/pmax) rounds; the
-  // smallest grid that still finishes in that many rounds is used, so no CTA idles through a ragged last round and the
-  // SMs not needed stay free for concurrent streams (250 backward tiles: 63 pairs x 4 rounds instead of 74 x 3.4).
-  auto balanced = [&](int pmax) {
-    if (num_tiles <= pmax) return num_tiles;
-    const int rounds = cdiv(num_tiles, pmax);
-    return cdiv(num_tiles, rounds);
-  };
-  if (CG == 1) {
-    int grid = balanced(cx.sms());
-    k_tc_gemm<BN, MODE, 1, EW><<<grid, THREADS, L::TOTAL, cx.stream>>>(tA, tB, em, p);
-  } else {
-    // CTA pairs: a 2-CTA cluster per 256-row tile, one pair per TPC (num_tiles counts 256-row tiles here)
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * balanced(cx.sms() / 2));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = L::TOTAL;
-    cfg.stream = cx.stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    VD_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_tc_gemm<BN, MODE, 2, EW>, tA, tB, em, p));
-  }
+  // Persistent grid, balanced waves: with pmax CTAs available the tiles need ceil(tiles/pmax) rounds; the smallest grid
+  // that still finishes in that many rounds is used, so no CTA idles through a ragged last round and the SMs not needed
+  // stay free for concurrent streams.
+  const int pmax = cx.sms();
+  int grid = num_tiles;
+  if (num_tiles > pmax) { const int rounds = cdiv(num_tiles, pmax); grid = cdiv(num_tiles, rounds); }
+  k_tc_gemm<BN, MODE><<<grid, GEMM_THREADS, L::TOTAL, cx.stream>>>(tA, tB, em, p);
   check_launch(cx, "k_tc_gemm");
-}
-
-static bool small_ew4() {          // VD_SMALL_EW4=0: the few-row kernels as one 320-thread CTA per SM (A/B)
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VD_SMALL_EW4"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
-
-static int small_narrow() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VD_SMALL_NARROW"); v = e ? atoi(e) : 0; }
-  return v;
-}
-
-static bool use_cta_pairs() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VD_CTA_PAIRS"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
 }
 
 }  // namespace tc
@@ -833,17 +578,13 @@ bool gemm_tn_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda,
   p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.beta = beta; p.bias = bias; p.act = act;
   EpiMaps em = {};
   em.g4 = make_tmap(C, M, N, ldc, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);      // C leaves through TMA tensor stores
-  const int tiles256 = cdiv(M, BM) * cdiv(N, 256);
-  if (N > 128 && tiles256 >= cx.sm_count / 2) {
-    CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 256);
-    launch<256, MODE_GENERIC>(cx, tA, tB, p, tiles256, &em);
-  } else if (N > 64 && cdiv(M, BM) * cdiv(N, 128) >= cx.sm_count / 2) {
-    CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);
+  CUtensorMap tA = make_tmap(A, M, K, lda, BM);
+  if (N > 64) {
+    CUtensorMap tB = make_tmap(B, N, K, ldb, 128);
     launch<128, MODE_GENERIC>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128), &em);
   } else {
-    CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 64);
-    if (small_ew4()) launch<64, MODE_GENERIC, 1, 4>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 64), &em);
-    else launch<64, MODE_GENERIC>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 64), &em);
+    CUtensorMap tB = make_tmap(B, N, K, ldb, 64);
+    launch<64, MODE_GENERIC>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 64), &em);
   }
   return true;
 }
@@ -855,30 +596,28 @@ bool gemm_atb_tc(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t
   if (M < 32 || N < 32 || K < 64) return false;
   if (!tma_ok(A, lda) || !tma_ok(B, ldb)) return false;
   const int tiles = cdiv(M, BM) * cdiv(N, ATB_BN);
-  // whole waves: the largest split count with tiles * splits <= 2 * #SM (one CTA per SM at this smem footprint)
+  // whole waves: the largest split count with tiles * splits <= 2 * #SM
   // (under an SM budget — the option stream sharing the GPU with the encoder's chains — a single wave of budget CTAs, so
   // that the reserved SMs really stay free: a second wave would be placed on them)
   const int64_t cta_cap = cx.sm_budget > 0 ? cx.sm_budget : 2LL * cx.sm_count;
   int64_t splits = std::max<int64_t>(1, std::min<int64_t>(cta_cap / tiles, K / (ATB_KB * 4)));
   int64_t kps = ((K + splits - 1) / splits + ATB_KB - 1) / ATB_KB * ATB_KB;
   splits = (K + kps - 1) / kps;
-  AtbParams p = {M, N, K, kps, C, ldc};
-  CUtensorMap tA = make_tmap(A, K, M, lda, ATB_KB, 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B),
-              tB = make_tmap(B, K, N, ldb, ATB_KB, 32, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+  AtbParams p = {M, N, K, kps, A, lda, B, ldb, C, ldc};
   static bool attr_set = false;
   if (!attr_set) {
-    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_atb, cudaFuncAttributeMaxDynamicSharedMemorySize, AtbSmem::TOTAL));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_atb, cudaFuncAttributeMaxDynamicSharedMemorySize, ATB_SMEM));
     attr_set = true;
   }
   dim3 grid(tiles, (unsigned)splits);
-  k_tc_atb<<<grid, ATB_THREADS, AtbSmem::TOTAL, cx.stream>>>(tA, tB, p);
+  k_tc_atb<<<grid, ATB_THREADS, ATB_SMEM, cx.stream>>>(p);
   check_launch(cx, "k_tc_atb");
   return true;
 }
 
 // Vocabulary projection with the softmax statistics fused into the epilogue (no (rows, V) tensor in HBM):
 //   part_max / part_sum (M, nparts): per column slice running max and sum of exp(x - max);  tgt_logit[m] = x[m, tgt[m]-1]
-int vocab_lse_nparts(int N) { return cdiv(N, 256) * (tc::EPI_WARPS / 4); }
+int vocab_lse_nparts(int N) { return cdiv(N, 128) * (tc::EPI_WARPS / 4); }
 bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
                   const int32_t* tgt, float* part_max, float* part_sum, float* tgt_logit) {
   using namespace tc;
@@ -887,8 +626,8 @@ bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t ld
   Params p = {};
   p.M = M; p.N = N; p.K = K; p.bias = bias; p.tgt = tgt; p.part_max = part_max; p.part_sum = part_sum; p.tgt_logit = tgt_logit;
   p.nparts = vocab_lse_nparts(N);
-  CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 256);
-  launch<256, MODE_LSE>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 256));
+  CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);
+  launch<128, MODE_LSE>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128));
   return true;
 }
 // C[m,n] = keep[m] * (exp(A B^T + bias - lse[m]) - [n == tgt[m]-1])   (backward of log-softmax + ClassNLL, recomputed)
@@ -901,8 +640,8 @@ bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_
   p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.bias = bias; p.tgt = tgt; p.row_ids = row_ids; p.lse = lse;
   EpiMaps em = {};
   em.g4 = make_tmap(C, M, N, ldc, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-  CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 256);
-  launch<256, MODE_DLOGIT>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 256), &em);
+  CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);
+  launch<128, MODE_DLOGIT>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128), &em);
   return true;
 }
 
@@ -920,24 +659,12 @@ bool lstm_step_fwd_tc(LaunchCtx& cx, int64_t R, int H, const float* h_prev, cons
   p.bias = bias; p.gates = gates; p.has_xproj = has_xproj; p.ptable = ptable; p.tok = tok;
   p.c_prev = c_prev; p.c_out = c_out; p.h_out = h_out; p.mask_ids = mask_ids;
   CUtensorMap tA = make_tmap(h_prev, p.K ? R : 128, H, H, BM);
-  const int tiles_big = cdiv(R, BM) * (H / 64);
-  if (tiles_big >= cx.sm_count) {            // 64 hidden units (x 4 gates = 256 columns) per tile
-    CUtensorMap tB = make_tmap(WtS_h, 4 * (int64_t)H, H, ldw, 64);
-    if (use_cta_pairs() && p.K > 0) {
-      EpiMaps em;                              // epilogue outputs leave through TMA tensor stores (64B-swizzled boxes)
-      em.g4 = make_tmap(gates ? gates : c_out, R, gates ? 4 * (int64_t)H : H, gates ? 4 * (int64_t)H : H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      em.c = make_tmap(c_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      em.h = make_tmap(h_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      launch<256, MODE_LSTM_FWD, 2>(cx, tA, tB, p, cdiv(R, 2 * BM) * (H / 64), &em);
-    }
-    else launch<256, MODE_LSTM_FWD>(cx, tA, tB, p, tiles_big);
-  } else if (small_narrow() == 2) {          // experiment: few fat CTAs (64 hidden units per tile)
-    CUtensorMap tB = make_tmap(WtS_h, 4 * (int64_t)H, H, ldw, 64);
-    launch<256, MODE_LSTM_FWD>(cx, tA, tB, p, tiles_big);
-  } else {                                   // few rows (encoder LSTMs): 16 hidden units per tile, 4x the CTAs
+  if (cdiv(R, BM) * (H / 32) >= cx.sm_count) {   // 32 hidden units (x 4 gates = 128 columns) per tile
+    CUtensorMap tB = make_tmap(WtS_h, 4 * (int64_t)H, H, ldw, 32);
+    launch<128, MODE_LSTM_FWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 32));
+  } else {                                   // few rows (encoder LSTMs): 16 hidden units per tile, 2x the CTAs
     CUtensorMap tB = make_tmap(WtS_h, 4 * (int64_t)H, H, ldw, 16);
-    if (small_ew4()) launch<64, MODE_LSTM_FWD, 1, 4>(cx, tA, tB, p, cdiv(R, BM) * (H / 16));
-    else launch<64, MODE_LSTM_FWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 16));
+    launch<64, MODE_LSTM_FWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 16));
   }
   return true;
 }
@@ -956,34 +683,12 @@ bool lstm_step_bwd_tc(LaunchCtx& cx, int64_t R, int H, const float* da_next, con
   p.gsave = gsave; p.c_prev = c_prev; p.c_cur = c_cur; p.dh_ext = dh_ext;
   p.dc_carry = dc_carry; p.mask_ids = mask_ids; p.da = da;
   CUtensorMap tA = make_tmap(da_next, p.K ? R : 128, 4 * (int64_t)H, 4 * (int64_t)H, BM);
-  const int tiles_big = cdiv(R, BM) * (H / 128);
-  if (tiles_big >= cx.sm_count) {
+  if (cdiv(R, BM) * (H / 128) >= cx.sm_count) {
     CUtensorMap tB = make_tmap(Wh, H, 4 * (int64_t)H, 4 * (int64_t)H, 128);
-    static int bwd_bn = -1;
-    if (bwd_bn < 0) { const char* e = getenv("VD_BWD_BN"); bwd_bn = (e && atoi(e) == 128) ? 128 : 256; }
-    if (use_cta_pairs() && p.K > 0 && bwd_bn == 256 && H % 256 == 0) {
-      EpiMaps em;
-      em.g4 = make_tmap(da, R, 4 * (int64_t)H, 4 * (int64_t)H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      em.c = make_tmap(dc_carry, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      em.h = em.c;
-      launch<256, MODE_LSTM_BWD, 2>(cx, tA, tB, p, cdiv(R, 2 * BM) * (H / 256), &em);
-    } else if (use_cta_pairs() && p.K > 0) {
-      // 128 hidden units per pair-tile: twice the tiles of the 256-wide variant -> a fuller last wave (250 vs 500
-      // tiles over 74 CTA pairs)
-      CUtensorMap tB64 = make_tmap(Wh, H, 4 * (int64_t)H, 4 * (int64_t)H, 64);
-      EpiMaps em;
-      em.g4 = make_tmap(da, R, 4 * (int64_t)H, 4 * (int64_t)H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      em.c = make_tmap(dc_carry, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-      em.h = em.c;
-      launch<128, MODE_LSTM_BWD, 2>(cx, tA, tB64, p, cdiv(R, 2 * BM) * (H / 128), &em);
-    } else launch<128, MODE_LSTM_BWD>(cx, tA, tB, p, tiles_big);
-  } else if (small_narrow() >= 1) {          // experiment: 128 hidden units per tile
-    CUtensorMap tB = make_tmap(Wh, H, 4 * (int64_t)H, 4 * (int64_t)H, 128);
-    launch<128, MODE_LSTM_BWD>(cx, tA, tB, p, tiles_big);
-  } else {
+    launch<128, MODE_LSTM_BWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 128));
+  } else {                                   // few rows: 32 hidden units per tile
     CUtensorMap tB = make_tmap(Wh, H, 4 * (int64_t)H, 4 * (int64_t)H, 32);
-    if (small_ew4()) launch<32, MODE_LSTM_BWD, 1, 4>(cx, tA, tB, p, cdiv(R, BM) * (H / 32));
-    else launch<32, MODE_LSTM_BWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 32));
+    launch<32, MODE_LSTM_BWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 32));
   }
   return true;
 }

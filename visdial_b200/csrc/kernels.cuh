@@ -15,7 +15,7 @@ void gemm_tn_simt(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t ld
 // C[m,n] += sum_k A[row(k),m] B[k,n]   (accGradParameters of Linear / SeqLSTM)
 void gemm_atb_simt(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t lda, const int32_t* a_gather,
                    const float* B, int64_t ldb, float* C, int64_t ldc);
-// tcgen05 / TMEM / TMA versions (gemm_tc.cu); return false when the shape is not taken.
+// wgmma / TMA versions (gemm_tc.cu); return false when the shape is not taken.
 bool gemm_tn_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const int32_t* a_gather,
                 const float* B, int64_t ldb, float* C, int64_t ldc, float beta, const float* bias, int act);
 bool gemm_atb_tc(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t lda, const int32_t* a_gather,

@@ -1,18 +1,17 @@
 // SeqLSTM over MANY rows (the disc decoder's option LSTM, decoders/disc.lua:4-20: R = N*100 = 32 000 rows at B = 32)
 // with 16-bit operands and 16-bit saved state: VD_MATH_F16.
 //
-// Why: ncu of the TF32 step kernels (profiles/r01_*) showed them bound by BYTES, not by the tensor pipe — the L2->SM
-// operand stream of fp32 tiles (1.0 GB per launch, ~80 % of the ~6300 B/clk LTS cap) and the HBM traffic of the fp32
-// saved activations (0.5 GB forward, 1.05 GB backward per step).  A TF32 operand keeps 10 mantissa bits of the fp32
+// Why: the TF32 step kernels are bound by BYTES, not by the tensor pipe — the L2->SM operand stream of fp32 tiles and the
+// HBM traffic of the fp32 saved activations (at B = 32: 0.5 GB forward, 1.05 GB backward per step).  A TF32 operand keeps 10 mantissa bits of the fp32
 // word it reads; an fp16 word carries the same 10 bits in half the bytes (the exponent range is what is given up: h and
 // the weights live well inside it, the gradients are scaled by a power of two chosen from max|dL/dh_T| so that they do
 // too — exact, undone in the weight-gradient epilogue).  So: h_t, the x-projection table, the activated gates and da_t
-// are stored as fp16, the contractions run as tcgen05 kind::f16 (2x the TF32 rate) with fp32 accumulation in TMEM,
+// are stored as fp16, the contractions run as f16 wgmma (2x the TF32 rate) with fp32 accumulation,
 // and c_t, dc, every accumulator, the weight gradients and the final h_T that meets the encoder stay fp32.
 //
-//   k_lstm16_fwd   : gates = h_{t-1} Wh^T (tcgen05, CTA pairs 256x256) + P16[token] + bias -> pointwise -> fp16 gates,
+//   k_lstm16_fwd   : gates = h_{t-1} Wh^T (wgmma, 128x128 tiles) + P16[token] + bias -> pointwise -> fp16 gates,
 //                    fp32 c_t, fp16 h_t (+ fp32 h_T on the last step)
-//   k_lstm16_bwd   : dh = da_{t+1} Wh (tcgen05) -> backward pointwise -> fp16 da_t, fp32 dc carry
+//   k_lstm16_bwd   : dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t, fp32 dc carry
 //   k_atb16        : dWh += inv_scale * h^T da  (both operands MN-major fp16, split-K, red.global.add)
 //   k_lstm16_first / k_lstm16_bwd_last / k_segsum16 / k_cvt16 / k_amax / k_pick_scale : streaming helpers
 #include <cuda.h>
@@ -24,31 +23,12 @@
 namespace vd {
 namespace tc {
 
-constexpr int BM16 = 128;        // rows per CTA (UMMA M = 256 per pair)
+constexpr int BM16 = 128;        // rows per tile (two 64-row wgmma slabs)
 constexpr int BK16 = 64;         // halves per k-block = one 128-byte swizzle row
-constexpr int UK16 = 16;         // kind::f16: 32 bytes per instruction
-// epilogue warps: 16 = four per TMEM lane quarter, each with its own share of the tile's columns.  The pointwise halves are
-// latency-bound per warp (gather / saved-activation loads, MUFU chains): four warps per scheduler hide what two could not
-// (forward step 176 -> 109 us, with the pad-token gather skip).  The backward step stays at 8: its 16-warp variant needs 160 KB
-// of staging, which leaves two 32 KB pipeline stages for a K = 2048 main loop — measured 209 us against 138 us with 8 warps / 4 stages
-template <int MODE> struct EW16T { static constexpr int N = MODE == 0 ? 16 : 8; };
-constexpr int STAGE16 = 32768;   // 16 KB of A (this CTA's 128 rows) + 16 KB of B (this CTA's half of the 256-column tile)
-
-// instruction descriptor, kind::f16: D = f32 (c_format 1), A = B = f16 (format 0)
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
-}
+constexpr int UK16 = 16;         // f16 wgmma: 32 bytes per instruction
+constexpr int BN16 = 128;        // accumulator columns per tile: forward 32 hidden units x 4 gates, backward 128 hidden units
+constexpr int EW16 = 8;          // consumer warps = epilogue warps: 2 per 32-row quarter
+constexpr int STAGE16 = 32768;   // 16 KB of A (128 rows) + 16 KB of B (128 rows)
 
 // sigmoid / tanh as {FMUL, MUFU.EX2, FADD, MUFU.RCP [, FFMA]}: abs error ~1e-7 like fsigmoid / ftanh of tc_ptx.cuh, without the
 // range fix-ups of __fdividef / copysign (ex2 -> +inf gives rcp -> 0, ex2 -> 0 gives 1: both limits are exact)
@@ -151,18 +131,18 @@ struct Lstm16Params {
 struct Lstm16Maps { CUtensorMap g16, c, h16; };   // [R,4H] fp16 gates / da ; [R,H] fp32 c / dc ; [R,H] fp16 h
 
 // ------------------------------------------------------------------------------------------------
-// MODE 0 = forward step, MODE 1 = backward step.  2-CTA clusters, persistent over the tile list.
+// MODE 0 = forward step, MODE 1 = backward step.  Persistent over the tile list; warpgroup 0 = TMA producer (one thread),
+// warpgroups 1-2 = consumers (64 rows each) that then run the pointwise epilogue "thread = row" from the accumulator tile.
 template <int MODE>
 struct Cfg16 {
-  static constexpr int EW = EW16T<MODE>::N;
-  static constexpr int THREADS = 64 + 32 * EW;
+  static constexpr int THREADS = 128 + 32 * EW16;
   // per-warp staging: forward {4 gate tiles S32, c tile S64, h tile S32} = 7 KB (inputs land here by cp.async, outputs
   // overwrite them in place and leave by TMA); backward {4 gate tiles S32, c_prev, c_t, dc S64} = 10 KB
   static constexpr int STG_PER_WARP = MODE == 0 ? (4 * S32_BYTES + S64_BYTES + S32_BYTES) : (4 * S32_BYTES + 3 * S64_BYTES);
-  static constexpr int BIAS_BYTES = MODE == 0 ? 4 * 512 * 4 : 0;                     // fp32 bias of all 4H gate columns (H <= 512)
-  static constexpr int STG_BYTES = EW * STG_PER_WARP + BIAS_BYTES;
-  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES) / STAGE16;      // fwd 3, bwd 4
-  static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + 1024 + 256;
+  static constexpr int STG_BYTES = EW16 * STG_PER_WARP;
+  static constexpr int ACC_BYTES = BN16 * ACC_LD * 4;
+  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES - ACC_BYTES) / STAGE16;      // fwd 3, bwd 2
+  static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + ACC_BYTES + 1024 + 256;
 };
 
 template <int MODE>
@@ -171,124 +151,101 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
          const __grid_constant__ Lstm16Maps em, const Lstm16Params p) {
   using C = Cfg16<MODE>;
   constexpr int STAGES = C::STAGES;
-  constexpr int BN = 256;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cta = (int)(blockIdx.x >> 1), ncta = (int)(gridDim.x >> 1);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* stg_all = smem + STAGES * STAGE16;
-  uint64_t* full = (uint64_t*)(stg_all + C::STG_BYTES);
+  float* acc = (float*)(stg_all + C::STG_BYTES);
+  uint64_t* full = (uint64_t*)(stg_all + C::STG_BYTES + C::ACC_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int H = p.H;
-  const int num_m = (p.R + 2 * BM16 - 1) / (2 * BM16);
-  const int num_n = MODE == 0 ? H / 64 : H / 256;
+  const int num_m = (p.R + BM16 - 1) / BM16;
+  const int num_n = MODE == 0 ? H / 32 : H / BN16;
   const int num_tiles = num_m * num_n;
   const int num_kb = (MODE == 0 ? H : 4 * H) / BK16;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], C::EW * 2); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  cluster_sync_all();
-  if (warp == 1) tmem_alloc_cg2(tmem_slot, 2 * BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ===== TMA producer: this CTA's 128 rows of A and its half of the B tile; all transactions of the pair
-      // complete on the LEADER's full barrier
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
+      // ===== TMA producer: 128 rows of A, 128 rows of B per k-block
       int s = 0; uint32_t ph = 0;
-      for (int tile = cta; tile < num_tiles; tile += ncta) {
-        const int m0 = (tile / num_n) * 2 * BM16 + (int)rank * BM16;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM16;
         const int nt = tile % num_n;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[s], ph ^ 1);
           uint8_t* sa = smem + s * STAGE16;
           uint8_t* sb = sa + 16384;
-          const uint32_t bar = mapa_u32(smem_u32(&full[s]), 0);
-          if (leader) mbar_expect_tx(&full[s], 2 * STAGE16);
-          tma_load_2d_cg2(sa, &tmA, bar, kb * BK16, m0);
+          mbar_expect_tx(&full[s], STAGE16);
+          tma_load_2d(sa, &tmA, &full[s], kb * BK16, m0);
           if (MODE == 0) {
-            // tile columns = [i | f | o | g] of 64 hidden units: the leader stages gate blocks i,f, the peer o,g
+            // tile columns = [i | f | o | g] of 32 hidden units
 #pragma unroll
-            for (int g = 0; g < 2; ++g)
-              tma_load_2d_cg2(sb + g * 8192, &tmB, bar, kb * BK16, ((int)rank * 2 + g) * H + nt * 64);
+            for (int g = 0; g < 4; ++g) tma_load_2d(sb + g * 4096, &tmB, &full[s], kb * BK16, g * H + nt * 32);
           } else {
-            tma_load_2d_cg2(sb, &tmB, bar, kb * BK16, nt * BN + (int)rank * 128);
+            tma_load_2d(sb, &tmB, &full[s], kb * BK16, nt * BN16);
           }
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1 && !leader) {
-    // peer CTA: its MMA warp only takes part in TMEM alloc / dealloc
-  } else if (warp == 1) {
-    // ===== MMA issuer (leader CTA) =====
-    constexpr uint32_t idesc = make_idesc_f16(2 * BM16, BN, 0, 0);
+  } else {
+    const int cw = warp - 4, wg = cw >> 2;
+    const int q = cw & 3;
+    const int half = cw >> 2;
+    uint8_t* stg = stg_all + cw * C::STG_PER_WARP;
+    const float* arow = acc + q * 32 + lane;
     int s = 0; uint32_t ph = 0;
-    int it = 0;
-    for (int tile = cta; tile < num_tiles; tile += ncta, ++it) {
-      const int buf = it & 1;
-      const uint32_t bph = (it >> 1) & 1;
-      mbar_wait(&tempty[buf], bph ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * BN;
+    // main loop of one tile: this warpgroup's 64 rows x 128 columns, then the accumulator tile in shared memory
+    auto contract = [&]() {
+      float d[BN16 / 2];
+#pragma unroll
+      for (int i = 0; i < BN16 / 2; ++i) d[i] = 0.f;
+      int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&full[s], ph);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = smem_u32(smem + s * STAGE16);
-          const uint64_t adesc = make_desc(sa, 16, 1024);
-          const uint64_t bdesc = make_desc(sa + 16384, 16, 1024);
+        const uint32_t sa = smem_u32(smem + s * STAGE16);
+        const uint64_t adesc = make_desc(sa + wg * 64 * 128, 16, 1024), bdesc = make_desc(sa + 16384, 16, 1024);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK16 / UK16; ++k)
-            umma_f16_cg2(d_tmem, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-          umma_commit_cg2(&empty[s]);
-          if (kb == num_kb - 1) umma_commit_cg2(&tfull[buf]);
-        }
-        __syncwarp();
+        for (int k = 0; k < BK16 / UK16; ++k)
+          wgmma_f16_n128(d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
-    }
-  } else {
-    // ===== epilogue: warps 2..9; TMEM lane quarter = warp % 4, column half = (warp - 2) / 4 =====
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    uint8_t* stg = stg_all + (warp - 2) * C::STG_PER_WARP;
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      bar_named(1, 32 * EW16);                       // the previous tile's epilogue is done with the accumulator tile
+      acc_store(acc, d, wg * 64);
+      bar_named(1, 32 * EW16);
+    };
     if constexpr (MODE == 0) {
-      // ---- forward.  64 hidden units per tile = four column groups of 16; the four warps of a TMEM lane quarter take one
-      // group each.  Per tile and warp: inputs (x-projection rows gathered from the fp16 table, previous cell) -> staging by
-      // cp.async (issued before the accumulator is awaited), TMEM + staging -> gates / c / h in place, out by TMA.
-      const int grp = (warp - 2) >> 2;
-      float* sBias = reinterpret_cast<float*>(stg_all + C::EW * C::STG_PER_WARP);
-      for (int i = (int)threadIdx.x - 64; i < 4 * H; i += 32 * C::EW) sBias[i] = __ldg(p.bias + i);
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * C::EW) : "memory");          // epilogue warps only
+      // ---- forward.  32 hidden units per tile = two column groups of 16; the two warps of a 32-row quarter take one group
+      // each.  Per tile and warp: inputs (x-projection rows gathered from the fp16 table, previous cell) -> staging by
+      // cp.async (issued before the contraction), accumulator + staging -> gates / c / h in place, out by TMA.
+      const int grp = half;
       uint8_t* sG = stg; uint8_t* sC = stg + 4 * S32_BYTES; uint8_t* sH = sC + S64_BYTES;
-      int it = 0;
-      for (int tile = cta; tile < num_tiles; tile += ncta, ++it) {
-        const int buf = it & 1;
-        const uint32_t bph = (it >> 1) & 1;
-        const int m0 = (tile / num_n) * 2 * BM16 + (int)rank * BM16;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM16;
         const int nt = tile % num_n;
         const int64_t row = (int64_t)m0 + q * 32 + lane;
         const bool row_ok = row < p.R;
         const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
         const int r0 = m0 + q * 32;
-        const int j = nt * 64 + grp * 16;                      // first hidden unit of this warp's group
-        const uint32_t taddr = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16) + grp * 16;
+        const int j = nt * 32 + grp * 16;                      // first hidden unit of this warp's group
         // A pad token's x-projection is exactly zero (LookupTableMaskZero: embedding row 0 is zero, and the table carries no
-        // bias), so finished sequences skip the gather: late time steps, where most of the 100 x 20-token options have ended,
-        // would otherwise send every row of the machine to the same 4 KB of L2 (measured: 143 us at t = 1 -> 219 us at t = 19)
+        // bias), so finished sequences skip the gather: at late time steps most of the 100 x 20-token options have ended, and
+        // every row would otherwise read the same 4 KB of L2
         const int32_t tk = row_ok ? __ldg(p.tok + row) : 0;
         const __half* prow = tk != 0 ? p.ptable + (int64_t)tk * 4 * H + j : nullptr;
         const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H + j : nullptr;
@@ -297,22 +254,20 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
 #pragma unroll
         for (int g = 0; g < 4; ++g) s32_load(sG + g * S32_BYTES, prow ? prow + g * H : nullptr, lane);
         s64_load(sC, cprow, lane);
-        mbar_wait(&tfull[buf], bph);                           // the loads fly while the MMAs of this tile finish
-        tc_fence_after();
+        contract();                                            // the loads fly while the MMAs of this tile run
         cp_wait_all();
 #pragma unroll 1
         for (int sub = 0; sub < 2; ++sub) {
           float a[4][8], cp[8], hn[8];
 #pragma unroll
-          for (int g = 0; g < 4; ++g) tmem_ld8(taddr + g * 64 + sub * 8, a[g]);
-          tmem_ld_wait();
+          for (int g = 0; g < 4; ++g) acc_ld8(arow, g * 32 + grp * 16 + sub * 8, a[g]);
           s64_get8(sC, lane, sub, cp);
 #pragma unroll
           for (int g = 0; g < 4; ++g) {
             float x[8];
             unpack8(*s32_at(sG + g * S32_BYTES, lane, sub), x);
-            const float4 b0 = *reinterpret_cast<const float4*>(sBias + g * H + j + sub * 8);
-            const float4 b1 = *reinterpret_cast<const float4*>(sBias + g * H + j + sub * 8 + 4);
+            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + g * H + j + sub * 8));
+            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + g * H + j + sub * 8 + 4));
             a[g][0] += x[0] + b0.x; a[g][1] += x[1] + b0.y; a[g][2] += x[2] + b0.z; a[g][3] += x[3] + b0.w;
             a[g][4] += x[4] + b1.x; a[g][5] += x[5] + b1.y; a[g][6] += x[6] + b1.z; a[g][7] += x[7] + b1.w;
           }
@@ -333,12 +288,9 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
             o[1] = make_float4(hn[4], hn[5], hn[6], hn[7]);
           }
         }
-        tc_fence_before();                            // the accumulator has been read: hand it back before the stores leave
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) {
-          if (!leader) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[buf]), 0));
-          else mbar_arrive(&tempty[buf]);
           if (p.save_gates) {
 #pragma unroll
             for (int g = 0; g < 4; ++g) tma_store_2d(&em.g16, sG + g * S32_BYTES, g * H + j, r0);
@@ -350,32 +302,27 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
         __syncwarp();
       }
     } else {
-    int it = 0;
-    for (int tile = cta; tile < num_tiles; tile += ncta, ++it) {
-      const int buf = it & 1;
-      const uint32_t bph = (it >> 1) & 1;
-      const int m0 = (tile / num_n) * 2 * BM16 + (int)rank * BM16;
-      const int nt = tile % num_n;
-      const int64_t row = (int64_t)m0 + q * 32 + lane;
-      const bool row_ok = row < p.R;
-      const bool masked = row_ok && p.mask_ids && p.mask_ids[row] == 0;
-      const float keep = masked ? 0.f : 1.f;
-      const int r0 = m0 + q * 32;
-      const uint32_t taddr = tmem_base + buf * BN + ((uint32_t)(q * 32) << 16);
-      {
-        // ---- backward: 256 hidden units per tile, the warp's column slice = 256 / (EW/4) of them, in groups of 16
-        constexpr int NSL = C::EW / 4, GPW = 256 / NSL / 16;      // column slices per tile, groups per warp
-        const int j0 = nt * 256 + half * (256 / NSL);
+      // ---- backward: 128 hidden units per tile, the warp's column slice = 64 of them, in groups of 16
+      constexpr int NSL = EW16 / 4, GPW = BN16 / NSL / 16;      // column slices per tile, groups per warp
+      uint8_t* sG = stg; uint8_t* sCP = stg + 4 * S32_BYTES; uint8_t* sCC = sCP + S64_BYTES; uint8_t* sDC = sCC + S64_BYTES;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / num_n) * BM16;
+        const int nt = tile % num_n;
+        const int64_t row = (int64_t)m0 + q * 32 + lane;
+        const bool row_ok = row < p.R;
+        const bool masked = row_ok && p.mask_ids && p.mask_ids[row] == 0;
+        const float keep = masked ? 0.f : 1.f;
+        const int r0 = m0 + q * 32;
+        const int j0 = nt * BN16 + half * (BN16 / NSL);
         const __half* grow = row_ok ? p.gsave + row * 4 * H : nullptr;
         const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H : nullptr;
         const float* ccrow = row_ok ? p.c_cur + row * H : nullptr;
         const float* dcrow = row_ok ? p.dc_carry + row * H : nullptr;
-        uint8_t* sG = stg; uint8_t* sCP = stg + 4 * S32_BYTES; uint8_t* sCC = sCP + S64_BYTES; uint8_t* sDC = sCC + S64_BYTES;
-        bool waited = false;
+        contract();
 #pragma unroll 1
         for (int grp = 0; grp < GPW; ++grp) {
           const int j = j0 + grp * 16;
-          const int tc0 = half * (256 / NSL) + grp * 16;
+          const int tc0 = half * (BN16 / NSL) + grp * 16;
           if (lane == 0) bulk_wait_read0();
           __syncwarp();
 #pragma unroll
@@ -383,13 +330,11 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
           s64_load(sCP, cprow ? cprow + j : nullptr, lane);
           s64_load(sCC, ccrow ? ccrow + j : nullptr, lane);
           s64_load(sDC, dcrow ? dcrow + j : nullptr, lane);
-          if (!waited) { mbar_wait(&tfull[buf], bph); tc_fence_after(); waited = true; }
           cp_wait_all();
 #pragma unroll 1
           for (int sub = 0; sub < 2; ++sub) {
             float dh[8], g[4][8], cp[8], cc[8], dc[8], out[4][8], dcn[8];
-            tmem_ld8(taddr + tc0 + sub * 8, dh);
-            tmem_ld_wait();
+            acc_ld8(arow, tc0 + sub * 8, dh);
 #pragma unroll
             for (int gg = 0; gg < 4; ++gg) unpack8(*s32_at(sG + gg * S32_BYTES, lane, sub), g[gg]);
             s64_get8(sCP, lane, sub, cp);
@@ -422,33 +367,24 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
           __syncwarp();
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                                // the accumulator buffer may be overwritten by the leader's MMAs
-        if (!leader) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty[buf]), 0));
-        else mbar_arrive(&tempty[buf]);
-      }
-    }
     }
     if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
   }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc_cg2(tmem_base, 2 * BN); }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Weight gradient of the recurrent block:  C[m,n] += inv_scale * sum_k A[k,m] B[k,n],  A = h (K rows x H) fp16,
 // B = da (K rows x 4H) fp16 — both MN-major (the contraction index is the row index in HBM).  A TMA box of 64 columns
 // x KB rows lands as KB rows of 128 bytes = the canonical MN-major SWIZZLE_128B layout (8 k-rows per 1024-byte atom:
-// SBO = 1024; 64-column groups LBO bytes apart); one K = 16 instruction consumes two atoms.
+// SBO = 1024; 64-column groups LBO bytes apart), which the f16 wgmma reads transposed; one K = 16 instruction consumes
+// two atoms.  Warpgroup 0 = TMA producer, warpgroups 1-2 = consumers (64 columns of A each).
 constexpr int A16_KB = 64;                 // k-rows per stage (4 MMAs)
-constexpr int A16_BN = 256;
-constexpr int A16_THREADS = 192;
+constexpr int A16_BN = 128;
+constexpr int A16_THREADS = 384;
 constexpr int A16_A_BYTES = 2 * A16_KB * 128;              // 128 columns of A = 2 boxes
-constexpr int A16_B_BYTES = (A16_BN / 64) * A16_KB * 128;  // 4 boxes
-constexpr int A16_STAGE = A16_A_BYTES + A16_B_BYTES;       // 48 KB
-constexpr int A16_STAGES = 4;
+constexpr int A16_B_BYTES = (A16_BN / 64) * A16_KB * 128;  // 2 boxes
+constexpr int A16_STAGE = A16_A_BYTES + A16_B_BYTES;       // 32 KB
+constexpr int A16_STAGES = 6;
 constexpr int A16_TOTAL = A16_STAGES * A16_STAGE + 1024 + 256;
 struct Atb16Params { int M, N; int64_t K, k_per_split; float* C; int64_t ldc; const float* inv_scale; };
 
@@ -458,9 +394,7 @@ k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full = (uint64_t*)(smem + A16_STAGES * A16_STAGE);
   uint64_t* empty = full + A16_STAGES;
-  uint64_t* tfull = empty + A16_STAGES;
-  uint32_t* tmem_slot = (uint32_t*)(tfull + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
   const int num_n = (p.N + A16_BN - 1) / A16_BN;
   const int m0 = (blockIdx.x / num_n) * BM16, n0 = (blockIdx.x % num_n) * A16_BN;
   const int64_t kbeg = (int64_t)blockIdx.y * p.k_per_split;
@@ -468,18 +402,13 @@ k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
   const int num_kb = (int)((kend - kbeg + A16_KB - 1) / A16_KB);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < A16_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(tfull, 1);
+    for (int s = 0; s < A16_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, A16_BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (threadIdx.x == 0) {
       int s = 0; uint32_t ph = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
@@ -494,57 +423,45 @@ k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         if (++s == A16_STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_f16(BM16, A16_BN, 1, 1);
-    int s = 0; uint32_t ph = 0;
+  } else if (num_kb > 0) {
+    const int wg = (warp - 4) >> 2;
+    float d[A16_BN / 2];
+#pragma unroll
+    for (int i = 0; i < A16_BN / 2; ++i) d[i] = 0.f;
+    int s = 0; uint32_t ph = 0; int prev = -1;
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full[s], ph);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t sa = smem_u32(smem + s * A16_STAGE);
-        const uint32_t sb = sa + A16_A_BYTES;
+      const uint32_t sa = smem_u32(smem + s * A16_STAGE);
+      const uint32_t sb = sa + A16_A_BYTES;
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < A16_KB / UK16; ++k) {
-          const uint64_t adesc = make_desc(sa + k * 2048, A16_KB * 128, 1024, 2);
-          const uint64_t bdesc = make_desc(sb + k * 2048, A16_KB * 128, 1024, 2);
-          umma_f16(tmem_base, adesc, bdesc, idesc, (kb | k) ? 1u : 0u);
-        }
-        umma_commit(&empty[s]);
-        if (kb == num_kb - 1) umma_commit(tfull);
-      }
-      __syncwarp();
+      for (int k = 0; k < A16_KB / UK16; ++k)
+        wgmma_f16_n128_mn(d, make_desc(sa + wg * A16_KB * 128 + k * 2048, A16_KB * 128, 1024),
+                          make_desc(sb + k * 2048, A16_KB * 128, 1024), (kb | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      prev = s;
       if (++s == A16_STAGES) { s = 0; ph ^= 1; }
     }
-  } else if (num_kb > 0) {
-    const int q = warp & 3;
+    wgmma_wait<0>();
+    wgmma_hold(d);
     const float sc = p.inv_scale ? __ldg(p.inv_scale) : 1.f;
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    const int m = m0 + q * 32 + lane;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-    for (int c = 0; c < A16_BN; c += 8) {
-      if (n0 + c >= p.N) break;
-      float v[8];
-      tmem_ld8(taddr + c, v);
-      tmem_ld_wait();
-      if (m < p.M) {
-        float* crow = p.C + (int64_t)m * p.ldc + n0 + c;
-        if (n0 + c + 8 <= p.N && ((p.ldc & 3) == 0)) {
-          red_add_v4(crow, v[0] * sc, v[1] * sc, v[2] * sc, v[3] * sc);
-          red_add_v4(crow + 4, v[4] * sc, v[5] * sc, v[6] * sc, v[7] * sc);
-        } else {
+    const int lane = threadIdx.x & 31, w = warp & 3;
+    const int r0 = m0 + wg * 64 + 16 * w + (lane >> 2), c0 = n0 + 2 * (lane & 3);
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            if (n0 + c + j < p.N) atomicAdd(crow + j, v[j] * sc);
+    for (int j = 0; j < A16_BN / 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = r0 + 8 * h, n = c0 + 8 * j;
+        if (m < p.M && n < p.N) {            // M, N multiples of 64
+          float* crow = p.C + (int64_t)m * p.ldc + n;
+          atomicAdd(crow, d[4 * j + 2 * h] * sc);
+          atomicAdd(crow + 1, d[4 * j + 2 * h + 1] * sc);
         }
       }
-      __syncwarp();
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, A16_BN); }
 }
 
 // ------------------------------------------------------------------------------------------------ streaming helpers
@@ -746,25 +663,16 @@ static void launch16(LaunchCtx& cx, const CUtensorMap& tA, const CUtensorMap& tB
     attr_set = true;
   }
   // persistent, balanced waves (see gemm_tc.cu::launch)
-  const int pmax = cx.sms() / 2;
-  int pairs = num_tiles;
-  if (num_tiles > pmax) { const int rounds = cdiv(num_tiles, pmax); pairs = cdiv(num_tiles, rounds); }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(C::THREADS);
-  cfg.dynamicSmemBytes = C::TOTAL;
-  cfg.stream = cx.stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  VD_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_lstm16<MODE>, tA, tB, em, p));
+  const int pmax = cx.sms();
+  int grid = num_tiles;
+  if (num_tiles > pmax) { const int rounds = cdiv(num_tiles, pmax); grid = cdiv(num_tiles, rounds); }
+  k_lstm16<MODE><<<grid, C::THREADS, C::TOTAL, cx.stream>>>(tA, tB, em, p);
   check_launch(cx, "k_lstm16");
 }
 
 }  // namespace tc
 
-bool lstm16_shape_ok(int64_t R, int H) { return H % 256 == 0 && H <= 512 && R >= 1024; }   // the forward kernel keeps the 4H bias in 8 KB of shared memory
+bool lstm16_shape_ok(int64_t R, int H) { return H % 256 == 0 && H <= 512 && R >= 1024; }
 
 void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, const __half* Wh16, const __half* ptable16,
                      const int32_t* tok, const float* bias, const float* c_prev, const int32_t* mask_ids, __half* gates16,
@@ -775,13 +683,13 @@ void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, co
   p.R = (int)R; p.H = H; p.ptable = ptable16; p.tok = tok; p.bias = bias; p.c_prev = c_prev; p.mask_ids = mask_ids;
   p.h32_out = h32_out; p.save_gates = gates16 != nullptr;
   CUtensorMap tA = tmap_h(h_prev16, R, H, H, BM16, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
-  CUtensorMap tB = tmap_h(Wh16, 4 * (int64_t)H, H, H, 64, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
+  CUtensorMap tB = tmap_h(Wh16, 4 * (int64_t)H, H, H, 32, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
   Lstm16Maps em;
   em.g16 = gates16 ? tmap_h(gates16, R, 4 * (int64_t)H, 4 * (int64_t)H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B)
                    : tmap_h(h16_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B);
   em.c = tmap_f(c_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
   em.h16 = tmap_h(h16_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B);
-  launch16<0>(cx, tA, tB, em, p, cdiv(R, 2 * BM16) * (H / 64));
+  launch16<0>(cx, tA, tB, em, p, cdiv(R, BM16) * (H / 32));
 }
 
 void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, const __half* Whb16, const __half* gates16,
@@ -796,7 +704,7 @@ void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, c
   em.g16 = tmap_h(da16, R, 4 * (int64_t)H, 4 * (int64_t)H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B);
   em.c = tmap_f(dc_carry, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
   em.h16 = em.c;
-  launch16<1>(cx, tA, tB, em, p, cdiv(R, 2 * BM16) * (H / 256));
+  launch16<1>(cx, tA, tB, em, p, cdiv(R, BM16) * (H / BN16));
 }
 
 void lstm16_first_step(LaunchCtx& cx, int64_t R, int H, const __half* ptable16, const int32_t* tok, const float* bias,
@@ -827,7 +735,7 @@ void cvt_f32_to_f16(LaunchCtx& cx, __half* dst, int64_t ldd, const float* src, i
 void pick_grad_scale(LaunchCtx& cx, const float* x, int64_t n, uint32_t* bits, float* scale2) {
   VD_REQUIRE(n % 4 == 0, VD_E_STATE, "pick_grad_scale: n % 4");
   VD_CUDA_CHECK(cudaMemsetAsync(bits, 0, sizeof(uint32_t), cx.stream));
-  const int blocks = (int)std::min<int64_t>((n / 4 + 255) / 256, 4 * 148);
+  const int blocks = (int)std::min<int64_t>((n / 4 + 255) / 256, 4 * cx.sm_count);
   tc::k_amax<<<blocks, 256, 0, cx.stream>>>(x, n / 4, bits);
   check_launch(cx, "k_amax");
   tc::k_pick_scale<<<1, 1, 0, cx.stream>>>(bits, scale2);

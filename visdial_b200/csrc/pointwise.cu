@@ -1255,7 +1255,7 @@ void segsum_rows(LaunchCtx& cx, const float* X, int64_t ldx, const int32_t* perm
   check_launch(cx, "k_segsum_rows");
 }
 void fill_l2_flush(LaunchCtx& cx, float* buf, int64_t n) {
-  k_fill<<<148 * 8, 256, 0, cx.stream>>>(buf, n, 0.f);
+  k_fill<<<cx.sm_count * 8, 256, 0, cx.stream>>>(buf, n, 0.f);
   check_launch(cx, "fill_l2_flush");
 }
 
