@@ -213,6 +213,23 @@ int vd_gemm_atb(vd_engine* e, int32_t M, int32_t N, int64_t K, const float* A, i
  * fp16, then C[m,n] += inv_scale * sum_k A[k,m] B[k,n] on f16 wgmma (both operands MN-major). */
 int vd_gemm_atb16(vd_engine* e, int32_t M, int32_t N, int64_t K, const float* A, int64_t lda, const float* B, int64_t ldb,
                   float* C, int64_t ldc, float inv_scale);
+/* test hooks of one SeqLSTM time step on caller-provided DEVICE buffers (fp32, row-major), routed exactly as the engine
+ * routes a step in its math mode: the fused tensor-core step kernel when it takes the shape, otherwise the recurrent GEMM
+ * and the pointwise kernel.  *path receives the tile width of the fused kernel that ran, or 0 for CUDA cores.
+ * fwd: z[r] = bias + (has_xproj ? gates[r] : ptable[tok[r]]) + h_prev[r] WhT^T      (h_prev NULL: no recurrent term)
+ *      gates <- [sigmoid(z_i) sigmoid(z_f) sigmoid(z_o) tanh(z_g)],  c_out = f c_prev + i g,  h_out = o tanh(c_out);
+ *      WhT (4H, ldw) = the h columns of the transposed weight; ptable (ptable_rows, 4H) is a gathered x-projection, which
+ *      only the tensor-core route takes; c_prev NULL = zeros; rows whose mask id is 0 are all zero.
+ * bwd: dh = da_next[r] Wh^T + dh_ext[r],  d = dc_carry + dh o (1 - tanh^2 c_cur),
+ *      da <- [d g i(1-i)  d c_prev f(1-f)  dh tanh(c_cur) o(1-o)  d i(1-g^2)],  dc_carry <- d f;
+ *      Wh (H, 4H) = the h rows of the weight; da_next / dh_ext / c_prev NULL = zeros; masked rows all zero.
+ * The fp16 option-LSTM steps of VD_MATH_F16 are not reachable through these hooks (an error). */
+int vd_lstm_step_fwd(vd_engine* e, int64_t R, int32_t H, const float* h_prev, const float* WhT, int64_t ldw, const float* bias,
+                     float* gates, int32_t has_xproj, const float* ptable, int64_t ptable_rows, const int32_t* tok,
+                     const float* c_prev, float* c_out, float* h_out, const int32_t* mask_ids, int32_t* path);
+int vd_lstm_step_bwd(vd_engine* e, int64_t R, int32_t H, const float* da_next, const float* Wh, const float* gates,
+                     const float* c_prev, const float* c_cur, const float* dh_ext, float* dc_carry, const int32_t* mask_ids,
+                     float* da, int32_t* path);
 /* cudaProfilerStart / cudaProfilerStop (ncu --profile-from-start off) */
 int vd_profiler_range(vd_engine* e, int32_t start);
 /* flush L2 by writing a scratch buffer larger than L2 (bench hygiene) */

@@ -62,3 +62,43 @@ def flat_from_named(params, named):
 def seg_slices(params):
     segs, _ = E.layout(params)
     return {s.name: slice(s.offset, s.offset + s.size) for s in segs}
+
+
+def lstm_step_fwd_ref(z_x, h_prev, Wh, c_prev, mask):
+    """One nn.SeqLSTM forward step in fp64 numpy.  z_x (R,4H): x-projection + bias; h_prev (R,H) or None;
+    Wh (H,4H): the h rows of the (D+H,4H) weight; c_prev (R,H) or None; mask (R,) bool = rows reset to zero.
+    Returns the activated gates [i f o g] (R,4H), c_t and h_t."""
+    z = np.asarray(z_x, np.float64).copy()
+    H = z.shape[1] // 4
+    if h_prev is not None:
+        z += np.asarray(h_prev, np.float64) @ np.asarray(Wh, np.float64)
+    a = np.empty_like(z)
+    a[:, :3 * H] = 1.0 / (1.0 + np.exp(-z[:, :3 * H]))
+    a[:, 3 * H:] = np.tanh(z[:, 3 * H:])
+    i, f, o, g = a[:, :H], a[:, H:2 * H], a[:, 2 * H:3 * H], a[:, 3 * H:]
+    cp = np.zeros_like(i) if c_prev is None else np.asarray(c_prev, np.float64)
+    c = f * cp + i * g
+    h = o * np.tanh(c)
+    if mask is not None:
+        a[mask] = 0
+        c[mask] = 0
+        h[mask] = 0
+    return a, c, h
+
+
+def lstm_step_bwd_ref(gates, c_prev, c_cur, dh, dc, mask):
+    """The matching backward step: gates = activated [i f o g] of step t, dh = gradient wrt h_t (recurrent + external),
+    dc = cell-gradient carry from step t+1.  Returns da_t (R,4H) and the carry for step t-1."""
+    a = np.asarray(gates, np.float64)
+    H = a.shape[1] // 4
+    i, f, o, g = a[:, :H], a[:, H:2 * H], a[:, 2 * H:3 * H], a[:, 3 * H:]
+    cp = np.zeros_like(i) if c_prev is None else np.asarray(c_prev, np.float64)
+    tc = np.tanh(np.asarray(c_cur, np.float64))
+    dh = np.asarray(dh, np.float64)
+    d = np.asarray(dc, np.float64) + dh * o * (1 - tc * tc)
+    da = np.concatenate([d * g * i * (1 - i), d * cp * f * (1 - f), dh * tc * o * (1 - o), d * i * (1 - g * g)], axis=1)
+    dc_prev = d * f
+    if mask is not None:
+        da[mask] = 0
+        dc_prev[mask] = 0
+    return da, dc_prev

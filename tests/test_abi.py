@@ -112,6 +112,18 @@ def test_bad_arguments_return_error_codes():
         encoders.load("no-such-encoder")
 
 
+@pytest.mark.parametrize("field,value", [("embedSize", 30), ("rnnHiddenSize", 100)])
+def test_sizes_the_kernels_cannot_take_are_refused_at_configuration(field, value):
+    """every LSTM input width is a sum of embedSize / rnnHiddenSize / imgEmbedSize / imgFeatureSize, so these checks are what
+    keeps every [4H, D+H] weight's h columns 16-byte aligned for the tensor-core step kernels"""
+    lib = _lib.load()
+    p = small_params("hre-ques-im-hist", "gen", **{field: value})
+    cp = E.to_c_params(p)
+    n = C.c_int64()
+    assert lib.vd_layout_count(C.byref(cp), None, C.byref(n)) == -1
+    assert b"multiples of 4" in lib.vd_last_error()
+
+
 def test_fails_loudly_without_a_gpu():
     """No CPU fallback: creating an engine on a box without an H100 is an error, not a silent CPU path."""
     import torch

@@ -9,7 +9,7 @@ import torch
 
 from oracle import philox
 from oracle import visdial_oracle as O
-from helpers import CONFIGS, small_batch, small_params, torch_batch, torch_params
+from helpers import CONFIGS, lstm_step_bwd_ref, lstm_step_fwd_ref, small_batch, small_params, torch_batch, torch_params
 from visdial_b200 import engine as E
 
 
@@ -66,6 +66,45 @@ def test_lstm_manual_bptt_matches_autograd(maskzero):
         h = grads[0][5]
         assert float(h[0, 1].abs().max()) == 0 and float(h[3, 3].abs().max()) == 0
         assert float(h[4, 3].abs().max()) > 0                  # restarts from zero state afterwards
+
+
+def test_numpy_lstm_step_matches_the_oracle():
+    """The fp64 numpy step the tensor-core step kernels are checked against (tests/helpers.py), chained over T steps,
+    gives the oracle's SeqLSTM outputs and, through the backward steps, its weight / bias / initial-state gradients."""
+    torch.manual_seed(3)
+    T, N, D, H = 4, 6, 5, 8
+    x = torch.randn(T, N, D, dtype=torch.float64)
+    x[0, 1] = 0; x[2, 4] = 0; x[3, 0] = 0                       # masked rows: first, mid-sequence, last step
+    W = torch.randn(D + H, 4 * H, dtype=torch.float64) * 0.4
+    b = torch.randn(4 * H, dtype=torch.float64) * 0.2
+    h0 = torch.randn(N, H, dtype=torch.float64)
+    c0 = torch.randn(N, H, dtype=torch.float64)
+    gh = torch.randn(T, N, H, dtype=torch.float64)
+    gc = torch.randn(T, N, H, dtype=torch.float64)
+    leaves = [t.clone().requires_grad_(True) for t in (W, b, h0, c0)]
+    h, c = O.seq_lstm(x, leaves[0], leaves[1], leaves[2], leaves[3], maskzero=True)
+    ((h * gh).sum() + (c * gc).sum()).backward()
+    Wn, bn, xn = W.numpy(), b.numpy(), x.numpy()
+    mask = xn.__abs__().sum(-1) == 0
+    gates, cs, hs = [], [], []
+    hp, cp = h0.numpy(), c0.numpy()
+    for t in range(T):
+        a, ct, ht = lstm_step_fwd_ref(xn[t] @ Wn[:D] + bn, hp, Wn[D:], cp, mask[t])
+        assert np.allclose(ht, h[t].detach().numpy(), atol=1e-12) and np.allclose(ct, c[t].detach().numpy(), atol=1e-12)
+        gates.append(a); cs.append(ct); hs.append(ht)
+        hp, cp = ht, ct
+    dW, db = np.zeros_like(Wn), np.zeros_like(bn)
+    dh_next, dc = np.zeros((N, H)), np.zeros((N, H))
+    for t in range(T - 1, -1, -1):
+        prev_h = hs[t - 1] if t else h0.numpy()
+        prev_c = cs[t - 1] if t else c0.numpy()
+        da, dc = lstm_step_bwd_ref(gates[t], prev_c, cs[t], gh[t].numpy() + dh_next, gc[t].numpy() + dc, mask[t])
+        dW[:D] += xn[t].T @ da
+        dW[D:] += prev_h.T @ da
+        db += da.sum(0)
+        dh_next = da @ Wn[D:].T
+    for got, ref in ((dW, leaves[0]), (db, leaves[1]), (dh_next, leaves[2]), (dc, leaves[3])):
+        assert np.allclose(got, ref.grad.numpy(), atol=1e-10, rtol=1e-10)
 
 
 def test_lstm_finite_difference():

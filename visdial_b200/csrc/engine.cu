@@ -363,7 +363,7 @@ void Engine::lstm_forward_begin(LstmRun& r, bool save) {
   // computed once per forward (E Wx^T: the 300-wide half of every step's contraction collapses into a
   // gather in the step epilogue); a dense input keeps the batched x-projection.  Each step is then ONE fused
   // kernel: recurrent wgmma GEMM + SeqLSTM pointwise epilogue.
-  r.tc = tcmode() && H % 64 == 0;
+  r.tc = tcmode() && lstm_step_fwd_tc_ok(H, WtS + D, D + H);
   r.ptable = nullptr;
   // VD_MATH_F16: a many-row LSTM over embedding-gathered tokens (the option LSTM) keeps h, the activated gates, da and
   // the projection table in fp16 and runs kind::f16 contractions (lstm16.cu); c, the accumulators and h_T stay fp32
@@ -542,7 +542,9 @@ void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaSt
     enc_pair_forward(cx, T, R, H, W1h, W2c, Wp(l2.wseg + 1), l1.mask, l1.gates, l1.c, l1.h, l1.h16, l2.gates, l2.c, l2.h, l2.h16, flags);
     return;
   }
-  const bool pipelined = tcmode() && l2.H % 64 == 0 && sb != nullptr && sb != sa && l2.R >= wavefront_min_rows();
+  // layer 2 projects its input per step on the tensor-core step path only (a batched projection would read h1 before it exists)
+  const bool pipelined = tcmode() && lstm_step_fwd_tc_ok(l2.H, Wtp(l2.wseg) + l2.D, l2.D + l2.H) && sb != nullptr && sb != sa &&
+                         l2.R >= wavefront_min_rows();
   const bool three = pipelined && sc != nullptr && sc != sa && sc != sb && three_streams_enabled();
   cx.stream = sa;
   if (!pipelined) {
@@ -603,7 +605,7 @@ void Engine::lstm_backward_begin(LstmRun& r, const float* dh_all, const float* d
     pick_grad_scale(cx, dh_last, R * H, reinterpret_cast<uint32_t*>(r.scale2 + 2), r.scale2);
     return;
   }
-  r.bw_tc = tcmode() && H % 128 == 0;
+  r.bw_tc = tcmode() && lstm_step_bwd_tc_ok(H, Wp(r.wseg) + (int64_t)r.D * G);
   if (r.bw_tc && dc_last)
     VD_CUDA_CHECK(cudaMemcpyAsync(r.dc_carry, dc_last, (size_t)R * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
   else

@@ -573,6 +573,9 @@ bool gemm_tn_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda,
   using namespace tc;
   if (a_gather) return false;                               // gathered rows go through the projection table instead
   if (M < 64 || N < 16 || K < 32) return false;             // tiny contractions stay on CUDA cores
+  // N % 4: the TMA store of C clips the box at N only in whole 16-byte chunks — with N % 4 != 0 it writes zeros into
+  // the (up to 3) columns of each row past N, which belong to the caller when ldc > N
+  if (N % 4 != 0) return false;
   if (!tma_ok(A, lda) || !tma_ok(B, ldb) || !tma_ok(C, ldc)) return false;
   Params p = {};
   p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.beta = beta; p.bias = bias; p.act = act;
@@ -618,11 +621,16 @@ bool gemm_atb_tc(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t
 // Vocabulary projection with the softmax statistics fused into the epilogue (no (rows, V) tensor in HBM):
 //   part_max / part_sum (M, nparts): per column slice running max and sum of exp(x - max);  tgt_logit[m] = x[m, tgt[m]-1]
 int vocab_lse_nparts(int N) { return cdiv(N, 128) * (tc::EPI_WARPS / 4); }
+// The shapes both halves of the fused vocabulary softmax take.  The backward writes its (M, N) d-logits with row pitch N
+// through TMA, so N must be a multiple of 4; the forward refuses that shape too, because once it has taken a shape the
+// logits are never materialised and the backward has no other route.
+bool vocab_tc_ok(int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb) {
+  return M >= 64 && N >= 256 && N % 4 == 0 && K >= 32 && tc::tma_ok(A, lda) && tc::tma_ok(B, ldb);
+}
 bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
                   const int32_t* tgt, float* part_max, float* part_sum, float* tgt_logit) {
   using namespace tc;
-  if (M < 64 || N < 256 || K < 32) return false;
-  if (!tma_ok(A, lda) || !tma_ok(B, ldb)) return false;
+  if (!vocab_tc_ok(M, N, K, A, lda, B, ldb)) return false;
   Params p = {};
   p.M = M; p.N = N; p.K = K; p.bias = bias; p.tgt = tgt; p.part_max = part_max; p.part_sum = part_sum; p.tgt_logit = tgt_logit;
   p.nparts = vocab_lse_nparts(N);
@@ -634,8 +642,7 @@ bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t ld
 bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
                       const int32_t* tgt, const int32_t* row_ids, const float* lse, float* C, int64_t ldc) {
   using namespace tc;
-  if (M < 64 || N < 256 || K < 32) return false;
-  if (!tma_ok(A, lda) || !tma_ok(B, ldb) || !tma_ok(C, ldc)) return false;
+  if (!vocab_tc_ok(M, N, K, A, lda, B, ldb) || !tma_ok(C, ldc)) return false;
   Params p = {};
   p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.bias = bias; p.tgt = tgt; p.row_ids = row_ids; p.lse = lse;
   EpiMaps em = {};
@@ -645,14 +652,18 @@ bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_
   return true;
 }
 
+// The weights the fused forward step takes; the engine routes a SeqLSTM to lstm_step_fwd_tc only if this holds.
+bool lstm_step_fwd_tc_ok(int H, const float* WtS_h, int64_t ldw) { return H % 64 == 0 && tc::tma_ok(WtS_h, ldw); }
+
 // One SeqLSTM forward step on the tensor cores: gates = h_prev Wh^T (+ xproj | + ptable[tok]) + bias, then the
 // pointwise half, fused.  WtS_h = transposed shadow weight offset to the h columns: [4H, ld] with K = H.
+// *tile (optional) receives the tile width that ran.
 bool lstm_step_fwd_tc(LaunchCtx& cx, int64_t R, int H, const float* h_prev, const float* WtS_h, int64_t ldw, const float* bias,
                       float* gates, int has_xproj, const float* ptable, const int32_t* tok, const float* c_prev, float* c_out,
-                      float* h_out, const int32_t* mask_ids) {
+                      float* h_out, const int32_t* mask_ids, int* tile) {
   using namespace tc;
-  if (H % 64 != 0 || R < 1) return false;
-  if (!tma_ok(WtS_h, ldw) || (h_prev && !tma_ok(h_prev, H))) return false;
+  if (!lstm_step_fwd_tc_ok(H, WtS_h, ldw) || R < 1) return false;
+  if (h_prev && !tma_ok(h_prev, H)) return false;
   Params p = {};
   p.M = (int)R; p.N = 4 * H; p.K = h_prev ? H : 0; p.H = H;      // K == 0: no recurrent term (t = 0 without h0)
   if (!h_prev) h_prev = WtS_h;                                      // any valid address for the (unused) tensor map
@@ -662,21 +673,26 @@ bool lstm_step_fwd_tc(LaunchCtx& cx, int64_t R, int H, const float* h_prev, cons
   if (cdiv(R, BM) * (H / 32) >= cx.sm_count) {   // 32 hidden units (x 4 gates = 128 columns) per tile
     CUtensorMap tB = make_tmap(WtS_h, 4 * (int64_t)H, H, ldw, 32);
     launch<128, MODE_LSTM_FWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 32));
+    if (tile) *tile = 128;
   } else {                                   // few rows (encoder LSTMs): 16 hidden units per tile, 2x the CTAs
     CUtensorMap tB = make_tmap(WtS_h, 4 * (int64_t)H, H, ldw, 16);
     launch<64, MODE_LSTM_FWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 16));
+    if (tile) *tile = 64;
   }
   return true;
 }
 
+// The weights the fused backward step takes; the engine routes a SeqLSTM's BPTT to lstm_step_bwd_tc only if this holds.
+bool lstm_step_bwd_tc_ok(int H, const float* Wh) { return H % 128 == 0 && tc::tma_ok(Wh, 4 * H); }
+
 // One SeqLSTM backward step: dh_rec = da_next Wh (Wh rows = reference layout rows D.., [H, 4H]) fused with the
-// backward pointwise half producing da_t and the cell-gradient carry.
+// backward pointwise half producing da_t and the cell-gradient carry.  *tile (optional) receives the tile width that ran.
 bool lstm_step_bwd_tc(LaunchCtx& cx, int64_t R, int H, const float* da_next, const float* Wh, const float* gsave,
                       const float* c_prev, const float* c_cur, const float* dh_ext, float* dc_carry, const int32_t* mask_ids,
-                      float* da) {
+                      float* da, int* tile) {
   using namespace tc;
-  if (H % 128 != 0 || R < 1) return false;
-  if (!tma_ok(Wh, 4 * H) || (da_next && !tma_ok(da_next, 4 * H))) return false;
+  if (!lstm_step_bwd_tc_ok(H, Wh) || R < 1) return false;
+  if (da_next && !tma_ok(da_next, 4 * H)) return false;
   Params p = {};
   p.M = (int)R; p.N = H; p.K = da_next ? 4 * H : 0; p.H = H;       // K == 0: last time step, no recurrent gradient
   if (!da_next) da_next = Wh;
@@ -686,9 +702,11 @@ bool lstm_step_bwd_tc(LaunchCtx& cx, int64_t R, int H, const float* da_next, con
   if (cdiv(R, BM) * (H / 128) >= cx.sm_count) {
     CUtensorMap tB = make_tmap(Wh, H, 4 * (int64_t)H, 4 * (int64_t)H, 128);
     launch<128, MODE_LSTM_BWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 128));
+    if (tile) *tile = 128;
   } else {                                   // few rows: 32 hidden units per tile
     CUtensorMap tB = make_tmap(Wh, H, 4 * (int64_t)H, 4 * (int64_t)H, 32);
     launch<32, MODE_LSTM_BWD>(cx, tA, tB, p, cdiv(R, BM) * (H / 32));
+    if (tile) *tile = 32;
   }
   return true;
 }

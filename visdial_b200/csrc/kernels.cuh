@@ -23,6 +23,7 @@ bool gemm_atb_tc(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t
 
 // fused vocabulary softmax (gemm_tc.cu, pointwise.cu): the (rows, V) logits of decoders/gen.lua:21-24 never reach HBM
 int vocab_lse_nparts(int N);
+bool vocab_tc_ok(int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb);   // both halves take exactly this
 bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
                   const int32_t* tgt, float* part_max, float* part_sum, float* tgt_logit);
 bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
@@ -139,13 +140,16 @@ void segsum_rows(LaunchCtx& cx, const float* X, int64_t ldx, const int32_t* perm
 }  // namespace vd
 
 namespace vd {
-// fused SeqLSTM steps on the tensor cores (gemm_tc.cu); return false when the shape is not taken
+// fused SeqLSTM steps on the tensor cores (gemm_tc.cu); return false when the shape is not taken.  The *_ok predicates
+// are the weight / width conditions of those decisions, for the engine to route with; *tile receives the tile width.
+bool lstm_step_fwd_tc_ok(int H, const float* WtS_h, int64_t ldw);
+bool lstm_step_bwd_tc_ok(int H, const float* Wh);
 bool lstm_step_fwd_tc(LaunchCtx& cx, int64_t R, int H, const float* h_prev, const float* WtS_h, int64_t ldw, const float* bias,
                       float* gates, int has_xproj, const float* ptable, const int32_t* tok, const float* c_prev, float* c_out,
-                      float* h_out, const int32_t* mask_ids);
+                      float* h_out, const int32_t* mask_ids, int* tile = nullptr);
 bool lstm_step_bwd_tc(LaunchCtx& cx, int64_t R, int H, const float* da_next, const float* Wh, const float* gsave,
                       const float* c_prev, const float* c_cur, const float* dh_ext, float* dc_carry, const int32_t* mask_ids,
-                      float* da);
+                      float* da, int* tile = nullptr);
 }  // namespace vd
 
 namespace vd {
