@@ -11,7 +11,6 @@ sys.path.insert(0, ROOT)
 
 
 def run(overlap):
-    os.environ["VD_OPT_OVERLAP"] = "1" if overlap else "0"
     from bench import headline_params
     from visdial_b200 import Batch, Model
     from visdial_b200.synthetic import make_batch
@@ -19,6 +18,7 @@ def run(overlap):
     p["batchSize"] = 32
     model = Model(p, seed=1)
     eng = model.engine
+    eng.set_option_overlap(overlap)
     batch = Batch(make_batch(p, 32, seed=5)).to_device(eng)
     phases = ["zero", "enc_fwd", "dec_fwd", "crit_fwd", "crit_bwd", "dec_bwd", "bconn", "enc_bwd", "adam"]
     acc = {k: 0.0 for k in phases}

@@ -69,8 +69,6 @@ void comm_init(Engine* e, const void* idbytes, int rank, int world) {
   if (world == 1) return;
   ncclUniqueId id;
   memcpy(&id, idbytes, sizeof(id));
-  // VD_NCCL_MAX_NCHANNELS=n: cap the SMs the overlapped all-reduce takes from the backward pass (A/B knob; unset = NCCL's choice)
-  if (const char* ch = getenv("VD_NCCL_MAX_NCHANNELS")) { if (ch[0] && atoi(ch) > 0) setenv("NCCL_MAX_NCHANNELS", ch, 0); }
   ncclComm_t comm;
   nccl_check(api().CommInitRank(&comm, world, id, rank), "ncclCommInitRank");
   e->nccl_comm = comm;

@@ -13,7 +13,7 @@
 //   BPTT      T   cell of layer 2:   dh2_t = da2_{t+1} Wh2 [+ dL/dh2 at the last step]                -> da2_t     K = 4H
 //             X   input half:        da1[t][:, 0:H] <- da2_t Wx2    (partial of dh1_t, parked in the output rows)  K = 4H
 //             B   cell of layer 1:   dh1_t = partial + da1_{t+1} Wh1 [+ dL/dh1 at the last step]      -> da1_t     K = 4H
-//   (BPTT as listed = k_enc_pair_bwd<false>, the split by hidden unit.  The default when H % 128 == 0 is the split BY GATE,
+//   (BPTT as listed = k_enc_pair_bwd<false>, the split by hidden unit.  When H % 128 == 0 the BPTT splits BY GATE instead,
 //   k_enc_pair_bwd<true>: CTA (gate, 128-unit slice) contracts K = H against N = 128 and the four gate CTAs of a slice sum their
 //   partials in a zeroed fp32 dh[t] with red.add before each runs the pointwise of 32 units — see the comment at the kernel.)
 //
@@ -91,19 +91,6 @@ __device__ __forceinline__ void zero16(float* d) {
   for (int e = 0; e < EP_HW; ++e) d[e] = 0.f;
 }
 
-// Optional phase trace (VD_ENC_TRACE=1, debugging only): per (CTA, step) stamps — clock64 at {0: flag seen, 1: panel issued, 2: MMAs
-// started, 3: MMAs issued, 4: accumulator ready, 5: epilogue math + stores issued, 6: published} and globaltimer at {7: published, 8: flag
-// seen}.  A null pointer (the normal case) costs one predicated branch per stamp.
-constexpr int EP_TRACE_SLOTS = 10;
-__device__ __forceinline__ void ep_stamp(unsigned long long* trace, int T, int t, int slot, bool wall = false) {
-  if (trace) {
-    unsigned long long v;
-    if (wall) asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(v));
-    else v = (unsigned long long)clock64();
-    trace[((size_t)blockIdx.x * T + t) * EP_TRACE_SLOTS + slot] = v;
-  }
-}
-
 enum { EP_CELL1 = 0, EP_PROJ = 1, EP_CELL2 = 2 };      // forward: L1, X2, L2;  BPTT: T (layer 2), X, B (layer 1) — see the header
 
 struct EncFwdParams {
@@ -114,7 +101,6 @@ struct EncFwdParams {
   const float* bias2;
   const int32_t* mask;             // (T,R) token ids for maskzero, or null
   int* flags;                      // [3][RB][T]: completed slices of (role, row block, step)
-  unsigned long long* trace;       // null, or [grid][T][EP_TRACE_SLOTS]
 };
 
 // carve-up shared by both kernels
@@ -148,9 +134,7 @@ template <int N> __device__ __forceinline__ void ep_wgmma(float (&d)[N / 2], uin
 }
 // contraction of one step by a consumer warpgroup: KB k-blocks of the streamed panel (its 64 rows) against the resident slice
 template <int N>
-__device__ __forceinline__ void ep_mma_step(const EpSmem& sm, float (&d)[N / 2], int wg, int KB, int koff, int& s, uint32_t& ph,
-                                            unsigned long long* trace, int T, int t) {
-  if (threadIdx.x == 0) ep_stamp(trace, T, t, 2);
+__device__ __forceinline__ void ep_mma_step(const EpSmem& sm, float (&d)[N / 2], int wg, int KB, int koff, int& s, uint32_t& ph) {
   int prev = -1;
   for (int kb = 0; kb < KB; ++kb) {
     mbar_wait(&sm.full[s], ph);
@@ -170,7 +154,6 @@ __device__ __forceinline__ void ep_mma_step(const EpSmem& sm, float (&d)[N / 2],
   wgmma_wait<0>();
   wgmma_hold(d);
   if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&sm.empty[prev]);
-  if (threadIdx.x == 0) { ep_stamp(trace, T, t, 3); ep_stamp(trace, T, t, 4); }
 }
 // accumulator columns [32 C, 32 C + 32) of this warpgroup's 64 rows -> the shared chunk (rows 64 wg ..); the warps of the warpgroup
 // then read their half row from it.  C is a compile-time constant at every call.
@@ -194,13 +177,9 @@ __device__ __forceinline__ void ep_ld16(const float* arow, float* v) {
 
 // publish step t of this slice: barrier of the consumer warps, then ONE gpu-scope release (cumulative over what the barrier made
 // visible to the signalling thread) that counts the slice in — the grid-sync idiom of cooperative groups
-__device__ __forceinline__ void ep_publish(int* flag, unsigned long long* trace, int T, int t) {
-  if (threadIdx.x == 0) ep_stamp(trace, T, t, 5);
+__device__ __forceinline__ void ep_publish(int* flag) {
   bar_named(1, 256);
-  if (threadIdx.x == 0) {
-    asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(flag) : "memory");
-    ep_stamp(trace, T, t, 6); ep_stamp(trace, T, t, 7, true);
-  }
+  if (threadIdx.x == 0) asm volatile("red.release.gpu.global.add.s32 [%0], 1;" ::"l"(flag) : "memory");
 }
 
 __global__ void __launch_bounds__(EP_THREADS, 1)
@@ -242,7 +221,6 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
             wait_flag((role == EP_CELL1 ? flagL1 : flagL2) + (size_t)rb * T + (t - 1), p.nS);
             tm = role == EP_CELL1 ? &tmH1 : &tmH2; ts = t - 1;
           }
-          ep_stamp(p.trace, T, t, 8, true); ep_stamp(p.trace, T, t, 0);
           for (int kb = 0; kb < KB; ++kb) {
             int kr = kb + koff; if (kr >= KB) kr -= KB;
             mbar_wait(&sm.empty[s], ph ^ 1);
@@ -250,7 +228,6 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
             tma_load_2d(sm.stages + s * EP_STAGE_BYTES, tm, &sm.full[s], kr * 64, ts * p.R + rb * 128);
             if (++s == EP_STAGES) { s = 0; ph ^= 1; }
           }
-          ep_stamp(p.trace, T, t, 1);
         }
       }
     }
@@ -271,7 +248,7 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
         for (int t = 0; t < T; ++t) {
           const int64_t tr = (int64_t)t * p.R + row;
           float d[N / 2];
-          ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
+          ep_mma_step<N>(sm, d, wg, KB, koff, s, ph);
 #pragma unroll
           for (int g = 0; g < 4; ++g) {                        // one gate = one 128-byte line of the row per pass
             ep_chunk(sm.acc, d, wg, g);
@@ -284,7 +261,7 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
               st16g(p.gates2 + tr * 4 * H + g * H + u0, a);
             }
           }
-          ep_publish(flagX + (size_t)rb * T + t, p.trace, T, t);
+          ep_publish(flagX + (size_t)rb * T + t);
         }
       }
     } else {
@@ -314,7 +291,7 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
             for (int g = 0; g < 4; ++g) asm volatile("prefetch.global.L2 [%0];" ::"l"(xrow + (int64_t)p.R * 4 * H + g * H) : "memory");
           }
           float d[N / 2];
-          if (has_acc) ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
+          if (has_acc) ep_mma_step<N>(sm, d, wg, KB, koff, s, ph);
           float x[EP_HW], a[EP_HW], ig[EP_HW];
           // ---- i
           if (has_acc) ep_chunk(sm.acc, d, wg, 0);
@@ -353,7 +330,7 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
             st16g(xrow + 2 * H, a);
             st16h(h16 + tr * H + u0, ig);                      // what the next step's TMA reads
           }
-          ep_publish(flag + (size_t)rb * T + t, p.trace, T, t);
+          ep_publish(flag + (size_t)rb * T + t);
           // after the flag: saved state for the backward pass
           if (row_ok) { st16g(cst + tr * H + u0, c); st16g(hst + tr * H + u0, ig); }
         }
@@ -375,7 +352,6 @@ struct EncBwdParams {
   const float* dh_last1; const float* dc_last1; const float* dh_last2; const float* dc_last2;   // (R,H) each or null
   const int32_t* mask;
   int* flags;                      // [3][RB][T] step flags, then (gate split) [2][RB][T][H/128] partial-sum counts
-  unsigned long long* trace;       // null, or [grid][T][EP_TRACE_SLOTS]
   float* dh2; float* dh1;          // gate split: (T*R, H) fp32 each, zeroed — the partial products of a step are summed here with red.add
 };
 
@@ -428,7 +404,6 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
             wait_flag((role == EP_CELL1 ? flagT : flagB) + (size_t)rb * T + (t + 1), p.nS);
             tm = role == EP_CELL1 ? &tmA2 : &tmA1; ts = t + 1;
           }
-          ep_stamp(p.trace, T, t, 8, true); ep_stamp(p.trace, T, t, 0);
           for (int kb = 0; kb < KB; ++kb) {
             int kr = kb + koff; if (kr >= KB) kr -= KB;
             mbar_wait(&sm.empty[s], ph ^ 1);
@@ -436,7 +411,6 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
             tma_load_2d(sm.stages + s * EP_STAGE_BYTES, tm, &sm.full[s], (GS ? gq * H : 0) + kr * 64, ts * p.R + rb * 128);
             if (++s == EP_STAGES) { s = 0; ph ^= 1; }
           }
-          ep_stamp(p.trace, T, t, 1);
         }
       }
     }
@@ -473,15 +447,13 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
         for (int t = T - 1; t >= 0; --t) {
           const int64_t tr = (int64_t)t * p.R + row;
           float d[N / 2];
-          ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
+          ep_mma_step<N>(sm, d, wg, KB, koff, s, ph);
           if constexpr (GS) {
-            if (threadIdx.x == 0) ep_stamp(p.trace, T, t, 5);
             add_partial(d, p.dh1, cntB, rb, t, tr, row_ok);
-            if (threadIdx.x == 0) { ep_stamp(p.trace, T, t, 6); ep_stamp(p.trace, T, t, 7, true); }
           } else {
             ep_chunk(sm.acc, d, wg, 0);
             if (row_ok) { float a[EP_HW]; ep_ld16(arow, a); st16g(p.da1 + tr * 4 * H + u0, a); }
-            ep_publish(flagX + (size_t)rb * T + t, p.trace, T, t);
+            ep_publish(flagX + (size_t)rb * T + t);
           }
         }
       }
@@ -512,7 +484,7 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
           __half* da16row = da16 + tr * 4 * H + u0;
           float va[EP_HW], vb[EP_HW], dh[EP_HW];
           float d[N / 2];
-          if (has_acc) ep_mma_step<N>(sm, d, wg, KB, koff, s, ph, p.trace, T, t);
+          if (has_acc) ep_mma_step<N>(sm, d, wg, KB, koff, s, ph);
           if constexpr (GS) {
             // my partial into dh[t]; then the complete sum of my 32 units once every contributor of the unit slice has counted in:
             // layer 2: its 4 gate CTAs; layer 1: 4 projection CTAs (every step) + its own 4 gate CTAs (all steps but the last)
@@ -564,7 +536,7 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
             for (int e = 0; e < EP_HW; ++e) { dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]); dc[e] *= va[e]; }
             st16h(da16row + 1 * H, dh); st16g(darow + 1 * H, dh);
           }
-          ep_publish(flag + (size_t)rb * T + t, p.trace, T, t);
+          ep_publish(flag + (size_t)rb * T + t);
         }
       }
     }
@@ -588,64 +560,6 @@ static CUtensorMap ep_tmap_h(const __half* base, int64_t rows, int64_t cols, int
   }
   return tm;
 }
-
-// VD_ENC_TRACE=1: run the launch with a stamp buffer, then print where a step's time goes (stderr).  Debugging aid, synchronises.
-struct EpTrace {
-  unsigned long long* dev = nullptr;
-  int grid = 0, T = 0;
-  static bool on() { static const bool v = [] { const char* e = getenv("VD_ENC_TRACE"); return e && atoi(e) != 0; }(); return v; }
-  unsigned long long* begin(int grid_, int T_) {
-    if (!on()) return nullptr;
-    grid = grid_; T = T_;
-    VD_CUDA_CHECK(cudaMalloc(&dev, (size_t)grid * T * EP_TRACE_SLOTS * 8));
-    VD_CUDA_CHECK(cudaMemset(dev, 0, (size_t)grid * T * EP_TRACE_SLOTS * 8));
-    return dev;
-  }
-  // role of a CTA = (index in its group) / nS; reverse = BPTT (step t consumes what step t+1 published)
-  void report(cudaStream_t st, const char* name, int nS, bool reverse) {
-    if (!dev) return;
-    VD_CUDA_CHECK(cudaStreamSynchronize(st));
-    std::vector<unsigned long long> h((size_t)grid * T * EP_TRACE_SLOTS);
-    VD_CUDA_CHECK(cudaMemcpy(h.data(), dev, h.size() * 8, cudaMemcpyDeviceToHost));
-    cudaFree(dev); dev = nullptr;
-    const int per_group = 3 * nS;
-    auto at = [&](int c, int t, int s) { return h[((size_t)c * T + t) * EP_TRACE_SLOTS + s]; };
-    auto role_of = [&](int c) { return (c % per_group) / nS; };
-    static const char* fwd_names[3] = {"L1 cell", "X2 proj", "L2 cell"};
-    static const char* bwd_names[3] = {"T cell (layer 2)", "X proj", "B cell (layer 1)"};
-    for (int role = 0; role < 3; ++role) {
-      double sum[8] = {0}; int n = 0; double cyc = 0; int ncyc = 0; double prop = 0; int nprop = 0;
-      const int dep = role == EP_PROJ ? EP_CELL1 : role;              // the role whose publish this role's producer waits on
-      for (int c = 0; c < grid; ++c) {
-        if (role_of(c) != role) continue;
-        for (int t = 1; t + 1 < T; ++t) {
-          if (!at(c, t, 0) || !at(c, t, 6)) continue;
-          sum[0] += (double)(at(c, t, 1) - at(c, t, 0));       // flag seen -> last TMA issued
-          sum[1] += (double)(at(c, t, 3) - at(c, t, 0));       // flag seen -> last chunk landed + MMAs issued
-          sum[2] += (double)(at(c, t, 4) - at(c, t, 3));       // -> accumulator ready in the epilogue
-          sum[3] += (double)(at(c, t, 5) - at(c, t, 4));       // epilogue math + stores issued
-          sum[4] += (double)(at(c, t, 6) - at(c, t, 5));       // barrier + fence + atomic
-          sum[5] += (double)((long long)at(c, t, 2) - (long long)at(c, t, 0));   // accumulator free relative to flag seen (<0: no stall)
-          ++n;
-          const int tn = reverse ? t + 1 : t - 1;
-          if (at(c, tn, 6)) { cyc += (double)(at(c, t, 6) - at(c, tn, 6)); ++ncyc; }
-          // flag propagation: my flag seen (wall) minus the latest publish (wall) among the CTAs of the awaited role in my group
-          const int tp = role == EP_PROJ ? t : tn;
-          unsigned long long latest = 0;
-          const int g0 = c / per_group * per_group;
-          for (int o = g0; o < g0 + per_group; ++o)
-            if (role_of(o) == dep && at(o, tp, 7) > latest) latest = at(o, tp, 7);
-          if (latest && at(c, t, 8)) { prop += (double)((long long)at(c, t, 8) - (long long)latest); ++nprop; }
-        }
-      }
-      if (!n) continue;
-      fprintf(stderr, "[enc trace] %s %s: step cycle %.0f clk | flag->TMA issued %.0f | flag->operands landed %.0f | ->acc ready %.0f | "
-              "epilogue %.0f | publish %.0f | acc-free minus flag %.0f | flag propagation %.0f ns  (n=%d)\n",
-              name, (reverse ? bwd_names : fwd_names)[role], ncyc ? cyc / ncyc : 0.0, sum[0] / n, sum[1] / n, sum[2] / n, sum[3] / n,
-              sum[4] / n, sum[5] / n, nprop ? prop / nprop : 0.0, n);
-    }
-  }
-};
 
 }  // namespace tc
 
@@ -675,21 +589,15 @@ void enc_pair_forward(LaunchCtx& cx, int T, int64_t R, int H, const __half* W1h1
     VD_CUDA_CHECK(cudaFuncSetAttribute(k_enc_pair_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, EP_SMEM));
     attr_set = true;
   }
-  EpTrace trace;
-  p.trace = trace.begin(p.groups * 3 * p.nS, T);
   k_enc_pair_fwd<<<p.groups * 3 * p.nS, EP_THREADS, EP_SMEM, cx.stream>>>(tH1, tH2, tW1, tW2, p);
   check_launch(cx, "k_enc_pair_fwd");
-  trace.report(cx.stream, "fwd", p.nS, false);
 }
 
 
 // gates*/c* = the activations the forward saved; da*/da*_16 out (all T steps); flags int32 [enc_pair_bwd_flag_ints()].
 // dh1 / dh2: (T*R, H) fp32 scratch each for the gate-split variant (H % 128 == 0), or null -> unit-split variant
 int64_t enc_pair_bwd_flag_ints(int T, int64_t R, int H) { return (int64_t)cdiv(R, 128) * T * (3 + 2 * std::max(1, H / 128)); }
-bool enc_pair_gate_split(int H) {
-  static const int v = [] { const char* e = getenv("VD_ENC_GATESPLIT"); return e ? atoi(e) : 1; }();      // VD_ENC_GATESPLIT=0: unit split
-  return v != 0 && H % 128 == 0;
-}
+bool enc_pair_gate_split(int H) { return H % 128 == 0; }
 void enc_pair_backward(LaunchCtx& cx, int T, int64_t R, int H, const __half* B1cat16, const __half* Whb2_16, const int32_t* mask,
                        const float* gates1, const float* c1, const float* gates2, const float* c2, const float* dh_last1,
                        const float* dc_last1, const float* dh_last2, const float* dc_last2, float* da1, __half* da1_16, float* da2,
@@ -721,12 +629,9 @@ void enc_pair_backward(LaunchCtx& cx, int T, int64_t R, int H, const __half* B1c
     VD_CUDA_CHECK(cudaFuncSetAttribute(k_enc_pair_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, EP_SMEM));
     attr_set = true;
   }
-  EpTrace trace;
-  p.trace = trace.begin(p.groups * 3 * p.nS, T);
   if (gs) k_enc_pair_bwd<true><<<p.groups * 3 * p.nS, EP_THREADS, EP_SMEM, cx.stream>>>(tA1, tA2, tW1, tW2, p);
   else k_enc_pair_bwd<false><<<p.groups * 3 * p.nS, EP_THREADS, EP_SMEM, cx.stream>>>(tA1, tA2, tW1, tW2, p);
   check_launch(cx, "k_enc_pair_bwd");
-  trace.report(cx.stream, gs ? "bwd(gate split)" : "bwd", p.nS, true);
 }
 
 }  // namespace vd

@@ -173,8 +173,6 @@ Engine::Engine(const vd_params* p) {
   VD_CUDA_CHECK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
   VD_CUDA_CHECK(cudaEventCreateWithFlags(&ev_opt_fork, cudaEventDisableTiming));
   VD_CUDA_CHECK(cudaEventCreateWithFlags(&ev_opt_done, cudaEventDisableTiming));
-  if (const char* s = getenv("VD_OPT_OVERLAP")) opt_overlap = atoi(s) != 0;
-  if (const char* s = getenv("VD_OPT_RESERVE_SMS")) opt_reserve_sms = std::max(0, std::min(atoi(s), cx.sm_count - 16)) & ~1;
   size_t bytes = (size_t)nparams * sizeof(float);
   VD_CUDA_CHECK(cudaMalloc((void**)&W, bytes));
   VD_CUDA_CHECK(cudaMalloc((void**)&dW, bytes));
@@ -450,7 +448,7 @@ void Engine::lstm_forward_step(LstmRun& r, int t) {
     const int32_t* mk = r.mask ? r.mask + (int64_t)t * R : nullptr;
     int has_x = 0;
     if (!r.ptable) {
-      if (per_step_x && !r.xproj_external)
+      if (!save)        // a saved run's projection is batched in lstm_forward_begin, or issued by lstm_pair_forward
         gemm_tn((int)R, G, D, r.x + (int64_t)t * R * D, lda, nullptr, WtS, D + H, g, G, 0.f, xbias, 0);
       has_x = 1;
     }
@@ -497,35 +495,20 @@ cudaEvent_t Engine::pool_event(size_t i) {
 }
 
 // Wavefront over two stacked layers: layer-2 step t only needs layer-1 step t, so the two recurrences run one step
-// apart on two streams instead of back to back (the per-step kernels of these 320-row LSTMs are latency-bound).
-// Below this many rows the per-step contractions leave the tensor-core path (M < 64) and the two-stream wavefront only
-// adds launches and event traffic.
-static int64_t wavefront_min_rows() {
-  static int64_t v = -1;
-  if (v < 0) { const char* e = getenv("VD_WAVEFRONT_MIN_ROWS"); v = e ? atoll(e) : 64; }
-  return v;
-}
-
-static bool three_streams_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VD_THREE_STREAMS"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
-
-static bool enc_persist_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("VD_ENC_PERSIST"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1;
-}
+// apart on streams sa and sb instead of back to back (the per-step kernels of these 320-row LSTMs are latency-bound), with
+// the contraction between the layers on a third stream sc.  Below this many rows the per-step contractions leave the
+// tensor-core path (M < 64) and the wavefront only adds launches and event traffic.
+constexpr int64_t kWavefrontMinRows = 64;
 
 void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc) {
   // VD_MATH_F16: both layers and all time steps in ONE persistent launch (enc_lstm.cu) — weight slices stationary in
   // shared memory, steps chained through global flags — instead of 3 launches per time step on three streams
-  if (math_mode == VD_MATH_F16 && enc_persist_enabled() && !l1.h0 && !l1.c0 && !l2.h0 && !l2.c0 && !l1.gather && l1.x &&
+  if (math_mode == VD_MATH_F16 && !l1.h0 && !l1.c0 && !l2.h0 && !l2.c0 && !l1.gather && l1.x &&
       l1.H == l2.H && l2.D == l1.H && l1.R == l2.R && l1.T == l2.T && l1.mask == l2.mask && enc_pair_shape_ok(l1.R, l1.H, cx.sm_count)) {
     const int H = l1.H, G = 4 * H, T = l1.T;
     const int64_t R = l1.R;
     cx.stream = sa;
+    l1.pair16 = l2.pair16 = true;
     lstm_forward_begin(l1, true);               // h / c / gates of layer 1; gates1 <- x-projection + bias (batched GEMM)
     l2.x = l1.h;
     l2.step_xproj = true;                       // no batched x-projection for layer 2: the kernel's projection CTAs compute it per step
@@ -543,9 +526,7 @@ void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaSt
     return;
   }
   // layer 2 projects its input per step on the tensor-core step path only (a batched projection would read h1 before it exists)
-  const bool pipelined = tcmode() && lstm_step_fwd_tc_ok(l2.H, Wtp(l2.wseg) + l2.D, l2.D + l2.H) && sb != nullptr && sb != sa &&
-                         l2.R >= wavefront_min_rows();
-  const bool three = pipelined && sc != nullptr && sc != sa && sc != sb && three_streams_enabled();
+  const bool pipelined = tcmode() && lstm_step_fwd_tc_ok(l2.H, Wtp(l2.wseg) + l2.D, l2.D + l2.H) && l2.R >= kWavefrontMinRows;
   cx.stream = sa;
   if (!pipelined) {
     lstm_forward(l1, true);
@@ -561,25 +542,20 @@ void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaSt
   VD_CUDA_CHECK(cudaStreamWaitEvent(sb, e0, 0));
   cx.stream = sb;
   lstm_forward_begin(l2, true);
-  l2.xproj_external = three;
   for (int t = 0; t < l1.T; ++t) {
     cx.stream = sa;
     lstm_forward_step(l1, t);
     cudaEvent_t e = pool_event(1 + t);
     VD_CUDA_CHECK(cudaEventRecord(e, sa));
-    if (three) {
-      // layer 2's x-projection of step t needs h1_t only: on its own stream it runs beside layer 2's step t-1, so
-      // each of the three chains advances by ONE kernel per time step
-      VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e, 0));
-      if (t == 0) VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e0, 0));
-      cx.stream = sc;
-      lstm_forward_xproj(l2, t);
-      cudaEvent_t ex = pool_event(1 + l1.T + t);
-      VD_CUDA_CHECK(cudaEventRecord(ex, sc));
-      VD_CUDA_CHECK(cudaStreamWaitEvent(sb, ex, 0));
-    } else {
-      VD_CUDA_CHECK(cudaStreamWaitEvent(sb, e, 0));
-    }
+    // layer 2's x-projection of step t needs h1_t only: on its own stream it runs beside layer 2's step t-1, so
+    // each of the three chains advances by ONE kernel per time step
+    VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e, 0));
+    if (t == 0) VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e0, 0));
+    cx.stream = sc;
+    lstm_forward_xproj(l2, t);
+    cudaEvent_t ex = pool_event(1 + l1.T + t);
+    VD_CUDA_CHECK(cudaEventRecord(ex, sc));
+    VD_CUDA_CHECK(cudaStreamWaitEvent(sb, ex, 0));
     cx.stream = sb;
     lstm_forward_step(l2, t);
   }
@@ -664,7 +640,7 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
   float* dWs = dWp(r.wseg);
   const float* A = r.x ? r.x : Wp(0);
   const int64_t lda = r.x ? D : cfg.E;
-  const bool pair16 = !r.f16 && r.h16 && r.da16 && H % 64 == 0 && TR - R >= 256;
+  const bool pair16 = r.pair16 && TR - R >= 256;
   if (r.f16) {
     if (r.T > 1) {
       LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * H * G * (double)(TR - R), 2.0 * (double)(TR - R) * (H + G));
@@ -672,7 +648,8 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
     }
   } else if (r.T > 1) {
     // persistent pair (enc_lstm.cu): its kernels left fp16 copies of h and da — the operands of the recurrence itself — so the weight
-    // gradients contract those on the fp16 tensor-core path (fp32 accumulation) instead of the TF32 one
+    // gradients contract those on the fp16 tensor-core path (fp32 accumulation) instead of the TF32 one.  The pair's shape check
+    // (enc_pair_shape_ok) already guarantees H % 64 == 0.
     if (pair16) {
       LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * H * G * (double)(TR - R), 2.0 * (double)(TR - R) * (H + G));
       gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, nullptr);
@@ -704,7 +681,7 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
     VD_REQUIRE(dx_out == nullptr, VD_E_STATE, "projected-space embedding gradient: caller must not ask for dx");
     return;
   }
-  if (pair16 && r.x16 && !r.gather && D % 64 == 0) {
+  if (pair16 && r.x16) {            // layer 2 of the pair: x = h1, D = H
     LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * D * G * (double)TR, 2.0 * (double)TR * (D + G));
     gemm_atb16(cx, D, G, TR, r.x16, D, r.da16, G, dWs, G, nullptr);
   } else gemm_atb(D, G, TR, A, lda, r.gather, da, G, dWs, G);
@@ -719,14 +696,13 @@ void Engine::lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last
   lstm_backward_end(r, dx_out, dh0_out, dc0_out);
 }
 
-// BPTT wavefront of two stacked layers: layer-1 step t needs d(h1_t) = da2_t Wx2^T, produced per step on layer 2's
-// stream, so the two recurrences again run one step apart.
+// BPTT wavefront of two stacked layers: layer-1 step t needs d(h1_t) = da2_t Wx2^T, produced per step on stream sc,
+// so the two recurrences again run one step apart (layer 2 on sb, layer 1 on sa).
 void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2, const float* dc_last2, const float* dh_last1,
                                 const float* dc_last1, float* dx1_out, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc) {
   const int H = l2.H, G = 4 * l2.H;
   const int64_t R = l2.R;
-  if (math_mode == VD_MATH_F16 && enc_persist_enabled() && l1.h16 && l2.h16 && l1.saved && l2.saved && l2.D == H && l1.T == l2.T &&
-      enc_pair_shape_ok(R, H, cx.sm_count)) {
+  if (l1.pair16) {
     // the forward of this pair ran as the persistent kernel: so does its BPTT (enc_lstm.cu::k_enc_pair_bwd) — one launch for
     // both layers and all time steps; the weight / input gradients follow as batched contractions over all T*R rows
     const int T = l2.T;
@@ -752,8 +728,8 @@ void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2,
     return;
   }
   float* dx2 = arena.get<float>((int64_t)l2.T * R * l2.D);      // = gradient wrt layer-1 outputs, all steps
-  const bool pipelined = tcmode() && H % 128 == 0 && sb != nullptr && sb != sa && R >= wavefront_min_rows();
-  const bool three = pipelined && sc != nullptr && sc != sa && sc != sb && three_streams_enabled();
+  const bool pipelined = tcmode() && lstm_step_bwd_tc_ok(H, Wp(l1.wseg) + (int64_t)l1.D * G) &&
+                         lstm_step_bwd_tc_ok(H, Wp(l2.wseg) + (int64_t)l2.D * G) && R >= kWavefrontMinRows;
   cx.stream = sa;
   if (!pipelined) {
     lstm_backward(l2, nullptr, dh_last2, dc_last2, dx2, nullptr, nullptr);
@@ -771,16 +747,14 @@ void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2,
   for (int t = l2.T - 1; t >= 0; --t) {
     cx.stream = sb;
     lstm_backward_step(l2, t);
+    // d(h1_t) = da2_t Wx2 needs layer 2's step t only: on its own stream it runs beside layer 2's step t-1
     cudaEvent_t e = pool_event(1 + t);
-    if (three) {
-      // d(h1_t) = da2_t Wx2 needs layer 2's step t only: on its own stream it runs beside layer 2's step t-1
-      VD_CUDA_CHECK(cudaEventRecord(e, sb));
-      VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e, 0));
-      cx.stream = sc;
-    }
+    VD_CUDA_CHECK(cudaEventRecord(e, sb));
+    VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e, 0));
+    cx.stream = sc;
     gemm_tn((int)R, l2.D, G, l2.da + (int64_t)t * R * G, G, nullptr, Wx2, G, dx2 + (int64_t)t * R * l2.D, l2.D, 0.f, nullptr, 0);
-    cudaEvent_t ex = three ? pool_event(1 + l2.T + t) : e;
-    VD_CUDA_CHECK(cudaEventRecord(ex, cx.stream));
+    cudaEvent_t ex = pool_event(1 + l2.T + t);
+    VD_CUDA_CHECK(cudaEventRecord(ex, sc));
     VD_CUDA_CHECK(cudaStreamWaitEvent(sa, ex, 0));
     cx.stream = sa;
     lstm_backward_step(l1, t);
@@ -944,7 +918,7 @@ void Engine::encoder_forward(const vd_batch* b) {
   // on the side stream (its tiny per-step kernels are latency-bound; overlapping the two chains hides half of it).
   // (the persistent pair kernels of VD_MATH_F16 are flag-chained grids that want every SM: two of them must never be
   //  co-scheduled — neither could become fully resident — so in that mode both pairs run on the main stream, in order)
-  const bool serial_pairs = math_mode == VD_MATH_F16 && enc_persist_enabled();
+  const bool serial_pairs = math_mode == VD_MATH_F16;
   if (cfg.useHist) {
     if (serial_pairs) { join_side(); run_two(hist1, hist2, main_stream, main2_stream, main3_stream); }
     else { fork_side(); run_two(hist1, hist2, side_stream, side2_stream, side3_stream); back_to_main(); }
@@ -1126,7 +1100,7 @@ void Engine::encoder_backward(const float* dEnc) {
   // concurrently on the side stream (disjoint weight segments; the shared embedding gradient is atomics-only)
   const bool embdrop = cfg.embdrop;
   // (persistent pair kernels must not be co-scheduled — see encoder_forward: in that mode both BPTTs run on the main stream)
-  const bool serial_pairs = math_mode == VD_MATH_F16 && enc_persist_enabled() && hist1.h16 != nullptr;
+  const bool serial_pairs = hist1.pair16;
   if (cfg.useHist) {
     if (serial_pairs) { join_side(); cx.stream = main_stream; } else fork_side();
     cudaStream_t hs = serial_pairs ? main_stream : side_stream;
@@ -1200,13 +1174,9 @@ void Engine::options_forward_async() {
   }
   cudaStream_t prev = cx.stream;
   cx.stream = s;
-  if (opt_overlap) {                                                // leave SMs to the encoder's concurrent chains
-    static int fwd_reserve = -1;                                    // VD_OPT_RESERVE_FWD: A/B knob, default = the common reserve
-    if (fwd_reserve < 0) { const char* e = getenv("VD_OPT_RESERVE_FWD"); fwd_reserve = e ? (atoi(e) & ~1) : 1 << 20; }
-    // with the persistent encoder forward (VD_MATH_F16) nothing latency-bound runs beside the option stream's forward: no reserve
-    const int dflt = (math_mode == VD_MATH_F16 && enc_persist_enabled()) ? 0 : opt_reserve_sms;
-    cx.sm_budget = cx.sm_count - (fwd_reserve == 1 << 20 ? dflt : std::min(fwd_reserve, cx.sm_count - 16));
-  }
+  // leave SMs to the encoder's concurrent chains; with the persistent encoder forward (VD_MATH_F16) nothing latency-bound
+  // runs beside the option stream's forward: no reserve
+  if (opt_overlap) cx.sm_budget = cx.sm_count - (math_mode == VD_MATH_F16 ? 0 : opt_reserve_sms);
   ids_o = arena.get<int32_t>(Ro * db.To);
   transpose_ids(cx, db.options, ids_o, Ro, db.To);
   opt = make_run(db.To, Ro, cfg.E, cfg.H, seg("opt.lstm.weight"), nullptr, ids_o, nullptr);   // disc.lua:4-5: no maskzero

@@ -68,8 +68,7 @@ struct LstmRun {
   float* demb_out = nullptr;         // projected-space embedding gradient goes here (overwritten) instead of dW(wordEmbed) +=
   // forward run state (lstm_forward_begin / _step)
   bool tc = false;                   // fused wgmma step kernels
-  bool step_xproj = false;           // dense input projected per step (layer-2 of a pipelined pair) instead of batched
-  bool xproj_external = false;       // ... and that per-step projection is issued by the caller (on its own stream)
+  bool step_xproj = false;           // layer 2 of a pair: lstm_pair_forward projects its input per step instead of batched
   const float* ptable = nullptr;     // (V+1, 4H) projection table for embedding-gathered inputs
   // backward run state (lstm_backward_begin / _step / _end)
   float* da = nullptr; float* dc_carry = nullptr; float* dh_rec = nullptr;
@@ -78,6 +77,9 @@ struct LstmRun {
   // VD_MATH_F16 run state (lstm16.cu): fp16 h / activated gates / da and x-projection table, fp32 c; `h` and `gates` stay null
   bool f16 = false;
   __half *h16 = nullptr, *gates16 = nullptr, *da16 = nullptr, *P16 = nullptr, *Wh16 = nullptr, *Whb16 = nullptr;
+  // set on both runs by lstm_pair_forward when the pair ran as the persistent kernel (enc_lstm.cu): the BPTT takes the same
+  // route, and the weight gradients contract the fp16 h / da it leaves
+  bool pair16 = false;
   const __half* x16 = nullptr;       // fp16 copy of x when a persistent pair produced one (layer 2: the h1 sequence)
   float* h32_last = nullptr;         // fp32 copy of the last step's h (what the fp32 consumers of the run read)
   float* scale2 = nullptr;           // device {s, 1/s}: power-of-two scale of the BPTT (chosen from max|dL/dh_T|)

@@ -30,21 +30,12 @@ constexpr int BN16 = 128;        // accumulator columns per tile: forward 32 hid
 constexpr int EW16 = 8;          // consumer warps = epilogue warps: 2 per 32-row quarter
 constexpr int STAGE16 = 32768;   // 16 KB of A (128 rows) + 16 KB of B (128 rows)
 
-// sigmoid / tanh as {FMUL, MUFU.EX2, FADD, MUFU.RCP [, FFMA]}: abs error ~1e-7 like fsigmoid / ftanh of tc_ptx.cuh, without the
-// range fix-ups of __fdividef / copysign (ex2 -> +inf gives rcp -> 0, ex2 -> 0 gives 1: both limits are exact)
-__device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 // Activations of the fp16 option LSTM: ONE special-function op each (tanh.approx.f32, relative error 2^-11 — the rounding class of the fp16
-// the gates and h are stored in right after; sigmoid(x) = 0.5 tanh(x/2) + 0.5) instead of ex2 + rcp (two): the pointwise half of the
-// forward step is issue / MUFU-bound.  Measured at the benched size (tests/test_c4_b32_gpu.py, DESIGN.md 7): rank agreement with the fp64
-// oracle 0.9781 vs 0.9777, top-1 0.99375 both, R@k deltas 0 both.  -DVD_F16_EX2_ACTIVATIONS restores the two-op forms.
-#ifndef VD_F16_EX2_ACTIVATIONS
+// the gates and h are stored in right after; sigmoid(x) = 0.5 tanh(x/2) + 0.5) instead of the two of ex2 + rcp: the pointwise half of the
+// forward step is issue / MUFU-bound.  Against the ex2 + rcp forms (abs error ~1e-7), measured at the benched size
+// (tests/test_c4_b32_gpu.py, DESIGN.md 7): rank agreement with the fp64 oracle 0.9781 vs 0.9777, top-1 0.99375 both, R@k deltas 0 both.
 __device__ __forceinline__ float tanh16(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sig16(float x) { return fmaf(0.5f, tanh16(0.5f * x), 0.5f); }
-#else
-__device__ __forceinline__ float sig16(float x) { return rcp_approx(1.f + ex2_approx(-1.4426950408889634f * x)); }
-__device__ __forceinline__ float tanh16(float x) { return fmaf(2.f, rcp_approx(1.f + ex2_approx(-2.8853900817779268f * x)), -1.f); }
-#endif
 
 // ---- fp16 <-> fp32 packing (round to nearest even, saturating: a scaled gradient that outgrows the range clamps to
 // +-65504 instead of becoming inf)
