@@ -366,18 +366,6 @@ int vd_gemm_atb16(vd_engine* h, int32_t M, int32_t N, int64_t K, const float* A,
     cudaFree(A16); cudaFree(B16); cudaFree(sc);
   })
 }
-// dst[r, :] = src[r, :] + bias  (the engine folds the bias into the x-projection before the fused step reads it)
-static __global__ void k_add_row_bias(float* dst, const float* src, const float* bias, int64_t rows, int cols) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < rows * cols) dst[i] = src[i] + bias[i % cols];
-}
-static void add_row_bias(vd::LaunchCtx& cx, float* dst, const float* src, const float* bias, int64_t rows, int cols) {
-  const int64_t n = rows * cols;
-  if (n == 0) return;
-  k_add_row_bias<<<(unsigned)((n + 255) / 256), 256, 0, cx.stream>>>(dst, src, bias, rows, cols);
-  vd::check_launch(cx, "k_add_row_bias");
-}
-
 int vd_lstm_step_fwd(vd_engine* h, int64_t R, int32_t H, const float* h_prev, const float* WhT, int64_t ldw, const float* bias,
                      float* gates, int32_t has_xproj, const float* ptable, int64_t ptable_rows, const int32_t* tok,
                      const float* c_prev, float* c_out, float* h_out, const int32_t* mask_ids, int32_t* path) {
@@ -388,37 +376,27 @@ int vd_lstm_step_fwd(vd_engine* h, int64_t R, int32_t H, const float* h_prev, co
     VD_REQUIRE((has_xproj != 0) != (ptable != nullptr) && (!ptable || (tok && ptable_rows > 0)), VD_E_BADARG,
                "vd_lstm_step_fwd: the x side is either a dense projection (has_xproj) or a table gather (ptable + tok)");
     VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
-    vd::LaunchCtx& cx = e->cx;
-    const int64_t G = 4 * (int64_t)H;
     *path = 0;
-    if (e->math_mode == VD_MATH_F16)
-      VD_REQUIRE(!(ptable && vd::lstm16_shape_ok(R, H)), VD_E_BADARG,
-                 "vd_lstm_step_fwd: the fp16 option-LSTM steps (lstm16.cu) have no test hook");
+    // routed as a step of a run without initial state over a gathered (ptable) or dense x side; the backward half of the
+    // route is not used here
+    const vd::LstmRoute rt = e->route_lstm(R, H, ptable != nullptr, false, WhT, ldw, nullptr);
+    VD_REQUIRE(rt.fwd != vd::LstmPath::Opt16, VD_E_BADARG, "vd_lstm_step_fwd: the fp16 option-LSTM steps (lstm16.cu) have no test hook");
+    // the CUDA-core route projects gathered inputs inside its x-projection GEMM, never through a table
+    VD_REQUIRE(rt.fwd == vd::LstmPath::Tc || !ptable, VD_E_BADARG, "vd_lstm_step_fwd: a table gather runs on the tensor-core route only");
+    vd::LstmFwdStep s;
+    s.R = R; s.H = H; s.WhT = WhT; s.ldw = ldw; s.bias = bias;
+    s.h_prev = h_prev; s.c_prev = c_prev; s.gates = gates; s.mask = mask_ids; s.c_out = c_out; s.h_out = h_out;
     float* pt = nullptr;
-    if (e->tcmode() && vd::lstm_step_fwd_tc_ok(H, WhT, ldw)) {
-      // Engine::lstm_forward_begin / _step, tensor-core route: the bias rides in the x-projection (table or dense)
-      if (ptable) {
-        VD_CUDA_CHECK(cudaMalloc((void**)&pt, (size_t)ptable_rows * G * sizeof(float)));
-        add_row_bias(cx, pt, ptable, bias, ptable_rows, (int)G);
-      } else {
-        add_row_bias(cx, gates, gates, bias, R, (int)G);
-      }
-      if (!h_prev) {
-        vd::lstm_first_step_fwd(cx, gates, pt, pt ? tok : nullptr, nullptr, c_prev, mask_ids, c_out, h_out, R, H);
-      } else {
-        int tile = 0;
-        bool ok = vd::lstm_step_fwd_tc(cx, R, H, h_prev, WhT, ldw, nullptr, gates, has_xproj, pt, pt ? tok : nullptr, c_prev, c_out,
-                                       h_out, mask_ids, &tile);
-        VD_REQUIRE(ok, VD_E_STATE, "lstm_step_fwd_tc refused a shape lstm_step_fwd_tc_ok accepts");
-        *path = tile;
-      }
-    } else {
-      // CUDA-core route: the engine projects gathered inputs inside its x-projection GEMM, never through a table
-      VD_REQUIRE(!ptable, VD_E_BADARG, "vd_lstm_step_fwd: a table gather runs on the tensor-core route only");
-      if (h_prev) e->gemm_tn((int)R, (int)G, H, h_prev, H, nullptr, WhT, ldw, gates, G, 1.f, nullptr, 0);
-      vd::lstm_pointwise_fwd(cx, gates, bias, c_prev, mask_ids, c_out, h_out, R, H);
+    if (rt.fwd == vd::LstmPath::Tc) {
+      // the tensor-core steps read the bias from the x-projection (table or dense), where the engine folds it in
+      const int64_t n = (ptable ? ptable_rows : R) * 4 * H;
+      VD_CUDA_CHECK(cudaMalloc((void**)&pt, (size_t)n * sizeof(float)));
+      vd::repeat_rows(e->cx, pt, bias, 1, (int)(n / (4 * H)), 4 * H);           // the bias in every row
+      vd::add_inplace(e->cx, ptable ? pt : gates, ptable ? ptable : pt, n);
+      if (ptable) { s.ptable = pt; s.tok = tok; }
     }
-    VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+    if (rt.fwd == vd::LstmPath::Tc) *path = e->lstm_tc_fwd_step(s); else e->lstm_simt_fwd_step(s);
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
     if (pt) cudaFree(pt);
   })
 }
@@ -431,26 +409,16 @@ int vd_lstm_step_bwd(vd_engine* h, int64_t R, int32_t H, const float* da_next, c
     NOTNULL(path);
     VD_REQUIRE(R >= 1 && H > 0 && Wh && gates && c_cur && dc_carry && da, VD_E_BADARG, "vd_lstm_step_bwd: arguments");
     VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
-    vd::LaunchCtx& cx = e->cx;
-    const int64_t G = 4 * (int64_t)H;
     *path = 0;
-    if (e->tcmode() && vd::lstm_step_bwd_tc_ok(H, Wh) && da_next) {
-      // Engine::lstm_backward_step, tensor-core route (its last step, without da_next, is the pointwise kernel below)
-      int tile = 0;
-      bool ok = vd::lstm_step_bwd_tc(cx, R, H, da_next, Wh, gates, c_prev, c_cur, dh_ext, dc_carry, mask_ids, da, &tile);
-      VD_REQUIRE(ok, VD_E_STATE, "lstm_step_bwd_tc refused a shape lstm_step_bwd_tc_ok accepts");
-      *path = tile;
-    } else {
-      float* dh_rec = nullptr;
-      if (da_next) {
-        VD_CUDA_CHECK(cudaMalloc((void**)&dh_rec, (size_t)R * H * sizeof(float)));
-        e->gemm_tn((int)R, H, (int)G, da_next, G, nullptr, Wh, G, dh_rec, H, 0.f, nullptr, 0);
-      }
-      vd::lstm_pointwise_bwd(cx, gates, c_prev, c_cur, dh_rec, dh_ext, nullptr, dc_carry, mask_ids, da, R, H);
-      VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
-      if (dh_rec) cudaFree(dh_rec);
-    }
-    VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+    // routed as a step of a run with a dense x side (the forward half of the route is not used here)
+    const vd::LstmRoute rt = e->route_lstm(R, H, false, false, nullptr, H, Wh);
+    vd::LstmBwdStep s;
+    s.R = R; s.H = H; s.Wh = Wh; s.da_next = da_next; s.dh_ext = dh_ext;
+    s.gates = gates; s.c_prev = c_prev; s.c_cur = c_cur; s.mask = mask_ids; s.dc_carry = dc_carry; s.da = da;
+    if (rt.bwd == vd::LstmPath::Simt && da_next) VD_CUDA_CHECK(cudaMalloc((void**)&s.dh_rec, (size_t)R * H * sizeof(float)));
+    if (rt.bwd == vd::LstmPath::Tc) *path = e->lstm_tc_bwd_step(s); else e->lstm_simt_bwd_step(s);
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+    if (s.dh_rec) cudaFree(s.dh_rec);
   })
 }
 

@@ -164,10 +164,9 @@ Engine::Engine(const vd_params* p) {
   VD_CUDA_CHECK(cudaStreamCreateWithPriority(&cx.stream, cudaStreamNonBlocking, prio_hi));
   main_stream = cx.stream;
   VD_CUDA_CHECK(cudaStreamCreateWithPriority(&side_stream, cudaStreamNonBlocking, prio_hi));
-  VD_CUDA_CHECK(cudaStreamCreateWithPriority(&main2_stream, cudaStreamNonBlocking, prio_hi));
-  VD_CUDA_CHECK(cudaStreamCreateWithPriority(&side2_stream, cudaStreamNonBlocking, prio_hi));
-  VD_CUDA_CHECK(cudaStreamCreateWithPriority(&main3_stream, cudaStreamNonBlocking, prio_hi));
-  VD_CUDA_CHECK(cudaStreamCreateWithPriority(&side3_stream, cudaStreamNonBlocking, prio_hi));
+  main_chain.a = main_stream; side_chain.a = side_stream;
+  for (cudaStream_t* s : {&main_chain.b, &side_chain.b, &main_chain.c, &side_chain.c})
+    VD_CUDA_CHECK(cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, prio_hi));
   VD_CUDA_CHECK(cudaStreamCreateWithPriority(&opt_stream, cudaStreamNonBlocking, prio_lo));
   VD_CUDA_CHECK(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
   VD_CUDA_CHECK(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
@@ -222,10 +221,8 @@ Engine::~Engine() {
   if (ev_fork) cudaEventDestroy(ev_fork);
   if (ev_join) cudaEventDestroy(ev_join);
   if (side_stream) { cudaStreamSynchronize(side_stream); cudaStreamDestroy(side_stream); }
-  if (main2_stream) { cudaStreamSynchronize(main2_stream); cudaStreamDestroy(main2_stream); }
-  if (side2_stream) { cudaStreamSynchronize(side2_stream); cudaStreamDestroy(side2_stream); }
-  if (main3_stream) { cudaStreamSynchronize(main3_stream); cudaStreamDestroy(main3_stream); }
-  if (side3_stream) { cudaStreamSynchronize(side3_stream); cudaStreamDestroy(side3_stream); }
+  for (cudaStream_t s : {main_chain.b, side_chain.b, main_chain.c, side_chain.c})
+    if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
   if (opt_stream) { cudaStreamSynchronize(opt_stream); cudaStreamDestroy(opt_stream); }
   if (ev_opt_fork) cudaEventDestroy(ev_opt_fork);
   if (ev_opt_done) cudaEventDestroy(ev_opt_done);
@@ -347,26 +344,96 @@ void Engine::release_img() {
 // nn.SeqLSTM [upstream rnn], SURVEY.md Appendix C.  Forward: one batched x-projection (or per step in
 // the non-saving mode) + per step {recurrent GEMM, pointwise}.
 // ------------------------------------------------------------------------------------------------
-void Engine::lstm_forward_begin(LstmRun& r, bool save) {
+// Wavefront over two stacked layers: layer-2 step t only needs layer-1 step t, so the two recurrences run one step
+// apart on two streams instead of back to back (the per-step kernels of these 320-row LSTMs are latency-bound), with
+// the contraction between the layers on a third stream.  Below this many rows the per-step contractions leave the
+// tensor-core path (M < 64) and the wavefront only adds launches and event traffic.
+constexpr int64_t kWavefrontMinRows = 64;
+
+LstmRoute Engine::route_lstm(int64_t R, int H, bool gathered, bool has_h0, const float* WhT, int64_t ldw, const float* Wh) const {
+  LstmRoute rt;
+  // VD_MATH_F16: a many-row LSTM over embedding-gathered tokens (the option LSTM) keeps h, the activated gates, da and
+  // the projection table in fp16 and runs f16 contractions (lstm16.cu); c, the accumulators and h_T stay fp32
+  if (math_mode == VD_MATH_F16 && gathered && !has_h0 && lstm16_shape_ok(R, H)) {
+    rt.fwd = rt.bwd = LstmPath::Opt16;
+  } else {
+    rt.fwd = tcmode() && lstm_step_fwd_tc_ok(H, WhT, ldw) ? LstmPath::Tc : LstmPath::Simt;
+    rt.bwd = tcmode() && lstm_step_bwd_tc_ok(H, Wh) ? LstmPath::Tc : LstmPath::Simt;
+  }
+  rt.table_grad = gathered && tcmode();
+  return rt;
+}
+
+void Engine::route_lstm_pair(LstmRun& l1, LstmRun& l2) const {
+  // VD_MATH_F16: both layers and all time steps in ONE persistent launch (enc_lstm.cu) — weight slices stationary in
+  // shared memory, steps chained through global flags — instead of 3 launches per time step on three streams.  The
+  // kernel takes a dense layer-1 input, no initial state, and one row count, length and mask for both layers.
+  if (math_mode == VD_MATH_F16 && !l1.h0 && !l1.c0 && !l2.h0 && !l2.c0 && !l1.gather && l1.x && l1.H == l2.H &&
+      l2.D == l1.H && l1.R == l2.R && l1.T == l2.T && l1.mask == l2.mask && enc_pair_shape_ok(l1.R, l1.H, cx.sm_count)) {
+    l1.route = l2.route = LstmRoute();
+    l1.route.fwd = l1.route.bwd = l2.route.fwd = l2.route.bwd = LstmPath::Pair16;
+    return;
+  }
+  l1.route = route_lstm(l1);
+  l2.route = route_lstm(l2);
+  // in the wavefront layer 2 projects its input per step, which the tensor-core step path takes (a batched projection
+  // would read h1 before it exists)
+  l1.route.wave_fwd = l2.route.wave_fwd = l2.route.fwd == LstmPath::Tc && l2.R >= kWavefrontMinRows;
+  l1.route.wave_bwd = l2.route.wave_bwd = l1.route.bwd == LstmPath::Tc && l2.route.bwd == LstmPath::Tc && l2.R >= kWavefrontMinRows;
+}
+
+void Engine::lstm_simt_fwd_step(const LstmFwdStep& s) {
+  const int G = 4 * s.H;
+  if (s.h_prev) gemm_tn((int)s.R, G, s.H, s.h_prev, s.H, nullptr, s.WhT, s.ldw, s.gates, G, 1.f, nullptr, 0);
+  lstm_pointwise_fwd(cx, s.gates, s.bias, s.c_prev, s.mask, s.c_out, s.h_out, s.R, s.H);
+}
+
+int Engine::lstm_tc_fwd_step(const LstmFwdStep& s) {
+  if (!s.h_prev) {      // no recurrent term: a plain streaming kernel (the x-projection already has the bias)
+    lstm_first_step_fwd(cx, s.gates, s.ptable, s.tok, nullptr, s.c_prev, s.mask, s.c_out, s.h_out, s.R, s.H);
+    return 0;
+  }
+  int tile = 0;
+  const bool ok = lstm_step_fwd_tc(cx, s.R, s.H, s.h_prev, s.WhT, s.ldw, nullptr, s.gates, s.ptable == nullptr, s.ptable, s.tok,
+                                   s.c_prev, s.c_out, s.h_out, s.mask, &tile);
+  VD_REQUIRE(ok, VD_E_STATE, "lstm_step_fwd_tc refused a shape the engine routed to it");
+  return tile;
+}
+
+void Engine::lstm_simt_bwd_step(const LstmBwdStep& s) {
+  const int G = 4 * s.H;
+  if (s.da_next) gemm_tn((int)s.R, s.H, G, s.da_next, G, nullptr, s.Wh, G, s.dh_rec, s.H, 0.f, nullptr, 0);
+  lstm_pointwise_bwd(cx, s.gates, s.c_prev, s.c_cur, s.da_next ? s.dh_rec : s.dh_last, s.dh_ext, nullptr, s.dc_carry, s.mask, s.da,
+                     s.R, s.H);
+}
+
+int Engine::lstm_tc_bwd_step(const LstmBwdStep& s) {
+  if (!s.da_next) { lstm_simt_bwd_step(s); return 0; }    // last step: no recurrent gradient yet, the pointwise kernel alone
+  // one fused kernel: dh_rec = da_{t+1} Wh^T on wgmma, backward pointwise in the epilogue
+  int tile = 0;
+  const bool ok = lstm_step_bwd_tc(cx, s.R, s.H, s.da_next, s.Wh, s.gates, s.c_prev, s.c_cur, s.dh_ext, s.dc_carry, s.mask,
+                                   s.da, &tile);
+  VD_REQUIRE(ok, VD_E_STATE, "lstm_step_bwd_tc refused a shape the engine routed to it");
+  return tile;
+}
+
+// gates of steps [t0, t0 + nt) <- x W_x^T; the Tc and Pair16 step kernels take the bias from here
+void Engine::lstm_xproj(const LstmRun& r, int t0, int nt, float* gates) {
+  const int64_t off = (int64_t)t0 * r.R;
+  gemm_tn((int)(nt * r.R), 4 * r.H, r.D, r.x ? r.x + off * r.D : Wp(0), r.x ? r.D : cfg.E, r.gather ? r.gather + off : nullptr,
+          Wtp(r.wseg), r.D + r.H, gates, 4 * r.H, 0.f, r.route.fwd == LstmPath::Simt ? nullptr : Wp(r.wseg + 1), 0);
+}
+
+void Engine::lstm_forward_begin(LstmRun& r, bool save, bool xproj_by_caller) {
   const Seg& ws = lay.segs[r.wseg];
   VD_REQUIRE(ws.rows == r.D + r.H && ws.cols == 4 * r.H, VD_E_STATE, "lstm weight shape");
+  VD_REQUIRE(!r.gather || r.D == cfg.E, VD_E_STATE, "gathered LSTM input must be the word embedding");
   const int H = r.H, D = r.D, G = 4 * r.H;
   const int64_t R = r.R;
   const float* WtS = Wtp(r.wseg);          // [4H, D+H]
-  const float* bias = Wp(r.wseg + 1);
-  const float* A = r.x ? r.x : Wp(0);
-  const int64_t lda = r.x ? D : cfg.E;
   r.saved = save;
-  // Tensor-core path: the x-projection of an embedding-gathered input becomes a (V+1, 4H) projection table
-  // computed once per forward (E Wx^T: the 300-wide half of every step's contraction collapses into a
-  // gather in the step epilogue); a dense input keeps the batched x-projection.  Each step is then ONE fused
-  // kernel: recurrent wgmma GEMM + SeqLSTM pointwise epilogue.
-  r.tc = tcmode() && lstm_step_fwd_tc_ok(H, WtS + D, D + H);
   r.ptable = nullptr;
-  // VD_MATH_F16: a many-row LSTM over embedding-gathered tokens (the option LSTM) keeps h, the activated gates, da and
-  // the projection table in fp16 and runs kind::f16 contractions (lstm16.cu); c, the accumulators and h_T stay fp32
-  r.f16 = math_mode == VD_MATH_F16 && r.gather && !r.x && !r.h0 && D == cfg.E && lstm16_shape_ok(R, H);
-  if (r.f16) {
+  if (r.route.fwd == LstmPath::Opt16) {
     float* pt = arena.get<float>((int64_t)(cfg.V + 1) * G);
     gemm_tn(cfg.V + 1, G, D, Wp(0), cfg.E, nullptr, WtS, D + H, pt, G, 0.f, nullptr, 0);     // bias stays fp32, added per step
     r.P16 = arena.get<__half>((int64_t)(cfg.V + 1) * G);
@@ -386,101 +453,65 @@ void Engine::lstm_forward_begin(LstmRun& r, bool save) {
     r.h = nullptr; r.gates = nullptr;
     return;
   }
-  // on the tensor-core path the bias is folded into the x-projection (table or GEMM epilogue), so the per-step
-  // kernel reads one array less
-  const float* xbias = r.tc ? bias : nullptr;
-  if (r.tc && r.gather) {
+  // Tensor-core path: the x-projection of an embedding-gathered input becomes a (V+1, 4H) projection table
+  // computed once per forward (E Wx^T: the 300-wide half of every step's contraction collapses into a
+  // gather in the step epilogue); a dense input keeps the batched x-projection.  Each step is then ONE fused
+  // kernel: recurrent wgmma GEMM + SeqLSTM pointwise epilogue.  The bias is folded into the x-projection (table or
+  // GEMM epilogue), so the per-step kernel reads one array less.
+  if (r.route.fwd == LstmPath::Tc && r.gather) {
     float* pt = arena.get<float>((int64_t)(cfg.V + 1) * G);
-    gemm_tn(cfg.V + 1, G, D, Wp(0), cfg.E, nullptr, WtS, D + H, pt, G, 0.f, xbias, 0);
+    gemm_tn(cfg.V + 1, G, D, Wp(0), cfg.E, nullptr, WtS, D + H, pt, G, 0.f, Wp(r.wseg + 1), 0);
     r.ptable = pt;
   }
-  if (save) {
-    r.h = arena.get<float>((int64_t)r.T * R * H);
-    r.c = arena.get<float>((int64_t)r.T * R * H);
-    r.gates = arena.get<float>((int64_t)r.T * R * G);
-    if (!r.ptable && !(r.tc && r.step_xproj))
-      gemm_tn((int)((int64_t)r.T * R), G, D, A, lda, r.gather, WtS, D + H, r.gates, G, 0.f, xbias, 0);
-  } else {
-    r.h = arena.get<float>(2 * R * H);
-    r.c = arena.get<float>(2 * R * H);
-    r.gates = arena.get<float>(R * G);
-  }
+  const int64_t slots = save ? r.T : 2;
+  r.h = arena.get<float>(slots * R * H);
+  r.c = arena.get<float>(slots * R * H);
+  r.gates = arena.get<float>((save ? r.T : 1) * R * G);
+  if (save && !r.ptable && !xproj_by_caller) lstm_xproj(r, 0, r.T, r.gates);
 }
 
-void Engine::lstm_forward_step(LstmRun& r, int t) {
-  const int H = r.H, D = r.D, G = 4 * r.H;
-  const int64_t R = r.R;
-  const bool save = r.saved;
-  const float* WtS = Wtp(r.wseg);
+void Engine::lstm_forward_step(LstmRun& r, int t, bool xproj_by_caller) {
+  const int H = r.H, G = 4 * r.H;
+  const int64_t R = r.R, RH = R * H;
+  const int64_t slot = r.saved ? t : (t & 1), pslot = r.saved ? t - 1 : ((t - 1) & 1);
   const float* bias = Wp(r.wseg + 1);
-  const float* A = r.x ? r.x : Wp(0);
-  const int64_t lda = r.x ? D : cfg.E;
-  const float* xbias = r.tc ? bias : nullptr;
-  const int64_t slot = save ? t : (t & 1), pslot = save ? t - 1 : ((t - 1) & 1);
-  float* g = save ? r.gates + (int64_t)t * R * G : r.gates;
-  const float* hp = t > 0 ? r.h + pslot * R * H : r.h0;
-  const float* cp = t > 0 ? r.c + pslot * R * H : r.c0;
-  const bool per_step_x = !r.ptable && (!save || (r.tc && r.step_xproj));
-  if (r.f16) {
-    __half* g16 = save ? r.gates16 + (int64_t)t * R * G : nullptr;
-    const int32_t* mk = r.mask ? r.mask + (int64_t)t * R : nullptr;
+  const float* cp = t > 0 ? r.c + pslot * RH : r.c0;
+  const int32_t* mk = r.mask ? r.mask + (int64_t)t * R : nullptr;
+  if (r.route.fwd == LstmPath::Opt16) {
+    __half* g16 = r.saved ? r.gates16 + (int64_t)t * R * G : nullptr;
     const int32_t* tok = r.gather + (int64_t)t * R;
     float* h32 = t == r.T - 1 ? r.h32_last : nullptr;
     if (t == 0) {       // no recurrent term: a streaming kernel, accounted outside the roofline class
       LaunchCtx::Scope sc(&cx, "lstm_step_first", 0.0, R * (2.0 * G + 2.0 * G + 6.0 * H));
-      lstm16_first_step(cx, R, H, r.P16, tok, bias, cp, mk, g16, r.c + slot * R * H, r.h16 + slot * R * H, h32);
+      lstm16_first_step(cx, R, H, r.P16, tok, bias, cp, mk, g16, r.c + slot * RH, r.h16 + slot * RH, h32);
     } else {
       // algorithmic HBM bytes: fp16 gates out, fp32 c in + out, fp16 h in + out (the fp16 table gather is L2-resident: not counted)
       LaunchCtx::Scope sc(&cx, "lstm_step", 2.0 * R * G * H, R * (2.0 * G + 4.0 * H + 4.0 * H + 2.0 * H + 2.0 * H));
-      lstm16_step_fwd(cx, R, H, r.h16 + pslot * R * H, r.Wh16, r.P16, tok, bias, cp, mk, g16, r.c + slot * R * H,
-                      r.h16 + slot * R * H, h32);
+      lstm16_step_fwd(cx, R, H, r.h16 + pslot * RH, r.Wh16, r.P16, tok, bias, cp, mk, g16, r.c + slot * RH, r.h16 + slot * RH, h32);
     }
     return;
   }
+  LstmFwdStep s;
+  s.R = R; s.H = H; s.WhT = Wtp(r.wseg) + r.D; s.ldw = r.D + H; s.bias = bias; s.c_prev = cp; s.mask = mk;
+  s.h_prev = t > 0 ? r.h + pslot * RH : r.h0;
+  s.gates = r.saved ? r.gates + (int64_t)t * R * G : r.ptable ? nullptr : r.gates;    // a table-fed step that is not saved keeps no gates
+  if (r.ptable) { s.ptable = r.ptable; s.tok = r.gather + (int64_t)t * R; }
+  s.c_out = r.c + slot * RH; s.h_out = r.h + slot * RH;
+  const bool tc = r.route.fwd == LstmPath::Tc;
+  const bool x_per_step = !r.ptable && (!r.saved || xproj_by_caller);
   // the big (option-LSTM) launches run alone on the GPU: they are the roofline kernel class; the 320-row encoder
   // steps overlap on 4 streams and are accounted separately
   // EXECUTED work only: a gathered x-projection is a table lookup, and a first step without initial state has no
   // recurrent contraction at all (it is a streaming kernel, kept out of the roofline class)
-  const bool first_no_rec = r.tc && !hp;
+  const bool first_no_rec = tc && !s.h_prev;
   LaunchCtx::Scope sc(&cx, first_no_rec ? "lstm_step_first" : (R >= 4096 ? "lstm_step" : "lstm_step_small"),
-                      first_no_rec ? 0.0 : 2.0 * R * G * (H + (per_step_x ? D : 0)), 4.0 * R * (G + 4.0 * H));
-  if (r.tc) {
-    const int32_t* mk = r.mask ? r.mask + (int64_t)t * R : nullptr;
-    int has_x = 0;
-    if (!r.ptable) {
-      if (!save)        // a saved run's projection is batched in lstm_forward_begin, or issued by lstm_pair_forward
-        gemm_tn((int)R, G, D, r.x + (int64_t)t * R * D, lda, nullptr, WtS, D + H, g, G, 0.f, xbias, 0);
-      has_x = 1;
-    }
-    const int32_t* tok = r.ptable ? r.gather + (int64_t)t * R : nullptr;
-    if (!hp) {          // t = 0 without h0: no recurrent term, a plain streaming kernel (x-projection already has the bias)
-      lstm_first_step_fwd(cx, (save || has_x) ? g : nullptr, r.ptable, tok, nullptr, cp, mk, r.c + slot * R * H,
-                          r.h + slot * R * H, R, H);
-      return;
-    }
-    bool ok = lstm_step_fwd_tc(cx, R, H, hp, WtS + D, D + H, nullptr, (save || has_x) ? g : nullptr, has_x, r.ptable, tok, cp,
-                               r.c + slot * R * H, r.h + slot * R * H, mk);
-    VD_REQUIRE(ok, VD_E_STATE, "lstm_step_fwd_tc refused a shape the engine routed to it");
-    return;
-  }
-  if (!save) {
-    const float* At = r.x ? r.x + (int64_t)t * R * D : A;
-    gemm_tn((int)R, G, D, At, lda, r.gather ? r.gather + (int64_t)t * R : nullptr, WtS, D + H, g, G, 0.f, nullptr, 0);
-  }
-  if (hp) gemm_tn((int)R, G, H, hp, H, nullptr, WtS + D, D + H, g, G, 1.f, nullptr, 0);
-  lstm_pointwise_fwd(cx, g, bias, cp, r.mask ? r.mask + (int64_t)t * R : nullptr, r.c + slot * R * H, r.h + slot * R * H, R, H);
-}
-
-// the per-step x-projection of a `step_xproj` run, issued by the caller on the stream of its choice (cx.stream)
-void Engine::lstm_forward_xproj(LstmRun& r, int t) {
-  const int H = r.H, D = r.D, G = 4 * r.H;
-  const int64_t R = r.R;
-  VD_REQUIRE(r.tc && r.step_xproj && r.saved && r.x, VD_E_STATE, "lstm_forward_xproj: not a per-step projected run");
-  gemm_tn((int)R, G, D, r.x + (int64_t)t * R * D, D, nullptr, Wtp(r.wseg), D + H, r.gates + (int64_t)t * R * G, G, 0.f,
-          Wp(r.wseg + 1), 0);
+                      first_no_rec ? 0.0 : 2.0 * R * G * (H + (x_per_step ? r.D : 0)), 4.0 * R * (G + 4.0 * H));
+  if (x_per_step && !r.saved) lstm_xproj(r, t, 1, s.gates);
+  if (tc) lstm_tc_fwd_step(s); else lstm_simt_fwd_step(s);
 }
 
 void Engine::lstm_forward(LstmRun& r, bool save) {
+  r.route = route_lstm(r);
   lstm_forward_begin(r, save);
   for (int t = 0; t < r.T; ++t) lstm_forward_step(r, t);
 }
@@ -494,25 +525,14 @@ cudaEvent_t Engine::pool_event(size_t i) {
   return ev_pool[i];
 }
 
-// Wavefront over two stacked layers: layer-2 step t only needs layer-1 step t, so the two recurrences run one step
-// apart on streams sa and sb instead of back to back (the per-step kernels of these 320-row LSTMs are latency-bound), with
-// the contraction between the layers on a third stream sc.  Below this many rows the per-step contractions leave the
-// tensor-core path (M < 64) and the wavefront only adds launches and event traffic.
-constexpr int64_t kWavefrontMinRows = 64;
-
-void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc) {
-  // VD_MATH_F16: both layers and all time steps in ONE persistent launch (enc_lstm.cu) — weight slices stationary in
-  // shared memory, steps chained through global flags — instead of 3 launches per time step on three streams
-  if (math_mode == VD_MATH_F16 && !l1.h0 && !l1.c0 && !l2.h0 && !l2.c0 && !l1.gather && l1.x &&
-      l1.H == l2.H && l2.D == l1.H && l1.R == l2.R && l1.T == l2.T && l1.mask == l2.mask && enc_pair_shape_ok(l1.R, l1.H, cx.sm_count)) {
+void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, const PairStreams& s) {
+  cx.stream = s.a;
+  if (l1.route.fwd == LstmPath::Pair16) {
     const int H = l1.H, G = 4 * H, T = l1.T;
     const int64_t R = l1.R;
-    cx.stream = sa;
-    l1.pair16 = l2.pair16 = true;
     lstm_forward_begin(l1, true);               // h / c / gates of layer 1; gates1 <- x-projection + bias (batched GEMM)
     l2.x = l1.h;
-    l2.step_xproj = true;                       // no batched x-projection for layer 2: the kernel's projection CTAs compute it per step
-    lstm_forward_begin(l2, true);
+    lstm_forward_begin(l2, true, true);         // the kernel's projection CTAs compute layer 2's x-projection per step
     l1.h16 = arena.get<__half>((int64_t)T * R * H);
     l2.h16 = arena.get<__half>((int64_t)T * R * H);
     l2.x16 = l1.h16;
@@ -525,43 +545,41 @@ void Engine::lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaSt
     enc_pair_forward(cx, T, R, H, W1h, W2c, Wp(l2.wseg + 1), l1.mask, l1.gates, l1.c, l1.h, l1.h16, l2.gates, l2.c, l2.h, l2.h16, flags);
     return;
   }
-  // layer 2 projects its input per step on the tensor-core step path only (a batched projection would read h1 before it exists)
-  const bool pipelined = tcmode() && lstm_step_fwd_tc_ok(l2.H, Wtp(l2.wseg) + l2.D, l2.D + l2.H) && l2.R >= kWavefrontMinRows;
-  cx.stream = sa;
-  if (!pipelined) {
-    lstm_forward(l1, true);
+  if (!l1.route.wave_fwd) {
+    lstm_forward_begin(l1, true);
+    for (int t = 0; t < l1.T; ++t) lstm_forward_step(l1, t);
     l2.x = l1.h;
-    lstm_forward(l2, true);
+    lstm_forward_begin(l2, true);
+    for (int t = 0; t < l2.T; ++t) lstm_forward_step(l2, t);
     return;
   }
   lstm_forward_begin(l1, true);
   l2.x = l1.h;
-  l2.step_xproj = true;
   cudaEvent_t e0 = pool_event(0);
-  VD_CUDA_CHECK(cudaEventRecord(e0, sa));
-  VD_CUDA_CHECK(cudaStreamWaitEvent(sb, e0, 0));
-  cx.stream = sb;
-  lstm_forward_begin(l2, true);
+  VD_CUDA_CHECK(cudaEventRecord(e0, s.a));
+  VD_CUDA_CHECK(cudaStreamWaitEvent(s.b, e0, 0));
+  cx.stream = s.b;
+  lstm_forward_begin(l2, true, true);
   for (int t = 0; t < l1.T; ++t) {
-    cx.stream = sa;
+    cx.stream = s.a;
     lstm_forward_step(l1, t);
     cudaEvent_t e = pool_event(1 + t);
-    VD_CUDA_CHECK(cudaEventRecord(e, sa));
+    VD_CUDA_CHECK(cudaEventRecord(e, s.a));
     // layer 2's x-projection of step t needs h1_t only: on its own stream it runs beside layer 2's step t-1, so
     // each of the three chains advances by ONE kernel per time step
-    VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e, 0));
-    if (t == 0) VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e0, 0));
-    cx.stream = sc;
-    lstm_forward_xproj(l2, t);
+    VD_CUDA_CHECK(cudaStreamWaitEvent(s.c, e, 0));
+    if (t == 0) VD_CUDA_CHECK(cudaStreamWaitEvent(s.c, e0, 0));
+    cx.stream = s.c;
+    lstm_xproj(l2, t, 1, l2.gates + (int64_t)t * l2.R * 4 * l2.H);
     cudaEvent_t ex = pool_event(1 + l1.T + t);
-    VD_CUDA_CHECK(cudaEventRecord(ex, sc));
-    VD_CUDA_CHECK(cudaStreamWaitEvent(sb, ex, 0));
-    cx.stream = sb;
-    lstm_forward_step(l2, t);
+    VD_CUDA_CHECK(cudaEventRecord(ex, s.c));
+    VD_CUDA_CHECK(cudaStreamWaitEvent(s.b, ex, 0));
+    cx.stream = s.b;
+    lstm_forward_step(l2, t, true);
   }
-  VD_CUDA_CHECK(cudaEventRecord(e0, sb));
-  VD_CUDA_CHECK(cudaStreamWaitEvent(sa, e0, 0));
-  cx.stream = sa;
+  VD_CUDA_CHECK(cudaEventRecord(e0, s.b));
+  VD_CUDA_CHECK(cudaStreamWaitEvent(s.a, e0, 0));
+  cx.stream = s.a;
 }
 
 void Engine::lstm_backward_begin(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last) {
@@ -569,99 +587,77 @@ void Engine::lstm_backward_begin(LstmRun& r, const float* dh_all, const float* d
   const int H = r.H, G = 4 * r.H;
   const int64_t R = r.R, TR = (int64_t)r.T * R;
   r.dc_carry = arena.get<float>(R * H);
-  if (!r.f16) {
-    r.da = arena.get<float>(TR * G);
-    r.dh_rec = arena.get<float>(R * H);
-  }
-  r.bw_dh_all = dh_all; r.bw_dh_last = dh_last; r.bw_dc_last = dc_last;
-  if (r.f16) {
+  r.bw_dh_all = dh_all; r.bw_dh_last = dh_last;
+  if (r.route.bwd == LstmPath::Opt16) {
     VD_REQUIRE(dh_last && !dh_all && !dc_last, VD_E_STATE, "fp16 BPTT takes its gradient from the last step only");
     r.da16 = arena.get<__half>(TR * G);
     r.scale2 = arena.get<float>(4);
     pick_grad_scale(cx, dh_last, R * H, reinterpret_cast<uint32_t*>(r.scale2 + 2), r.scale2);
     return;
   }
-  r.bw_tc = tcmode() && lstm_step_bwd_tc_ok(H, Wp(r.wseg) + (int64_t)r.D * G);
-  if (r.bw_tc && dc_last)
+  r.da = arena.get<float>(TR * G);
+  r.dh_rec = arena.get<float>(R * H);
+  if (dc_last)
     VD_CUDA_CHECK(cudaMemcpyAsync(r.dc_carry, dc_last, (size_t)R * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
   else
     VD_CUDA_CHECK(cudaMemsetAsync(r.dc_carry, 0, (size_t)R * H * sizeof(float), cx.stream));
 }
 
 void Engine::lstm_backward_step(LstmRun& r, int t) {
-  const int H = r.H, D = r.D, G = 4 * r.H;
-  const int64_t R = r.R;
-  const float* Ws = Wp(r.wseg);            // (D+H, 4H)
-  const float* cp = t > 0 ? r.c + (int64_t)(t - 1) * R * H : r.c0;
-  const int32_t* mk = r.mask ? r.mask + (int64_t)t * R : nullptr;
-  float* da_t = r.da + (int64_t)t * R * G;
+  const int H = r.H, G = 4 * r.H;
+  const int64_t R = r.R, RH = R * H, RG = R * G;
   const bool last = t == r.T - 1;
-  const float* ext = r.bw_dh_all ? r.bw_dh_all + (int64_t)t * R * H : nullptr;
-  if (r.f16) {
-    const __half* g16 = r.gates16 + (int64_t)t * R * G;
-    __half* da16_t = r.da16 + (int64_t)t * R * G;
+  const float* cp = t > 0 ? r.c + (t - 1) * RH : r.c0;
+  const int32_t* mk = r.mask ? r.mask + (int64_t)t * R : nullptr;
+  if (r.route.bwd == LstmPath::Opt16) {
+    const __half* g16 = r.gates16 + t * RG;
+    __half* da16_t = r.da16 + t * RG;
     if (last) {
       LaunchCtx::Scope sc(&cx, "lstm_step_bwd_last", 0.0, R * (2.0 * G + 2.0 * G + 16.0 * H));
-      lstm16_bwd_last(cx, R, H, g16, cp, r.c + (int64_t)t * R * H, r.bw_dh_last, r.scale2, mk, r.dc_carry, da16_t);
+      lstm16_bwd_last(cx, R, H, g16, cp, r.c + t * RH, r.bw_dh_last, r.scale2, mk, r.dc_carry, da16_t);
     } else {
       LaunchCtx::Scope sc(&cx, "lstm_step_bwd", 2.0 * R * G * H, R * (3.0 * 2.0 * G + 16.0 * H));
-      lstm16_step_bwd(cx, R, H, r.da16 + (int64_t)(t + 1) * R * G, r.Whb16, g16, cp, r.c + (int64_t)t * R * H, r.dc_carry, mk, da16_t);
+      lstm16_step_bwd(cx, R, H, r.da16 + (t + 1) * RG, r.Whb16, g16, cp, r.c + t * RH, r.dc_carry, mk, da16_t);
     }
     return;
   }
-  LaunchCtx::Scope sc(&cx, (last && r.bw_tc) ? "lstm_step_bwd_last" : (R >= 4096 ? "lstm_step_bwd" : "lstm_step_bwd_small"), last ? 0.0 : 2.0 * R * G * H, 4.0 * R * (2.0 * G + 5.0 * H));
-  if (r.bw_tc) {
-    // one fused kernel per step: dh_rec = da_{t+1} Wh on wgmma, backward pointwise in the epilogue
-    if (last) {         // no recurrent gradient yet: pointwise only (dh_last rides in the recurrent slot)
-      lstm_pointwise_bwd(cx, r.gates + (int64_t)t * R * G, cp, r.c + (int64_t)t * R * H, r.bw_dh_last, ext, nullptr, r.dc_carry, mk,
-                         da_t, R, H);
-      return;
-    }
-    bool ok = lstm_step_bwd_tc(cx, R, H, r.da + (int64_t)(t + 1) * R * G, Ws + (int64_t)D * G, r.gates + (int64_t)t * R * G, cp,
-                               r.c + (int64_t)t * R * H, ext, r.dc_carry, mk, da_t);
-    VD_REQUIRE(ok, VD_E_STATE, "lstm_step_bwd_tc refused a shape the engine routed to it");
-    return;
-  }
-  const float* rec = last ? r.bw_dh_last : r.dh_rec;
-  lstm_pointwise_bwd(cx, r.gates + (int64_t)t * R * G, cp, r.c + (int64_t)t * R * H, rec, ext, last ? r.bw_dc_last : nullptr,
-                     r.dc_carry, mk, da_t, R, H);
-  if (t > 0) gemm_tn((int)R, H, G, da_t, G, nullptr, Ws + (int64_t)D * G, G, r.dh_rec, H, 0.f, nullptr, 0);
+  LstmBwdStep s;
+  s.R = R; s.H = H; s.Wh = Wp(r.wseg) + (int64_t)r.D * G; s.dc_carry = r.dc_carry; s.dh_rec = r.dh_rec; s.mask = mk;
+  s.da_next = last ? nullptr : r.da + (t + 1) * RG; s.dh_last = last ? r.bw_dh_last : nullptr;
+  s.dh_ext = r.bw_dh_all ? r.bw_dh_all + t * RH : nullptr;
+  s.gates = r.gates + t * RG; s.c_prev = cp; s.c_cur = r.c + t * RH; s.da = r.da + t * RG;
+  const bool tc = r.route.bwd == LstmPath::Tc;
+  LaunchCtx::Scope sc(&cx, (last && tc) ? "lstm_step_bwd_last" : (R >= 4096 ? "lstm_step_bwd" : "lstm_step_bwd_small"),
+                      last ? 0.0 : 2.0 * R * G * H, 4.0 * R * (2.0 * G + 5.0 * H));
+  if (tc) lstm_tc_bwd_step(s); else lstm_simt_bwd_step(s);
 }
 
 void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float* dc0_out) {
   const int H = r.H, D = r.D, G = 4 * r.H;
   const int64_t R = r.R, TR = (int64_t)r.T * R;
   const float* Ws = Wp(r.wseg);
-  float* da = r.da;
-  if (r.f16) VD_REQUIRE(!dh0_out && !dc0_out && !dx_out && !r.h0, VD_E_STATE, "fp16 BPTT: no initial-state / input gradients");
-  if (dh0_out) gemm_tn((int)R, H, G, da, G, nullptr, Ws + (int64_t)D * G, G, dh0_out, H, 0.f, nullptr, 0);
-  if (dc0_out) VD_CUDA_CHECK(cudaMemcpyAsync(dc0_out, r.dc_carry, (size_t)R * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
-  // accGradParameters
   float* dWs = dWp(r.wseg);
-  const float* A = r.x ? r.x : Wp(0);
-  const int64_t lda = r.x ? D : cfg.E;
-  const bool pair16 = r.pair16 && TR - R >= 256;
-  if (r.f16) {
-    if (r.T > 1) {
+  const bool opt16 = r.route.bwd == LstmPath::Opt16;
+  if (opt16) VD_REQUIRE(!dh0_out && !dc0_out && !dx_out && !r.h0, VD_E_STATE, "fp16 BPTT: no initial-state / input gradients");
+  if (dh0_out) gemm_tn((int)R, H, G, r.da, G, nullptr, Ws + (int64_t)D * G, G, dh0_out, H, 0.f, nullptr, 0);
+  if (dc0_out) VD_CUDA_CHECK(cudaMemcpyAsync(dc0_out, r.dc_carry, (size_t)R * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
+  // accGradParameters.  The fp16 routes' kernels left fp16 copies of h and da — the operands of the recurrence itself —
+  // so the weight gradients contract those on the fp16 tensor-core path (fp32 accumulation) instead of the TF32 one.  The
+  // persistent pair's shape check (enc_pair_shape_ok) already guarantees H % 64 == 0.
+  const bool wgrad16 = opt16 || (r.route.bwd == LstmPath::Pair16 && TR - R >= 256);
+  if (r.T > 1) {
+    if (wgrad16) {
       LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * H * G * (double)(TR - R), 2.0 * (double)(TR - R) * (H + G));
-      gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, r.scale2 + 1);
-    }
-  } else if (r.T > 1) {
-    // persistent pair (enc_lstm.cu): its kernels left fp16 copies of h and da — the operands of the recurrence itself — so the weight
-    // gradients contract those on the fp16 tensor-core path (fp32 accumulation) instead of the TF32 one.  The pair's shape check
-    // (enc_pair_shape_ok) already guarantees H % 64 == 0.
-    if (pair16) {
-      LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * H * G * (double)(TR - R), 2.0 * (double)(TR - R) * (H + G));
-      gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, nullptr);
-    } else gemm_atb(H, G, TR - R, r.h, H, nullptr, da + R * G, G, dWs + (int64_t)D * G, G);
+      gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, opt16 ? r.scale2 + 1 : nullptr);
+    } else gemm_atb(H, G, TR - R, r.h, H, nullptr, r.da + R * G, G, dWs + (int64_t)D * G, G);
   }
-  if (r.h0) gemm_atb(H, G, R, r.h0, H, nullptr, da, G, dWs + (int64_t)D * G, G);
-  if (!r.x && tcmode()) {
+  if (r.h0) gemm_atb(H, G, R, r.h0, H, nullptr, r.da, G, dWs + (int64_t)D * G, G);
+  if (r.route.table_grad) {
     // Embedding-gathered input: every x_t is a row of the (V+1, E) table, so the three x-side gradients collapse
     // onto the table.  dP[v] = sum of da over the rows whose token is v (counting sort + balanced segmented sum,
     // HBM-bound) and then  dWx += E^T dP,  db += colsum(dP),  dEmb += dP Wx^T  are (V+1)-row contractions instead
     // of T*R-row ones (2 x 786 GFLOP -> 2 x 12 GFLOP for the 100 x 20-token option LSTM).
-    VD_REQUIRE(D == cfg.E, VD_E_STATE, "gathered LSTM input must be the word embedding");
+    VD_REQUIRE(dx_out == nullptr, VD_E_STATE, "projected-space embedding gradient: caller must not ask for dx");
     const int V1 = cfg.V + 1;
     float* dP = arena.get<float>((int64_t)V1 * G);
     VD_CUDA_CHECK(cudaMemsetAsync(dP, 0, (size_t)V1 * G * sizeof(float), cx.stream));
@@ -669,24 +665,23 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
     int32_t* perm = arena.get<int32_t>(TR);
     int32_t* stok = arena.get<int32_t>(TR);
     {
-      LaunchCtx::Scope sc(&cx, "embed_grad_segsum", 0.0, (r.f16 ? 2.0 : 4.0) * TR * G);
+      LaunchCtx::Scope sc(&cx, "embed_grad_segsum", 0.0, (opt16 ? 2.0 : 4.0) * TR * G);
       group_rows_by_token(cx, r.gather, TR, V1, scratch, perm, stok);
-      if (r.f16) segsum_rows16(cx, r.da16, G, perm, stok, TR, dP, G, r.scale2 + 1);
-      else segsum_rows(cx, da, G, perm, stok, TR, dP, G);
+      if (opt16) segsum_rows16(cx, r.da16, G, perm, stok, TR, dP, G, r.scale2 + 1);
+      else segsum_rows(cx, r.da, G, perm, stok, TR, dP, G);
     }
     gemm_atb(D, G, V1, Wp(0), cfg.E, nullptr, dP, G, dWs, G);
     colsum_add(cx, dWp(r.wseg + 1), dP, V1, G, G);
     if (r.demb_out) gemm_tn(V1, D, G, dP, G, nullptr, Ws, G, r.demb_out, cfg.E, 0.f, nullptr, 0);   // folded in by the caller
     else gemm_tn(V1, D, G, dP, G, nullptr, Ws, G, dWp(0), cfg.E, 1.f, nullptr, 0);
-    VD_REQUIRE(dx_out == nullptr, VD_E_STATE, "projected-space embedding gradient: caller must not ask for dx");
     return;
   }
-  if (pair16 && r.x16) {            // layer 2 of the pair: x = h1, D = H
+  if (wgrad16 && r.x16) {            // layer 2 of the pair: x = h1, D = H
     LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * D * G * (double)TR, 2.0 * (double)TR * (D + G));
     gemm_atb16(cx, D, G, TR, r.x16, D, r.da16, G, dWs, G, nullptr);
-  } else gemm_atb(D, G, TR, A, lda, r.gather, da, G, dWs, G);
-  colsum_add(cx, dWp(r.wseg + 1), da, TR, G, G);
-  if (dx_out) gemm_tn((int)TR, D, G, da, G, nullptr, Ws, G, dx_out, D, 0.f, nullptr, 0);
+  } else gemm_atb(D, G, TR, r.x ? r.x : Wp(0), r.x ? D : cfg.E, r.gather, r.da, G, dWs, G);
+  colsum_add(cx, dWp(r.wseg + 1), r.da, TR, G, G);
+  if (dx_out) gemm_tn((int)TR, D, G, r.da, G, nullptr, Ws, G, dx_out, D, 0.f, nullptr, 0);
 }
 
 void Engine::lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last, float* dx_out,
@@ -696,18 +691,18 @@ void Engine::lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last
   lstm_backward_end(r, dx_out, dh0_out, dc0_out);
 }
 
-// BPTT wavefront of two stacked layers: layer-1 step t needs d(h1_t) = da2_t Wx2^T, produced per step on stream sc,
-// so the two recurrences again run one step apart (layer 2 on sb, layer 1 on sa).
+// BPTT wavefront of two stacked layers: layer-1 step t needs d(h1_t) = da2_t Wx2^T, produced per step on stream c,
+// so the two recurrences again run one step apart (layer 2 on b, layer 1 on a).
 void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2, const float* dc_last2, const float* dh_last1,
-                                const float* dc_last1, float* dx1_out, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc) {
+                                const float* dc_last1, float* dx1_out, const PairStreams& s) {
   const int H = l2.H, G = 4 * l2.H;
   const int64_t R = l2.R;
-  if (l1.pair16) {
-    // the forward of this pair ran as the persistent kernel: so does its BPTT (enc_lstm.cu::k_enc_pair_bwd) — one launch for
-    // both layers and all time steps; the weight / input gradients follow as batched contractions over all T*R rows
+  cx.stream = s.a;
+  if (l1.route.bwd == LstmPath::Pair16) {
+    // one launch for both layers and all time steps (enc_lstm.cu::k_enc_pair_bwd); the weight / input gradients follow
+    // as batched contractions over all T*R rows
     const int T = l2.T;
     const int64_t TR = (int64_t)T * R;
-    cx.stream = sa;
     l1.da = arena.get<float>(TR * G); l2.da = arena.get<float>(TR * G);
     l1.da16 = arena.get<__half>(TR * G); l2.da16 = arena.get<__half>(TR * G);
     __half* Whb2 = arena.get<__half>((int64_t)H * G);
@@ -728,43 +723,40 @@ void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2,
     return;
   }
   float* dx2 = arena.get<float>((int64_t)l2.T * R * l2.D);      // = gradient wrt layer-1 outputs, all steps
-  const bool pipelined = tcmode() && lstm_step_bwd_tc_ok(H, Wp(l1.wseg) + (int64_t)l1.D * G) &&
-                         lstm_step_bwd_tc_ok(H, Wp(l2.wseg) + (int64_t)l2.D * G) && R >= kWavefrontMinRows;
-  cx.stream = sa;
-  if (!pipelined) {
+  if (!l1.route.wave_bwd) {
     lstm_backward(l2, nullptr, dh_last2, dc_last2, dx2, nullptr, nullptr);
     lstm_backward(l1, dx2, dh_last1, dc_last1, dx1_out, nullptr, nullptr);
     return;
   }
   const float* Wx2 = Wp(l2.wseg);            // rows 0..D2 of (D2+H, 4H): [N = D2, K = 4H]
   cudaEvent_t e0 = pool_event(0);
-  VD_CUDA_CHECK(cudaEventRecord(e0, sa));
-  VD_CUDA_CHECK(cudaStreamWaitEvent(sb, e0, 0));
-  cx.stream = sb;
+  VD_CUDA_CHECK(cudaEventRecord(e0, s.a));
+  VD_CUDA_CHECK(cudaStreamWaitEvent(s.b, e0, 0));
+  cx.stream = s.b;
   lstm_backward_begin(l2, nullptr, dh_last2, dc_last2);
-  cx.stream = sa;
+  cx.stream = s.a;
   lstm_backward_begin(l1, dx2, dh_last1, dc_last1);
   for (int t = l2.T - 1; t >= 0; --t) {
-    cx.stream = sb;
+    cx.stream = s.b;
     lstm_backward_step(l2, t);
     // d(h1_t) = da2_t Wx2 needs layer 2's step t only: on its own stream it runs beside layer 2's step t-1
     cudaEvent_t e = pool_event(1 + t);
-    VD_CUDA_CHECK(cudaEventRecord(e, sb));
-    VD_CUDA_CHECK(cudaStreamWaitEvent(sc, e, 0));
-    cx.stream = sc;
+    VD_CUDA_CHECK(cudaEventRecord(e, s.b));
+    VD_CUDA_CHECK(cudaStreamWaitEvent(s.c, e, 0));
+    cx.stream = s.c;
     gemm_tn((int)R, l2.D, G, l2.da + (int64_t)t * R * G, G, nullptr, Wx2, G, dx2 + (int64_t)t * R * l2.D, l2.D, 0.f, nullptr, 0);
     cudaEvent_t ex = pool_event(1 + l2.T + t);
-    VD_CUDA_CHECK(cudaEventRecord(ex, sc));
-    VD_CUDA_CHECK(cudaStreamWaitEvent(sa, ex, 0));
-    cx.stream = sa;
+    VD_CUDA_CHECK(cudaEventRecord(ex, s.c));
+    VD_CUDA_CHECK(cudaStreamWaitEvent(s.a, ex, 0));
+    cx.stream = s.a;
     lstm_backward_step(l1, t);
   }
-  cx.stream = sb;
+  cx.stream = s.b;
   lstm_backward_end(l2, nullptr, nullptr, nullptr);       // weight gradients of layer 2 (its dx was produced per step)
-  VD_CUDA_CHECK(cudaEventRecord(e0, sb));
-  cx.stream = sa;
+  VD_CUDA_CHECK(cudaEventRecord(e0, s.b));
+  cx.stream = s.a;
   lstm_backward_end(l1, dx1_out, nullptr, nullptr);
-  VD_CUDA_CHECK(cudaStreamWaitEvent(sa, e0, 0));
+  VD_CUDA_CHECK(cudaStreamWaitEvent(s.a, e0, 0));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -911,17 +903,12 @@ void Engine::encoder_forward(const vd_batch* b) {
     embed_rows(cx, xh, Wp(0), ids_h, N * db.Th, E, embdrop ? d05 : dnone, SITE_HEMBED);
     hist1 = make_run(db.Th, N, E, H, seg("hist.lstm1.weight"), xh, nullptr, ids_h);
     hist2 = make_run(db.Th, N, H, H, seg("hist.lstm2.weight"), nullptr, nullptr, ids_h);
-  }
-  // The 2nd layer consumes every step of the 1st, so encoder LSTMs always keep all steps (T*N*H is small).
-  auto run_two = [&](LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc) { lstm_pair_forward(l1, l2, sa, sb, sc); };
-  // The history and question LSTM chains are independent until the fusion/attention stage: the history chain runs
-  // on the side stream (its tiny per-step kernels are latency-bound; overlapping the two chains hides half of it).
-  // (the persistent pair kernels of VD_MATH_F16 are flag-chained grids that want every SM: two of them must never be
-  //  co-scheduled — neither could become fully resident — so in that mode both pairs run on the main stream, in order)
-  const bool serial_pairs = math_mode == VD_MATH_F16;
-  if (cfg.useHist) {
-    if (serial_pairs) { join_side(); run_two(hist1, hist2, main_stream, main2_stream, main3_stream); }
-    else { fork_side(); run_two(hist1, hist2, side_stream, side2_stream, side3_stream); back_to_main(); }
+    route_lstm_pair(hist1, hist2);
+    // The 2nd layer consumes every step of the 1st, so encoder LSTMs always keep all steps (T*N*H is small).
+    // The history and question LSTM chains are independent until the fusion/attention stage: the history chain runs
+    // on the side stream (its tiny per-step kernels are latency-bound; overlapping the two chains hides half of it).
+    if (serial_pairs()) { join_side(); lstm_pair_forward(hist1, hist2, main_chain); }
+    else { lstm_pair_forward(hist1, hist2, side_chain); back_to_main(); }
   }
   // question branch
   xq = arena.get<float>(N * db.Tq * E);
@@ -941,7 +928,8 @@ void Engine::encoder_forward(const vd_batch* b) {
     ques1 = make_run(db.Tq, N, E, H, seg("ques.lstm1.weight"), xq, nullptr, ids_q);
   }
   ques2 = make_run(db.Tq, N, H, H, seg("ques.lstm2.weight"), nullptr, nullptr, ids_q);
-  run_two(ques1, ques2, main_stream, main2_stream, main3_stream);
+  route_lstm_pair(ques1, ques2);
+  lstm_pair_forward(ques1, ques2, main_chain);
   join_side();
   const float* q3 = ques2.h_last();
   const float* h3 = cfg.useHist ? hist2.h_last() : nullptr;
@@ -1099,22 +1087,19 @@ void Engine::encoder_backward(const float* dEnc) {
   // question LSTMs (+ gradients handed back by the gen decoder, gen.lua:45-60); the history chain's BPTT runs
   // concurrently on the side stream (disjoint weight segments; the shared embedding gradient is atomics-only)
   const bool embdrop = cfg.embdrop;
-  // (persistent pair kernels must not be co-scheduled — see encoder_forward: in that mode both BPTTs run on the main stream)
-  const bool serial_pairs = hist1.pair16;
   if (cfg.useHist) {
-    if (serial_pairs) { join_side(); cx.stream = main_stream; } else fork_side();
-    cudaStream_t hs = serial_pairs ? main_stream : side_stream;
+    if (serial_pairs()) join_side(); else fork_side();
+    const PairStreams& hs = serial_pairs() ? main_chain : side_chain;
     float* dx1 = arena.get<float>(N * db.Th * E);
-    lstm_pair_backward(hist1, hist2, dh3, nullptr, nullptr, nullptr, dx1, hs, serial_pairs ? main2_stream : side2_stream,
-                       serial_pairs ? main3_stream : side3_stream);
-    reduce_segments(seg("hist.lstm1.weight"), seg("hist.lstm2.weight") + 1, hs);                // bucket 2
+    lstm_pair_backward(hist1, hist2, dh3, nullptr, nullptr, nullptr, dx1, hs);
+    reduce_segments(seg("hist.lstm1.weight"), seg("hist.lstm2.weight") + 1, hs.a);              // bucket 2
     embed_scatter_add(cx, dWp(0), dx1, E, ids_h, N * db.Th, E, embdrop ? d05 : dnone, SITE_HEMBED);
     back_to_main();
   }
   {
     int D1 = ques1.D;
     float* dx1 = arena.get<float>(N * db.Tq * D1);
-    lstm_pair_backward(ques1, ques2, dq3, conn_dc_l2, conn_dh_l1, conn_dc_l1, dx1, main_stream, main2_stream, main3_stream);
+    lstm_pair_backward(ques1, ques2, dq3, conn_dc_l2, conn_dh_l1, conn_dc_l1, dx1, main_chain);
     reduce_segments(seg("ques.lstm1.weight"), seg("ques.lstm2.weight") + 1, main_stream);       // bucket 3
     embed_scatter_add(cx, dWp(0), dx1, D1, ids_q, N * db.Tq, E, embdrop ? d05 : dnone, SITE_QEMBED);
     if (cfg.img_in_q) {
@@ -1314,7 +1299,7 @@ void Engine::decoder_backward() {
       cx.stream = opt_stream;
       cx.sm_budget = cx.sm_count - opt_reserve_sms;
     }
-    if (tcmode()) {
+    if (opt.route.table_grad) {
       // embedding gradient in projected space; written to a private (V+1,E) buffer when overlapped, because the
       // encoder's embedding gradients accumulate into dW(wordEmbed) with atomics at the same time
       opt.demb_out = opt_overlap ? (opt_demb = arena.get<float>((int64_t)(cfg.V + 1) * E)) : nullptr;

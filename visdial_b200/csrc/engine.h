@@ -55,6 +55,17 @@ struct Arena {
   void release();
 };
 
+// The kernels an nn.SeqLSTM run executes on.  Simt: a GEMM and a pointwise kernel per step on the CUDA cores.  Tc: fused
+// wgmma step kernels (lstm_step_fwd_tc / _bwd_tc).  Opt16: VD_MATH_F16 many-row LSTM over embedding-gathered tokens with
+// fp16 h / gates / da / table (lstm16.cu).  Pair16: VD_MATH_F16 persistent kernel of two stacked layers (enc_lstm.cu).
+enum class LstmPath { Simt, Tc, Opt16, Pair16 };
+// Decided once per run by Engine::route_lstm / route_lstm_pair, when the run's forward begins
+struct LstmRoute {
+  LstmPath fwd = LstmPath::Simt, bwd = LstmPath::Simt;   // the forward and backward step kernels have different predicates
+  bool table_grad = false;           // embedding-gathered input: the x-side gradients contract the (V+1, 4H) projected table
+  bool wave_fwd = false, wave_bwd = false;   // stacked pair: the two layers run one step apart on three streams
+};
+
 // one nn.SeqLSTM execution (forward state kept for BPTT)
 struct LstmRun {
   int T = 0; int64_t R = 0; int D = 0, H = 0;
@@ -66,25 +77,37 @@ struct LstmRun {
   float* h = nullptr; float* c = nullptr; float* gates = nullptr;
   bool saved = false;
   float* demb_out = nullptr;         // projected-space embedding gradient goes here (overwritten) instead of dW(wordEmbed) +=
-  // forward run state (lstm_forward_begin / _step)
-  bool tc = false;                   // fused wgmma step kernels
-  bool step_xproj = false;           // layer 2 of a pair: lstm_pair_forward projects its input per step instead of batched
-  const float* ptable = nullptr;     // (V+1, 4H) projection table for embedding-gathered inputs
+  LstmRoute route;
+  const float* ptable = nullptr;     // Tc, gathered input: (V+1, 4H) projection table (+ bias)
   // backward run state (lstm_backward_begin / _step / _end)
   float* da = nullptr; float* dc_carry = nullptr; float* dh_rec = nullptr;
-  const float* bw_dh_all = nullptr; const float* bw_dh_last = nullptr; const float* bw_dc_last = nullptr;
-  bool bw_tc = false;
-  // VD_MATH_F16 run state (lstm16.cu): fp16 h / activated gates / da and x-projection table, fp32 c; `h` and `gates` stay null
-  bool f16 = false;
+  const float* bw_dh_all = nullptr; const float* bw_dh_last = nullptr;
+  // fp16 state of Opt16 (`h` and `gates` stay null) and Pair16
   __half *h16 = nullptr, *gates16 = nullptr, *da16 = nullptr, *P16 = nullptr, *Wh16 = nullptr, *Whb16 = nullptr;
-  // set on both runs by lstm_pair_forward when the pair ran as the persistent kernel (enc_lstm.cu): the BPTT takes the same
-  // route, and the weight gradients contract the fp16 h / da it leaves
-  bool pair16 = false;
-  const __half* x16 = nullptr;       // fp16 copy of x when a persistent pair produced one (layer 2: the h1 sequence)
-  float* h32_last = nullptr;         // fp32 copy of the last step's h (what the fp32 consumers of the run read)
-  float* scale2 = nullptr;           // device {s, 1/s}: power-of-two scale of the BPTT (chosen from max|dL/dh_T|)
-  const float* h_last() const { return f16 ? h32_last : h + (int64_t)(saved ? T - 1 : (T - 1) & 1) * R * H; }
+  const __half* x16 = nullptr;       // Pair16 layer 2: fp16 copy of x (the h1 sequence)
+  float* h32_last = nullptr;         // Opt16: fp32 copy of the last step's h (what the fp32 consumers of the run read)
+  float* scale2 = nullptr;           // Opt16: device {s, 1/s}, power-of-two scale of the BPTT (chosen from max|dL/dh_T|)
+  const float* h_last() const { return route.fwd == LstmPath::Opt16 ? h32_last : h + (int64_t)(saved ? T - 1 : (T - 1) & 1) * R * H; }
   const float* c_last() const { return c + (int64_t)(saved ? T - 1 : (T - 1) & 1) * R * H; }
+};
+
+// Operands of one step on the fp32 routes.  Forward: h_prev null = first step without initial state, c_prev null = zero;
+// gates holds the x-projection on entry (null with a table x side when the run keeps no gates) and the activated gates on
+// exit; bias is read by Simt only (the Tc kernels take it from the x-projection).  WhT = [4H, ldw] h columns of the
+// transposed shadow.  Backward: Wh = [H, 4H] h rows of the weight; da_next null at the last step, where dh_last takes the
+// recurrent slot; dc_carry in: dc from step t+1, out: dc for step t-1; dh_rec: Simt scratch (R, H).
+struct LstmFwdStep {
+  int64_t R = 0, ldw = 0; int H = 0;
+  const float *WhT = nullptr, *bias = nullptr, *h_prev = nullptr, *c_prev = nullptr, *ptable = nullptr;
+  const int32_t *tok = nullptr, *mask = nullptr;
+  float *gates = nullptr, *c_out = nullptr, *h_out = nullptr;
+};
+struct LstmBwdStep {
+  int64_t R = 0; int H = 0;
+  const float *Wh = nullptr, *da_next = nullptr, *dh_last = nullptr, *dh_ext = nullptr, *gates = nullptr, *c_prev = nullptr,
+              *c_cur = nullptr;
+  const int32_t* mask = nullptr;
+  float *dc_carry = nullptr, *da = nullptr, *dh_rec = nullptr;
 };
 
 struct DevBatch {
@@ -131,6 +154,10 @@ struct Engine {
   cudaEvent_t t0 = nullptr, t1 = nullptr;
   // side stream for the independent history-LSTM chain (cx.stream is switched while its kernels are issued)
   cudaStream_t main_stream = nullptr, side_stream = nullptr;
+  // the streams of one chain's LSTM pair: a = the chain's own stream (layer 1), b = layer 2, c = the contraction between the
+  // layers of every step (layer 2's x-projection forward, layer 1's incoming gradient backward)
+  struct PairStreams { cudaStream_t a = nullptr, b = nullptr, c = nullptr; };
+  PairStreams main_chain, side_chain;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   bool side_active = false;
   void fork_side();
@@ -190,20 +217,36 @@ struct Engine {
   void linear_bwd(int wseg, const float* x, const float* dy, int64_t rows, float* dx, float beta_dx);
   void refresh_shadows();
   void stage_batch(const vd_batch* b);
-  void lstm_forward(LstmRun& r, bool save);
-  void lstm_forward_begin(LstmRun& r, bool save);
-  void lstm_forward_step(LstmRun& r, int t);
+  // The route of one SeqLSTM run, the only place where the math mode and the kernels' predicates pick an LSTM's kernels.
+  // gathered: rows of the word embedding; WhT / ldw: h columns of the transposed shadow; Wh: h rows of the weight.
+  LstmRoute route_lstm(int64_t R, int H, bool gathered, bool has_h0, const float* WhT, int64_t ldw, const float* Wh) const;
+  LstmRoute route_lstm(const LstmRun& r) const {
+    return route_lstm(r.R, r.H, r.gather != nullptr, r.h0 != nullptr, Wtp(r.wseg) + r.D, r.D + r.H,
+                      Wp(r.wseg) + (int64_t)r.D * 4 * r.H);
+  }
+  // the routes of two stacked runs (layer 2 reads layer 1's h): both layers as one persistent kernel, or the wavefront
+  void route_lstm_pair(LstmRun& l1, LstmRun& l2) const;
+  // one step on each fp32 route; the Tc steps return the tile width that ran (0: the pointwise kernel)
+  void lstm_simt_fwd_step(const LstmFwdStep& s);
+  int lstm_tc_fwd_step(const LstmFwdStep& s);
+  void lstm_simt_bwd_step(const LstmBwdStep& s);
+  int lstm_tc_bwd_step(const LstmBwdStep& s);
+  void lstm_forward(LstmRun& r, bool save);          // routes the run, then runs it
+  // xproj_by_caller: layer 2 of a pair, whose x-projection lstm_pair_forward (or the persistent kernel) issues per step
+  void lstm_forward_begin(LstmRun& r, bool save, bool xproj_by_caller = false);
+  void lstm_forward_step(LstmRun& r, int t, bool xproj_by_caller = false);
+  void lstm_xproj(const LstmRun& r, int t0, int nt, float* gates);   // gates of steps [t0, t0 + nt) <- x W_x^T (+ bias)
   void lstm_backward_begin(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last);
   void lstm_backward_step(LstmRun& r, int t);
   void lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float* dc0_out);
-  // two stacked SeqLSTMs as a wavefront: layer 2 step t runs (on its own stream) as soon as layer 1 step t is done
-  // (sc: a third stream for the inter-layer contraction of every step — layer 2's x-projection forward, layer 1's
-  //  incoming gradient backward — which depends on one layer's step t only, not on the other layer's recurrence)
-  void lstm_pair_forward(LstmRun& l1, LstmRun& l2, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc);
+  // two stacked SeqLSTMs, routed by route_lstm_pair.  As a wavefront, layer 2 step t runs (on its own stream) as soon as
+  // layer 1 step t is done, and the inter-layer contraction of every step depends on one layer's step t only.
+  void lstm_pair_forward(LstmRun& l1, LstmRun& l2, const PairStreams& s);
   void lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2, const float* dc_last2, const float* dh_last1,
-                          const float* dc_last1, float* dx1_out, cudaStream_t sa, cudaStream_t sb, cudaStream_t sc);
-  void lstm_forward_xproj(LstmRun& r, int t);
-  cudaStream_t main2_stream = nullptr, side2_stream = nullptr, main3_stream = nullptr, side3_stream = nullptr;
+                          const float* dc_last1, float* dx1_out, const PairStreams& s);
+  // Persistent pair kernels are flag-chained grids that want every SM: two of them must never be co-scheduled (neither
+  // could become fully resident), so when the encoder's pairs run as such the two chains run in order on the main stream.
+  bool serial_pairs() const { return cfg.useHist && hist1.route.fwd == LstmPath::Pair16; }
   // The disc decoder's option LSTM (disc.lua:4-20) does not depend on the encoder until the final dot product, and its
   // BPTT does not feed the encoder's: both run on their own low-priority stream, concurrently with the encoder's
   // latency-bound chains (which keep priority for SMs as they free up).
