@@ -230,6 +230,19 @@ int vd_lstm_step_fwd(vd_engine* e, int64_t R, int32_t H, const float* h_prev, co
 int vd_lstm_step_bwd(vd_engine* e, int64_t R, int32_t H, const float* da_next, const float* Wh, const float* gates,
                      const float* c_prev, const float* c_cur, const float* dh_ext, float* dc_carry, const int32_t* mask_ids,
                      float* da, int32_t* path);
+/* test hooks of the VD_MATH_F16 option-LSTM step kernels (lstm16.cu) on caller-provided DEVICE buffers, row-major; "16"
+ * buffers hold IEEE binary16, the others fp32.  Shapes as the engine routes them there: H % 256 == 0, H <= 512, R >= 1024.
+ * fwd: z[r] = bias + ptable16[tok[r]] + h_prev16[r] Wh16^T   (Wh16 (4H, H), ptable16 (V, 4H) without bias, whose row 0 =
+ *      the pad token's = zeros), gates16 (R, 4H) <- [sigmoid(z_i) sigmoid(z_f) sigmoid(z_o) tanh(z_g)] unless NULL,
+ *      c_out = f c_prev + i g (c_prev NULL = zeros), h16_out = o tanh(c_out), h32_out (NULL or fp32) = the same h;
+ *      rows whose mask id is 0 are all zero.
+ * bwd: dh = da_next16[r] Whb16^T (Whb16 (H, 4H)), d = dc_carry + dh o (1 - tanh^2 c_cur),
+ *      da16 <- [d g i(1-i)  d c_prev f(1-f)  dh tanh(c_cur) o(1-o)  d i(1-g^2)], dc_carry <- d f; c_prev NULL = zeros. */
+int vd_lstm16_step_fwd(vd_engine* e, int64_t R, int32_t H, const void* h_prev16, const void* Wh16, const void* ptable16,
+                       const int32_t* tok, const float* bias, const float* c_prev, const int32_t* mask_ids, void* gates16,
+                       float* c_out, void* h16_out, float* h32_out);
+int vd_lstm16_step_bwd(vd_engine* e, int64_t R, int32_t H, const void* da_next16, const void* Whb16, const void* gates16,
+                       const float* c_prev, const float* c_cur, float* dc_carry, const int32_t* mask_ids, void* da16);
 /* cudaProfilerStart / cudaProfilerStop (ncu --profile-from-start off) */
 int vd_profiler_range(vd_engine* e, int32_t start);
 /* flush L2 by writing a scratch buffer larger than L2 (bench hygiene) */

@@ -421,6 +421,31 @@ int vd_lstm_step_bwd(vd_engine* h, int64_t R, int32_t H, const float* da_next, c
     if (s.dh_rec) cudaFree(s.dh_rec);
   })
 }
+int vd_lstm16_step_fwd(vd_engine* h, int64_t R, int32_t H, const void* h_prev16, const void* Wh16, const void* ptable16,
+                       const int32_t* tok, const float* bias, const float* c_prev, const int32_t* mask_ids, void* gates16,
+                       float* c_out, void* h16_out, float* h32_out) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(h_prev16 && Wh16 && ptable16 && tok && bias && c_out && h16_out, VD_E_BADARG, "vd_lstm16_step_fwd: arguments");
+    VD_REQUIRE(vd::lstm16_shape_ok(R, H), VD_E_BADARG, "vd_lstm16_step_fwd: shape");
+    VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
+    vd::lstm16_step_fwd(e->cx, R, H, (const __half*)h_prev16, (const __half*)Wh16, (const __half*)ptable16, tok, bias, c_prev,
+                        mask_ids, (__half*)gates16, c_out, (__half*)h16_out, h32_out);
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+  })
+}
+int vd_lstm16_step_bwd(vd_engine* h, int64_t R, int32_t H, const void* da_next16, const void* Whb16, const void* gates16,
+                       const float* c_prev, const float* c_cur, float* dc_carry, const int32_t* mask_ids, void* da16) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(da_next16 && Whb16 && gates16 && c_cur && dc_carry && da16, VD_E_BADARG, "vd_lstm16_step_bwd: arguments");
+    VD_REQUIRE(vd::lstm16_shape_ok(R, H), VD_E_BADARG, "vd_lstm16_step_bwd: shape");
+    VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
+    vd::lstm16_step_bwd(e->cx, R, H, (const __half*)da_next16, (const __half*)Whb16, (const __half*)gates16, c_prev, c_cur,
+                        dc_carry, mask_ids, (__half*)da16);
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+  })
+}
 
 int vd_profiler_range(vd_engine* h, int32_t start) {
   VD_TRY({

@@ -9,9 +9,12 @@
 // are stored as fp16, the contractions run as f16 wgmma (2x the TF32 rate) with fp32 accumulation,
 // and c_t, dc, every accumulator, the weight gradients and the final h_T that meets the encoder stay fp32.
 //
-//   k_lstm16_fwd   : gates = h_{t-1} Wh^T (wgmma, 128x128 tiles) + P16[token] + bias -> pointwise -> fp16 gates,
+//   k_lstm16<0>    : gates = h_{t-1} Wh^T (wgmma, 128x128 tiles) + P16[token] + bias -> pointwise -> fp16 gates,
 //                    fp32 c_t, fp16 h_t (+ fp32 h_T on the last step)
-//   k_lstm16_bwd   : dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t, fp32 dc carry
+//   k_lstm16<1>    : dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t, fp32 dc carry
+//   Both run their pointwise epilogue on the accumulator registers (no shared-memory accumulator tile), which leaves room
+//   for a 5-stage (forward) / 4-stage (backward) operand ring of 32 KB stages; the epilogue inputs are fetched by cp.async
+//   before the tile's contraction (the backward: those of its first 32 hidden units).
 //   k_atb16        : dWh += inv_scale * h^T da  (both operands MN-major fp16, split-K, red.global.add)
 //   k_lstm16_first / k_lstm16_bwd_last / k_segsum16 / k_cvt16 / k_amax / k_pick_scale : streaming helpers
 #include <cuda.h>
@@ -27,7 +30,7 @@ constexpr int BM16 = 128;        // rows per tile (two 64-row wgmma slabs)
 constexpr int BK16 = 64;         // halves per k-block = one 128-byte swizzle row
 constexpr int UK16 = 16;         // f16 wgmma: 32 bytes per instruction
 constexpr int BN16 = 128;        // accumulator columns per tile: forward 32 hidden units x 4 gates, backward 128 hidden units
-constexpr int EW16 = 8;          // consumer warps = epilogue warps: 2 per 32-row quarter
+constexpr int EW16 = 8;          // consumer warps = epilogue warps: 16 rows of a tile each
 constexpr int STAGE16 = 32768;   // 16 KB of A (128 rows) + 16 KB of B (128 rows)
 
 // Activations of the fp16 option LSTM: ONE special-function op each (tanh.approx.f32, relative error 2^-11 — the rounding class of the fp16
@@ -54,17 +57,18 @@ __device__ __forceinline__ void unpack8(const uint4 u, float* v) {
   for (int i = 0; i < 4; ++i) { const float2 f = __half22float2(h[i]); v[2 * i] = f.x; v[2 * i + 1] = f.y; }
 }
 
-// ---- epilogue staging tiles (one set per epilogue warp, 32 rows each).  Two geometries, both laid out exactly like the
-// TMA box that leaves (or could enter) them, so stores are single bulk-tensor instructions:
-//   S32: [32 rows][16 halves] = 32-byte rows, 16-byte chunk c of row r at  r*32 + ((c ^ ((r>>2)&1)) << 4)   (SWIZZLE_32B)
-//   S64: [32 rows][16 floats] = 64-byte rows, 16-byte chunk c of row r at  r*64 + ((c ^ ((r>>1)&3)) << 4)   (SWIZZLE_64B)
-// Both are bank-conflict free for "thread = row" 16-byte accesses and for the coalesced global side.
-constexpr int S32_BYTES = 1024, S64_BYTES = 2048;
-__device__ __forceinline__ uint4* s32_at(uint8_t* base, int row, int c) {
-  return reinterpret_cast<uint4*>(base + row * 32 + ((c ^ ((row >> 2) & 1)) << 4));
+// ---- epilogue staging tiles (one set per consumer warp: the warp's 16 rows x 32 hidden units).  Laid out exactly like the
+// TMA box that leaves them, so stores are single bulk-tensor instructions:
+//   T16: [16 rows][32 halves] = 64-byte rows, 16-byte chunk c of row r at  r*64 + ((c ^ ((r>>1)&3)) << 4)    (SWIZZLE_64B)
+//   T32: [16 rows][32 floats] = 128-byte rows, 16-byte chunk c of row r at r*128 + ((c ^ (r&7)) << 4)        (SWIZZLE_128B)
+// A thread reads and writes them at its accumulator fragment's positions (rows l/4 and l/4 + 8, units 2(l%4) + 8jj, +1):
+// a warp's half2 / float2 accesses are bank-conflict free.  The inputs land here by cp.async, 16-byte chunks per lane.
+constexpr int T16_BYTES = 1024, T32_BYTES = 2048;
+__device__ __forceinline__ uint8_t* t16_at(uint8_t* base, int row, int unit) {   // the half2 at (row, unit), unit even
+  return base + row * 64 + (((unit >> 3) ^ ((row >> 1) & 3)) << 4) + (unit & 7) * 2;
 }
-__device__ __forceinline__ float4* s64_at(uint8_t* base, int row, int c) {
-  return reinterpret_cast<float4*>(base + row * 64 + ((c ^ ((row >> 1) & 3)) << 4));
+__device__ __forceinline__ uint8_t* t32_at(uint8_t* base, int row, int unit) {   // the float2 at (row, unit), unit even
+  return base + row * 128 + (((unit >> 2) ^ (row & 7)) << 4) + (unit & 3) * 4;
 }
 __device__ __forceinline__ const void* shfl_vptr(const void* p, int src_lane) {
   unsigned long long v = (unsigned long long)p;
@@ -74,38 +78,32 @@ __device__ __forceinline__ const void* shfl_vptr(const void* p, int src_lane) {
 __device__ __forceinline__ void cp16(void* dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
-// global -> S32 tile: `mine` = this lane's row base (16 halves) or nullptr (zeros); 2 lanes per row, 2 passes
-__device__ __forceinline__ void s32_load(uint8_t* base, const void* mine, int lane) {
+// global -> T16 tile: `mine` = the row base (32 halves) of row (lane & 15), or nullptr (zeros); 4 lanes per row, 2 passes
+__device__ __forceinline__ void t16_load(uint8_t* base, const void* mine, int lane) {
 #pragma unroll
   for (int ps = 0; ps < 2; ++ps) {
-    const int row = ps * 16 + (lane >> 1), c = lane & 1;
-    const uint8_t* src = (const uint8_t*)shfl_vptr(mine, row);
-    uint4* dst = s32_at(base, row, c);
-    if (src) cp16(dst, src + c * 16); else *dst = make_uint4(0, 0, 0, 0);
-  }
-}
-// global -> S64 tile: 4 lanes per row, 4 passes
-__device__ __forceinline__ void s64_load(uint8_t* base, const void* mine, int lane) {
-#pragma unroll
-  for (int ps = 0; ps < 4; ++ps) {
     const int row = ps * 8 + (lane >> 2), c = lane & 3;
     const uint8_t* src = (const uint8_t*)shfl_vptr(mine, row);
-    float4* dst = s64_at(base, row, c);
-    if (src) cp16(dst, src + c * 16); else *dst = make_float4(0.f, 0.f, 0.f, 0.f);
+    uint8_t* dst = base + row * 64 + ((c ^ ((row >> 1) & 3)) << 4);
+    if (src) cp16(dst, src + c * 16); else *reinterpret_cast<uint4*>(dst) = make_uint4(0, 0, 0, 0);
+  }
+}
+// global -> T32 tile: 8 lanes per row, 4 passes
+__device__ __forceinline__ void t32_load(uint8_t* base, const void* mine, int lane) {
+#pragma unroll
+  for (int ps = 0; ps < 4; ++ps) {
+    const int row = ps * 4 + (lane >> 3), c = lane & 7;
+    const uint8_t* src = (const uint8_t*)shfl_vptr(mine, row);
+    uint8_t* dst = base + row * 128 + ((c ^ (row & 7)) << 4);
+    if (src) cp16(dst, src + c * 16); else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
 __device__ __forceinline__ void cp_wait_all() {
   asm volatile("cp.async.wait_all;" ::: "memory");
   __syncwarp();
 }
-__device__ __forceinline__ void s64_get8(uint8_t* base, int row, int sub, float* d) {
-  const float4 a = *s64_at(base, row, sub * 2), b = *s64_at(base, row, sub * 2 + 1);
-  d[0] = a.x; d[1] = a.y; d[2] = a.z; d[3] = a.w; d[4] = b.x; d[5] = b.y; d[6] = b.z; d[7] = b.w;
-}
-__device__ __forceinline__ void s64_put8(uint8_t* base, int row, int sub, const float* v) {
-  *s64_at(base, row, sub * 2) = make_float4(v[0], v[1], v[2], v[3]);
-  *s64_at(base, row, sub * 2 + 1) = make_float4(v[4], v[5], v[6], v[7]);
-}
+__device__ __forceinline__ float2 ld_h2(uint8_t* p) { return __half22float2(*reinterpret_cast<const __half2*>(p)); }
+__device__ __forceinline__ void st_h2(uint8_t* p, float a, float b) { *reinterpret_cast<uint32_t*>(p) = pack2(a, b); }
 
 struct Lstm16Params {
   int R, H;
@@ -119,21 +117,21 @@ struct Lstm16Params {
   // backward
   const __half* gsave; const float* c_cur; float* dc_carry;
 };
-struct Lstm16Maps { CUtensorMap g16, c, h16; };   // [R,4H] fp16 gates / da ; [R,H] fp32 c / dc ; [R,H] fp16 h
+struct Lstm16Maps { CUtensorMap g16, c, h16; };   // [R,4H] fp16 gates / da ; [R,H] fp32 c / dc ; [R,H] fp16 h: 16 x 32 boxes
 
 // ------------------------------------------------------------------------------------------------
 // MODE 0 = forward step, MODE 1 = backward step.  Persistent over the tile list; warpgroup 0 = TMA producer (one thread),
-// warpgroups 1-2 = consumers (64 rows each) that then run the pointwise epilogue "thread = row" from the accumulator tile.
+// warpgroups 1-2 = consumers (64 rows each).  Each consumer warp runs the pointwise epilogue of its 16 rows straight from
+// its accumulator registers, 32 hidden units at a time, with the inputs staged by cp.async in the T16 / T32 tiles above.
 template <int MODE>
 struct Cfg16 {
   static constexpr int THREADS = 128 + 32 * EW16;
-  // per-warp staging: forward {4 gate tiles S32, c tile S64, h tile S32} = 7 KB (inputs land here by cp.async, outputs
-  // overwrite them in place and leave by TMA); backward {4 gate tiles S32, c_prev, c_t, dc S64} = 10 KB
-  static constexpr int STG_PER_WARP = MODE == 0 ? (4 * S32_BYTES + S64_BYTES + S32_BYTES) : (4 * S32_BYTES + 3 * S64_BYTES);
+  // per-warp staging: forward {4 gate tiles T16, c tile T32, h tile T16} = 7 KB (the inputs, x-projection rows and c_prev,
+  // land in the gate and c tiles; the outputs overwrite them in place); backward {4 gate tiles T16, c_prev, c_t, dc T32} = 10 KB
+  static constexpr int STG_PER_WARP = MODE == 0 ? (5 * T16_BYTES + T32_BYTES) : (4 * T16_BYTES + 3 * T32_BYTES);
   static constexpr int STG_BYTES = EW16 * STG_PER_WARP;
-  static constexpr int ACC_BYTES = BN16 * ACC_LD * 4;
-  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES - ACC_BYTES) / STAGE16;      // fwd 3, bwd 2
-  static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + ACC_BYTES + 1024 + 256;
+  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES) / STAGE16;      // fwd 5, bwd 4
+  static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + 1024 + 256;
 };
 
 template <int MODE>
@@ -145,8 +143,7 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* stg_all = smem + STAGES * STAGE16;
-  float* acc = (float*)(stg_all + C::STG_BYTES);
-  uint64_t* full = (uint64_t*)(stg_all + C::STG_BYTES + C::ACC_BYTES);
+  uint64_t* full = (uint64_t*)(stg_all + C::STG_BYTES);
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -188,14 +185,12 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
     }
   } else {
     const int cw = warp - 4, wg = cw >> 2;
-    const int q = cw & 3;
-    const int half = cw >> 2;
     uint8_t* stg = stg_all + cw * C::STG_PER_WARP;
-    const float* arow = acc + q * 32 + lane;
+    // fragment rows of this thread within the warp's 16, and the unit pair within a group of 8 columns
+    const int fr = lane >> 2, fu = 2 * (lane & 3);
     int s = 0; uint32_t ph = 0;
-    // main loop of one tile: this warpgroup's 64 rows x 128 columns, then the accumulator tile in shared memory
-    auto contract = [&]() {
-      float d[BN16 / 2];
+    // main loop of one tile: this warpgroup's 64 rows x 128 columns, accumulated in registers
+    auto contract = [&](float (&d)[BN16 / 2]) {
 #pragma unroll
       for (int i = 0; i < BN16 / 2; ++i) d[i] = 0.f;
       int prev = -1;
@@ -216,67 +211,64 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
       wgmma_wait<0>();
       wgmma_hold(d);
       if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
-      bar_named(1, 32 * EW16);                       // the previous tile's epilogue is done with the accumulator tile
-      acc_store(acc, d, wg * 64);
-      bar_named(1, 32 * EW16);
     };
     if constexpr (MODE == 0) {
-      // ---- forward.  32 hidden units per tile = two column groups of 16; the two warps of a 32-row quarter take one group
-      // each.  Per tile and warp: inputs (x-projection rows gathered from the fp16 table, previous cell) -> staging by
-      // cp.async (issued before the contraction), accumulator + staging -> gates / c / h in place, out by TMA.
-      const int grp = half;
-      uint8_t* sG = stg; uint8_t* sC = stg + 4 * S32_BYTES; uint8_t* sH = sC + S64_BYTES;
+      // ---- forward.  Tile columns [i | f | o | g] x 32 hidden units, so the thread holding column 8jj + fu of gate i holds
+      // the same unit of f, o and g in fragments jj + 4, jj + 8, jj + 12: the pointwise step runs where the accumulators are.
+      uint8_t* sG = stg; uint8_t* sH = stg + 4 * T16_BYTES; uint8_t* sC = sH + T16_BYTES;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m0 = (tile / num_n) * BM16;
         const int nt = tile % num_n;
-        const int64_t row = (int64_t)m0 + q * 32 + lane;
+        const int r0 = m0 + wg * 64 + (cw & 3) * 16;          // first of the warp's 16 rows
+        const int j0 = nt * 32;                                // first hidden unit of the tile
+        const int64_t row = (int64_t)r0 + (lane & 15);         // lanes l and l + 16 both describe row l % 16
         const bool row_ok = row < p.R;
         const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
-        const int r0 = m0 + q * 32;
-        const int j = nt * 32 + grp * 16;                      // first hidden unit of this warp's group
         // A pad token's x-projection is exactly zero (LookupTableMaskZero: embedding row 0 is zero, and the table carries no
         // bias), so finished sequences skip the gather: at late time steps most of the 100 x 20-token options have ended, and
         // every row would otherwise read the same 4 KB of L2
         const int32_t tk = row_ok ? __ldg(p.tok + row) : 0;
-        const __half* prow = tk != 0 ? p.ptable + (int64_t)tk * 4 * H + j : nullptr;
-        const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H + j : nullptr;
+        const __half* prow = tk != 0 ? p.ptable + (int64_t)tk * 4 * H + j0 : nullptr;
+        const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H + j0 : nullptr;
         if (lane == 0) bulk_wait_read0();                      // the previous tile's TMA stores have read the staging tiles
         __syncwarp();
 #pragma unroll
-        for (int g = 0; g < 4; ++g) s32_load(sG + g * S32_BYTES, prow ? prow + g * H : nullptr, lane);
-        s64_load(sC, cprow, lane);
-        contract();                                            // the loads fly while the MMAs of this tile run
+        for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, prow ? prow + g * H : nullptr, lane);
+        t32_load(sC, cprow, lane);
+        float d[BN16 / 2];
+        contract(d);                                           // the loads fly while the MMAs of this tile run
         cp_wait_all();
-#pragma unroll 1
-        for (int sub = 0; sub < 2; ++sub) {
-          float a[4][8], cp[8], hn[8];
 #pragma unroll
-          for (int g = 0; g < 4; ++g) acc_ld8(arow, g * 32 + grp * 16 + sub * 8, a[g]);
-          s64_get8(sC, lane, sub, cp);
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = fr + 8 * hh;
+          const float kp = __shfl_sync(0xffffffffu, keep, r);
+          const int64_t grow = (int64_t)r0 + r;
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float x[8];
-            unpack8(*s32_at(sG + g * S32_BYTES, lane, sub), x);
-            const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + g * H + j + sub * 8));
-            const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + g * H + j + sub * 8 + 4));
-            a[g][0] += x[0] + b0.x; a[g][1] += x[1] + b0.y; a[g][2] += x[2] + b0.z; a[g][3] += x[3] + b0.w;
-            a[g][4] += x[4] + b1.x; a[g][5] += x[5] + b1.y; a[g][6] += x[6] + b1.z; a[g][7] += x[7] + b1.w;
-          }
+          for (int jj = 0; jj < 4; ++jj) {
+            const int u = 8 * jj + fu;
+            float a[4][2], cp[2], hn[2];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float gi = sig16(a[0][e]), gf = sig16(a[1][e]), go = sig16(a[2][e]), gg = tanh16(a[3][e]);
-            const float c_ = (gf * cp[e] + gi * gg) * keep;
-            a[0][e] = gi * keep; a[1][e] = gf * keep; a[2][e] = go * keep; a[3][e] = gg * keep;
-            cp[e] = c_; hn[e] = go * tanh16(c_) * keep;
-          }
+            for (int g = 0; g < 4; ++g) {
+              const float2 x = ld_h2(t16_at(sG + g * T16_BYTES, r, u));
+              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + g * H + j0 + u));
+              a[g][0] = d[4 * (jj + 4 * g) + 2 * hh] + (x.x + b.x);
+              a[g][1] = d[4 * (jj + 4 * g) + 2 * hh + 1] + (x.y + b.y);
+            }
+            const float2 c2 = *reinterpret_cast<const float2*>(t32_at(sC, r, u));
+            cp[0] = c2.x; cp[1] = c2.y;
 #pragma unroll
-          for (int g = 0; g < 4; ++g) *s32_at(sG + g * S32_BYTES, lane, sub) = pack8(a[g]);
-          s64_put8(sC, lane, sub, cp);
-          *s32_at(sH, lane, sub) = pack8(hn);
-          if (p.h32_out && row_ok) {                  // last step only: the fp32 h that meets the encoder output
-            float4* o = reinterpret_cast<float4*>(p.h32_out + row * H + j + sub * 8);
-            o[0] = make_float4(hn[0], hn[1], hn[2], hn[3]);
-            o[1] = make_float4(hn[4], hn[5], hn[6], hn[7]);
+            for (int e = 0; e < 2; ++e) {
+              const float gi = sig16(a[0][e]), gf = sig16(a[1][e]), go = sig16(a[2][e]), gg = tanh16(a[3][e]);
+              const float c_ = (gf * cp[e] + gi * gg) * kp;
+              a[0][e] = gi * kp; a[1][e] = gf * kp; a[2][e] = go * kp; a[3][e] = gg * kp;
+              cp[e] = c_; hn[e] = go * tanh16(c_) * kp;
+            }
+#pragma unroll
+            for (int g = 0; g < 4; ++g) st_h2(t16_at(sG + g * T16_BYTES, r, u), a[g][0], a[g][1]);
+            *reinterpret_cast<float2*>(t32_at(sC, r, u)) = make_float2(cp[0], cp[1]);
+            st_h2(t16_at(sH, r, u), hn[0], hn[1]);
+            if (p.h32_out && grow < p.R)                  // last step only: the fp32 h that meets the encoder output
+              *reinterpret_cast<float2*>(p.h32_out + grow * H + j0 + u) = make_float2(hn[0], hn[1]);
           }
         }
         fence_proxy_async_smem();
@@ -284,74 +276,86 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
         if (lane == 0) {
           if (p.save_gates) {
 #pragma unroll
-            for (int g = 0; g < 4; ++g) tma_store_2d(&em.g16, sG + g * S32_BYTES, g * H + j, r0);
+            for (int g = 0; g < 4; ++g) tma_store_2d(&em.g16, sG + g * T16_BYTES, g * H + j0, r0);
           }
-          tma_store_2d(&em.c, sC, j, r0);
-          tma_store_2d(&em.h16, sH, j, r0);
+          tma_store_2d(&em.c, sC, j0, r0);
+          tma_store_2d(&em.h16, sH, j0, r0);
           bulk_commit();
         }
         __syncwarp();
       }
     } else {
-      // ---- backward: 128 hidden units per tile, the warp's column slice = 64 of them, in groups of 16
-      constexpr int NSL = EW16 / 4, GPW = BN16 / NSL / 16;      // column slices per tile, groups per warp
-      uint8_t* sG = stg; uint8_t* sCP = stg + 4 * S32_BYTES; uint8_t* sCC = sCP + S64_BYTES; uint8_t* sDC = sCC + S64_BYTES;
+      // ---- backward: 128 hidden units per tile = 4 groups of 32; fragment columns are hidden units, so the thread reads the
+      // gates / c / dc of exactly the units its accumulators hold.  The first group's inputs are fetched before the contraction.
+      uint8_t* sG = stg; uint8_t* sCP = stg + 4 * T16_BYTES; uint8_t* sCC = sCP + T32_BYTES; uint8_t* sDC = sCC + T32_BYTES;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m0 = (tile / num_n) * BM16;
         const int nt = tile % num_n;
-        const int64_t row = (int64_t)m0 + q * 32 + lane;
+        const int r0 = m0 + wg * 64 + (cw & 3) * 16;
+        const int64_t row = (int64_t)r0 + (lane & 15);
         const bool row_ok = row < p.R;
-        const bool masked = row_ok && p.mask_ids && p.mask_ids[row] == 0;
-        const float keep = masked ? 0.f : 1.f;
-        const int r0 = m0 + q * 32;
-        const int j0 = nt * BN16 + half * (BN16 / NSL);
+        const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
         const __half* grow = row_ok ? p.gsave + row * 4 * H : nullptr;
         const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H : nullptr;
         const float* ccrow = row_ok ? p.c_cur + row * H : nullptr;
         const float* dcrow = row_ok ? p.dc_carry + row * H : nullptr;
-        contract();
-#pragma unroll 1
-        for (int grp = 0; grp < GPW; ++grp) {
-          const int j = j0 + grp * 16;
-          const int tc0 = half * (BN16 / NSL) + grp * 16;
+        auto fetch = [&](int j) {                              // inputs of hidden units j .. j + 31 -> staging
           if (lane == 0) bulk_wait_read0();
           __syncwarp();
 #pragma unroll
-          for (int g = 0; g < 4; ++g) s32_load(sG + g * S32_BYTES, grow ? grow + g * H + j : nullptr, lane);
-          s64_load(sCP, cprow ? cprow + j : nullptr, lane);
-          s64_load(sCC, ccrow ? ccrow + j : nullptr, lane);
-          s64_load(sDC, dcrow ? dcrow + j : nullptr, lane);
+          for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, grow ? grow + g * H + j : nullptr, lane);
+          t32_load(sCP, cprow ? cprow + j : nullptr, lane);
+          t32_load(sCC, ccrow ? ccrow + j : nullptr, lane);
+          t32_load(sDC, dcrow ? dcrow + j : nullptr, lane);
+        };
+        fetch(nt * BN16);
+        float d[BN16 / 2];
+        contract(d);
+#pragma unroll
+        for (int grp = 0; grp < BN16 / 32; ++grp) {
+          const int j = nt * BN16 + grp * 32;
+          if (grp > 0) fetch(j);
           cp_wait_all();
-#pragma unroll 1
-          for (int sub = 0; sub < 2; ++sub) {
-            float dh[8], g[4][8], cp[8], cc[8], dc[8], out[4][8], dcn[8];
-            acc_ld8(arow, tc0 + sub * 8, dh);
 #pragma unroll
-            for (int gg = 0; gg < 4; ++gg) unpack8(*s32_at(sG + gg * S32_BYTES, lane, sub), g[gg]);
-            s64_get8(sCP, lane, sub, cp);
-            s64_get8(sCC, lane, sub, cc);
-            s64_get8(sDC, lane, sub, dc);
+          for (int hh = 0; hh < 2; ++hh) {
+            const int r = fr + 8 * hh;
+            const float keep_r = __shfl_sync(0xffffffffu, keep, r);
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
-              const float tcv = tanh16(cc[e]);
-              const float d = (dc[e] + dh[e] * go * (1.f - tcv * tcv)) * keep;
-              const float dhe = dh[e] * keep;
-              out[0][e] = d * gg_ * gi * (1.f - gi);
-              out[1][e] = d * cp[e] * gf * (1.f - gf);
-              out[2][e] = dhe * tcv * go * (1.f - go);
-              out[3][e] = d * gi * (1.f - gg_ * gg_);
-              dcn[e] = d * gf;
+            for (int jj = 0; jj < 4; ++jj) {
+              const int u = 8 * jj + fu;
+              float g[4][2], cp[2], cc[2], dc[2], out[4][2], dcn[2];
+#pragma unroll
+              for (int gg = 0; gg < 4; ++gg) {
+                const float2 x = ld_h2(t16_at(sG + gg * T16_BYTES, r, u));
+                g[gg][0] = x.x; g[gg][1] = x.y;
+              }
+              const float2 cp2 = *reinterpret_cast<const float2*>(t32_at(sCP, r, u));
+              const float2 cc2 = *reinterpret_cast<const float2*>(t32_at(sCC, r, u));
+              const float2 dc2 = *reinterpret_cast<const float2*>(t32_at(sDC, r, u));
+              cp[0] = cp2.x; cp[1] = cp2.y; cc[0] = cc2.x; cc[1] = cc2.y; dc[0] = dc2.x; dc[1] = dc2.y;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float dh = d[4 * (4 * grp + jj) + 2 * hh + e];
+                const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
+                const float tcv = tanh16(cc[e]);
+                const float dd = (dc[e] + dh * go * (1.f - tcv * tcv)) * keep_r;
+                const float dhe = dh * keep_r;
+                out[0][e] = dd * gg_ * gi * (1.f - gi);
+                out[1][e] = dd * cp[e] * gf * (1.f - gf);
+                out[2][e] = dhe * tcv * go * (1.f - go);
+                out[3][e] = dd * gi * (1.f - gg_ * gg_);
+                dcn[e] = dd * gf;
+              }
+#pragma unroll
+              for (int gg = 0; gg < 4; ++gg) st_h2(t16_at(sG + gg * T16_BYTES, r, u), out[gg][0], out[gg][1]);
+              *reinterpret_cast<float2*>(t32_at(sDC, r, u)) = make_float2(dcn[0], dcn[1]);
             }
-#pragma unroll
-            for (int gg = 0; gg < 4; ++gg) *s32_at(sG + gg * S32_BYTES, lane, sub) = pack8(out[gg]);
-            s64_put8(sDC, lane, sub, dcn);
           }
           fence_proxy_async_smem();
           __syncwarp();
           if (lane == 0) {
 #pragma unroll
-            for (int gg = 0; gg < 4; ++gg) tma_store_2d(&em.g16, sG + gg * S32_BYTES, gg * H + j, r0);
+            for (int gg = 0; gg < 4; ++gg) tma_store_2d(&em.g16, sG + gg * T16_BYTES, gg * H + j, r0);
             tma_store_2d(&em.c, sDC, j, r0);
             bulk_commit();
           }
@@ -676,10 +680,10 @@ void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, co
   CUtensorMap tA = tmap_h(h_prev16, R, H, H, BM16, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
   CUtensorMap tB = tmap_h(Wh16, 4 * (int64_t)H, H, H, 32, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
   Lstm16Maps em;
-  em.g16 = gates16 ? tmap_h(gates16, R, 4 * (int64_t)H, 4 * (int64_t)H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B)
-                   : tmap_h(h16_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B);
-  em.c = tmap_f(c_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
-  em.h16 = tmap_h(h16_out, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B);
+  em.g16 = gates16 ? tmap_h(gates16, R, 4 * (int64_t)H, 4 * (int64_t)H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B)
+                   : tmap_h(h16_out, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
+  em.c = tmap_f(c_out, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_128B);
+  em.h16 = tmap_h(h16_out, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
   launch16<0>(cx, tA, tB, em, p, cdiv(R, BM16) * (H / 32));
 }
 
@@ -692,8 +696,8 @@ void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, c
   CUtensorMap tA = tmap_h(da_next16, R, 4 * (int64_t)H, 4 * (int64_t)H, BM16, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
   CUtensorMap tB = tmap_h(Whb16, H, 4 * (int64_t)H, 4 * (int64_t)H, 128, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
   Lstm16Maps em;
-  em.g16 = tmap_h(da16, R, 4 * (int64_t)H, 4 * (int64_t)H, 32, 16, CU_TENSOR_MAP_SWIZZLE_32B);
-  em.c = tmap_f(dc_carry, R, H, H, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
+  em.g16 = tmap_h(da16, R, 4 * (int64_t)H, 4 * (int64_t)H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
+  em.c = tmap_f(dc_carry, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_128B);
   em.h16 = em.c;
   launch16<1>(cx, tA, tB, em, p, cdiv(R, BM16) * (H / BN16));
 }
