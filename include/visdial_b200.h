@@ -169,6 +169,15 @@ int vd_gen_decoder_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, 
 int vd_gen_beam_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, const int32_t* parent_host,
                      const float* const* init_h_host, const float* const* init_c_host, int32_t k, float* topv_host,
                      int32_t* topi_host);
+/* Model:generateAnswers' beam search (model.lua:472-579) for EVERY round of every dialog of the last vd_encoder_forward
+ * (N = B * maxQuesCount searches, N * beam_size hypotheses per step), entirely on the device: the decoder steps, the top-k,
+ * the candidate merge with all of the reference's quirks, and the best finished hypothesis.  One synchronisation, at the end.
+ * answer_host (N, beam_len) int32: the best finished beam (position 0 = start_token, zero-padded), length_host (N): its
+ * length (0 = no hypothesis reached end_token; the reference indexes nil there, :575), score_host (N) fp64: its score.
+ * VD_E_STATE for a disc engine or before any vd_encoder_forward; VD_E_BADARG unless 1 <= beam_size <= min(32, vocabSize)
+ * and beam_len >= 2.  Ends any search vd_gen_beam_step was continuing. */
+int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
+                       int32_t* answer_host, int32_t* length_host, double* score_host);
 
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.

@@ -1,8 +1,18 @@
-"""Model:generateAnswers (model.lua:432-613) wall time per dialog: beam search (beamSize 5, beamLen 20) over the 10 rounds of a
-dialog, decoder stepped on the device through vd_gen_decoder_step, hypothesis bookkeeping on the host like the reference.
-usage: python tools/bench_generate.py [encoder] [dialogs]"""
+"""Model:generateAnswers (model.lua:432-613) wall time per dialog: beam search (beamSize 5, beamLen 20) over the 10 rounds of
+each dialog, V = 10 000, for `hrea-ques-im-hist + gen` (C3's graph) and `mn-att-ques-im-hist + gen`, in the F16 and FP32 math
+modes.  Paths, all in one run:
+  device/<d>  the default: vd_gen_beam_search, d dialogs per encoder forward and call (params.dialogsPerCall)
+  host_merge  the search as the engine ran it before it moved to the device: per dialog, the candidate merge on the host
+              over vd_gen_beam_step (tests/test_beam_search_gpu.py::host_beam_search)
+  host_beam   params.hostBeam = 1: the reference's loop structure, one round at a time through vd_gen_decoder_step
+Every path is warmed up at its shape first, then timed over whole calls until the window lasts at least --window seconds
+(host clock; every call ends in a device synchronisation).  Prints one JSON line per (encoder, mode, path) and the card's name
+and power limit, read in the same run.
+usage: python tools/bench_generate.py [--encoders a,b] [--modes f16,fp32] [--dpc 1,8,32,128] [--window 1.0] [--out FILE]"""
+import argparse
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -10,29 +20,92 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from visdial_b200 import VD_MATH_F16, Model  # noqa: E402
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+from visdial_b200 import VD_MATH_F16, VD_MATH_FP32, Model  # noqa: E402
 from visdial_b200.dataloader import Dataloader  # noqa: E402
 from visdial_b200.engine import DEFAULT_PARAMS, derive_flags  # noqa: E402
 from visdial_b200.synthetic import make_corpus  # noqa: E402
+from test_beam_search_gpu import host_beam_search  # noqa: E402
 
-enc = sys.argv[1] if len(sys.argv) > 1 else "hrea-ques-im-hist"
-nd = int(sys.argv[2]) if len(sys.argv) > 2 else 8
-p = dict(DEFAULT_PARAMS)
-p.update(encoder=enc, decoder="gen", vocabSize=10000, imgFeatureSize=512 if "att" in enc else 4096, batchSize=1)
-p = derive_flags(p)
-raw = make_corpus(p, nd, 2000, seed=5)
-m = Model(p, seed=3)
-m.engine.set_math_mode(VD_MATH_F16)
-dl = Dataloader(m.engine).initialize(dict(p, maxHistoryLen=60), ["val"], {"val": raw})
-m.generateAnswers(dl, "val", {"beamSize": 5, "beamLen": 20, "maxThreads": 1}, strict=False)
-t0 = time.perf_counter()
-out = m.generateAnswers(dl, "val", {"beamSize": 5, "beamLen": 20, "maxThreads": nd}, strict=False)
-dt = time.perf_counter() - t0
-t0 = time.perf_counter()
-m.generateAnswers(dl, "val", {"beamSize": 5, "beamLen": 20, "maxThreads": max(1, nd // 2), "hostBeam": 1}, strict=False)
-dt_host = (time.perf_counter() - t0) / max(1, nd // 2)
-done = sum(1 for d in out for r in d["dialog"] if r is not None)
-print(json.dumps({"encoder": enc, "dialogs": nd, "ms_per_dialog": dt / nd * 1e3, "ms_per_round": dt / nd / 10 * 1e3,
-                  "rounds_with_a_finished_beam": done,
-                  "ms_per_dialog_reference_structure": dt_host * 1e3, "beamSize": 5, "beamLen": 20, "vocabSize": 10000}))
-dl.close(); m.engine.close()
+BEAM, LEN, V = 5, 20, 10000
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    except FileNotFoundError:
+        q = None
+    if q is None or q.returncode != 0:
+        raise SystemExit("nvidia-smi failed: this benchmark needs the GPU")
+    name, power = [s.strip() for s in q.stdout.splitlines()[0].split(",")]
+    return name, power
+
+
+def window(call, dialogs_per_call, seconds):
+    """ms per dialog over whole calls, after one warm-up call of the same shape"""
+    call()
+    n, t0 = 0, time.perf_counter()
+    while True:
+        call()
+        n += dialogs_per_call
+        dt = time.perf_counter() - t0
+        if dt >= seconds:
+            return dt / n * 1e3, n, dt
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--encoders", default="hrea-ques-im-hist,mn-att-ques-im-hist")
+    ap.add_argument("--modes", default="f16,fp32")
+    ap.add_argument("--dpc", default="1,8,32,128")
+    ap.add_argument("--window", type=float, default=1.0)
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    dpcs = [int(x) for x in a.dpc.split(",")]
+    name, power = card()
+    rows = []
+    for enc in a.encoders.split(","):
+        p = dict(DEFAULT_PARAMS)
+        p.update(encoder=enc, decoder="gen", vocabSize=V, imgFeatureSize=512 if "att" in enc else 4096, batchSize=1)
+        p = derive_flags(p)
+        raw = make_corpus(p, max(dpcs), 2000, seed=5)
+        m = Model(p, seed=3)
+        dl = Dataloader(m.engine).initialize(dict(p, maxHistoryLen=60), ["val"], {"val": raw})
+        start, end = dl.word2ind["<START>"], dl.word2ind["<END>"]
+        for mode in a.modes.split(","):
+            m.engine.set_math_mode({"f16": VD_MATH_F16, "fp32": VD_MATH_FP32}[mode])
+            beam = {"beamSize": BEAM, "beamLen": LEN}
+
+            def host_merge():
+                m.wrapper.evaluate()
+                b = dl.getIndexData(np.array([0]), m.params, "val")
+                encOut = m.forwardBackward(b, True, True).numpy()
+                host_beam_search(m.engine, encOut, BEAM, LEN, start, end)
+                m.wrapper.training()
+
+            paths = [("device/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(beam, maxThreads=d, dialogsPerCall=d),
+                                                                        strict=False)) for d in dpcs]
+            paths += [("host_merge", 1, host_merge),
+                      ("host_beam", 1, lambda: m.generateAnswers(dl, "val", dict(beam, maxThreads=1, hostBeam=1), strict=False))]
+            for path, d, call in paths:
+                ms, n, dt = window(call, d, a.window)
+                r = {"encoder": enc, "mode": mode, "path": path, "ms_per_dialog": round(ms, 3), "dialogs_timed": n,
+                     "window_s": round(dt, 2), "beamSize": BEAM, "beamLen": LEN, "vocabSize": V, "gpu": name, "power_limit": power}
+                print(json.dumps(r), flush=True)
+                rows.append(r)
+        dl.close(); m.engine.close()
+    print("\n%s, power limit %s: ms per dialog (beam %d x %d, V = %d)" % (name, power, BEAM, LEN, V))
+    paths = sorted({r["path"] for r in rows}, key=lambda s: (not s.startswith("device"), int(s.split("/")[1]) if "/" in s else 0, s))
+    print("| encoder | mode | " + " | ".join(paths) + " |")
+    print("|---|---|" + "---|" * len(paths))
+    for enc in a.encoders.split(","):
+        for mode in a.modes.split(","):
+            got = {r["path"]: r["ms_per_dialog"] for r in rows if r["encoder"] == enc and r["mode"] == mode}
+            print("| %s | %s | " % (enc, mode) + " | ".join("%.2f" % got[p] for p in paths) + " |")
+    if a.out:
+        with open(a.out, "w") as f:
+            json.dump(rows, f, indent=1)
+
+
+if __name__ == "__main__":
+    main()

@@ -10,6 +10,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvisdial_b200.so")
 
 VD_OK = 0
+VD_E_BADARG = -1
+VD_E_STATE = -6
 VD_MATH_TF32 = 0
 VD_MATH_FP32 = 1
 VD_MATH_F16 = 2
@@ -115,6 +117,7 @@ SIGNATURES = {
                     C.c_int64],
     "vd_set_lazy_decout": [_H, C.c_int32],
     "vd_gen_beam_step": [_H, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p],
+    "vd_gen_beam_search": [_H, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gemm_atb16": [_H, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                       C.c_int64, C.c_float],
     "vd_lstm_step_fwd": [_H, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,

@@ -132,6 +132,10 @@ void* Arena::alloc(size_t bytes) {
 }
 void Arena::reset() { for (auto& c : chunks) c.used = 0; cur = 0; }
 void Arena::release() { for (auto& c : chunks) cudaFree(c.p); chunks.clear(); cur = 0; }
+void Arena::rewind(const Mark& m) {
+  for (size_t i = m.chunk; i < chunks.size(); ++i) chunks[i].used = i == m.chunk ? m.used : 0;   // chunks past `cur` are unused
+  cur = m.chunk;
+}
 
 void* GrowBuf::ensure(size_t bytes) {
   if (bytes > cap) {
@@ -1419,10 +1423,15 @@ void Engine::gen_decoder_step(int64_t rows, const int32_t* tokens_host, const fl
   VD_REQUIRE(rows > 0 && tokens_host != nullptr, VD_E_BADARG, "rows / tokens");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
-  const int E = cfg.E, H = cfg.H, V = cfg.V;
   int32_t* tok = arena.get<int32_t>(rows);
   VD_CUDA_CHECK(cudaMemcpyAsync(tok, tokens_host, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));               // tokens_host may be a temporary of the caller
+  gen_decoder_step_logits(rows, tok, h_prev, c_prev);
+  logsoftmax_rows(cx, gstep_logp, tok, rows, cfg.V);            // gen.lua:23-24 (MaskZero)
+}
+
+void Engine::gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev) {
+  const int E = cfg.E, H = cfg.H, V = cfg.V;
   float* xa = arena.get<float>(rows * E);
   embed_rows(cx, xa, Wp(0), tok, rows, E, dropcfg(0.f), 0);
   gstep1 = make_run(1, rows, E, H, seg("dec.lstm1.weight"), xa, nullptr, tok);
@@ -1433,7 +1442,6 @@ void Engine::gen_decoder_step(int64_t rows, const int32_t* tokens_host, const fl
   lstm_forward(gstep2, true);
   gstep_logp = arena.get<float>(rows * V);
   linear_fwd(seg("dec.out.weight"), gstep2.h, rows, gstep_logp, 0);
-  logsoftmax_rows(cx, gstep_logp, tok, rows, V);                // gen.lua:23-24 (MaskZero)
 }
 
 // One beam-search step (model.lua:510-570) for `rows` hypotheses at once (all rounds of a dialog x beamSize).  The state of
@@ -1475,6 +1483,69 @@ void Engine::gen_beam_step(int64_t rows, const int32_t* tokens_host, const int32
   topk_rows(cx, gstep_logp, rows, cfg.V, k, tv, ti);
   VD_CUDA_CHECK(cudaMemcpyAsync(topv_host, tv, (size_t)rows * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(topi_host, ti, (size_t)rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+// Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once: row n*k + j is
+// hypothesis j of round n.  Every step runs gen_beam_step's kernels on device-resident tokens and parents — state gather,
+// decoder step, vocabulary projection — then the fused log-softmax + top-k and the candidate merge, which writes the next
+// step's tokens and parents.  Nothing returns to the host until the final copy of each round's best finished hypothesis.
+void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
+                             double* score_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_search needs the gen decoder after encoder_forward");
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  cx.stream = main_stream;
+  forward_connect();
+  const int H = cfg.H;
+  const int64_t N = db.N, rows = N * k;
+  // allocated once per call.  Two sets of fed states {h1, h2, c1, c2}: the gather of step s reads the set step s-1 was
+  // fed (a column that got no candidate keeps it) and writes the other; beams / scores ping-pong because the merge fills
+  // columns from the pre-merge beams.
+  float* st[2][4];
+  for (auto& s : st)
+    for (auto& p : s) p = arena.get<float>(rows * H);
+  int32_t* beams[2] = {arena.get<int32_t>(rows * L), arena.get<int32_t>(rows * L)};
+  double* scores[2] = {arena.get<double>(rows), arena.get<double>(rows)};
+  int32_t* tok = arena.get<int32_t>(rows);
+  int32_t* parent = arena.get<int32_t>(rows);
+  float* tv = arena.get<float>(rows * k);
+  int32_t* ti = arena.get<int32_t>(rows * k);
+  int32_t* ans = arena.get<int32_t>(N * L);
+  int32_t* ans_len = arena.get<int32_t>(N);
+  double* ans_score = arena.get<double>(N);
+  VD_CUDA_CHECK(cudaMemsetAsync(ans, 0, (size_t)N * L * sizeof(int32_t), cx.stream));
+  VD_CUDA_CHECK(cudaMemsetAsync(ans_len, 0, (size_t)N * sizeof(int32_t), cx.stream));
+  VD_CUDA_CHECK(cudaMemsetAsync(ans_score, 0, (size_t)N * sizeof(double), cx.stream));
+  // model.lua:478-503: h = {layer-1 h at Tq, encOut}, c = {layer-1 c, layer-2 c}, each round's row repeated k times.  Encoders
+  // without .rnnLayers feed explicit zero rows, not "no initial state": the first step's kernels differ between the two.
+  const float* init[4] = {gen_h0[0], gen_h0[1], gen_c0[0], gen_c0[1]};
+  for (int i = 0; i < 4; ++i) {
+    if (init[i]) repeat_rows(cx, st[0][i], init[i], N, k, H);
+    else VD_CUDA_CHECK(cudaMemsetAsync(st[0][i], 0, (size_t)rows * H * sizeof(float), cx.stream));
+  }
+  beam_init(cx, rows, L, start_token, beams[0], tok, scores[0]);
+  const Arena::Mark step_mark = arena.mark();
+  for (int stp = 1; stp < L; ++stp) {
+    float* const* fed = st[(stp - 1) & 1];
+    if (stp > 1) {
+      const float* out[4] = {gstep1.h, gstep2.h, gstep1.c, gstep2.c};
+      for (int i = 0; i < 4; ++i) beam_gather(cx, fed[i], out[i], st[stp & 1][i], parent, rows, H);
+    }
+    arena.rewind(step_mark);                       // every step's decoder buffers land where the last step's were
+    const float* h[2] = {fed[0], fed[1]};
+    const float* c[2] = {fed[2], fed[3]};
+    gen_decoder_step_logits(rows, tok, h, c);
+    logsoftmax_topk_rows(cx, gstep_logp, tok, rows, cfg.V, k, tv, ti);
+    const int a = (stp - 1) & 1;
+    beam_merge(cx, N, stp, k, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, ans, ans_len,
+               ans_score);
+  }
+  beam_rows = 0;                                   // gstep1 / gstep2 hold this search's state now: vd_gen_beam_step starts over
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, ans_len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, ans_score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 

@@ -53,6 +53,11 @@ struct Arena {
   template <typename T> T* get(int64_t n) { return reinterpret_cast<T*>(alloc((size_t)n * sizeof(T))); }
   void reset();
   void release();
+  // a loop that allocates the same buffers every iteration rewinds to a mark taken before it, so it reuses them instead of
+  // growing the arena (stream order keeps the previous iteration's readers ahead of the new writers)
+  struct Mark { size_t chunk, used; };
+  Mark mark() const { return {cur, cur < chunks.size() ? chunks[cur].used : 0}; }
+  void rewind(const Mark& m);
 };
 
 // The kernels an nn.SeqLSTM run executes on.  Simt: a GEMM and a pointwise kernel per step on the CUDA cores.  Tc: fused
@@ -283,12 +288,16 @@ struct Engine {
   LstmRun gstep1, gstep2;
   float* gstep_logp = nullptr;
   void gen_decoder_step(int64_t rows, const int32_t* tokens_host, const float* const* h_prev, const float* const* c_prev);
+  // its core on device-resident tokens, up to the vocabulary projection: gstep_logp holds the LOGITS on return
+  void gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // beam search with the decoder state and the (rows, V) log-probabilities kept on the device: per step only the tokens and
   // parent indices go up and the k best (log-prob, class) pairs per hypothesis come down
   const float *beam_in_h[2] = {nullptr, nullptr}, *beam_in_c[2] = {nullptr, nullptr};
   int64_t beam_rows = 0;
   void gen_beam_step(int64_t rows, const int32_t* tokens_host, const int32_t* parent_host, const float* const* init_h_host,
                      const float* const* init_c_host, int k, float* topv_host, int32_t* topi_host);
+  // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device
+  void gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
   void clamp_adam_step(float lr);
   void allreduce_grads();
   // Overlapped gradient sync (world > 1): dW is all-reduced in buckets on `comm_stream` as soon as each bucket's last

@@ -124,6 +124,16 @@ void lhood_accumulate(LaunchCtx& cx, const float* logits, const int32_t* tgt, co
 // beam search on the device (model.lua:510-570): k best classes per row (value desc, index asc); state shuffle by parent index
 void topk_rows(LaunchCtx& cx, const float* x, int64_t rows, int V, int k, float* topv, int32_t* topi);
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H);
+// logsoftmax_rows + topk_rows in one pass that never writes the log-probabilities (bit-identical results), k <= 32
+void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
+                          int32_t* topi);
+// the whole search on the device (Engine::gen_beam_search): beams (rows, L) = <start> then pads, tokens = <start>, scores = 0
+void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* beams, int32_t* tokens, double* scores);
+// the candidate merge of step stp for N rounds of k hypotheses (model.lua:529-569): next beams / scores / tokens / parents,
+// and each round's best finished hypothesis (ans (N, L), ans_len (N) = 0 while there is none, ans_score (N))
+void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int L, int end_token, const float* topv, const int32_t* topi,
+                const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out, int32_t* tokens,
+                int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score);
 
 // ---- optimiser (model.lua:96-99, optim_updates.lua:62-91) ------------------------------------------
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1,

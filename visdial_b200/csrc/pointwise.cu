@@ -858,6 +858,18 @@ __global__ void k_rank_rows(const float* __restrict__ scores, const int32_t* __r
   }
 }
 
+// log-sum-exp of one row, by the whole block.  k_logsoftmax_rows and k_logsoftmax_topk_rows both take their lse from here
+// (same strided loops, same block reductions), so the log-probabilities x - lse they form are the same bits.
+__device__ __forceinline__ float row_lse(const float* row, int V, float* red) {
+  float mx = -INFINITY;
+  for (int c = threadIdx.x; c < V; c += blockDim.x) mx = fmaxf(mx, row[c]);
+  mx = block_max(mx, red);
+  float sum = 0.f;
+  for (int c = threadIdx.x; c < V; c += blockDim.x) sum += expf(row[c] - mx);
+  sum = block_sum(sum, red);
+  return mx + logf(sum);
+}
+
 // block per row
 __global__ void k_logsoftmax_rows(float* __restrict__ x, const int32_t* __restrict__ mask_ids, int V) {
   __shared__ float red[33];
@@ -867,14 +879,165 @@ __global__ void k_logsoftmax_rows(float* __restrict__ x, const int32_t* __restri
     for (int c = threadIdx.x; c < V; c += blockDim.x) row[c] = 0.f;
     return;
   }
-  float mx = -INFINITY;
-  for (int c = threadIdx.x; c < V; c += blockDim.x) mx = fmaxf(mx, row[c]);
-  mx = block_max(mx, red);
-  float sum = 0.f;
-  for (int c = threadIdx.x; c < V; c += blockDim.x) sum += expf(row[c] - mx);
-  sum = block_sum(sum, red);
-  float lse = mx + logf(sum);
+  const float lse = row_lse(row, V, red);
   for (int c = threadIdx.x; c < V; c += blockDim.x) row[c] -= lse;
+}
+
+// (v, c) precedes (w, d) in torch.topk's order with the pinned tie rule: value descending, class ascending
+__device__ __forceinline__ bool topk_before(float v, int c, float w, int d) { return v > w || (v == w && c < d); }
+
+// k_logsoftmax_rows followed by k_topk_rows, without writing the (rows, V) log-probabilities: the logits are read three
+// times whatever k is.  Each thread keeps the KMAX best (x - lse, class) pairs of its strided columns, sorted, in
+// registers; the block then pops k winners from the thread heads.  Same values and order as the two-kernel path, bit for
+// bit.  A row whose mask id is 0 is all zeros there: its top k is classes 0..k-1 with value 0.
+template <int KMAX>
+__global__ void __launch_bounds__(256) k_logsoftmax_topk_rows(const float* __restrict__ x, const int32_t* __restrict__ mask_ids,
+                                                              int V, int k, float* __restrict__ topv, int32_t* __restrict__ topi) {
+  __shared__ float red[33];
+  __shared__ float sv[8];
+  __shared__ int si[8];
+  __shared__ int win;
+  const int64_t r = blockIdx.x;
+  if (mask_ids && mask_ids[r] == 0) {
+    for (int j = threadIdx.x; j < k; j += blockDim.x) { topv[r * k + j] = 0.f; topi[r * k + j] = j; }
+    return;
+  }
+  const float* row = x + r * V;
+  const float lse = row_lse(row, V, red);
+  float lv[KMAX]; int lc[KMAX];
+#pragma unroll
+  for (int i = 0; i < KMAX; ++i) { lv[i] = -INFINITY; lc[i] = 0x7fffffff; }
+  for (int c = threadIdx.x; c < V; c += blockDim.x) {
+    float v = row[c] - lse;
+    if (!topk_before(v, c, lv[KMAX - 1], lc[KMAX - 1])) continue;
+    int ci = c;
+#pragma unroll
+    for (int i = 0; i < KMAX; ++i) {         // insertion: (v, ci) displaces every later entry by one
+      if (topk_before(v, ci, lv[i], lc[i])) {
+        const float tv = lv[i]; const int tc = lc[i];
+        lv[i] = v; lc[i] = ci; v = tv; ci = tc;
+      }
+    }
+  }
+  for (int j = 0; j < k; ++j) {
+    float bv = lv[0]; int bi = lc[0];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(FULL, bv, o);
+      const int oi = __shfl_xor_sync(FULL, bi, o);
+      if (topk_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = bv; si[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+        if (topk_before(sv[w], si[w], bv, bi)) { bv = sv[w]; bi = si[w]; }
+      topv[r * k + j] = bv; topi[r * k + j] = bi;
+      win = bi;
+    }
+    __syncthreads();
+    if (lc[0] == win) {                        // the owner of the winning column pops its head
+#pragma unroll
+      for (int i = 0; i < KMAX - 1; ++i) { lv[i] = lv[i + 1]; lc[i] = lc[i + 1]; }
+      lv[KMAX - 1] = -INFINITY; lc[KMAX - 1] = 0x7fffffff;
+    }
+    __syncthreads();
+  }
+}
+
+// The candidate merge of one beam-search step (model.lua:529-569 as model.py restates it), one warp per round n.  Row
+// n*k + w is hypothesis (column) w of round n; candidate q = w*k + j is the j-th best class of row n*k + w, scored
+// scores[w] + topv in fp64.  At step 1 only column 0 is explored.  Candidates whose token is end_token compete for the
+// round's best finished hypothesis (strictly greater replaces: the first maximum in (step, q) order wins, as the
+// reference's stable sort keeps it); the others are ranked by (score desc, q asc) and the first min(#, k) fill columns
+// 0.. from the PRE-merge beams.  A column left unfilled keeps its beam and score, and is fed next step the state it was
+// fed this step (parent -1 - row) and its beam's next position (a pad, 0).  beams: (N, k, L) token histories.
+__global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int L, int end_token, const float* __restrict__ topv,
+                                                   const int32_t* __restrict__ topi, const double* __restrict__ sc_in,
+                                                   double* __restrict__ sc_out, const int32_t* __restrict__ beams_in,
+                                                   int32_t* __restrict__ beams_out, int32_t* __restrict__ tokens,
+                                                   int32_t* __restrict__ parent, int32_t* __restrict__ ans, int32_t* __restrict__ ans_len,
+                                                   double* __restrict__ ans_score) {
+  __shared__ int win_q[32];
+  __shared__ double win_s[32];
+  const int n = blockIdx.x, lane = threadIdx.x;
+  const int ncand = (stp == 1 ? 1 : k) * k;
+  const float* tv = topv + (int64_t)n * k * k;          // rows n*k .. n*k+k-1, k entries each: index q
+  const int32_t* ti = topi + (int64_t)n * k * k;
+  const double* sc = sc_in + (int64_t)n * k;
+  const int32_t* bin = beams_in + (int64_t)n * k * L;
+  // finished hypotheses of this step: the first maximum, then against the round's best so far
+  bool fnd = false; double fs = 0.0; int fq = 0x7fffffff;
+  for (int q = lane; q < ncand; q += 32) {
+    if (ti[q] + 1 != end_token) continue;
+    const double s = sc[q / k] + (double)tv[q];
+    if (!fnd || s > fs) { fnd = true; fs = s; fq = q; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const bool of = __shfl_xor_sync(FULL, fnd, o);
+    const double os = __shfl_xor_sync(FULL, fs, o);
+    const int oq = __shfl_xor_sync(FULL, fq, o);
+    if (of && (!fnd || os > fs || (os == fs && oq < fq))) { fnd = true; fs = os; fq = oq; }
+  }
+  const bool better = fnd && (ans_len[n] == 0 || fs > ans_score[n]);    // warp-uniform
+  __syncwarp();                                            // every lane has read the best so far before lane 0 replaces it
+  if (better) {
+    const int w = fq / k;
+    for (int p = lane; p < stp; p += 32) ans[(int64_t)n * L + p] = bin[(int64_t)w * L + p];
+    if (lane == 0) { ans[(int64_t)n * L + stp] = end_token; ans_len[n] = stp + 1; ans_score[n] = fs; }
+  }
+  // the k best other candidates: round j takes the best one strictly after round j-1's winner
+  int nfill = 0;
+  double ps = INFINITY; int pq = -1;
+  for (int j = 0; j < k; ++j) {
+    bool ok = false; double bs = 0.0; int bq = 0x7fffffff;
+    for (int q = lane; q < ncand; q += 32) {
+      if (ti[q] + 1 == end_token) continue;
+      const double s = sc[q / k] + (double)tv[q];
+      if (!(s < ps || (s == ps && q > pq))) continue;
+      if (!ok || s > bs) { ok = true; bs = s; bq = q; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const bool of = __shfl_xor_sync(FULL, ok, o);
+      const double os = __shfl_xor_sync(FULL, bs, o);
+      const int oq = __shfl_xor_sync(FULL, bq, o);
+      if (of && (!ok || os > bs || (os == bs && oq < bq))) { ok = true; bs = os; bq = oq; }
+    }
+    if (!ok) break;                                        // warp-uniform
+    if (lane == 0) { win_q[j] = bq; win_s[j] = bs; }
+    nfill = j + 1; ps = bs; pq = bq;
+  }
+  __syncwarp();
+  const int row0 = n * k;
+  for (int i = lane; i < k * (stp + 1); i += 32) {
+    const int c = i / (stp + 1), p = i % (stp + 1);
+    int32_t t;
+    if (c < nfill) {
+      const int q = win_q[c];
+      t = p < stp ? bin[(int64_t)(q / k) * L + p] : ti[q] + 1;
+    } else {
+      t = p < stp ? bin[(int64_t)c * L + p] : 0;
+    }
+    beams_out[((int64_t)row0 + c) * L + p] = t;
+    if (p == stp) tokens[row0 + c] = t;
+  }
+  for (int c = lane; c < k; c += 32) {
+    const bool f = c < nfill;
+    sc_out[row0 + c] = f ? win_s[c] : sc[c];
+    parent[row0 + c] = f ? row0 + win_q[c] / k : -1 - (row0 + c);
+  }
+}
+
+// start of a search: every hypothesis is <start> with score 0, no round has a finished hypothesis yet
+__global__ void k_beam_init(int64_t rows, int L, int start_token, int32_t* __restrict__ beams, int32_t* __restrict__ tokens,
+                            double* __restrict__ scores) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * L) return;
+  const int64_t r = i / L; const int p = (int)(i % L);
+  beams[i] = p == 0 ? start_token : 0;
+  if (p == 0) { tokens[r] = start_token; scores[r] = 0.0; }
 }
 __global__ void k_nll_fwd(const float* __restrict__ logp, const int32_t* __restrict__ tgt, const int32_t* __restrict__ mask_ids,
                           float* __restrict__ row_loss, int64_t rows, int V) {
@@ -1231,6 +1394,29 @@ void topk_rows(LaunchCtx& cx, const float* x, int64_t rows, int V, int k, float*
 }
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H) {
   L1D(k_beam_gather, rows * H, dst, out_prev, in_prev, parent, rows, H);
+}
+void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
+                          int32_t* topi) {
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= V, VD_E_BADARG, "logsoftmax_topk_rows: k");
+  if (rows == 0) return;
+  const unsigned g = (unsigned)rows;
+  if (k <= 4) k_logsoftmax_topk_rows<4><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
+  else if (k <= 8) k_logsoftmax_topk_rows<8><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
+  else if (k <= 16) k_logsoftmax_topk_rows<16><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
+  else k_logsoftmax_topk_rows<32><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
+  check_launch(cx, "k_logsoftmax_topk_rows");
+}
+void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* beams, int32_t* tokens, double* scores) {
+  L1D(k_beam_init, rows * L, rows, L, start_token, beams, tokens, scores);
+}
+void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int L, int end_token, const float* topv, const int32_t* topi,
+                const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out, int32_t* tokens,
+                int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score) {
+  VD_REQUIRE(k >= 1 && k <= 32 && stp >= 1 && stp < L, VD_E_BADARG, "beam_merge: k / step");
+  if (N == 0) return;
+  k_beam_merge<<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, L, end_token, topv, topi, scores_in, scores_out, beams_in, beams_out,
+                                                  tokens, parent, ans, ans_len, ans_score);
+  check_launch(cx, "k_beam_merge");
 }
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1, float beta2,
                 float eps, float grad_scale) {

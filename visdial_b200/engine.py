@@ -195,6 +195,7 @@ class Engine:
         h = C.c_void_p()
         check(self.lib.vd_create(C.byref(self.cparams), C.byref(h)))
         self.h = h
+        self._enc_rows = None          # N of the last encoder forward: the row count of vd_gen_beam_search's outputs
         n = C.c_int64()
         check(self.lib.vd_num_params(self.h, C.byref(n)))
         self.num_params = n.value
@@ -268,7 +269,9 @@ class Engine:
 
     def encoder_forward(self, batch: Batch) -> DeviceTensor:
         p = C.c_void_p()
+        self._enc_rows = None
         check(self.lib.vd_encoder_forward(self.h, C.byref(batch.c), C.byref(p)))
+        self._enc_rows = self._N(batch)
         return DeviceTensor(self, p.value, (self._N(batch), self.params["rnnHiddenSize"]))
 
     def forward_connect(self):
@@ -305,13 +308,17 @@ class Engine:
     # ---- fused ------------------------------------------------------------------------------------
     def forward_backward(self, batch: Batch, only_forward: bool = False) -> float:
         loss = C.c_float()
+        self._enc_rows = None
         check(self.lib.vd_forward_backward(self.h, C.byref(batch.c), int(only_forward), C.byref(loss)))
+        self._enc_rows = self._N(batch)
         return loss.value
 
     def retrieve(self, batch: Batch, use_gt: bool = True) -> np.ndarray:
         N = self._N(batch)
         out = np.empty((N,) if use_gt else (N, self.params["numOptions"]), dtype=np.int32)
+        self._enc_rows = None
         check(self.lib.vd_retrieve(self.h, C.byref(batch.c), int(use_gt), out.ctypes.data))
+        self._enc_rows = N
         return out
 
     # ---- Model:generateAnswers building blocks (model.lua:432-613) ---------------------------------------------
@@ -357,6 +364,19 @@ class Engine:
             check(self.lib.vd_gen_beam_step(self.h, rows, tokens.ctypes.data, par.ctypes.data, None, None, k, topv.ctypes.data,
                                             topi.ctypes.data))
         return topv, topi
+
+    def gen_beam_search(self, k: int, L: int, start: int, end: int):
+        """The whole beam search for every round of the last encoder forward on the device (vd_gen_beam_search).  Returns
+        (answer (N, L) int32, length (N) int32 — 0 where no beam reached `end` — and score (N) float64)."""
+        N = self._enc_rows
+        if N is None:
+            raise _lib.VdError(_lib.VD_E_STATE, "gen_beam_search before encoder_forward")
+        ans = np.zeros((N, int(L)), dtype=np.int32)
+        length = np.zeros(N, dtype=np.int32)
+        score = np.zeros(N, dtype=np.float64)
+        check(self.lib.vd_gen_beam_search(self.h, int(k), int(L), int(start), int(end), ans.ctypes.data, length.ctypes.data,
+                                          score.ctypes.data))
+        return ans, length, score
 
     def upload(self, dev_ptr: int, a: np.ndarray):
         a = np.ascontiguousarray(a, dtype=np.float32)

@@ -1,7 +1,8 @@
 """Mirror of the reference's `Model` class (/root/reference/model.lua:8-430) over the C engine.
 Same method names, argument meaning and call order as the Lua original, so that the parity tests
-read like the reference's own driver code.  `generateAnswers` (beam search / sampling, model.lua:432-613) steps the
-decoder on the device through vd_gen_decoder_step and keeps the hypothesis bookkeeping on the host like the Lua."""
+read like the reference's own driver code.  `generateAnswers` (beam search / sampling, model.lua:432-613) runs the beam
+search entirely on the device (vd_gen_beam_search); sampling and the reference-structured beam loop step the decoder through
+vd_gen_decoder_step and keep the hypothesis bookkeeping on the host like the Lua."""
 from __future__ import annotations
 
 import numpy as np
@@ -179,11 +180,12 @@ class Model:
 
     # ---- beam search / sampling (model.lua:432-613, generate.lua) ---------------------------------------------
     def generateAnswers(self, dataloader, dtype="val", params=None, strict=True):
-        """Model:generateAnswers: per dialog, encoder forward on the device, then the decoder driven one step at a time
-        through vd_gen_decoder_step; the hypothesis bookkeeping runs on the host exactly as the Lua does (it indexes
-        GPU tensors scalar by scalar).  Returns the reference's answerTable with token-id lists (and text when the
-        dataloader carries ind2word).  `strict=False` yields None for a round where no beam reached <END> (the
-        reference indexes nil there, model.lua:575)."""
+        """Model:generateAnswers.  Beam search (the default) runs entirely on the device through vd_gen_beam_search, for
+        `params.dialogsPerCall` dialogs (default 1) per encoder forward: every round of those dialogs is searched at once.
+        `hostBeam = 1` (the reference's loop structure) and sampling go one dialog at a time, the decoder stepped through
+        vd_gen_decoder_step and the hypothesis bookkeeping on the host as the Lua does it.  Returns the reference's
+        answerTable with token-id lists (and text when the dataloader carries ind2word).  `strict=False` yields None for a
+        round where no beam reached <END> (the reference indexes nil there, model.lua:575)."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
@@ -196,6 +198,23 @@ class Model:
         rng = np.random.default_rng(int(params.get("seed", 1234)))
         eng, H = self.engine, self.params["rnnHiddenSize"]
         words = (lambda ids: " ".join(ind2word.get(int(t), "<UNK>") for t in ids if int(t) > 0)) if ind2word else None
+        img = getattr(dataloader, "unique_img_" + dtype, None)
+        # getIndexData hands out this rank's slice of the split: the image list is indexed by the global dialog id
+        first = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
+
+        def image_id(convId):
+            gid = convId + first
+            return _image_id(img[gid]) if img is not None else gid
+
+        def entry(q, answer, score, length):
+            e = {"question": q.tolist(), "answer": answer.tolist(), "score": score, "length": length}
+            if words:
+                e["question_text"], e["answer_text"] = words(q), words(answer)
+            return e
+
+        if not sampleWords and not params.get("hostBeam"):
+            return self._generate_beam(dataloader, dtype, numThreads, max(1, int(params.get("dialogsPerCall", 1))), beamSize,
+                                       beamLen, startToken, endToken, strict, image_id, entry)
         state_buf = [eng.device_alloc(max(beamSize, self.params["maxQuesCount"]) * H * 4) for _ in range(4)]
         answerTable = []
         try:
@@ -216,64 +235,9 @@ class Model:
                         eng.upload(state_buf[i], a[:n])
                     return eng.gen_decoder_step(tokens, state_buf[0:2], state_buf[2:4])
 
-                if not sampleWords and not params.get("hostBeam"):
-                    # All N rounds of the dialog are searched at once (N * beamSize hypotheses per decoder step).  The LSTM state
-                    # and the (rows, V) log-probabilities stay on the device (vd_gen_beam_step): per step the tokens and parent
-                    # indices go up, the beamSize best (log-prob, class) pairs of every hypothesis come down; the candidate merge
-                    # of model.lua:529-569 — including its quirks — runs on those few numbers.
-                    bs = beamSize
-                    beams = np.zeros((N, beamLen, bs), dtype=np.int64)                  # :479
-                    beams[:, 0, :] = startToken                                         # :506
-                    scores = np.zeros((N, bs), dtype=np.float64)                        # :507
-                    finish = [[] for _ in range(N)]                                     # :508
-                    if has_layers:                                                      # :482-491
-                        iH = [np.repeat(encH[0][0], bs, 0), np.repeat(encOut, bs, 0)]
-                        iC = [np.repeat(encH[0][1], bs, 0), np.repeat(encH[1][1], bs, 0)]
-                    else:                                                               # :493-501
-                        z = np.zeros((N * bs, H), np.float32)
-                        iH, iC = [z, np.repeat(encOut, bs, 0)], [z, z]
-                    parent = None
-                    for stp in range(1, beamLen):                                       # :510
-                        topv, topi = eng.gen_beam_step(beams[:, stp - 1, :].reshape(-1), parent, iH, iC, bs)   # :519-542
-                        parent = -1 - np.arange(N * bs, dtype=np.int32)                 # default: the column keeps its old content
-                        exploreSize = 1 if stp == 1 else bs                             # :516
-                        for it in range(N):
-                            cands = []
-                            for wordId in range(exploreSize):                           # :529
-                                r = it * bs + wordId
-                                for candId in range(bs):                                # :544
-                                    tok = int(topi[r, candId]) + 1
-                                    sc = float(scores[it, wordId]) + float(topv[r, candId])
-                                    if tok == endToken:                                 # :548
-                                        cb = beams[it, :, wordId].copy()
-                                        cb[stp] = tok
-                                        finish[it].append({"beam": cb, "length": stp + 1, "score": sc})
-                                    else:
-                                        cands.append((sc, wordId, tok))
-                            cands.sort(key=lambda t: -t[0])                             # :558 (stable)
-                            old = beams[it].copy()
-                            for candId in range(min(len(cands), bs)):                   # :560-569
-                                sc, wordId, tok = cands[candId]
-                                beams[it, :, candId] = old[:, wordId]
-                                beams[it, stp, candId] = tok
-                                scores[it, candId] = sc
-                                parent[it * bs + candId] = it * bs + wordId
-                    for it in range(N):
-                        finish[it].sort(key=lambda d: -d["score"])                      # :572
-                        if not finish[it]:
-                            if strict:
-                                raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
-                            threadAnswers.append(None)
-                            continue
-                        best = finish[it][0]
-                        entry = {"question": ques[it].tolist(), "answer": best["beam"].tolist(), "score": best["score"],
-                                 "length": best["length"]}
-                        if words:
-                            entry["question_text"], entry["answer_text"] = words(ques[it]), words(best["beam"])
-                        threadAnswers.append(entry)
-                elif not sampleWords:
+                if not sampleWords:
                     # the reference's own loop structure (one round at a time, log-probabilities and state through the host):
-                    # kept as the cross-check of the batched search above (params.hostBeam = 1)
+                    # kept as the cross-check of the device search (params.hostBeam = 1)
                     for it in range(N):                                                 # :472
                         beams = np.zeros((beamLen, beamSize), dtype=np.int64)           # :479
                         if has_layers:                                                  # :482-491
@@ -316,11 +280,7 @@ class Model:
                             threadAnswers.append(None)
                             continue
                         best = finishBeams[0]
-                        entry = {"question": ques[it].tolist(), "answer": best["beam"].tolist(), "score": best["score"],
-                                 "length": best["length"]}
-                        if words:
-                            entry["question_text"], entry["answer_text"] = words(ques[it]), words(best["beam"])
-                        threadAnswers.append(entry)
+                        threadAnswers.append(entry(ques[it], best["beam"], best["score"], best["length"]))
                 else:                                                                   # :581-602
                     if has_layers:                                                      # forwardConnect, gen.lua:30-42
                         Hs, Cs = [encH[0][0], encOut], [encH[0][1], encH[1][1]]
@@ -336,18 +296,52 @@ class Model:
                         seq.append(tok.copy())
                     ans = np.stack(seq, 1)
                     for it in range(N):
-                        entry = {"question": ques[it].tolist(), "answer": ans[it].tolist()}
+                        e = {"question": ques[it].tolist(), "answer": ans[it].tolist()}
                         if words:
-                            entry["question_text"], entry["answer_text"] = words(ques[it]), words(ans[it])
-                        threadAnswers.append(entry)
+                            e["question_text"], e["answer_text"] = words(ques[it]), words(ans[it])
+                        threadAnswers.append(e)
                 self.wrapper.training()                                                 # :605
-                img = getattr(dataloader, "unique_img_" + dtype, None)
-                # getIndexData hands out this rank's slice of the split: the image list is indexed by the global dialog id
-                gid = convId + (dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0)
-                answerTable.append({"image_id": _image_id(img[gid]) if img is not None else gid, "dialog": threadAnswers})   # :606
+                answerTable.append({"image_id": image_id(convId), "dialog": threadAnswers})   # :606
         finally:
             for p in state_buf:
                 eng.device_free(p)
+        return answerTable
+
+    def _generate_beam(self, dataloader, dtype, numThreads, dialogsPerCall, beamSize, beamLen, startToken, endToken, strict,
+                       image_id, entry):
+        """generateAnswers' beam search, `dialogsPerCall` dialogs per encoder forward and per vd_gen_beam_search call.  One
+        dialog per call gives exactly the per-dialog trimming and kernel shapes of the reference's loop; more dialogs per call
+        run wider kernels (in the tensor-core math modes their rounding can differ from per-dialog runs)."""
+        answerTable = []
+        ques_len = None
+        for first in range(0, numThreads, dialogsPerCall):
+            inds = np.arange(first, min(numThreads, first + dialogsPerCall))
+            self.wrapper.evaluate()                                                     # :460
+            batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
+            self.forwardBackward(batch, True, True)                                     # :467
+            ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
+            Tq = ques.shape[2]
+            answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)   # :472-579
+            answer = answer.reshape(len(inds), -1, beamLen)
+            length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
+            self.wrapper.training()                                                     # :605
+            for d, convId in enumerate(inds):
+                # a one-dialog batch keeps the rightmost (its longest question) columns (dataloader.lua:380-384)
+                if len(inds) == 1:
+                    w = Tq
+                else:
+                    if ques_len is None:
+                        ques_len = dataloader.corpus[dtype].raw["ques_length"]
+                    w = int(ques_len[dataloader.part[dtype][0] + convId].max())
+                threadAnswers = []
+                for it in range(ques.shape[1]):
+                    if length[d, it] == 0:
+                        if strict:
+                            raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
+                        threadAnswers.append(None)
+                        continue
+                    threadAnswers.append(entry(ques[d, it, Tq - w:], answer[d, it], float(score[d, it]), int(length[d, it])))
+                answerTable.append({"image_id": image_id(int(convId)), "dialog": threadAnswers})   # :606
         return answerTable
 
     # ---- checkpoints (train.lua:33-34,78-80,99-102,120-121; evaluate.lua:58-91) -------------------------------
