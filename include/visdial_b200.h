@@ -178,6 +178,18 @@ int vd_gen_beam_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, con
  * and beam_len >= 2.  Ends any search vd_gen_beam_step was continuing. */
 int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
                        int32_t* answer_host, int32_t* length_host, double* score_host);
+/* Model:generateAnswers' sampling (model.lua:581-602, sampleWords = 1) for EVERY round of the last vd_encoder_forward (N =
+ * B * maxQuesCount rows), entirely on the device, the decoder fed its own samples (gen.lua:63-68).  One synchronisation, at
+ * the end.  Draw rule (Gumbel-max over x / temperature, counter-based Philox; see DESIGN §14): the token of step t of row r
+ * depends only on (seed, row_offset + r, t, the logits), so rounds sampled in different calls or on different ranks draw
+ * the same tokens when row_offset is the global index of the call's first round.
+ * answer_host (N, beam_len + 1) int32: column 0 = start_token, columns 1..beam_len the samples.  logp_host (N, beam_len) or
+ * NULL: each sampled token's log-probability under the un-tempered LogSoftMax output (decOut).
+ * VD_E_STATE for a disc engine or before any vd_encoder_forward; VD_E_BADARG unless beam_len >= 1, temperature is finite and
+ * > 0, row_offset >= 0, 1 <= start_token <= vocabSize and answer_host != NULL.  Ends any search vd_gen_beam_step was
+ * continuing. */
+int vd_gen_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
+                  int32_t* answer_host, float* logp_host);
 
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.

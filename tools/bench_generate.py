@@ -1,14 +1,18 @@
-"""Model:generateAnswers (model.lua:432-613) wall time per dialog: beam search (beamSize 5, beamLen 20) over the 10 rounds of
-each dialog, V = 10 000, for `hrea-ques-im-hist + gen` (C3's graph) and `mn-att-ques-im-hist + gen`, in the F16 and FP32 math
-modes.  Paths, all in one run:
-  device/<d>  the default: vd_gen_beam_search, d dialogs per encoder forward and call (params.dialogsPerCall)
+"""Model:generateAnswers (model.lua:432-613) wall time per dialog: beam search (beamSize 5, beamLen 20) or sampling (beamLen
+20, sampleWords = 1) over the 10 rounds of each dialog, V = 10 000, for `hrea-ques-im-hist + gen` (C3's graph) and
+`mn-att-ques-im-hist + gen`, in the F16 and FP32 math modes.  Paths, all in one run:
+  device/<d>  beam search, the default: vd_gen_beam_search, d dialogs per encoder forward and call (params.dialogsPerCall)
   host_merge  the search as the engine ran it before it moved to the device: per dialog, the candidate merge on the host
               over vd_gen_beam_step (tests/test_beam_search_gpu.py::host_beam_search)
   host_beam   params.hostBeam = 1: the reference's loop structure, one round at a time through vd_gen_decoder_step
+  sample/<d>  sampling: vd_gen_sample, d dialogs per encoder forward and call
+  host_sample sampling as the engine ran it before it moved to the device: per dialog and step, the state up, one
+              vd_gen_decoder_step, the log-probabilities and state down, one numpy categorical draw per round (host_sample)
 Every path is warmed up at its shape first, then timed over whole calls until the window lasts at least --window seconds
 (host clock; every call ends in a device synchronisation).  Prints one JSON line per (encoder, mode, path) and the card's name
 and power limit, read in the same run.
-usage: python tools/bench_generate.py [--encoders a,b] [--modes f16,fp32] [--dpc 1,8,32,128] [--window 1.0] [--out FILE]"""
+usage: python tools/bench_generate.py [--encoders a,b] [--modes f16,fp32] [--dpc 1,8,32,128] [--kinds beam,sample]
+                                      [--window 1.0] [--out FILE]"""
 import argparse
 import json
 import os
@@ -41,6 +45,32 @@ def card():
     return name, power
 
 
+def host_sample(eng, encOut, L, start, T, rng):
+    """the sampling branch of Model.generateAnswers before it moved to the device (one dialog: all its rounds per step)"""
+    N, H = encOut.shape
+    (h1, c1), (_, c2) = [eng.encoder_rnn_state(l, N) for l in range(2)]
+    if h1 is not None:                                                          # forwardConnect, gen.lua:30-42
+        Hs, Cs = [h1.numpy(), encOut], [c1.numpy(), c2.numpy()]
+    else:
+        Hs, Cs = [np.zeros((N, H), np.float32), encOut], [np.zeros((N, H), np.float32)] * 2
+    bufs = [eng.device_alloc(N * H * 4) for _ in range(4)]
+    try:
+        tok = np.full(N, start, dtype=np.int64)
+        seq = [tok.copy()]
+        for _ in range(L):
+            for i, a in enumerate(Hs + Cs):
+                eng.upload(bufs[i], a)
+            decOut, Hs, Cs = eng.gen_decoder_step(tok, bufs[0:2], bufs[2:4])     # :586-588 (+ decoderConnect)
+            p = np.exp(decOut.astype(np.float64) / T)                           # :590
+            p /= p.sum(1, keepdims=True)
+            tok = np.array([rng.choice(p.shape[1], p=p[i]) + 1 for i in range(N)], dtype=np.int64)
+            seq.append(tok.copy())
+    finally:
+        for b in bufs:
+            eng.device_free(b)
+    return np.stack(seq, 1)
+
+
 def window(call, dialogs_per_call, seconds):
     """ms per dialog over whole calls, after one warm-up call of the same shape"""
     call()
@@ -58,10 +88,12 @@ def main():
     ap.add_argument("--encoders", default="hrea-ques-im-hist,mn-att-ques-im-hist")
     ap.add_argument("--modes", default="f16,fp32")
     ap.add_argument("--dpc", default="1,8,32,128")
+    ap.add_argument("--kinds", default="beam,sample")
     ap.add_argument("--window", type=float, default=1.0)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     dpcs = [int(x) for x in a.dpc.split(",")]
+    kinds = a.kinds.split(",")
     name, power = card()
     rows = []
     for enc in a.encoders.split(","):
@@ -83,10 +115,26 @@ def main():
                 host_beam_search(m.engine, encOut, BEAM, LEN, start, end)
                 m.wrapper.training()
 
-            paths = [("device/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(beam, maxThreads=d, dialogsPerCall=d),
-                                                                        strict=False)) for d in dpcs]
-            paths += [("host_merge", 1, host_merge),
-                      ("host_beam", 1, lambda: m.generateAnswers(dl, "val", dict(beam, maxThreads=1, hostBeam=1), strict=False))]
+            samp = {"sampleWords": 1, "beamLen": LEN, "temperature": 1.0}
+            rng = np.random.default_rng(1234)
+
+            def host_samp():
+                m.wrapper.evaluate()
+                b = dl.getIndexData(np.array([0]), m.params, "val")
+                encOut = m.forwardBackward(b, True, True).numpy()
+                host_sample(m.engine, encOut, LEN, start, 1.0, rng)
+                m.wrapper.training()
+
+            paths = []
+            if "beam" in kinds:
+                paths += [("device/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(beam, maxThreads=d, dialogsPerCall=d),
+                                                                             strict=False)) for d in dpcs]
+                paths += [("host_merge", 1, host_merge),
+                          ("host_beam", 1, lambda: m.generateAnswers(dl, "val", dict(beam, maxThreads=1, hostBeam=1), strict=False))]
+            if "sample" in kinds:
+                paths += [("sample/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(samp, maxThreads=d, dialogsPerCall=d)))
+                          for d in dpcs]
+                paths += [("host_sample", 1, host_samp)]
             for path, d, call in paths:
                 ms, n, dt = window(call, d, a.window)
                 r = {"encoder": enc, "mode": mode, "path": path, "ms_per_dialog": round(ms, 3), "dialogs_timed": n,
@@ -94,8 +142,9 @@ def main():
                 print(json.dumps(r), flush=True)
                 rows.append(r)
         dl.close(); m.engine.close()
-    print("\n%s, power limit %s: ms per dialog (beam %d x %d, V = %d)" % (name, power, BEAM, LEN, V))
-    paths = sorted({r["path"] for r in rows}, key=lambda s: (not s.startswith("device"), int(s.split("/")[1]) if "/" in s else 0, s))
+    print("\n%s, power limit %s: ms per dialog (beam %d x %d / sampling x %d, V = %d)" % (name, power, BEAM, LEN, LEN, V))
+    order = ["device", "host_merge", "host_beam", "sample", "host_sample"]
+    paths = sorted({r["path"] for r in rows}, key=lambda s: (order.index(s.split("/")[0]), int(s.split("/")[1]) if "/" in s else 0))
     print("| encoder | mode | " + " | ".join(paths) + " |")
     print("|---|---|" + "---|" * len(paths))
     for enc in a.encoders.split(","):

@@ -254,6 +254,11 @@ int vd_gen_beam_search(vd_engine* h, int32_t beam_size, int32_t beam_len, int32_
   VD_TRY({ ENG(h)->gen_beam_search(beam_size, beam_len, start_token, end_token, answer_host, length_host, score_host); })
 }
 
+int vd_gen_sample(vd_engine* h, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
+                  int32_t* answer_host, float* logp_host) {
+  VD_TRY({ ENG(h)->gen_sample(beam_len, start_token, temperature, seed, row_offset, answer_host, logp_host); })
+}
+
 int vd_clamp_adam_step(vd_engine* h, float lr) { VD_TRY({ ENG(h)->clamp_adam_step(lr); }) }
 
 int vd_comm_unique_id(void* id_out) { VD_TRY({ NOTNULL(id_out); vd::comm_unique_id(id_out); }) }

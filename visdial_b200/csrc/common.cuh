@@ -82,8 +82,41 @@ __device__ __forceinline__ void drop_factor4(const DropCfg& d, uint32_t site, ui
 // Dropout sites (mirrors oracle/visdial_oracle.py)
 enum : uint32_t {
   SITE_QEMBED = 0, SITE_HEMBED = 1, SITE_HATT = 2, SITE_IMG_TR = 3, SITE_U_OUT = 5,
-  SITE_FUSION = 6, SITE_IMG_FC7 = 7, SITE_HOP0 = 16
+  SITE_FUSION = 6, SITE_IMG_FC7 = 7, SITE_HOP0 = 16,
+  SITE_SAMPLE = 64          // generateAnswers' sampling draws (not a dropout site)
 };
+
+// ---------------------------------------------------------------------------------------------
+// Sampling (Engine::gen_sample, model.lua:584-602) by the Gumbel-max trick: the token drawn from step `step`'s row r is
+// 1 + argmax_j (x_j / T + g_j), x = the vocabulary logits with bias, ties to the lower class.  g_j = -log(-log(u_j)),
+// u_j = ((w >> 8) + 0.5) 2^-24, w = Philox4x32-10 word idx % 4 at counter (idx/4 lo, idx/4 hi, SITE_SAMPLE, step), key =
+// seed, idx = (row_offset + r) V + j: the element index of the step's (rows, V) decOut over the whole split, so a draw
+// depends only on (seed, global round, step, class).  Exactly a draw from softmax(x / T) = exp(logp / T) / sum.  Every
+// device route evaluates the key with these full-precision functions, so equal logits give equal tokens on every route.
+// The numpy twin is tests/sampling_twin.py.
+// ---------------------------------------------------------------------------------------------
+struct SampleCfg {
+  uint32_t seed_lo, seed_hi, step;
+  float temperature;
+  int64_t row_offset;       // global round of row 0
+};
+// largest Gumbel value the rule can produce (u = 1 - 2^-25: -log(-log u) = 17.33): an element whose x / T + GUMBEL_MAX is
+// below the best key so far cannot win, so its Philox word and logarithms need not be computed
+constexpr float GUMBEL_MAX = 17.5f;
+
+// g of one Philox word.  u has 25 significant bits, so -log(u) is formed from an exact operand: u itself below 1/2,
+// 1 - u (through log1p) above it.
+__device__ __forceinline__ float gumbel_of_word(uint32_t w) {
+  const uint32_t m = w >> 8;
+  const float t = m < (1u << 23) ? -logf(((float)m + 0.5f) * 0x1p-24f)
+                                 : -log1pf(-(((float)((1u << 24) - m) - 0.5f) * 0x1p-24f));
+  return -logf(t);
+}
+__device__ __forceinline__ void sample_words(const SampleCfg& s, uint64_t q, uint32_t o[4]) {
+  philox4x32_10((uint32_t)q, (uint32_t)(q >> 32), SITE_SAMPLE, s.step, s.seed_lo, s.seed_hi, o);
+}
+// (key, class) beats (key2, class2): key descending, class ascending
+__device__ __forceinline__ bool sample_before(float k, int c, float k2, int c2) { return k > k2 || (k == k2 && c < c2); }
 
 // ---------------------------------------------------------------------------------------------
 // Launch context: stream + launch accounting + optional per-class event bracketing.

@@ -3,6 +3,7 @@
 #include "engine.h"
 #include <string.h>
 #include <math.h>
+#include <cmath>
 
 namespace vd {
 
@@ -1431,7 +1432,13 @@ void Engine::gen_decoder_step(int64_t rows, const int32_t* tokens_host, const fl
 }
 
 void Engine::gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev) {
-  const int E = cfg.E, H = cfg.H, V = cfg.V;
+  gen_decoder_step_lstm(rows, tok, h_prev, c_prev);
+  gstep_logp = arena.get<float>(rows * cfg.V);
+  linear_fwd(seg("dec.out.weight"), gstep2.h, rows, gstep_logp, 0);
+}
+
+void Engine::gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev) {
+  const int E = cfg.E, H = cfg.H;
   float* xa = arena.get<float>(rows * E);
   embed_rows(cx, xa, Wp(0), tok, rows, E, dropcfg(0.f), 0);
   gstep1 = make_run(1, rows, E, H, seg("dec.lstm1.weight"), xa, nullptr, tok);
@@ -1440,8 +1447,6 @@ void Engine::gen_decoder_step_logits(int64_t rows, const int32_t* tok, const flo
   gstep2 = make_run(1, rows, H, H, seg("dec.lstm2.weight"), gstep1.h, nullptr, tok);
   gstep2.h0 = h_prev ? h_prev[1] : nullptr; gstep2.c0 = c_prev ? c_prev[1] : nullptr;
   lstm_forward(gstep2, true);
-  gstep_logp = arena.get<float>(rows * V);
-  linear_fwd(seg("dec.out.weight"), gstep2.h, rows, gstep_logp, 0);
 }
 
 // One beam-search step (model.lua:510-570) for `rows` hypotheses at once (all rounds of a dialog x beamSize).  The state of
@@ -1546,6 +1551,78 @@ void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(length_host, ans_len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(score_host, ans_score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+// Model:generateAnswers' sampling (model.lua:581-602) for all N rounds of the last encoder forward at once, on the device.
+// Every step runs the decoder step of gen_decoder_step_logits on the device-resident tokens, then draws with the Gumbel-max
+// rule of common.cuh: fused into the vocabulary projection's epilogue (tensor-core modes, vocab_tc_ok's shapes) or from
+// materialised logits (k_logsoftmax_sample_rows).  The draw writes the next step's tokens, so nothing returns to the host
+// until the final copy of the answers and log-probabilities.
+void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
+                        float* logp_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_sample needs the gen decoder after encoder_forward");
+  VD_REQUIRE(L >= 1 && std::isfinite(temperature) && temperature > 0.f && row_offset >= 0 && start_token >= 1 &&
+             start_token <= cfg.V, VD_E_BADARG, "beam_len >= 1, finite temperature > 0, row_offset >= 0, start_token in [1, V]");
+  VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  cx.stream = main_stream;
+  forward_connect();
+  const int H = cfg.H, V = cfg.V;
+  const int64_t N = db.N;
+  const int wo = seg("dec.out.weight");
+  // allocated once per call
+  float* zero = arena.get<float>(N * H);
+  int32_t* tok = arena.get<int32_t>(N);
+  int32_t* ans = arena.get<int32_t>(N * (L + 1));
+  float* lp = arena.get<float>(N * L);
+  double* unused_scores = arena.get<double>(N);
+  const int nparts = vocab_lse_nparts(V);
+  float *pm = nullptr, *ps = nullptr, *pk = nullptr, *px = nullptr;
+  int32_t* pc = nullptr;
+  if (tcmode()) {
+    pm = arena.get<float>(N * nparts); ps = arena.get<float>(N * nparts); pk = arena.get<float>(N * nparts);
+    px = arena.get<float>(N * nparts); pc = arena.get<int32_t>(N * nparts);
+  }
+  VD_CUDA_CHECK(cudaMemsetAsync(zero, 0, (size_t)N * H * sizeof(float), cx.stream));
+  beam_init(cx, N, L + 1, start_token, ans, tok, unused_scores);       // answer column 0 = <START>, tokens = <START>
+  // h = {layer-1 h at Tq, encOut}, c = {layer-1 c, layer-2 c} (gen.lua:30-42); encoders without .rnnLayers feed explicit zero
+  // rows, not "no initial state", as gen_beam_search does
+  const float* h[2] = {gen_h0[0] ? gen_h0[0] : zero, gen_h0[1]};
+  const float* c[2] = {gen_c0[0] ? gen_c0[0] : zero, gen_c0[1] ? gen_c0[1] : zero};
+  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset};
+  // The step's decoder buffers alternate between two arena regions: step s reads the state step s-1 wrote into the other
+  // one, so the new state feeds the next step without a copy.  Same allocations every step, so a region lands where it
+  // did two steps earlier and the arena does not grow with L.
+  Arena::Mark region[2] = {arena.mark(), {}};
+  bool fused = false;
+  for (int stp = 1; stp <= L; ++stp) {
+    if (stp == 2) region[1] = arena.mark();
+    arena.rewind(region[(stp - 1) & 1]);
+    gen_decoder_step_lstm(N, tok, h, c);
+    smp.step = (uint32_t)stp;
+    bool took = false;
+    if (tcmode() && (stp == 1 || fused)) {
+      LaunchCtx::Scope sc(&cx, "vocab_sample", 2.0 * N * V * H, 4.0 * (N * (double)H + (double)V * H + 5.0 * N * nparts));
+      took = vocab_sample_tc(cx, (int)N, V, H, gstep2.h, H, Wp(wo), H, Wp(wo + 1), smp, pm, ps, pk, pc, px);
+      if (took) vocab_sample_finish(cx, pm, ps, pk, pc, px, nparts, N, stp, L, tok, ans, lp);
+    }
+    if (stp == 1) fused = took;
+    VD_REQUIRE(took == fused, VD_E_STATE, "vocab_sample_tc changed its mind between steps");
+    if (!fused) {
+      // logits written once, read by the row's lse (two passes) and the draw
+      LaunchCtx::Scope sc(&cx, "sample_rows", 2.0 * N * V * H, 4.0 * (N * (double)H + (double)V * H + 2.0 * N * V));
+      float* logits = arena.get<float>(N * V);
+      linear_fwd(wo, gstep2.h, N, logits, 0);
+      logsoftmax_sample_rows(cx, logits, N, V, smp, L, tok, ans, lp);
+    }
+    h[0] = gstep1.h; h[1] = gstep2.h;
+    c[0] = gstep1.c; c[1] = gstep2.c;
+  }
+  beam_rows = 0;                                   // gstep1 / gstep2 hold this call's state now: vd_gen_beam_step starts over
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  if (logp_host)
+    VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, lp, (size_t)N * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 

@@ -298,6 +298,11 @@ struct Engine {
                      const float* const* init_c_host, int k, float* topv_host, int32_t* topi_host);
   // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device
   void gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
+  // the decoder step up to the second LSTM layer (gstep1 / gstep2 hold the new state on return)
+  void gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
+  // Model:generateAnswers' sampling for every round of the last encoder forward, entirely on the device
+  void gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
+                  float* logp_host);
   void clamp_adam_step(float lr);
   void allreduce_grads();
   // Overlapped gradient sync (world > 1): dW is all-reduced in buckets on `comm_stream` as soon as each bucket's last

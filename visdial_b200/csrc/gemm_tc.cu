@@ -22,11 +22,13 @@ constexpr int MMA_K = 8;         // tf32: 32 bytes per instruction
 constexpr int EPI_WARPS = 8;     // the consumer warps: 2 per 32-row quarter, each takes half of the tile's columns
 constexpr int GEMM_THREADS = 128 + 32 * EPI_WARPS;
 
-enum { MODE_GENERIC = 0, MODE_LSTM_FWD = 1, MODE_LSTM_BWD = 2, MODE_LSE = 3, MODE_DLOGIT = 4 };
+enum { MODE_GENERIC = 0, MODE_LSTM_FWD = 1, MODE_LSTM_BWD = 2, MODE_LSE = 3, MODE_DLOGIT = 4, MODE_SAMPLE = 5 };
 // MODE_LSE    : vocabulary projection whose (rows, V) logits never leave the chip: per row and column slice only the running
 //               max, the sum of exponentials and the target's logit are written (gen.lua:23-24 + the criterion of model.lua:33-36
 //               / utils.computeLhood, utils.lua:86-102)
 // MODE_DLOGIT : the same contraction recomputed in the backward pass with the epilogue  C = keep * (exp(x - lse[row]) - onehot)
+// MODE_SAMPLE : MODE_LSE's statistics plus the slice's best Gumbel key x / T + g (common.cuh), its class and its logit
+//               (the sampling step of model.lua:584-593 without the logits in HBM)
 
 struct Params {
   int M, N, K;                    // GEMM sizes (N = output columns; LSTM_FWD: N = 4H, LSTM_BWD: N = H)
@@ -43,6 +45,8 @@ struct Params {
   // fused vocabulary softmax (MODE_LSE / MODE_DLOGIT): 1-based target class per row (0 = none), maskzero ids per row
   const int32_t* tgt; const int32_t* row_ids; const float* lse;
   float* part_max; float* part_sum; float* tgt_logit; int nparts;      // (M, nparts) partials, nparts = column tiles * slices
+  // MODE_SAMPLE: (M, nparts) best key, its class and its logit
+  float* part_key; int32_t* part_cls; float* part_x; SampleCfg smp;
 };
 
 __device__ __forceinline__ void ld8(const float* p, float* d) {
@@ -208,12 +212,17 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       const int64_t row = (int64_t)m0 + q * 32 + lane;
       const bool row_ok = row < p.M;
 
-      if (MODE == MODE_LSE) {
+      if (MODE == MODE_LSE || MODE == MODE_SAMPLE) {
         // online softmax statistics of this warp's column slice of the tile: nothing but (max, sum exp, target logit) leaves
         const int n0 = nt * BN;
-        const int tcol = row_ok ? p.tgt[row] - 1 : -1;
+        const int tcol = (MODE == MODE_LSE && row_ok) ? p.tgt[row] - 1 : -1;
         float mrun = -INFINITY, srun = 0.f, tl = 0.f;
         bool has = false;
+        // MODE_SAMPLE: the slice's best (key, class, logit); columns ascend, so a strictly greater key keeps ties on the
+        // lower class.  N % 4 == 0 and 8-column groups: element (row, n0 + c) starts a Philox quadruple.
+        float bkey = -INFINITY, bx = 0.f;
+        int bcls = 0x7fffffff;
+        const uint64_t ebase = MODE == MODE_SAMPLE ? (uint64_t)(p.smp.row_offset + row) * (uint64_t)p.N : 0;
 #pragma unroll 1
         for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 8) {
           if (n0 + c >= p.N) break;                 // warp-uniform
@@ -235,11 +244,31 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           for (int j = 0; j < 8; ++j) add += __expf(v[j] - mnew);      // exp(-inf) = 0 for the clipped columns
           srun = srun * __expf(mrun - mnew) + add;
           mrun = mnew;
+          if (MODE == MODE_SAMPLE && row_ok) {
+#pragma unroll
+            for (int h4 = 0; h4 < 2; ++h4) {
+              const int nb = n0 + c + 4 * h4;
+              if (nb >= p.N) break;
+              float y[4];
+              float ymax = -INFINITY;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) { y[j] = v[4 * h4 + j] / p.smp.temperature; ymax = fmaxf(ymax, y[j]); }
+              if (ymax + GUMBEL_MAX < bkey) continue;          // no key of the quadruple can reach the best one
+              uint32_t o[4];
+              sample_words(p.smp, (ebase + (uint64_t)nb) >> 2, o);
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+                const float key = y[j] + gumbel_of_word(o[j]);
+                if (key > bkey) { bkey = key; bcls = nb + j; bx = v[4 * h4 + j]; }
+              }
+            }
+          }
         }
         if (row_ok) {
           const int64_t pi = row * p.nparts + nt * NH + half;
           p.part_max[pi] = mrun; p.part_sum[pi] = srun;
-          if (has) p.tgt_logit[row] = tl;
+          if (MODE == MODE_SAMPLE) { p.part_key[pi] = bkey; p.part_cls[pi] = bcls; p.part_x[pi] = bx; }
+          else if (has) p.tgt_logit[row] = tl;
         }
       } else if (MODE == MODE_GENERIC || MODE == MODE_DLOGIT) {
         // 16 output columns at a time through the warp's staging array; C leaves (and, for beta != 0, enters)
@@ -636,6 +665,20 @@ bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t ld
   p.nparts = vocab_lse_nparts(N);
   CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);
   launch<128, MODE_LSE>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128));
+  return true;
+}
+// Vocabulary projection with the sampling step fused into the epilogue: vocab_lse_tc's part_max / part_sum plus, per column
+// slice, the best Gumbel key, its class and its logit (M, nparts each).  vocab_sample_finish reduces them.
+bool vocab_sample_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
+                     const SampleCfg& smp, float* part_max, float* part_sum, float* part_key, int32_t* part_cls, float* part_x) {
+  using namespace tc;
+  if (!vocab_tc_ok(M, N, K, A, lda, B, ldb)) return false;
+  Params p = {};
+  p.M = M; p.N = N; p.K = K; p.bias = bias; p.part_max = part_max; p.part_sum = part_sum;
+  p.part_key = part_key; p.part_cls = part_cls; p.part_x = part_x; p.smp = smp;
+  p.nparts = vocab_lse_nparts(N);
+  CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);
+  launch<128, MODE_SAMPLE>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128));
   return true;
 }
 // C[m,n] = keep[m] * (exp(A B^T + bias - lse[m]) - [n == tgt[m]-1])   (backward of log-softmax + ClassNLL, recomputed)

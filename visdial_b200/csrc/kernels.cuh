@@ -31,6 +31,14 @@ bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_
 // lse[r] from the partials; then  out[r] (+)= keep ? sign * (tgt_logit[r] - lse[r]) : 0   (keep: row id != 0 and target > 0)
 void vocab_lse_finish(LaunchCtx& cx, const float* part_max, const float* part_sum, int nparts, const float* tgt_logit,
                       const int32_t* tgt, const int32_t* row_ids, float* lse, float* out, float sign, int accumulate, int64_t rows);
+// sampling (Engine::gen_sample, rule in common.cuh): the projection with the Gumbel-max draw in its epilogue (same shapes as
+// vocab_lse_tc), then the reduction of the slices — lse as vocab_lse_finish forms it, the winner by (key desc, class asc) —
+// which writes what every sampling route writes for step smp.step (1-based): tokens[r] = class + 1 (the next step's
+// input), answer[r * (L + 1) + step] = the same, logp[r * L + step - 1] = x_tok - lse (logp may be null)
+bool vocab_sample_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
+                     const SampleCfg& smp, float* part_max, float* part_sum, float* part_key, int32_t* part_cls, float* part_x);
+void vocab_sample_finish(LaunchCtx& cx, const float* part_max, const float* part_sum, const float* part_key, const int32_t* part_cls,
+                         const float* part_x, int nparts, int64_t rows, int step, int L, int32_t* tokens, int32_t* answer, float* logp);
 
 // ---- ids / embedding ---------------------------------------------------------------------------
 // (rows,T) batch-major -> (T,rows) time-major: the `view(-1,T):t()` of model.lua:256,276,308.
@@ -134,6 +142,10 @@ void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* bea
 void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int L, int end_token, const float* topv, const int32_t* topi,
                 const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out, int32_t* tokens,
                 int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score);
+// the sampling step from materialised logits, one block per row: lse from the same row_lse as logsoftmax_rows (so logp is
+// the bits it would give), the Gumbel-max draw of common.cuh; writes as vocab_sample_finish
+void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,
+                            int32_t* answer, float* logp);
 
 // ---- optimiser (model.lua:96-99, optim_updates.lua:62-91) ------------------------------------------
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1,

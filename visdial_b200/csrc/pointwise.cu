@@ -256,24 +256,47 @@ __global__ void k_beam_gather(float* __restrict__ dst, const float* __restrict__
   dst[i] = p >= 0 ? out_prev[(int64_t)p * H + c] : in_prev[(int64_t)(-1 - p) * H + c];
 }
 
-// row log-sum-exp from the per-slice partials of the fused vocabulary projection, then the criterion / likelihood term
+// row log-sum-exp from the per-slice (max, sum exp) partials of the fused vocabulary projection
+__device__ __forceinline__ float parts_lse(const float* m, const float* s, int nparts) {
+  float mx = -INFINITY;
+  for (int i = 0; i < nparts; ++i) mx = fmaxf(mx, m[i]);
+  float sum = 0.f;
+  for (int i = 0; i < nparts; ++i) sum += s[i] * expf(m[i] - mx);
+  return mx + logf(sum);
+}
+
+// row log-sum-exp from the partials, then the criterion / likelihood term
 __global__ void k_vocab_lse_finish(const float* __restrict__ pm, const float* __restrict__ ps, int nparts,
                                    const float* __restrict__ tl, const int32_t* __restrict__ tgt, const int32_t* __restrict__ ids,
                                    float* __restrict__ lse, float* __restrict__ out, float sign, int accumulate, int64_t rows) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= rows) return;
-  const float* m = pm + r * nparts; const float* s = ps + r * nparts;
-  float mx = -INFINITY;
-  for (int i = 0; i < nparts; ++i) mx = fmaxf(mx, m[i]);
-  float sum = 0.f;
-  for (int i = 0; i < nparts; ++i) sum += s[i] * expf(m[i] - mx);
-  const float l = mx + logf(sum);
+  const float l = parts_lse(pm + r * nparts, ps + r * nparts, nparts);
   if (lse) lse[r] = l;
   if (out) {
     const bool keep = ids[r] != 0 && tgt[r] > 0;
     const float v = keep ? sign * (tl[r] - l) : 0.f;
     out[r] = accumulate ? out[r] + v : v;
   }
+}
+
+// the sampling step's reduction over the slices of MODE_SAMPLE (thread per row): lse as k_vocab_lse_finish forms it, the
+// winning slice by (key desc, class asc), then the token, the answer column and x_tok - lse
+__global__ void k_vocab_sample_finish(const float* __restrict__ pm, const float* __restrict__ ps, const float* __restrict__ pk,
+                                      const int32_t* __restrict__ pc, const float* __restrict__ px, int nparts, int64_t rows,
+                                      int step, int L, int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
+                                      float* __restrict__ logp) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  const int64_t o = r * nparts;
+  const float l = parts_lse(pm + o, ps + o, nparts);
+  float bk = pk[o], bx = px[o];
+  int bc = pc[o];
+  for (int i = 1; i < nparts; ++i)
+    if (sample_before(pk[o + i], pc[o + i], bk, bc)) { bk = pk[o + i]; bc = pc[o + i]; bx = px[o + i]; }
+  tokens[r] = bc + 1;
+  answer[r * (L + 1) + step] = bc + 1;
+  if (logp) logp[r * L + step - 1] = bx - l;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -945,6 +968,60 @@ __global__ void __launch_bounds__(256) k_logsoftmax_topk_rows(const float* __res
   }
 }
 
+// The sampling step from materialised logits, one block per row.  The lse comes from row_lse, so x_tok - lse is the
+// log-probability k_logsoftmax_rows would write.  Each thread takes Philox quadruples (4 consecutive element indices, one
+// call) strided over the row, keeps its best (key, class), and the block reduces them with the same order.
+__global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __restrict__ x, int V, SampleCfg smp, int L,
+                                                                int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
+                                                                float* __restrict__ logp) {
+  __shared__ float red[33];
+  __shared__ float sk[8];
+  __shared__ int sc[8];
+  const int64_t r = blockIdx.x;
+  const float* row = x + r * V;
+  const float lse = row_lse(row, V, red);
+  const uint64_t base = (uint64_t)(smp.row_offset + r) * (uint64_t)V;
+  const uint64_t q0 = base >> 2, q1 = (base + V - 1) >> 2;
+  float bk = -INFINITY;
+  int bc = 0x7fffffff;
+  for (uint64_t q = q0 + threadIdx.x; q <= q1; q += blockDim.x) {
+    const int64_t j0 = (int64_t)(q * 4 - base);                 // class of word 0 (< 0 or >= V outside the row)
+    float y[4];
+    float ymax = -INFINITY;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int64_t j = j0 + e;
+      y[e] = (j >= 0 && j < V) ? row[j] / smp.temperature : -INFINITY;
+      ymax = fmaxf(ymax, y[e]);
+    }
+    if (ymax + GUMBEL_MAX < bk) continue;                        // no key of the quadruple can reach the best one
+    uint32_t o[4];
+    sample_words(smp, q, o);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int64_t j = j0 + e;
+      if (j < 0 || j >= V) continue;
+      const float key = y[e] + gumbel_of_word(o[e]);
+      if (sample_before(key, (int)j, bk, bc)) { bk = key; bc = (int)j; }
+    }
+  }
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) {
+    const float ok = __shfl_xor_sync(FULL, bk, off);
+    const int oc = __shfl_xor_sync(FULL, bc, off);
+    if (sample_before(ok, oc, bk, bc)) { bk = ok; bc = oc; }
+  }
+  if ((threadIdx.x & 31) == 0) { sk[threadIdx.x >> 5] = bk; sc[threadIdx.x >> 5] = bc; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+      if (sample_before(sk[w], sc[w], bk, bc)) { bk = sk[w]; bc = sc[w]; }
+    tokens[r] = bc + 1;
+    answer[r * (L + 1) + smp.step] = bc + 1;
+    if (logp) logp[r * L + smp.step - 1] = row[bc] - lse;
+  }
+}
+
 // The candidate merge of one beam-search step (model.lua:529-569 as model.py restates it), one warp per round n.  Row
 // n*k + w is hypothesis (column) w of round n; candidate q = w*k + j is the j-th best class of row n*k + w, scored
 // scores[w] + topv in fp64.  At step 1 only column 0 is explored.  Candidates whose token is end_token compete for the
@@ -1385,6 +1462,16 @@ void lhood_accumulate(LaunchCtx& cx, const float* logits, const int32_t* tgt, co
 void vocab_lse_finish(LaunchCtx& cx, const float* part_max, const float* part_sum, int nparts, const float* tgt_logit,
                       const int32_t* tgt, const int32_t* row_ids, float* lse, float* out, float sign, int accumulate, int64_t rows) {
   L1D(k_vocab_lse_finish, rows, part_max, part_sum, nparts, tgt_logit, tgt, row_ids, lse, out, sign, accumulate, rows);
+}
+void vocab_sample_finish(LaunchCtx& cx, const float* part_max, const float* part_sum, const float* part_key, const int32_t* part_cls,
+                         const float* part_x, int nparts, int64_t rows, int step, int L, int32_t* tokens, int32_t* answer, float* logp) {
+  L1D(k_vocab_sample_finish, rows, part_max, part_sum, part_key, part_cls, part_x, nparts, rows, step, L, tokens, answer, logp);
+}
+void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,
+                            int32_t* answer, float* logp) {
+  if (rows <= 0) return;
+  k_logsoftmax_sample_rows<<<(unsigned)rows, 256, 0, cx.stream>>>(logits, V, smp, L, tokens, answer, logp);
+  check_launch(cx, "k_logsoftmax_sample_rows");
 }
 void topk_rows(LaunchCtx& cx, const float* x, int64_t rows, int V, int k, float* topv, int32_t* topi) {
   VD_REQUIRE(k >= 1 && k <= V, VD_E_BADARG, "topk_rows: k");

@@ -378,6 +378,19 @@ class Engine:
                                           score.ctypes.data))
         return ans, length, score
 
+    def gen_sample(self, L: int, start: int, temperature: float, seed: int, row_offset: int = 0):
+        """Ancestral sampling for every round of the last encoder forward on the device (vd_gen_sample).  Returns (answer
+        (N, L+1) int32 — column 0 = `start` — and logp (N, L) float32, each sample's un-tempered log-probability).  Row r's
+        draws depend only on (seed, row_offset + r, step): pass the global index of the call's first round."""
+        N = self._enc_rows
+        if N is None:
+            raise _lib.VdError(_lib.VD_E_STATE, "gen_sample before encoder_forward")
+        ans = np.zeros((N, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((N, int(L)), dtype=np.float32)
+        check(self.lib.vd_gen_sample(self.h, int(L), int(start), float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                     int(row_offset), ans.ctypes.data, logp.ctypes.data))
+        return ans, logp
+
     def upload(self, dev_ptr: int, a: np.ndarray):
         a = np.ascontiguousarray(a, dtype=np.float32)
         check(self.lib.vd_memcpy_h2d(self.h, C.c_void_p(dev_ptr), a.ctypes.data, a.nbytes))

@@ -1,8 +1,8 @@
 """Mirror of the reference's `Model` class (/root/reference/model.lua:8-430) over the C engine.
 Same method names, argument meaning and call order as the Lua original, so that the parity tests
 read like the reference's own driver code.  `generateAnswers` (beam search / sampling, model.lua:432-613) runs the beam
-search entirely on the device (vd_gen_beam_search); sampling and the reference-structured beam loop step the decoder through
-vd_gen_decoder_step and keep the hypothesis bookkeeping on the host like the Lua."""
+search and the sampling entirely on the device (vd_gen_beam_search, vd_gen_sample); the reference-structured beam loop steps
+the decoder through vd_gen_decoder_step and keeps the hypothesis bookkeeping on the host like the Lua."""
 from __future__ import annotations
 
 import numpy as np
@@ -26,6 +26,17 @@ def _image_id(x):
     import re
     mt = re.search(r"000\d+", str(x))
     return int(mt.group(0)) if mt else x
+
+
+def _question_width(dataloader, dtype, inds, convId, Tq, ques_len):
+    """The `question` columns of dialog convId in a batch of the dialogs `inds` (padded to Tq): a one-dialog batch keeps
+    the rightmost (its longest question) columns (dataloader.lua:380-384), so a wider batch keeps that many too.  Returns
+    (width, the split's ques_length array, loaded at the first multi-dialog batch)."""
+    if len(inds) == 1:
+        return Tq, ques_len
+    if ques_len is None:
+        ques_len = dataloader.corpus[dtype].raw["ques_length"]
+    return int(ques_len[dataloader.part[dtype][0] + convId].max()), ques_len
 
 
 def _num_tokens(batch) -> int:
@@ -180,12 +191,13 @@ class Model:
 
     # ---- beam search / sampling (model.lua:432-613, generate.lua) ---------------------------------------------
     def generateAnswers(self, dataloader, dtype="val", params=None, strict=True):
-        """Model:generateAnswers.  Beam search (the default) runs entirely on the device through vd_gen_beam_search, for
-        `params.dialogsPerCall` dialogs (default 1) per encoder forward: every round of those dialogs is searched at once.
-        `hostBeam = 1` (the reference's loop structure) and sampling go one dialog at a time, the decoder stepped through
-        vd_gen_decoder_step and the hypothesis bookkeeping on the host as the Lua does it.  Returns the reference's
-        answerTable with token-id lists (and text when the dataloader carries ind2word).  `strict=False` yields None for a
-        round where no beam reached <END> (the reference indexes nil there, model.lua:575)."""
+        """Model:generateAnswers.  Beam search (the default) and sampling (`sampleWords = 1`) run entirely on the device
+        through vd_gen_beam_search / vd_gen_sample, for `params.dialogsPerCall` dialogs (default 1) per encoder forward:
+        every round of those dialogs is searched or sampled at once.  `hostBeam = 1` (the reference's loop structure) goes
+        one dialog at a time, the decoder stepped through vd_gen_decoder_step and the hypothesis bookkeeping on the host as
+        the Lua does it.  Returns the reference's answerTable with token-id lists (and text when the dataloader carries
+        ind2word).  `strict=False` yields None for a round where no beam reached <END> (the reference indexes nil there,
+        model.lua:575)."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
@@ -195,7 +207,6 @@ class Model:
         startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
         numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
         ind2word = getattr(dataloader, "ind2word", None)
-        rng = np.random.default_rng(int(params.get("seed", 1234)))
         eng, H = self.engine, self.params["rnnHiddenSize"]
         words = (lambda ids: " ".join(ind2word.get(int(t), "<UNK>") for t in ids if int(t) > 0)) if ind2word else None
         img = getattr(dataloader, "unique_img_" + dtype, None)
@@ -212,9 +223,13 @@ class Model:
                 e["question_text"], e["answer_text"] = words(q), words(answer)
             return e
 
-        if not sampleWords and not params.get("hostBeam"):
-            return self._generate_beam(dataloader, dtype, numThreads, max(1, int(params.get("dialogsPerCall", 1))), beamSize,
-                                       beamLen, startToken, endToken, strict, image_id, entry)
+        dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
+        if sampleWords:
+            return self._generate_sample(dataloader, dtype, numThreads, dialogsPerCall, beamLen, startToken, temperature,
+                                         int(params.get("seed", 1234)), first, image_id, words)
+        if not params.get("hostBeam"):
+            return self._generate_beam(dataloader, dtype, numThreads, dialogsPerCall, beamSize, beamLen, startToken, endToken,
+                                       strict, image_id, entry)
         state_buf = [eng.device_alloc(max(beamSize, self.params["maxQuesCount"]) * H * 4) for _ in range(4)]
         answerTable = []
         try:
@@ -235,71 +250,51 @@ class Model:
                         eng.upload(state_buf[i], a[:n])
                     return eng.gen_decoder_step(tokens, state_buf[0:2], state_buf[2:4])
 
-                if not sampleWords:
-                    # the reference's own loop structure (one round at a time, log-probabilities and state through the host):
-                    # kept as the cross-check of the device search (params.hostBeam = 1)
-                    for it in range(N):                                                 # :472
-                        beams = np.zeros((beamLen, beamSize), dtype=np.int64)           # :479
-                        if has_layers:                                                  # :482-491
-                            Hs = [encH[0][0][it], encOut[it]]
-                            Cs = [encH[0][1][it], encH[1][1][it]]
-                        else:                                                           # :493-501
-                            Hs = [np.zeros(H, np.float32), encOut[it]]
-                            Cs = [np.zeros(H, np.float32), np.zeros(H, np.float32)]
-                        Hs = [np.repeat(h[None], beamSize, 0).astype(np.float32) for h in Hs]
-                        Cs = [np.repeat(c[None], beamSize, 0).astype(np.float32) for c in Cs]
-                        beams[0] = startToken                                           # :506
-                        scores = np.zeros(beamSize, dtype=np.float64)                   # :507
-                        finishBeams = []
-                        for stp in range(1, beamLen):                                   # :510
-                            cands = []
-                            exploreSize = 1 if stp == 1 else beamSize                   # :516
-                            decOut, nH, nC = step(beams[stp - 1], Hs, Cs)               # :519-526
-                            for wordId in range(exploreSize):                           # :529
-                                order = np.argsort(-decOut[wordId], kind="stable")[:beamSize]   # :538-542 topk, sorted
-                                for candId in range(beamSize):                          # :544
-                                    candBeam = beams[:, wordId].copy()
-                                    tok = int(order[candId]) + 1
-                                    candBeam[stp] = tok
-                                    sc = float(scores[wordId]) + float(decOut[wordId, order[candId]])
-                                    if tok == endToken:                                 # :548
-                                        finishBeams.append({"beam": candBeam, "length": stp + 1, "score": sc})
-                                    else:
-                                        cands.append((sc, candBeam, [h[wordId].copy() for h in nH], [c[wordId].copy() for c in nC]))
-                            cands.sort(key=lambda t: -t[0])                             # :558
-                            for candId in range(min(len(cands), beamSize)):             # :560-569
-                                beams[:, candId] = cands[candId][1]
-                                for lv in range(2):
-                                    Hs[lv][candId] = cands[candId][2][lv]
-                                    Cs[lv][candId] = cands[candId][3][lv]
-                                scores[candId] = cands[candId][0]
-                        finishBeams.sort(key=lambda d: -d["score"])                     # :572
-                        if not finishBeams:
-                            if strict:
-                                raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
-                            threadAnswers.append(None)
-                            continue
-                        best = finishBeams[0]
-                        threadAnswers.append(entry(ques[it], best["beam"], best["score"], best["length"]))
-                else:                                                                   # :581-602
-                    if has_layers:                                                      # forwardConnect, gen.lua:30-42
-                        Hs, Cs = [encH[0][0], encOut], [encH[0][1], encH[1][1]]
-                    else:
-                        Hs, Cs = [np.zeros((N, H), np.float32), encOut], [np.zeros((N, H), np.float32)] * 2
-                    tok = np.full(N, startToken, dtype=np.int64)
-                    seq = [tok.copy()]
-                    for _ in range(beamLen):
-                        decOut, Hs, Cs = step(tok, Hs, Cs)                              # :586-588 (+ decoderConnect)
-                        p = np.exp(decOut.astype(np.float64) / temperature)             # :590
-                        p /= p.sum(1, keepdims=True)
-                        tok = np.array([rng.choice(p.shape[1], p=p[i]) + 1 for i in range(N)], dtype=np.int64)
-                        seq.append(tok.copy())
-                    ans = np.stack(seq, 1)
-                    for it in range(N):
-                        e = {"question": ques[it].tolist(), "answer": ans[it].tolist()}
-                        if words:
-                            e["question_text"], e["answer_text"] = words(ques[it]), words(ans[it])
-                        threadAnswers.append(e)
+                # the reference's own loop structure (one round at a time, log-probabilities and state through the host):
+                # kept as the cross-check of the device search (params.hostBeam = 1)
+                for it in range(N):                                                 # :472
+                    beams = np.zeros((beamLen, beamSize), dtype=np.int64)           # :479
+                    if has_layers:                                                  # :482-491
+                        Hs = [encH[0][0][it], encOut[it]]
+                        Cs = [encH[0][1][it], encH[1][1][it]]
+                    else:                                                           # :493-501
+                        Hs = [np.zeros(H, np.float32), encOut[it]]
+                        Cs = [np.zeros(H, np.float32), np.zeros(H, np.float32)]
+                    Hs = [np.repeat(h[None], beamSize, 0).astype(np.float32) for h in Hs]
+                    Cs = [np.repeat(c[None], beamSize, 0).astype(np.float32) for c in Cs]
+                    beams[0] = startToken                                           # :506
+                    scores = np.zeros(beamSize, dtype=np.float64)                   # :507
+                    finishBeams = []
+                    for stp in range(1, beamLen):                                   # :510
+                        cands = []
+                        exploreSize = 1 if stp == 1 else beamSize                   # :516
+                        decOut, nH, nC = step(beams[stp - 1], Hs, Cs)               # :519-526
+                        for wordId in range(exploreSize):                           # :529
+                            order = np.argsort(-decOut[wordId], kind="stable")[:beamSize]   # :538-542 topk, sorted
+                            for candId in range(beamSize):                          # :544
+                                candBeam = beams[:, wordId].copy()
+                                tok = int(order[candId]) + 1
+                                candBeam[stp] = tok
+                                sc = float(scores[wordId]) + float(decOut[wordId, order[candId]])
+                                if tok == endToken:                                 # :548
+                                    finishBeams.append({"beam": candBeam, "length": stp + 1, "score": sc})
+                                else:
+                                    cands.append((sc, candBeam, [h[wordId].copy() for h in nH], [c[wordId].copy() for c in nC]))
+                        cands.sort(key=lambda t: -t[0])                             # :558
+                        for candId in range(min(len(cands), beamSize)):             # :560-569
+                            beams[:, candId] = cands[candId][1]
+                            for lv in range(2):
+                                Hs[lv][candId] = cands[candId][2][lv]
+                                Cs[lv][candId] = cands[candId][3][lv]
+                            scores[candId] = cands[candId][0]
+                    finishBeams.sort(key=lambda d: -d["score"])                     # :572
+                    if not finishBeams:
+                        if strict:
+                            raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
+                        threadAnswers.append(None)
+                        continue
+                    best = finishBeams[0]
+                    threadAnswers.append(entry(ques[it], best["beam"], best["score"], best["length"]))
                 self.wrapper.training()                                                 # :605
                 answerTable.append({"image_id": image_id(convId), "dialog": threadAnswers})   # :606
         finally:
@@ -326,13 +321,7 @@ class Model:
             length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
             self.wrapper.training()                                                     # :605
             for d, convId in enumerate(inds):
-                # a one-dialog batch keeps the rightmost (its longest question) columns (dataloader.lua:380-384)
-                if len(inds) == 1:
-                    w = Tq
-                else:
-                    if ques_len is None:
-                        ques_len = dataloader.corpus[dtype].raw["ques_length"]
-                    w = int(ques_len[dataloader.part[dtype][0] + convId].max())
+                w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
                 threadAnswers = []
                 for it in range(ques.shape[1]):
                     if length[d, it] == 0:
@@ -341,6 +330,37 @@ class Model:
                         threadAnswers.append(None)
                         continue
                     threadAnswers.append(entry(ques[d, it, Tq - w:], answer[d, it], float(score[d, it]), int(length[d, it])))
+                answerTable.append({"image_id": image_id(int(convId)), "dialog": threadAnswers})   # :606
+        return answerTable
+
+    def _generate_sample(self, dataloader, dtype, numThreads, dialogsPerCall, beamLen, startToken, temperature, seed,
+                         split_offset, image_id, words):
+        """generateAnswers' sampling (model.lua:581-602), `dialogsPerCall` dialogs per encoder forward and per vd_gen_sample
+        call.  The draws of a round depend only on (seed, its global round index, the step): the call passes the index of
+        its first round in the split (this rank's offset included), so the answers do not depend on dialogsPerCall or on
+        how the split is sharded over ranks, only on the logits."""
+        R = self.params["maxQuesCount"]
+        answerTable = []
+        ques_len = None
+        for first in range(0, numThreads, dialogsPerCall):
+            inds = np.arange(first, min(numThreads, first + dialogsPerCall))
+            self.wrapper.evaluate()                                                     # :460
+            batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
+            self.forwardBackward(batch, True, True)                                     # :467
+            ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
+            Tq = ques.shape[2]
+            answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, (split_offset + first) * R)   # :582-594
+            answer = answer.reshape(len(inds), -1, beamLen + 1)
+            self.wrapper.training()                                                     # :605
+            for d, convId in enumerate(inds):
+                w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
+                threadAnswers = []
+                for it in range(ques.shape[1]):
+                    q, a = ques[d, it, Tq - w:], answer[d, it]
+                    e = {"question": q.tolist(), "answer": a.tolist()}
+                    if words:
+                        e["question_text"], e["answer_text"] = words(q), words(a)
+                    threadAnswers.append(e)
                 answerTable.append({"image_id": image_id(int(convId)), "dialog": threadAnswers})   # :606
         return answerTable
 
