@@ -214,6 +214,8 @@ class Dataloader:
             self.corpus[dtype] = c
             self.part[dtype] = eval_partition(c.numThreads, self.rank, self.world) if dtype != "train" else (0, c.numThreads)
             self.numThreads[dtype] = self.part[dtype][1] - self.part[dtype][0]      # :94-105 (this rank's share)
+            if c.num_rounds is not None:                                            # :110, read by Model.retrieve / predict
+                setattr(self, dtype + "_num_rounds", c.num_rounds)
             self.maxQuesCount = c.R                                                 # :122
             self.numOptions = c.K                                                   # :112
             self.maxQuesLen = int(c.desc.maxQuesLen)                                # :124
@@ -238,19 +240,30 @@ class Dataloader:
         for k, v in info.items():
             setattr(self, k, v)
         n_words = len(info["word2ind"])                                             # :17-22
-        ques = h5lite.read(opt["inputQues"])                                        # :33-34
-        imgs = h5lite.read(opt["inputImg"]) if opt.get("useIm") else {}             # :36-37
+        ques = h5lite.read(opt["inputQues"])                                        # :33-34 (memory-mapped)
         data = {}
         for dtype in subsets:
             d = h5lite.split(ques, dtype)                                           # :45-57,108-129
             if not d:
                 raise ValueError("no '%s' datasets in %s" % (dtype, opt["inputQues"]))
-            if opt.get("useIm"):
-                if "images_" + dtype not in imgs:
-                    raise ValueError("no 'images_%s' in %s" % (dtype, opt["inputImg"]))
-                d["images"] = imgs["images_" + dtype]                               # :61
+            if opt.get("useIm"):                                                    # :36-37,61: only the asked splits
+                try:
+                    d["images"] = h5lite.read(opt["inputImg"], ["images_" + dtype])["images_" + dtype]
+                except h5lite.H5Error as e:
+                    raise ValueError("no 'images_%s' in %s (%s)" % (dtype, opt["inputImg"], e))
             data[dtype] = d
         return self.initialize(dict(opt, vocabSize=n_words + 2), subsets, data, vocab_size_no_specials=n_words)
+
+    def restrict(self, dtype: str, n: int):
+        """Keep the first `n` dialogs of evaluation split `dtype` and re-partition that prefix over the ranks (generate.lua's
+        maxThreads on several GPUs).  Dialog indices stay global, so rank r's share of the prefix is the dialogs a 1-GPU run
+        generates at those positions, with the same sampling row offsets."""
+        lo, hi = eval_partition(min(int(n), self.corpus[dtype].numThreads), self.rank, self.world)
+        self.part[dtype] = (lo, hi)
+        self.numThreads[dtype] = hi - lo
+        if dtype in ("val", "test"):
+            setattr(self, "num%sThreads" % dtype.capitalize(), hi - lo)
+        return self
 
     def getTrainBatch(self, params: dict, batchSize: int = None) -> DeviceBatch:
         size = int(batchSize or params["batchSize"])                                # :325

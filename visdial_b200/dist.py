@@ -49,6 +49,24 @@ def gather_ranks(local: np.ndarray, rank: int, world: int) -> Optional[np.ndarra
     return np.concatenate(objs, 0)
 
 
+def gather_objects(local: list, world: int) -> list:
+    """Rank-ordered concatenation of every rank's list (evaluation tables, generated dialogs)."""
+    import torch.distributed as dist
+    objs = [None] * world
+    dist.all_gather_object(objs, local)
+    return [x for part in objs for x in part]
+
+
+def mean_over_ranks(value: float, world: int) -> float:
+    import torch
+    import torch.distributed as dist
+    t = torch.tensor([value], dtype=torch.float64)
+    if dist.get_backend() == "nccl":
+        t = t.cuda()
+    dist.all_reduce(t, op=dist.ReduceOp.SUM)
+    return float(t.item()) / world
+
+
 def max_over_ranks(value: float) -> float:
     import torch
     import torch.distributed as dist

@@ -17,6 +17,7 @@ against `write()` round trips.  Reading a real `visdial_data.h5` has not been po
 """
 from __future__ import annotations
 
+import mmap
 import struct
 import zlib
 from typing import Dict, List, Optional, Tuple
@@ -33,8 +34,11 @@ class H5Error(ValueError):
 
 # ====================================================================================================== reader
 class _Reader:
-    def __init__(self, buf: bytes):
+    def __init__(self, buf, path: Optional[str] = None):
+        """`buf`: the file's bytes (bytes or a read-only mmap).  With `path`, contiguous uncompressed native-order datasets
+        come back as read-only np.memmap views of the file instead of copies."""
         self.b = buf
+        self.path = path
         base = 0
         while base < len(buf) and buf[base:base + 8] != SIG:      # the superblock may sit at 0, 512, 1024, ...
             base = 512 if base == 0 else base * 2
@@ -62,7 +66,9 @@ class _Reader:
         return self.u64(p), self.u64(p + 8)
 
     def _cstr(self, p) -> str:
-        e = self.b.index(b"\x00", p)
+        e = self.b.find(b"\x00", p)
+        if e < 0:
+            raise H5Error("unterminated name in the local heap")
         return self.b[p:e].decode("utf-8")
 
     # ---- object headers
@@ -191,7 +197,7 @@ class _Reader:
                 addr, size = self.u64(d + 2), self.u64(d + 10)
                 if addr == UNDEF:
                     return np.zeros(shape, dt.newbyteorder("="))
-                raw = self.b[addr + self.base_addr: addr + self.base_addr + n * dt.itemsize]
+                return self._contiguous(addr, shape, dt, n)
             elif cls == 0:                                         # compact
                 size = self.u16(d + 2)
                 raw = self.b[d + 4: d + 4 + size]
@@ -207,13 +213,27 @@ class _Reader:
             rank, cls = self.u8(d + 1), self.u8(d + 2)
             if cls != 1:
                 raise H5Error("layout version %d: only contiguous storage is supported" % ver)
-            addr = self.u64(d + 8)
-            raw = self.b[addr + self.base_addr: addr + self.base_addr + n * dt.itemsize]
+            return self._contiguous(self.u64(d + 8), shape, dt, n)
         else:
             raise H5Error("data layout version %d is not supported" % ver)
+        return self._decode(raw, shape, dt, n)
+
+    @staticmethod
+    def _decode(raw, shape, dt: np.dtype, n: int) -> np.ndarray:
         if len(raw) < n * dt.itemsize:
             raise H5Error("dataset data truncated")
         return np.frombuffer(raw, dtype=dt, count=n).reshape(shape).astype(dt.newbyteorder("="))
+
+    def _contiguous(self, addr: int, shape, dt: np.dtype, n: int) -> np.ndarray:
+        """A contiguous dataset: a read-only memmap at its data offset when it is already in native byte order (no host
+        copy of a multi-GB feature file), else a decoded copy."""
+        start = addr + self.base_addr
+        native = dt == dt.newbyteorder("=")
+        if self.path is None or not native or not shape or n == 0:
+            return self._decode(self.b[start:start + n * dt.itemsize], shape, dt, n)
+        if start + n * dt.itemsize > len(self.b):
+            raise H5Error("dataset data truncated")
+        return np.memmap(self.path, dtype=dt.newbyteorder("="), mode="r", offset=start, shape=tuple(shape))
 
     def _chunked(self, btree: int, shape, dt: np.dtype, cdims: List[int], filters) -> np.ndarray:
         if btree == UNDEF:
@@ -257,16 +277,22 @@ class _Reader:
 
 def read(path: str, names: Optional[List[str]] = None) -> Dict[str, np.ndarray]:
     """All (or the named) datasets of an HDF5 file as native-endian numpy arrays: the `file:read(name):all()` of
-    dataloader.lua:45-129."""
+    dataloader.lua:45-129.  Contiguous, uncompressed, native-byte-order datasets are read-only np.memmap views of the file
+    (pages are read when touched); chunked, filtered, compact and byte-swapped ones are decoded into new arrays."""
     with open(path, "rb") as f:
-        r = _Reader(f.read())
-    table = r.walk()
-    if names is not None:
-        missing = [n for n in names if n.lstrip("/") not in table]
-        if missing:
-            raise H5Error("datasets not in file: %s" % ", ".join(missing))
-        table = {n.lstrip("/"): table[n.lstrip("/")] for n in names}
-    return {k: r.read(v) for k, v in table.items()}
+        try:
+            buf = mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ)
+        except ValueError:                                         # an empty file cannot be mapped
+            raise H5Error("not an HDF5 file (empty)")
+    with buf:
+        r = _Reader(buf, path)
+        table = r.walk()
+        if names is not None:
+            missing = [n for n in names if n.lstrip("/") not in table]
+            if missing:
+                raise H5Error("datasets not in file: %s" % ", ".join(missing))
+            table = {n.lstrip("/"): table[n.lstrip("/")] for n in names}
+        return {k: r.read(v) for k, v in table.items()}
 
 
 def split(datasets: Dict[str, np.ndarray], dtype: str) -> Dict[str, np.ndarray]:

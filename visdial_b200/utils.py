@@ -2,6 +2,21 @@
 import numpy as np
 
 
+def idToWords(vector, ind2word) -> str:
+    """utils.lua:48-63: every non-pad id becomes ' ' + its word (so the text starts with a space); <START> is kept, and
+    the walk stops after the first <END>."""
+    sentence = ""
+    nextWord = None
+    for wordId in vector:
+        wordId = int(wordId)
+        if wordId > 0:
+            nextWord = ind2word[wordId]
+            sentence += " " + nextWord
+        if nextWord == "<END>":
+            break
+    return sentence
+
+
 def processRanks(ranks, verbose=True):
     """utils.lua:131-160: R@1/5/10, median, mean rank, MRR."""
     r = np.asarray(ranks, dtype=np.float64).reshape(-1)
