@@ -141,6 +141,15 @@ int vd_encoder_backward(vd_engine* e, const vd_batch* b, const float* gradEncOut
 
 /* ---- fused fast paths ----------------------------------------------------------------------- */
 int vd_forward_backward(vd_engine* e, const vd_batch* b, int32_t only_forward, float* loss_host);  /* Model:forwardBackward, model.lua:249-342 */
+/* One training step on dense relevance targets (disc decoder only).  b: a disc training batch exactly as for
+ * vd_forward_backward; round_host (B) 0-based annotated round of each dialog; relevance_host (B, numOptions) >= 0 with a
+ * positive sum per row.  loss = mean over the B rows of  lse(s_b) - sum_k p_bk s_bk,  p_b = relevance_b / sum(relevance_b),
+ * s_b = the disc scores of round round_host[b] of dialog b.  Gradients accumulate into dW as vd_forward_backward's do.
+ * The encoder runs over all rounds (same dropout masks as vd_forward_backward); the option LSTM only over the B selected
+ * rounds' options.  VD_E_STATE for a gen engine; VD_E_BADARG for a null pointer, a round outside [0, maxQuesCount) or a
+ * negative, non-finite or zero-sum relevance row. */
+int vd_forward_backward_dense(vd_engine* e, const vd_batch* b, const int32_t* round_host, const float* relevance_host,
+                              float* loss_host);
 /* Model:retrieveBatch (model.lua:344-430).  use_gt != 0: ranks_host is (N) = rank of the ground
  * truth; else (N,100) = rank of every option.  Ranks are 1-based; ties: lower index wins. */
 int vd_retrieve(vd_engine* e, const vd_batch* b, int32_t use_gt, int32_t* ranks_host);

@@ -87,6 +87,7 @@ SIGNATURES = {
     "vd_backward_connect": [_H, _P(C.c_void_p)],
     "vd_encoder_backward": [_H, _P(vd_batch), C.c_void_p],
     "vd_forward_backward": [_H, _P(vd_batch), C.c_int32, _P(C.c_float)],
+    "vd_forward_backward_dense": [_H, _P(vd_batch), C.c_void_p, C.c_void_p, _P(C.c_float)],
     "vd_retrieve": [_H, _P(vd_batch), C.c_int32, C.c_void_p],
     "vd_compute_ranks": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p],
     "vd_gen_option_lhood": [_H, _P(vd_batch), _P(C.c_void_p)],

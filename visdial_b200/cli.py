@@ -43,6 +43,11 @@ TRAIN_OPTIONS = [
     ("backend", "cudnn", "nn|cudnn (accepted, no effect)"),
 ]
 
+# the finetune command: train's options and the dense relevance annotations of the train split
+FINETUNE_OPTIONS = TRAIN_OPTIONS + [
+    ("denseAnnotations", "data/visdial_1.0_train_dense_sample.json", "VisDial v1.0 dense relevance annotations (train split)"),
+]
+
 # evaluate.lua:15-30
 EVALUATE_OPTIONS = [
     ("inputImg", "data/data_img.h5", "h5file path with image feature"),
@@ -130,9 +135,9 @@ def parse(options, argv=None, prog=None) -> dict:
     return opt
 
 
-def train_opts(argv=None, now=None) -> dict:
+def train_opts(argv=None, now=None, options=TRAIN_OPTIONS, prog="python -m visdial_b200.train") -> dict:
     """opts.lua:42-67: parsed options, the time-stamped default savePath and the flags derived from the encoder name."""
-    opt = parse(TRAIN_OPTIONS, argv, "python -m visdial_b200.train")
+    opt = parse(options, argv, prog)
     if opt["savePath"] == "checkpoints/":                                           # :44-52
         t = now or time.localtime()
         opt["savePath"] = "checkpoints/model-%d-%d-%d-%d:%d:%d-%s-%s/" % (

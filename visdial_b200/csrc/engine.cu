@@ -211,6 +211,7 @@ Engine::~Engine() {
   if (opt_stream) cudaStreamSynchronize(opt_stream);
   arena.release();
   for (auto& g : stage) g.release();
+  for (auto& g : dense_buf) g.release();
   if (copy_stream) {
     cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream);
     cudaEventDestroy(ev_img_ready); cudaEventDestroy(ev_copy_fork);
@@ -1156,7 +1157,7 @@ void Engine::forward_connect() {
 // disc.lua:4-20: the option LSTM over all N*100 candidate answers.  Depends only on the batch and the weights, so it
 // is enqueued on opt_stream before the encoder's kernels and meets the encoder output at disc_scores_fwd.
 void Engine::options_forward_async() {
-  const int64_t Ro = db.N * cfg.K;
+  const int64_t Ro = (dense_round ? db.B : db.N) * cfg.K;
   cudaStream_t s = opt_overlap ? opt_stream : main_stream;
   if (opt_overlap) {
     VD_CUDA_CHECK(cudaEventRecord(ev_opt_fork, main_stream));          // batch staged, shadows refreshed
@@ -1168,7 +1169,8 @@ void Engine::options_forward_async() {
   // runs beside the option stream's forward: no reserve
   if (opt_overlap) cx.sm_budget = cx.sm_count - (math_mode == VD_MATH_F16 ? 0 : opt_reserve_sms);
   ids_o = arena.get<int32_t>(Ro * db.To);
-  transpose_ids(cx, db.options, ids_o, Ro, db.To);
+  if (dense_round) transpose_ids_rounds(cx, db.options, dense_round, ids_o, db.B, cfg.R, cfg.K, db.To);
+  else transpose_ids(cx, db.options, ids_o, Ro, db.To);
   opt = make_run(db.To, Ro, cfg.E, cfg.H, seg("opt.lstm.weight"), nullptr, ids_o, nullptr);   // disc.lua:4-5: no maskzero
   lstm_forward(opt, save_acts);
   VD_CUDA_CHECK(cudaEventRecord(ev_opt_done, s));
@@ -1295,31 +1297,7 @@ void Engine::decoder_backward() {
     const int64_t Ro = N * K;
     float* dfeat = arena.get<float>(Ro * H);
     disc_scores_bwd(cx, dscores, opt.h_last(), encOut, dfeat, dEncFromDec, N, K, H);
-    // The option BPTT feeds only opt.lstm's weights and the word embedding: it runs on opt_stream while the caller
-    // goes on to the encoder's backward; join_options_backward() (encoder_backward / any gradient consumer) waits.
-    cudaStream_t prev = cx.stream;
-    if (opt_overlap) {
-      VD_CUDA_CHECK(cudaEventRecord(ev_opt_fork, cx.stream));
-      VD_CUDA_CHECK(cudaStreamWaitEvent(opt_stream, ev_opt_fork, 0));
-      cx.stream = opt_stream;
-      cx.sm_budget = cx.sm_count - opt_reserve_sms;
-    }
-    if (opt.route.table_grad) {
-      // embedding gradient in projected space; written to a private (V+1,E) buffer when overlapped, because the
-      // encoder's embedding gradients accumulate into dW(wordEmbed) with atomics at the same time
-      opt.demb_out = opt_overlap ? (opt_demb = arena.get<float>((int64_t)(cfg.V + 1) * E)) : nullptr;
-      lstm_backward(opt, nullptr, dfeat, nullptr, nullptr, nullptr, nullptr);
-    } else {
-      float* dx = arena.get<float>(Ro * db.To * E);
-      lstm_backward(opt, nullptr, dfeat, nullptr, dx, nullptr, nullptr);
-      embed_scatter_add(cx, dWp(0), dx, E, ids_o, Ro * db.To, E, dropcfg(0.f), 0);   // atomics: safe next to the encoder's
-    }
-    if (opt_overlap) {
-      VD_CUDA_CHECK(cudaEventRecord(ev_opt_done, opt_stream));
-      cx.stream = prev;
-      cx.sm_budget = 0;
-      opt_bwd_pending = true;
-    }
+    options_backward(dfeat);
   } else {
     VD_REQUIRE(dlogits, VD_E_STATE, "decoder_backward before criterion_backward");
     float* do2 = arena.get<float>(N * db.Ta * H);
@@ -1331,6 +1309,95 @@ void Engine::decoder_backward() {
     lstm_backward(dec1, dx2, nullptr, nullptr, dx1, gen_dh0[0], gen_dc0[0]);
     embed_scatter_add(cx, dWp(0), dx1, E, ids_ai, N * db.Ta, E, dropcfg(0.f), 0);
   }
+}
+
+void Engine::options_backward(const float* dfeat) {
+  const int E = cfg.E;
+  // The option BPTT feeds only opt.lstm's weights and the word embedding: it runs on opt_stream while the caller
+  // goes on to the encoder's backward; join_options_backward() (encoder_backward / any gradient consumer) waits.
+  cudaStream_t prev = cx.stream;
+  if (opt_overlap) {
+    VD_CUDA_CHECK(cudaEventRecord(ev_opt_fork, cx.stream));
+    VD_CUDA_CHECK(cudaStreamWaitEvent(opt_stream, ev_opt_fork, 0));
+    cx.stream = opt_stream;
+    cx.sm_budget = cx.sm_count - opt_reserve_sms;
+  }
+  if (opt.route.table_grad) {
+    // embedding gradient in projected space; written to a private (V+1,E) buffer when overlapped, because the
+    // encoder's embedding gradients accumulate into dW(wordEmbed) with atomics at the same time
+    opt.demb_out = opt_overlap ? (opt_demb = arena.get<float>((int64_t)(cfg.V + 1) * E)) : nullptr;
+    lstm_backward(opt, nullptr, dfeat, nullptr, nullptr, nullptr, nullptr);
+  } else {
+    float* dx = arena.get<float>(opt.R * db.To * E);
+    lstm_backward(opt, nullptr, dfeat, nullptr, dx, nullptr, nullptr);
+    embed_scatter_add(cx, dWp(0), dx, E, ids_o, opt.R * db.To, E, dropcfg(0.f), 0);   // atomics: safe next to the encoder's
+  }
+  if (opt_overlap) {
+    VD_CUDA_CHECK(cudaEventRecord(ev_opt_done, opt_stream));
+    cx.stream = prev;
+    cx.sm_budget = 0;
+    opt_bwd_pending = true;
+  }
+}
+
+// vd_forward_backward_dense: the encoder over all N rounds as in vd_forward_backward (same dropout sites and masks), the
+// disc decoder on the one annotated round per dialog only (B*K option rows instead of N*K), the soft-target cross-entropy
+// against the relevance rows, and the encoder backward from a dEnc that is zero on every unselected round.
+float Engine::forward_backward_dense(const vd_batch* b, const int32_t* round_host, const float* relevance_host) {
+  VD_REQUIRE(cfg.dec == DEC_DISC, VD_E_STATE, "dense fine-tuning runs the disc decoder only");
+  VD_REQUIRE(b && round_host && relevance_host, VD_E_BADARG, "batch / rounds / relevance is null");
+  VD_REQUIRE(b->B > 0, VD_E_SHAPE, "batch B must be > 0");
+  const int B = b->B, R = cfg.R, K = cfg.K, H = cfg.H;
+  for (int i = 0; i < B; ++i) {
+    VD_REQUIRE(round_host[i] >= 0 && round_host[i] < R, VD_E_BADARG, "round outside [0, maxQuesCount)");
+    double sum = 0.0;
+    for (int k = 0; k < K; ++k) {
+      const float r = relevance_host[(int64_t)i * K + k];
+      VD_REQUIRE(std::isfinite(r) && r >= 0.f, VD_E_BADARG, "relevance must be finite and >= 0");
+      sum += r;
+    }
+    VD_REQUIRE(sum > 0.0, VD_E_BADARG, "a relevance row sums to 0");
+  }
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  if (opt_fwd_pending || opt_bwd_pending) {       // as encoder_forward: nothing of an abandoned call may still read these
+    VD_CUDA_CHECK(cudaStreamSynchronize(opt_stream));
+    opt_fwd_pending = opt_bwd_pending = false;
+  }
+  int32_t* rd = static_cast<int32_t*>(dense_buf[0].ensure((size_t)B * sizeof(int32_t)));
+  float* rel = static_cast<float*>(dense_buf[1].ensure((size_t)B * K * sizeof(float)));
+  VD_CUDA_CHECK(cudaMemcpyAsync(rd, round_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, main_stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(rel, relevance_host, (size_t)B * K * sizeof(float), cudaMemcpyHostToDevice, main_stream));
+  struct Reset { const int32_t*& p; ~Reset() { p = nullptr; } } reset{dense_round};
+  dense_round = rd;
+  encoder_forward(b);                             // starts the option LSTM on the selected rows (options_forward_async)
+  VD_REQUIRE(db.options && db.To > 0, VD_E_SHAPE, "disc decoder: options / To missing");
+  VD_REQUIRE(save_acts, VD_E_STATE, "the dense step needs a training-mode forward");
+  if (world > 1)
+    for (char c : seg_reduced)
+      VD_REQUIRE(!c, VD_E_STATE, "world > 1: vd_zero_grad is required between backward passes (gradients already all-reduced)");
+  if (!opt_fwd_pending) options_forward_async();
+  VD_CUDA_CHECK(cudaStreamWaitEvent(main_stream, ev_opt_done, 0));
+  opt_fwd_pending = false;
+  cx.stream = main_stream;
+  float* enc_sel = arena.get<float>((int64_t)B * H);
+  gather_round_rows(cx, encOut, rd, enc_sel, B, R, H);
+  scores = arena.get<float>((int64_t)B * K);
+  disc_scores_fwd(cx, opt.h_last(), enc_sel, scores, B, K, H);
+  row_loss = arena.get<float>(B);
+  dscores = arena.get<float>((int64_t)B * K);
+  soft_xent(cx, scores, rel, row_loss, dscores, B, K);
+  reduce_sum(cx, row_loss, scalars_dev, B, 1.f / (float)B);
+  float loss = 0.f;
+  VD_CUDA_CHECK(cudaMemcpyAsync(&loss, scalars_dev, sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));                    // read where vd_forward_backward reads its loss
+  float* dfeat = arena.get<float>((int64_t)B * K * H);
+  float* denc_sel = arena.get<float>((int64_t)B * H);
+  disc_scores_bwd(cx, dscores, opt.h_last(), enc_sel, dfeat, denc_sel, B, K, H);
+  options_backward(dfeat);
+  dEncFromDec = arena.get<float>(db.N * H);
+  scatter_round_rows(cx, denc_sel, rd, dEncFromDec, B, R, H);
+  encoder_backward(dEncFromDec);
+  return loss;
 }
 
 const float* Engine::backward_connect() {

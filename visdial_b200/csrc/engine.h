@@ -261,7 +261,13 @@ struct Engine {
   int opt_reserve_sms = 16;         // SMs the option stream's persistent kernels leave free while they overlap the encoder
   float* opt_demb = nullptr;
   void options_forward_async();
+  void options_backward(const float* dfeat);   // the option BPTT from d(h_T) (opt.R, H), on opt_stream when overlapped
   void join_options_backward();      // main stream waits for the option BPTT and folds its embedding gradient in
+  // dense fine-tuning step (vd_forward_backward_dense): while dense_round (B, device, 0-based) is set, the option LSTM runs
+  // on the K options of round dense_round[b] of each dialog b only
+  const int32_t* dense_round = nullptr;
+  GrowBuf dense_buf[2];              // the step's rounds and relevance rows, uploaded before the encoder forward
+  float forward_backward_dense(const vd_batch* b, const int32_t* round_host, const float* relevance_host);
   std::vector<cudaEvent_t> ev_pool;
   cudaEvent_t pool_event(size_t i);
   void lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last, float* dx_out,

@@ -43,6 +43,12 @@ void vocab_sample_finish(LaunchCtx& cx, const float* part_max, const float* part
 // ---- ids / embedding ---------------------------------------------------------------------------
 // (rows,T) batch-major -> (T,rows) time-major: the `view(-1,T):t()` of model.lua:256,276,308.
 void transpose_ids(LaunchCtx& cx, const int32_t* src, int32_t* dst, int64_t rows, int T);
+// dense fine-tuning (Engine::forward_backward_dense): one selected round per dialog, round[b] in [0, R).
+// transpose_ids over the K option rows of round round[b] of each dialog b: src (B*R*K, T) -> dst (T, B*K)
+void transpose_ids_rounds(LaunchCtx& cx, const int32_t* src, const int32_t* round, int32_t* dst, int64_t B, int R, int K, int T);
+// dst (B,H) <- rows b*R + round[b] of src (B*R,H);  and back: a zeroed (B*R,H) dst with src's rows at b*R + round[b]
+void gather_round_rows(LaunchCtx& cx, const float* src, const int32_t* round, float* dst, int64_t B, int R, int H);
+void scatter_round_rows(LaunchCtx& cx, const float* src, const int32_t* round, float* dst, int64_t B, int R, int H);
 // nn.LookupTableMaskZero forward (+ the nn.Dropout that follows it in mn-att-ques-im-hist.lua:24-25)
 void embed_rows(LaunchCtx& cx, float* out, const float* emb, const int32_t* ids, int64_t rows, int E,
                 DropCfg d, uint32_t site);
@@ -117,6 +123,9 @@ void disc_scores_bwd(LaunchCtx& cx, const float* dscores, const float* feat, con
 // nn.CrossEntropyCriterion (model.lua:38,330,334): mean over rows; writes loss[0] and dscores
 void xent_fwd(LaunchCtx& cx, const float* scores, const int32_t* gt, float* row_loss, int64_t N, int K);
 void xent_bwd(LaunchCtx& cx, const float* scores, const int32_t* gt, float* dscores, int64_t N, int K);
+// soft-target cross-entropy over rows with relevance rel >= 0 (positive row sums): p = rel / sum(rel),
+// row_loss[n] = lse(s_n) - sum_k p_k s_nk,  dscores = (softmax(s_n) - p_n) / N
+void soft_xent(LaunchCtx& cx, const float* scores, const float* rel, float* row_loss, float* dscores, int64_t N, int K);
 void reduce_sum(LaunchCtx& cx, const float* x, float* out, int64_t n, float scale);
 // utils.computeRanks (utils.lua:106-128); tie rule: lower index wins
 void rank_rows(LaunchCtx& cx, const float* scores, const int32_t* gt, int32_t* ranks, int64_t N, int K);

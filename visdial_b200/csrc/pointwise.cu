@@ -56,6 +56,24 @@ __global__ void k_transpose_ids(const int32_t* __restrict__ src, int32_t* __rest
   int64_t t = i / rows, r = i % rows;
   dst[i] = src[r * T + t];
 }
+// the same transpose over the K option rows of one selected round per dialog: dst row j = b*K + k reads source row
+// (b*R + round[b])*K + k
+__global__ void k_transpose_ids_rounds(const int32_t* __restrict__ src, const int32_t* __restrict__ round, int32_t* __restrict__ dst,
+                                       int64_t rows, int T, int R, int K) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= rows * T) return;
+  int64_t t = i / rows, j = i % rows, b = j / K;
+  dst[i] = src[(((b * R + round[b]) * K) + j % K) * T + t];
+}
+// dst[b,:] = src[b*R + round[b], :]  (gather = 1);  dst[b*R + round[b], :] = src[b,:] into a zeroed dst  (gather = 0)
+__global__ void k_round_rows(const float* __restrict__ src, const int32_t* __restrict__ round, float* __restrict__ dst, int64_t B,
+                             int R, int H, int gather) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * H) return;
+  int64_t b = i / H, c = i % H, n = b * R + round[b];
+  if (gather) dst[i] = src[n * H + c];
+  else dst[n * H + c] = src[i];
+}
 
 __global__ void k_embed_rows(float* __restrict__ out, const float* __restrict__ emb, const int32_t* __restrict__ ids,
                              int64_t rows, int E4, DropCfg d, uint32_t site) {
@@ -858,6 +876,26 @@ __global__ void k_xent_bwd(const float* __restrict__ scores, const int32_t* __re
   for (int k = threadIdx.x; k < K; k += blockDim.x)
     dscores[n * K + k] = (expf(scores[n * K + k] - mx) / sum - (k == g ? 1.f : 0.f)) * inv_n;
 }
+// block per row, soft targets p = rel / sum(rel): row_loss = lse(s) - sum_k p_k s_k, dscores = (softmax(s) - p) * inv_n.
+// Block reductions in a fixed order (no atomics): fp32 runs repeat bit for bit.
+__global__ void k_soft_xent(const float* __restrict__ scores, const float* __restrict__ rel, float* __restrict__ row_loss,
+                            float* __restrict__ dscores, int K, float inv_n) {
+  __shared__ float red[33];
+  const int64_t n = blockIdx.x;
+  const float* s = scores + n * K;
+  const float* r = rel + n * K;
+  float mx = -INFINITY, rs = 0.f;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) { mx = fmaxf(mx, s[k]); rs += r[k]; }
+  mx = block_max(mx, red);
+  rs = block_sum(rs, red);
+  float sum = 0.f, dot = 0.f;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) { sum += expf(s[k] - mx); dot += r[k] * s[k]; }
+  sum = block_sum(sum, red);
+  dot = block_sum(dot, red);
+  const float inv_rs = 1.f / rs;
+  if (threadIdx.x == 0) row_loss[n] = mx + logf(sum) - dot * inv_rs;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) dscores[n * K + k] = (expf(s[k] - mx) / sum - r[k] * inv_rs) * inv_n;
+}
 __global__ void k_reduce_sum(const float* __restrict__ x, float* __restrict__ out, int64_t n, float scale) {
   __shared__ float red[33];
   float acc = 0.f;
@@ -1266,6 +1304,16 @@ void set_smem(F f, size_t bytes) {
 void transpose_ids(LaunchCtx& cx, const int32_t* src, int32_t* dst, int64_t rows, int T) {
   L1D(k_transpose_ids, rows * T, src, dst, rows, T);
 }
+void transpose_ids_rounds(LaunchCtx& cx, const int32_t* src, const int32_t* round, int32_t* dst, int64_t B, int R, int K, int T) {
+  L1D(k_transpose_ids_rounds, B * K * T, src, round, dst, B * K, T, R, K);
+}
+void gather_round_rows(LaunchCtx& cx, const float* src, const int32_t* round, float* dst, int64_t B, int R, int H) {
+  L1D(k_round_rows, B * H, src, round, dst, B, R, H, 1);
+}
+void scatter_round_rows(LaunchCtx& cx, const float* src, const int32_t* round, float* dst, int64_t B, int R, int H) {
+  VD_CUDA_CHECK(cudaMemsetAsync(dst, 0, (size_t)B * R * H * sizeof(float), cx.stream));
+  L1D(k_round_rows, B * H, src, round, dst, B, R, H, 0);
+}
 void embed_rows(LaunchCtx& cx, float* out, const float* emb, const int32_t* ids, int64_t rows, int E, DropCfg d, uint32_t site) {
   VD_REQUIRE(E % 4 == 0, -1, "embedSize must be a multiple of 4");
   L1D(k_embed_rows, rows * (E / 4), out, emb, ids, rows, E / 4, d, site);
@@ -1432,6 +1480,11 @@ void xent_bwd(LaunchCtx& cx, const float* scores, const int32_t* gt, float* dsco
   if (N <= 0) return;
   k_xent_bwd<<<(int)N, 128, 0, cx.stream>>>(scores, gt, dscores, K, 1.f / (float)N);
   check_launch(cx, "xent_bwd");
+}
+void soft_xent(LaunchCtx& cx, const float* scores, const float* rel, float* row_loss, float* dscores, int64_t N, int K) {
+  if (N <= 0) return;
+  k_soft_xent<<<(int)N, 128, 0, cx.stream>>>(scores, rel, row_loss, dscores, K, 1.f / (float)N);
+  check_launch(cx, "soft_xent");
 }
 void reduce_sum(LaunchCtx& cx, const float* x, float* out, int64_t n, float scale) {
   k_reduce_sum<<<1, 1024, 0, cx.stream>>>(x, out, n, scale);

@@ -270,6 +270,14 @@ class Dataloader:
         inds = self.rng.integers(0, self.numThreads["train"], size=size)            # :326 (uniform with replacement)
         return self.corpus["train"].get_batch(inds, 0 if params["decoder"] == "disc" else 1)   # :329-337
 
+    def getDenseTrainBatch(self, params: dict, dense):
+        """A disc training batch of `batchSize` annotated entries of `dense` (visdial_b200.dense.read against the train
+        split), drawn uniformly with replacement with this rank's generator.  Returns (batch, the 0-based annotated round
+        of each dialog (B,), their relevance rows (B, numOptions))."""
+        pick = self.rng.integers(0, len(dense), size=int(params["batchSize"]))
+        batch = self.corpus["train"].get_batch(dense.dialog[pick], 0)
+        return batch, (dense.round_id[pick] - 1).astype(np.int32), dense.relevance[pick]
+
     def getIndexData(self, inds0, params: dict, dtype: str) -> DeviceBatch:
         """dataloader.getIndexData (dataloader.lua:378-433) for explicit dialog indices (0-based, within this rank's
         share of the split): the call Model:generateAnswers makes per dialog (model.lua:464)."""

@@ -313,6 +313,21 @@ class Engine:
         self._enc_rows = self._N(batch)
         return loss.value
 
+    def forward_backward_dense(self, batch: Batch, rounds, relevance) -> float:
+        """vd_forward_backward_dense: one step of the soft-target cross-entropy against dense relevances.  rounds (B,)
+        0-based annotated round of each dialog, relevance (B, numOptions) >= 0 with positive row sums."""
+        B, K = batch.c.B, self.params["numOptions"]
+        rounds = np.ascontiguousarray(rounds, dtype=np.int32).reshape(-1)
+        relevance = np.ascontiguousarray(relevance, dtype=np.float32)
+        if rounds.shape != (B,) or relevance.shape != (B, K):
+            raise ValueError("rounds must be (%d,) and relevance (%d, %d)" % (B, B, K))
+        loss = C.c_float()
+        self._enc_rows = None
+        check(self.lib.vd_forward_backward_dense(self.h, C.byref(batch.c), rounds.ctypes.data, relevance.ctypes.data,
+                                                 C.byref(loss)))
+        self._enc_rows = self._N(batch)
+        return loss.value
+
     def retrieve(self, batch: Batch, use_gt: bool = True) -> np.ndarray:
         N = self._N(batch)
         out = np.empty((N,) if use_gt else (N, self.params["numOptions"]), dtype=np.int32)

@@ -10,6 +10,7 @@ import numpy as np
 from . import decoders, encoders
 from .engine import Batch, DEFAULT_PARAMS, derive_flags
 from .modules import Criterion, Sequential
+from .utils import image_id as _image_id
 
 
 def _as_batch(b):
@@ -17,15 +18,6 @@ def _as_batch(b):
     if isinstance(b, tuple):
         b = b[0]
     return b if isinstance(b, Batch) else Batch(b)
-
-
-def _image_id(x):
-    """dataloader.lua:42-44: `tonumber(string.match(name, '000%d+'))` on the json image names; ints pass through."""
-    if isinstance(x, (int, np.integer)):
-        return int(x)
-    import re
-    mt = re.search(r"000\d+", str(x))
-    return int(mt.group(0)) if mt else x
 
 
 def _question_width(dataloader, dtype, inds, convId, Tq, ques_len):
@@ -86,12 +78,28 @@ class Model:
             cur = curLoss / max(numTokens, 1)
         else:                                                             # :86-93
             cur = curLoss
+        self._finish_iteration(cur)
+        return curLoss
+
+    def trainIterationDense(self, dataloader, dense):
+        """trainIteration with the dense fine-tuning step (vd_forward_backward_dense) in place of the standard one: a batch
+        of annotated dialogs of `dense` (visdial_b200.dense), the soft-target cross-entropy on their annotated rounds."""
+        if self.params["decoder"] != "disc":
+            raise ValueError("dense fine-tuning needs a disc model")
+        self.wrapper.zeroGradParameters()
+        batch, rounds, relevance = dataloader.getDenseTrainBatch(self.params, dense)
+        self.iteration += 1
+        self.engine.set_dropout_seed(self.params.get("seed", 1234), self.iteration)
+        curLoss = self.engine.forward_backward_dense(batch, rounds, relevance)
+        self._finish_iteration(curLoss)
+        return curLoss
+
+    def _finish_iteration(self, cur):
         self.runningLoss = 0.95 * self.runningLoss + 0.05 * cur if self.runningLoss > 0 else cur
-        # :96-99 clamp(-5,5) + adam, fused with the gradient all-reduce when world > 1
+        # model.lua:96-99 clamp(-5,5) + adam, fused with the gradient all-reduce when world > 1
         self.engine.clamp_adam_step(self.optims["learningRate"])
         if self.optims["learningRate"] > self.params["minLRate"]:          # :102-105
             self.optims["learningRate"] *= self.params["lrDecayRate"]
-        return curLoss
 
     def forwardBackward(self, batch, onlyForward=False, encOutOnly=False):   # model.lua:249-342
         if not isinstance(batch, Batch):

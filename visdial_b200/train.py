@@ -18,7 +18,14 @@ import time
 from . import cli
 
 
-def main(opt: dict, rank: int = 0, world: int = 1):
+def standard_iteration(model, dl, opt, say):
+    """train's iteration and epoch: Model.trainIteration, over the training split's dialogs.  Returns (the iteration
+    function, the number of items an epoch covers)."""
+    return (lambda: model.trainIteration(dl)), model.params["numTrainThreads"]
+
+
+def main(opt: dict, rank: int = 0, world: int = 1, iteration=standard_iteration):
+    """`iteration(model, dataloader, opt, say)` gives the loop its step and epoch size (standard_iteration: train's)."""
     from . import dist as vdist
     from .checkpoint import load_checkpoint
     say = (lambda *a: print(*a, flush=True)) if rank == 0 else (lambda *a: None)
@@ -39,12 +46,13 @@ def main(opt: dict, rank: int = 0, world: int = 1):
     savePath = opt["savePath"]                                                      # :62-65
     if rank == 0:
         os.makedirs(savePath, exist_ok=True)
-    numIterPerEpoch = p["numIterPerEpoch"] = math.ceil(p["numTrainThreads"] / (world * p["batchSize"]))   # :68-69
+    step, epoch_items = iteration(model, dl, opt, say)
+    numIterPerEpoch = p["numIterPerEpoch"] = math.ceil(epoch_items / (world * p["batchSize"]))   # :68-69
     say("\n%d iter per epoch." % numIterPerEpoch)
     say("Training..")
     saveEvery = int(p["saveIter"]) * numIterPerEpoch
     for it in range(1, int(p["numEpochs"]) * numIterPerEpoch + 1):                  # :90-117
-        model.trainIteration(dl)
+        step()
         if saveEvery > 0 and it % saveEvery == 0 and rank == 0:
             model.save(os.path.join(savePath, "model_epoch_%d.t7" % (it // numIterPerEpoch)))
         if it % 100 == 0:

@@ -17,6 +17,15 @@ def idToWords(vector, ind2word) -> str:
     return sentence
 
 
+def image_id(x):
+    """dataloader.lua:42-44: `tonumber(string.match(name, '000%d+'))` on the json image names; ints pass through."""
+    if isinstance(x, (int, np.integer)):
+        return int(x)
+    import re
+    mt = re.search(r"000\d+", str(x))
+    return int(mt.group(0)) if mt else x
+
+
 def processRanks(ranks, verbose=True):
     """utils.lua:131-160: R@1/5/10, median, mean rank, MRR."""
     r = np.asarray(ranks, dtype=np.float64).reshape(-1)
