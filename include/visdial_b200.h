@@ -169,22 +169,13 @@ int vd_gen_option_lhood(vd_engine* e, const vd_batch* b, const float** lhood_dev
 int vd_encoder_rnn_state(vd_engine* e, int32_t level, const float** h_last_dev, const float** c_last_dev);
 int vd_gen_decoder_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, const float* const* h_prev,
                         const float* const* c_prev, const float** logp_dev, const float** h_out, const float** c_out);
-/* Beam search with the search state on the device (model.lua:510-570, all rounds of a dialog at once): one decoder step on
- * `rows` hypotheses.  parent_host == NULL starts a search: init_h_host / init_c_host[2] are (rows, rnnHiddenSize) HOST arrays
- * (model.lua:480-501).  Otherwise parent_host[r] >= 0 continues hypothesis r from the state row `parent` PRODUCED in the
- * previous call, parent_host[r] < 0 from the state row (-1 - parent) was FED in the previous call (a beam column that received
- * no candidate keeps its old content, :560-569).  Only the k best (log-prob, 0-based class) pairs of every row come back
- * (torch.topk sorted; ties: lower class first) — the (rows, vocabSize) log-probabilities and the LSTM state stay in HBM. */
-int vd_gen_beam_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, const int32_t* parent_host,
-                     const float* const* init_h_host, const float* const* init_c_host, int32_t k, float* topv_host,
-                     int32_t* topi_host);
 /* Model:generateAnswers' beam search (model.lua:472-579) for EVERY round of every dialog of the last vd_encoder_forward
  * (N = B * maxQuesCount searches, N * beam_size hypotheses per step), entirely on the device: the decoder steps, the top-k,
  * the candidate merge with all of the reference's quirks, and the best finished hypothesis.  One synchronisation, at the end.
  * answer_host (N, beam_len) int32: the best finished beam (position 0 = start_token, zero-padded), length_host (N): its
  * length (0 = no hypothesis reached end_token; the reference indexes nil there, :575), score_host (N) fp64: its score.
  * VD_E_STATE for a disc engine or before any vd_encoder_forward; VD_E_BADARG unless 1 <= beam_size <= min(32, vocabSize)
- * and beam_len >= 2.  Ends any search vd_gen_beam_step was continuing. */
+ * and beam_len >= 2. */
 int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
                        int32_t* answer_host, int32_t* length_host, double* score_host);
 /* Model:generateAnswers' sampling (model.lua:581-602, sampleWords = 1) for EVERY round of the last vd_encoder_forward (N =
@@ -195,8 +186,7 @@ int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_
  * answer_host (N, beam_len + 1) int32: column 0 = start_token, columns 1..beam_len the samples.  logp_host (N, beam_len) or
  * NULL: each sampled token's log-probability under the un-tempered LogSoftMax output (decOut).
  * VD_E_STATE for a disc engine or before any vd_encoder_forward; VD_E_BADARG unless beam_len >= 1, temperature is finite and
- * > 0, row_offset >= 0, 1 <= start_token <= vocabSize and answer_host != NULL.  Ends any search vd_gen_beam_step was
- * continuing. */
+ * > 0, row_offset >= 0, 1 <= start_token <= vocabSize and answer_host != NULL. */
 int vd_gen_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
                   int32_t* answer_host, float* logp_host);
 

@@ -1,12 +1,12 @@
-"""Model:generateAnswers' beam search on the device (vd_gen_beam_search, model.lua:472-579) against the search it replaces:
-the candidate merge on the host over vd_gen_beam_step, which steps the decoder with the same kernels and returns each
-hypothesis' top k.  The two walk the same hypotheses, so answers, lengths and fp64 scores must agree bit for bit."""
-import ctypes as C
-
+"""Model:generateAnswers' beam search on the device (vd_gen_beam_search, model.lua:472-579) against the host reference
+(tests/host_decode.py): the decoder stepped through vd_gen_decoder_step with the same kernels at the same row count, the
+top k and the candidate merge on the host.  The two walk the same hypotheses, so answers, lengths and fp64 scores must
+agree bit for bit."""
 import numpy as np
 import pytest
 
 from helpers import small_batch, small_params
+from host_decode import host_beam_search
 from visdial_b200 import VD_MATH_F16, VD_MATH_FP32, VD_MATH_TF32, init_parameters
 from visdial_b200 import _lib
 from visdial_b200.engine import Batch, Engine, split_parameters
@@ -16,68 +16,6 @@ pytestmark = pytest.mark.gpu
 # per-step launches of the search in the FP32 math mode (DESIGN §14): 4 state gathers, the embedding, 3 per LSTM layer
 # (x-projection, recurrent GEMM, pointwise), the vocabulary projection, the fused log-softmax + top-k and the merge
 STEP_LAUNCHES_FP32 = 14
-
-
-def host_beam_search(eng, encOut, k, L, start, end, stats=None):
-    """The beam branch of Model.generateAnswers as the engine ran it before the search moved to the device: all rounds
-    of the encoder forward at once, the decoder state and log-probabilities on the device (vd_gen_beam_step), the
-    candidate merge of model.lua:529-569 — with its quirks — on the host.  Returns (answer (N, L), length (N), score (N))
-    in vd_gen_beam_search's format.  `stats` counts the cases worth covering: beam columns left without a candidate,
-    pad tokens fed to the decoder, and the steps at which some hypothesis reached `end`."""
-    N, H = encOut.shape
-    (h1, c1), (_, c2) = [eng.encoder_rnn_state(l, N) for l in range(2)]
-    if h1 is not None:                                                          # :482-491
-        iH = [np.repeat(h1.numpy(), k, 0), np.repeat(encOut, k, 0)]
-        iC = [np.repeat(c1.numpy(), k, 0), np.repeat(c2.numpy(), k, 0)]
-    else:                                                                       # :493-501
-        z = np.zeros((N * k, H), np.float32)
-        iH, iC = [z, np.repeat(encOut, k, 0)], [z, z]
-    beams = np.zeros((N, L, k), dtype=np.int64)                                 # :479
-    beams[:, 0, :] = start                                                      # :506
-    scores = np.zeros((N, k), dtype=np.float64)                                 # :507
-    finish = [[] for _ in range(N)]                                             # :508
-    parent = None
-    for stp in range(1, L):                                                     # :510
-        fed = beams[:, stp - 1, :].reshape(-1)
-        topv, topi = eng.gen_beam_step(fed, parent, iH, iC, k)                  # :519-542
-        parent = -1 - np.arange(N * k, dtype=np.int32)                          # default: the column keeps its old content
-        exploreSize = 1 if stp == 1 else k                                      # :516
-        if stats is not None:
-            stats["pad_rows"] += int((fed == 0).sum())
-        for it in range(N):
-            cands = []
-            for wordId in range(exploreSize):                                   # :529
-                r = it * k + wordId
-                for candId in range(k):                                         # :544
-                    tok = int(topi[r, candId]) + 1
-                    sc = float(scores[it, wordId]) + float(topv[r, candId])
-                    if tok == end:                                              # :548
-                        cb = beams[it, :, wordId].copy()
-                        cb[stp] = tok
-                        finish[it].append({"beam": cb, "length": stp + 1, "score": sc})
-                        if stats is not None:
-                            stats["end_steps"].add(stp)
-                    else:
-                        cands.append((sc, wordId, tok))
-            cands.sort(key=lambda t: -t[0])                                     # :558 (stable)
-            if stats is not None and len(cands) < k:
-                stats["stale"] += k - len(cands)
-            old = beams[it].copy()
-            for candId in range(min(len(cands), k)):                            # :560-569
-                sc, wordId, tok = cands[candId]
-                beams[it, :, candId] = old[:, wordId]
-                beams[it, stp, candId] = tok
-                scores[it, candId] = sc
-                parent[it * k + candId] = it * k + wordId
-    answer = np.zeros((N, L), np.int32)
-    length = np.zeros(N, np.int32)
-    score = np.zeros(N, np.float64)
-    for it in range(N):
-        finish[it].sort(key=lambda d: -d["score"])                              # :572
-        if finish[it]:
-            best = finish[it][0]
-            answer[it], length[it], score[it] = best["beam"], best["length"], best["score"]
-    return answer, length, score
 
 
 def _engine(enc, mode, V, H, E, end_bias, seed=5):
@@ -102,7 +40,7 @@ SIZES = {"small": dict(V=9, H=32, E=12, D=3, k=3, L=8, end_bias=1.0),
 @pytest.mark.parametrize("size", sorted(SIZES))
 @pytest.mark.parametrize("mode", [VD_MATH_FP32, VD_MATH_TF32, VD_MATH_F16], ids=["fp32", "tf32", "f16"])
 @pytest.mark.parametrize("enc", ["lf-ques", "hrea-ques-im-hist", "mn-att-ques-im-hist", "lf-att-ques-im-hist"])
-def test_device_search_matches_host_merge(enc, mode, size):
+def test_device_search_matches_host_search(enc, mode, size):
     s = SIZES[size]
     V, k, L = s["V"], s["k"], s["L"]
     params, eng = _engine(enc, mode, V, s["H"], s["E"], s["end_bias"])
@@ -120,7 +58,7 @@ def test_device_search_matches_host_merge(enc, mode, size):
 
 @pytest.mark.parametrize("enc", ["lf-ques", "mn-att-ques-im-hist"])
 @pytest.mark.parametrize("k,L", [(1, 8), (9, 6), (3, 2)], ids=["beam1", "beam_eq_V", "len2"])
-def test_device_search_edges(enc, k, L):
+def test_device_search_edges_match_host_search(enc, k, L):
     params, eng = _engine(enc, VD_MATH_FP32, 9, 32, 12, 1.0)
     encOut = _forward(eng, params, 2)
     want = host_beam_search(eng, encOut, k, L, 8, 9)

@@ -6,6 +6,7 @@ import pytest
 
 from oracle import dataloader_oracle as D
 from helpers import small_params
+from host_decode import host_beam_search
 from visdial_b200._lib import VdError
 from visdial_b200.dataloader import Dataloader
 from visdial_b200.engine import Batch, Engine
@@ -220,8 +221,9 @@ def test_model_retrieve_over_the_device_dataloader(enc, dec):
 @pytest.mark.parametrize("enc", ["lf-ques", "hrea-ques-im-hist", "mn-att-ques-im-hist", "lf-ques-im-hist", "lf-ques-im", "hre-ques-im-hist",
                                  "mn-ques-hist", "lf-att-ques-im-hist"])
 def test_generate_answers_matches_oracle(enc):
-    """Model:generateAnswers (model.lua:432-613) — beam search and sampling driven through vd_gen_decoder_step on
-    batches the device dataloader assembles — against oracle.generate_answers on the same dialog (fp32 math mode)."""
+    """Model:generateAnswers (model.lua:432-613) — beam search and sampling on batches the device dataloader assembles —
+    against the host reference search (tests/host_decode.py) on the same encoder forward, and against
+    oracle.generate_answers on the same dialog (fp32 math mode)."""
     import torch
     from helpers import torch_batch, torch_params
     from oracle import visdial_oracle as O
@@ -241,12 +243,14 @@ def test_generate_answers_matches_oracle(enc):
     P = torch_params(params, flat)
     for conv in (0, 3, 7):
         got = model.generateAnswers(dl, "val", {"beamSize": 3, "beamLen": 6, "maxThreads": conv + 1}, strict=False)[conv]["dialog"]
-        # the batched search (all rounds per step, state + log-probabilities on the device, top-k on the device) walks exactly
-        # the hypotheses of the reference-structured loop (one round at a time, everything through the host)
-        host = model.generateAnswers(dl, "val", {"beamSize": 3, "beamLen": 6, "maxThreads": conv + 1, "hostBeam": 1},
-                                     strict=False)[conv]["dialog"]
+        # the device search walks exactly the hypotheses of the host reference (state, log-probabilities, top-k and merge
+        # through the host) on the same dialog's encoder forward
+        model.wrapper.evaluate()
+        encOut = model.forwardBackward(dl.getIndexData(np.array([conv]), model.params, "val"), True, True).numpy()
+        model.wrapper.training()
+        answer, length, score = host_beam_search(model.engine, encOut, 3, 6, dl.word2ind["<START>"], dl.word2ind["<END>"])
         assert [None if g is None else (g["answer"], g["length"], g["score"]) for g in got] == \
-               [None if h is None else (h["answer"], h["length"], h["score"]) for h in host]
+               [None if n == 0 else (a.tolist(), int(n), float(s)) for a, n, s in zip(answer, length, score)]
         tb = torch_batch(orc.get_index_data(np.array([conv])))
         with torch.no_grad():
             want = O.generate_answers(O.Ctx(), params, P, tb, V - 1, V, beam_size=3, beam_len=6, strict=False)

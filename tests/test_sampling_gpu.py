@@ -9,6 +9,7 @@ import pytest
 from scipy import stats
 
 from helpers import small_batch, small_params
+from host_decode import HostStep, start_state
 from sampling_twin import draw
 from visdial_b200 import VD_MATH_F16, VD_MATH_FP32, VD_MATH_TF32, init_parameters
 from visdial_b200 import _lib
@@ -118,24 +119,12 @@ def test_distribution(route):
 def replay(eng, encOut, tokens):
     """the sampled tokens (N, L + 1) fed back through vd_gen_decoder_step with explicit state, as the host sampler stepped
     the decoder: model.lua:581-588 with decoderConnect (gen.lua:63-68).  Returns the (N, V) log-probabilities of every step."""
-    N, H = encOut.shape
-    (h1, c1), (_, c2) = [eng.encoder_rnn_state(l, N) for l in range(2)]
-    if h1 is not None:                                                          # forwardConnect, gen.lua:30-42
-        Hs, Cs = [h1.numpy(), encOut], [c1.numpy(), c2.numpy()]
-    else:
-        z = np.zeros((N, H), np.float32)
-        Hs, Cs = [z, encOut], [z, z]
-    bufs = [eng.device_alloc(N * H * 4) for _ in range(4)]
+    h, c = start_state(eng, encOut)                                             # forwardConnect, gen.lua:30-42
     out = []
-    try:
+    with HostStep(eng, encOut.shape[0]) as step:
         for t in range(tokens.shape[1] - 1):
-            for i, a in enumerate(Hs + Cs):
-                eng.upload(bufs[i], a)
-            lp, Hs, Cs = eng.gen_decoder_step(tokens[:, t], bufs[0:2], bufs[2:4])
+            lp, h, c = step(tokens[:, t], h, c)
             out.append(lp.astype(np.float64))
-    finally:
-        for b in bufs:
-            eng.device_free(b)
     return out
 
 

@@ -1,13 +1,12 @@
 """Model:generateAnswers (model.lua:432-613) wall time per dialog: beam search (beamSize 5, beamLen 20) or sampling (beamLen
 20, sampleWords = 1) over the 10 rounds of each dialog, V = 10 000, for `hrea-ques-im-hist + gen` (C3's graph) and
 `mn-att-ques-im-hist + gen`, in the F16 and FP32 math modes.  Paths, all in one run:
-  device/<d>  beam search, the default: vd_gen_beam_search, d dialogs per encoder forward and call (params.dialogsPerCall)
-  host_merge  the search as the engine ran it before it moved to the device: per dialog, the candidate merge on the host
-              over vd_gen_beam_step (tests/test_beam_search_gpu.py::host_beam_search)
-  host_beam   params.hostBeam = 1: the reference's loop structure, one round at a time through vd_gen_decoder_step
-  sample/<d>  sampling: vd_gen_sample, d dialogs per encoder forward and call
-  host_sample sampling as the engine ran it before it moved to the device: per dialog and step, the state up, one
-              vd_gen_decoder_step, the log-probabilities and state down, one numpy categorical draw per round (host_sample)
+  device/<d>   beam search, the default: vd_gen_beam_search, d dialogs per encoder forward and call (params.dialogsPerCall)
+  host_search  the tests' host reference search (tests/host_decode.py::host_beam_search), per dialog: the state and
+               log-probabilities through the host at every vd_gen_decoder_step, the top-k and the candidate merge on the host
+  sample/<d>   sampling: vd_gen_sample, d dialogs per encoder forward and call
+  host_sample  sampling as the engine ran it before it moved to the device: per dialog and step, the state up, one
+               vd_gen_decoder_step, the log-probabilities and state down, one numpy categorical draw per round (host_sample)
 Every path is warmed up at its shape first, then timed over whole calls until the window lasts at least --window seconds
 (host clock; every call ends in a device synchronisation).  Prints one JSON line per (encoder, mode, path) and the card's name
 and power limit, read in the same run.
@@ -29,7 +28,7 @@ from visdial_b200 import VD_MATH_F16, VD_MATH_FP32, Model  # noqa: E402
 from visdial_b200.dataloader import Dataloader  # noqa: E402
 from visdial_b200.engine import DEFAULT_PARAMS, derive_flags  # noqa: E402
 from visdial_b200.synthetic import make_corpus  # noqa: E402
-from test_beam_search_gpu import host_beam_search  # noqa: E402
+from host_decode import HostStep, host_beam_search, start_state  # noqa: E402
 
 BEAM, LEN, V = 5, 20, 10000
 
@@ -47,27 +46,16 @@ def card():
 
 def host_sample(eng, encOut, L, start, T, rng):
     """the sampling branch of Model.generateAnswers before it moved to the device (one dialog: all its rounds per step)"""
-    N, H = encOut.shape
-    (h1, c1), (_, c2) = [eng.encoder_rnn_state(l, N) for l in range(2)]
-    if h1 is not None:                                                          # forwardConnect, gen.lua:30-42
-        Hs, Cs = [h1.numpy(), encOut], [c1.numpy(), c2.numpy()]
-    else:
-        Hs, Cs = [np.zeros((N, H), np.float32), encOut], [np.zeros((N, H), np.float32)] * 2
-    bufs = [eng.device_alloc(N * H * 4) for _ in range(4)]
-    try:
-        tok = np.full(N, start, dtype=np.int64)
-        seq = [tok.copy()]
+    h, c = start_state(eng, encOut)                                             # forwardConnect, gen.lua:30-42
+    tok = np.full(encOut.shape[0], start, dtype=np.int64)
+    seq = [tok.copy()]
+    with HostStep(eng, encOut.shape[0]) as step:
         for _ in range(L):
-            for i, a in enumerate(Hs + Cs):
-                eng.upload(bufs[i], a)
-            decOut, Hs, Cs = eng.gen_decoder_step(tok, bufs[0:2], bufs[2:4])     # :586-588 (+ decoderConnect)
+            decOut, h, c = step(tok, h, c)                                      # :586-588 (+ decoderConnect)
             p = np.exp(decOut.astype(np.float64) / T)                           # :590
             p /= p.sum(1, keepdims=True)
-            tok = np.array([rng.choice(p.shape[1], p=p[i]) + 1 for i in range(N)], dtype=np.int64)
+            tok = np.array([rng.choice(p.shape[1], p=p[i]) + 1 for i in range(len(tok))], dtype=np.int64)
             seq.append(tok.copy())
-    finally:
-        for b in bufs:
-            eng.device_free(b)
     return np.stack(seq, 1)
 
 
@@ -108,7 +96,7 @@ def main():
             m.engine.set_math_mode({"f16": VD_MATH_F16, "fp32": VD_MATH_FP32}[mode])
             beam = {"beamSize": BEAM, "beamLen": LEN}
 
-            def host_merge():
+            def host_search():
                 m.wrapper.evaluate()
                 b = dl.getIndexData(np.array([0]), m.params, "val")
                 encOut = m.forwardBackward(b, True, True).numpy()
@@ -129,8 +117,7 @@ def main():
             if "beam" in kinds:
                 paths += [("device/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(beam, maxThreads=d, dialogsPerCall=d),
                                                                              strict=False)) for d in dpcs]
-                paths += [("host_merge", 1, host_merge),
-                          ("host_beam", 1, lambda: m.generateAnswers(dl, "val", dict(beam, maxThreads=1, hostBeam=1), strict=False))]
+                paths += [("host_search", 1, host_search)]
             if "sample" in kinds:
                 paths += [("sample/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(samp, maxThreads=d, dialogsPerCall=d)))
                           for d in dpcs]
@@ -143,7 +130,7 @@ def main():
                 rows.append(r)
         dl.close(); m.engine.close()
     print("\n%s, power limit %s: ms per dialog (beam %d x %d / sampling x %d, V = %d)" % (name, power, BEAM, LEN, LEN, V))
-    order = ["device", "host_merge", "host_beam", "sample", "host_sample"]
+    order = ["device", "host_search", "sample", "host_sample"]
     paths = sorted({r["path"] for r in rows}, key=lambda s: (order.index(s.split("/")[0]), int(s.split("/")[1]) if "/" in s else 0))
     print("| encoder | mode | " + " | ".join(paths) + " |")
     print("|---|---|" + "---|" * len(paths))

@@ -251,12 +251,6 @@ int vd_gen_decoder_step(vd_engine* h, int32_t rows, const int32_t* tokens_host, 
   })
 }
 
-int vd_gen_beam_step(vd_engine* h, int32_t rows, const int32_t* tokens_host, const int32_t* parent_host,
-                     const float* const* init_h_host, const float* const* init_c_host, int32_t k, float* topv_host,
-                     int32_t* topi_host) {
-  VD_TRY({ ENG(h)->gen_beam_step(rows, tokens_host, parent_host, init_h_host, init_c_host, k, topv_host, topi_host); })
-}
-
 int vd_gen_beam_search(vd_engine* h, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
                        int32_t* answer_host, int32_t* length_host, double* score_host) {
   VD_TRY({ ENG(h)->gen_beam_search(beam_size, beam_len, start_token, end_token, answer_host, length_host, score_host); })

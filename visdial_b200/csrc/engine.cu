@@ -1516,52 +1516,10 @@ void Engine::gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float
   lstm_forward(gstep2, true);
 }
 
-// One beam-search step (model.lua:510-570) for `rows` hypotheses at once (all rounds of a dialog x beamSize).  The state of
-// the previous call stays on the device: parent_host[r] >= 0 takes the state hypothesis parent produced, < 0 the state row
-// (-1 - parent) was fed (stale beam column).  parent_host == NULL starts a search from the host arrays init_h / init_c.
-void Engine::gen_beam_step(int64_t rows, const int32_t* tokens_host, const int32_t* parent_host, const float* const* init_h_host,
-                           const float* const* init_c_host, int k, float* topv_host, int32_t* topi_host) {
-  VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_step needs the gen decoder after encoder_forward");
-  VD_REQUIRE(rows > 0 && tokens_host && topv_host && topi_host && k >= 1 && k <= cfg.V, VD_E_BADARG, "rows / tokens / k");
-  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
-  cx.stream = main_stream;
-  const int H = cfg.H;
-  float* hp[2]; float* cp[2];
-  for (int l = 0; l < 2; ++l) { hp[l] = arena.get<float>(rows * H); cp[l] = arena.get<float>(rows * H); }
-  if (!parent_host) {
-    VD_REQUIRE(init_h_host && init_c_host, VD_E_BADARG, "first beam step needs the initial state");
-    for (int l = 0; l < 2; ++l) {
-      VD_CUDA_CHECK(cudaMemcpyAsync(hp[l], init_h_host[l], (size_t)rows * H * sizeof(float), cudaMemcpyHostToDevice, cx.stream));
-      VD_CUDA_CHECK(cudaMemcpyAsync(cp[l], init_c_host[l], (size_t)rows * H * sizeof(float), cudaMemcpyHostToDevice, cx.stream));
-    }
-  } else {
-    VD_REQUIRE(beam_rows == rows && beam_in_h[0], VD_E_STATE, "gen_beam_step: no previous step with this many rows");
-    int32_t* par = arena.get<int32_t>(rows);
-    VD_CUDA_CHECK(cudaMemcpyAsync(par, parent_host, (size_t)rows * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
-    const float* out_h[2] = {gstep1.h, gstep2.h};
-    const float* out_c[2] = {gstep1.c, gstep2.c};
-    for (int l = 0; l < 2; ++l) {
-      beam_gather(cx, hp[l], out_h[l], beam_in_h[l], par, rows, H);
-      beam_gather(cx, cp[l], out_c[l], beam_in_c[l], par, rows, H);
-    }
-  }
-  const float* hpc[2] = {hp[0], hp[1]};
-  const float* cpc[2] = {cp[0], cp[1]};
-  gen_decoder_step(rows, tokens_host, hpc, cpc);            // synchronises once for the token upload
-  for (int l = 0; l < 2; ++l) { beam_in_h[l] = hp[l]; beam_in_c[l] = cp[l]; }
-  beam_rows = rows;
-  float* tv = arena.get<float>(rows * k);
-  int32_t* ti = arena.get<int32_t>(rows * k);
-  topk_rows(cx, gstep_logp, rows, cfg.V, k, tv, ti);
-  VD_CUDA_CHECK(cudaMemcpyAsync(topv_host, tv, (size_t)rows * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(topi_host, ti, (size_t)rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
-}
-
 // Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once: row n*k + j is
-// hypothesis j of round n.  Every step runs gen_beam_step's kernels on device-resident tokens and parents — state gather,
-// decoder step, vocabulary projection — then the fused log-softmax + top-k and the candidate merge, which writes the next
-// step's tokens and parents.  Nothing returns to the host until the final copy of each round's best finished hypothesis.
+// hypothesis j of round n.  Every step runs on device-resident tokens and parents: the state gather, the decoder step of
+// gen_decoder_step_logits, the fused log-softmax + top-k and the candidate merge, which writes the next step's tokens and
+// parents.  Nothing returns to the host until the final copy of each round's best finished hypothesis.
 void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
                              double* score_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_search needs the gen decoder after encoder_forward");
@@ -1614,7 +1572,6 @@ void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32
     beam_merge(cx, N, stp, k, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, ans, ans_len,
                ans_score);
   }
-  beam_rows = 0;                                   // gstep1 / gstep2 hold this search's state now: vd_gen_beam_step starts over
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(length_host, ans_len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(score_host, ans_score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
@@ -1686,7 +1643,6 @@ void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed
     h[0] = gstep1.h; h[1] = gstep2.h;
     c[0] = gstep1.c; c[1] = gstep2.c;
   }
-  beam_rows = 0;                                   // gstep1 / gstep2 hold this call's state now: vd_gen_beam_step starts over
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   if (logp_host)
     VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, lp, (size_t)N * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));

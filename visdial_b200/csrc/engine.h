@@ -296,12 +296,6 @@ struct Engine {
   void gen_decoder_step(int64_t rows, const int32_t* tokens_host, const float* const* h_prev, const float* const* c_prev);
   // its core on device-resident tokens, up to the vocabulary projection: gstep_logp holds the LOGITS on return
   void gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
-  // beam search with the decoder state and the (rows, V) log-probabilities kept on the device: per step only the tokens and
-  // parent indices go up and the k best (log-prob, class) pairs per hypothesis come down
-  const float *beam_in_h[2] = {nullptr, nullptr}, *beam_in_c[2] = {nullptr, nullptr};
-  int64_t beam_rows = 0;
-  void gen_beam_step(int64_t rows, const int32_t* tokens_host, const int32_t* parent_host, const float* const* init_h_host,
-                     const float* const* init_c_host, int k, float* topv_host, int32_t* topi_host);
   // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device
   void gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
   // the decoder step up to the second LSTM layer (gstep1 / gstep2 hold the new state on return)

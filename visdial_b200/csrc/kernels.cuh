@@ -138,10 +138,10 @@ void nll_bwd(LaunchCtx& cx, const float* logp, const int32_t* tgt, const int32_t
 void lhood_accumulate(LaunchCtx& cx, const float* logits, const int32_t* tgt, const int32_t* mask_ids, float* lh,
                       int64_t rows, int V);
 
-// beam search on the device (model.lua:510-570): k best classes per row (value desc, index asc); state shuffle by parent index
-void topk_rows(LaunchCtx& cx, const float* x, int64_t rows, int V, int k, float* topv, int32_t* topi);
+// beam search on the device (model.lua:510-570): state shuffle by parent index
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H);
-// logsoftmax_rows + topk_rows in one pass that never writes the log-probabilities (bit-identical results), k <= 32
+// the k <= 32 best log-probabilities per row and their classes (value desc, class asc), never writing the log-probabilities:
+// lse from the same row_lse as logsoftmax_rows, so the values are logsoftmax_rows' bits
 void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
                           int32_t* topi);
 // the whole search on the device (Engine::gen_beam_search): beams (rows, L) = <start> then pads, tokens = <start>, scores = 0

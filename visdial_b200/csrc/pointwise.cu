@@ -226,43 +226,7 @@ __global__ void k_lstm_pw_bwd(const float* __restrict__ gates, const float* __re
   dc_carry[idx] = dc * gf;
 }
 
-// ---- beam search on the device (model.lua:510-570): the k best continuations of every hypothesis, and the state shuffle
-// Total order of torch.topk(sorted) with the pinned tie rule: value descending, class index ascending.  Round r of the loop
-// finds the greatest element strictly AFTER the previous winner in that order, so no "taken" flags are needed.
-__global__ void __launch_bounds__(256) k_topk_rows(const float* __restrict__ x, int V, int k, float* __restrict__ topv,
-                                                   int32_t* __restrict__ topi) {
-  __shared__ float sv[8];
-  __shared__ int si[8];
-  __shared__ float wv; __shared__ int wi;
-  const float* row = x + (int64_t)blockIdx.x * V;
-  float pv = INFINITY; int pi = -1;
-  for (int r = 0; r < k; ++r) {
-    float bv = -INFINITY; int bi = 0x7fffffff;
-    for (int c = threadIdx.x; c < V; c += blockDim.x) {
-      const float v = row[c];
-      const bool after = v < pv || (v == pv && c > pi);
-      if (after && (v > bv || (v == bv && c < bi))) { bv = v; bi = c; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
-    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = bv; si[threadIdx.x >> 5] = bi; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
-        if (sv[w] > bv || (sv[w] == bv && si[w] < bi)) { bv = sv[w]; bi = si[w]; }
-      wv = bv; wi = bi;
-      topv[(int64_t)blockIdx.x * k + r] = bv;
-      topi[(int64_t)blockIdx.x * k + r] = bi;
-    }
-    __syncthreads();
-    pv = wv; pi = wi;
-    __syncthreads();
-  }
-}
+// ---- beam search on the device (model.lua:510-570): the state shuffle
 // next step's previous state of row r: parent >= 0 -> the state hypothesis `parent` PRODUCED in the last step; parent < 0 -> the
 // state row (-1 - parent) was FED in the last step (a beam column that received no candidate keeps its old content, model.lua:560-569)
 __global__ void k_beam_gather(float* __restrict__ dst, const float* __restrict__ out_prev, const float* __restrict__ in_prev,
@@ -947,10 +911,12 @@ __global__ void k_logsoftmax_rows(float* __restrict__ x, const int32_t* __restri
 // (v, c) precedes (w, d) in torch.topk's order with the pinned tie rule: value descending, class ascending
 __device__ __forceinline__ bool topk_before(float v, int c, float w, int d) { return v > w || (v == w && c < d); }
 
-// k_logsoftmax_rows followed by k_topk_rows, without writing the (rows, V) log-probabilities: the logits are read three
-// times whatever k is.  Each thread keeps the KMAX best (x - lse, class) pairs of its strided columns, sorted, in
-// registers; the block then pops k winners from the thread heads.  Same values and order as the two-kernel path, bit for
-// bit.  A row whose mask id is 0 is all zeros there: its top k is classes 0..k-1 with value 0.
+// The k best log-probabilities of every row and their classes, in torch.topk(sorted)'s order with the pinned tie rule
+// (value descending, class ascending), without writing the (rows, V) log-probabilities: the logits are read three times
+// whatever k is.  The lse comes from row_lse, so each x - lse is the value k_logsoftmax_rows would write, bit for bit.
+// Each thread keeps the KMAX best (x - lse, class) pairs of its strided columns, sorted, in registers; the block then pops
+// k winners from the thread heads.  A row whose mask id is 0 is all zeros in k_logsoftmax_rows (MaskZero): its top k is
+// classes 0..k-1 with value 0.
 template <int KMAX>
 __global__ void __launch_bounds__(256) k_logsoftmax_topk_rows(const float* __restrict__ x, const int32_t* __restrict__ mask_ids,
                                                               int V, int k, float* __restrict__ topv, int32_t* __restrict__ topi) {
@@ -1525,12 +1491,6 @@ void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, in
   if (rows <= 0) return;
   k_logsoftmax_sample_rows<<<(unsigned)rows, 256, 0, cx.stream>>>(logits, V, smp, L, tokens, answer, logp);
   check_launch(cx, "k_logsoftmax_sample_rows");
-}
-void topk_rows(LaunchCtx& cx, const float* x, int64_t rows, int V, int k, float* topv, int32_t* topi) {
-  VD_REQUIRE(k >= 1 && k <= V, VD_E_BADARG, "topk_rows: k");
-  if (rows == 0) return;
-  k_topk_rows<<<(unsigned)rows, 256, 0, cx.stream>>>(x, V, k, topv, topi);
-  check_launch(cx, "k_topk_rows");
 }
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H) {
   L1D(k_beam_gather, rows * H, dst, out_prev, in_prev, parent, rows, H);

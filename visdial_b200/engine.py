@@ -361,25 +361,6 @@ class Engine:
                 [DeviceTensor(self, ho[i], (rows, H)).numpy() for i in range(2)],
                 [DeviceTensor(self, co[i], (rows, H)).numpy() for i in range(2)])
 
-    def gen_beam_step(self, tokens: np.ndarray, parent, init_h, init_c, k: int):
-        """One beam-search step with the state kept on the device (vd_gen_beam_step).  parent None = first step (init_h /
-        init_c: two (rows, H) float32 arrays each).  Returns (top log-probs (rows,k), top 0-based classes (rows,k))."""
-        tokens = np.ascontiguousarray(tokens, dtype=np.int32)
-        rows = tokens.shape[0]
-        topv = np.empty((rows, k), dtype=np.float32)
-        topi = np.empty((rows, k), dtype=np.int32)
-        arr = C.c_void_p * 2
-        if parent is None:
-            ih = [np.ascontiguousarray(a, dtype=np.float32) for a in init_h]
-            ic = [np.ascontiguousarray(a, dtype=np.float32) for a in init_c]
-            check(self.lib.vd_gen_beam_step(self.h, rows, tokens.ctypes.data, None, arr(*[a.ctypes.data for a in ih]),
-                                            arr(*[a.ctypes.data for a in ic]), k, topv.ctypes.data, topi.ctypes.data))
-        else:
-            par = np.ascontiguousarray(parent, dtype=np.int32)
-            check(self.lib.vd_gen_beam_step(self.h, rows, tokens.ctypes.data, par.ctypes.data, None, None, k, topv.ctypes.data,
-                                            topi.ctypes.data))
-        return topv, topi
-
     def gen_beam_search(self, k: int, L: int, start: int, end: int):
         """The whole beam search for every round of the last encoder forward on the device (vd_gen_beam_search).  Returns
         (answer (N, L) int32, length (N) int32 — 0 where no beam reached `end` — and score (N) float64)."""

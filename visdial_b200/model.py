@@ -1,8 +1,7 @@
 """Mirror of the reference's `Model` class (/root/reference/model.lua:8-430) over the C engine.
 Same method names, argument meaning and call order as the Lua original, so that the parity tests
 read like the reference's own driver code.  `generateAnswers` (beam search / sampling, model.lua:432-613) runs the beam
-search and the sampling entirely on the device (vd_gen_beam_search, vd_gen_sample); the reference-structured beam loop steps
-the decoder through vd_gen_decoder_step and keeps the hypothesis bookkeeping on the host like the Lua."""
+search and the sampling entirely on the device (vd_gen_beam_search, vd_gen_sample)."""
 from __future__ import annotations
 
 import numpy as np
@@ -200,121 +199,37 @@ class Model:
     # ---- beam search / sampling (model.lua:432-613, generate.lua) ---------------------------------------------
     def generateAnswers(self, dataloader, dtype="val", params=None, strict=True):
         """Model:generateAnswers.  Beam search (the default) and sampling (`sampleWords = 1`) run entirely on the device
-        through vd_gen_beam_search / vd_gen_sample, for `params.dialogsPerCall` dialogs (default 1) per encoder forward:
-        every round of those dialogs is searched or sampled at once.  `hostBeam = 1` (the reference's loop structure) goes
-        one dialog at a time, the decoder stepped through vd_gen_decoder_step and the hypothesis bookkeeping on the host as
-        the Lua does it.  Returns the reference's answerTable with token-id lists (and text when the dataloader carries
+        through vd_gen_beam_search / vd_gen_sample, for `params.dialogsPerCall` dialogs (default 1) per encoder forward and
+        engine call: every round of those dialogs is searched or sampled at once.  One dialog per call gives exactly the
+        per-dialog trimming and kernel shapes of the reference's loop; more dialogs per call run wider kernels (in the
+        tensor-core math modes their rounding can differ from per-dialog runs).  The draws of a sampled round depend only on
+        (seed, its global round index, the step): each call passes the index of its first round in the split (this rank's
+        offset included), so the samples do not depend on dialogsPerCall or on how the split is sharded over ranks, only on
+        the logits.  Returns the reference's answerTable with token-id lists (and text when the dataloader carries
         ind2word).  `strict=False` yields None for a round where no beam reached <END> (the reference indexes nil there,
         model.lua:575)."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
         sampleWords = bool(params.get("sampleWords", 0) == 1)                           # :443
-        temperature = float(params.get("temperature", 1.0))
+        temperature, seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
         beamSize, beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
         startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
         numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
+        dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
         ind2word = getattr(dataloader, "ind2word", None)
-        eng, H = self.engine, self.params["rnnHiddenSize"]
         words = (lambda ids: " ".join(ind2word.get(int(t), "<UNK>") for t in ids if int(t) > 0)) if ind2word else None
         img = getattr(dataloader, "unique_img_" + dtype, None)
-        # getIndexData hands out this rank's slice of the split: the image list is indexed by the global dialog id
-        first = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
+        # getIndexData hands out this rank's slice of the split: the image list and the sampled rounds' global indices
+        # count from the slice's first dialog
+        offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
 
-        def image_id(convId):
-            gid = convId + first
-            return _image_id(img[gid]) if img is not None else gid
-
-        def entry(q, answer, score, length):
-            e = {"question": q.tolist(), "answer": answer.tolist(), "score": score, "length": length}
+        def entry(q, answer, **scored):
+            e = {"question": q.tolist(), "answer": answer.tolist(), **scored}
             if words:
                 e["question_text"], e["answer_text"] = words(q), words(answer)
             return e
 
-        dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
-        if sampleWords:
-            return self._generate_sample(dataloader, dtype, numThreads, dialogsPerCall, beamLen, startToken, temperature,
-                                         int(params.get("seed", 1234)), first, image_id, words)
-        if not params.get("hostBeam"):
-            return self._generate_beam(dataloader, dtype, numThreads, dialogsPerCall, beamSize, beamLen, startToken, endToken,
-                                       strict, image_id, entry)
-        state_buf = [eng.device_alloc(max(beamSize, self.params["maxQuesCount"]) * H * 4) for _ in range(4)]
-        answerTable = []
-        try:
-            for convId in range(numThreads):
-                self.wrapper.evaluate()                                                 # :460
-                batch = dataloader.getIndexData(np.array([convId]), self.params, dtype)  # :462-463
-                encOut = self.forwardBackward(batch, True, True).numpy()                # :467 (N,H), N = 10
-                ques = batch["ques_fwd"].reshape(-1, batch.c.Tq)
-                N = encOut.shape[0]
-                layers = [eng.encoder_rnn_state(l, N) for l in range(2)]
-                has_layers = layers[0][0] is not None
-                encH = [(layers[l][0].numpy(), layers[l][1].numpy()) for l in range(2)] if has_layers else None
-                threadAnswers = []
-
-                def step(tokens, Hs, Cs):
-                    n = len(tokens)
-                    for i, a in enumerate(Hs + Cs):
-                        eng.upload(state_buf[i], a[:n])
-                    return eng.gen_decoder_step(tokens, state_buf[0:2], state_buf[2:4])
-
-                # the reference's own loop structure (one round at a time, log-probabilities and state through the host):
-                # kept as the cross-check of the device search (params.hostBeam = 1)
-                for it in range(N):                                                 # :472
-                    beams = np.zeros((beamLen, beamSize), dtype=np.int64)           # :479
-                    if has_layers:                                                  # :482-491
-                        Hs = [encH[0][0][it], encOut[it]]
-                        Cs = [encH[0][1][it], encH[1][1][it]]
-                    else:                                                           # :493-501
-                        Hs = [np.zeros(H, np.float32), encOut[it]]
-                        Cs = [np.zeros(H, np.float32), np.zeros(H, np.float32)]
-                    Hs = [np.repeat(h[None], beamSize, 0).astype(np.float32) for h in Hs]
-                    Cs = [np.repeat(c[None], beamSize, 0).astype(np.float32) for c in Cs]
-                    beams[0] = startToken                                           # :506
-                    scores = np.zeros(beamSize, dtype=np.float64)                   # :507
-                    finishBeams = []
-                    for stp in range(1, beamLen):                                   # :510
-                        cands = []
-                        exploreSize = 1 if stp == 1 else beamSize                   # :516
-                        decOut, nH, nC = step(beams[stp - 1], Hs, Cs)               # :519-526
-                        for wordId in range(exploreSize):                           # :529
-                            order = np.argsort(-decOut[wordId], kind="stable")[:beamSize]   # :538-542 topk, sorted
-                            for candId in range(beamSize):                          # :544
-                                candBeam = beams[:, wordId].copy()
-                                tok = int(order[candId]) + 1
-                                candBeam[stp] = tok
-                                sc = float(scores[wordId]) + float(decOut[wordId, order[candId]])
-                                if tok == endToken:                                 # :548
-                                    finishBeams.append({"beam": candBeam, "length": stp + 1, "score": sc})
-                                else:
-                                    cands.append((sc, candBeam, [h[wordId].copy() for h in nH], [c[wordId].copy() for c in nC]))
-                        cands.sort(key=lambda t: -t[0])                             # :558
-                        for candId in range(min(len(cands), beamSize)):             # :560-569
-                            beams[:, candId] = cands[candId][1]
-                            for lv in range(2):
-                                Hs[lv][candId] = cands[candId][2][lv]
-                                Cs[lv][candId] = cands[candId][3][lv]
-                            scores[candId] = cands[candId][0]
-                    finishBeams.sort(key=lambda d: -d["score"])                     # :572
-                    if not finishBeams:
-                        if strict:
-                            raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
-                        threadAnswers.append(None)
-                        continue
-                    best = finishBeams[0]
-                    threadAnswers.append(entry(ques[it], best["beam"], best["score"], best["length"]))
-                self.wrapper.training()                                                 # :605
-                answerTable.append({"image_id": image_id(convId), "dialog": threadAnswers})   # :606
-        finally:
-            for p in state_buf:
-                eng.device_free(p)
-        return answerTable
-
-    def _generate_beam(self, dataloader, dtype, numThreads, dialogsPerCall, beamSize, beamLen, startToken, endToken, strict,
-                       image_id, entry):
-        """generateAnswers' beam search, `dialogsPerCall` dialogs per encoder forward and per vd_gen_beam_search call.  One
-        dialog per call gives exactly the per-dialog trimming and kernel shapes of the reference's loop; more dialogs per call
-        run wider kernels (in the tensor-core math modes their rounding can differ from per-dialog runs)."""
         answerTable = []
         ques_len = None
         for first in range(0, numThreads, dialogsPerCall):
@@ -324,52 +239,30 @@ class Model:
             self.forwardBackward(batch, True, True)                                     # :467
             ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
             Tq = ques.shape[2]
-            answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)   # :472-579
-            answer = answer.reshape(len(inds), -1, beamLen)
-            length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
-            self.wrapper.training()                                                     # :605
-            for d, convId in enumerate(inds):
-                w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
-                threadAnswers = []
-                for it in range(ques.shape[1]):
-                    if length[d, it] == 0:
-                        if strict:
-                            raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
-                        threadAnswers.append(None)
-                        continue
-                    threadAnswers.append(entry(ques[d, it, Tq - w:], answer[d, it], float(score[d, it]), int(length[d, it])))
-                answerTable.append({"image_id": image_id(int(convId)), "dialog": threadAnswers})   # :606
-        return answerTable
-
-    def _generate_sample(self, dataloader, dtype, numThreads, dialogsPerCall, beamLen, startToken, temperature, seed,
-                         split_offset, image_id, words):
-        """generateAnswers' sampling (model.lua:581-602), `dialogsPerCall` dialogs per encoder forward and per vd_gen_sample
-        call.  The draws of a round depend only on (seed, its global round index, the step): the call passes the index of
-        its first round in the split (this rank's offset included), so the answers do not depend on dialogsPerCall or on
-        how the split is sharded over ranks, only on the logits."""
-        R = self.params["maxQuesCount"]
-        answerTable = []
-        ques_len = None
-        for first in range(0, numThreads, dialogsPerCall):
-            inds = np.arange(first, min(numThreads, first + dialogsPerCall))
-            self.wrapper.evaluate()                                                     # :460
-            batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
-            self.forwardBackward(batch, True, True)                                     # :467
-            ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
-            Tq = ques.shape[2]
-            answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, (split_offset + first) * R)   # :582-594
-            answer = answer.reshape(len(inds), -1, beamLen + 1)
+            if sampleWords:                                                             # :582-594
+                answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed,
+                                                   (offset + first) * self.params["maxQuesCount"])
+            else:                                                                       # :472-579
+                answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
+                length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
+            answer = answer.reshape(len(inds), -1, answer.shape[1])
             self.wrapper.training()                                                     # :605
             for d, convId in enumerate(inds):
                 w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
                 threadAnswers = []
                 for it in range(ques.shape[1]):
                     q, a = ques[d, it, Tq - w:], answer[d, it]
-                    e = {"question": q.tolist(), "answer": a.tolist()}
-                    if words:
-                        e["question_text"], e["answer_text"] = words(q), words(a)
-                    threadAnswers.append(e)
-                answerTable.append({"image_id": image_id(int(convId)), "dialog": threadAnswers})   # :606
+                    if sampleWords:
+                        threadAnswers.append(entry(q, a))
+                    elif length[d, it] > 0:
+                        threadAnswers.append(entry(q, a, score=float(score[d, it]), length=int(length[d, it])))
+                    elif strict:
+                        raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
+                    else:
+                        threadAnswers.append(None)
+                gid = offset + int(convId)
+                answerTable.append({"image_id": _image_id(img[gid]) if img is not None else gid,
+                                    "dialog": threadAnswers})                           # :606
         return answerTable
 
     # ---- checkpoints (train.lua:33-34,78-80,99-102,120-121; evaluate.lua:58-91) -------------------------------
