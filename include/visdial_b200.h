@@ -189,6 +189,26 @@ int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_
  * > 0, row_offset >= 0, 1 <= start_token <= vocabSize and answer_host != NULL. */
 int vd_gen_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
                   int32_t* answer_host, float* logp_host);
+/* Dialogs on the model's own answers (DESIGN §17): for every dialog of batch b (gen, history encoders), round by round
+ * r = 0 .. maxQuesCount-1, the encoder forward in eval mode on a history whose rows 0..r hold the batch's caption row, the
+ * batch's questions and the answers the call generated for the earlier rounds, then vd_gen_beam_search's search (or
+ * vd_gen_sample's draw) on round r's rows only, then round r's write into history row r+1 by dataloader.lua:202-278's rule:
+ * Q ++ A right-aligned, or for the concatenated history of the late-fusion encoders row r ++ <END> ++ Q ++ A.  A = the
+ * non-pad words between <START> and <END> of the best finished hypothesis (empty when none finished), or the samples before
+ * the first end_token, cut to their first max_ans_len words; a question of pads only writes no Q and no A.  History rows
+ * are hist_width wide and keep their rightmost hist_width words.  The whole loop is enqueued on the device: one
+ * synchronisation, at the end.
+ * Outputs are those of vd_gen_beam_search / vd_gen_sample for the N = B * maxQuesCount rounds of the batch; sampled round r
+ * of dialog b draws as global round row_offset + b * maxQuesCount + r.  hist_host: NULL or (B, maxQuesCount, hist_width)
+ * int32, the history rows the encoder read.
+ * VD_E_STATE for a disc engine or an encoder without history; VD_E_BADARG for the arguments vd_gen_beam_search /
+ * vd_gen_sample refuse, hist_width < b->Th or max_ans_len < 1 (and end_token outside [1, vocabSize] when sampling). */
+int vd_gen_dialog_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size, int32_t beam_len, int32_t start_token,
+                              int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
+                              int32_t* length_host, double* score_host, int32_t* hist_host);
+int vd_gen_dialog_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t hist_width, int32_t max_ans_len,
+                         int32_t* answer_host, float* logp_host, int32_t* hist_host);
 
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.

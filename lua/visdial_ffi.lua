@@ -43,6 +43,12 @@ int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_
                        int32_t* answer_host, int32_t* length_host, double* score_host);
 int vd_gen_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
                   int32_t* answer_host, float* logp_host);
+int vd_gen_dialog_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size, int32_t beam_len, int32_t start_token,
+                              int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
+                              int32_t* length_host, double* score_host, int32_t* hist_host);
+int vd_gen_dialog_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t hist_width, int32_t max_ans_len,
+                         int32_t* answer_host, float* logp_host, int32_t* hist_host);
 int vd_clamp_adam_step(vd_engine* e, float learning_rate);
 int vd_comm_unique_id(void* id_out);
 int vd_comm_init(vd_engine* e, const void* id, int32_t rank, int32_t world);

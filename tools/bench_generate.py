@@ -7,10 +7,18 @@
   sample/<d>   sampling: vd_gen_sample, d dialogs per encoder forward and call
   host_sample  sampling as the engine ran it before it moved to the device: per dialog and step, the state up, one
                vd_gen_decoder_step, the log-probabilities and state down, one numpy categorical draw per round (host_sample)
+Dialogs on the model's own answers (history "generated", DESIGN §17; kinds dialog-beam, dialog-sample; history encoders):
+  dialog/<d>         vd_gen_dialog_beam_search, d dialogs per call
+  host_dialog/<d>    the loop a user would otherwise write: per round, the history rebuilt on the host, the batch uploaded,
+                     the encoder forward and vd_gen_beam_search over all the batch's rounds, one round kept (10 calls)
+  enc/<d>            the device loop's 10 encoder forwards alone (same batch and history width), for the encoder's share
+  dsample/<d>        vd_gen_dialog_sample, d dialogs per call
+  host_dsample/<d>   the host loop with vd_gen_sample
 Every path is warmed up at its shape first, then timed over whole calls until the window lasts at least --window seconds
 (host clock; every call ends in a device synchronisation).  Prints one JSON line per (encoder, mode, path) and the card's name
 and power limit, read in the same run.
-usage: python tools/bench_generate.py [--encoders a,b] [--modes f16,fp32] [--dpc 1,8,32,128] [--kinds beam,sample]
+usage: python tools/bench_generate.py [--encoders a,b] [--modes f16,fp32] [--dpc 1,8,32,128]
+                                      [--kinds beam,sample,dialog-beam,dialog-sample]
                                       [--window 1.0] [--out FILE]"""
 import argparse
 import json
@@ -29,6 +37,8 @@ from visdial_b200.dataloader import Dataloader  # noqa: E402
 from visdial_b200.engine import DEFAULT_PARAMS, derive_flags  # noqa: E402
 from visdial_b200.synthetic import make_corpus  # noqa: E402
 from host_decode import HostStep, host_beam_search, start_state  # noqa: E402
+from dialog_history import beam_words, next_row, right_aligned, row_words, sample_words  # noqa: E402
+from visdial_b200.engine import Batch  # noqa: E402
 
 BEAM, LEN, V = 5, 20, 10000
 
@@ -57,6 +67,49 @@ def host_sample(eng, encOut, L, start, T, rng):
             tok = np.array([rng.choice(p.shape[1], p=p[i]) + 1 for i in range(len(tok))], dtype=np.int64)
             seq.append(tok.copy())
     return np.stack(seq, 1)
+
+
+def hist_width(dl):
+    """the history width generateAnswers passes for generated history"""
+    return dl.maxHistoryLen if dl.concatHistory else min(dl.maxQuesLen + dl.maxAnsLen, dl.maxHistoryLen)
+
+
+def host_dialog(m, dl, d, start, end, sample):
+    """d dialogs on their own answers with one engine call per round: the history rebuilt and uploaded every round"""
+    m.wrapper.evaluate()
+    nb = dl.getIndexData(np.arange(d), m.params, "val").numpy()
+    B, R = nb["ques_fwd"].shape[:2]
+    W, mal = hist_width(dl), dl.maxAnsLen
+    hist = np.zeros((B, R, W), np.int32)
+    for b in range(B):
+        hist[b, 0] = right_aligned(row_words(nb["hist"][b, 0]), W)
+    for r in range(R):
+        m.engine.encoder_forward(Batch(dict(nb, hist=hist)))
+        if sample:
+            ans, _ = m.engine.gen_sample(LEN, start, 1.0, 1234, 0)
+            words = [sample_words(ans[b * R + r], end) for b in range(B)]
+        else:
+            ans, length, _ = m.engine.gen_beam_search(BEAM, LEN, start, end)
+            words = [beam_words(ans[b * R + r], length[b * R + r]) for b in range(B)]
+        if r + 1 < R:
+            for b in range(B):
+                hist[b, r + 1] = next_row(hist[b, r], row_words(nb["ques_fwd"][b, r]), words[b], dl.concatHistory, end, W, mal)
+    m.wrapper.training()
+
+
+def encoders_only(m, dl, d):
+    """the device loop's R encoder forwards on d dialogs at the loop's history width"""
+    m.wrapper.evaluate()
+    nb = dl.getIndexData(np.arange(d), m.params, "val").numpy()
+    B, R = nb["ques_fwd"].shape[:2]
+    W = hist_width(dl)
+    hist = np.zeros((B, R, W), np.int32)
+    hist[:, :, W - nb["hist"].shape[2]:] = nb["hist"]
+    b = Batch(dict(nb, hist=hist)).to_device(m.engine)
+    for _ in range(R):
+        m.engine.encoder_forward(b)
+    m.engine.synchronize()
+    m.wrapper.training()
 
 
 def window(call, dialogs_per_call, seconds):
@@ -88,7 +141,8 @@ def main():
         p = dict(DEFAULT_PARAMS)
         p.update(encoder=enc, decoder="gen", vocabSize=V, imgFeatureSize=512 if "att" in enc else 4096, batchSize=1)
         p = derive_flags(p)
-        raw = make_corpus(p, max(dpcs), 2000, seed=5)
+        raw = make_corpus(p, max(dpcs), 2000, seed=5, ques_len_cap=8 if p["concatHistory"] else None,
+                          ans_len_cap=8 if p["concatHistory"] else None)
         m = Model(p, seed=3)
         dl = Dataloader(m.engine).initialize(dict(p, maxHistoryLen=60), ["val"], {"val": raw})
         start, end = dl.word2ind["<START>"], dl.word2ind["<END>"]
@@ -122,6 +176,17 @@ def main():
                 paths += [("sample/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(samp, maxThreads=d, dialogsPerCall=d)))
                           for d in dpcs]
                 paths += [("host_sample", 1, host_samp)]
+            dialog = {"history": "generated", "beamSize": BEAM, "beamLen": LEN}
+            if "dialog-beam" in kinds:
+                paths += [("dialog/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(dialog, maxThreads=d, dialogsPerCall=d),
+                                                                             strict=False)) for d in dpcs]
+                paths += [("host_dialog/%d" % d, d, lambda d=d: host_dialog(m, dl, d, start, end, False)) for d in dpcs]
+                paths += [("enc/%d" % d, d, lambda d=d: encoders_only(m, dl, d)) for d in dpcs]
+            if "dialog-sample" in kinds:
+                paths += [("dsample/%d" % d, d, lambda d=d: m.generateAnswers(dl, "val", dict(dialog, sampleWords=1,
+                                                                                              maxThreads=d, dialogsPerCall=d)))
+                          for d in dpcs]
+                paths += [("host_dsample/%d" % d, d, lambda d=d: host_dialog(m, dl, d, start, end, True)) for d in dpcs]
             for path, d, call in paths:
                 ms, n, dt = window(call, d, a.window)
                 r = {"encoder": enc, "mode": mode, "path": path, "ms_per_dialog": round(ms, 3), "dialogs_timed": n,
@@ -130,7 +195,7 @@ def main():
                 rows.append(r)
         dl.close(); m.engine.close()
     print("\n%s, power limit %s: ms per dialog (beam %d x %d / sampling x %d, V = %d)" % (name, power, BEAM, LEN, LEN, V))
-    order = ["device", "host_search", "sample", "host_sample"]
+    order = ["device", "host_search", "sample", "host_sample", "dialog", "host_dialog", "enc", "dsample", "host_dsample"]
     paths = sorted({r["path"] for r in rows}, key=lambda s: (order.index(s.split("/")[0]), int(s.split("/")[1]) if "/" in s else 0))
     print("| encoder | mode | " + " | ".join(paths) + " |")
     print("|---|---|" + "---|" * len(paths))

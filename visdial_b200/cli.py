@@ -79,6 +79,11 @@ GENERATE_OPTIONS = [
     ("backend", "cudnn", "nn|cudnn (accepted, no effect)"),
     ("dialogsPerCall", 1, "Dialogs per encoder forward and device search call (1 = the reference's per-dialog loop)"),
 ]
+# the generate command's table: generate.lua's options above, and which history each round is answered with
+HISTORY_MODES = ("gt", "generated")
+GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + [
+    ("history", "gt", "History each round is answered with: gt (the dataset's) | generated (the dialog's own answers)"),
+]
 
 # options of every command that the reference does not have: how the run is spread over GPUs and which math it uses
 MATH_MODES = ("fp32", "tf32", "f16")
@@ -128,6 +133,8 @@ def parse(options, argv=None, prog=None) -> dict:
         i += 2
     if opt["math"] not in MATH_MODES:
         fail("-math is one of %s" % "|".join(MATH_MODES))
+    if "history" in opt and opt["history"] not in HISTORY_MODES:
+        fail("-history is one of %s" % "|".join(HISTORY_MODES))
     if opt["gpus"] < 1:
         fail("-gpus must be at least 1")
     if opt["gpuid"] < 0:

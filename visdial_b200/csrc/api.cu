@@ -261,6 +261,20 @@ int vd_gen_sample(vd_engine* h, int32_t beam_len, int32_t start_token, float tem
   VD_TRY({ ENG(h)->gen_sample(beam_len, start_token, temperature, seed, row_offset, answer_host, logp_host); })
 }
 
+int vd_gen_dialog_beam_search(vd_engine* h, const vd_batch* b, int32_t beam_size, int32_t beam_len, int32_t start_token,
+                              int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
+                              int32_t* length_host, double* score_host, int32_t* hist_host) {
+  VD_TRY({ ENG(h)->gen_dialog_beam_search(b, beam_size, beam_len, start_token, end_token, hist_width, max_ans_len, answer_host,
+                                          length_host, score_host, hist_host); })
+}
+
+int vd_gen_dialog_sample(vd_engine* h, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t hist_width, int32_t max_ans_len,
+                         int32_t* answer_host, float* logp_host, int32_t* hist_host) {
+  VD_TRY({ ENG(h)->gen_dialog_sample(b, beam_len, start_token, end_token, temperature, seed, row_offset, hist_width, max_ans_len,
+                                     answer_host, logp_host, hist_host); })
+}
+
 int vd_clamp_adam_step(vd_engine* h, float lr) { VD_TRY({ ENG(h)->clamp_adam_step(lr); }) }
 
 int vd_comm_unique_id(void* id_out) { VD_TRY({ NOTNULL(id_out); vd::comm_unique_id(id_out); }) }

@@ -90,8 +90,9 @@ enum : uint32_t {
 // Sampling (Engine::gen_sample, model.lua:584-602) by the Gumbel-max trick: the token drawn from step `step`'s row r is
 // 1 + argmax_j (x_j / T + g_j), x = the vocabulary logits with bias, ties to the lower class.  g_j = -log(-log(u_j)),
 // u_j = ((w >> 8) + 0.5) 2^-24, w = Philox4x32-10 word idx % 4 at counter (idx/4 lo, idx/4 hi, SITE_SAMPLE, step), key =
-// seed, idx = (row_offset + r) V + j: the element index of the step's (rows, V) decOut over the whole split, so a draw
-// depends only on (seed, global round, step, class).  Exactly a draw from softmax(x / T) = exp(logp / T) / sum.  Every
+// seed, idx = (row_offset + r row_stride) V + j: the element index of the step's (rows, V) decOut over the whole split, so a
+// draw depends only on (seed, global round, step, class).  row_stride = 1 when the rows are consecutive rounds; the dialog
+// loop (Engine::gen_dialog) samples round r of B dialogs, rows b R + r, with row_offset = first round + r and stride R.  Exactly a draw from softmax(x / T) = exp(logp / T) / sum.  Every
 // device route evaluates the key with these full-precision functions, so equal logits give equal tokens on every route.
 // The numpy twin is tests/sampling_twin.py.
 // ---------------------------------------------------------------------------------------------
@@ -99,6 +100,7 @@ struct SampleCfg {
   uint32_t seed_lo, seed_hi, step;
   float temperature;
   int64_t row_offset;       // global round of row 0
+  int64_t row_stride;       // global rounds between consecutive rows
 };
 // largest Gumbel value the rule can produce (u = 1 - 2^-25: -log(-log u) = 17.33): an element whose x / T + GUMBEL_MAX is
 // below the best key so far cannot win, so its Philox word and logarithms need not be computed

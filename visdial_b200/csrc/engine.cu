@@ -212,6 +212,8 @@ Engine::~Engine() {
   arena.release();
   for (auto& g : stage) g.release();
   for (auto& g : dense_buf) g.release();
+  dialog_hist.release();
+  for (auto& g : dialog_out) g.release();
   if (copy_stream) {
     cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream);
     cudaEventDestroy(ev_img_ready); cudaEventDestroy(ev_copy_fork);
@@ -1516,10 +1518,7 @@ void Engine::gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float
   lstm_forward(gstep2, true);
 }
 
-// Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once: row n*k + j is
-// hypothesis j of round n.  Every step runs on device-resident tokens and parents: the state gather, the decoder step of
-// gen_decoder_step_logits, the fused log-softmax + top-k and the candidate merge, which writes the next step's tokens and
-// parents.  Nothing returns to the host until the final copy of each round's best finished hypothesis.
+// Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once.
 void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
                              double* score_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_search needs the gen decoder after encoder_forward");
@@ -1527,9 +1526,24 @@ void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
+  const int64_t N = db.N;
+  const BeamResult res = beam_search_rows(N, 1, 0, k, L, start_token, end_token);
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+// The search itself, enqueued on cx.stream, for n rounds whose start state is row i * stride + off of the last encoder
+// forward (i < n; stride 1, off 0: every round): row i*k + j is hypothesis j of round i.  Every step runs on device-resident
+// tokens and parents: the state gather, the decoder step of gen_decoder_step_logits, the fused log-softmax + top-k and the
+// candidate merge, which writes the next step's tokens and parents.  Returns each round's best finished hypothesis in the
+// arena (n rows), valid until the next encoder forward.
+Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int L, int start_token,
+                                            int end_token) {
   forward_connect();
   const int H = cfg.H;
-  const int64_t N = db.N, rows = N * k;
+  const int64_t N = n, rows = N * k;
   // allocated once per call.  Two sets of fed states {h1, h2, c1, c2}: the gather of step s reads the set step s-1 was
   // fed (a column that got no candidate keeps it) and writes the other; beams / scores ping-pong because the merge fills
   // columns from the pre-merge beams.
@@ -1552,7 +1566,7 @@ void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32
   // without .rnnLayers feed explicit zero rows, not "no initial state": the first step's kernels differ between the two.
   const float* init[4] = {gen_h0[0], gen_h0[1], gen_c0[0], gen_c0[1]};
   for (int i = 0; i < 4; ++i) {
-    if (init[i]) repeat_rows(cx, st[0][i], init[i], N, k, H);
+    if (init[i]) repeat_rows(cx, st[0][i], init[i] + off * H, N, k, H, stride * H);
     else VD_CUDA_CHECK(cudaMemsetAsync(st[0][i], 0, (size_t)rows * H * sizeof(float), cx.stream));
   }
   beam_init(cx, rows, L, start_token, beams[0], tok, scores[0]);
@@ -1572,28 +1586,41 @@ void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32
     beam_merge(cx, N, stp, k, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, ans, ans_len,
                ans_score);
   }
-  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, ans_len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, ans_score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  return {ans, ans_len, ans_score};
 }
 
 // Model:generateAnswers' sampling (model.lua:581-602) for all N rounds of the last encoder forward at once, on the device.
-// Every step runs the decoder step of gen_decoder_step_logits on the device-resident tokens, then draws with the Gumbel-max
-// rule of common.cuh: fused into the vocabulary projection's epilogue (tensor-core modes, vocab_tc_ok's shapes) or from
-// materialised logits (k_logsoftmax_sample_rows).  The draw writes the next step's tokens, so nothing returns to the host
-// until the final copy of the answers and log-probabilities.
 void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
                         float* logp_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_sample needs the gen decoder after encoder_forward");
-  VD_REQUIRE(L >= 1 && std::isfinite(temperature) && temperature > 0.f && row_offset >= 0 && start_token >= 1 &&
-             start_token <= cfg.V, VD_E_BADARG, "beam_len >= 1, finite temperature > 0, row_offset >= 0, start_token in [1, V]");
+  check_sample_args(L, start_token, temperature, row_offset);
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
+  const int64_t N = db.N;
+  const SampleResult res = sample_rows(N, 1, 0, L, start_token, temperature, seed, row_offset);
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)N * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  if (logp_host)
+    VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)N * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+void Engine::check_sample_args(int L, int start_token, float temperature, int64_t row_offset) const {
+  VD_REQUIRE(L >= 1 && std::isfinite(temperature) && temperature > 0.f && row_offset >= 0 && start_token >= 1 &&
+             start_token <= cfg.V, VD_E_BADARG, "beam_len >= 1, finite temperature > 0, row_offset >= 0, start_token in [1, V]");
+}
+
+// The sampling itself, enqueued on cx.stream, for n rounds whose start state is row i * stride + off of the last encoder
+// forward; search row i draws as global round row_offset + i * stride + off.  Every step runs the decoder step of
+// gen_decoder_step_logits on the device-resident tokens, then draws with the Gumbel-max rule of common.cuh: fused into the
+// vocabulary projection's epilogue (tensor-core modes, vocab_tc_ok's shapes) or from materialised logits
+// (k_logsoftmax_sample_rows).  The draw writes the next step's tokens, so nothing waits for the host.  Returns the answers
+// (n, L + 1) and log-probabilities (n, L) in the arena, valid until the next encoder forward.
+Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature,
+                                         uint64_t seed, int64_t row_offset) {
   forward_connect();
   const int H = cfg.H, V = cfg.V;
-  const int64_t N = db.N;
+  const int64_t N = n;
   const int wo = seg("dec.out.weight");
   // allocated once per call
   float* zero = arena.get<float>(N * H);
@@ -1614,7 +1641,16 @@ void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed
   // rows, not "no initial state", as gen_beam_search does
   const float* h[2] = {gen_h0[0] ? gen_h0[0] : zero, gen_h0[1]};
   const float* c[2] = {gen_c0[0] ? gen_c0[0] : zero, gen_c0[1] ? gen_c0[1] : zero};
-  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset};
+  if (stride != 1 || off != 0) {                     // the start state's rows i * stride + off, gathered once
+    const float** init[4] = {&h[0], &h[1], &c[0], &c[1]};
+    for (const float** p : init) {
+      if (*p == zero) continue;
+      float* t = arena.get<float>(N * H);
+      repeat_rows(cx, t, *p + off * H, N, 1, H, stride * H);
+      *p = t;
+    }
+  }
+  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset + off, stride};
   // The step's decoder buffers alternate between two arena regions: step s reads the state step s-1 wrote into the other
   // one, so the new state feeds the next step without a copy.  Same allocations every step, so a region lands where it
   // did two steps earlier and the arena does not grow with L.
@@ -1643,6 +1679,95 @@ void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed
     h[0] = gstep1.h; h[1] = gstep2.h;
     c[0] = gstep1.c; c[1] = gstep2.c;
   }
+  return {ans, lp};
+}
+
+// Dialogs on the model's own answers (DESIGN §17): for r = 0 .. R-1, the encoder forward in eval mode on the batch with the
+// engine-owned history (B, R, W), the search of round r's rows b*R + r only, its answers written into the outputs' rows
+// b*R + r, and the history append of round r+1.  Everything is enqueued on the main stream; the batch's questions and
+// image are staged once and the host waits only for the final copies.  `search(r)` enqueues round r's search and says where
+// its answers are (DialogAnswers).
+void Engine::gen_dialog(const vd_batch* b, int W, int max_ans_len, const std::function<DialogAnswers(int)>& search,
+                        int32_t* hist_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN && cfg.useHist, VD_E_STATE, "dialog generation needs the gen decoder and a history encoder");
+  VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0 && b->Th > 0, VD_E_SHAPE, "batch with B, Tq and Th > 0");
+  VD_REQUIRE(W >= b->Th && max_ans_len >= 1, VD_E_BADARG, "hist_width >= the batch's Th, max_ans_len >= 1");
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  cx.stream = main_stream;
+  const int saved_training = training;
+  training = 0;
+  try {
+    stage_batch(b);
+    wait_img();                                      // the rounds' batch aliases the staged image
+    const int R = cfg.R, B = db.B;
+    const int64_t N = db.N;
+    int32_t* hist = (int32_t*)dialog_hist.ensure((size_t)N * W * sizeof(int32_t));
+    hist_append(cx, hist, B, R, W, -1, db.hist, db.Th, nullptr, 0, nullptr, 0, 0, 0, false);   // round 0 <- the caption row
+    vd_batch rb = {};
+    rb.B = B; rb.Tq = db.Tq; rb.Th = W; rb.ques_fwd = db.ques; rb.hist = hist; rb.img_feat = db.img; rb.on_device = 1;
+    for (int r = 0; r < R; ++r) {
+      encoder_forward(&rb);
+      const DialogAnswers a = search(r);
+      if (r + 1 < R)
+        hist_append(cx, hist, B, R, W, r, rb.ques_fwd, rb.Tq, a.tokens, a.ld, a.len, a.max_tokens, a.end_token, max_ans_len,
+                    cfg.fam_lf);             // the late-fusion encoders read concatenated history (opts.lua:59)
+    }
+    if (hist_host)
+      VD_CUDA_CHECK(cudaMemcpyAsync(hist_host, hist, (size_t)N * W * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  } catch (...) { training = saved_training; throw; }
+  training = saved_training;
+}
+
+// copies round r's n = B result rows (row pitch `bytes`) into rows b*R + r of an engine-owned (B*R, bytes) output
+static void scatter_round(cudaStream_t s, void* dst, const void* src, size_t bytes, int R, int r, int64_t B) {
+  VD_CUDA_CHECK(cudaMemcpy2DAsync((char*)dst + (size_t)r * bytes, (size_t)R * bytes, src, bytes, bytes, (size_t)B,
+                                  cudaMemcpyDeviceToDevice, s));
+}
+
+void Engine::gen_dialog_beam_search(const vd_batch* b, int k, int L, int start_token, int end_token, int W, int max_ans_len,
+                                    int32_t* answer_host, int32_t* length_host, double* score_host, int32_t* hist_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_beam_search needs the gen decoder");
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
+  VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
+  const int R = cfg.R;
+  const int64_t B = b->B, N = B * R;
+  int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)N * L * sizeof(int32_t));
+  int32_t* len = (int32_t*)dialog_out[1].ensure((size_t)N * sizeof(int32_t));
+  double* score = (double*)dialog_out[2].ensure((size_t)N * sizeof(double));
+  gen_dialog(b, W, max_ans_len, [&](int r) {
+    const BeamResult res = beam_search_rows(B, R, r, k, L, start_token, end_token);
+    scatter_round(cx.stream, ans, res.ans, (size_t)L * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, len, res.len, sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, score, res.score, sizeof(double), R, r, B);
+    // the tokens between <START> and the hypothesis' <END>
+    return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
+  }, hist_host);
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+void Engine::gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
+                               int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host,
+                               int32_t* hist_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_sample needs the gen decoder");
+  check_sample_args(L, start_token, temperature, row_offset);
+  VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
+  VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
+  VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
+  const int R = cfg.R;
+  const int64_t B = b->B, N = B * R;
+  int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)N * (L + 1) * sizeof(int32_t));
+  float* lp = (float*)dialog_out[3].ensure((size_t)N * L * sizeof(float));
+  gen_dialog(b, W, max_ans_len, [&](int r) {
+    const SampleResult res = sample_rows(B, R, r, L, start_token, temperature, seed, row_offset);
+    scatter_round(cx.stream, ans, res.ans, (size_t)(L + 1) * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, lp, res.logp, (size_t)L * sizeof(float), R, r, B);
+    // the samples before the first <END>
+    return DialogAnswers{res.ans + 1, L + 1, nullptr, L, end_token};
+  }, hist_host);
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   if (logp_host)
     VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, lp, (size_t)N * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));

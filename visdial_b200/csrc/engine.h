@@ -1,6 +1,7 @@
 // Engine: owns parameters, activations and the per-batch forward/backward orchestration that
 // replaces Model:forwardBackward / Model:retrieveBatch (/root/reference/model.lua:249-430).
 #pragma once
+#include <functional>
 #include <string>
 #include <vector>
 #include "../../include/visdial_b200.h"
@@ -298,11 +299,33 @@ struct Engine {
   void gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device
   void gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
+  // its search on n rounds whose start state is row i * stride + off of the last encoder forward; results in the arena
+  struct BeamResult { int32_t* ans; int32_t* len; double* score; };     // (n, L), (n), (n)
+  BeamResult beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int L, int start_token, int end_token);
   // the decoder step up to the second LSTM layer (gstep1 / gstep2 hold the new state on return)
   void gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // Model:generateAnswers' sampling for every round of the last encoder forward, entirely on the device
   void gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
                   float* logp_host);
+  void check_sample_args(int L, int start_token, float temperature, int64_t row_offset) const;
+  // its sampling on n rounds as beam_search_rows takes them; row i draws as global round row_offset + i * stride + off
+  struct SampleResult { int32_t* ans; float* logp; };                   // (n, L + 1), (n, L)
+  SampleResult sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature, uint64_t seed,
+                           int64_t row_offset);
+  // dialogs on the model's own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample): R rounds of {encoder forward on
+  // the engine-owned history, round r's search, the history append} on the device
+  struct DialogAnswers {             // where round r's answers are, for the history append
+    const int32_t* tokens; int64_t ld;   // row b's answer tokens start at tokens + b * ld
+    const int32_t* len;              // beam: hypothesis lengths (the tokens are len - 2 words); null: sampling
+    int max_tokens;                  // sampling: the words per row (cut at the first end_token)
+    int end_token;
+  };
+  GrowBuf dialog_hist, dialog_out[4];   // (B, R, W) history; answers, lengths, scores / log-probabilities of all rounds
+  void gen_dialog(const vd_batch* b, int W, int max_ans_len, const std::function<DialogAnswers(int)>& search, int32_t* hist_host);
+  void gen_dialog_beam_search(const vd_batch* b, int k, int L, int start_token, int end_token, int W, int max_ans_len,
+                              int32_t* answer_host, int32_t* length_host, double* score_host, int32_t* hist_host);
+  void gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
+                         int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host, int32_t* hist_host);
   void clamp_adam_step(float lr);
   void allreduce_grads();
   // Overlapped gradient sync (world > 1): dW is all-reduced in buckets on `comm_stream` as soon as each bucket's last

@@ -76,7 +76,8 @@ void tanh_bwd(LaunchCtx& cx, float* dpre, const float* dy, const float* y, int64
 void add_inplace(LaunchCtx& cx, float* a, const float* b, int64_t n);
 void add_out(LaunchCtx& cx, float* out, const float* a, const float* b, int64_t n);
 void copy_cols(LaunchCtx& cx, float* dst, int64_t ldd, const float* src, int64_t lds, int64_t rows, int cols);
-void repeat_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols);      // model.lua:267-269
+// model.lua:267-269: dst row n <- src row n / R; src rows lds apart (lds < 0: cols, contiguous)
+void repeat_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols, int64_t lds = -1);
 void sum_repeated_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols);
 void transpose_segments(LaunchCtx& cx, const float* W, float* Wt, const int64_t* seg_table_dev, int nseg,
                         int64_t max_elems);
@@ -155,6 +156,14 @@ void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int L, int end_token, 
 // the bits it would give), the Gumbel-max draw of common.cuh; writes as vocab_sample_finish
 void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,
                             int32_t* answer, float* logp);
+// the dialog loop's history (Engine::gen_dialog), one CTA per dialog b of hist (B, R, W), right-aligned rows.
+// r < 0: row 0 <- row b*R of src (B*R, src_w), right-aligned into W >= src_w; rows 1.. <- pads.
+// r >= 0: row r+1 <- round r's write (DESIGN §17): Q = the words of question row b*R + r of src (B*R, src_w), A = the first
+// max_ans_len non-pad words of ans + b*ans_ld before the first end_token, of ans_len[b] - 2 words (ans_len null: ans_max);
+// an empty Q empties A.  Per-round: Q ++ A; concat: row r ++ <END> ++ Q ++ A; the rightmost W words.  An empty row r leaves
+// row r+1 empty (rightAlign's break, utils.lua:20-22).
+void hist_append(LaunchCtx& cx, int32_t* hist, int64_t B, int R, int W, int r, const int32_t* src, int src_w, const int32_t* ans,
+                 int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat);
 
 // ---- optimiser (model.lua:96-99, optim_updates.lua:62-91) ------------------------------------------
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1,

@@ -348,11 +348,62 @@ __global__ void k_copy_cols(float* __restrict__ dst, int64_t ldd, const float* _
   int64_t r = i / cols; int c = (int)(i % cols);
   dst[r * ldd + c] = src[r * lds + c];
 }
-__global__ void k_repeat_rows(float* __restrict__ dst, const float* __restrict__ src, int64_t B, int R, int64_t cols) {
+__global__ void k_repeat_rows(float* __restrict__ dst, const float* __restrict__ src, int64_t B, int R, int64_t cols,
+                              int64_t lds) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * R * cols) return;
   int64_t n = i / cols, c = i % cols;
-  dst[i] = src[(n / R) * cols + c];
+  dst[i] = src[(n / R) * lds + c];
+}
+
+// the dialog loop's history rows (hist_append in kernels.cuh), one CTA per dialog
+__global__ void k_hist_append(int32_t* __restrict__ hist, int R, int W, int r, const int32_t* __restrict__ src, int src_w,
+                              const int32_t* __restrict__ ans, int64_t ans_ld, const int32_t* __restrict__ ans_len, int ans_max,
+                              int end_token, int max_ans_len, int concat) {
+  extern __shared__ int32_t a_s[];                        // the answer's kept words (max_ans_len)
+  __shared__ int s_len[3];
+  const int64_t b = blockIdx.x;
+  int32_t* rows = hist + b * R * W;
+  if (r < 0) {
+    const int32_t* s = src + b * R * src_w;
+    for (int j = threadIdx.x; j < R * W; j += blockDim.x) {
+      const int c = j - (W - src_w);
+      rows[j] = (j < W && c >= 0) ? s[c] : 0;
+    }
+    return;
+  }
+  const int32_t* prev = rows + (int64_t)r * W;
+  const int32_t* q = src + (b * R + r) * src_w;
+  if (threadIdx.x == 0) {
+    int lp = 0, lq = 0, la = 0;                            // rows are pads then words: count the words from the right
+    while (lp < W && prev[W - 1 - lp] != 0) ++lp;
+    while (lq < src_w && q[src_w - 1 - lq] != 0) ++lq;
+    if (lp > 0 && lq > 0) {
+      const int32_t* a = ans + b * ans_ld;
+      const int n = ans_len ? max(ans_len[b] - 2, 0) : ans_max;
+      for (int i = 0; i < n && la < max_ans_len; ++i) {
+        const int32_t t = a[i];
+        if (t == end_token) break;
+        if (t != 0) a_s[la++] = t;                          // a pad a stale beam column carried is not a word
+      }
+    }
+    s_len[0] = lp; s_len[1] = lq; s_len[2] = la;
+  }
+  __syncthreads();
+  const int lp = s_len[0], lq = s_len[1], la = s_len[2];
+  const int keep = concat ? lp + 1 : 0;                    // row r ++ <END>
+  const int total = lp == 0 ? 0 : keep + lq + la;
+  int32_t* out = rows + (int64_t)(r + 1) * W;
+  for (int j = threadIdx.x; j < W; j += blockDim.x) {
+    const int s = total - W + j;                           // position in the unbounded row; the rightmost W are kept
+    int32_t t = 0;
+    if (s >= 0) {
+      if (s < keep) t = s < lp ? prev[W - lp + s] : end_token;
+      else if (s < keep + lq) t = q[src_w - lq + (s - keep)];
+      else t = a_s[s - keep - lq];
+    }
+    out[j] = t;
+  }
 }
 __global__ void k_sum_repeated_rows(float* __restrict__ dst, const float* __restrict__ src, int64_t B, int R, int64_t cols) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -984,7 +1035,7 @@ __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __r
   const int64_t r = blockIdx.x;
   const float* row = x + r * V;
   const float lse = row_lse(row, V, red);
-  const uint64_t base = (uint64_t)(smp.row_offset + r) * (uint64_t)V;
+  const uint64_t base = (uint64_t)(smp.row_offset + r * smp.row_stride) * (uint64_t)V;
   const uint64_t q0 = base >> 2, q1 = (base + V - 1) >> 2;
   float bk = -INFINITY;
   int bc = 0x7fffffff;
@@ -1322,8 +1373,17 @@ void add_out(LaunchCtx& cx, float* out, const float* a, const float* b, int64_t 
 void copy_cols(LaunchCtx& cx, float* dst, int64_t ldd, const float* src, int64_t lds, int64_t rows, int cols) {
   L1D(k_copy_cols, rows * cols, dst, ldd, src, lds, rows, cols);
 }
-void repeat_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols) {
-  L1D(k_repeat_rows, B * R * cols, dst, src, B, R, cols);
+void repeat_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols, int64_t lds) {
+  L1D(k_repeat_rows, B * R * cols, dst, src, B, R, cols, lds < 0 ? cols : lds);
+}
+void hist_append(LaunchCtx& cx, int32_t* hist, int64_t B, int R, int W, int r, const int32_t* src, int src_w, const int32_t* ans,
+                 int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat) {
+  VD_REQUIRE(W >= src_w && src_w > 0 && r < R - 1 && (r < 0 || max_ans_len >= 1), VD_E_BADARG, "hist_append: widths / round");
+  if (B <= 0) return;
+  const int cap = r < 0 ? 0 : (int)std::min<int64_t>(max_ans_len, ans_ld);   // an answer row holds at most ans_ld words
+  k_hist_append<<<(unsigned)B, 128, (size_t)cap * sizeof(int32_t), cx.stream>>>(hist, R, W, r, src, src_w, ans, ans_ld, ans_len,
+                                                                               ans_max, end_token, cap, concat ? 1 : 0);
+  check_launch(cx, "k_hist_append");
 }
 void sum_repeated_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols) {
   L1D(k_sum_repeated_rows, B * cols, dst, src, B, R, cols);

@@ -387,6 +387,37 @@ class Engine:
                                      int(row_offset), ans.ctypes.data, logp.ctypes.data))
         return ans, logp
 
+    def gen_dialog_beam_search(self, batch: Batch, k: int, L: int, start: int, end: int, hist_width: int, max_ans_len: int):
+        """Dialogs on the model's own answers with the beam search (vd_gen_dialog_beam_search): every round of `batch`,
+        round r's encoder reading the answers generated for rounds < r.  Returns (answer (N, L), length (N), score (N),
+        the history rows the encoder read (B, maxQuesCount, hist_width)), the first three as gen_beam_search's."""
+        B, R = batch.c.B, self.params["maxQuesCount"]
+        ans = np.zeros((B * R, int(L)), dtype=np.int32)
+        length = np.zeros(B * R, dtype=np.int32)
+        score = np.zeros(B * R, dtype=np.float64)
+        hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
+        self._enc_rows = None
+        check(self.lib.vd_gen_dialog_beam_search(self.h, C.byref(batch.c), int(k), int(L), int(start), int(end),
+                                                 int(hist_width), int(max_ans_len), ans.ctypes.data, length.ctypes.data,
+                                                 score.ctypes.data, hist.ctypes.data))
+        self._enc_rows = B * R
+        return ans, length, score, hist
+
+    def gen_dialog_sample(self, batch: Batch, L: int, start: int, end: int, temperature: float, seed: int, row_offset: int,
+                          hist_width: int, max_ans_len: int):
+        """Dialogs on the model's own answers with sampling (vd_gen_dialog_sample).  Returns (answer (N, L+1), logp (N, L),
+        history rows (B, maxQuesCount, hist_width)); round r of dialog b draws as global round row_offset + b R + r."""
+        B, R = batch.c.B, self.params["maxQuesCount"]
+        ans = np.zeros((B * R, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((B * R, int(L)), dtype=np.float32)
+        hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
+        self._enc_rows = None
+        check(self.lib.vd_gen_dialog_sample(self.h, C.byref(batch.c), int(L), int(start), int(end), float(temperature),
+                                            int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset), int(hist_width), int(max_ans_len),
+                                            ans.ctypes.data, logp.ctypes.data, hist.ctypes.data))
+        self._enc_rows = B * R
+        return ans, logp, hist
+
     def upload(self, dev_ptr: int, a: np.ndarray):
         a = np.ascontiguousarray(a, dtype=np.float32)
         check(self.lib.vd_memcpy_h2d(self.h, C.c_void_p(dev_ptr), a.ctypes.data, a.nbytes))

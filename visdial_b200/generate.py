@@ -5,7 +5,9 @@ with `-sampleWords 1`, sampling at `temperature`, over the first `maxThreads` di
 `<resultPath>/results.json` = {opts, data}, data = [{image_id, dialog: [{question, answer}]}] with the text of
 utils.idToWords, which is what vis/static/main.js shows.  A round where no beam reaches <END> stops the command before
 anything is written (the reference dies there too, model.lua:575).  `-dialogsPerCall D` searches D dialogs per device
-call; 1 (the default) is the reference's per-dialog loop.
+call; 1 (the default) is the reference's per-dialog loop.  `-history generated` answers every round with the dialog's own
+earlier answers in its history instead of the dataset's (`-history gt`, the default and the reference's behaviour; DESIGN
+§17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.
 
 `-gpus N` splits those first `maxThreads` dialogs into contiguous shares over GPUs gpuid .. gpuid+N-1 and rank 0 writes
 them in order; with per-dialog calls the file is the one a single GPU writes."""
@@ -22,6 +24,7 @@ def rank_share(model, dl, opt: dict) -> list:
     from .utils import idToWords
     dl.restrict("val", max(0, opt["maxThreads"]))                                   # model.lua:455 over the ranks
     sampleParams = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "dialogsPerCall")}   # :88-94
+    sampleParams["history"] = opt.get("history", "gt")
     answers = model.generateAnswers(dl, "val", sampleParams)                        # :96
     words = dl.ind2word
     return [{"image_id": a["image_id"],
@@ -51,4 +54,4 @@ def main(opt: dict, rank: int = 0, world: int = 1):
 
 
 if __name__ == "__main__":
-    cli.run("visdial_b200.generate", "main", cli.parse(cli.GENERATE_OPTIONS, prog="python -m visdial_b200.generate"))
+    cli.run("visdial_b200.generate", "main", cli.parse(cli.GENERATE_COMMAND_OPTIONS, prog="python -m visdial_b200.generate"))

@@ -9,6 +9,7 @@ import numpy as np
 from . import decoders, encoders
 from .engine import Batch, DEFAULT_PARAMS, derive_flags
 from .modules import Criterion, Sequential
+from .cli import HISTORY_MODES
 from .utils import image_id as _image_id
 
 
@@ -207,10 +208,24 @@ class Model:
         offset included), so the samples do not depend on dialogsPerCall or on how the split is sharded over ranks, only on
         the logits.  Returns the reference's answerTable with token-id lists (and text when the dataloader carries
         ind2word).  `strict=False` yields None for a round where no beam reached <END> (the reference indexes nil there,
-        model.lua:575)."""
+        model.lua:575).
+
+        `history`: "gt" (the default, the reference's behaviour) answers every round with the dataset's history;
+        "generated" runs each dialog on its own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample, DESIGN §17):
+        round r's history holds the answers generated for rounds < r.  Encoders without history have nothing to feed back
+        and answer as with "gt"."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
+        history = params.get("history", "gt")
+        if history not in HISTORY_MODES:
+            raise ValueError("history is one of %s, not %r" % ("|".join(HISTORY_MODES), history))
+        generated = history == "generated" and bool(self.params.get("useHistory"))
+        if generated:
+            # the width the dataloader sizes history rows for (dataloader.lua:217-225, getIndexData's cut :387-392)
+            maxAnsLen = dataloader.maxAnsLen
+            histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
+                min(dataloader.maxQuesLen + maxAnsLen, dataloader.maxHistoryLen)
         sampleWords = bool(params.get("sampleWords", 0) == 1)                           # :443
         temperature, seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
         beamSize, beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
@@ -236,15 +251,24 @@ class Model:
             inds = np.arange(first, min(numThreads, first + dialogsPerCall))
             self.wrapper.evaluate()                                                     # :460
             batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
-            self.forwardBackward(batch, True, True)                                     # :467
+            rowOffset = (offset + first) * self.params["maxQuesCount"]
+            if generated:
+                if sampleWords:
+                    answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
+                                                                 rowOffset, histWidth, maxAnsLen)
+                else:
+                    answer, length, score, _ = self.engine.gen_dialog_beam_search(batch, beamSize, beamLen, startToken,
+                                                                                  endToken, histWidth, maxAnsLen)
+            else:
+                self.forwardBackward(batch, True, True)                                 # :467
+                if sampleWords:                                                         # :582-594
+                    answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
+                else:                                                                   # :472-579
+                    answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
+            if not sampleWords:
+                length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
             ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
             Tq = ques.shape[2]
-            if sampleWords:                                                             # :582-594
-                answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed,
-                                                   (offset + first) * self.params["maxQuesCount"])
-            else:                                                                       # :472-579
-                answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
-                length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
             answer = answer.reshape(len(inds), -1, answer.shape[1])
             self.wrapper.training()                                                     # :605
             for d, convId in enumerate(inds):
