@@ -236,7 +236,8 @@ int vd_stream(vd_engine* e, void** cuda_stream);
 int vd_timer_start(vd_engine* e);
 int vd_timer_stop(vd_engine* e, float* ms);
 /* launch accounting: every kernel the engine launches is counted; kernels of class `name`
- * ("lstm_step", "gemm", ...) are additionally bracketed by events when profiling is on. */
+ * ("lstm_step", "gemm", ...) are additionally bracketed by events when profiling is on.  With profiling 1 every launch
+ * is also counted under its launch-site name ("k_segsum_rows", "rank_rows", ...; launches only, no time). */
 int vd_profile_enable(vd_engine* e, int32_t on);
 int vd_profile_reset(vd_engine* e);
 int vd_launch_count(vd_engine* e, int64_t* n_launches);
@@ -283,6 +284,13 @@ int vd_lstm16_step_fwd(vd_engine* e, int64_t R, int32_t H, const void* h_prev16,
                        float* c_out, void* h16_out, float* h32_out);
 int vd_lstm16_step_bwd(vd_engine* e, int64_t R, int32_t H, const void* da_next16, const void* Whb16, const void* gates16,
                        const float* c_prev, const float* c_cur, float* dc_carry, const int32_t* mask_ids, void* da16);
+/* test hook of the engine's pointwise, attention, criterion and decoding kernels: calls the launcher `name` (the table in
+ * visdial_b200/csrc/test_hooks.cu lists each one's pointer / int / real arguments) on caller-provided DEVICE buffers, on the
+ * engine's stream, then synchronises.  Dropout factors are the engine's own for the seed and iteration of
+ * vd_set_dropout_seed (identity unless training mode 1).  VD_E_BADARG for an unknown name or wrong argument counts; a
+ * launcher's refusal comes back as its error code. */
+int vd_test_kernel(vd_engine* e, const char* name, void* const* ptrs, int32_t n_ptrs, const int64_t* ints, int32_t n_ints,
+                   const double* reals, int32_t n_reals);
 /* cudaProfilerStart / cudaProfilerStop (ncu --profile-from-start off) */
 int vd_profiler_range(vd_engine* e, int32_t start);
 /* flush L2 by writing a scratch buffer larger than L2 (bench hygiene) */

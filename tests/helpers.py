@@ -1,8 +1,11 @@
-"""Shared test helpers: small configs, batches, oracle <-> engine parameter plumbing."""
+"""Shared test helpers: small configs, batches, oracle <-> engine parameter plumbing, device buffers with guard bands."""
+import ctypes as C
+
 import numpy as np
 import torch
 
 from visdial_b200 import engine as E
+from visdial_b200._lib import check
 from visdial_b200.synthetic import make_batch
 
 CONFIGS = [("lf-ques", "gen"), ("lf-ques-im-hist", "disc"), ("hrea-ques-im-hist", "gen"),
@@ -62,6 +65,40 @@ def flat_from_named(params, named):
 def seg_slices(params):
     segs, _ = E.layout(params)
     return {s.name: slice(s.offset, s.offset + s.size) for s in segs}
+
+
+class Buf:
+    """One device allocation holding a host image (any numpy dtype); ptr(off) = address of element `off`."""
+
+    def __init__(self, eng, img):
+        self.eng, self.img = eng, np.ascontiguousarray(img)
+        p = C.c_void_p()
+        check(eng.lib.vd_device_alloc(eng.h, C.byref(p), self.img.nbytes))
+        self.p = p
+        check(eng.lib.vd_memcpy_h2d(eng.h, p, self.img.ctypes.data, self.img.nbytes))
+
+    def ptr(self, off=0):
+        return C.c_void_p(self.p.value + self.img.itemsize * off)
+
+    def get(self):
+        out = np.empty_like(self.img)
+        check(self.eng.lib.vd_memcpy_d2h(self.eng.h, out.ctypes.data, self.p, out.nbytes))
+        return out
+
+    def free(self):
+        check(self.eng.lib.vd_device_free(self.eng.h, self.p))
+
+
+def _image(X, off, ld, rows_extra=0, fill=np.nan):
+    """X (r, c) placed at element offset `off` with row pitch ld; everything else (offset, padding columns, extra rows) = fill"""
+    r, c = X.shape
+    img = np.full(off + (r + rows_extra) * ld, fill, np.float32)
+    img[off:off + r * ld].reshape(r, ld)[:, :c] = X
+    return img
+
+
+def _view(img, off, rows, cols, ld):
+    return img[off:off + rows * ld].reshape(rows, ld)[:, :cols]
 
 
 def lstm_step_fwd_ref(z_x, h_prev, Wh, c_prev, mask):

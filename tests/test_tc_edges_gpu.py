@@ -22,7 +22,8 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import lstm_step_bwd_ref, lstm_step_fwd_ref, seg_slices, small_params, torch_batch, torch_params
+from helpers import (Buf, _image, _view, lstm_step_bwd_ref, lstm_step_fwd_ref, seg_slices, small_params, torch_batch,
+                     torch_params)
 from oracle import philox
 from oracle import visdial_oracle as O
 from visdial_b200 import VD_MATH_F16, VD_MATH_FP32, VD_MATH_TF32, Batch, Engine, init_parameters
@@ -30,40 +31,6 @@ from visdial_b200._lib import check
 from visdial_b200.synthetic import make_batch
 
 pytestmark = pytest.mark.gpu
-
-
-class Buf:
-    """One device allocation holding a host image (float32 or int32); ptr(off) = address of element `off`."""
-
-    def __init__(self, eng, img):
-        self.eng, self.img = eng, np.ascontiguousarray(img)
-        p = C.c_void_p()
-        check(eng.lib.vd_device_alloc(eng.h, C.byref(p), self.img.nbytes))
-        self.p = p
-        check(eng.lib.vd_memcpy_h2d(eng.h, p, self.img.ctypes.data, self.img.nbytes))
-
-    def ptr(self, off=0):
-        return C.c_void_p(self.p.value + 4 * off)
-
-    def get(self):
-        out = np.empty_like(self.img)
-        check(self.eng.lib.vd_memcpy_d2h(self.eng.h, out.ctypes.data, self.p, out.nbytes))
-        return out
-
-    def free(self):
-        check(self.eng.lib.vd_device_free(self.eng.h, self.p))
-
-
-def _image(X, off, ld, rows_extra=0, fill=np.nan):
-    """X (r, c) placed at element offset `off` with row pitch ld; everything else (offset, padding columns, extra rows) = fill"""
-    r, c = X.shape
-    img = np.full(off + (r + rows_extra) * ld, fill, np.float32)
-    img[off:off + r * ld].reshape(r, ld)[:, :c] = X
-    return img
-
-
-def _view(img, off, rows, cols, ld):
-    return img[off:off + rows * ld].reshape(rows, ld)[:, :cols]
 
 
 def _aligned(off, ld):

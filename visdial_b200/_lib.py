@@ -131,6 +131,7 @@ SIGNATURES = {
                          C.c_void_p, C.c_void_p, C.c_void_p, _P(C.c_int32)],
     "vd_lstm16_step_fwd": [_H, C.c_int64, C.c_int32] + [C.c_void_p] * 11,
     "vd_lstm16_step_bwd": [_H, C.c_int64, C.c_int32] + [C.c_void_p] * 8,
+    "vd_test_kernel": [_H, C.c_char_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32],
     "vd_profiler_range": [_H, C.c_int32],
     "vd_flush_l2": [_H],
     "vd_corpus_create": [_H, _P(vd_corpus_desc), _P(C.c_void_p)],

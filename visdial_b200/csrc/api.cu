@@ -14,6 +14,8 @@ void corpus_destroy(Corpus* c);
 void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd_batch* out);
 void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems);
 void corpus_batch_bytes(Corpus* c, int64_t* bytes, int32_t* launches);
+void test_kernel(Engine* e, const char* name, void* const* ptrs, int n_ptrs, const int64_t* ints, int n_ints, const double* reals,
+                 int n_reals);
 }  // namespace vd
 
 using vd::Engine;
@@ -470,6 +472,15 @@ int vd_lstm16_step_bwd(vd_engine* h, int64_t R, int32_t H, const void* da_next16
     vd::lstm16_step_bwd(e->cx, R, H, (const __half*)da_next16, (const __half*)Whb16, (const __half*)gates16, c_prev, c_cur,
                         dc_carry, mask_ids, (__half*)da16);
     VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+  })
+}
+
+int vd_test_kernel(vd_engine* h, const char* name, void* const* ptrs, int32_t n_ptrs, const int64_t* ints, int32_t n_ints,
+                   const double* reals, int32_t n_reals) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
+    vd::test_kernel(e, name, ptrs, n_ptrs, ints, n_ints, reals, n_reals);
   })
 }
 

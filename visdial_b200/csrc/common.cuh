@@ -23,6 +23,7 @@ struct CudaError : std::runtime_error {
       char _buf[512];                                                                    \
       snprintf(_buf, sizeof(_buf), "%s:%d: %s -> %s", __FILE__, __LINE__, #expr,         \
                cudaGetErrorString(_e));                                                  \
+      (void)cudaGetLastError(); /* a refused call must not fail the next check_launch */ \
       throw vd::CudaError(_e == cudaErrorMemoryAllocation ? -5 : -3, _buf);              \
     }                                                                                    \
   } while (0)
@@ -175,8 +176,10 @@ struct LaunchCtx {
   }
 };
 
+// counts the launch; with profiling 1 also under its own name in stats (launch count only, no events)
 inline void check_launch(LaunchCtx& cx, const char* what) {
   cx.launches++;
+  if (cx.profiling == 1) cx.stats[what].launches++;
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     char buf[512];

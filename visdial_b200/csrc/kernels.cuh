@@ -204,7 +204,10 @@ void lstm16_first_step(LaunchCtx& cx, int64_t R, int H, const __half* ptable16, 
                        const float* c_prev, const int32_t* mask_ids, __half* gates16, float* c_out, __half* h16_out, float* h32_out);
 void lstm16_bwd_last(LaunchCtx& cx, int64_t R, int H, const __half* gates16, const float* c_prev, const float* c_cur,
                      const float* dh_last, const float* scale, const int32_t* mask_ids, float* dc_carry, __half* da16);
+// round to nearest even, saturating: |x| > 65504 (inf included) becomes +-65504, NaN stays NaN (cvt.rn.satfinite)
 void cvt_f32_to_f16(LaunchCtx& cx, __half* dst, int64_t ldd, const float* src, int64_t lds, int64_t rows, int cols);
+// scale2 = {s, 1/s}: the power of two s = 2^clamp(10 - e, -60, 60) with max|x| = f 2^e, f in [1/2, 1), so max|x| s lies
+// in [2^9, 2^10); s = 1 when max|x| is 0 or infinite.  NaN elements do not take part in the maximum (fmaxf).
 void pick_grad_scale(LaunchCtx& cx, const float* x, int64_t n, uint32_t* bits, float* scale2);
 void segsum_rows16(LaunchCtx& cx, const __half* X, int64_t ldx, const int32_t* perm, const int32_t* sorted_tok, int64_t n,
                    float* out, int ncols, const float* inv_scale);
