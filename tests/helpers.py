@@ -89,6 +89,32 @@ class Buf:
         check(self.eng.lib.vd_device_free(self.eng.h, self.p))
 
 
+def call(eng, name, ptrs, ints=(), reals=()):
+    """vd_test_kernel by name; ptrs are device buffers (anything with .ptr()), ctypes pointers or None.  Returns the code."""
+    P = (C.c_void_p * max(1, len(ptrs)))(*[None if p is None else (p.ptr().value if hasattr(p, "ptr") else p.value)
+                                           for p in ptrs])
+    I = (C.c_int64 * max(1, len(ints)))(*[int(i) for i in ints])
+    X = (C.c_double * max(1, len(reals)))(*[float(x) for x in reals])
+    return eng.lib.vd_test_kernel(eng.h, name.encode(), P, len(ptrs), I, len(ints), X, len(reals))
+
+
+def run(eng, name, ptrs, ints=(), reals=()):
+    check(call(eng, name, ptrs, ints, reals))
+
+
+def within(got, ref, bound, what):
+    """|got - ref| <= bound elementwise (bound broadcasts), got finite; names the worst element otherwise"""
+    got = np.asarray(got)
+    ref = np.broadcast_to(np.asarray(ref, np.float64), got.shape)
+    assert np.isfinite(got).all(), (what, "non-finite output: a NaN-poisoned element was read, or an overflow")
+    err = np.abs(got.astype(np.float64) - ref)
+    bad = err > bound
+    if bad.any():
+        i = np.unravel_index(np.argmax(err - bound), err.shape)
+        raise AssertionError("%s: %d elements out of bound, worst at %s: got %r ref %r bound %r"
+                             % (what, int(bad.sum()), i, got[i], ref[i], np.broadcast_to(bound, err.shape)[i]))
+
+
 def _image(X, off, ld, rows_extra=0, fill=np.nan):
     """X (r, c) placed at element offset `off` with row pitch ld; everything else (offset, padding columns, extra rows) = fill"""
     r, c = X.shape

@@ -13,7 +13,6 @@ exp / log / tanh cost a few ulp each (CUDA's expf, logf, tanhf: <= 2 ulp), and t
 carries an absolute error of about 1e-7 (TANH_E_ABS).  A softmax turns an absolute error d of its inputs into a relative
 error of at most 2 d of its outputs.  Outputs the code calls bit-identical, integer outputs and pure data movement are
 compared with ==."""
-import ctypes as C
 
 import numpy as np
 import pytest
@@ -21,7 +20,7 @@ import torch
 
 import dense_oracle
 import sampling_twin
-from helpers import Buf, small_params
+from helpers import Buf, call, run, small_params, within
 from oracle import philox
 from oracle import visdial_oracle as O
 from visdial_b200 import Engine
@@ -104,32 +103,8 @@ def pool(eng):
     p.free()
 
 
-def call(eng, name, ptrs, ints=(), reals=()):
-    P = (C.c_void_p * max(1, len(ptrs)))(*[None if p is None else (p.ptr().value if isinstance(p, Dev) else p.value)
-                                           for p in ptrs])
-    I = (C.c_int64 * max(1, len(ints)))(*[int(i) for i in ints])
-    X = (C.c_double * max(1, len(reals)))(*[float(x) for x in reals])
-    return eng.lib.vd_test_kernel(eng.h, name.encode(), P, len(ptrs), I, len(ints), X, len(reals))
-
-
-def run(eng, name, ptrs, ints=(), reals=()):
-    check(call(eng, name, ptrs, ints, reals))
-
-
 def f32(x):
     return np.asarray(x, np.float32)
-
-
-def within(got, ref, bound, what):
-    got = np.asarray(got)
-    ref = np.broadcast_to(np.asarray(ref, np.float64), got.shape)
-    assert np.isfinite(got).all(), (what, "non-finite output: a NaN-poisoned element was read, or an overflow")
-    err = np.abs(got.astype(np.float64) - ref)
-    bad = err > bound
-    if bad.any():
-        i = np.unravel_index(np.argmax(err - bound), err.shape)
-        raise AssertionError("%s: %d elements out of bound, worst at %s: got %r ref %r bound %r"
-                             % (what, int(bad.sum()), i, got[i], ref[i], np.broadcast_to(bound, err.shape)[i]))
 
 
 def dropout_setup(eng, p):

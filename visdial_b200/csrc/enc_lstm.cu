@@ -26,7 +26,9 @@
 // enc_pair_shape_ok.
 //
 // Numerics: fp16 operands (h, da, weights) with fp32 accumulation = the VD_MATH_F16 class (10-bit mantissa like TF32); cell
-// state, gate pre-activations, saved activations and all gradients fp32.
+// state, gate pre-activations, saved activations and all gradients fp32.  The BPTT runs in a power-of-two scaled space (s from
+// the largest dL/dh_T, dL/dc_T input, enc_pair_backward): the encoder gradients are small enough (~1e-6 for da at B = 32) that
+// fp16 da would otherwise be subnormal, with a few significant bits or none.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include "../../include/visdial_b200.h"
@@ -79,6 +81,11 @@ __device__ __forceinline__ void ld16g(const float* p, float* d) {
 __device__ __forceinline__ void st16g(float* p, const float* v) {
 #pragma unroll
   for (int i = 0; i < 4; ++i) reinterpret_cast<float4*>(p)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+}
+__device__ __forceinline__ void st16gs(float* p, const float* v, float s) {     // v * s
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    reinterpret_cast<float4*>(p)[i] = make_float4(v[4 * i] * s, v[4 * i + 1] * s, v[4 * i + 2] * s, v[4 * i + 3] * s);
 }
 __device__ __forceinline__ void st16h(__half* p, const float* v) {            // 16 halves = 32 bytes
 #pragma unroll
@@ -344,6 +351,8 @@ k_enc_pair_fwd(const __grid_constant__ CUtensorMap tmH1, const __grid_constant__
 // BPTT of the pair, same structure mirrored in time (roles T / X / B of the header).  The SeqLSTM backward pointwise reads the saved
 // gates, c_{t-1}, c_t, carries dc in registers and writes da_t as fp32 (what the weight / input gradients after the kernel read) and
 // fp16 (the A operand of the steps that follow).  Layer 2 runs ahead; the X CTAs turn each da2_t into the layer-1 partial right behind it.
+// Everything inside runs scaled by s = scale2[0]: dh_last / dc_last are multiplied by s when loaded, so dh, dc, the partials and the
+// fp16 da are s times the true values; only the fp32 da is stored times 1/s (exact: s is a power of two).
 struct EncBwdParams {
   int T, R, H, RB;
   int nS, groups;
@@ -353,6 +362,7 @@ struct EncBwdParams {
   const int32_t* mask;
   int* flags;                      // [3][RB][T] step flags, then (gate split) [2][RB][T][H/128] partial-sum counts
   float* dh2; float* dh1;          // gate split: (T*R, H) fp32 each, zeroed — the partial products of a step are summed here with red.add
+  const float* scale2;             // device {s, 1/s}
 };
 
 // GS = gate split (H % 128 == 0): a CTA contracts ONE gate's quarter of the da panel (K = H) against a 128-unit slice of the weight
@@ -470,6 +480,7 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
       int* flag = top ? flagT : flagB;
       float* dhbuf = top ? p.dh2 : p.dh1;
       int* cnt = top ? cntT : cntB;
+      const float sc = p.scale2[0], isc = p.scale2[1];
       for (int rb = group; rb < p.RB; rb += p.groups) {
         const int64_t row = (int64_t)rb * 128 + rloc;
         const bool row_ok = row < p.R;
@@ -509,8 +520,10 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
             if (t == T - 1) {
               if (dh_last) { ld16g(dh_last + row * H + u0, va);
 #pragma unroll
-                for (int e = 0; e < EP_HW; ++e) dh[e] += va[e]; }
-              if (dc_last) ld16g(dc_last + row * H + u0, dc);
+                for (int e = 0; e < EP_HW; ++e) dh[e] += va[e] * sc; }
+              if (dc_last) { ld16g(dc_last + row * H + u0, dc);
+#pragma unroll
+                for (int e = 0; e < EP_HW; ++e) dc[e] *= sc; }
             }
             // ---- o:  da_o = dh tanh(c) o (1-o);  d = dc + dh o (1 - tanh(c)^2)
             ld16g(grow + 2 * H, va); ld16g(cst + tr * H + u0, vb);
@@ -520,25 +533,61 @@ k_enc_pair_bwd(const __grid_constant__ CUtensorMap tmA1, const __grid_constant__
               dc[e] = (dc[e] + dhe * go * (1.f - tcv * tcv)) * keep;           // dc <- d
               dh[e] = dhe * tcv * go * (1.f - go);
             }
-            st16h(da16row + 2 * H, dh); st16g(darow + 2 * H, dh);
+            st16h(da16row + 2 * H, dh); st16gs(darow + 2 * H, dh, isc);
             // ---- i, g:  da_i = d g i (1-i);  da_g = d i (1-g^2)
             ld16g(grow, va); ld16g(grow + 3 * H, vb);
 #pragma unroll
             for (int e = 0; e < EP_HW; ++e) dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]);
-            st16h(da16row, dh); st16g(darow, dh);
+            st16h(da16row, dh); st16gs(darow, dh, isc);
 #pragma unroll
             for (int e = 0; e < EP_HW; ++e) dh[e] = dc[e] * va[e] * (1.f - vb[e] * vb[e]);
-            st16h(da16row + 3 * H, dh); st16g(darow + 3 * H, dh);
+            st16h(da16row + 3 * H, dh); st16gs(darow + 3 * H, dh, isc);
             // ---- f:  da_f = d c_{t-1} f (1-f);  dc_{t-1} = d f
             ld16g(grow + 1 * H, va);
             if (t > 0) ld16g(cst + (tr - p.R) * H + u0, vb); else zero16(vb);
 #pragma unroll
             for (int e = 0; e < EP_HW; ++e) { dh[e] = dc[e] * vb[e] * va[e] * (1.f - va[e]); dc[e] *= va[e]; }
-            st16h(da16row + 1 * H, dh); st16g(darow + 1 * H, dh);
+            st16h(da16row + 1 * H, dh); st16gs(darow + 1 * H, dh, isc);
           }
           ep_publish(flag + (size_t)rb * T + t);
         }
       }
+    }
+  }
+}
+
+// scale2 = {s, 1/s}: the power of two s that brings the largest |x| over the non-null inputs (n4 float4 each) to [2^5, 2^6); s = 1
+// when that is 0 or infinite, NaN elements do not take part (fmaxf).  One CTA: the inputs are (R, H), a few hundred KB each, and one
+// launch costs less on the BPTT's critical path than a grid-wide reduction and a second launch.
+__global__ void __launch_bounds__(1024) k_ep_pick_scale(const float* x0, const float* x1, const float* x2, const float* x3, int64_t n4,
+                                                        float* __restrict__ scale2) {
+  __shared__ float red[32];
+  const float* xs[4] = {x0, x1, x2, x3};
+  float m = 0.f;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    if (!xs[k]) continue;
+    const float4* x = reinterpret_cast<const float4*>(xs[k]);
+    for (int64_t i = threadIdx.x; i < n4; i += blockDim.x) {
+      const float4 v = __ldg(x + i);
+      m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    m = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (threadIdx.x == 0) {
+      float sc = 1.f;
+      if (m > 0.f && isfinite(m)) {
+        int e; frexpf(m, &e);                        // m = f * 2^e, f in [0.5, 1)
+        sc = ldexpf(1.f, max(-60, min(60, 6 - e)));
+      }
+      scale2[0] = sc; scale2[1] = 1.f / sc;
     }
   }
 }
@@ -595,13 +644,17 @@ void enc_pair_forward(LaunchCtx& cx, int T, int64_t R, int H, const __half* W1h1
 
 
 // gates*/c* = the activations the forward saved; da*/da*_16 out (all T steps); flags int32 [enc_pair_bwd_flag_ints()].
-// dh1 / dh2: (T*R, H) fp32 scratch each for the gate-split variant (H % 128 == 0), or null -> unit-split variant
+// dh1 / dh2: (T*R, H) fp32 scratch each for the gate-split variant (H % 128 == 0), or null -> unit-split variant.
+// scale: float[2] out, {s, 1/s}: da*_16 = fp16(s da*), so the fp16 weight gradients take 1/s as their inv_scale.
+// s brings the largest |dh_last*|, |dc_last*| to [2^5, 2^6): 10 binades of head-room below the fp16 maximum, because dc sums the
+// dh of up to T steps and da_f = d c_{t-1} f (1-f) grows with |c|, which can reach T; the fp16 normal range still reaches
+// 20 binades below the largest input, where the option LSTM's 2^10 target would leave only 6 binades of head-room.
 int64_t enc_pair_bwd_flag_ints(int T, int64_t R, int H) { return (int64_t)cdiv(R, 128) * T * (3 + 2 * std::max(1, H / 128)); }
 bool enc_pair_gate_split(int H) { return H % 128 == 0; }
 void enc_pair_backward(LaunchCtx& cx, int T, int64_t R, int H, const __half* B1cat16, const __half* Whb2_16, const int32_t* mask,
                        const float* gates1, const float* c1, const float* gates2, const float* c2, const float* dh_last1,
                        const float* dc_last1, const float* dh_last2, const float* dc_last2, float* da1, __half* da1_16, float* da2,
-                       __half* da2_16, int* flags, float* dh1, float* dh2) {
+                       __half* da2_16, int* flags, float* dh1, float* dh2, float* scale) {
   using namespace tc;
   VD_REQUIRE(enc_pair_shape_ok(R, H, cx.sm_count), VD_E_STATE, "enc_pair_backward: shape");
   const bool gs = dh1 && dh2 && enc_pair_gate_split(H);
@@ -612,7 +665,9 @@ void enc_pair_backward(LaunchCtx& cx, int T, int64_t R, int H, const __half* B1c
   p.gates1 = gates1; p.c1 = c1; p.da1 = da1; p.da1_16 = da1_16;
   p.gates2 = gates2; p.c2 = c2; p.da2 = da2; p.da2_16 = da2_16;
   p.dh_last1 = dh_last1; p.dc_last1 = dc_last1; p.dh_last2 = dh_last2; p.dc_last2 = dc_last2;
-  p.mask = mask; p.flags = flags; p.dh1 = dh1; p.dh2 = dh2;
+  p.mask = mask; p.flags = flags; p.dh1 = dh1; p.dh2 = dh2; p.scale2 = scale;
+  k_ep_pick_scale<<<1, 1024, 0, cx.stream>>>(dh_last1, dc_last1, dh_last2, dc_last2, R * H / 4, scale);
+  check_launch(cx, "k_ep_pick_scale");
   VD_CUDA_CHECK(cudaMemsetAsync(flags, 0, (size_t)enc_pair_bwd_flag_ints(T, R, H) * sizeof(int), cx.stream));
   const int64_t TR = (int64_t)T * R;
   const int64_t G = 4 * (int64_t)H;

@@ -656,7 +656,7 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
   if (r.T > 1) {
     if (wgrad16) {
       LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * H * G * (double)(TR - R), 2.0 * (double)(TR - R) * (H + G));
-      gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, opt16 ? r.scale2 + 1 : nullptr);
+      gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, r.scale2 + 1);
     } else gemm_atb(H, G, TR - R, r.h, H, nullptr, r.da + R * G, G, dWs + (int64_t)D * G, G);
   }
   if (r.h0) gemm_atb(H, G, R, r.h0, H, nullptr, r.da, G, dWs + (int64_t)D * G, G);
@@ -686,7 +686,7 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
   }
   if (wgrad16 && r.x16) {            // layer 2 of the pair: x = h1, D = H
     LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * D * G * (double)TR, 2.0 * (double)TR * (D + G));
-    gemm_atb16(cx, D, G, TR, r.x16, D, r.da16, G, dWs, G, nullptr);
+    gemm_atb16(cx, D, G, TR, r.x16, D, r.da16, G, dWs, G, r.scale2 + 1);
   } else gemm_atb(D, G, TR, r.x ? r.x : Wp(0), r.x ? D : cfg.E, r.gather, r.da, G, dWs, G);
   colsum_add(cx, dWp(r.wseg + 1), r.da, TR, G, G);
   if (dx_out) gemm_tn((int)TR, D, G, r.da, G, nullptr, Ws, G, dx_out, D, 0.f, nullptr, 0);
@@ -721,10 +721,11 @@ void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2,
     int* flags = arena.get<int>(enc_pair_bwd_flag_ints(T, R, H));
     float* dh1 = nullptr; float* dh2 = nullptr;
     if (enc_pair_gate_split(H)) { dh1 = arena.get<float>(TR * H); dh2 = arena.get<float>(TR * H); }
+    l1.scale2 = l2.scale2 = arena.get<float>(2);       // da16 of both layers = fp16(s da); the weight gradients take 1/s
     {
       LaunchCtx::Scope sc2(&cx, "enc_pair_bwd", 2.0 * T * R * (double)H * 3.0 * G, 4.0 * T * R * (4.0 * G + 4.0 * H));
       enc_pair_backward(cx, T, R, H, B1cat, Whb2, l1.mask, l1.gates, l1.c, l2.gates, l2.c, dh_last1, dc_last1, dh_last2, dc_last2,
-                        l1.da, l1.da16, l2.da, l2.da16, flags, dh1, dh2);
+                        l1.da, l1.da16, l2.da, l2.da16, flags, dh1, dh2, l1.scale2);
     }
     lstm_backward_end(l2, nullptr, nullptr, nullptr);
     lstm_backward_end(l1, dx1_out, nullptr, nullptr);

@@ -92,7 +92,7 @@ struct LstmRun {
   __half *h16 = nullptr, *gates16 = nullptr, *da16 = nullptr, *P16 = nullptr, *Wh16 = nullptr, *Whb16 = nullptr;
   const __half* x16 = nullptr;       // Pair16 layer 2: fp16 copy of x (the h1 sequence)
   float* h32_last = nullptr;         // Opt16: fp32 copy of the last step's h (what the fp32 consumers of the run read)
-  float* scale2 = nullptr;           // Opt16: device {s, 1/s}, power-of-two scale of the BPTT (chosen from max|dL/dh_T|)
+  float* scale2 = nullptr;           // Opt16, Pair16: device {s, 1/s}, power-of-two scale of the BPTT (from max|dL/dh_T|, |dL/dc_T|)
   const float* h_last() const { return route.fwd == LstmPath::Opt16 ? h32_last : h + (int64_t)(saved ? T - 1 : (T - 1) & 1) * R * H; }
   const float* c_last() const { return c + (int64_t)(saved ? T - 1 : (T - 1) & 1) * R * H; }
 };

@@ -221,7 +221,7 @@ void enc_pair_forward(LaunchCtx& cx, int T, int64_t R, int H, const __half* W1h1
 void enc_pair_backward(LaunchCtx& cx, int T, int64_t R, int H, const __half* B1cat16, const __half* Whb2_16, const int32_t* mask,
                        const float* gates1, const float* c1, const float* gates2, const float* c2, const float* dh_last1,
                        const float* dc_last1, const float* dh_last2, const float* dc_last2, float* da1, __half* da1_16, float* da2,
-                       __half* da2_16, int* flags, float* dh1, float* dh2);
+                       __half* da2_16, int* flags, float* dh1, float* dh2, float* scale);
 int64_t enc_pair_bwd_flag_ints(int T, int64_t R, int H);
 bool enc_pair_gate_split(int H);
 }  // namespace vd

@@ -1,6 +1,6 @@
-// vd_test_kernel: the kernels.cuh launchers of pointwise.cu and lstm16.cu's streaming helpers, called by name on
-// caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory attribute and route are the
-// engine's own.  The table below is the whole surface: name, pointer / int / real counts, and the call.
+// vd_test_kernel: the kernels.cuh launchers of pointwise.cu, lstm16.cu's streaming helpers and enc_lstm.cu's persistent
+// encoder LSTM pair, called by name on caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory
+// attribute and route are the engine's own.  The table below is the whole surface: name, pointer / int / real counts, and the call.
 //   dropout:  p = reals[0], the site an int; the factors are Engine::dropcfg(p)'s (identity unless training == 1).
 //   sampling: SampleCfg from ints (seed, step, row_offset, row_stride) and reals (temperature).
 // Pointers may be null where the launcher accepts null (mask ids, gt, inv_scale, ...).
@@ -21,6 +21,7 @@ struct Entry {
 #define I32(i) (static_cast<int32_t*>(P[i]))
 #define CI32(i) (static_cast<const int32_t*>(P[i]))
 #define H16(i) (static_cast<__half*>(P[i]))
+#define CH16(i) (static_cast<const __half*>(P[i]))
 #define IN(i) ((int)I[i])
 #define DROP(k) e->dropcfg((float)X[k])
 
@@ -143,6 +144,26 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        segsum_rows16(e->cx, static_cast<const __half*>(P[0]), I[0], CI32(1), CI32(2), I[1], F(3), IN(2), CF(4));
      }},
+    // ---- persistent encoder LSTM pair (enc_lstm.cu), ints T, R, H.  forward ptrs W1h16, W2cat16, bias2, mask, gates1, c1, h1,
+    // h1_16, gates2, c2, h2, h2_16, flags;  backward ptrs B1cat16, Whb2_16, mask, gates1, c1, gates2, c2, dh_last1, dc_last1,
+    // dh_last2, dc_last2, da1, da1_16, da2, da2_16, flags, dh1, dh2, scale (null dh1 / dh2 = the unit split at any H)
+    {"enc_pair_forward", 13, 3, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       enc_pair_forward(e->cx, IN(0), I[1], IN(2), CH16(0), CH16(1), CF(2), CI32(3), F(4), F(5), F(6), H16(7), F(8), F(9), F(10),
+                        H16(11), I32(12));
+     }},
+    {"enc_pair_backward", 19, 3, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       enc_pair_backward(e->cx, IN(0), I[1], IN(2), CH16(0), CH16(1), CI32(2), CF(3), CF(4), CF(5), CF(6), CF(7), CF(8), CF(9), CF(10),
+                         F(11), H16(12), F(13), H16(14), I32(15), F(16), F(17), F(18));
+     }},
+    // writes enc_pair_bwd_flag_ints(T, R, H) into the device int64 at ptrs[0]
+    {"enc_pair_bwd_flag_ints", 1, 3, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       const int64_t n = enc_pair_bwd_flag_ints(IN(0), I[1], IN(2));
+       VD_CUDA_CHECK(cudaMemcpyAsync(P[0], &n, sizeof(n), cudaMemcpyHostToDevice, e->cx.stream));
+       VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+     }},
     // ---- small helpers
     {"colsum_add", 2, 3, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) { colsum_add(e->cx, F(0), CF(1), I[0], IN(1), I[2]); }},
@@ -188,6 +209,7 @@ const Entry TABLE[] = {
 #undef I32
 #undef CI32
 #undef H16
+#undef CH16
 #undef IN
 #undef DROP
 
