@@ -210,6 +210,30 @@ int vd_gen_dialog_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int3
                          float temperature, uint64_t seed, int64_t row_offset, int32_t hist_width, int32_t max_ans_len,
                          int32_t* answer_host, float* logp_host, int32_t* hist_host);
 
+/* ---- answer-pool retrieval: disc models answer (DESIGN §18) --------------------------------------------------------
+ * A disc model answers a question by retrieval: it scores every answer of the split's answer pool (opt_list_<split>, every
+ * distinct candidate answer of the split) with disc.lua:22-29's dot product and takes the best.
+ *  vd_answer_pool_encode: tokens_host (m, width) int32 HOST, the pool's token rows as opt_list stores them (left-aligned,
+ *    zero-padded; width = the corpus's maxAnsLen gives each answer the encoding the disc decoder computes for it in any
+ *    batch).  Runs opt.lstm (no maskzero, disc.lua:4-20) forward-only over every row in the current math mode and keeps
+ *    h_T, (m, rnnHiddenSize) fp32, replacing any earlier pool.  VD_E_STATE for a gen engine; VD_E_BADARG for m < 1,
+ *    width < 1 or a token outside [0, vocabSize].
+ *  vd_answer_pool: the pool embeddings (m, rnnHiddenSize) as a DEVICE pointer, valid until the next encode.
+ *  vd_answer_pool_retrieve: the encoder forward in eval mode on batch b (its options, if any, are not read), then per round
+ *    n of the N = B * maxQuesCount rounds the k best pool rows by (score desc, pool index asc), score = encOut[n] . e_j:
+ *    index_host (N, k) 0-based pool rows, score_host (N, k) fp32.  One synchronisation, at the end.  1 <= k <= min(32, m).
+ *  vd_answer_pool_dialog: vd_gen_dialog_*'s loop (history rule, widths, hist_host and their refusals) with this retrieval
+ *    as round r's search; the top-1 pool row's non-pad words (before any <END> = vocabSize) are round r's answer.
+ *    Outputs as vd_answer_pool_retrieve's for all N rounds.  VD_E_STATE for an encoder without history.
+ * The pool belongs to the weights and the math mode it was encoded with: vd_set_parameters, vd_clamp_adam_step and
+ * vd_set_math_mode drop it, and a retrieval without a current pool is refused (VD_E_STATE), as it is on a gen engine.
+ * Writes a caller makes to the weights through vd_param_buffers do not drop it: re-encode after them. */
+int vd_answer_pool_encode(vd_engine* e, const int32_t* tokens_host, int64_t m, int32_t width);
+int vd_answer_pool(vd_engine* e, const float** emb_dev, int64_t* m);
+int vd_answer_pool_retrieve(vd_engine* e, const vd_batch* b, int32_t k, int32_t* index_host, float* score_host);
+int vd_answer_pool_dialog(vd_engine* e, const vd_batch* b, int32_t k, int32_t hist_width, int32_t max_ans_len,
+                          int32_t* index_host, float* score_host, int32_t* hist_host);
+
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.
  * The LR decay (model.lua:102-105) stays with the caller, as in the reference. */
@@ -351,7 +375,8 @@ int vd_corpus_destroy(vd_corpus* c);
  * vd_corpus_get_batch on this corpus (two buffer sets, alternating). */
 int vd_corpus_get_batch(vd_corpus* c, const int64_t* inds, int32_t n, int32_t decoder_gen, vd_batch* out);
 /* Read one PREPARED tensor back to the host (parity tests): name in {"ques_fwd","hist","hist_len","ans_in","ans_out",
- * "opt_in","opt_out","img_fv"}; *elems receives the element count (call with host_dst = NULL to size). */
+ * "opt_in","opt_out","img_fv"}, or "opt_list": the raw (numOptList, maxAnsLen) answer pool as uploaded, which the host no
+ * longer keeps (the pool vd_answer_pool_encode takes); *elems receives the element count (call with host_dst = NULL to size). */
 int vd_corpus_read(vd_corpus* c, const char* name, void* host_dst, int64_t* elems);
 /* bytes the last vd_corpus_get_batch read + wrote in HBM (algorithmic) and the number of kernels it launched */
 int vd_corpus_batch_bytes(vd_corpus* c, int64_t* bytes, int32_t* launches);

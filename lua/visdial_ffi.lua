@@ -49,6 +49,11 @@ int vd_gen_dialog_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size
 int vd_gen_dialog_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
                          float temperature, uint64_t seed, int64_t row_offset, int32_t hist_width, int32_t max_ans_len,
                          int32_t* answer_host, float* logp_host, int32_t* hist_host);
+int vd_answer_pool_encode(vd_engine* e, const int32_t* tokens_host, int64_t m, int32_t width);
+int vd_answer_pool(vd_engine* e, const float** emb_dev, int64_t* m);
+int vd_answer_pool_retrieve(vd_engine* e, const vd_batch* b, int32_t k, int32_t* index_host, float* score_host);
+int vd_answer_pool_dialog(vd_engine* e, const vd_batch* b, int32_t k, int32_t hist_width, int32_t max_ans_len,
+                          int32_t* index_host, float* score_host, int32_t* hist_host);
 int vd_clamp_adam_step(vd_engine* e, float learning_rate);
 int vd_comm_unique_id(void* id_out);
 int vd_comm_init(vd_engine* e, const void* id, int32_t rank, int32_t world);

@@ -123,6 +123,10 @@ SIGNATURES = {
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gen_dialog_sample": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_int32,
                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_answer_pool_encode": [_H, C.c_void_p, C.c_int64, C.c_int32],
+    "vd_answer_pool": [_H, _P(C.c_void_p), _P(C.c_int64)],
+    "vd_answer_pool_retrieve": [_H, _P(vd_batch), C.c_int32, C.c_void_p, C.c_void_p],
+    "vd_answer_pool_dialog": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gemm_atb16": [_H, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                       C.c_int64, C.c_float],
     "vd_lstm_step_fwd": [_H, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,

@@ -110,6 +110,7 @@ int vd_set_parameters(vd_engine* h, const float* src, int64_t n) {
   VD_TRY({
     Engine* e = ENG(h);
     VD_REQUIRE(src && n == e->nparams, VD_E_SHAPE, "vd_set_parameters: n must equal vd_num_params");
+    e->pool_valid = false;           // before the copy: a failed copy may have written part of the weights
     VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
     VD_CUDA_CHECK(cudaMemcpyAsync(e->W, src, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, e->cx.stream));
     VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
@@ -161,7 +162,12 @@ int vd_set_option_overlap(vd_engine* h, int32_t on, int32_t reserve_sms) {
   })
 }
 int vd_set_math_mode(vd_engine* h, int32_t mode) {
-  VD_TRY({ VD_REQUIRE(mode == VD_MATH_TF32 || mode == VD_MATH_FP32 || mode == VD_MATH_F16, VD_E_BADARG, "unknown math mode"); ENG(h)->math_mode = mode; })
+  VD_TRY({
+    VD_REQUIRE(mode == VD_MATH_TF32 || mode == VD_MATH_FP32 || mode == VD_MATH_F16, VD_E_BADARG, "unknown math mode");
+    Engine* e = ENG(h);
+    e->pool_valid = false;           // the pool was encoded on the previous mode's option-LSTM route
+    e->math_mode = mode;
+  })
 }
 
 int vd_encoder_forward(vd_engine* h, const vd_batch* b, const float** encOut) {
@@ -275,6 +281,25 @@ int vd_gen_dialog_sample(vd_engine* h, const vd_batch* b, int32_t beam_len, int3
                          int32_t* answer_host, float* logp_host, int32_t* hist_host) {
   VD_TRY({ ENG(h)->gen_dialog_sample(b, beam_len, start_token, end_token, temperature, seed, row_offset, hist_width, max_ans_len,
                                      answer_host, logp_host, hist_host); })
+}
+
+int vd_answer_pool_encode(vd_engine* h, const int32_t* tokens_host, int64_t m, int32_t width) {
+  VD_TRY({ ENG(h)->answer_pool_encode(tokens_host, m, width); })
+}
+int vd_answer_pool(vd_engine* h, const float** emb_dev, int64_t* m) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    e->check_pool(1);
+    if (emb_dev) *emb_dev = (const float*)e->pool_emb.p;
+    if (m) *m = e->pool_m;
+  })
+}
+int vd_answer_pool_retrieve(vd_engine* h, const vd_batch* b, int32_t k, int32_t* index_host, float* score_host) {
+  VD_TRY({ ENG(h)->answer_pool_retrieve(b, k, index_host, score_host); })
+}
+int vd_answer_pool_dialog(vd_engine* h, const vd_batch* b, int32_t k, int32_t hist_width, int32_t max_ans_len, int32_t* index_host,
+                          float* score_host, int32_t* hist_host) {
+  VD_TRY({ ENG(h)->answer_pool_dialog(b, k, hist_width, max_ans_len, index_host, score_host, hist_host); })
 }
 
 int vd_clamp_adam_step(vd_engine* h, float lr) { VD_TRY({ ENG(h)->clamp_adam_step(lr); }) }

@@ -493,6 +493,7 @@ void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems) {
   else if (k == "opt_in") { p = c->opt_in; cnt = (int64_t)c->m * (c->La + 1); }
   else if (k == "opt_out") { p = c->opt_out; cnt = (int64_t)c->m * (c->La + 1); }
   else if (k == "img_fv") { p = c->img_fv; cnt = (int64_t)c->nimg * c->img_elems; }
+  else if (k == "opt_list") { p = c->opt_list; cnt = (int64_t)c->m * c->La; }       // the split's answer pool (DESIGN §18)
   else VD_REQUIRE(false, VD_E_BADARG, "unknown prepared tensor name");
   VD_REQUIRE(p != nullptr, VD_E_STATE, "this corpus does not hold that tensor (useHistory / useIm off)");
   *elems = cnt;

@@ -1690,7 +1690,8 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
 // its answers are (DialogAnswers).
 void Engine::gen_dialog(const vd_batch* b, int W, int max_ans_len, const std::function<DialogAnswers(int)>& search,
                         int32_t* hist_host) {
-  VD_REQUIRE(cfg.dec == DEC_GEN && cfg.useHist, VD_E_STATE, "dialog generation needs the gen decoder and a history encoder");
+  // the decoder is the caller's to check: the gen searches, or the disc answer-pool retrieval
+  VD_REQUIRE(cfg.useHist, VD_E_STATE, "dialogs on the model's own answers need a history encoder");
   VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0 && b->Th > 0, VD_E_SHAPE, "batch with B, Tq and Th > 0");
   VD_REQUIRE(W >= b->Th && max_ans_len >= 1, VD_E_BADARG, "hist_width >= the batch's Th, max_ans_len >= 1");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
@@ -1775,9 +1776,132 @@ void Engine::gen_dialog_sample(const vd_batch* b, int L, int start_token, int en
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
+// ---- answer pool (DESIGN §18) ------------------------------------------------------------------------------------------
+// Rows per option-LSTM run of the pool encoding.  Chunks are balanced (m split into equal parts of at most this many rows),
+// so that at any m above 1 024 every chunk has at least 1 024 rows: the fp16 route of VD_MATH_F16 (lstm16_shape_ok) then runs
+// for all of them, as it does for a batch's 100-option rows.
+constexpr int64_t kPoolChunkRows = 16384;
+
+void Engine::answer_pool_encode(const int32_t* tokens_host, int64_t m, int w) {
+  VD_REQUIRE(cfg.dec == DEC_DISC, VD_E_STATE, "the answer pool is the disc decoder's (a gen engine has no option LSTM)");
+  VD_REQUIRE(tokens_host && m >= 1 && m <= INT32_MAX && w >= 1, VD_E_BADARG, "answer pool: tokens, 1 <= m < 2^31, width >= 1");
+  for (int64_t i = 0; i < m * w; ++i)
+    VD_REQUIRE(tokens_host[i] >= 0 && tokens_host[i] <= cfg.V, VD_E_BADARG, "answer pool: a token outside [0, vocabSize]");
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  cx.stream = main_stream;
+  join_options_backward();
+  if (opt_fwd_pending) { VD_CUDA_CHECK(cudaStreamSynchronize(opt_stream)); opt_fwd_pending = false; }
+  pool_valid = false;
+  const int H = cfg.H, E = cfg.E;
+  int32_t* tok = (int32_t*)pool_tok.ensure((size_t)m * w * sizeof(int32_t));
+  float* emb = (float*)pool_emb.ensure((size_t)m * H * sizeof(float));
+  VD_CUDA_CHECK(cudaMemcpyAsync(tok, tokens_host, (size_t)m * w * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+  refresh_shadows();
+  const int64_t nchunks = (m + kPoolChunkRows - 1) / kPoolChunkRows, chunk = (m + nchunks - 1) / nchunks;
+  const Arena::Mark mk = arena.mark();           // the last forward's activations stay as they are
+  {
+    LaunchCtx::Scope sc(&cx, "pool_encode", 2.0 * m * w * 4.0 * H * H, 4.0 * m * w + 4.0 * m * H);
+    for (int64_t off = 0; off < m; off += chunk) {
+      const int64_t n = std::min(chunk, m - off);
+      int32_t* ids = arena.get<int32_t>(n * w);
+      transpose_ids(cx, tok + off * w, ids, n, w);
+      LstmRun r = make_run(w, n, E, H, seg("opt.lstm.weight"), nullptr, ids, nullptr);   // disc.lua:4-5: no maskzero
+      lstm_forward(r, false);
+      VD_CUDA_CHECK(cudaMemcpyAsync(emb + off * H, r.h_last(), (size_t)n * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
+      arena.rewind(mk);
+    }
+  }
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  pool_m = m; pool_w = w; pool_valid = true;
+}
+
+void Engine::pool_topk(const float* Q, int64_t ldq, int64_t rows, const float* E, int64_t m, int H, int k, float* topv,
+                       int32_t* topi) {
+  VD_REQUIRE(Q && E && topv && topi && rows >= 1 && m >= 1 && m <= INT32_MAX && H >= 1 && ldq >= H, VD_E_BADARG,
+             "pool_topk: operands / shape");
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= m, VD_E_BADARG, "pool_topk: k in [1, min(32, m)]");
+  const bool tc = tcmode() && pool_tc_ok(H, Q, ldq, E);
+  PoolTcGeom g;
+  const int slots = tc ? (g = pool_topk_tc_geom(cx, rows, m)).slots : pool_topk_simt_slots(cx, rows, m);
+  const int64_t n = rows * slots * (int64_t)k;
+  char* s = (char*)pool_scratch.ensure((size_t)n * 8);
+  float* pv = (float*)s;
+  int32_t* pi = (int32_t*)(s + n * 4);
+  {
+    LaunchCtx::Scope sc(&cx, tc ? "pool_topk" : "pool_topk_simt", 2.0 * rows * m * H,
+                        4.0 * ((double)rows * H + (double)m * H) + 8.0 * n);
+    if (tc) pool_topk_tc(cx, g, Q, ldq, rows, E, m, H, k, pv, pi);
+    else pool_topk_simt(cx, slots, Q, ldq, rows, E, m, H, k, pv, pi);
+  }
+  LaunchCtx::Scope sc(&cx, "pool_topk_rows", 0.0, 8.0 * n + 8.0 * rows * k);
+  pool_topk_merge(cx, pv, pi, rows, slots, k, tc ? g.num_n : 0, tc ? g.grid : 0, topv, topi);
+}
+
+void Engine::check_pool(int k) const {
+  VD_REQUIRE(cfg.dec == DEC_DISC, VD_E_STATE, "answer-pool retrieval needs the disc decoder");
+  VD_REQUIRE(pool_valid, VD_E_STATE, "no answer pool for the current weights and math mode: call vd_answer_pool_encode");
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= pool_m, VD_E_BADARG, "k in [1, min(32, pool rows)]");
+}
+
+// the batch as the encoder reads it: the retrieval never runs the batch's option LSTM (encoder_forward would start it)
+static vd_batch encoder_only(const vd_batch* b) {
+  vd_batch e = *b;
+  e.To = 0; e.Ta = 0;
+  e.options = e.answer_ind = e.answer_in = e.answer_out = e.option_in = e.option_out = nullptr;
+  return e;
+}
+
+void Engine::answer_pool_retrieve(const vd_batch* b, int k, int32_t* index_host, float* score_host) {
+  check_pool(k);
+  VD_REQUIRE(b != nullptr && index_host && score_host, VD_E_BADARG, "null batch or output pointer");
+  const vd_batch eb = encoder_only(b);
+  const int saved_training = training;
+  training = 0;
+  try {
+    encoder_forward(&eb);
+    const int64_t N = db.N;
+    float* tv = arena.get<float>(N * k);
+    int32_t* ti = arena.get<int32_t>(N * k);
+    pool_topk(encOut, cfg.H, N, (const float*)pool_emb.p, pool_m, cfg.H, k, tv, ti);
+    VD_CUDA_CHECK(cudaMemcpyAsync(index_host, ti, (size_t)N * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, tv, (size_t)N * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  } catch (...) { training = saved_training; throw; }
+  training = saved_training;
+}
+
+// gen_dialog with the retrieval as the round's search: round r's rows of encOut (b*R + r, pitch R*H) against the pool, the
+// top-1 pool row's tokens appended as the answer (its zero pads are not words; <END> = vocabSize ends it, as it ends a
+// sampled answer)
+void Engine::answer_pool_dialog(const vd_batch* b, int k, int W, int max_ans_len, int32_t* index_host, float* score_host,
+                                int32_t* hist_host) {
+  check_pool(k);
+  VD_REQUIRE(index_host && score_host, VD_E_BADARG, "null output pointer");
+  VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
+  const int R = cfg.R, H = cfg.H;
+  const int64_t B = b->B, N = B * R;
+  int32_t* idx = (int32_t*)dialog_out[0].ensure((size_t)N * k * sizeof(int32_t));
+  int32_t* words = (int32_t*)dialog_out[1].ensure((size_t)B * pool_w * sizeof(int32_t));
+  float* score = (float*)dialog_out[3].ensure((size_t)N * k * sizeof(float));
+  const vd_batch eb = encoder_only(b);
+  gen_dialog(&eb, W, max_ans_len, [&](int r) {
+    float* tv = arena.get<float>(B * k);
+    int32_t* ti = arena.get<int32_t>(B * k);
+    pool_topk(encOut + (int64_t)r * H, (int64_t)R * H, B, (const float*)pool_emb.p, pool_m, H, k, tv, ti);
+    scatter_round(cx.stream, idx, ti, (size_t)k * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, score, tv, (size_t)k * sizeof(float), R, r, B);
+    gather_pool_rows(cx, (const int32_t*)pool_tok.p, pool_w, ti, k, B, words);
+    return DialogAnswers{words, pool_w, nullptr, pool_w, cfg.V};
+  }, hist_host);
+  VD_CUDA_CHECK(cudaMemcpyAsync(index_host, idx, (size_t)N * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, score, (size_t)N * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
 // model.lua:96-99 + optim_updates.lua:62-91
 void Engine::clamp_adam_step(float lr) {
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  pool_valid = false;                 // the pool's encoding belongs to the weights before this step
   join_options_backward();
   float gscale = 1.f;
   if (world > 1) {

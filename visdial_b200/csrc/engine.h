@@ -326,6 +326,18 @@ struct Engine {
                               int32_t* answer_host, int32_t* length_host, double* score_host, int32_t* hist_host);
   void gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
                          int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host, int32_t* hist_host);
+  // answer pool (DESIGN §18): a disc model answers by retrieval from the split's answer pool.  pool_tok (m, w) are the pool's
+  // token rows, pool_emb (m, H) opt.lstm's h_T of each; pool_valid drops when the weights or the math mode change.
+  GrowBuf pool_tok, pool_emb, pool_scratch;
+  int64_t pool_m = 0; int pool_w = 0; bool pool_valid = false;
+  void answer_pool_encode(const int32_t* tokens_host, int64_t m, int w);
+  // the k best rows of E (m, H) for each of `rows` query rows of Q (row pitch ldq), by (score desc, index asc), into topv /
+  // topi (rows, k); the route (tensor cores or CUDA cores) from the math mode and pool_tc_ok
+  void pool_topk(const float* Q, int64_t ldq, int64_t rows, const float* E, int64_t m, int H, int k, float* topv, int32_t* topi);
+  void check_pool(int k) const;
+  void answer_pool_retrieve(const vd_batch* b, int k, int32_t* index_host, float* score_host);
+  void answer_pool_dialog(const vd_batch* b, int k, int W, int max_ans_len, int32_t* index_host, float* score_host,
+                          int32_t* hist_host);
   void clamp_adam_step(float lr);
   void allreduce_grads();
   // Overlapped gradient sync (world > 1): dW is all-reduced in buckets on `comm_stream` as soon as each bucket's last

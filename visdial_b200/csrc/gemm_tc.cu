@@ -10,6 +10,7 @@
 //   k_tc_atb     : C += A^T B with both operands MN-major                   (weight gradients, split-K)
 #include <cuda.h>
 #include <mutex>
+#include "../../include/visdial_b200.h"
 #include "kernels.cuh"
 #include "tc_ptx.cuh"
 
@@ -22,7 +23,11 @@ constexpr int MMA_K = 8;         // tf32: 32 bytes per instruction
 constexpr int EPI_WARPS = 8;     // the consumer warps: 2 per 32-row quarter, each takes half of the tile's columns
 constexpr int GEMM_THREADS = 128 + 32 * EPI_WARPS;
 
-enum { MODE_GENERIC = 0, MODE_LSTM_FWD = 1, MODE_LSTM_BWD = 2, MODE_LSE = 3, MODE_DLOGIT = 4, MODE_SAMPLE = 5 };
+enum { MODE_GENERIC = 0, MODE_LSTM_FWD = 1, MODE_LSTM_BWD = 2, MODE_LSE = 3, MODE_DLOGIT = 4, MODE_SAMPLE = 5, MODE_TOPK = 6 };
+// MODE_TOPK   : answer-pool retrieval (DESIGN §18): scores A B^T whose (rows, N) matrix never leaves the chip.  Each epilogue
+//               thread keeps, in shared memory, the running k best (score desc, column asc) of its row over the consecutive
+//               column tiles its CTA walks for one row block, and writes one list per (row, CTA, column half) when the row
+//               block changes: the partials scale with the grid, not with N.  k travels in Params::H.
 // MODE_LSE    : vocabulary projection whose (rows, V) logits never leave the chip: per row and column slice only the running
 //               max, the sum of exponentials and the target's logit are written (gen.lua:23-24 + the criterion of model.lua:33-36
 //               / utils.computeLhood, utils.lua:86-102)
@@ -71,10 +76,13 @@ __device__ __forceinline__ void st8_cs(float* p, const float* v) {
 // chunks of a row are XOR-swizzled by (row>>1)&3 so that both access patterns are bank-conflict free: "thread = row" and
 // "4 lanes = one row's 64 bytes" (coalesced 64-byte runs on the global side).  C leaves by TMA tensor stores.
 constexpr int STG_ARR_BYTES = 32 * 16 * 4;
+constexpr int TOPK_MAX = 32;                           // MODE_TOPK: list capacity per epilogue thread
+constexpr int TOPK_THREADS = 32 * EPI_WARPS;
 template <int MODE> struct StageCfg {
   static constexpr bool ON = MODE == MODE_GENERIC || MODE == MODE_DLOGIT;
   static constexpr int ARR = ON ? 1 : 0;
-  static constexpr int BYTES = EPI_WARPS * ARR * STG_ARR_BYTES;
+  // MODE_TOPK: the epilogue threads' (score, column) lists, entry i of thread t at [i * TOPK_THREADS + t] (no bank conflicts)
+  static constexpr int BYTES = MODE == MODE_TOPK ? TOPK_MAX * TOPK_THREADS * 8 : EPI_WARPS * ARR * STG_ARR_BYTES;
 };
 template <int BN, int STG_BYTES = 0> struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 4;        // 16 KB
@@ -114,6 +122,14 @@ __device__ __forceinline__ void stg_get8(float* stg, int arr, int row, int sub, 
 __device__ __forceinline__ void stg_put8(float* stg, int arr, int row, int sub, const float* v) {
   *stg_at(stg, arr, row, sub * 2) = make_float4(v[0], v[1], v[2], v[3]);
   *stg_at(stg, arr, row, sub * 2 + 1) = make_float4(v[4], v[5], v[6], v[7]);
+}
+
+// MODE_TOPK: thread t's list (k entries, best first) -> partial list `slot` of `row`
+__device__ __forceinline__ void topk_flush(const Params& p, const float* lv, const int32_t* li, int t, int64_t row, int slot) {
+  if (row >= p.M) return;
+  const int k = p.H;
+  const int64_t o = (row * p.nparts + slot) * k;
+  for (int i = 0; i < k; ++i) { p.part_key[o + i] = lv[i * TOPK_THREADS + t]; p.part_cls[o + i] = li[i * TOPK_THREADS + t]; }
 }
 
 template <int BN> __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t acc) {
@@ -182,6 +198,8 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     const int half = cw >> 2;
     const float* arow = acc + q * 32 + lane;
     int s = 0; uint32_t ph = 0;
+    int topk_mb = -1;                                 // MODE_TOPK: the row block whose lists this CTA holds
+    float thr = -INFINITY;                            // MODE_TOPK: the k-th score of this thread's list
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m0 = (tile / num_n) * BM;
       const int nt = tile % num_n;
@@ -212,7 +230,43 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       const int64_t row = (int64_t)m0 + q * 32 + lane;
       const bool row_ok = row < p.M;
 
-      if (MODE == MODE_LSE || MODE == MODE_SAMPLE) {
+      if constexpr (MODE == MODE_TOPK) {
+        float* lv = stg_all;
+        int32_t* li = reinterpret_cast<int32_t*>(stg_all + TOPK_MAX * TOPK_THREADS);
+        const int t = cw * 32 + lane, k = p.H, mb = tile / num_n;
+        if (mb != topk_mb) {                          // a new row block: hand the last one's lists on, start empty ones
+          if (topk_mb >= 0) topk_flush(p, lv, li, t, (int64_t)topk_mb * BM + q * 32 + lane, blockIdx.x * NH + half);
+          for (int i = 0; i < k; ++i) { lv[i * TOPK_THREADS + t] = -INFINITY; li[i * TOPK_THREADS + t] = -1; }
+          thr = -INFINITY;
+          topk_mb = mb;
+        }
+        // the columns of one (CTA, column half) ascend across its tiles, so an equal score never displaces an entry: it
+        // enters only strictly above the k-th score, and moves up only past strictly lower scores (NaN never enters)
+        const int n0 = nt * BN;
+#pragma unroll 1
+        for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 8) {
+          if (n0 + c >= p.N) break;                   // warp-uniform
+          float v[8];
+          acc_ld8(arow, c, v);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int n = n0 + c + j;
+            const float x = v[j];
+            if (n >= p.N || !(x > thr)) continue;
+            int pos = k - 1;
+            while (pos > 0) {
+              const float pv = lv[(pos - 1) * TOPK_THREADS + t];
+              if (!(x > pv)) break;
+              lv[pos * TOPK_THREADS + t] = pv;
+              li[pos * TOPK_THREADS + t] = li[(pos - 1) * TOPK_THREADS + t];
+              --pos;
+            }
+            lv[pos * TOPK_THREADS + t] = x;
+            li[pos * TOPK_THREADS + t] = n;
+            thr = lv[(k - 1) * TOPK_THREADS + t];
+          }
+        }
+      } else if (MODE == MODE_LSE || MODE == MODE_SAMPLE) {
         // online softmax statistics of this warp's column slice of the tile: nothing but (max, sum exp, target logit) leaves
         const int n0 = nt * BN;
         const int tcol = (MODE == MODE_LSE && row_ok) ? p.tgt[row] - 1 : -1;
@@ -433,6 +487,11 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         }
       }
     }
+    if constexpr (MODE == MODE_TOPK) {
+      if (topk_mb >= 0)
+        topk_flush(p, stg_all, reinterpret_cast<const int32_t*>(stg_all + TOPK_MAX * TOPK_THREADS), cw * 32 + lane,
+                   (int64_t)topk_mb * BM + q * 32 + lane, blockIdx.x * NH + half);
+    }
     if (SC::ON && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
   }
 }
@@ -573,9 +632,19 @@ static CUtensorMap make_tmap(const float* base, int64_t rows, int64_t cols, int6
 
 static bool tma_ok(const float* p, int64_t ld) { return ((uintptr_t)p % 16 == 0) && (ld % 4 == 0); }
 
+// Persistent grid, balanced waves: with pmax CTAs available the tiles need ceil(tiles/pmax) rounds; the smallest grid
+// that still finishes in that many rounds is used, so no CTA idles through a ragged last round and the SMs not needed
+// stay free for concurrent streams.
+static int persistent_grid(const LaunchCtx& cx, int num_tiles) {
+  const int pmax = cx.sms();
+  int grid = num_tiles;
+  if (num_tiles > pmax) { const int rounds = cdiv(num_tiles, pmax); grid = cdiv(num_tiles, rounds); }
+  return grid;
+}
+
 template <int BN, int MODE>
 static void launch(LaunchCtx& cx, const CUtensorMap& tA, const CUtensorMap& tB, const Params& p, int num_tiles,
-                   const EpiMaps* epi = nullptr) {
+                   const EpiMaps* epi = nullptr, int grid_given = 0) {
   using L = SmemLayout<BN, StageCfg<MODE>::BYTES>;
   static EpiMaps none = {};
   const EpiMaps& em = epi ? *epi : none;
@@ -584,12 +653,8 @@ static void launch(LaunchCtx& cx, const CUtensorMap& tA, const CUtensorMap& tB, 
     VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_gemm<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
     attr_set = true;
   }
-  // Persistent grid, balanced waves: with pmax CTAs available the tiles need ceil(tiles/pmax) rounds; the smallest grid
-  // that still finishes in that many rounds is used, so no CTA idles through a ragged last round and the SMs not needed
-  // stay free for concurrent streams.
-  const int pmax = cx.sms();
-  int grid = num_tiles;
-  if (num_tiles > pmax) { const int rounds = cdiv(num_tiles, pmax); grid = cdiv(num_tiles, rounds); }
+  // grid_given: a mode whose outputs are laid out by the grid (MODE_TOPK's slots) passes the grid it sized them for
+  const int grid = grid_given > 0 ? grid_given : persistent_grid(cx, num_tiles);
   k_tc_gemm<BN, MODE><<<grid, GEMM_THREADS, L::TOTAL, cx.stream>>>(tA, tB, em, p);
   check_launch(cx, "k_tc_gemm");
 }
@@ -693,6 +758,30 @@ bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_
   CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);
   launch<128, MODE_DLOGIT>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128), &em);
   return true;
+}
+
+// Answer-pool retrieval on the tensor cores (MODE_TOPK, 64-column tiles: the lists leave room for a 5-stage ring).
+bool pool_tc_ok(int H, const float* Q, int64_t ldq, const float* E) { return H >= 32 && H % 4 == 0 && tc::tma_ok(Q, ldq) && tc::tma_ok(E, H); }
+constexpr int POOL_BN = 64;
+PoolTcGeom pool_topk_tc_geom(const LaunchCtx& cx, int64_t rows, int64_t m) {
+  PoolTcGeom g;
+  g.num_n = cdiv(m, POOL_BN);
+  g.tiles = cdiv(rows, tc::BM) * (int64_t)g.num_n;
+  g.grid = tc::persistent_grid(cx, (int)g.tiles);
+  g.slots = g.grid * (tc::EPI_WARPS / 4);
+  return g;
+}
+void pool_topk_tc(LaunchCtx& cx, const PoolTcGeom& g, const float* Q, int64_t ldq, int64_t rows, const float* E, int64_t m, int H,
+                  int k, float* part_v, int32_t* part_i) {
+  using namespace tc;
+  VD_REQUIRE(pool_tc_ok(H, Q, ldq, E) && k >= 1 && k <= TOPK_MAX && rows >= 1 && m >= 1, VD_E_BADARG, "pool_topk_tc: shape");
+  VD_REQUIRE(g.grid >= 1 && g.slots == g.grid * (EPI_WARPS / 4) && g.num_n == cdiv(m, POOL_BN) &&
+             g.tiles == cdiv(rows, BM) * (int64_t)g.num_n, VD_E_BADARG, "pool_topk_tc: geometry of another shape");
+  Params p = {};
+  p.M = (int)rows; p.N = (int)m; p.K = H; p.H = k;
+  p.part_key = part_v; p.part_cls = part_i; p.nparts = g.slots;
+  CUtensorMap tA = make_tmap(Q, rows, H, ldq, BM), tB = make_tmap(E, m, H, H, POOL_BN);
+  launch<POOL_BN, MODE_TOPK>(cx, tA, tB, p, (int)g.tiles, nullptr, g.grid);   // the slots were numbered for g.grid CTAs
 }
 
 // The weights the fused forward step takes; the engine routes a SeqLSTM to lstm_step_fwd_tc only if this holds.

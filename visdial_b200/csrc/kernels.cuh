@@ -225,3 +225,22 @@ void enc_pair_backward(LaunchCtx& cx, int T, int64_t R, int H, const __half* B1c
 int64_t enc_pair_bwd_flag_ints(int T, int64_t R, int H);
 bool enc_pair_gate_split(int H);
 }  // namespace vd
+
+namespace vd {
+// answer-pool retrieval (DESIGN §18; answer_pool.cu, gemm_tc.cu): per query row of Q (rows, H; row pitch ldq) the k <= 32 best
+// rows of the pool embeddings E (m, H) by (score desc, index asc), score = Q[r] . E[j], never writing the (rows, m) scores.
+// A route writes partial lists part_v / part_i (rows, slots, k), best first, (-inf, -1) = empty; pool_topk_merge reduces them.
+struct PoolTcGeom { int num_n = 0; int64_t tiles = 0; int grid = 0, slots = 0; };
+bool pool_tc_ok(int H, const float* Q, int64_t ldq, const float* E);          // the shapes the tensor-core route takes
+PoolTcGeom pool_topk_tc_geom(const LaunchCtx& cx, int64_t rows, int64_t m);
+void pool_topk_tc(LaunchCtx& cx, const PoolTcGeom& g, const float* Q, int64_t ldq, int64_t rows, const float* E, int64_t m, int H,
+                  int k, float* part_v, int32_t* part_i);
+int pool_topk_simt_slots(const LaunchCtx& cx, int64_t rows, int64_t m);
+void pool_topk_simt(LaunchCtx& cx, int slots, const float* Q, int64_t ldq, int64_t rows, const float* E, int64_t m, int H, int k,
+                    float* part_v, int32_t* part_i);
+// tc_grid > 0: lists of the tensor-core route (geometry tc_num_n / tc_grid), of which only the walked ones are read
+void pool_topk_merge(LaunchCtx& cx, const float* part_v, const int32_t* part_i, int64_t rows, int slots, int k, int tc_num_n,
+                     int tc_grid, float* topv, int32_t* topi);
+// out (n, w) <- pool_tok rows idx[b * idx_ld]
+void gather_pool_rows(LaunchCtx& cx, const int32_t* pool_tok, int w, const int32_t* idx, int64_t idx_ld, int64_t n, int32_t* out);
+}  // namespace vd

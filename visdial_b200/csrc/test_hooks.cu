@@ -164,6 +164,11 @@ const Entry TABLE[] = {
        VD_CUDA_CHECK(cudaMemcpyAsync(P[0], &n, sizeof(n), cudaMemcpyHostToDevice, e->cx.stream));
        VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
      }},
+    // ---- answer-pool top-k (DESIGN §18), routed as the engine routes it: ptrs Q, E, topv, topi; ints rows, ldq, m, H, k
+    {"answer_pool_topk", 4, 5, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       e->pool_topk(CF(0), I[1], I[0], CF(1), I[2], IN(3), IN(4), F(2), I32(3));
+     }},
     // ---- small helpers
     {"colsum_add", 2, 3, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) { colsum_add(e->cx, F(0), CF(1), I[0], IN(1), I[2]); }},

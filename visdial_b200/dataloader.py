@@ -284,6 +284,11 @@ class Dataloader:
         inds = self.part[dtype][0] + np.asarray(inds0, dtype=np.int64).reshape(-1)
         return self.corpus[dtype].get_batch(inds, 1)
 
+    def answerPool(self, dtype: str) -> np.ndarray:
+        """The split's answer pool opt_list_<dtype> (numOptList, maxAnsLen), read back from the device corpus (the host copy
+        is dropped after the upload): what Model.retrieveAnswers encodes."""
+        return self.corpus[dtype].read("opt_list").reshape(-1, int(self.corpus[dtype].desc.maxAnsLen))
+
     def getTestBatch(self, startId: int, params: dict, dtype: str = "val"):
         """`startId` is 0-based here (Lua's startId - 1); returns (batch, nextStartId) like :344-375."""
         inds, nxt = test_batch_indices(startId, int(params["batchSize"]), *self.part[dtype])   # :347-357

@@ -418,6 +418,43 @@ class Engine:
         self._enc_rows = B * R
         return ans, logp, hist
 
+    def answer_pool_encode(self, tokens: np.ndarray):
+        """Encode the split's answer pool (vd_answer_pool_encode): tokens (m, width) as opt_list stores them; replaces any
+        earlier pool."""
+        t = np.ascontiguousarray(tokens, dtype=np.int32)
+        if t.ndim != 2:
+            raise ValueError("answer pool tokens must be (m, width)")
+        check(self.lib.vd_answer_pool_encode(self.h, t.ctypes.data, int(t.shape[0]), int(t.shape[1])))
+
+    def answer_pool(self) -> DeviceTensor:
+        """The pool embeddings (m, rnnHiddenSize) of the last encode (vd_answer_pool)."""
+        p, m = C.c_void_p(), C.c_int64()
+        check(self.lib.vd_answer_pool(self.h, C.byref(p), C.byref(m)))
+        return DeviceTensor(self, p.value, (m.value, self.params["rnnHiddenSize"]))
+
+    def answer_pool_retrieve(self, batch: Batch, k: int = 1):
+        """The k best pool rows of every round of `batch` (vd_answer_pool_retrieve): (index (N, k) 0-based, score (N, k))."""
+        N = batch.c.B * self.params["maxQuesCount"]
+        index = np.zeros((N, int(k)), dtype=np.int32)
+        score = np.zeros((N, int(k)), dtype=np.float32)
+        self._enc_rows = None
+        check(self.lib.vd_answer_pool_retrieve(self.h, C.byref(batch.c), int(k), index.ctypes.data, score.ctypes.data))
+        self._enc_rows = N
+        return index, score
+
+    def answer_pool_dialog(self, batch: Batch, k: int, hist_width: int, max_ans_len: int):
+        """Dialogs on the model's own retrieved answers (vd_answer_pool_dialog): (index (N, k), score (N, k), the history
+        rows the encoder read (B, maxQuesCount, hist_width))."""
+        B, R = batch.c.B, self.params["maxQuesCount"]
+        index = np.zeros((B * R, int(k)), dtype=np.int32)
+        score = np.zeros((B * R, int(k)), dtype=np.float32)
+        hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
+        self._enc_rows = None
+        check(self.lib.vd_answer_pool_dialog(self.h, C.byref(batch.c), int(k), int(hist_width), int(max_ans_len),
+                                             index.ctypes.data, score.ctypes.data, hist.ctypes.data))
+        self._enc_rows = B * R
+        return index, score, hist
+
     def upload(self, dev_ptr: int, a: np.ndarray):
         a = np.ascontiguousarray(a, dtype=np.float32)
         check(self.lib.vd_memcpy_h2d(self.h, C.c_void_p(dev_ptr), a.ctypes.data, a.nbytes))

@@ -7,7 +7,9 @@ utils.idToWords, which is what vis/static/main.js shows.  A round where no beam 
 anything is written (the reference dies there too, model.lua:575).  `-dialogsPerCall D` searches D dialogs per device
 call; 1 (the default) is the reference's per-dialog loop.  `-history generated` answers every round with the dialog's own
 earlier answers in its history instead of the dataset's (`-history gt`, the default and the reference's behaviour; DESIGN
-§17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.
+§17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.  A disc checkpoint answers every round with the
+best answer of the split's answer pool (Model.retrieveAnswers, DESIGN §18); the beam and sampling options do not apply
+to it, and its answer text is the pool row's words.
 
 `-gpus N` splits those first `maxThreads` dialogs into contiguous shares over GPUs gpuid .. gpuid+N-1 and rank 0 writes
 them in order; with per-dialog calls the file is the one a single GPU writes."""
@@ -25,7 +27,11 @@ def rank_share(model, dl, opt: dict) -> list:
     dl.restrict("val", max(0, opt["maxThreads"]))                                   # model.lua:455 over the ranks
     sampleParams = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "dialogsPerCall")}   # :88-94
     sampleParams["history"] = opt.get("history", "gt")
-    answers = model.generateAnswers(dl, "val", sampleParams)                        # :96
+    if model.params["decoder"] == "disc":
+        # a disc model answers by retrieval from the split's answer pool (DESIGN §18); model.lua:434-437 stops here
+        answers = model.retrieveAnswers(dl, "val", {k: sampleParams[k] for k in ("dialogsPerCall", "history")})
+    else:
+        answers = model.generateAnswers(dl, "val", sampleParams)                    # :96
     words = dl.ind2word
     return [{"image_id": a["image_id"],
              "dialog": [{"question": idToWords(r["question"], words), "answer": idToWords(r["answer"], words)}

@@ -289,6 +289,68 @@ class Model:
                                     "dialog": threadAnswers})                           # :606
         return answerTable
 
+    def retrieveAnswers(self, dataloader, dtype="val", params=None):
+        """What a disc model answers (DESIGN §18): every round of the first `maxThreads` dialogs of split `dtype` answered
+        by retrieval from the split's answer pool (opt_list_<dtype>).  The pool is encoded once per call
+        (vd_answer_pool_encode); then `dialogsPerCall` dialogs (default 1) per engine call retrieve their `topK` (default 1)
+        best pool rows by (score desc, pool index asc): vd_answer_pool_retrieve on the dataset's history (`history` "gt",
+        the default), or vd_answer_pool_dialog on the answers retrieved for the dialog's earlier rounds ("generated";
+        encoders without history answer as with "gt").  Returns generateAnswers' answerTable: per round the question, the
+        top-1 pool row's tokens as `answer` (its non-pad words, no <START>), its 0-based pool `index` and `score`, and the
+        `topK` list of {index, score, answer}; with text when the dataloader carries ind2word."""
+        if self.params["decoder"] != "disc":
+            raise ValueError("retrieveAnswers answers with the disc decoder; gen models use generateAnswers")
+        params = params or {}
+        history = params.get("history", "gt")
+        if history not in HISTORY_MODES:
+            raise ValueError("history is one of %s, not %r" % ("|".join(HISTORY_MODES), history))
+        generated = history == "generated" and bool(self.params.get("useHistory"))
+        maxAnsLen = dataloader.maxAnsLen
+        if generated:
+            histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
+                min(dataloader.maxQuesLen + maxAnsLen, dataloader.maxHistoryLen)
+        topK = int(params.get("topK", 1))
+        numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])
+        dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
+        pool = dataloader.answerPool(dtype)
+        self.engine.answer_pool_encode(pool)
+        ind2word = getattr(dataloader, "ind2word", None)
+        words = (lambda ids: " ".join(ind2word.get(int(t), "<UNK>") for t in ids if int(t) > 0)) if ind2word else None
+        img = getattr(dataloader, "unique_img_" + dtype, None)
+        offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
+
+        def answer_of(j):
+            return np.array([t for t in pool[j] if t != 0], dtype=pool.dtype)
+
+        def entry(q, idx, sc):
+            a = answer_of(int(idx[0]))
+            e = {"question": q.tolist(), "answer": a.tolist(), "index": int(idx[0]), "score": float(sc[0]),
+                 "topK": [{"index": int(i), "score": float(v), "answer": answer_of(int(i)).tolist()} for i, v in zip(idx, sc)]}
+            if words:
+                e["question_text"], e["answer_text"] = words(q), words(a)
+            return e
+
+        answerTable = []
+        ques_len = None
+        R = self.params["maxQuesCount"]
+        for first in range(0, numThreads, dialogsPerCall):
+            inds = np.arange(first, min(numThreads, first + dialogsPerCall))
+            batch = dataloader.getIndexData(inds, self.params, dtype)
+            if generated:
+                index, score, _ = self.engine.answer_pool_dialog(batch, topK, histWidth, maxAnsLen)
+            else:
+                index, score = self.engine.answer_pool_retrieve(batch, topK)
+            index, score = index.reshape(len(inds), R, topK), score.reshape(len(inds), R, topK)
+            ques = batch["ques_fwd"]
+            Tq = ques.shape[2]
+            for d, convId in enumerate(inds):
+                w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
+                gid = offset + int(convId)
+                answerTable.append({"image_id": _image_id(img[gid]) if img is not None else gid,
+                                    "dialog": [entry(ques[d, it, Tq - w:], index[d, it], score[d, it])
+                                               for it in range(ques.shape[1])]})
+        return answerTable
+
     # ---- checkpoints (train.lua:33-34,78-80,99-102,120-121; evaluate.lua:58-91) -------------------------------
     def save(self, path: str, final: bool = False):
         """torch.save(path, {modelW, optims, modelParams}) — `final` = the model_final.t7 form (float weights, no optims)."""
