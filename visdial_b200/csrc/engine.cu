@@ -656,7 +656,12 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
   if (r.T > 1) {
     if (wgrad16) {
       LaunchCtx::Scope sc(&cx, "gemm_wgrad", 2.0 * H * G * (double)(TR - R), 2.0 * (double)(TR - R) * (H + G));
+      // stream-K: a CTA whose SM is still busy with another stream's kernel starts late and claims less work, so the
+      // weight gradient is sized to the whole GPU even under the option stream's overlap budget
+      const int budget = cx.sm_budget;
+      cx.sm_budget = 0;
       gemm_atb16(cx, H, G, TR - R, r.h16, H, r.da16 + R * G, G, dWs + (int64_t)D * G, G, r.scale2 + 1);
+      cx.sm_budget = budget;
     } else gemm_atb(H, G, TR - R, r.h, H, nullptr, r.da + R * G, G, dWs + (int64_t)D * G, G);
   }
   if (r.h0) gemm_atb(H, G, R, r.h0, H, nullptr, r.da, G, dWs + (int64_t)D * G, G);

@@ -15,10 +15,12 @@
 //   Both run their pointwise epilogue on the accumulator registers (no shared-memory accumulator tile), which leaves room
 //   for a 5-stage (forward) / 4-stage (backward) operand ring of 32 KB stages; the epilogue inputs are fetched by cp.async
 //   before the tile's contraction (the backward: those of its first 32 hidden units).
-//   k_atb16        : dWh += inv_scale * h^T da  (both operands MN-major fp16, split-K, red.global.add)
+//   k_atb16        : dWh += inv_scale * h^T da  (both operands MN-major fp16, 128 x 256 tiles, stream-K, red.global.add)
 //   k_lstm16_first / k_lstm16_bwd_last / k_segsum16 / k_cvt16 / k_amax / k_pick_scale : streaming helpers
 #include <cuda.h>
 #include <cuda_fp16.h>
+#include <map>
+#include <mutex>
 #include "../../include/visdial_b200.h"
 #include "kernels.cuh"
 #include "tc_ptx.cuh"
@@ -372,29 +374,41 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
 // B = da (K rows x 4H) fp16 — both MN-major (the contraction index is the row index in HBM).  A TMA box of 64 columns
 // x KB rows lands as KB rows of 128 bytes = the canonical MN-major SWIZZLE_128B layout (8 k-rows per 1024-byte atom:
 // SBO = 1024; 64-column groups LBO bytes apart), which the f16 wgmma reads transposed; one K = 16 instruction consumes
-// two atoms.  Warpgroup 0 = TMA producer, warpgroups 1-2 = consumers (64 columns of A each).
+// two atoms.  Warpgroup 0 = TMA producer, warpgroups 1-2 = consumers (64 rows of the 128 x 256 tile each, m64n256k16).
+//
+// Stream-K: every tile's k-blocks are cut into chunks of `chunk` k-blocks (the last one of a tile shorter), numbered
+// k-range-major — chunk c = (k-range c / tiles, tile c % tiles) — so that the CTAs running at one time work on the same rows
+// of A and B for different tiles, and those rows come from HBM once and are reused from L2 (tile-major order would read
+// the operands once per tile).  The producer claims chunks from a device counter and tags the chunk's first stage with its
+// number; the consumers add each finished partial tile into C with red.global.add (C is accumulated with atomics anyway,
+// so no fix-up pass).  A CTA that starts late, behind kernels of other streams, claims fewer chunks.  The last CTA to
+// finish resets the counter, so one zeroed counter per stream serves every launch on it.
 constexpr int A16_KB = 64;                 // k-rows per stage (4 MMAs)
-constexpr int A16_BN = 128;
+constexpr int A16_BM = 128, A16_BN = 256;
 constexpr int A16_THREADS = 384;
-constexpr int A16_A_BYTES = 2 * A16_KB * 128;              // 128 columns of A = 2 boxes
-constexpr int A16_B_BYTES = (A16_BN / 64) * A16_KB * 128;  // 2 boxes
-constexpr int A16_STAGE = A16_A_BYTES + A16_B_BYTES;       // 32 KB
-constexpr int A16_STAGES = 6;
+constexpr int A16_A_BYTES = (A16_BM / 64) * A16_KB * 128;  // 2 boxes of 64 columns
+constexpr int A16_B_BYTES = (A16_BN / 64) * A16_KB * 128;  // 4 boxes
+constexpr int A16_STAGE = A16_A_BYTES + A16_B_BYTES;       // 48 KB
+constexpr int A16_STAGES = 4;
 constexpr int A16_TOTAL = A16_STAGES * A16_STAGE + 1024 + 256;
-struct Atb16Params { int M, N; int64_t K, k_per_split; float* C; int64_t ldc; const float* inv_scale; };
+constexpr int A16_CHUNKS_PER_CTA = 24;     // chunk length: ~24 claims per CTA (tail imbalance < 1/24), at least
+constexpr int A16_MIN_CHUNK = 32;          // 32 k-blocks (the partial-tile reduction stays a few % of the chunk)
+struct Atb16Params {
+  int M, N, tiles_n, tiles, kbt;           // kbt = k-blocks per tile
+  int chunk, num_chunks;                   // k-blocks per chunk, chunks (tiles x k-ranges)
+  float* C; int64_t ldc; const float* inv_scale;
+  int* counter;                            // [0] next chunk, [1] CTAs done; both zero between launches
+};
 
+template <bool VEC4>   // C 16-byte aligned with ldc % 4 == 0: the partial tiles go out as red.global.add.v4
 __global__ void __launch_bounds__(A16_THREADS, 1)
 k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Atb16Params p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full = (uint64_t*)(smem + A16_STAGES * A16_STAGE);
   uint64_t* empty = full + A16_STAGES;
+  int* tag = (int*)(empty + A16_STAGES);                     // chunk of a chunk's first stage, -1 = no more work
   const int warp = threadIdx.x >> 5;
-  const int num_n = (p.N + A16_BN - 1) / A16_BN;
-  const int m0 = (blockIdx.x / num_n) * BM16, n0 = (blockIdx.x % num_n) * A16_BN;
-  const int64_t kbeg = (int64_t)blockIdx.y * p.k_per_split;
-  const int64_t kend = min(p.K, kbeg + p.k_per_split);
-  const int num_kb = (int)((kend - kbeg + A16_KB - 1) / A16_KB);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < A16_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
@@ -405,54 +419,94 @@ k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
   if (warp < 4) {
     if (threadIdx.x == 0) {
       int s = 0; uint32_t ph = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* sa = smem + s * A16_STAGE;
-        uint8_t* sb = sa + A16_A_BYTES;
-        mbar_expect_tx(&full[s], A16_STAGE);
-        const int krow = (int)(kbeg + (int64_t)kb * A16_KB);     // k_per_split % A16_KB == 0: only the global K tail is partial
+      for (;;) {
+        const int c = atomicAdd(p.counter, 1);
+        if (c >= p.num_chunks) break;
+        const int tile = c % p.tiles, kb0 = (c / p.tiles) * p.chunk, kb1 = min(p.kbt, kb0 + p.chunk);
+        const int m0 = (tile / p.tiles_n) * A16_BM, n0 = (tile % p.tiles_n) * A16_BN;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          const int krow = kb * A16_KB;
+          mbar_wait(&empty[s], ph ^ 1);
+          uint8_t* sa = smem + s * A16_STAGE;
+          uint8_t* sb = sa + A16_A_BYTES;
+          if (kb == kb0) tag[s] = c;
+          mbar_expect_tx(&full[s], A16_STAGE);       // out-of-range rows / columns land as zeros and still count
 #pragma unroll
-        for (int g = 0; g < 2; ++g) tma_load_2d(sa + g * A16_KB * 128, &tmA, &full[s], m0 + g * 64, krow);
+          for (int b = 0; b < A16_BM / 64; ++b) tma_load_2d(sa + b * A16_KB * 128, &tmA, &full[s], m0 + b * 64, krow);
 #pragma unroll
-        for (int g = 0; g < A16_BN / 64; ++g) tma_load_2d(sb + g * A16_KB * 128, &tmB, &full[s], n0 + g * 64, krow);
-        if (++s == A16_STAGES) { s = 0; ph ^= 1; }
+          for (int b = 0; b < A16_BN / 64; ++b) tma_load_2d(sb + b * A16_KB * 128, &tmB, &full[s], n0 + b * 64, krow);
+          if (++s == A16_STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+      mbar_wait(&empty[s], ph ^ 1);
+      tag[s] = -1;
+      mbar_arrive(&full[s]);
+      // every CTA has made its last claim once all have counted themselves here: the last one resets the counter
+      __threadfence();
+      if (atomicAdd(p.counter + 1, 1) == (int)gridDim.x - 1) {
+        atomicExch(p.counter, 0);
+        atomicExch(p.counter + 1, 0);
       }
     }
-  } else if (num_kb > 0) {
-    const int wg = (warp - 4) >> 2;
-    float d[A16_BN / 2];
-#pragma unroll
-    for (int i = 0; i < A16_BN / 2; ++i) d[i] = 0.f;
-    int s = 0; uint32_t ph = 0; int prev = -1;
-    for (int kb = 0; kb < num_kb; ++kb) {
-      mbar_wait(&full[s], ph);
-      const uint32_t sa = smem_u32(smem + s * A16_STAGE);
-      const uint32_t sb = sa + A16_A_BYTES;
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < A16_KB / UK16; ++k)
-        wgmma_f16_n128_mn(d, make_desc(sa + wg * A16_KB * 128 + k * 2048, A16_KB * 128, 1024),
-                          make_desc(sb + k * 2048, A16_KB * 128, 1024), (kb | k) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
-      prev = s;
-      if (++s == A16_STAGES) { s = 0; ph ^= 1; }
-    }
-    wgmma_wait<0>();
-    wgmma_hold(d);
+  } else {
+    const int wg = (warp - 4) >> 2, lane = threadIdx.x & 31, w = warp & 3;
     const float sc = p.inv_scale ? __ldg(p.inv_scale) : 1.f;
-    const int lane = threadIdx.x & 31, w = warp & 3;
-    const int r0 = m0 + wg * 64 + 16 * w + (lane >> 2), c0 = n0 + 2 * (lane & 3);
+    float d[A16_BN / 2];
+    int s = 0; uint32_t ph = 0;
+    for (;;) {
+      mbar_wait(&full[s], ph);
+      const int c = tag[s];
+      if (c < 0) break;
+      const int tile = c % p.tiles, kb0 = (c / p.tiles) * p.chunk;
+      const int nseg = min(p.kbt - kb0, p.chunk);        // k-blocks of this partial tile
+      int prev = -1;
+      for (int i = 0; i < nseg; ++i) {
+        if (i > 0) mbar_wait(&full[s], ph);
+        const uint32_t sa = smem_u32(smem + s * A16_STAGE);
+        const uint32_t sb = sa + A16_A_BYTES;
+        wgmma_fence();
 #pragma unroll
-    for (int j = 0; j < A16_BN / 8; ++j) {
+        for (int k = 0; k < A16_KB / UK16; ++k)
+          wgmma_f16_n256_mn(d, make_desc(sa + wg * A16_KB * 128 + k * 2048, A16_KB * 128, 1024),
+                            make_desc(sb + k * 2048, A16_KB * 128, 1024), (i | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == A16_STAGES) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      const int m = (tile / p.tiles_n) * A16_BM + wg * 64 + 16 * w + (lane >> 2);
+      const int n0 = (tile % p.tiles_n) * A16_BN + 2 * (lane & 3);
+      if constexpr (VEC4) {
+        // lane pairs (q, q^1) swap half their fragment: the even lane adds 4 consecutive columns of row m, the odd one of row m + 8
+        const bool odd = lane & 1;
+        const int row = odd ? m + 8 : m;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = r0 + 8 * h, n = c0 + 8 * j;
-        if (m < p.M && n < p.N) {            // M, N multiples of 64
-          float* crow = p.C + (int64_t)m * p.ldc + n;
-          atomicAdd(crow, d[4 * j + 2 * h] * sc);
-          atomicAdd(crow + 1, d[4 * j + 2 * h + 1] * sc);
+        for (int j = 0; j < A16_BN / 8; ++j) {
+          const float s0 = odd ? d[4 * j] : d[4 * j + 2], s1 = odd ? d[4 * j + 1] : d[4 * j + 3];
+          const float k0 = odd ? d[4 * j + 2] : d[4 * j], k1 = odd ? d[4 * j + 3] : d[4 * j + 1];
+          const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
+          const int col = n0 + 8 * j - (odd ? 2 : 0);
+          const float4 v = odd ? make_float4(r0 * sc, r1 * sc, k0 * sc, k1 * sc) : make_float4(k0 * sc, k1 * sc, r0 * sc, r1 * sc);
+          if (row < p.M && col < p.N)                  // M, N multiples of 64: a 4-column group is all in or all out
+            red_add_v4(p.C + (int64_t)row * p.ldc + col, v.x, v.y, v.z, v.w);
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < A16_BN / 8; ++j) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = m + 8 * h, col = n0 + 8 * j;
+            const float v0 = d[4 * j + 2 * h] * sc, v1 = d[4 * j + 2 * h + 1] * sc;
+            if (row < p.M && col < p.N) {
+              float* dst = p.C + (int64_t)row * p.ldc + col;
+              atomicAdd(dst, v0);
+              atomicAdd(dst + 1, v1);
+            }
+          }
         }
       }
     }
@@ -746,26 +800,46 @@ void segsum_rows16(LaunchCtx& cx, const __half* X, int64_t ldx, const int32_t* p
   check_launch(cx, "k_segsum16");
 }
 
-// C[M,N] += inv_scale * A^T B, A (K x M) and B (K x N) fp16 row-major
+// one zeroed claim / done counter pair per (device, stream): launches on one stream are ordered, and each leaves it zeroed
+static int* atb16_counter(cudaStream_t stream) {
+  static std::mutex mu;
+  static std::map<std::pair<int, cudaStream_t>, int*> counters;
+  int dev = 0;
+  VD_CUDA_CHECK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  int*& c = counters[{dev, stream}];
+  if (!c) {
+    VD_CUDA_CHECK(cudaMalloc((void**)&c, 2 * sizeof(int)));
+    VD_CUDA_CHECK(cudaMemsetAsync(c, 0, 2 * sizeof(int), stream));
+  }
+  return c;
+}
+
+// C[M,N] += inv_scale * A^T B, A (K x M) and B (K x N) fp16 row-major; stream-K over at most cx.sms() CTAs
 void gemm_atb16(LaunchCtx& cx, int M, int N, int64_t K, const __half* A, int64_t lda, const __half* B, int64_t ldb, float* C,
                 int64_t ldc, const float* inv_scale) {
   using namespace tc;
   VD_REQUIRE(M % 64 == 0 && N % 64 == 0 && K >= A16_KB && lda % 8 == 0 && ldb % 8 == 0, VD_E_STATE, "gemm_atb16: shape");
-  const int tiles = cdiv(M, BM16) * cdiv(N, A16_BN);
-  const int64_t cta_cap = cx.sm_budget > 0 ? cx.sm_budget : 2LL * cx.sm_count;
-  int64_t splits = std::max<int64_t>(1, std::min<int64_t>(cta_cap / tiles, K / (A16_KB * 4)));
-  int64_t kps = ((K + splits - 1) / splits + A16_KB - 1) / A16_KB * A16_KB;
-  splits = (K + kps - 1) / kps;
-  Atb16Params p = {M, N, K, kps, C, ldc, inv_scale};
+  Atb16Params p = {};
+  p.M = M; p.N = N; p.tiles_n = cdiv(N, A16_BN); p.tiles = cdiv(M, A16_BM) * p.tiles_n;
+  VD_REQUIRE((K + A16_KB - 1) / A16_KB <= INT32_MAX, VD_E_STATE, "gemm_atb16: K");
+  p.kbt = (int)((K + A16_KB - 1) / A16_KB);
+  const int64_t sms = cx.sms(), total = (int64_t)p.tiles * p.kbt;
+  p.chunk = (int)std::min<int64_t>(p.kbt, std::max<int64_t>(A16_MIN_CHUNK, cdiv(total, sms * A16_CHUNKS_PER_CTA)));
+  p.num_chunks = p.tiles * cdiv(p.kbt, p.chunk);
+  p.C = C; p.ldc = ldc; p.inv_scale = inv_scale;
+  p.counter = atb16_counter(cx.stream);
   CUtensorMap tA = tmap_h(A, K, M, lda, A16_KB, 64, CU_TENSOR_MAP_SWIZZLE_128B),
               tB = tmap_h(B, K, N, ldb, A16_KB, 64, CU_TENSOR_MAP_SWIZZLE_128B);
   static bool attr_set = false;
   if (!attr_set) {
-    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
     attr_set = true;
   }
-  dim3 grid(tiles, (unsigned)splits);
-  k_atb16<<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
+  const unsigned grid = (unsigned)std::min<int64_t>(sms, p.num_chunks);
+  if (ldc % 4 == 0 && ((uintptr_t)C & 15) == 0) k_atb16<true><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
+  else k_atb16<false><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
   check_launch(cx, "k_atb16");
 }
 

@@ -140,6 +140,30 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        pick_grad_scale(e->cx, CF(0), I[0], static_cast<uint32_t*>(P[1]), F(2));
      }},
+    // ptrs A16, B16, C, inv_scale; ints M, N, K, lda, ldb, ldc, CTAs (0 = the engine's), launches, streams (1 or 2: launch i
+    // goes to stream i % streams, the second one a fresh stream that starts after and ends before the engine's)
+    {"gemm_atb16", 4, 9, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       VD_REQUIRE(I[8] == 1 || I[8] == 2, VD_E_BADARG, "gemm_atb16: streams");
+       LaunchCtx cs[2];
+       for (LaunchCtx& c : cs) { c.sm_count = e->cx.sm_count; c.sm_budget = IN(6); c.stream = e->cx.stream; }
+       cudaEvent_t ev = nullptr;
+       if (I[8] == 2) {
+         VD_CUDA_CHECK(cudaStreamCreateWithFlags(&cs[1].stream, cudaStreamNonBlocking));
+         VD_CUDA_CHECK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+         VD_CUDA_CHECK(cudaEventRecord(ev, cs[0].stream));
+         VD_CUDA_CHECK(cudaStreamWaitEvent(cs[1].stream, ev, 0));
+       }
+       for (int64_t i = 0; i < I[7]; ++i)
+         gemm_atb16(cs[i % I[8]], IN(0), IN(1), I[2], CH16(0), I[3], CH16(1), I[4], F(2), I[5], CF(3));
+       if (I[8] == 2) {
+         VD_CUDA_CHECK(cudaEventRecord(ev, cs[1].stream));
+         VD_CUDA_CHECK(cudaStreamWaitEvent(cs[0].stream, ev, 0));
+         VD_CUDA_CHECK(cudaStreamSynchronize(cs[1].stream));
+         VD_CUDA_CHECK(cudaEventDestroy(ev));
+         VD_CUDA_CHECK(cudaStreamDestroy(cs[1].stream));
+       }
+     }},
     {"segsum_rows16", 5, 3, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        segsum_rows16(e->cx, static_cast<const __half*>(P[0]), I[0], CI32(1), CI32(2), I[1], F(3), IN(2), CF(4));
