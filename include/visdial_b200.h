@@ -150,6 +150,17 @@ int vd_forward_backward(vd_engine* e, const vd_batch* b, int32_t only_forward, f
  * negative, non-finite or zero-sum relevance row. */
 int vd_forward_backward_dense(vd_engine* e, const vd_batch* b, const int32_t* round_host, const float* relevance_host,
                               float* loss_host);
+/* The same step for the gen decoder (DESIGN §16).  b: a gen batch carrying option_in / option_out (vd_corpus_get_batch
+ * mode 2), To its option width; round_host and relevance_host as above.  s_bk = the log-likelihood of option k of round
+ * round_host[b] under the teacher-forced gen decoder started from that round's state, exactly what vd_gen_option_lhood
+ * gives for that row (sum over t of keep * (x_t[tgt_t] - lse_t), keep = input token != 0 and target > 0); the loss is the
+ * soft-target cross-entropy above.  The encoder runs over all rounds (same dropout masks as vd_forward_backward); the
+ * decoder only over the B*numOptions selected option rows, and the encoder receives gradient through the annotated
+ * rounds' initial decoder state only.  Gradients accumulate into dW as vd_forward_backward's do (world > 1: vd_zero_grad
+ * between backward passes).  VD_E_STATE for a disc engine; VD_E_SHAPE for a batch without option_in / option_out;
+ * VD_E_BADARG as vd_forward_backward_dense.  The engine stays usable after any refusal. */
+int vd_forward_backward_dense_gen(vd_engine* e, const vd_batch* b, const int32_t* round_host, const float* relevance_host,
+                                  float* loss_host);
 /* Model:retrieveBatch (model.lua:344-430).  use_gt != 0: ranks_host is (N) = rank of the ground
  * truth; else (N,100) = rank of every option.  Ranks are 1-based; ties: lower index wins. */
 int vd_retrieve(vd_engine* e, const vd_batch* b, int32_t use_gt, int32_t* ranks_host);
@@ -313,7 +324,8 @@ int vd_lstm16_step_bwd(vd_engine* e, int64_t R, int32_t H, const void* da_next16
  * DEVICE buffers, on the
  * engine's stream, then synchronises.  Dropout factors are the engine's own for the seed and iteration of
  * vd_set_dropout_seed (identity unless training mode 1).  VD_E_BADARG for an unknown name or wrong argument counts; a
- * launcher's refusal comes back as its error code. */
+ * launcher's refusal comes back as its error code.  Two entries reach the gen dense step rather than a kernel:
+ * "dense_gen_chunk_bytes" sets its d-logit budget, "dense_scores" copies out the last dense step's (B, numOptions) scores. */
 int vd_test_kernel(vd_engine* e, const char* name, void* const* ptrs, int32_t n_ptrs, const int64_t* ints, int32_t n_ints,
                    const double* reals, int32_t n_reals);
 /* cudaProfilerStart / cudaProfilerStop (ncu --profile-from-start off) */

@@ -38,6 +38,8 @@ int vd_encoder_backward(vd_engine* e, const vd_batch* b, const float* gradEncOut
 int vd_forward_backward(vd_engine* e, const vd_batch* b, int32_t only_forward, float* loss_host);
 int vd_forward_backward_dense(vd_engine* e, const vd_batch* b, const int32_t* round_host, const float* relevance_host,
                               float* loss_host);
+int vd_forward_backward_dense_gen(vd_engine* e, const vd_batch* b, const int32_t* round_host, const float* relevance_host,
+                                  float* loss_host);
 int vd_retrieve(vd_engine* e, const vd_batch* b, int32_t use_gt, int32_t* ranks_host);
 int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
                        int32_t* answer_host, int32_t* length_host, double* score_host);

@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libvisdial_b200.so")
 
 VD_OK = 0
 VD_E_BADARG = -1
+VD_E_SHAPE = -2
 VD_E_STATE = -6
 VD_MATH_TF32 = 0
 VD_MATH_FP32 = 1
@@ -88,6 +89,7 @@ SIGNATURES = {
     "vd_encoder_backward": [_H, _P(vd_batch), C.c_void_p],
     "vd_forward_backward": [_H, _P(vd_batch), C.c_int32, _P(C.c_float)],
     "vd_forward_backward_dense": [_H, _P(vd_batch), C.c_void_p, C.c_void_p, _P(C.c_float)],
+    "vd_forward_backward_dense_gen": [_H, _P(vd_batch), C.c_void_p, C.c_void_p, _P(C.c_float)],
     "vd_retrieve": [_H, _P(vd_batch), C.c_int32, C.c_void_p],
     "vd_compute_ranks": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p],
     "vd_gen_option_lhood": [_H, _P(vd_batch), _P(C.c_void_p)],

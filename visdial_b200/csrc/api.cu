@@ -223,6 +223,14 @@ int vd_forward_backward_dense(vd_engine* h, const vd_batch* b, const int32_t* ro
   })
 }
 
+int vd_forward_backward_dense_gen(vd_engine* h, const vd_batch* b, const int32_t* round_host, const float* relevance_host,
+                                  float* loss_host) {
+  VD_TRY({
+    const float l = ENG(h)->forward_backward_dense_gen(b, round_host, relevance_host);
+    if (loss_host) *loss_host = l;
+  })
+}
+
 int vd_retrieve(vd_engine* h, const vd_batch* b, int32_t use_gt, int32_t* ranks_host) {
   VD_TRY({ ENG(h)->retrieve(b, use_gt, ranks_host); })
 }

@@ -1348,14 +1348,11 @@ void Engine::options_backward(const float* dfeat) {
   }
 }
 
-// vd_forward_backward_dense: the encoder over all N rounds as in vd_forward_backward (same dropout sites and masks), the
-// disc decoder on the one annotated round per dialog only (B*K option rows instead of N*K), the soft-target cross-entropy
-// against the relevance rows, and the encoder backward from a dEnc that is zero on every unselected round.
-float Engine::forward_backward_dense(const vd_batch* b, const int32_t* round_host, const float* relevance_host) {
-  VD_REQUIRE(cfg.dec == DEC_DISC, VD_E_STATE, "dense fine-tuning runs the disc decoder only");
+void Engine::dense_targets(const vd_batch* b, const int32_t* round_host, const float* relevance_host, int32_t** rd_out,
+                           float** rel_out) {
   VD_REQUIRE(b && round_host && relevance_host, VD_E_BADARG, "batch / rounds / relevance is null");
   VD_REQUIRE(b->B > 0, VD_E_SHAPE, "batch B must be > 0");
-  const int B = b->B, R = cfg.R, K = cfg.K, H = cfg.H;
+  const int B = b->B, R = cfg.R, K = cfg.K;
   for (int i = 0; i < B; ++i) {
     VD_REQUIRE(round_host[i] >= 0 && round_host[i] < R, VD_E_BADARG, "round outside [0, maxQuesCount)");
     double sum = 0.0;
@@ -1375,6 +1372,30 @@ float Engine::forward_backward_dense(const vd_batch* b, const int32_t* round_hos
   float* rel = static_cast<float*>(dense_buf[1].ensure((size_t)B * K * sizeof(float)));
   VD_CUDA_CHECK(cudaMemcpyAsync(rd, round_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, main_stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(rel, relevance_host, (size_t)B * K * sizeof(float), cudaMemcpyHostToDevice, main_stream));
+  *rd_out = rd;
+  *rel_out = rel;
+}
+
+float Engine::dense_loss(const float* sc, const float* rel, int B) {
+  const int K = cfg.K;
+  row_loss = arena.get<float>(B);
+  dscores = arena.get<float>((int64_t)B * K);
+  soft_xent(cx, sc, rel, row_loss, dscores, B, K);
+  reduce_sum(cx, row_loss, scalars_dev, B, 1.f / (float)B);
+  float loss = 0.f;
+  VD_CUDA_CHECK(cudaMemcpyAsync(&loss, scalars_dev, sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));                    // read where vd_forward_backward reads its loss
+  return loss;
+}
+
+// vd_forward_backward_dense: the encoder over all N rounds as in vd_forward_backward (same dropout sites and masks), the
+// disc decoder on the one annotated round per dialog only (B*K option rows instead of N*K), the soft-target cross-entropy
+// against the relevance rows, and the encoder backward from a dEnc that is zero on every unselected round.
+float Engine::forward_backward_dense(const vd_batch* b, const int32_t* round_host, const float* relevance_host) {
+  VD_REQUIRE(cfg.dec == DEC_DISC, VD_E_STATE, "dense fine-tuning runs the disc decoder only");
+  int32_t* rd = nullptr; float* rel = nullptr;
+  dense_targets(b, round_host, relevance_host, &rd, &rel);
+  const int B = b->B, R = cfg.R, K = cfg.K, H = cfg.H;
   struct Reset { const int32_t*& p; ~Reset() { p = nullptr; } } reset{dense_round};
   dense_round = rd;
   encoder_forward(b);                             // starts the option LSTM on the selected rows (options_forward_async)
@@ -1391,13 +1412,7 @@ float Engine::forward_backward_dense(const vd_batch* b, const int32_t* round_hos
   gather_round_rows(cx, encOut, rd, enc_sel, B, R, H);
   scores = arena.get<float>((int64_t)B * K);
   disc_scores_fwd(cx, opt.h_last(), enc_sel, scores, B, K, H);
-  row_loss = arena.get<float>(B);
-  dscores = arena.get<float>((int64_t)B * K);
-  soft_xent(cx, scores, rel, row_loss, dscores, B, K);
-  reduce_sum(cx, row_loss, scalars_dev, B, 1.f / (float)B);
-  float loss = 0.f;
-  VD_CUDA_CHECK(cudaMemcpyAsync(&loss, scalars_dev, sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));                    // read where vd_forward_backward reads its loss
+  const float loss = dense_loss(scores, rel, B);
   float* dfeat = arena.get<float>((int64_t)B * K * H);
   float* denc_sel = arena.get<float>((int64_t)B * H);
   disc_scores_bwd(cx, dscores, opt.h_last(), enc_sel, dfeat, denc_sel, B, K, H);
@@ -1405,6 +1420,133 @@ float Engine::forward_backward_dense(const vd_batch* b, const int32_t* round_hos
   dEncFromDec = arena.get<float>(db.N * H);
   scatter_round_rows(cx, denc_sel, rd, dEncFromDec, B, R, H);
   encoder_backward(dEncFromDec);
+  return loss;
+}
+
+// vd_forward_backward_dense_gen (DESIGN §16): the encoder over all N rounds as in vd_forward_backward; the gen decoder,
+// teacher-forced, over the K candidate answers of the annotated round of each dialog only (B*K rows), started from that
+// round's forward_connect() state; the scores s_bk = sum_t keep (x_t[tgt_t] - lse_t) as gen_option_lhood forms them; the
+// soft-target cross-entropy; and the backward with d-logits  -g_bk keep (softmax(x_t) - onehot(tgt_t)),  g = dscores.
+float Engine::forward_backward_dense_gen(const vd_batch* b, const int32_t* round_host, const float* relevance_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "the gen dense step runs the gen decoder only");
+  int32_t* rd = nullptr; float* rel = nullptr;
+  dense_targets(b, round_host, relevance_host, &rd, &rel);
+  VD_REQUIRE(b->option_in && b->option_out && b->To > 0, VD_E_SHAPE, "gen dense step: option_in / option_out / To missing");
+  encoder_forward(b);
+  VD_REQUIRE(save_acts, VD_E_STATE, "the dense step needs a training-mode forward");
+  if (world > 1)
+    for (char c : seg_reduced)
+      VD_REQUIRE(!c, VD_E_STATE, "world > 1: vd_zero_grad is required between backward passes (gradients already all-reduced)");
+  cx.stream = main_stream;
+  forward_connect();
+  const int B = b->B, R = cfg.R, K = cfg.K, E = cfg.E, H = cfg.H, V = cfg.V, To = db.To;
+  const int64_t Ro = (int64_t)B * K, TR = (int64_t)To * Ro;
+  // the annotated rounds' option tokens, time-major (To, B*K) as the disc options are taken
+  int32_t* oi = arena.get<int32_t>(TR);
+  int32_t* oo = arena.get<int32_t>(TR);
+  transpose_ids_rounds(cx, db.option_in, rd, oi, B, R, K, To);
+  transpose_ids_rounds(cx, db.option_out, rd, oo, B, R, K, To);
+  // initial state: row b*K + k <- round rd[b] of dialog b (null layer-1 state stays null: encoders without .rnnLayers)
+  const float* st0[4] = {gen_h0[0], gen_h0[1], gen_c0[0], gen_c0[1]};
+  const float* st[4] = {nullptr, nullptr, nullptr, nullptr};
+  float* sel = arena.get<float>((int64_t)B * H);
+  for (int i = 0; i < 4; ++i) {
+    if (!st0[i]) continue;
+    float* t = arena.get<float>(Ro * H);
+    gather_round_rows(cx, st0[i], rd, sel, B, R, H);
+    repeat_rows(cx, t, sel, B, K, H);
+    st[i] = t;
+  }
+  // decoders/gen.lua:3-27 over the selected options, activations saved (decoder_forward's kernels)
+  float* xo = arena.get<float>(TR * E);
+  embed_rows(cx, xo, Wp(0), oi, TR, E, dropcfg(0.f), 0);
+  LstmRun l1 = make_run(To, Ro, E, H, seg("dec.lstm1.weight"), xo, nullptr, oi);
+  l1.h0 = st[0]; l1.c0 = st[2];
+  lstm_forward(l1, true);
+  LstmRun l2 = make_run(To, Ro, H, H, seg("dec.lstm2.weight"), l1.h, nullptr, oi);
+  l2.h0 = st[1]; l2.c0 = st[3];
+  lstm_forward(l2, true);
+  // per-step vocabulary statistics on gen_option_lhood's two routes; lse (To, B*K) is kept for the backward
+  const int wo = seg("dec.out.weight");
+  float* lse = arena.get<float>(TR);
+  scores = arena.get<float>(Ro);
+  VD_CUDA_CHECK(cudaMemsetAsync(scores, 0, (size_t)Ro * sizeof(float), cx.stream));
+  bool fused = tcmode();
+  for (int t = 0; t < To && fused; ++t) fused = vocab_tc_ok((int)Ro, V, H, l2.h + (int64_t)t * Ro * H, H, Wp(wo), H);
+  if (fused) {
+    const int nparts = vocab_lse_nparts(V);
+    float* pm = arena.get<float>(Ro * nparts);
+    float* ps = arena.get<float>(Ro * nparts);
+    float* tl = arena.get<float>(Ro);
+    for (int t = 0; t < To; ++t) {
+      const int64_t o = (int64_t)t * Ro;
+      {
+        LaunchCtx::Scope sc(&cx, "vocab_lse", 2.0 * Ro * V * H, 4.0 * (Ro * (double)H + (double)V * H + 2.0 * Ro * nparts));
+        const bool ok = vocab_lse_tc(cx, (int)Ro, V, H, l2.h + o * H, H, Wp(wo), H, Wp(wo + 1), oo + o, pm, ps, tl);
+        VD_REQUIRE(ok, VD_E_STATE, "vocab_lse_tc refused a shape vocab_tc_ok took");
+      }
+      vocab_lse_finish(cx, pm, ps, nparts, tl, oo + o, oi + o, lse + o, scores, 1.f, 1, Ro);
+    }
+  } else {
+    float* logits = arena.get<float>(Ro * V);
+    for (int t = 0; t < To; ++t) {
+      const int64_t o = (int64_t)t * Ro;
+      linear_fwd(wo, l2.h + o * H, Ro, logits, 0);
+      LaunchCtx::Scope sc(&cx, "vocab_lse_rows", 0.0, 4.0 * Ro * (double)V);
+      lhood_accumulate(cx, logits, oo + o, oi + o, scores, Ro, V, lse + o);
+    }
+  }
+  const float loss = dense_loss(scores, rel, B);
+  float* nscale = arena.get<float>(Ro);
+  scale_copy(cx, nscale, dscores, Ro, -1.f);        // d loss / d s_bk = g_bk; s_bk enters the logits with sign -1
+  // d-logits a chunk of time steps at a time: at most dense_gen_chunk_bytes of them live (never (To*B*K, V)); per chunk,
+  // dec.out's dW / db accumulate and the chunk's rows of dh2 (the gradient at layer 2's outputs) are written
+  float* dh2 = arena.get<float>(TR * H);
+  const int64_t step_bytes = Ro * V * (int64_t)sizeof(float);
+  const int per_chunk = (int)std::max<int64_t>(1, std::min<int64_t>(To, dense_gen_chunk_bytes / step_bytes));
+  const Arena::Mark mk = arena.mark();
+  for (int t0 = 0; t0 < To; t0 += per_chunk) {
+    const int nt = std::min(per_chunk, To - t0);
+    arena.rewind(mk);
+    float* dl = arena.get<float>((int64_t)nt * Ro * V);
+    for (int t = t0; t < t0 + nt; ++t) {
+      const int64_t o = (int64_t)t * Ro;
+      float* dlt = dl + (int64_t)(t - t0) * Ro * V;
+      if (fused) {
+        LaunchCtx::Scope sc(&cx, "vocab_dlogits", 2.0 * Ro * V * H, 4.0 * Ro * (double)V);
+        const bool ok = vocab_dlogits_tc(cx, (int)Ro, V, H, l2.h + o * H, H, Wp(wo), H, Wp(wo + 1), oo + o, oi + o, lse + o, dlt, V,
+                                         nscale);
+        VD_REQUIRE(ok, VD_E_STATE, "vocab_dlogits_tc refused a shape vocab_lse_tc took");
+      } else {
+        linear_fwd(wo, l2.h + o * H, Ro, dlt, 0);
+        LaunchCtx::Scope sc(&cx, "vocab_dlogits_rows", 0.0, 8.0 * Ro * (double)V);
+        nll_bwd_scaled(cx, dlt, lse + o, oo + o, oi + o, nscale, dlt, Ro, V);
+      }
+    }
+    linear_bwd(wo, l2.h + (int64_t)t0 * Ro * H, dl, (int64_t)nt * Ro, dh2 + (int64_t)t0 * Ro * H, 0.f);
+  }
+  arena.rewind(mk);
+  // BPTT through both layers, then the embedding gradient of option_in (decoder_backward's kernels)
+  float* dst[4] = {nullptr, nullptr, nullptr, nullptr};      // d(h0, c0) per option row, for the initial states that exist
+  for (int i = 0; i < 4; ++i) if (st[i]) dst[i] = arena.get<float>(Ro * H);
+  float* dx2 = arena.get<float>(TR * H);
+  lstm_backward(l2, dh2, nullptr, nullptr, dx2, dst[1], dst[3]);
+  float* dx1 = arena.get<float>(TR * E);
+  lstm_backward(l1, dx2, nullptr, nullptr, dx1, dst[0], dst[2]);
+  embed_scatter_add(cx, dWp(0), dx1, E, oi, TR, E, dropcfg(0.f), 0);
+  // the K options' initial-state gradients summed per dialog (fixed k order, no atomics), onto the annotated round
+  float** gout[4] = {&gen_dh0[0], &gen_dh0[1], &gen_dc0[0], &gen_dc0[1]};
+  for (int i = 0; i < 4; ++i) {
+    *gout[i] = nullptr;
+    if (!dst[i]) continue;
+    *gout[i] = arena.get<float>(db.N * H);
+    {
+      LaunchCtx::Scope sc(&cx, "dense_state_sum", (double)Ro * H, 4.0 * (Ro + B) * (double)H);
+      sum_repeated_rows(cx, sel, dst[i], B, K, H);
+    }
+    scatter_round_rows(cx, sel, rd, *gout[i], B, R, H);
+  }
+  encoder_backward(backward_connect());
   return loss;
 }
 

@@ -269,6 +269,16 @@ struct Engine {
   const int32_t* dense_round = nullptr;
   GrowBuf dense_buf[2];              // the step's rounds and relevance rows, uploaded before the encoder forward
   float forward_backward_dense(const vd_batch* b, const int32_t* round_host, const float* relevance_host);
+  // what both dense steps share: the argument checks, the upload into dense_buf (rd (B), rel (B, K) on return), and the
+  // soft-target cross-entropy of the (B, K) scores with its loss readback (dscores on return)
+  void dense_targets(const vd_batch* b, const int32_t* round_host, const float* relevance_host, int32_t** rd, float** rel);
+  float dense_loss(const float* sc, const float* rel, int B);
+  // the gen dense step (vd_forward_backward_dense_gen, DESIGN §16): the scores are the annotated rounds' option
+  // log-likelihoods.  Its backward writes the vocabulary d-logits dense_gen_chunk_bytes at a time (kDenseGenChunkBytes
+  // unless a test sets it; at least one time step per chunk)
+  static constexpr int64_t kDenseGenChunkBytes = (int64_t)256 << 20;
+  int64_t dense_gen_chunk_bytes = kDenseGenChunkBytes;
+  float forward_backward_dense_gen(const vd_batch* b, const int32_t* round_host, const float* relevance_host);
   std::vector<cudaEvent_t> ev_pool;
   cudaEvent_t pool_event(size_t i);
   void lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last, float* dx_out,

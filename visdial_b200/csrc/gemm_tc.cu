@@ -31,7 +31,8 @@ enum { MODE_GENERIC = 0, MODE_LSTM_FWD = 1, MODE_LSTM_BWD = 2, MODE_LSE = 3, MOD
 // MODE_LSE    : vocabulary projection whose (rows, V) logits never leave the chip: per row and column slice only the running
 //               max, the sum of exponentials and the target's logit are written (gen.lua:23-24 + the criterion of model.lua:33-36
 //               / utils.computeLhood, utils.lua:86-102)
-// MODE_DLOGIT : the same contraction recomputed in the backward pass with the epilogue  C = keep * (exp(x - lse[row]) - onehot)
+// MODE_DLOGIT : the same contraction recomputed in the backward pass with the epilogue  C = keep * (exp(x - lse[row]) - onehot),
+//               times row_scale[row] when a scale is given (the dense gen step's per-option weight, DESIGN §16)
 // MODE_SAMPLE : MODE_LSE's statistics plus the slice's best Gumbel key x / T + g (common.cuh), its class and its logit
 //               (the sampling step of model.lua:584-593 without the logits in HBM)
 
@@ -49,6 +50,7 @@ struct Params {
   const float* gsave; const float* c_cur; const float* dh_ext; float* dc_carry; float* da;
   // fused vocabulary softmax (MODE_LSE / MODE_DLOGIT): 1-based target class per row (0 = none), maskzero ids per row
   const int32_t* tgt; const int32_t* row_ids; const float* lse;
+  const float* row_scale;         // MODE_DLOGIT: optional per-row factor of the d-logits (null: none)
   float* part_max; float* part_sum; float* tgt_logit; int nparts;      // (M, nparts) partials, nparts = column tiles * slices
   // MODE_SAMPLE: (M, nparts) best key, its class and its logit
   float* part_key; int32_t* part_cls; float* part_x; SampleCfg smp;
@@ -358,11 +360,21 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
               const int tg = row_ok ? p.tgt[row] : 0;
               const bool keepr = row_ok && tg > 0 && p.row_ids[row] != 0;
               const float l = keepr ? p.lse[row] : 0.f;
+              if (p.row_scale) {
+                const float s = keepr ? p.row_scale[row] : 0.f;
 #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const int n = n0 + c + sub * 8 + j;
-                const float x = v[j] + ((p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f);
-                v[j] = keepr ? __expf(x - l) - (n == tg - 1 ? 1.f : 0.f) : 0.f;
+                for (int j = 0; j < 8; ++j) {
+                  const int n = n0 + c + sub * 8 + j;
+                  const float x = v[j] + ((p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f);
+                  v[j] = keepr ? s * (__expf(x - l) - (n == tg - 1 ? 1.f : 0.f)) : 0.f;
+                }
+              } else {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                  const int n = n0 + c + sub * 8 + j;
+                  const float x = v[j] + ((p.bias && n < p.N) ? __ldg(p.bias + n) : 0.f);
+                  v[j] = keepr ? __expf(x - l) - (n == tg - 1 ? 1.f : 0.f) : 0.f;
+                }
               }
             } else {
 #pragma unroll
@@ -746,13 +758,15 @@ bool vocab_sample_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t
   launch<128, MODE_SAMPLE>(cx, tA, tB, p, cdiv(M, BM) * cdiv(N, 128));
   return true;
 }
-// C[m,n] = keep[m] * (exp(A B^T + bias - lse[m]) - [n == tgt[m]-1])   (backward of log-softmax + ClassNLL, recomputed)
+// C[m,n] = keep[m] * (exp(A B^T + bias - lse[m]) - [n == tgt[m]-1])   (backward of log-softmax + ClassNLL, recomputed),
+// times row_scale[m] when row_scale is not null
 bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
-                      const int32_t* tgt, const int32_t* row_ids, const float* lse, float* C, int64_t ldc) {
+                      const int32_t* tgt, const int32_t* row_ids, const float* lse, float* C, int64_t ldc, const float* row_scale) {
   using namespace tc;
   if (!vocab_tc_ok(M, N, K, A, lda, B, ldb) || !tma_ok(C, ldc)) return false;
   Params p = {};
   p.M = M; p.N = N; p.K = K; p.C = C; p.ldc = ldc; p.bias = bias; p.tgt = tgt; p.row_ids = row_ids; p.lse = lse;
+  p.row_scale = row_scale;
   EpiMaps em = {};
   em.g4 = make_tmap(C, M, N, ldc, 32, 16, CU_TENSOR_MAP_SWIZZLE_64B);
   CUtensorMap tA = make_tmap(A, M, K, lda, BM), tB = make_tmap(B, N, K, ldb, 128);

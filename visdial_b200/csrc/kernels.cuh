@@ -27,7 +27,8 @@ bool vocab_tc_ok(int M, int N, int K, const float* A, int64_t lda, const float* 
 bool vocab_lse_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
                   const int32_t* tgt, float* part_max, float* part_sum, float* tgt_logit);
 bool vocab_dlogits_tc(LaunchCtx& cx, int M, int N, int K, const float* A, int64_t lda, const float* B, int64_t ldb, const float* bias,
-                      const int32_t* tgt, const int32_t* row_ids, const float* lse, float* C, int64_t ldc);
+                      const int32_t* tgt, const int32_t* row_ids, const float* lse, float* C, int64_t ldc,
+                      const float* row_scale = nullptr);   // row_scale: C[m,:] *= row_scale[m] (null: today's epilogue)
 // lse[r] from the partials; then  out[r] (+)= keep ? sign * (tgt_logit[r] - lse[r]) : 0   (keep: row id != 0 and target > 0)
 void vocab_lse_finish(LaunchCtx& cx, const float* part_max, const float* part_sum, int nparts, const float* tgt_logit,
                       const int32_t* tgt, const int32_t* row_ids, float* lse, float* out, float sign, int accumulate, int64_t rows);
@@ -136,8 +137,15 @@ void logsoftmax_rows(LaunchCtx& cx, float* logits, const int32_t* mask_ids, int6
 void nll_fwd(LaunchCtx& cx, const float* logp, const int32_t* tgt, const int32_t* mask_ids, float* row_loss, int64_t rows, int V);
 void nll_bwd(LaunchCtx& cx, const float* logp, const int32_t* tgt, const int32_t* mask_ids, float* dlogits, int64_t rows, int V);
 // utils.computeLhood (utils.lua:86-102) from raw logits: lh[r] += logits[r,tgt-1] - logsumexp(logits[r,:])
+// (lse, when not null, receives logsumexp(logits[r,:]) of the kept rows)
 void lhood_accumulate(LaunchCtx& cx, const float* logits, const int32_t* tgt, const int32_t* mask_ids, float* lh,
-                      int64_t rows, int V);
+                      int64_t rows, int V, float* lse = nullptr);
+// nll_bwd on raw logits with a per-row factor: dlogits[r,:] = keep ? scale[r] * (exp(logits[r,:] - lse[r]) - onehot) : 0
+// (the dense gen step's rows route; dlogits may alias logits)
+void nll_bwd_scaled(LaunchCtx& cx, const float* logits, const float* lse, const int32_t* tgt, const int32_t* mask_ids,
+                    const float* scale, float* dlogits, int64_t rows, int V);
+// dst[i] = alpha * src[i]
+void scale_copy(LaunchCtx& cx, float* dst, const float* src, int64_t n, float alpha);
 
 // beam search on the device (model.lua:510-570): state shuffle by parent index
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H);

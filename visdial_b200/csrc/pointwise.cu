@@ -1188,7 +1188,7 @@ __global__ void k_nll_bwd(const float* __restrict__ logp, const int32_t* __restr
 }
 // block per row of raw logits
 __global__ void k_lhood_accumulate(const float* __restrict__ logits, const int32_t* __restrict__ tgt,
-                                   const int32_t* __restrict__ mask_ids, float* __restrict__ lh, int V) {
+                                   const int32_t* __restrict__ mask_ids, float* __restrict__ lh, int V, float* __restrict__ lse) {
   __shared__ float red[33];
   const int64_t r = blockIdx.x;
   if (mask_ids[r] == 0 || tgt[r] <= 0) return;      // gen.lua:23-24 MaskZero rows are zero; utils.lua:92-97
@@ -1199,7 +1199,24 @@ __global__ void k_lhood_accumulate(const float* __restrict__ logits, const int32
   float sum = 0.f;
   for (int c = threadIdx.x; c < V; c += blockDim.x) sum += expf(row[c] - mx);
   sum = block_sum(sum, red);
-  if (threadIdx.x == 0) lh[r] += row[tgt[r] - 1] - (mx + logf(sum));
+  if (threadIdx.x == 0) {
+    const float l = mx + logf(sum);
+    lh[r] += row[tgt[r] - 1] - l;
+    if (lse) lse[r] = l;
+  }
+}
+__global__ void k_nll_bwd_scaled(const float* logits, const float* __restrict__ lse, const int32_t* __restrict__ tgt,
+                                 const int32_t* __restrict__ mask_ids, const float* __restrict__ scale, float* dlogits,
+                                 int64_t total, int V) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  int64_t r = i / V; int c = (int)(i % V);
+  bool keep = mask_ids[r] != 0 && tgt[r] > 0;
+  dlogits[i] = keep ? scale[r] * (expf(logits[i] - lse[r]) - (c == tgt[r] - 1 ? 1.f : 0.f)) : 0.f;
+}
+__global__ void k_scale_copy(float* __restrict__ dst, const float* __restrict__ src, int64_t n, float alpha) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = alpha * src[i];
 }
 
 __global__ void k_clamp_adam(float* __restrict__ W, float* __restrict__ dW, float* __restrict__ m, float* __restrict__ v,
@@ -1533,11 +1550,16 @@ void nll_bwd(LaunchCtx& cx, const float* logp, const int32_t* tgt, const int32_t
   L1D(k_nll_bwd, rows * V, logp, tgt, mask_ids, dlogits, rows * V, V);
 }
 void lhood_accumulate(LaunchCtx& cx, const float* logits, const int32_t* tgt, const int32_t* mask_ids, float* lh, int64_t rows,
-                      int V) {
+                      int V, float* lse) {
   if (rows <= 0) return;
-  k_lhood_accumulate<<<(int)rows, 256, 0, cx.stream>>>(logits, tgt, mask_ids, lh, V);
+  k_lhood_accumulate<<<(int)rows, 256, 0, cx.stream>>>(logits, tgt, mask_ids, lh, V, lse);
   check_launch(cx, "lhood_accumulate");
 }
+void nll_bwd_scaled(LaunchCtx& cx, const float* logits, const float* lse, const int32_t* tgt, const int32_t* mask_ids,
+                    const float* scale, float* dlogits, int64_t rows, int V) {
+  L1D(k_nll_bwd_scaled, rows * V, logits, lse, tgt, mask_ids, scale, dlogits, rows * V, V);
+}
+void scale_copy(LaunchCtx& cx, float* dst, const float* src, int64_t n, float alpha) { L1D(k_scale_copy, n, dst, src, n, alpha); }
 void vocab_lse_finish(LaunchCtx& cx, const float* part_max, const float* part_sum, int nparts, const float* tgt_logit,
                       const int32_t* tgt, const int32_t* row_ids, float* lse, float* out, float sign, int accumulate, int64_t rows) {
   L1D(k_vocab_lse_finish, rows, part_max, part_sum, nparts, tgt_logit, tgt, row_ids, lse, out, sign, accumulate, rows);

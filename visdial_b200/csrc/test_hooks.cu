@@ -193,6 +193,17 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        e->pool_topk(CF(0), I[1], I[0], CF(1), I[2], IN(3), IN(4), F(2), I32(3));
      }},
+    // ---- the gen dense step's d-logit budget in bytes (ints[0] <= 0: the default, Engine::kDenseGenChunkBytes)
+    {"dense_gen_chunk_bytes", 0, 1, 0,
+     [](Engine* e, void* const*, const int64_t* I, const double*) {
+       e->dense_gen_chunk_bytes = I[0] > 0 ? I[0] : Engine::kDenseGenChunkBytes;
+     }},
+    // the (B, numOptions) scores of the last dense step into the device floats at ptrs[0]; ints B * numOptions
+    {"dense_scores", 1, 1, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       VD_REQUIRE(e->scores && I[0] > 0, VD_E_STATE, "dense_scores: no step has run");
+       VD_CUDA_CHECK(cudaMemcpyAsync(P[0], e->scores, (size_t)I[0] * sizeof(float), cudaMemcpyDeviceToDevice, e->cx.stream));
+     }},
     // ---- small helpers
     {"colsum_add", 2, 3, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) { colsum_add(e->cx, F(0), CF(1), I[0], IN(1), I[2]); }},

@@ -271,11 +271,12 @@ class Dataloader:
         return self.corpus["train"].get_batch(inds, 0 if params["decoder"] == "disc" else 1)   # :329-337
 
     def getDenseTrainBatch(self, params: dict, dense):
-        """A disc training batch of `batchSize` annotated entries of `dense` (visdial_b200.dense.read against the train
-        split), drawn uniformly with replacement with this rank's generator.  Returns (batch, the 0-based annotated round
-        of each dialog (B,), their relevance rows (B, numOptions))."""
+        """A training batch of `batchSize` annotated entries of `dense` (visdial_b200.dense.read against the train
+        split), drawn uniformly with replacement with this rank's generator: a disc batch for disc models, a batch with
+        option_in / option_out (getTestBatch's gen layout) for gen models.  Returns (batch, the 0-based annotated round of
+        each dialog (B,), their relevance rows (B, numOptions))."""
         pick = self.rng.integers(0, len(dense), size=int(params["batchSize"]))
-        batch = self.corpus["train"].get_batch(dense.dialog[pick], 0)
+        batch = self.corpus["train"].get_batch(dense.dialog[pick], 0 if params["decoder"] == "disc" else 2)
         return batch, (dense.round_id[pick] - 1).astype(np.int32), dense.relevance[pick]
 
     def getIndexData(self, inds0, params: dict, dtype: str) -> DeviceBatch:

@@ -328,6 +328,22 @@ class Engine:
         self._enc_rows = self._N(batch)
         return loss.value
 
+    def forward_backward_dense_gen(self, batch: Batch, rounds, relevance) -> float:
+        """vd_forward_backward_dense_gen: the same step for the gen decoder, whose scores are the annotated rounds' option
+        log-likelihoods.  batch carries option_in / option_out (a mode-2 batch); rounds and relevance as
+        forward_backward_dense."""
+        B, K = batch.c.B, self.params["numOptions"]
+        rounds = np.ascontiguousarray(rounds, dtype=np.int32).reshape(-1)
+        relevance = np.ascontiguousarray(relevance, dtype=np.float32)
+        if rounds.shape != (B,) or relevance.shape != (B, K):
+            raise ValueError("rounds must be (%d,) and relevance (%d, %d)" % (B, B, K))
+        loss = C.c_float()
+        self._enc_rows = None
+        check(self.lib.vd_forward_backward_dense_gen(self.h, C.byref(batch.c), rounds.ctypes.data, relevance.ctypes.data,
+                                                     C.byref(loss)))
+        self._enc_rows = self._N(batch)
+        return loss.value
+
     def retrieve(self, batch: Batch, use_gt: bool = True) -> np.ndarray:
         N = self._N(batch)
         out = np.empty((N,) if use_gt else (N, self.params["numOptions"]), dtype=np.int32)

@@ -12,8 +12,8 @@ from __future__ import annotations
 from . import cli, train
 
 
-def dense_iteration(model, dl, opt, say):
-    """train.main's iteration hook: Model.trainIterationDense over the annotated dialogs of the train split."""
+def read_annotations(model, dl, opt, say):
+    """opt's denseAnnotations read against the train split, with the counts finetune prints."""
     from . import dense
     K = model.params["numOptions"]
     ann = dense.read(opt["denseAnnotations"], K, unique_img=dl.unique_img_train,
@@ -23,6 +23,12 @@ def dense_iteration(model, dl, opt, say):
     if len(ann) == 0:
         raise ValueError("%s has no usable annotated round" % opt["denseAnnotations"])
     say("%d annotated rounds" % len(ann))
+    return ann
+
+
+def dense_iteration(model, dl, opt, say):
+    """train.main's iteration hook: Model.trainIterationDense over the annotated dialogs of the train split."""
+    ann = read_annotations(model, dl, opt, say)
     return (lambda: model.trainIterationDense(dl, ann)), len(ann)
 
 

@@ -94,6 +94,19 @@ class Model:
         self._finish_iteration(curLoss)
         return curLoss
 
+    def trainIterationDenseGen(self, dataloader, dense):
+        """trainIterationDense for gen models (vd_forward_backward_dense_gen): the scores of the annotated round's options
+        are their log-likelihoods under the decoder, the ones evaluate ranks gen models by."""
+        if self.params["decoder"] != "gen":
+            raise ValueError("trainIterationDenseGen needs a gen model")
+        self.wrapper.zeroGradParameters()
+        batch, rounds, relevance = dataloader.getDenseTrainBatch(self.params, dense)
+        self.iteration += 1
+        self.engine.set_dropout_seed(self.params.get("seed", 1234), self.iteration)
+        curLoss = self.engine.forward_backward_dense_gen(batch, rounds, relevance)
+        self._finish_iteration(curLoss)
+        return curLoss
+
     def _finish_iteration(self, cur):
         self.runningLoss = 0.95 * self.runningLoss + 0.05 * cur if self.runningLoss > 0 else cur
         # model.lua:96-99 clamp(-5,5) + adam, fused with the gradient all-reduce when world > 1
