@@ -319,12 +319,14 @@ int vd_lstm16_step_fwd(vd_engine* e, int64_t R, int32_t H, const void* h_prev16,
                        float* c_out, void* h16_out, float* h32_out);
 int vd_lstm16_step_bwd(vd_engine* e, int64_t R, int32_t H, const void* da_next16, const void* Whb16, const void* gates16,
                        const float* c_prev, const float* c_cur, float* dc_carry, const int32_t* mask_ids, void* da16);
-/* test hook of the engine's pointwise, attention, criterion, decoding and encoder-pair LSTM kernels: calls the launcher
+/* test hook of the engine's pointwise, attention, criterion, decoding and encoder-pair LSTM kernels and of its fused
+ * vocabulary projections (the softmax-statistics, d-logit and sampling epilogues of the tensor-core GEMM): calls the launcher
  * `name` (the table in visdial_b200/csrc/test_hooks.cu lists each one's pointer / int / real arguments) on caller-provided
  * DEVICE buffers, on the
  * engine's stream, then synchronises.  Dropout factors are the engine's own for the seed and iteration of
  * vd_set_dropout_seed (identity unless training mode 1).  VD_E_BADARG for an unknown name or wrong argument counts; a
- * launcher's refusal comes back as its error code.  Two entries reach the gen dense step rather than a kernel:
+ * launcher's refusal comes back as its error code; a fused vocabulary projection refuses a shape with VD_E_SHAPE and launches
+ * nothing.  Two entries reach the gen dense step rather than a kernel:
  * "dense_gen_chunk_bytes" sets its d-logit budget, "dense_scores" copies out the last dense step's (B, numOptions) scores. */
 int vd_test_kernel(vd_engine* e, const char* name, void* const* ptrs, int32_t n_ptrs, const int64_t* ints, int32_t n_ints,
                    const double* reals, int32_t n_reals);

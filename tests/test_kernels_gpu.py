@@ -20,7 +20,7 @@ import torch
 
 import dense_oracle
 import sampling_twin
-from helpers import Buf, call, run, small_params, within
+from helpers import ISENT, Pool, call, run, small_params, within
 from oracle import philox
 from oracle import visdial_oracle as O
 from visdial_b200 import Engine
@@ -31,63 +31,10 @@ pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
 TANH_E_ABS = 3e-7            # tanh_e: __expf (2 ulp near 0, i.e. ~2.4e-7 absolute on 1 - e) and __fdividef
 ULP_FN = 4 * U               # relative error of one expf / logf / tanhf, with margin
-G = 64                       # guard elements on each side of every buffer (256 bytes keeps float4 alignment)
-ISENT = -123456789           # int32 guard sentinel of outputs
 SEED, ITER = 0x1234_5678_9ABC, 7
 
 
 # ---------------------------------------------------------------------------------------------- plumbing
-class Dev:
-    """A device copy of array x between guard bands.  Float buffers use NaN guards, int32 inputs 0 (a stray id read stays
-    in bounds), int32 outputs the sentinel; fp16 buffers are passed as uint16 bit patterns with 0x7e00 (NaN) guards."""
-
-    def __init__(self, eng, x, guard_fill=None):
-        x = np.ascontiguousarray(x)
-        self.shape, self.n, self.dtype = x.shape, x.size, x.dtype
-        if guard_fill is None:
-            guard_fill = {np.dtype(np.float32): np.nan, np.dtype(np.int32): 0, np.dtype(np.uint16): 0x7e00,
-                          np.dtype(np.uint32): 0}[x.dtype]
-        self.fill = guard_fill
-        img = np.full(self.n + 2 * G, guard_fill, x.dtype)
-        img[G:G + self.n] = x.reshape(-1)
-        self.buf = Buf(eng, img)
-
-    def ptr(self, off=0):
-        return self.buf.ptr(G + off)
-
-    def get(self):
-        img = self.buf.get()
-        guard = np.concatenate([img[:G], img[G + self.n:]])
-        if self.dtype == np.float32 and np.isnan(self.fill):
-            assert np.isnan(guard).all(), "a kernel wrote outside its output"
-        else:
-            assert (guard == self.fill).all(), "a kernel wrote outside its output"
-        return img[G:G + self.n].reshape(self.shape)
-
-    def free(self):
-        self.buf.free()
-
-
-class Pool:
-    def __init__(self, eng):
-        self.eng, self.bufs = eng, []
-
-    def __call__(self, x, guard_fill=None):
-        d = Dev(self.eng, x, guard_fill)
-        self.bufs.append(d)
-        return d
-
-    def out(self, shape, dtype=np.float32):
-        """an "out =" buffer: NaN (or sentinel) inside and outside"""
-        fill = {np.float32: np.nan, np.int32: ISENT, np.uint16: 0x7e00}[dtype]
-        return self(np.full(shape, fill, dtype), fill)
-
-    def free(self):
-        for d in self.bufs:
-            d.free()
-        self.bufs = []
-
-
 @pytest.fixture(scope="module")
 def eng():
     e = Engine(small_params("lf-ques", "disc"))

@@ -1,5 +1,5 @@
-// vd_test_kernel: the kernels.cuh launchers of pointwise.cu, lstm16.cu's streaming helpers and enc_lstm.cu's persistent
-// encoder LSTM pair, called by name on caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory
+// vd_test_kernel: the kernels.cuh launchers of pointwise.cu, lstm16.cu's streaming helpers, enc_lstm.cu's persistent
+// encoder LSTM pair and gemm_tc.cu's fused vocabulary projections, called by name on caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory
 // attribute and route are the engine's own.  The table below is the whole surface: name, pointer / int / real counts, and the call.
 //   dropout:  p = reals[0], the site an int; the factors are Engine::dropcfg(p)'s (identity unless training == 1).
 //   sampling: SampleCfg from ints (seed, step, row_offset, row_stride) and reals (temperature).
@@ -115,6 +115,42 @@ const Entry TABLE[] = {
        s.seed_lo = (uint32_t)(uint64_t)I[3]; s.seed_hi = (uint32_t)((uint64_t)I[3] >> 32); s.step = (uint32_t)I[4];
        s.temperature = (float)X[0]; s.row_offset = I[5]; s.row_stride = I[6];
        logsoftmax_sample_rows(e->cx, CF(0), I[0], IN(1), s, IN(2), I32(1), I32(2), F(3));
+     }},
+    // ptrs logits, lse, tgt, mask_ids, scale, dlogits (may alias logits); ints rows, V
+    {"nll_bwd_scaled", 6, 2, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       nll_bwd_scaled(e->cx, CF(0), CF(1), CI32(2), CI32(3), CF(4), F(5), I[0], IN(1));
+     }},
+    {"scale_copy", 2, 1, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) { scale_copy(e->cx, F(0), CF(1), I[0], (float)X[0]); }},
+    // ---- fused vocabulary projections (gemm_tc.cu): a shape vocab_tc_ok refuses comes back as VD_E_SHAPE, nothing launched.
+    // ptrs A, B, bias, tgt, part_max, part_sum, tgt_logit; ints M, N, K, lda, ldb
+    {"vocab_lse_tc", 7, 5, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       VD_REQUIRE(vocab_lse_tc(e->cx, IN(0), IN(1), IN(2), CF(0), I[3], CF(1), I[4], CF(2), CI32(3), F(4), F(5), F(6)), VD_E_SHAPE,
+                  "vocab_lse_tc: shape refused");
+     }},
+    // ptrs A, B, bias, tgt, row_ids, lse, C, row_scale (null: unscaled); ints M, N, K, lda, ldb, ldc
+    {"vocab_dlogits_tc", 8, 6, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       VD_REQUIRE(vocab_dlogits_tc(e->cx, IN(0), IN(1), IN(2), CF(0), I[3], CF(1), I[4], CF(2), CI32(3), CI32(4), CF(5), F(6), I[5],
+                                   CF(7)),
+                  VD_E_SHAPE, "vocab_dlogits_tc: shape refused");
+     }},
+    // ptrs A, B, bias, part_max, part_sum, part_key, part_cls, part_x; ints M, N, K, lda, ldb, seed, step, row_offset, row_stride;
+    // reals temperature
+    {"vocab_sample_tc", 8, 9, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       SampleCfg s;
+       s.seed_lo = (uint32_t)(uint64_t)I[5]; s.seed_hi = (uint32_t)((uint64_t)I[5] >> 32); s.step = (uint32_t)I[6];
+       s.temperature = (float)X[0]; s.row_offset = I[7]; s.row_stride = I[8];
+       VD_REQUIRE(vocab_sample_tc(e->cx, IN(0), IN(1), IN(2), CF(0), I[3], CF(1), I[4], CF(2), s, F(3), F(4), F(5), I32(6), F(7)),
+                  VD_E_SHAPE, "vocab_sample_tc: shape refused");
+     }},
+    // ptrs part_max, part_sum, part_key, part_cls, part_x, tokens, answer, logp (may be null); ints nparts, rows, step, L
+    {"vocab_sample_finish", 8, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       vocab_sample_finish(e->cx, CF(0), CF(1), CF(2), CI32(3), CF(4), IN(0), I[1], IN(2), IN(3), I32(5), I32(6), F(7));
      }},
     // ---- embedding and token grouping
     {"embed_rows", 3, 3, 1,
