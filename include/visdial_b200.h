@@ -175,8 +175,8 @@ int vd_gen_option_lhood(vd_engine* e, const vd_batch* b, const float** lhood_dev
  *    pointers, level = 0 | 1 (model.lua:480-483); both NULL for encoders without .rnnLayers (mn-att, :491-501).
  *  vd_gen_decoder_step: decoder:forward(tokens) for ONE time step on `rows` independent rows with
  *    .userPrevOutput / .userPrevCell = h_prev[l] / c_prev[l] (l = 0, 1; (rows,H) device pointers, NULL = zeros)
- *    (model.lua:517-526, gen.lua:3-27).  tokens: HOST int32 (rows).  Returns device pointers, valid until the next
- *    vd_encoder_forward: log-probabilities (rows,V) (all-zero row for a pad token, MaskZero) and the new state. */
+ *    (model.lua:517-526, gen.lua:3-27).  tokens: HOST int32 (rows).  Callable after vd_encoder_forward or a
+ *    vd_dialog_ask_* (DESIGN §19).  Returns device pointers, valid until the next vd_encoder_forward: log-probabilities (rows,V) (all-zero row for a pad token, MaskZero) and the new state. */
 int vd_encoder_rnn_state(vd_engine* e, int32_t level, const float** h_last_dev, const float** c_last_dev);
 int vd_gen_decoder_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, const float* const* h_prev,
                         const float* const* c_prev, const float** logp_dev, const float** h_out, const float** c_out);
@@ -244,6 +244,43 @@ int vd_answer_pool(vd_engine* e, const float** emb_dev, int64_t* m);
 int vd_answer_pool_retrieve(vd_engine* e, const vd_batch* b, int32_t k, int32_t* index_host, float* score_host);
 int vd_answer_pool_dialog(vd_engine* e, const vd_batch* b, int32_t k, int32_t hist_width, int32_t max_ans_len,
                           int32_t* index_host, float* score_host, int32_t* hist_host);
+
+/* ---- dialog sessions: questions asked one round at a time (DESIGN §19) ---------------------- */
+/* A session holds the B dialogs of batch b on the engine (one session per engine; a new begin replaces it).  It takes b's
+ * image rows and round-0 history row (the caption) and ignores its questions, answers and options.  Each ask supplies one
+ * question row per dialog for the next round r: ques (B, Tq) int32 HOST, right-aligned and zero-padded as ques_fwd, with
+ * 1 <= Tq <= b's Tq.  The ask encodes round r's B rows in eval mode over the session's cached history facts, image
+ * products and dialog-LSTM state, answers them, and appends Q_r and the answer to the history by vd_gen_dialog_*'s rule
+ * (hist_width, max_ans_len, pad questions and concatenated history as there).  Fed the batch's own questions, a session
+ * gives vd_gen_dialog_beam_search's / vd_gen_dialog_sample's / vd_answer_pool_dialog's round-r results.  Encoders without
+ * history (lf-ques, lf-ques-im) encode just the question (and image); hist_width and max_ans_len are not read for them.
+ *  vd_dialog_ask_beam: vd_gen_beam_search's search on the B rows: answer (B, beam_len), length (B), score (B).
+ *  vd_dialog_ask_sample: vd_gen_sample's draw: answer (B, beam_len + 1), logp (B, beam_len) or NULL; row b draws as global
+ *    round row_offset + b * maxQuesCount + r, as vd_gen_dialog_sample's round r.
+ *  vd_dialog_ask_pool: vd_answer_pool_retrieve's top-k (disc, current pool): index (B, k), score (B, k).
+ *  vd_dialog_round: the next round to be asked and B.  vd_dialog_history: the (B, maxQuesCount, hist_width) rows.
+ *  vd_dialog_encoding: the last ask's encoder output (B, rnnHiddenSize), a DEVICE pointer valid until the next ask.
+ *  vd_dialog_rnn_state: vd_encoder_rnn_state for the last ask: question-LSTM layer `level`'s h and c at Tq, (B, H)
+ *    DEVICE pointers valid until the next ask, NULL for encoders without .rnnLayers.  With vd_dialog_encoding it is the
+ *    decoder start state the ask's answerer used.
+ * Each ask ends in one synchronisation.  Session state lives outside the activation arena, so any other engine call
+ * between two asks leaves it intact; begin and each ask end the last vd_encoder_forward (as a new forward would).
+ * hist_width must hold the batch's round-0 row and a whole question row (hist_width >= its Th and Tq), as
+ * vd_gen_dialog_*'s history append needs.
+ * Refusals, before any state changes: VD_E_STATE for no session, a full one (maxQuesCount asks done), weights or math
+ * mode changed since begin (vd_set_parameters, vd_clamp_adam_step, vd_set_math_mode), an answerer the decoder lacks,
+ * or a stale pool; VD_E_SHAPE / VD_E_BADARG for widths, B, and tokens outside [0, vocabSize]. */
+int vd_dialog_begin(vd_engine* e, const vd_batch* b, int32_t hist_width, int32_t max_ans_len);
+int vd_dialog_ask_beam(vd_engine* e, const int32_t* ques, int32_t Tq, int32_t beam_size, int32_t beam_len, int32_t start_token,
+                       int32_t end_token, int32_t* answer, int32_t* length, double* score);
+int vd_dialog_ask_sample(vd_engine* e, const int32_t* ques, int32_t Tq, int32_t beam_len, int32_t start_token, int32_t end_token,
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t* answer, float* logp);
+int vd_dialog_ask_pool(vd_engine* e, const int32_t* ques, int32_t Tq, int32_t k, int32_t* index, float* score);
+int vd_dialog_round(vd_engine* e, int32_t* round, int32_t* B);
+int vd_dialog_history(vd_engine* e, int32_t* hist_host);
+int vd_dialog_encoding(vd_engine* e, const float** encOut_dev);
+int vd_dialog_rnn_state(vd_engine* e, int32_t level, const float** h_last, const float** c_last);
+int vd_dialog_end(vd_engine* e);
 
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.

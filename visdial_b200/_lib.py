@@ -129,6 +129,17 @@ SIGNATURES = {
     "vd_answer_pool": [_H, _P(C.c_void_p), _P(C.c_int64)],
     "vd_answer_pool_retrieve": [_H, _P(vd_batch), C.c_int32, C.c_void_p, C.c_void_p],
     "vd_answer_pool_dialog": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_dialog_begin": [_H, _P(vd_batch), C.c_int32, C.c_int32],
+    "vd_dialog_ask_beam": [_H, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                           C.c_void_p],
+    "vd_dialog_ask_sample": [_H, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64,
+                             C.c_void_p, C.c_void_p],
+    "vd_dialog_ask_pool": [_H, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p],
+    "vd_dialog_round": [_H, _P(C.c_int32), _P(C.c_int32)],
+    "vd_dialog_history": [_H, C.c_void_p],
+    "vd_dialog_encoding": [_H, _P(C.c_void_p)],
+    "vd_dialog_rnn_state": [_H, C.c_int32, _P(C.c_void_p), _P(C.c_void_p)],
+    "vd_dialog_end": [_H],
     "vd_gemm_atb16": [_H, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                       C.c_int64, C.c_float],
     "vd_lstm_step_fwd": [_H, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,

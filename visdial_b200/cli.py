@@ -85,6 +85,13 @@ GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + [
     ("history", "gt", "History each round is answered with: gt (the dataset's) | generated (the dialog's own answers)"),
 ]
 
+# the chat command: generate's options, and which images are talked about with which questions
+CHAT_OPTIONS = GENERATE_OPTIONS + [
+    ("split", "val", "Split the images and captions come from"),
+    ("imageIds", "", "Comma-separated COCO image ids of the split (default: the -questions file's, else its first image)"),
+    ("questions", "", "JSON {image_id: [question, ...]}: ask these and write results.json; else read stdin, one per line"),
+]
+
 # options of every command that the reference does not have: how the run is spread over GPUs and which math it uses
 MATH_MODES = ("fp32", "tf32", "f16")
 RUN_OPTIONS = [

@@ -111,6 +111,7 @@ int vd_set_parameters(vd_engine* h, const float* src, int64_t n) {
     Engine* e = ENG(h);
     VD_REQUIRE(src && n == e->nparams, VD_E_SHAPE, "vd_set_parameters: n must equal vd_num_params");
     e->pool_valid = false;           // before the copy: a failed copy may have written part of the weights
+    e->dses.valid = false;
     VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
     VD_CUDA_CHECK(cudaMemcpyAsync(e->W, src, (size_t)n * sizeof(float), cudaMemcpyHostToDevice, e->cx.stream));
     VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
@@ -166,6 +167,7 @@ int vd_set_math_mode(vd_engine* h, int32_t mode) {
     VD_REQUIRE(mode == VD_MATH_TF32 || mode == VD_MATH_FP32 || mode == VD_MATH_F16, VD_E_BADARG, "unknown math mode");
     Engine* e = ENG(h);
     e->pool_valid = false;           // the pool was encoded on the previous mode's option-LSTM route
+    e->dses.valid = false;           // and a dialog session's cache on its routes
     e->math_mode = mode;
   })
 }
@@ -309,6 +311,59 @@ int vd_answer_pool_dialog(vd_engine* h, const vd_batch* b, int32_t k, int32_t hi
                           float* score_host, int32_t* hist_host) {
   VD_TRY({ ENG(h)->answer_pool_dialog(b, k, hist_width, max_ans_len, index_host, score_host, hist_host); })
 }
+
+int vd_dialog_begin(vd_engine* h, const vd_batch* b, int32_t hist_width, int32_t max_ans_len) {
+  VD_TRY({ ENG(h)->dialog_begin(b, hist_width, max_ans_len); })
+}
+int vd_dialog_ask_beam(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t beam_size, int32_t beam_len, int32_t start_token,
+                       int32_t end_token, int32_t* answer, int32_t* length, double* score) {
+  VD_TRY({ ENG(h)->dialog_ask_beam(ques, Tq, beam_size, beam_len, start_token, end_token, answer, length, score); })
+}
+int vd_dialog_ask_sample(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t beam_len, int32_t start_token, int32_t end_token,
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t* answer, float* logp) {
+  VD_TRY({ ENG(h)->dialog_ask_sample(ques, Tq, beam_len, start_token, end_token, temperature, seed, row_offset, answer, logp); })
+}
+int vd_dialog_ask_pool(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t k, int32_t* index, float* score) {
+  VD_TRY({ ENG(h)->dialog_ask_pool(ques, Tq, k, index, score); })
+}
+int vd_dialog_round(vd_engine* h, int32_t* round, int32_t* B) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(e->dses.open, VD_E_STATE, "no dialog session");
+    if (round) *round = e->dses.round;
+    if (B) *B = e->dses.B;
+  })
+}
+int vd_dialog_history(vd_engine* h, int32_t* hist_host) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(e->dses.open, VD_E_STATE, "no dialog session");
+    NOTNULL(hist_host);
+    VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
+    const size_t n = (size_t)e->dses.B * e->cfg.R * e->dses.W;
+    if (n) VD_CUDA_CHECK(cudaMemcpyAsync(hist_host, e->dses.hist.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, e->main_stream));
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->main_stream));
+  })
+}
+int vd_dialog_encoding(vd_engine* h, const float** encOut_dev) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(e->dses.open && e->dses.encOut, VD_E_STATE, "no dialog session, or no round asked yet");
+    NOTNULL(encOut_dev);
+    *encOut_dev = e->dses.encOut;
+  })
+}
+int vd_dialog_rnn_state(vd_engine* h, int32_t level, const float** h_last, const float** c_last) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(e->dses.open && e->dses.encOut, VD_E_STATE, "no dialog session, or no round asked yet");
+    VD_REQUIRE(level == 0 || level == 1, VD_E_BADARG, "level must be 0 or 1");
+    const bool has_layers = e->cfg.rnn_layers;
+    if (h_last) *h_last = has_layers ? (const float*)e->dses.rnn[2 * level].p : nullptr;
+    if (c_last) *c_last = has_layers ? (const float*)e->dses.rnn[2 * level + 1].p : nullptr;
+  })
+}
+int vd_dialog_end(vd_engine* h) { VD_TRY({ ENG(h)->dialog_end(); }) }
 
 int vd_clamp_adam_step(vd_engine* h, float lr) { VD_TRY({ ENG(h)->clamp_adam_step(lr); }) }
 

@@ -783,13 +783,15 @@ static LstmRun make_run(int T, int64_t R, int D, int H, int wseg, const float* x
 
 // ---- blocks shared by several encoder graphs -----------------------------------------------------------------------
 // memory network over the history facts (mn-*.lua): MM -> MaskSoftMax (causal) -> MM -> Dropout -> Linear -> Tanh, residual query, Linear -> Tanh
-void Engine::mn_block_fwd(const float* qin, const float* h3, float* out) {
-  const int H = cfg.H, R = cfg.R, B = db.B;
-  const int64_t N = db.N;
+// Rounds [r0, r1) of B dialogs: qin / out have B*(r1-r0) rows, the facts of dialog b are rows 0..r1-1 of facts + b*fpitch
+// (the full forward: [0, R) over hist2's h_T; a dialog session: [r, r+1) over its cached facts)
+void Engine::mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1) {
+  const int H = cfg.H, R = cfg.R;
+  const int64_t N = (int64_t)B * (r1 - r0);
   const DropCfg d05 = dropcfg(0.5f);
-  probs = arena.get<float>((int64_t)B * R * R);
+  probs = arena.get<float>(N * R);
   hAtt = arena.get<float>(N * H);
-  mn_attention_fwd(cx, qin, h3, probs, hAtt, B, R, H);
+  mn_attention_rows_fwd(cx, qin, facts, fpitch, probs, hAtt, B, R, H, r0, r1);
   hAtt_d = arena.get<float>(N * H);
   dropout_apply(cx, hAtt_d, hAtt, N * H, d05, SITE_HATT);
   hAttTr = arena.get<float>(N * H);
@@ -816,16 +818,18 @@ void Engine::mn_block_bwd(const float* dout, const float* out, float* dqin, floa
 }
 // SAN (mn-att-ques-im-hist.lua:67-106, lf-att-ques-im-hist.lua:43-86): tanh(Linear(img)) is computed once per dialog; Dropout then
 // acts on the repeated tensor; hops of {img_common + ques_common -> tanh -> dropout -> score -> softmax -> weighted sum + u}
-void Engine::san_block_fwd(const float* u0) {
-  const int H = cfg.H, R = cfg.R, B = db.B;
-  const int64_t N = db.N;
+void Engine::san_image(const float* pool5, int64_t B, float* t) {
+  wait_img();
+  linear_fwd(seg("san.img.weight"), pool5, B * cfg.S * cfg.S, t, 1);
+}
+void Engine::san_block_fwd(const float* u0, const float* timg, int B, int nr, float* out) {
+  const int H = cfg.H;
+  const int64_t N = (int64_t)B * nr;
   const int P = cfg.S * cfg.S, Cm = cfg.Cm;
   const DropCfg d05 = dropcfg(0.5f);
-  t_img = arena.get<float>((int64_t)B * P * H);
-  wait_img();
-  linear_fwd(seg("san.img.weight"), db.img, (int64_t)B * P, t_img, 1);
+  t_img = const_cast<float*>(timg);
   img_tr = arena.get<float>(N * P * H);
-  san_expand_dropout(cx, img_tr, t_img, B, R, P, H, d05, SITE_IMG_TR);
+  san_expand_dropout(cx, img_tr, t_img, B, nr, P, H, d05, SITE_IMG_TR);
   img_common.assign(cfg.hops, nullptr); ques_common.assign(cfg.hops, nullptr);
   sc.assign(cfg.hops, nullptr); pr.assign(cfg.hops, nullptr); u_hop.assign(cfg.hops + 1, nullptr);
   u_hop[0] = const_cast<float*>(u0);
@@ -845,7 +849,7 @@ void Engine::san_block_fwd(const float* u0) {
   }
   u_d = arena.get<float>(N * H);
   dropout_apply(cx, u_d, u_hop[cfg.hops], N * H, d05, SITE_U_OUT);
-  linear_fwd(seg("san.out.weight"), u_d, N, encOut, 1);
+  linear_fwd(seg("san.out.weight"), u_d, N, out, 1);
 }
 void Engine::san_block_bwd(const float* dEnc, float* du) {
   const int H = cfg.H, R = cfg.R, B = db.B;
@@ -882,7 +886,101 @@ void Engine::san_block_bwd(const float* dEnc, float* du) {
   release_img();                                   // last reader of this step's image staging buffer
 }
 
-void Engine::encoder_forward(const vd_batch* b) {
+// late fusion (lf-ques.lua:29-33 / lf-ques-im.lua / lf-ques-hist.lua / lf-ques-im-hist.lua:49-59): JoinTable [q | img | h] ->
+// Dropout -> Linear -> Tanh.  lf-att-ques-im-hist.lua:41: Tanh(Linear([q | h])) with no dropout, then the SAN block on pool5.
+// q3 / h3 / out: B*nr rows (nr rounds per dialog); fc7: B rows, repeated per round (model.lua:267-269); timg: the SAN's
+// tanh(Linear(pool5)) of the B dialogs (san_image)
+void Engine::lf_block_fwd(const float* q3, const float* fc7, const float* timg, const float* h3, int B, int nr, float* out) {
+  const int H = cfg.H;
+  const int64_t N = (int64_t)B * nr;
+  const bool use_fc7 = cfg.useIm && !cfg.san;
+  joinK = H + (use_fc7 ? cfg.F : 0) + (cfg.useHist ? H : 0);
+  join_d = arena.get<float>(N * joinK);
+  copy_cols(cx, join_d, joinK, q3, H, N, H);
+  if (use_fc7) {
+    float* tmp = arena.get<float>(N * cfg.F);
+    wait_img();
+    repeat_rows(cx, tmp, fc7, B, nr, cfg.F);
+    copy_cols(cx, join_d + H, joinK, tmp, cfg.F, N, cfg.F);
+  }
+  if (cfg.useHist) copy_cols(cx, join_d + H + (use_fc7 ? cfg.F : 0), joinK, h3, H, N, H);
+  if (!cfg.san) {
+    dropout_apply(cx, join_d, join_d, N * joinK, dropcfg(cfg.dropout), SITE_FUSION);
+    linear_fwd(seg("fusion.weight"), join_d, N, out, 1);
+  } else {
+    qh2 = arena.get<float>(N * H);
+    linear_fwd(seg("fusion.weight"), join_d, N, qh2, 1);
+    san_block_fwd(qh2, timg, B, nr, out);
+  }
+}
+
+// hre / hrea: the dialog LSTM's input rows j (B*(r1-r0), 2H) of rounds [r0, r1).  hrea-ques-im-hist.lua:89-129: attention
+// of the round's sq over the scores sh (B, R) and facts (dialog b at facts + b*fpitch) of rounds <= it, then [att | q];
+// hre-ques-*.lua: [q | h]
+void Engine::hre_join_fwd(const float* q3, const float* facts, const float* sq_, const float* sh_, int64_t fpitch, int B, int r0,
+                          int r1, float* j) {
+  const int H = cfg.H, R = cfg.R;
+  const int64_t N = (int64_t)B * (r1 - r0);
+  if (cfg.hre_att) {
+    probs = arena.get<float>(N * R);
+    att = arena.get<float>(N * H);
+    hrea_attention_rows_fwd(cx, sq_, sh_, facts, fpitch, probs, att, B, R, H, r0, r1);
+    copy_cols(cx, j, 2 * H, att, H, N, H);
+    copy_cols(cx, j + H, 2 * H, q3, H, N, H);
+  } else {
+    copy_cols(cx, j, 2 * H, q3, H, N, H);              // nr == 1 or the full forward: the facts are h3's own rows
+    copy_cols(cx, j + H, 2 * H, facts, H, N, H);
+  }
+}
+
+// the dialog-level LSTM over nr rounds of B dialogs from (h0, c0) (null: the first round), rows j (B*nr, 2H) in dialog-major
+// order.  View(-1,10,2H), Transpose(1,2): row (r,b) <- row (b,r), a strided 2-D copy per round; out (B*nr, H) dialog-major.
+// h_out / c_out (a session's carried state, nr == 1): where the step writes its h and c instead of the arena.
+void Engine::hre_dialog_fwd(const float* j, int B, int nr, const float* h0, const float* c0, float* h_out, float* c_out,
+                            float* out) {
+  const int H = cfg.H;
+  const int64_t N = (int64_t)B * nr;
+  jt = arena.get<float>(N * 2 * H);
+  for (int rr = 0; rr < nr; ++rr)
+    copy_cols(cx, jt + (int64_t)rr * B * 2 * H, 2 * H, j + (int64_t)rr * 2 * H, (int64_t)nr * 2 * H, B, 2 * H);
+  dialog = make_run(nr, B, 2 * H, H, seg("dialog.lstm.weight"), jt, nullptr, nullptr);
+  dialog.h0 = h0; dialog.c0 = c0;
+  dialog.route = route_lstm(dialog);
+  lstm_forward_begin(dialog, true);
+  if (h_out) { dialog.h = h_out; dialog.c = c_out; }  // one saved step: slot 0 is the whole of h and c
+  for (int t = 0; t < nr; ++t) lstm_forward_step(dialog, t);
+  for (int rr = 0; rr < nr; ++rr)
+    copy_cols(cx, out + (int64_t)rr * H, (int64_t)nr * H, dialog.h + (int64_t)rr * B * H, H, B, H);
+}
+
+// mn-ques-hist.lua / mn-ques-im-hist.lua / mn-att-ques-im-hist.lua:48-106 on rounds [r0, r1): q3 / out B*(r1-r0) rows, img
+// the B dialogs' fc7 (mn-ques-im-hist), timg as lf_block_fwd's, facts as mn_block_fwd takes them
+void Engine::mn_family_fwd(const float* q3, const float* img, const float* timg, const float* facts, int64_t fpitch, int B, int r0,
+                           int r1, float* out) {
+  const int H = cfg.H, nr = r1 - r0;
+  const int64_t N = (int64_t)B * nr;
+  mn_query_in = q3;
+  if (cfg.mn_qi) {                                    // mn-ques-im-hist.lua: qi_proj = Tanh(Linear([q | fc7]))
+    qi_join = arena.get<float>(N * (H + cfg.F));
+    copy_cols(cx, qi_join, H + cfg.F, q3, H, N, H);
+    float* tmp = arena.get<float>(N * cfg.F);
+    wait_img();
+    repeat_rows(cx, tmp, img, B, nr, cfg.F);
+    copy_cols(cx, qi_join + H, H + cfg.F, tmp, cfg.F, N, cfg.F);
+    qi_proj = arena.get<float>(N * H);
+    linear_fwd(seg("mn.qi.weight"), qi_join, N, qi_proj, 1);
+    mn_query_in = qi_proj;
+  }
+  if (cfg.san) {
+    qh2 = arena.get<float>(N * H);
+    mn_block_fwd(mn_query_in, facts, fpitch, qh2, B, r0, r1);
+    san_block_fwd(qh2, timg, B, nr, out);
+  } else {
+    mn_block_fwd(mn_query_in, facts, fpitch, out, B, r0, r1);
+  }
+}
+
+void Engine::quiesce() {
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   if (side_active) { cudaStreamSynchronize(side_stream); side_active = false; }   // only after an aborted call
   cx.stream = main_stream;
@@ -892,31 +990,22 @@ void Engine::encoder_forward(const vd_batch* b) {
   }
   arena.reset();
   have_fwd = false;
-  stage_batch(b);
-  save_acts = training != 0;
-  refresh_shadows();
-  if (opt_overlap && cfg.dec == DEC_DISC && db.options && db.To > 0) options_forward_async();
-  conn_dh_l1 = conn_dc_l1 = conn_dc_l2 = nullptr;
-  gen_h0[0] = gen_h0[1] = gen_c0[0] = gen_c0[1] = nullptr;
-  const int E = cfg.E, H = cfg.H, R = cfg.R;
-  const int64_t N = db.N;
-  const int B = db.B;
-  const DropCfg d05 = dropcfg(0.5f), dp = dropcfg(cfg.dropout), dnone = dropcfg(0.f);
-  // time-major ids: the view(-1,T):t() of model.lua:255-257,274-278
-  ids_q = arena.get<int32_t>(N * db.Tq);
-  transpose_ids(cx, db.ques, ids_q, N, db.Tq);
-  if (cfg.useHist) {
-    ids_h = arena.get<int32_t>(N * db.Th);
-    transpose_ids(cx, db.hist, ids_h, N, db.Th);
-  }
+}
+
+// The question and history LSTM pairs over `rows` rows of time-major ids ids_q (Tq, rows) / ids_h (Th, rows).  img_rows
+// (rows, IE): the image embedding MaskTime joins to the question LSTM's input (img_in_q), else null.
+void Engine::encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows) {
+  const int E = cfg.E, H = cfg.H;
+  const int64_t N = rows;
+  const DropCfg d05 = dropcfg(0.5f), dnone = dropcfg(0.f);
   const bool embdrop = cfg.embdrop;                        // mn-*.lua / lf-att-*.lua: Dropout(0.5) on both embeddings
   // history branch
   if (cfg.useHist) {
     fork_side();
-    xh = arena.get<float>(N * db.Th * E);
-    embed_rows(cx, xh, Wp(0), ids_h, N * db.Th, E, embdrop ? d05 : dnone, SITE_HEMBED);
-    hist1 = make_run(db.Th, N, E, H, seg("hist.lstm1.weight"), xh, nullptr, ids_h);
-    hist2 = make_run(db.Th, N, H, H, seg("hist.lstm2.weight"), nullptr, nullptr, ids_h);
+    xh = arena.get<float>(N * Th * E);
+    embed_rows(cx, xh, Wp(0), ids_h, N * Th, E, embdrop ? d05 : dnone, SITE_HEMBED);
+    hist1 = make_run(Th, N, E, H, seg("hist.lstm1.weight"), xh, nullptr, ids_h);
+    hist2 = make_run(Th, N, H, H, seg("hist.lstm2.weight"), nullptr, nullptr, ids_h);
     route_lstm_pair(hist1, hist2);
     // The 2nd layer consumes every step of the 1st, so encoder LSTMs always keep all steps (T*N*H is small).
     // The history and question LSTM chains are independent until the fusion/attention stage: the history chain runs
@@ -925,98 +1014,77 @@ void Engine::encoder_forward(const vd_batch* b) {
     else { lstm_pair_forward(hist1, hist2, side_chain); back_to_main(); }
   }
   // question branch
-  xq = arena.get<float>(N * db.Tq * E);
-  embed_rows(cx, xq, Wp(0), ids_q, N * db.Tq, E, embdrop ? d05 : dnone, SITE_QEMBED);
+  xq = arena.get<float>(N * Tq * E);
+  embed_rows(cx, xq, Wp(0), ids_q, N * Tq, E, embdrop ? d05 : dnone, SITE_QEMBED);
+  if (img_rows) {
+    // hre(a)-ques-im-hist.lua:41-55: MaskTime, JoinTable(-1)
+    qi_in = arena.get<float>(N * Tq * (E + cfg.IE));
+    masktime_concat_fwd(cx, qi_in, xq, img_rows, ids_q, Tq, N, E, cfg.IE);
+    ques1 = make_run(Tq, N, E + cfg.IE, H, seg("ques.lstm1.weight"), qi_in, nullptr, ids_q);
+  } else {
+    ques1 = make_run(Tq, N, E, H, seg("ques.lstm1.weight"), xq, nullptr, ids_q);
+  }
+  ques2 = make_run(Tq, N, H, H, seg("ques.lstm2.weight"), nullptr, nullptr, ids_q);
+  route_lstm_pair(ques1, ques2);
+  lstm_pair_forward(ques1, ques2, main_chain);
+  join_side();
+}
+
+void Engine::encoder_forward(const vd_batch* b) {
+  quiesce();
+  stage_batch(b);
+  save_acts = training != 0;
+  refresh_shadows();
+  if (opt_overlap && cfg.dec == DEC_DISC && db.options && db.To > 0) options_forward_async();
+  conn_dh_l1 = conn_dc_l1 = conn_dc_l2 = nullptr;
+  gen_h0[0] = gen_h0[1] = gen_c0[0] = gen_c0[1] = nullptr;
+  const int H = cfg.H, R = cfg.R;
+  const int64_t N = db.N;
+  const int B = db.B;
+  const DropCfg d05 = dropcfg(0.5f);
+  // time-major ids: the view(-1,T):t() of model.lua:255-257,274-278
+  ids_q = arena.get<int32_t>(N * db.Tq);
+  transpose_ids(cx, db.ques, ids_q, N, db.Tq);
+  if (cfg.useHist) {
+    ids_h = arena.get<int32_t>(N * db.Th);
+    transpose_ids(cx, db.hist, ids_h, N, db.Th);
+  }
+  const float* img_rows = nullptr;
   if (cfg.img_in_q) {
-    // hre(a)-ques-im-hist.lua:41-55: [Dropout(0.5) ->] Linear(F,IE) on the 10x repeated fc7, MaskTime, JoinTable(-1)
+    // hre(a)-ques-im-hist.lua:41-55: [Dropout(0.5) ->] Linear(F,IE) on the 10x repeated fc7
     img_d = arena.get<float>(N * cfg.F);
     wait_img();
     repeat_rows(cx, img_d, db.img, B, R, cfg.F);
     if (cfg.img_drop) dropout_apply(cx, img_d, img_d, N * cfg.F, d05, SITE_IMG_FC7);
     img_e = arena.get<float>(N * cfg.IE);
     linear_fwd(seg("img.embed.weight"), img_d, N, img_e, 0);
-    qi_in = arena.get<float>(N * db.Tq * (E + cfg.IE));
-    masktime_concat_fwd(cx, qi_in, xq, img_e, ids_q, db.Tq, N, E, cfg.IE);
-    ques1 = make_run(db.Tq, N, E + cfg.IE, H, seg("ques.lstm1.weight"), qi_in, nullptr, ids_q);
-  } else {
-    ques1 = make_run(db.Tq, N, E, H, seg("ques.lstm1.weight"), xq, nullptr, ids_q);
+    img_rows = img_e;
   }
-  ques2 = make_run(db.Tq, N, H, H, seg("ques.lstm2.weight"), nullptr, nullptr, ids_q);
-  route_lstm_pair(ques1, ques2);
-  lstm_pair_forward(ques1, ques2, main_chain);
-  join_side();
+  encoder_lstms(N, db.Tq, db.Th, img_rows);
   const float* q3 = ques2.h_last();
   const float* h3 = cfg.useHist ? hist2.h_last() : nullptr;
   encOut = arena.get<float>(N * H);
 
+  const float* timg = nullptr;
+  if (cfg.san) {
+    float* t = arena.get<float>((int64_t)B * cfg.S * cfg.S * H);
+    san_image(db.img, B, t);
+    timg = t;
+  }
   if (cfg.fam_lf) {
-    // lf-ques.lua:29-33 / lf-ques-im.lua / lf-ques-hist.lua / lf-ques-im-hist.lua:49-59: JoinTable [q | img | h] -> Dropout -> Linear
-    // -> Tanh.  lf-att-ques-im-hist.lua:41: Tanh(Linear([q | h])) with no dropout, then the SAN block on pool5.
-    const bool fc7 = cfg.useIm && !cfg.san;
-    joinK = H + (fc7 ? cfg.F : 0) + (cfg.useHist ? H : 0);
-    join_d = arena.get<float>(N * joinK);
-    copy_cols(cx, join_d, joinK, q3, H, N, H);
-    if (fc7) {                                          // image repeated per round (model.lua:267-269)
-      float* tmp = arena.get<float>(N * cfg.F);
-      wait_img();
-      repeat_rows(cx, tmp, db.img, B, R, cfg.F);
-      copy_cols(cx, join_d + H, joinK, tmp, cfg.F, N, cfg.F);
-    }
-    if (cfg.useHist) copy_cols(cx, join_d + H + (fc7 ? cfg.F : 0), joinK, h3, H, N, H);
-    if (!cfg.san) {
-      dropout_apply(cx, join_d, join_d, N * joinK, dp, SITE_FUSION);
-      linear_fwd(seg("fusion.weight"), join_d, N, encOut, 1);
-    } else {
-      qh2 = arena.get<float>(N * H);
-      linear_fwd(seg("fusion.weight"), join_d, N, qh2, 1);
-      san_block_fwd(qh2);
-    }
+    lf_block_fwd(q3, db.img, timg, h3, B, R, encOut);
   } else if (cfg.fam_hre) {
-    // hrea-ques-im-hist.lua:89-137 (attention over the rounds, [att | q]) / hre-ques-*.lua ([q | h]) -> dialog-level LSTM
-    jt = arena.get<float>(N * 2 * H);
     float* j = arena.get<float>(N * 2 * H);
     if (cfg.hre_att) {
       sq = arena.get<float>(N); sh = arena.get<float>(N);
       int sq_w = seg("att.q.weight"), sh_w = seg("att.h.weight");
       rowdot_fwd(cx, sq, q3, Wp(sq_w), Wp(sq_w + 1), N, H);
       rowdot_fwd(cx, sh, h3, Wp(sh_w), Wp(sh_w + 1), N, H);
-      probs = arena.get<float>((int64_t)B * R * R);
-      att = arena.get<float>(N * H);
-      hrea_attention_fwd(cx, sq, sh, h3, probs, att, B, R, H);
-      copy_cols(cx, j, 2 * H, att, H, N, H);
-      copy_cols(cx, j + H, 2 * H, q3, H, N, H);
-    } else {
-      copy_cols(cx, j, 2 * H, q3, H, N, H);
-      copy_cols(cx, j + H, 2 * H, h3, H, N, H);
     }
-    // View(-1,10,2H), Transpose(1,2): row (r,b) <- row (b,r), a strided 2-D copy per round
-    for (int rr = 0; rr < R; ++rr)
-      copy_cols(cx, jt + (int64_t)rr * B * 2 * H, 2 * H, j + (int64_t)rr * 2 * H, (int64_t)R * 2 * H, B, 2 * H);
-    dialog = make_run(R, B, 2 * H, H, seg("dialog.lstm.weight"), jt, nullptr, nullptr);
-    lstm_forward(dialog, true);
-    for (int rr = 0; rr < R; ++rr)
-      copy_cols(cx, encOut + (int64_t)rr * H, (int64_t)R * H, dialog.h + (int64_t)rr * B * H, H, B, H);
+    hre_join_fwd(q3, h3, sq, sh, (int64_t)R * H, B, 0, R, j);
+    hre_dialog_fwd(j, B, R, nullptr, nullptr, nullptr, nullptr, encOut);
   } else {
-    // mn-ques-hist.lua / mn-ques-im-hist.lua / mn-att-ques-im-hist.lua:48-106
-    mn_query_in = q3;
-    if (cfg.mn_qi) {                                    // mn-ques-im-hist.lua: qi_proj = Tanh(Linear([q | fc7]))
-      qi_join = arena.get<float>(N * (H + cfg.F));
-      copy_cols(cx, qi_join, H + cfg.F, q3, H, N, H);
-      float* tmp = arena.get<float>(N * cfg.F);
-      wait_img();
-      repeat_rows(cx, tmp, db.img, B, R, cfg.F);
-      copy_cols(cx, qi_join + H, H + cfg.F, tmp, cfg.F, N, cfg.F);
-      qi_proj = arena.get<float>(N * H);
-      linear_fwd(seg("mn.qi.weight"), qi_join, N, qi_proj, 1);
-      mn_query_in = qi_proj;
-    }
-    if (cfg.san) {
-      qh2 = arena.get<float>(N * H);
-      mn_block_fwd(mn_query_in, h3, qh2);
-      san_block_fwd(qh2);
-    } else {
-      mn_block_fwd(mn_query_in, h3, encOut);
-    }
+    mn_family_fwd(q3, db.img, timg, h3, (int64_t)R * H, B, 0, R, encOut);
   }
   wait_img();                // (an encoder that never reads the image still has to retire the copy before the buffer is reused)
   release_img();             // forward-only callers never reach the backward's release; a later one simply overrides this
@@ -1637,7 +1705,9 @@ void Engine::gen_option_lhood() {
 // Ta = 1 (dense embedded input, maskzero on the token, MaskZero'd Linear + LogSoftMax).
 void Engine::gen_decoder_step(int64_t rows, const int32_t* tokens_host, const float* const* h_prev, const float* const* c_prev) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_decoder_step needs the gen decoder");
-  VD_REQUIRE(have_fwd, VD_E_STATE, "gen_decoder_step before encoder_forward");
+  // the step reads only its explicit state and the weights' transposed shadow, which an encoder forward and a dialog ask
+  // both refresh: after an ask it replays the ask's search from vd_dialog_encoding / vd_dialog_rnn_state
+  VD_REQUIRE(have_fwd || dses.encOut, VD_E_STATE, "gen_decoder_step before encoder_forward or a dialog ask");
   VD_REQUIRE(rows > 0 && tokens_host != nullptr, VD_E_BADARG, "rows / tokens");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
@@ -1765,7 +1835,7 @@ void Engine::check_sample_args(int L, int start_token, float temperature, int64_
 // (k_logsoftmax_sample_rows).  The draw writes the next step's tokens, so nothing waits for the host.  Returns the answers
 // (n, L + 1) and log-probabilities (n, L) in the arena, valid until the next encoder forward.
 Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature,
-                                         uint64_t seed, int64_t row_offset) {
+                                         uint64_t seed, int64_t row_offset, int64_t draw_stride, int64_t draw_off) {
   forward_connect();
   const int H = cfg.H, V = cfg.V;
   const int64_t N = n;
@@ -1798,7 +1868,8 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
       *p = t;
     }
   }
-  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset + off, stride};
+  if (draw_stride < 0) { draw_stride = stride; draw_off = off; }
+  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset + draw_off, draw_stride};
   // The step's decoder buffers alternate between two arena regions: step s reads the state step s-1 wrote into the other
   // one, so the new state feeds the next step without a copy.  Same allocations every step, so a region lands where it
   // did two steps earlier and the arena does not grow with L.
@@ -2045,10 +2116,212 @@ void Engine::answer_pool_dialog(const vd_batch* b, int k, int W, int max_ans_len
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
+// ---- dialog sessions (DESIGN §19) ---------------------------------------------------------------------------------------
+// B dialogs from batch b: its image rows and its round-0 history row; its questions, answers and options are not read.
+// The per-dialog image products every round repeats are computed here once, with the weights of this call.
+void Engine::dialog_begin(const vd_batch* b, int W, int max_ans_len) {
+  VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0, VD_E_SHAPE, "session batch with B, Tq > 0");
+  if (cfg.useHist) {
+    VD_REQUIRE(b->hist && b->Th > 0, VD_E_SHAPE, "a history encoder's session needs the batch's round-0 history row");
+    // hist_append (as vd_gen_dialog_*'s loop calls it) needs a row to hold the caption row and a whole question row
+    VD_REQUIRE(W >= b->Th && W >= b->Tq && max_ans_len >= 1, VD_E_BADARG,
+               "hist_width >= the batch's Th and Tq, max_ans_len >= 1");
+  }
+  const vd_batch eb = encoder_only(b);
+  dses.open = dses.valid = false;
+  quiesce();
+  stage_batch(&eb);
+  refresh_shadows();
+  wait_img();
+  const int R = cfg.R, H = cfg.H, B = db.B, Tq = db.Tq;
+  if (!cfg.useHist) W = 0;
+  if (cfg.useHist) {
+    int32_t* hist = (int32_t*)dses.hist.ensure((size_t)B * R * W * sizeof(int32_t));
+    hist_append(cx, hist, B, R, W, -1, db.hist, db.Th, nullptr, 0, nullptr, 0, 0, 0, false);   // round 0 <- the caption row
+    if (cfg.fam_mn || cfg.hre_att) dses.facts.ensure((size_t)B * R * H * sizeof(float));   // the attention's facts
+    if (cfg.hre_att) dses.shc.ensure((size_t)B * R * sizeof(float));
+    if (cfg.fam_hre)
+      for (auto& g : dses.state) g.ensure((size_t)B * H * sizeof(float));
+  }
+  if (cfg.rnn_layers)
+    for (auto& g : dses.rnn) g.ensure((size_t)B * H * sizeof(float));
+  VD_CUDA_CHECK(cudaMemsetAsync(dses.ques.ensure((size_t)B * R * Tq * sizeof(int32_t)), 0, (size_t)B * R * Tq * sizeof(int32_t),
+                                cx.stream));
+  if (cfg.san) {
+    san_image(db.img, B, (float*)dses.t_img.ensure((size_t)B * cfg.S * cfg.S * H * sizeof(float)));
+  } else if (cfg.useIm) {
+    float* fc7 = (float*)dses.fc7.ensure((size_t)B * cfg.F * sizeof(float));
+    VD_CUDA_CHECK(cudaMemcpyAsync(fc7, db.img, (size_t)B * cfg.F * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
+    if (cfg.img_in_q)        // eval mode: hrea's Dropout before img.embed is the identity
+      linear_fwd(seg("img.embed.weight"), fc7, B, (float*)dses.img_e.ensure((size_t)B * cfg.IE * sizeof(float)), 0);
+  }
+  dses.enc.ensure((size_t)B * H * sizeof(float));
+  release_img();
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  dses.B = B; dses.Tq = Tq; dses.W = W; dses.max_ans_len = max_ans_len; dses.round = 0; dses.encOut = nullptr;
+  dses.open = dses.valid = true;
+}
+
+void Engine::dialog_end() { dses.open = dses.valid = false; dses.round = 0; dses.encOut = nullptr; }
+
+void Engine::dialog_check_ask(const int32_t* ques_host, int Tq) const {
+  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session: call vd_dialog_begin");
+  VD_REQUIRE(dses.valid, VD_E_STATE, "the weights or the math mode changed since vd_dialog_begin");
+  VD_REQUIRE(dses.round < cfg.R, VD_E_STATE, "the session is full: all maxQuesCount rounds have been asked");
+  VD_REQUIRE(ques_host != nullptr, VD_E_BADARG, "null question rows");
+  VD_REQUIRE(Tq >= 1 && Tq <= dses.Tq, VD_E_SHAPE, "question width in [1, the session's question width]");
+  for (int64_t i = 0; i < (int64_t)dses.B * Tq; ++i)
+    VD_REQUIRE(ques_host[i] >= 0 && ques_host[i] <= cfg.V, VD_E_BADARG, "a question token outside [0, vocabSize]");
+}
+
+// Round r = dses.round of the B dialogs in eval mode: the question pair over the B new questions, the history pair over the
+// B history rows r, then the family block for round r over the cached state.  Leaves encOut = the session's (B, H) rows and
+// ques1 / ques2 = this pass's runs, which forward_connect() reads; the last encoder_forward is no longer current.
+void Engine::dialog_encode(const int32_t* ques_host, int Tq) {
+  quiesce();
+  refresh_shadows();
+  const int R = cfg.R, H = cfg.H, B = dses.B, Tw = dses.Tq, W = dses.W, r = dses.round;
+  std::vector<int32_t> q((size_t)B * Tw, 0);                // right-aligned into the session's width, as ques_fwd
+  for (int b = 0; b < B; ++b)
+    for (int t = 0; t < Tq; ++t) q[(size_t)b * Tw + Tw - Tq + t] = ques_host[(size_t)b * Tq + t];
+  int32_t* qd = arena.get<int32_t>((int64_t)B * Tw);
+  VD_CUDA_CHECK(cudaMemcpyAsync(qd, q.data(), q.size() * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpy2DAsync((int32_t*)dses.ques.p + (size_t)r * Tw, (size_t)R * Tw * sizeof(int32_t), qd,
+                                  (size_t)Tw * sizeof(int32_t), (size_t)Tw * sizeof(int32_t), (size_t)B, cudaMemcpyDeviceToDevice,
+                                  cx.stream));
+  ids_q = arena.get<int32_t>((int64_t)B * Tw);
+  transpose_ids(cx, qd, ids_q, B, Tw);
+  if (cfg.useHist) {                                        // history row r: fact r, or the concatenated row r
+    int32_t* hd = arena.get<int32_t>((int64_t)B * W);
+    VD_CUDA_CHECK(cudaMemcpy2DAsync(hd, (size_t)W * sizeof(int32_t), (const int32_t*)dses.hist.p + (size_t)r * W,
+                                    (size_t)R * W * sizeof(int32_t), (size_t)W * sizeof(int32_t), (size_t)B,
+                                    cudaMemcpyDeviceToDevice, cx.stream));
+    ids_h = arena.get<int32_t>((int64_t)B * W);
+    transpose_ids(cx, hd, ids_h, B, W);
+  }
+  encoder_lstms(B, Tw, W, cfg.img_in_q ? (const float*)dses.img_e.p : nullptr);
+  if (cfg.rnn_layers) {                  // the question LSTMs' last state, forward_connect's source, kept for vd_dialog_rnn_state
+    const float* src[4] = {ques1.h_last(), ques1.c_last(), ques2.h_last(), ques2.c_last()};
+    for (int i = 0; i < 4; ++i)
+      VD_CUDA_CHECK(cudaMemcpyAsync(dses.rnn[i].p, src[i], (size_t)B * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
+  }
+  const float* q3 = ques2.h_last();
+  const float* h3 = cfg.useHist ? hist2.h_last() : nullptr;
+  float* out = (float*)dses.enc.p;
+  float* facts = (float*)dses.facts.p;
+  const int64_t fpitch = (int64_t)R * H;
+  if (cfg.fam_lf) {
+    lf_block_fwd(q3, (const float*)dses.fc7.p, (const float*)dses.t_img.p, h3, B, 1, out);
+  } else if (cfg.fam_hre) {
+    float* j = arena.get<float>((int64_t)B * 2 * H);
+    if (cfg.hre_att) {
+      sq = arena.get<float>(B); sh = arena.get<float>(B);
+      int sq_w = seg("att.q.weight"), sh_w = seg("att.h.weight");
+      rowdot_fwd(cx, sq, q3, Wp(sq_w), Wp(sq_w + 1), B, H);
+      rowdot_fwd(cx, sh, h3, Wp(sh_w), Wp(sh_w + 1), B, H);
+      dialog_cache_write(cx, facts, (float*)dses.shc.p, h3, sh, B, R, H, r);
+      hre_join_fwd(q3, facts, sq, (const float*)dses.shc.p, fpitch, B, r, r + 1, j);
+    } else {                             // [q | h]: round r's own fact, no cache
+      hre_join_fwd(q3, h3, nullptr, nullptr, fpitch, B, r, r + 1, j);
+    }
+    // the dialog LSTM's state after round r-1 is state[r & 1] (none at round 0); round r's goes to the other pair
+    const int cur = r & 1, nxt = cur ^ 1;
+    hre_dialog_fwd(j, B, 1, r > 0 ? (const float*)dses.state[2 * cur].p : nullptr,
+                   r > 0 ? (const float*)dses.state[2 * cur + 1].p : nullptr, (float*)dses.state[2 * nxt].p,
+                   (float*)dses.state[2 * nxt + 1].p, out);
+  } else {
+    dialog_cache_write(cx, facts, nullptr, h3, nullptr, B, R, H, r);
+    mn_family_fwd(q3, (const float*)dses.fc7.p, (const float*)dses.t_img.p, facts, fpitch, B, r, r + 1, out);
+  }
+  encOut = out;
+  dses.encOut = out;
+  conn_dh_l1 = conn_dc_l1 = conn_dc_l2 = nullptr;
+  have_fwd = true;                       // for forward_connect(); dialog_finish drops it again
+}
+
+void Engine::dialog_finish(const DialogAnswers& a) {
+  const int r = dses.round;
+  if (cfg.useHist && r + 1 < cfg.R)
+    hist_append(cx, (int32_t*)dses.hist.p, dses.B, cfg.R, dses.W, r, (const int32_t*)dses.ques.p, dses.Tq, a.tokens, a.ld, a.len,
+                a.max_tokens, a.end_token, dses.max_ans_len, cfg.fam_lf);
+}
+
+// runs one ask: the encoder pass, `answer` (which enqueues the answerer and its copies to the host and says where the answers
+// are), the history append, one synchronisation; eval mode throughout.  The round advances only when all of it succeeded.
+template <typename F>
+static void run_ask(Engine* e, const int32_t* ques_host, int Tq, F&& answer) {
+  const int saved_training = e->training;
+  e->training = 0;
+  try {
+    e->dialog_encode(ques_host, Tq);
+    const Engine::DialogAnswers a = answer();
+    e->dialog_finish(a);
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+  } catch (...) { e->training = saved_training; e->have_fwd = false; throw; }
+  e->training = saved_training;
+  e->have_fwd = false;
+  e->dses.round += 1;
+}
+
+void Engine::dialog_ask_beam(const int32_t* ques_host, int Tq, int k, int L, int start_token, int end_token, int32_t* answer_host,
+                             int32_t* length_host, double* score_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a beam-search ask needs the gen decoder");
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  VD_REQUIRE(start_token >= 1 && start_token <= cfg.V && end_token >= 1 && end_token <= cfg.V, VD_E_BADARG,
+             "start_token and end_token in [1, vocabSize]");
+  VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
+  dialog_check_ask(ques_host, Tq);
+  const int64_t B = dses.B;
+  run_ask(this, ques_host, Tq, [&] {
+    const BeamResult res = beam_search_rows(B, 1, 0, k, L, start_token, end_token);
+    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)B * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.len, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.score, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+    return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
+  });
+}
+
+void Engine::dialog_ask_sample(const int32_t* ques_host, int Tq, int L, int start_token, int end_token, float temperature,
+                               uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host) {
+  VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a sampling ask needs the gen decoder");
+  check_sample_args(L, start_token, temperature, row_offset);
+  VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
+  VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
+  dialog_check_ask(ques_host, Tq);
+  const int64_t B = dses.B;
+  const int R = cfg.R, r = dses.round;
+  run_ask(this, ques_host, Tq, [&] {
+    // row b draws as global round row_offset + b*R + r, as vd_gen_dialog_sample's round r does
+    const SampleResult res = sample_rows(B, 1, 0, L, start_token, temperature, seed, row_offset, R, r);
+    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)B * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    if (logp_host)
+      VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)B * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+    return DialogAnswers{res.ans + 1, L + 1, nullptr, L, end_token};
+  });
+}
+
+void Engine::dialog_ask_pool(const int32_t* ques_host, int Tq, int k, int32_t* index_host, float* score_host) {
+  check_pool(k);
+  VD_REQUIRE(index_host && score_host, VD_E_BADARG, "null output pointer");
+  dialog_check_ask(ques_host, Tq);
+  const int64_t B = dses.B;
+  run_ask(this, ques_host, Tq, [&] {
+    float* tv = arena.get<float>(B * k);
+    int32_t* ti = arena.get<int32_t>(B * k);
+    pool_topk(encOut, cfg.H, B, (const float*)pool_emb.p, pool_m, cfg.H, k, tv, ti);
+    int32_t* words = arena.get<int32_t>(B * pool_w);
+    gather_pool_rows(cx, (const int32_t*)pool_tok.p, pool_w, ti, k, B, words);
+    VD_CUDA_CHECK(cudaMemcpyAsync(index_host, ti, (size_t)B * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, tv, (size_t)B * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+    return DialogAnswers{words, pool_w, nullptr, pool_w, cfg.V};
+  });
+}
+
 // model.lua:96-99 + optim_updates.lua:62-91
 void Engine::clamp_adam_step(float lr) {
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   pool_valid = false;                 // the pool's encoding belongs to the weights before this step
+  dses.valid = false;                 // so do a dialog session's cached facts and image products
   join_options_backward();
   float gscale = 1.f;
   if (world > 1) {

@@ -284,14 +284,26 @@ struct Engine {
   void lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last, float* dx_out,
                      float* dh0_out, float* dc0_out);
 
+  void quiesce();                    // drains what an abandoned call left pending, resets the arena; no forward is current
   void encoder_forward(const vd_batch* b);
+  void encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows);   // the question and history LSTM pairs
   void encoder_backward(const float* dEnc);
   // blocks shared by several encoder graphs
   float *qi_join = nullptr, *qi_proj = nullptr;                 // mn-ques-im-hist: [q | fc7] and tanh(Linear(.))
   const float* mn_query_in = nullptr;                           // what enters the memory attention as the query (q3 or qi_proj)
-  void mn_block_fwd(const float* qin, const float* h3, float* out);      // MM -> MaskSoftMax -> MM -> fact -> (+q) -> query
+  // The forward blocks run on rounds [r0, r1) (nr = r1 - r0 rounds) of B dialogs: the full forward passes [0, R), a dialog
+  // session [r, r+1) over its cached facts and image products.
+  // MM -> MaskSoftMax -> MM -> fact -> (+q) -> query; facts of dialog b: rows 0..r1-1 of facts + b*fpitch
+  void mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1);
   void mn_block_bwd(const float* dout, const float* out, float* dqin, float* dh3);   // dqin / dh3 are overwritten
-  void san_block_fwd(const float* u0);                          // SAN hops + out layer -> encOut
+  void san_image(const float* pool5, int64_t B, float* t);      // t (B, S*S, H) = tanh(Linear(pool5)), once per dialog
+  void san_block_fwd(const float* u0, const float* timg, int B, int nr, float* out);   // SAN hops + out layer -> out
+  void lf_block_fwd(const float* q3, const float* fc7, const float* timg, const float* h3, int B, int nr, float* out);
+  void hre_join_fwd(const float* q3, const float* facts, const float* sq, const float* sh, int64_t fpitch, int B, int r0, int r1,
+                    float* j);
+  void hre_dialog_fwd(const float* j, int B, int nr, const float* h0, const float* c0, float* h_out, float* c_out, float* out);
+  void mn_family_fwd(const float* q3, const float* img, const float* timg, const float* facts, int64_t fpitch, int B, int r0,
+                     int r1, float* out);
   void san_block_bwd(const float* dEnc, float* du0);            // du0 (overwritten) = gradient wrt u0
   void forward_connect();
   void decoder_forward();
@@ -318,10 +330,11 @@ struct Engine {
   void gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
                   float* logp_host);
   void check_sample_args(int L, int start_token, float temperature, int64_t row_offset) const;
-  // its sampling on n rounds as beam_search_rows takes them; row i draws as global round row_offset + i * stride + off
+  // its sampling on n rounds as beam_search_rows takes them; row i draws as global round
+  // row_offset + i * draw_stride + draw_off (draw_stride < 0: the state's stride and offset)
   struct SampleResult { int32_t* ans; float* logp; };                   // (n, L + 1), (n, L)
   SampleResult sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature, uint64_t seed,
-                           int64_t row_offset);
+                           int64_t row_offset, int64_t draw_stride = -1, int64_t draw_off = 0);
   // dialogs on the model's own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample): R rounds of {encoder forward on
   // the engine-owned history, round r's search, the history append} on the device
   struct DialogAnswers {             // where round r's answers are, for the history append
@@ -348,6 +361,28 @@ struct Engine {
   void answer_pool_retrieve(const vd_batch* b, int k, int32_t* index_host, float* score_host);
   void answer_pool_dialog(const vd_batch* b, int k, int W, int max_ans_len, int32_t* index_host, float* score_host,
                           int32_t* hist_host);
+  // dialog session (DESIGN §19): B dialogs asked one round at a time.  Its state lives in engine-owned buffers, so any
+  // other call between two asks leaves it intact; an ask encodes round r's B rows only, over the cached facts, image
+  // products and dialog-LSTM state, then answers them and appends round r to the history.
+  struct DialogSession {
+    bool open = false, valid = false;  // valid drops when the weights or the math mode change
+    int B = 0, Tq = 0, W = 0, max_ans_len = 0, round = 0;
+    // state: the dialog-LSTM's {h, c} x 2 (ping-pong, hre / hrea); facts: mn, hrea; rnn: the last ask's question-LSTM
+    // {h1, c1, h2, c2} (encoders with .rnnLayers), the decoder start state besides encOut
+    GrowBuf hist, ques, fc7, img_e, t_img, facts, shc, state[4], rnn[4], enc;
+    const float* encOut = nullptr;   // the last ask's (B, H) encoding
+  } dses;
+  void dialog_begin(const vd_batch* b, int W, int max_ans_len);
+  void dialog_end();
+  void dialog_check_ask(const int32_t* ques_host, int Tq) const;
+  // the ask's encoder pass on round dses.round (questions already checked): encOut and the decoder start state on B rows
+  void dialog_encode(const int32_t* ques_host, int Tq);
+  void dialog_finish(const DialogAnswers& a);   // round r's history append, the round counter
+  void dialog_ask_beam(const int32_t* ques_host, int Tq, int k, int L, int start_token, int end_token, int32_t* answer_host,
+                       int32_t* length_host, double* score_host);
+  void dialog_ask_sample(const int32_t* ques_host, int Tq, int L, int start_token, int end_token, float temperature, uint64_t seed,
+                         int64_t row_offset, int32_t* answer_host, float* logp_host);
+  void dialog_ask_pool(const int32_t* ques_host, int Tq, int k, int32_t* index_host, float* score_host);
   void clamp_adam_step(float lr);
   void allreduce_grads();
   // Overlapped gradient sync (world > 1): dW is all-reduced in buckets on `comm_stream` as soon as each bucket's last

@@ -90,11 +90,21 @@ void rowdot_bwd(LaunchCtx& cx, const float* ds, const float* x, const float* w, 
 // ---- attention over history ----------------------------------------------------------------------
 // mn-att-ques-im-hist.lua:48-62 + MaskSoftMax.lua (mask j>i generated in-kernel, model.lua:281-288)
 void mn_attention_fwd(LaunchCtx& cx, const float* q, const float* h, float* probs, float* hAtt, int B, int R, int H);
+// rounds [r0, r1) only (a dialog session: [r, r+1)): q / hAtt (B*(r1-r0), H), the facts of dialog b rows 0..r1-1 of
+// h + b*hpitch, probs (B, r1-r0, R); row r of the full form's output, bit for bit
+void mn_attention_rows_fwd(LaunchCtx& cx, const float* q, const float* h, int64_t hpitch, float* probs, float* hAtt, int B,
+                           int R, int H, int r0, int r1);
 void mn_attention_bwd(LaunchCtx& cx, const float* q, const float* h, const float* probs, const float* dhAtt,
                       float* dq, float* dh, int B, int R, int H);
 // hrea-ques-im-hist.lua:89-129 + MaskFuture.lua + ReplaceZero.lua
 void hrea_attention_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, float* probs, float* att,
                         int B, int R, int H);
+// rounds [r0, r1) as mn_attention_rows_fwd: sq / att rows B*(r1-r0), sh (B, R), Hs rows of dialog b at Hs + b*hpitch
+void hrea_attention_rows_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, int64_t hpitch, float* probs,
+                             float* att, int B, int R, int H, int r0, int r1);
+// a dialog session's cache write of round r: h3 (B, H) -> row r of facts (B, R, H); sh (B) -> column r of shc (B, R)
+// (both null unless hrea)
+void dialog_cache_write(LaunchCtx& cx, float* facts, float* shc, const float* h3, const float* sh, int64_t B, int R, int H, int r);
 void hrea_attention_bwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, const float* probs,
                         const float* datt, float* dsq, float* dsh, float* dHs, int B, int R, int H);
 // MaskTime.lua:12-28 + JoinTable(-1) (hrea-ques-im-hist.lua:52-55,67-69)

@@ -467,25 +467,30 @@ __global__ void k_rowdot_bwd(const float* __restrict__ ds, const float* __restri
 }
 
 // ------------------------------------------------------------------------------------------------
-// history attention; one block per dialog, dynamic smem = (2 or 3)*R*H + R*R floats
+// history attention; one block per dialog, dynamic smem = (2 or 3)*R*H + R*R floats.  The forwards take a round range
+// [r0, r1): the query / output rows are rounds r0..r1-1 of each dialog (B*(r1-r0) rows), the facts of dialog b are rows
+// 0..r1-1 of h + b*hpitch, probs is (B, r1-r0, R).  The full forward passes [0, R) and hpitch = R*H; a dialog session
+// passes [r, r+1) over its cached facts.  Each output element is reduced in the same order whatever the range.
 __global__ void k_mn_att_fwd(const float* __restrict__ q, const float* __restrict__ h, float* __restrict__ probs,
-                             float* __restrict__ hAtt, int R, int H) {
+                             float* __restrict__ hAtt, int R, int H, int r0, int r1, int64_t hpitch) {
   extern __shared__ float sm[];
-  float* sq = sm; float* shh = sm + R * H; float* S = shh + R * H;
+  const int nr = r1 - r0;
+  float* sq = sm; float* shh = sm + nr * H; float* S = shh + r1 * H;
   const int b = blockIdx.x, tid = threadIdx.x, nw = blockDim.x >> 5, w = tid >> 5, l = tid & 31;
-  for (int i = tid; i < R * H; i += blockDim.x) { sq[i] = q[(int64_t)b * R * H + i]; shh[i] = h[(int64_t)b * R * H + i]; }
+  for (int i = tid; i < nr * H; i += blockDim.x) sq[i] = q[(int64_t)b * nr * H + i];
+  for (int i = tid; i < r1 * H; i += blockDim.x) shh[i] = h[(int64_t)b * hpitch + i];
   __syncthreads();
-  for (int p = w; p < R * R; p += nw) {
-    int i = p / R, j = p % R;
+  for (int p = w; p < nr * R; p += nw) {
+    int i = r0 + p / R, j = p % R;
     float acc = 0.f;
     if (j <= i) {
-      for (int c = l; c < H; c += 32) acc += sq[i * H + c] * shh[j * H + c];
+      for (int c = l; c < H; c += 32) acc += sq[(i - r0) * H + c] * shh[j * H + c];
       acc = warp_sum(acc);
     }
     if (l == 0) S[p] = (j <= i) ? acc : -9999999.f;       // MaskSoftMax.lua:12
   }
   __syncthreads();
-  if (tid < R) {
+  if (tid < nr) {
     float mx = -INFINITY;
     for (int j = 0; j < R; ++j) mx = fmaxf(mx, S[tid * R + j]);
     float sum = 0.f;
@@ -493,12 +498,12 @@ __global__ void k_mn_att_fwd(const float* __restrict__ q, const float* __restric
     for (int j = 0; j < R; ++j) S[tid * R + j] /= sum;
   }
   __syncthreads();
-  for (int i = tid; i < R * R; i += blockDim.x) probs[(int64_t)b * R * R + i] = S[i];
-  for (int o = tid; o < R * H; o += blockDim.x) {
+  for (int i = tid; i < nr * R; i += blockDim.x) probs[(int64_t)b * nr * R + i] = S[i];
+  for (int o = tid; o < nr * H; o += blockDim.x) {
     int i = o / H, c = o % H;
     float acc = 0.f;
-    for (int j = 0; j <= i; ++j) acc += S[i * R + j] * shh[j * H + c];
-    hAtt[(int64_t)b * R * H + o] = acc;
+    for (int j = 0; j <= i + r0; ++j) acc += S[i * R + j] * shh[j * H + c];
+    hAtt[(int64_t)b * nr * H + o] = acc;
   }
 }
 
@@ -539,32 +544,50 @@ __global__ void k_mn_att_bwd(const float* __restrict__ q, const float* __restric
   }
 }
 
+// rounds [r0, r1) as k_mn_att_fwd: sq (B*(r1-r0)), sh (B, R) with only columns j <= i read, Hs rows 0..r1-1 of
+// Hs + b*hpitch.  The weighted sum runs over j <= i: a masked probability is exactly 0, so the terms j > i the sum skips
+// add exact zeros (for finite facts) and the full forward keeps its bits.
 __global__ void k_hrea_att_fwd(const float* __restrict__ sq, const float* __restrict__ sh, const float* __restrict__ Hs,
-                               float* __restrict__ probs, float* __restrict__ att, int R, int H) {
+                               float* __restrict__ probs, float* __restrict__ att, int R, int H, int r0, int r1, int64_t hpitch) {
   extern __shared__ float sm[];
-  float* shh = sm; float* S = shh + R * H;
+  const int nr = r1 - r0;
+  float* shh = sm; float* S = shh + r1 * H;
   const int b = blockIdx.x, tid = threadIdx.x;
-  for (int i = tid; i < R * H; i += blockDim.x) shh[i] = Hs[(int64_t)b * R * H + i];
-  if (tid < R) {
-    int i = tid;
+  for (int i = tid; i < r1 * H; i += blockDim.x) shh[i] = Hs[(int64_t)b * hpitch + i];
+  if (tid < nr) {
+    int i = r0 + tid;
     float row[32];
     float mx = -INFINITY;
     for (int j = 0; j < R; ++j) {
-      float v = (j > i) ? 0.f : sq[b * R + i] + sh[b * R + j];      // MaskFuture.lua:17-19
+      float v = (j > i) ? 0.f : sq[b * nr + tid] + sh[b * R + j];  // MaskFuture.lua:17-19
       if (v == 0.f) v = -INFINITY;                                  // ReplaceZero.lua:13-18
       row[j] = v; mx = fmaxf(mx, v);
     }
     float sum = 0.f;
     for (int j = 0; j < R; ++j) { row[j] = expf(row[j] - mx); sum += row[j]; }
-    for (int j = 0; j < R; ++j) S[i * R + j] = row[j] / sum;
+    for (int j = 0; j < R; ++j) S[tid * R + j] = row[j] / sum;
   }
   __syncthreads();
-  for (int i = tid; i < R * R; i += blockDim.x) probs[(int64_t)b * R * R + i] = S[i];
-  for (int o = tid; o < R * H; o += blockDim.x) {
+  for (int i = tid; i < nr * R; i += blockDim.x) probs[(int64_t)b * nr * R + i] = S[i];
+  for (int o = tid; o < nr * H; o += blockDim.x) {
     int i = o / H, c = o % H;
     float acc = 0.f;
-    for (int j = 0; j < R; ++j) acc += S[i * R + j] * shh[j * H + c];
-    att[(int64_t)b * R * H + o] = acc;
+    for (int j = 0; j <= i + r0; ++j) acc += S[i * R + j] * shh[j * H + c];
+    att[(int64_t)b * nr * H + o] = acc;
+  }
+}
+
+// a dialog session's round-r cache write: fact h3 (B, H) into row r of facts (B, R, H) and, for hrea, its score sh (B)
+// into column r of shc (B, R), in one launch
+__global__ void k_dialog_cache_write(float* __restrict__ facts, float* __restrict__ shc, const float* __restrict__ h3,
+                                     const float* __restrict__ sh, int64_t B, int R, int H, int r) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < B * H) {
+    const int64_t b = i / H;
+    facts[(b * R + r) * H + i % H] = h3[i];
+  } else if (shc && i < B * H + B) {
+    const int64_t b = i - B * H;
+    shc[b * R + r] = sh[b];
   }
 }
 
@@ -1423,9 +1446,14 @@ void rowdot_bwd(LaunchCtx& cx, const float* ds, const float* x, const float* w, 
 }
 
 void mn_attention_fwd(LaunchCtx& cx, const float* q, const float* h, float* probs, float* hAtt, int B, int R, int H) {
-  size_t smem = (size_t)(2 * R * H + R * R) * sizeof(float);
+  mn_attention_rows_fwd(cx, q, h, (int64_t)R * H, probs, hAtt, B, R, H, 0, R);
+}
+void mn_attention_rows_fwd(LaunchCtx& cx, const float* q, const float* h, int64_t hpitch, float* probs, float* hAtt, int B,
+                           int R, int H, int r0, int r1) {
+  VD_REQUIRE(0 <= r0 && r0 < r1 && r1 <= R && hpitch >= (int64_t)r1 * H, VD_E_BADARG, "mn_attention: round range / fact pitch");
+  size_t smem = (size_t)((r1 - r0) * H + r1 * H + (r1 - r0) * R) * sizeof(float);
   set_smem(k_mn_att_fwd, smem);
-  k_mn_att_fwd<<<B, 256, smem, cx.stream>>>(q, h, probs, hAtt, R, H);
+  k_mn_att_fwd<<<B, 256, smem, cx.stream>>>(q, h, probs, hAtt, R, H, r0, r1, hpitch);
   check_launch(cx, "mn_attention_fwd");
 }
 void mn_attention_bwd(LaunchCtx& cx, const float* q, const float* h, const float* probs, const float* dhAtt, float* dq,
@@ -1437,11 +1465,20 @@ void mn_attention_bwd(LaunchCtx& cx, const float* q, const float* h, const float
 }
 void hrea_attention_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, float* probs, float* att, int B,
                         int R, int H) {
+  hrea_attention_rows_fwd(cx, sq, sh, Hs, (int64_t)R * H, probs, att, B, R, H, 0, R);
+}
+void hrea_attention_rows_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, int64_t hpitch, float* probs,
+                             float* att, int B, int R, int H, int r0, int r1) {
   VD_REQUIRE(R <= 32, -2, "maxQuesCount must be <= 32");
-  size_t smem = (size_t)(R * H + R * R) * sizeof(float);
+  VD_REQUIRE(0 <= r0 && r0 < r1 && r1 <= R && hpitch >= (int64_t)r1 * H, VD_E_BADARG, "hrea_attention: round range / fact pitch");
+  size_t smem = (size_t)(r1 * H + (r1 - r0) * R) * sizeof(float);
   set_smem(k_hrea_att_fwd, smem);
-  k_hrea_att_fwd<<<B, 256, smem, cx.stream>>>(sq, sh, Hs, probs, att, R, H);
+  k_hrea_att_fwd<<<B, 256, smem, cx.stream>>>(sq, sh, Hs, probs, att, R, H, r0, r1, hpitch);
   check_launch(cx, "hrea_attention_fwd");
+}
+void dialog_cache_write(LaunchCtx& cx, float* facts, float* shc, const float* h3, const float* sh, int64_t B, int R, int H, int r) {
+  VD_REQUIRE(0 <= r && r < R && (shc == nullptr) == (sh == nullptr), VD_E_BADARG, "dialog_cache_write: round / sh pair");
+  L1D(k_dialog_cache_write, B * H + (shc ? B : 0), facts, shc, h3, sh, B, R, H, r);
 }
 void hrea_attention_bwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, const float* probs,
                         const float* datt, float* dsq, float* dsh, float* dHs, int B, int R, int H) {

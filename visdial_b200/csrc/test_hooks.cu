@@ -41,6 +41,20 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        hrea_attention_bwd(e->cx, CF(0), CF(1), CF(2), CF(3), CF(4), F(5), F(6), F(7), IN(0), IN(1), IN(2));
      }},
+    // round-range forms (a dialog session's [r, r+1)): ints B, R, H, r0, r1, fact pitch
+    {"mn_attention_rows_fwd", 4, 6, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       mn_attention_rows_fwd(e->cx, CF(0), CF(1), I[5], F(2), F(3), IN(0), IN(1), IN(2), IN(3), IN(4));
+     }},
+    {"hrea_attention_rows_fwd", 5, 6, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       hrea_attention_rows_fwd(e->cx, CF(0), CF(1), CF(2), I[5], F(3), F(4), IN(0), IN(1), IN(2), IN(3), IN(4));
+     }},
+    // facts, shc (or null), h3, sh (or null); ints B, R, H, r
+    {"dialog_cache_write", 4, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       dialog_cache_write(e->cx, F(0), F(1), CF(2), CF(3), I[0], IN(1), IN(2), IN(3));
+     }},
     // ---- SAN: ints as the launcher's, the dropout site last; reals p
     {"san_expand_dropout", 2, 5, 1,
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {

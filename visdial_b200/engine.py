@@ -471,6 +471,94 @@ class Engine:
         self._enc_rows = B * R
         return index, score, hist
 
+    # ---- dialog sessions (DESIGN §19): one session per engine; begin and each ask end the last encoder forward
+    def dialog_begin(self, batch: Batch, hist_width: int, max_ans_len: int):
+        """Open a session on the B dialogs of `batch` (vd_dialog_begin): their image rows and round-0 history rows."""
+        self._enc_rows = None
+        check(self.lib.vd_dialog_begin(self.h, C.byref(batch.c), int(hist_width), int(max_ans_len)))
+
+    def _questions(self, ques) -> np.ndarray:
+        """the ask's (B, Tq) rows: the C side reads and writes as many rows as the open session has dialogs"""
+        q = np.ascontiguousarray(ques, dtype=np.int32)
+        if q.ndim != 2:
+            raise ValueError("question rows must be (B, Tq)")
+        B = self.dialog_round()[1]
+        if q.shape[0] != B:
+            raise ValueError("one question row per dialog: the session has %d dialogs, %d rows given" % (B, q.shape[0]))
+        return q
+
+    def dialog_ask_beam(self, ques, k: int, L: int, start: int, end: int):
+        """Ask the next round (vd_dialog_ask_beam): ques (B, Tq) right-aligned rows.  Returns (answer (B, L), length (B),
+        score (B)) as gen_beam_search's."""
+        q = self._questions(ques)
+        B = q.shape[0]
+        ans = np.zeros((B, int(L)), dtype=np.int32)
+        length = np.zeros(B, dtype=np.int32)
+        score = np.zeros(B, dtype=np.float64)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_beam(self.h, q.ctypes.data, int(q.shape[1]), int(k), int(L), int(start), int(end),
+                                          ans.ctypes.data, length.ctypes.data, score.ctypes.data))
+        return ans, length, score
+
+    def dialog_ask_sample(self, ques, L: int, start: int, end: int, temperature: float, seed: int, row_offset: int):
+        """Ask the next round r with sampling (vd_dialog_ask_sample): (answer (B, L+1), logp (B, L)); row b draws as global
+        round row_offset + b maxQuesCount + r."""
+        q = self._questions(ques)
+        B = q.shape[0]
+        ans = np.zeros((B, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((B, int(L)), dtype=np.float32)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_sample(self.h, q.ctypes.data, int(q.shape[1]), int(L), int(start), int(end),
+                                            float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset),
+                                            ans.ctypes.data, logp.ctypes.data))
+        return ans, logp
+
+    def dialog_ask_pool(self, ques, k: int = 1):
+        """Ask the next round of a disc model (vd_dialog_ask_pool): (index (B, k) 0-based pool rows, score (B, k))."""
+        q = self._questions(ques)
+        B = q.shape[0]
+        index = np.zeros((B, int(k)), dtype=np.int32)
+        score = np.zeros((B, int(k)), dtype=np.float32)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_pool(self.h, q.ctypes.data, int(q.shape[1]), int(k), index.ctypes.data,
+                                          score.ctypes.data))
+        return index, score
+
+    def dialog_round(self):
+        """(next round to be asked, B) of the open session (vd_dialog_round)."""
+        r, b = C.c_int32(), C.c_int32()
+        check(self.lib.vd_dialog_round(self.h, C.byref(r), C.byref(b)))
+        return r.value, b.value
+
+    def dialog_history(self, hist_width: int) -> np.ndarray:
+        """The session's history rows (B, maxQuesCount, hist_width) (vd_dialog_history)."""
+        _, B = self.dialog_round()
+        hist = np.zeros((B, self.params["maxQuesCount"], int(hist_width)), dtype=np.int32)
+        check(self.lib.vd_dialog_history(self.h, hist.ctypes.data))
+        return hist
+
+    def dialog_encoding(self) -> DeviceTensor:
+        """The last ask's encoder output (B, rnnHiddenSize) on the device (vd_dialog_encoding)."""
+        _, B = self.dialog_round()
+        p = C.c_void_p()
+        check(self.lib.vd_dialog_encoding(self.h, C.byref(p)))
+        return DeviceTensor(self, p.value, (B, self.params["rnnHiddenSize"]))
+
+    def dialog_rnn_state(self, level: int):
+        """encoder_rnn_state for the last ask (vd_dialog_rnn_state): question-LSTM layer `level`'s (h, c) as (B, H) device
+        tensors, or (None, None) for encoders without .rnnLayers."""
+        _, B = self.dialog_round()
+        hp, cp = C.c_void_p(), C.c_void_p()
+        check(self.lib.vd_dialog_rnn_state(self.h, int(level), C.byref(hp), C.byref(cp)))
+        if not hp.value:
+            return None, None
+        H = self.params["rnnHiddenSize"]
+        return DeviceTensor(self, hp.value, (B, H)), DeviceTensor(self, cp.value, (B, H))
+
+    def dialog_end(self):
+        """Close the session (vd_dialog_end)."""
+        check(self.lib.vd_dialog_end(self.h))
+
     def upload(self, dev_ptr: int, a: np.ndarray):
         a = np.ascontiguousarray(a, dtype=np.float32)
         check(self.lib.vd_memcpy_h2d(self.h, C.c_void_p(dev_ptr), a.ctypes.data, a.nbytes))

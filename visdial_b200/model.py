@@ -364,6 +364,12 @@ class Model:
                                                for it in range(ques.shape[1])]})
         return answerTable
 
+    def openDialogs(self, dataloader, dtype="val", inds=(0,), params=None) -> "DialogSession":
+        """A dialog session (DESIGN §19) on dialogs `inds` (0-based) of split `dtype`: their images and captions, and
+        questions asked one round at a time with DialogSession.ask.  `params` are generateAnswers' beamSize / beamLen /
+        sampleWords / temperature for gen models, retrieveAnswers' topK for disc ones."""
+        return DialogSession(self, dataloader, dtype, inds, params or {})
+
     # ---- checkpoints (train.lua:33-34,78-80,99-102,120-121; evaluate.lua:58-91) -------------------------------
     def save(self, path: str, final: bool = False):
         """torch.save(path, {modelW, optims, modelParams}) — `final` = the model_final.t7 form (float weights, no optims)."""
@@ -376,3 +382,86 @@ class Model:
         ck = load_checkpoint(path, permutation)
         restore(self, ck, restore_adam_state)
         return ck
+
+
+class DialogSession:
+    """Dialogs that are asked one question per round, each round answered before the next is asked (vd_dialog_*, DESIGN
+    §19).  The session opens on the dataset's images and captions; its questions come from `ask`.  The history rule, the
+    widths and the answers are generateAnswers' / retrieveAnswers' with `history = "generated"`: fed the dataset's
+    questions, a session answers as they do."""
+
+    def __init__(self, model, dataloader, dtype, inds, params):
+        self.model, self.dl, self.eng = model, dataloader, model.engine
+        self.inds = np.asarray(list(inds), dtype=np.int64)
+        self.R = model.params["maxQuesCount"]
+        self.disc = model.params["decoder"] == "disc"
+        self.sampleWords = int(params.get("sampleWords", 0)) == 1
+        self.temperature, self.seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
+        self.beamSize, self.beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
+        self.topK = int(params.get("topK", 1))
+        self.start, self.end = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]
+        self.width = dataloader.maxQuesLen
+        maxAnsLen = dataloader.maxAnsLen
+        self.histWidth = 0
+        if model.params.get("useHistory"):
+            self.histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
+                min(dataloader.maxQuesLen + maxAnsLen, dataloader.maxHistoryLen)
+        offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
+        self.rowOffset = (offset + int(self.inds[0])) * self.R      # sampled draws as generateAnswers' for consecutive inds
+        img = getattr(dataloader, "unique_img_" + dtype, None)
+        self.image_ids = [_image_id(img[offset + int(i)]) if img is not None else offset + int(i) for i in self.inds]
+        batch = dataloader.getIndexData(self.inds, model.params, dtype)
+        # the session reads the images and round-0 history rows; questions are asked at the corpus's full width
+        host = {"ques_fwd": np.zeros((len(self.inds), self.R, self.width), np.int32)}
+        for k in ("hist", "img_feat"):
+            if k in batch:
+                host[k] = np.ascontiguousarray(batch[k])
+        if self.disc:
+            self.pool = dataloader.answerPool(dtype)
+            self.eng.answer_pool_encode(self.pool)
+        self.eng.dialog_begin(Batch(host), self.histWidth, maxAnsLen)
+        self.caption = host["hist"][:, 0] if "hist" in host else None      # round 0's history row
+        self.words = getattr(dataloader, "ind2word", None)
+
+    @property
+    def round(self) -> int:
+        return self.eng.dialog_round()[0]
+
+    def ask(self, questions) -> list:
+        """Asks the next round: one question per dialog, text (utils.question_words, unknown words as UNK) or token ids.
+        Returns one entry per dialog as generateAnswers' (question, answer token lists, score / length for the beam, and
+        their text), or retrieveAnswers' for disc models; None where no beam reached <END>."""
+        from .utils import idToWords, question_ids
+        if len(questions) != len(self.inds):
+            raise ValueError("one question per dialog: %d dialogs, %d questions" % (len(self.inds), len(questions)))
+        q = np.stack([question_ids(x, self.dl.word2ind, self.width) for x in questions])
+        text = (lambda ids: idToWords(ids, self.words)) if self.words else None
+        out = []
+        if self.disc:
+            index, score = self.eng.dialog_ask_pool(q, self.topK)
+            for b in range(len(q)):
+                a = [int(t) for t in self.pool[index[b, 0]] if t != 0]
+                out.append({"question": [int(t) for t in q[b] if t], "answer": a, "index": int(index[b, 0]),
+                            "score": float(score[b, 0]),
+                            "topK": [{"index": int(i), "score": float(v),
+                                      "answer": [int(t) for t in self.pool[i] if t != 0]} for i, v in zip(index[b], score[b])]})
+        elif self.sampleWords:
+            ans, _ = self.eng.dialog_ask_sample(q, self.beamLen, self.start, self.end, self.temperature, self.seed,
+                                                self.rowOffset)
+            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
+        else:
+            ans, length, score = self.eng.dialog_ask_beam(q, self.beamSize, self.beamLen, self.start, self.end)
+            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist(), "score": float(score[b]),
+                    "length": int(length[b])} if length[b] > 0 else None for b in range(len(q))]
+        if text:
+            for e in out:
+                if e is not None:
+                    e["question_text"], e["answer_text"] = text(e["question"]), text(e["answer"])
+        return out
+
+    def history(self) -> np.ndarray:
+        """The history rows the encoder reads, (dialogs, maxQuesCount, width)."""
+        return self.eng.dialog_history(self.histWidth)
+
+    def close(self):
+        self.eng.dialog_end()

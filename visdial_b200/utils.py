@@ -1,4 +1,6 @@
 """utils.lua counterparts that stay on the host."""
+import re
+
 import numpy as np
 
 
@@ -15,6 +17,41 @@ def idToWords(vector, ind2word) -> str:
         if nextWord == "<END>":
             break
     return sentence
+
+
+_PUNCT = re.compile(r"([?!.,;:()\[\]{}\"`])")
+_CONTRACTION = re.compile(r"(?<=\w)(n't|'s|'re|'ve|'ll|'d|'m)\b")
+
+
+def question_words(text: str) -> list:
+    """A typed question as prepro.py's `word_tokenize(q + '?')` splits the dataset's questions, on the cases that matter
+    for them: lower case; punctuation split off; the Treebank contractions n't 's 're 've 'll 'd 'm split from their word
+    ("can't" -> "ca n't"); exactly one trailing '?' (one the user typed is not doubled)."""
+    t = text.strip().lower()
+    while t.endswith("?"):
+        t = t[:-1].rstrip()
+    t = _CONTRACTION.sub(r" \1", _PUNCT.sub(r" \1 ", t))
+    return t.split() + ["?"]
+
+
+def question_ids(question, word2ind: dict, width: int) -> np.ndarray:
+    """One question row as a batch's ques_fwd holds it: (width,) int32, right-aligned, zero-padded.  `question` is text
+    (question_words; words missing from word2ind become UNK) or a list of token ids; either is cut to its first `width`
+    tokens, as prepro.py cuts questions to maxQuesLen."""
+    if isinstance(question, str):
+        unk = word2ind.get("UNK")
+        ids = []
+        for w in question_words(question):
+            if w not in word2ind and unk is None:
+                raise ValueError("%r is not in the vocabulary, which has no UNK" % w)
+            ids.append(word2ind.get(w, unk))
+    else:
+        ids = [int(t) for t in question if int(t) != 0]
+    ids = ids[:width]
+    row = np.zeros(width, np.int32)
+    if ids:
+        row[width - len(ids):] = ids
+    return row
 
 
 def image_id(x):
