@@ -282,6 +282,45 @@ int vd_dialog_encoding(vd_engine* e, const float** encOut_dev);
 int vd_dialog_rnn_state(vd_engine* e, int32_t level, const float** h_last, const float** c_last);
 int vd_dialog_end(vd_engine* e);
 
+/* ---- dialog pools: many conversations, each at its own round (DESIGN §20) --------------------- */
+/* A session has a capacity of C slots (vd_dialog_begin's is C = B, all joined at once).  A slot is free or holds one
+ * conversation with its own round r_s in [0, maxQuesCount] and its own cached state (history rows, asked questions,
+ * facts, image products, dialog-LSTM state, draw base).  Conversations join, are asked and leave independently; fed the
+ * same questions, a conversation's answers do not depend on its slot, on when it joined or on which other conversations
+ * share its asks (in VD_MATH_FP32 bit for bit).
+ *  vd_dialog_open: a pool of `capacity` free slots with question width Tq and hist_width / max_ans_len as
+ *    vd_dialog_begin's (hist_width >= Tq); replaces any session.
+ *  vd_dialog_join: batch b's B dialogs (image rows and round-0 history row, as vd_dialog_begin reads them) into the B
+ *    lowest free slots, their ids into slots (B), each at round 0.  draw_base (B) or NULL (all 0): the global round a
+ *    conversation's round 0 draws as in sampling asks.  Fewer than B free slots: VD_E_STATE, nothing joined.
+ *  vd_dialog_leave: frees n slots; a freed slot's cache is never read again and a later join may reuse it.
+ *  vd_dialog_ask_*_slots: one row per asked slot, slots (n) distinct and occupied, ques (n, Tq) HOST as vd_dialog_ask_*'s.
+ *    Row i is encoded at round r of slot slots[i] over that slot's cache, answered as vd_dialog_ask_* answers, appended to
+ *    the slot's history, and the slot's round advances.  Results are in row order.  Sampling: row i draws as global round
+ *    row_offset + draw_base[slot] + r.  vd_dialog_encoding / vd_dialog_rnn_state then have n rows in row order.
+ *  vd_dialog_slots: rounds (capacity) HOST or NULL: each slot's next round, -1 when free; and the capacity.
+ *  vd_dialog_slot_history: the (n, maxQuesCount, hist_width) history rows of n distinct occupied slots.
+ * vd_dialog_ask_* / vd_dialog_round / vd_dialog_history are the all-slots case: an ask of slots 0..C-1, and the round and
+ * rows when every slot is occupied at one round (else VD_E_STATE), as a vd_dialog_begin session is until its first leave.
+ * Refusals, before any state changes: VD_E_STATE for no session, stale weights or math mode (vd_set_parameters,
+ * vd_clamp_adam_step and vd_set_math_mode invalidate the whole pool until it is reopened), a free slot asked or left, a
+ * conversation that has had maxQuesCount asks, a join beyond capacity, an answerer the decoder lacks, a stale pool;
+ * VD_E_BADARG for n < 1, slot ids outside [0, capacity) or named twice, tokens and search arguments; VD_E_SHAPE for a
+ * question width outside [1, Tq]. */
+int vd_dialog_open(vd_engine* e, int32_t capacity, int32_t Tq, int32_t hist_width, int32_t max_ans_len);
+int vd_dialog_join(vd_engine* e, const vd_batch* b, const int64_t* draw_base, int32_t* slots);
+int vd_dialog_leave(vd_engine* e, const int32_t* slots, int32_t n);
+int vd_dialog_ask_beam_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                             int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length,
+                             double* score);
+int vd_dialog_ask_sample_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_len,
+                               int32_t start_token, int32_t end_token, float temperature, uint64_t seed, int64_t row_offset,
+                               int32_t* answer, float* logp);
+int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t k,
+                             int32_t* index, float* score);
+int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
+int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
+
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.
  * The LR decay (model.lua:102-105) stays with the caller, as in the reference. */

@@ -67,6 +67,19 @@ int vd_dialog_history(vd_engine* e, int32_t* hist_host);
 int vd_dialog_encoding(vd_engine* e, const float** encOut_dev);
 int vd_dialog_rnn_state(vd_engine* e, int32_t level, const float** h_last, const float** c_last);
 int vd_dialog_end(vd_engine* e);
+int vd_dialog_open(vd_engine* e, int32_t capacity, int32_t Tq, int32_t hist_width, int32_t max_ans_len);
+int vd_dialog_join(vd_engine* e, const vd_batch* b, const int64_t* draw_base, int32_t* slots);
+int vd_dialog_leave(vd_engine* e, const int32_t* slots, int32_t n);
+int vd_dialog_ask_beam_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                             int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length,
+                             double* score);
+int vd_dialog_ask_sample_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_len,
+                               int32_t start_token, int32_t end_token, float temperature, uint64_t seed, int64_t row_offset,
+                               int32_t* answer, float* logp);
+int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t k,
+                             int32_t* index, float* score);
+int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
+int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
 int vd_clamp_adam_step(vd_engine* e, float learning_rate);
 int vd_comm_unique_id(void* id_out);
 int vd_comm_init(vd_engine* e, const void* id, int32_t rank, int32_t world);

@@ -140,6 +140,16 @@ SIGNATURES = {
     "vd_dialog_encoding": [_H, _P(C.c_void_p)],
     "vd_dialog_rnn_state": [_H, C.c_int32, _P(C.c_void_p), _P(C.c_void_p)],
     "vd_dialog_end": [_H],
+    "vd_dialog_open": [_H, C.c_int32, C.c_int32, C.c_int32, C.c_int32],
+    "vd_dialog_join": [_H, _P(vd_batch), C.c_void_p, C.c_void_p],
+    "vd_dialog_leave": [_H, C.c_void_p, C.c_int32],
+    "vd_dialog_ask_beam_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_dialog_ask_sample_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                   C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p],
+    "vd_dialog_ask_pool_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p],
+    "vd_dialog_slots": [_H, C.c_void_p, _P(C.c_int32)],
+    "vd_dialog_slot_history": [_H, C.c_void_p, C.c_int32, C.c_void_p],
     "vd_gemm_atb16": [_H, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                       C.c_int64, C.c_float],
     "vd_lstm_step_fwd": [_H, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32,

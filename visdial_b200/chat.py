@@ -9,11 +9,22 @@ With `-questions file.json` ({image_id: [question, ...]}, at most maxQuesCount p
 token ids) every image of the file (or of `-imageIds`) is asked its questions, round by round, and
 `<resultPath>/results.json` is written in generate's {opts, data} layout, which the visualiser in vis/ shows.  Without
 it the command talks about one image (the first of `-imageIds`, else the split's first): it reads one question per line
-from stdin and prints each answer.  One GPU only."""
+from stdin and prints each answer.  One GPU only.
+
+With `-serve 1` it serves many conversations at once from a dialog pool of `-capacity` slots (Model.openDialogPool,
+DESIGN §20), reading JSON lines on stdin and writing JSON lines on stdout:
+  in:  {"id": "u1", "image_id": 185565, "question": "is it sunny?"}   (the first line of an id joins it, with its image)
+       {"id": "u1", "leave": true}
+  out: {"id", "round", "question", "answer", ...} for each answer; {"id", "error"} for a refused line (an unknown image, a
+       full pool, an unknown id).  A conversation that has had maxQuesCount answers is left, its last answer with
+       "done": true.
+The server reads every line available without blocking, applies its joins and leaves in arrival order, then asks every
+conversation with a pending question its oldest one, all in one device call (serve_step)."""
 from __future__ import annotations
 
 import json
 import os
+import select
 import sys
 
 from . import cli
@@ -25,6 +36,128 @@ def _image_index(dl, split: str) -> dict:
         raise ValueError("the data has no image ids for split %r" % split)
     from .utils import image_id
     return {image_id(x): i for i, x in enumerate(img)}
+
+
+def serve_step(lines, convs: dict, queues: dict, free: int, images) -> tuple:
+    """One step of the serve loop, without the device.  lines: the JSON objects read since the last ask, in arrival order;
+    convs: the open conversations' ids (each mapped to its slot; None for one joined in this step); queues: {id: [pending
+    question, ...]}; free: the free slots; images: the image ids conversations may join with.  Updates convs and queues and
+    returns (joins [(id, image_id)] new conversations to join, leaves [slot] the slots to free, errors [(id, message)],
+    asks [(id, question)]: each conversation with a pending question, with its oldest)."""
+    joins, leaves, errors = [], [], []
+    for obj in lines:
+        cid = obj.get("id") if isinstance(obj, dict) else None
+        if cid is None:
+            errors.append((None, "a line needs an id"))
+            continue
+        if obj.get("leave"):
+            if cid not in convs:
+                errors.append((cid, "unknown id"))
+                continue
+            if convs[cid] is None:                         # joined in this step: it never reaches the device
+                joins = [j for j in joins if j[0] != cid]
+            else:
+                leaves.append(convs[cid])
+            del convs[cid]
+            queues.pop(cid, None)
+            free += 1
+            continue
+        if cid not in convs:
+            if "image_id" not in obj:
+                errors.append((cid, "unknown id"))
+                continue
+            if obj["image_id"] not in images:
+                errors.append((cid, "unknown image %r" % (obj["image_id"],)))
+                continue
+            if free < 1:
+                errors.append((cid, "the pool is full"))
+                continue
+            free -= 1
+            convs[cid] = None
+            joins.append((cid, obj["image_id"]))
+        if obj.get("question") is not None:
+            queues.setdefault(cid, []).append(obj["question"])
+    asks = [(cid, q.pop(0)) for cid, q in queues.items() if q]
+    for cid in [c for c, q in queues.items() if not q]:
+        del queues[cid]
+    return joins, leaves, errors, asks
+
+
+class _Lines:
+    """stdin's complete lines: read(block) returns those available now, waiting for the first one only when `block`"""
+
+    def __init__(self, fd):
+        self.fd, self.buf, self.eof = fd, b"", False
+
+    def read(self, block: bool) -> list:
+        while not self.eof:
+            ready = b"\n" in self.buf and not select.select([self.fd], [], [], 0)[0]
+            if ready or (not block and not select.select([self.fd], [], [], 0)[0]):
+                break
+            chunk = os.read(self.fd, 1 << 16)
+            if not chunk:
+                self.eof = True
+            self.buf += chunk
+        parts = self.buf.split(b"\n")
+        self.buf = b"" if self.eof else parts.pop()
+        return [p.decode() for p in parts if p.strip()]
+
+
+def serve(model, dl, split: str, index: dict, params: dict, capacity: int, out=sys.stdout):
+    """The -serve loop: JSON lines on stdin, answers as JSON lines on `out`, until stdin ends and nothing is pending."""
+    from .utils import idToWords
+    pool = model.openDialogPool(dl, split, capacity, params)
+    R = model.params["maxQuesCount"]
+    convs, queues, free = {}, {}, capacity
+    src = _Lines(sys.stdin.fileno())
+
+    def emit(obj):
+        out.write(json.dumps(obj) + "\n")
+        out.flush()
+
+    try:
+        while True:
+            raw = src.read(block=not queues)
+            if not raw and not queues and src.eof:
+                break
+            objs = []
+            for line in raw:
+                try:
+                    objs.append(json.loads(line))
+                except ValueError:
+                    objs.append({"id": None})
+            joins, leaves, errors, asks = serve_step(objs, convs, queues, free, index)
+            for cid, msg in errors:
+                emit({"id": cid, "error": msg})
+            if leaves:
+                pool.leave(leaves)
+            if joins:
+                for (cid, _), s in zip(joins, pool.join([index[img] for _, img in joins])):
+                    convs[cid] = s
+            free = capacity - len(convs)
+            if not asks:
+                continue
+            got = pool.ask({convs[cid]: q for cid, q in asks})
+            done = []
+            for cid, q in asks:
+                s = convs[cid]
+                e = got[s]
+                r = pool.round(s)
+                line = {"id": cid, "round": r - 1, "question": idToWords(e["question"], dl.ind2word) if e else None,
+                        "answer": idToWords(e["answer"], dl.ind2word).strip() if e else None}
+                if e and "score" in e:
+                    line["score"] = e["score"]
+                if r == R:
+                    line["done"] = True
+                    done.append(cid)
+                emit(line)
+            if done:
+                pool.leave([convs.pop(c) for c in done])
+                for c in done:
+                    queues.pop(c, None)
+                free = capacity - len(convs)
+    finally:
+        pool.close()
 
 
 def parse(argv=None) -> dict:
@@ -56,6 +189,9 @@ def main(opt: dict, rank: int = 0, world: int = 1):
             raise SystemExit("image ids not in split %s: %s" % (split, missing))
         params = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature")}
         R = model.params["maxQuesCount"]
+        if opt["serve"]:
+            serve(model, dl, split, index, params, opt["capacity"])
+            return
         if asked is None:
             session = model.openDialogs(dl, split, [index[ids[0]]], params)
             if session.caption is not None:

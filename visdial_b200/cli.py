@@ -90,6 +90,8 @@ CHAT_OPTIONS = GENERATE_OPTIONS + [
     ("split", "val", "Split the images and captions come from"),
     ("imageIds", "", "Comma-separated COCO image ids of the split (default: the -questions file's, else its first image)"),
     ("questions", "", "JSON {image_id: [question, ...]}: ask these and write results.json; else read stdin, one per line"),
+    ("serve", 0, "1: serve many conversations from JSON lines on stdin, each answer a JSON line on stdout (DESIGN §20)"),
+    ("capacity", 128, "-serve: how many conversations the dialog pool holds at once"),
 ]
 
 # options of every command that the reference does not have: how the run is spread over GPUs and which math it uses

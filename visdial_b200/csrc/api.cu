@@ -317,30 +317,43 @@ int vd_dialog_begin(vd_engine* h, const vd_batch* b, int32_t hist_width, int32_t
 }
 int vd_dialog_ask_beam(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t beam_size, int32_t beam_len, int32_t start_token,
                        int32_t end_token, int32_t* answer, int32_t* length, double* score) {
-  VD_TRY({ ENG(h)->dialog_ask_beam(ques, Tq, beam_size, beam_len, start_token, end_token, answer, length, score); })
+  VD_TRY({
+    Engine* e = ENG(h);
+    const std::vector<int32_t> s = e->dialog_all_slots();
+    e->dialog_ask_beam(s.data(), (int64_t)s.size(), ques, Tq, beam_size, beam_len, start_token, end_token, answer, length, score);
+  })
 }
 int vd_dialog_ask_sample(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t beam_len, int32_t start_token, int32_t end_token,
                          float temperature, uint64_t seed, int64_t row_offset, int32_t* answer, float* logp) {
-  VD_TRY({ ENG(h)->dialog_ask_sample(ques, Tq, beam_len, start_token, end_token, temperature, seed, row_offset, answer, logp); })
+  VD_TRY({
+    Engine* e = ENG(h);
+    const std::vector<int32_t> s = e->dialog_all_slots();
+    e->dialog_ask_sample(s.data(), (int64_t)s.size(), ques, Tq, beam_len, start_token, end_token, temperature, seed, row_offset,
+                         answer, logp);
+  })
 }
 int vd_dialog_ask_pool(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t k, int32_t* index, float* score) {
-  VD_TRY({ ENG(h)->dialog_ask_pool(ques, Tq, k, index, score); })
+  VD_TRY({
+    Engine* e = ENG(h);
+    const std::vector<int32_t> s = e->dialog_all_slots();
+    e->dialog_ask_pool(s.data(), (int64_t)s.size(), ques, Tq, k, index, score);
+  })
 }
 int vd_dialog_round(vd_engine* h, int32_t* round, int32_t* B) {
   VD_TRY({
     Engine* e = ENG(h);
-    VD_REQUIRE(e->dses.open, VD_E_STATE, "no dialog session");
-    if (round) *round = e->dses.round;
-    if (B) *B = e->dses.B;
+    const int r = e->dialog_lockstep_round();
+    if (round) *round = r;
+    if (B) *B = e->dses.C;
   })
 }
 int vd_dialog_history(vd_engine* h, int32_t* hist_host) {
   VD_TRY({
     Engine* e = ENG(h);
-    VD_REQUIRE(e->dses.open, VD_E_STATE, "no dialog session");
+    e->dialog_lockstep_round();
     NOTNULL(hist_host);
     VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
-    const size_t n = (size_t)e->dses.B * e->cfg.R * e->dses.W;
+    const size_t n = (size_t)e->dses.C * e->cfg.R * e->dses.W;
     if (n) VD_CUDA_CHECK(cudaMemcpyAsync(hist_host, e->dses.hist.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, e->main_stream));
     VD_CUDA_CHECK(cudaStreamSynchronize(e->main_stream));
   })
@@ -364,6 +377,53 @@ int vd_dialog_rnn_state(vd_engine* h, int32_t level, const float** h_last, const
   })
 }
 int vd_dialog_end(vd_engine* h) { VD_TRY({ ENG(h)->dialog_end(); }) }
+
+int vd_dialog_open(vd_engine* h, int32_t capacity, int32_t Tq, int32_t hist_width, int32_t max_ans_len) {
+  VD_TRY({ ENG(h)->dialog_open(capacity, Tq, hist_width, max_ans_len); })
+}
+int vd_dialog_join(vd_engine* h, const vd_batch* b, const int64_t* draw_base, int32_t* slots) {
+  VD_TRY({ ENG(h)->dialog_join(b, draw_base, slots); })
+}
+int vd_dialog_leave(vd_engine* h, const int32_t* slots, int32_t n) { VD_TRY({ ENG(h)->dialog_leave(slots, n); }) }
+int vd_dialog_ask_beam_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                             int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length,
+                             double* score) {
+  VD_TRY({ ENG(h)->dialog_ask_beam(slots, n, ques, Tq, beam_size, beam_len, start_token, end_token, answer, length, score); })
+}
+int vd_dialog_ask_sample_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_len,
+                               int32_t start_token, int32_t end_token, float temperature, uint64_t seed, int64_t row_offset,
+                               int32_t* answer, float* logp) {
+  VD_TRY({
+    ENG(h)->dialog_ask_sample(slots, n, ques, Tq, beam_len, start_token, end_token, temperature, seed, row_offset, answer, logp);
+  })
+}
+int vd_dialog_ask_pool_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t k,
+                             int32_t* index, float* score) {
+  VD_TRY({ ENG(h)->dialog_ask_pool(slots, n, ques, Tq, k, index, score); })
+}
+int vd_dialog_slots(vd_engine* h, int32_t* rounds, int32_t* capacity) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(e->dses.open, VD_E_STATE, "no dialog session");
+    if (rounds) std::copy(e->dses.round.begin(), e->dses.round.end(), rounds);
+    if (capacity) *capacity = e->dses.C;
+  })
+}
+int vd_dialog_slot_history(vd_engine* h, const int32_t* slots, int32_t n, int32_t* hist_host) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(e->dses.open, VD_E_STATE, "no dialog session");
+    e->dialog_check_slots(slots, n);
+    NOTNULL(hist_host);
+    VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
+    const size_t rw = (size_t)e->cfg.R * e->dses.W;
+    if (rw)
+      for (int32_t i = 0; i < n; ++i)
+        VD_CUDA_CHECK(cudaMemcpyAsync(hist_host + i * rw, (const int32_t*)e->dses.hist.p + slots[i] * rw, rw * sizeof(int32_t),
+                                      cudaMemcpyDeviceToHost, e->main_stream));
+    VD_CUDA_CHECK(cudaStreamSynchronize(e->main_stream));
+  })
+}
 
 int vd_clamp_adam_step(vd_engine* h, float lr) { VD_TRY({ ENG(h)->clamp_adam_step(lr); }) }
 

@@ -102,7 +102,13 @@ struct SampleCfg {
   float temperature;
   int64_t row_offset;       // global round of row 0
   int64_t row_stride;       // global rounds between consecutive rows
+  // device (rows): row r's global round, replacing row_offset + r row_stride (a dialog pool's ask, whose rows are
+  // conversations at their own rounds); null: the affine rule
+  const int64_t* row_round = nullptr;
 };
+__device__ __forceinline__ int64_t sample_round(const SampleCfg& s, int64_t r) {
+  return s.row_round ? s.row_round[r] : s.row_offset + r * s.row_stride;
+}
 // largest Gumbel value the rule can produce (u = 1 - 2^-25: -log(-log u) = 17.33): an element whose x / T + GUMBEL_MAX is
 // below the best key so far cannot win, so its Philox word and logarithms need not be computed
 constexpr float GUMBEL_MAX = 17.5f;

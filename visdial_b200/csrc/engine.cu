@@ -785,13 +785,14 @@ static LstmRun make_run(int T, int64_t R, int D, int H, int wseg, const float* x
 // memory network over the history facts (mn-*.lua): MM -> MaskSoftMax (causal) -> MM -> Dropout -> Linear -> Tanh, residual query, Linear -> Tanh
 // Rounds [r0, r1) of B dialogs: qin / out have B*(r1-r0) rows, the facts of dialog b are rows 0..r1-1 of facts + b*fpitch
 // (the full forward: [0, R) over hist2's h_T; a dialog session: [r, r+1) over its cached facts)
-void Engine::mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1) {
+void Engine::mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1,
+                          const int32_t* slot, const int32_t* round) {
   const int H = cfg.H, R = cfg.R;
   const int64_t N = (int64_t)B * (r1 - r0);
   const DropCfg d05 = dropcfg(0.5f);
   probs = arena.get<float>(N * R);
   hAtt = arena.get<float>(N * H);
-  mn_attention_rows_fwd(cx, qin, facts, fpitch, probs, hAtt, B, R, H, r0, r1);
+  mn_attention_rows_fwd(cx, qin, facts, fpitch, probs, hAtt, B, R, H, r0, r1, slot, round);
   hAtt_d = arena.get<float>(N * H);
   dropout_apply(cx, hAtt_d, hAtt, N * H, d05, SITE_HATT);
   hAttTr = arena.get<float>(N * H);
@@ -918,13 +919,13 @@ void Engine::lf_block_fwd(const float* q3, const float* fc7, const float* timg, 
 // of the round's sq over the scores sh (B, R) and facts (dialog b at facts + b*fpitch) of rounds <= it, then [att | q];
 // hre-ques-*.lua: [q | h]
 void Engine::hre_join_fwd(const float* q3, const float* facts, const float* sq_, const float* sh_, int64_t fpitch, int B, int r0,
-                          int r1, float* j) {
+                          int r1, float* j, const int32_t* slot, const int32_t* round) {
   const int H = cfg.H, R = cfg.R;
   const int64_t N = (int64_t)B * (r1 - r0);
   if (cfg.hre_att) {
     probs = arena.get<float>(N * R);
     att = arena.get<float>(N * H);
-    hrea_attention_rows_fwd(cx, sq_, sh_, facts, fpitch, probs, att, B, R, H, r0, r1);
+    hrea_attention_rows_fwd(cx, sq_, sh_, facts, fpitch, probs, att, B, R, H, r0, r1, slot, round);
     copy_cols(cx, j, 2 * H, att, H, N, H);
     copy_cols(cx, j + H, 2 * H, q3, H, N, H);
   } else {
@@ -935,9 +936,8 @@ void Engine::hre_join_fwd(const float* q3, const float* facts, const float* sq_,
 
 // the dialog-level LSTM over nr rounds of B dialogs from (h0, c0) (null: the first round), rows j (B*nr, 2H) in dialog-major
 // order.  View(-1,10,2H), Transpose(1,2): row (r,b) <- row (b,r), a strided 2-D copy per round; out (B*nr, H) dialog-major.
-// h_out / c_out (a session's carried state, nr == 1): where the step writes its h and c instead of the arena.
-void Engine::hre_dialog_fwd(const float* j, int B, int nr, const float* h0, const float* c0, float* h_out, float* c_out,
-                            float* out) {
+// The run (`dialog`) keeps its last h and c, which a dialog session carries to the next round.
+void Engine::hre_dialog_fwd(const float* j, int B, int nr, const float* h0, const float* c0, float* out) {
   const int H = cfg.H;
   const int64_t N = (int64_t)B * nr;
   jt = arena.get<float>(N * 2 * H);
@@ -947,7 +947,6 @@ void Engine::hre_dialog_fwd(const float* j, int B, int nr, const float* h0, cons
   dialog.h0 = h0; dialog.c0 = c0;
   dialog.route = route_lstm(dialog);
   lstm_forward_begin(dialog, true);
-  if (h_out) { dialog.h = h_out; dialog.c = c_out; }  // one saved step: slot 0 is the whole of h and c
   for (int t = 0; t < nr; ++t) lstm_forward_step(dialog, t);
   for (int rr = 0; rr < nr; ++rr)
     copy_cols(cx, out + (int64_t)rr * H, (int64_t)nr * H, dialog.h + (int64_t)rr * B * H, H, B, H);
@@ -956,7 +955,7 @@ void Engine::hre_dialog_fwd(const float* j, int B, int nr, const float* h0, cons
 // mn-ques-hist.lua / mn-ques-im-hist.lua / mn-att-ques-im-hist.lua:48-106 on rounds [r0, r1): q3 / out B*(r1-r0) rows, img
 // the B dialogs' fc7 (mn-ques-im-hist), timg as lf_block_fwd's, facts as mn_block_fwd takes them
 void Engine::mn_family_fwd(const float* q3, const float* img, const float* timg, const float* facts, int64_t fpitch, int B, int r0,
-                           int r1, float* out) {
+                           int r1, float* out, const int32_t* slot, const int32_t* round) {
   const int H = cfg.H, nr = r1 - r0;
   const int64_t N = (int64_t)B * nr;
   mn_query_in = q3;
@@ -973,10 +972,10 @@ void Engine::mn_family_fwd(const float* q3, const float* img, const float* timg,
   }
   if (cfg.san) {
     qh2 = arena.get<float>(N * H);
-    mn_block_fwd(mn_query_in, facts, fpitch, qh2, B, r0, r1);
+    mn_block_fwd(mn_query_in, facts, fpitch, qh2, B, r0, r1, slot, round);
     san_block_fwd(qh2, timg, B, nr, out);
   } else {
-    mn_block_fwd(mn_query_in, facts, fpitch, out, B, r0, r1);
+    mn_block_fwd(mn_query_in, facts, fpitch, out, B, r0, r1, slot, round);
   }
 }
 
@@ -1082,7 +1081,7 @@ void Engine::encoder_forward(const vd_batch* b) {
       rowdot_fwd(cx, sh, h3, Wp(sh_w), Wp(sh_w + 1), N, H);
     }
     hre_join_fwd(q3, h3, sq, sh, (int64_t)R * H, B, 0, R, j);
-    hre_dialog_fwd(j, B, R, nullptr, nullptr, nullptr, nullptr, encOut);
+    hre_dialog_fwd(j, B, R, nullptr, nullptr, encOut);
   } else {
     mn_family_fwd(q3, db.img, timg, h3, (int64_t)R * H, B, 0, R, encOut);
   }
@@ -1835,7 +1834,8 @@ void Engine::check_sample_args(int L, int start_token, float temperature, int64_
 // (k_logsoftmax_sample_rows).  The draw writes the next step's tokens, so nothing waits for the host.  Returns the answers
 // (n, L + 1) and log-probabilities (n, L) in the arena, valid until the next encoder forward.
 Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature,
-                                         uint64_t seed, int64_t row_offset, int64_t draw_stride, int64_t draw_off) {
+                                         uint64_t seed, int64_t row_offset, int64_t draw_stride, int64_t draw_off,
+                                         const int64_t* draw_rounds) {
   forward_connect();
   const int H = cfg.H, V = cfg.V;
   const int64_t N = n;
@@ -1869,7 +1869,7 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
     }
   }
   if (draw_stride < 0) { draw_stride = stride; draw_off = off; }
-  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset + draw_off, draw_stride};
+  SampleCfg smp = {(uint32_t)seed, (uint32_t)(seed >> 32), 0, temperature, row_offset + draw_off, draw_stride, draw_rounds};
   // The step's decoder buffers alternate between two arena regions: step s reads the state step s-1 wrote into the other
   // one, so the new state feeds the next step without a copy.  Same allocations every step, so a region lands where it
   // did two steps earlier and the arena does not grow with L.
@@ -2116,94 +2116,196 @@ void Engine::answer_pool_dialog(const vd_batch* b, int k, int W, int max_ans_len
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
-// ---- dialog sessions (DESIGN §19) ---------------------------------------------------------------------------------------
-// B dialogs from batch b: its image rows and its round-0 history row; its questions, answers and options are not read.
-// The per-dialog image products every round repeats are computed here once, with the weights of this call.
-void Engine::dialog_begin(const vd_batch* b, int W, int max_ans_len) {
-  VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0, VD_E_SHAPE, "session batch with B, Tq > 0");
-  if (cfg.useHist) {
-    VD_REQUIRE(b->hist && b->Th > 0, VD_E_SHAPE, "a history encoder's session needs the batch's round-0 history row");
-    // hist_append (as vd_gen_dialog_*'s loop calls it) needs a row to hold the caption row and a whole question row
-    VD_REQUIRE(W >= b->Th && W >= b->Tq && max_ans_len >= 1, VD_E_BADARG,
-               "hist_width >= the batch's Th and Tq, max_ans_len >= 1");
-  }
-  const vd_batch eb = encoder_only(b);
+// ---- dialog sessions (DESIGN §19, §20) ----------------------------------------------------------------------------------
+// A pool of C slots, each free (round -1) or one conversation at its own round.  Its state is allocated here, once, and
+// indexed by slot; open changes nothing on the device.
+void Engine::dialog_open(int C, int Tq, int W, int max_ans_len) {
+  VD_REQUIRE(C >= 1 && Tq >= 1, VD_E_SHAPE, "a dialog pool with capacity and question width >= 1");
+  // hist_append (as vd_gen_dialog_*'s loop calls it) needs a row to hold the caption row and a whole question row
+  if (cfg.useHist) VD_REQUIRE(W >= Tq && max_ans_len >= 1, VD_E_BADARG, "hist_width >= the question width, max_ans_len >= 1");
   dses.open = dses.valid = false;
+  dses.encOut = nullptr; dses.last_n = 0;
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  const int R = cfg.R, H = cfg.H;
+  if (!cfg.useHist) W = 0;
+  dses.img_cols = cfg.san ? (int64_t)cfg.S * cfg.S * H : cfg.img_in_q ? cfg.IE : cfg.useIm ? cfg.F : 0;
+  if (cfg.useHist) {
+    dses.hist.ensure((size_t)C * R * W * sizeof(int32_t));
+    if (cfg.fam_mn || cfg.hre_att) dses.facts.ensure((size_t)C * R * H * sizeof(float));   // the attention's facts
+    if (cfg.hre_att) dses.shc.ensure((size_t)C * R * sizeof(float));
+    if (cfg.fam_hre)
+      for (auto& g : dses.state) g.ensure((size_t)C * H * sizeof(float));
+  }
+  if (cfg.rnn_layers)
+    for (auto& g : dses.rnn) g.ensure((size_t)C * H * sizeof(float));
+  dses.ques.ensure((size_t)C * R * Tq * sizeof(int32_t));
+  if (dses.img_cols) dses.img.ensure((size_t)C * dses.img_cols * sizeof(float));
+  dses.enc.ensure((size_t)C * H * sizeof(float));
+  dses.C = C; dses.Tq = Tq; dses.W = W; dses.max_ans_len = max_ans_len;
+  dses.round.assign(C, -1);
+  dses.draw_base.assign(C, 0);
+  dses.open = dses.valid = true;
+}
+
+// b's B dialogs (its image rows and round-0 history row; its questions, answers and options are not read) into the lowest
+// free slots.  Their image products, which every round repeats, are computed here once, with the weights of this call.
+void Engine::dialog_join(const vd_batch* b, const int64_t* draw_base, int32_t* slots_host) {
+  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session: call vd_dialog_open");
+  VD_REQUIRE(dses.valid, VD_E_STATE, "the weights or the math mode changed since the session was opened");
+  VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0, VD_E_SHAPE, "join batch with B, Tq > 0");
+  VD_REQUIRE(slots_host != nullptr, VD_E_BADARG, "null slot output");
+  if (cfg.useHist) {
+    VD_REQUIRE(b->hist && b->Th > 0, VD_E_SHAPE, "a history encoder's join needs the batch's round-0 history row");
+    VD_REQUIRE(dses.W >= b->Th, VD_E_BADARG, "hist_width >= the batch's Th");
+  }
+  const int B = b->B;
+  if (draw_base)
+    for (int i = 0; i < B; ++i) VD_REQUIRE(draw_base[i] >= 0, VD_E_BADARG, "draw_base >= 0");
+  std::vector<int32_t> slots;
+  for (int s = 0; s < dses.C && (int)slots.size() < B; ++s)
+    if (dses.round[s] < 0) slots.push_back(s);
+  VD_REQUIRE((int)slots.size() == B, VD_E_STATE, "the pool has fewer free slots than dialogs to join");
+  const vd_batch eb = encoder_only(b);
   quiesce();
   stage_batch(&eb);
   refresh_shadows();
   wait_img();
-  const int R = cfg.R, H = cfg.H, B = db.B, Tq = db.Tq;
-  if (!cfg.useHist) W = 0;
-  if (cfg.useHist) {
-    int32_t* hist = (int32_t*)dses.hist.ensure((size_t)B * R * W * sizeof(int32_t));
-    hist_append(cx, hist, B, R, W, -1, db.hist, db.Th, nullptr, 0, nullptr, 0, 0, 0, false);   // round 0 <- the caption row
-    if (cfg.fam_mn || cfg.hre_att) dses.facts.ensure((size_t)B * R * H * sizeof(float));   // the attention's facts
-    if (cfg.hre_att) dses.shc.ensure((size_t)B * R * sizeof(float));
-    if (cfg.fam_hre)
-      for (auto& g : dses.state) g.ensure((size_t)B * H * sizeof(float));
-  }
-  if (cfg.rnn_layers)
-    for (auto& g : dses.rnn) g.ensure((size_t)B * H * sizeof(float));
-  VD_CUDA_CHECK(cudaMemsetAsync(dses.ques.ensure((size_t)B * R * Tq * sizeof(int32_t)), 0, (size_t)B * R * Tq * sizeof(int32_t),
-                                cx.stream));
+  int32_t* sd = arena.get<int32_t>(B);
+  VD_CUDA_CHECK(cudaMemcpyAsync(sd, slots.data(), (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+  if (cfg.useHist)                   // round 0 <- the caption row
+    hist_append(cx, (int32_t*)dses.hist.p, B, cfg.R, dses.W, -1, db.hist, db.Th, nullptr, 0, nullptr, 0, 0, 0, false, sd);
+  float* img = (float*)dses.img.p;
   if (cfg.san) {
-    san_image(db.img, B, (float*)dses.t_img.ensure((size_t)B * cfg.S * cfg.S * H * sizeof(float)));
+    float* t = arena.get<float>((int64_t)B * dses.img_cols);
+    san_image(db.img, B, t);
+    scatter_rows(cx, img, t, sd, B, dses.img_cols);
+  } else if (cfg.img_in_q) {         // eval mode: hrea's Dropout before img.embed is the identity
+    float* e = arena.get<float>((int64_t)B * cfg.IE);
+    linear_fwd(seg("img.embed.weight"), db.img, B, e, 0);
+    scatter_rows(cx, img, e, sd, B, cfg.IE);
   } else if (cfg.useIm) {
-    float* fc7 = (float*)dses.fc7.ensure((size_t)B * cfg.F * sizeof(float));
-    VD_CUDA_CHECK(cudaMemcpyAsync(fc7, db.img, (size_t)B * cfg.F * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
-    if (cfg.img_in_q)        // eval mode: hrea's Dropout before img.embed is the identity
-      linear_fwd(seg("img.embed.weight"), fc7, B, (float*)dses.img_e.ensure((size_t)B * cfg.IE * sizeof(float)), 0);
+    scatter_rows(cx, img, db.img, sd, B, cfg.F);
   }
-  dses.enc.ensure((size_t)B * H * sizeof(float));
   release_img();
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
-  dses.B = B; dses.Tq = Tq; dses.W = W; dses.max_ans_len = max_ans_len; dses.round = 0; dses.encOut = nullptr;
-  dses.open = dses.valid = true;
+  for (int i = 0; i < B; ++i) {
+    dses.round[slots[i]] = 0;
+    dses.draw_base[slots[i]] = draw_base ? draw_base[i] : 0;
+    slots_host[i] = slots[i];
+  }
 }
 
-void Engine::dialog_end() { dses.open = dses.valid = false; dses.round = 0; dses.encOut = nullptr; }
+void Engine::dialog_check_slots(const int32_t* slots, int64_t n) const {
+  VD_REQUIRE(slots != nullptr && n >= 1, VD_E_BADARG, "at least one slot");
+  std::vector<char> seen(dses.C, 0);
+  for (int64_t i = 0; i < n; ++i) {
+    VD_REQUIRE(slots[i] >= 0 && slots[i] < dses.C, VD_E_BADARG, "a slot id outside [0, capacity)");
+    VD_REQUIRE(!seen[slots[i]], VD_E_BADARG, "a slot named twice");
+    seen[slots[i]] = 1;
+  }
+  for (int64_t i = 0; i < n; ++i) VD_REQUIRE(dses.round[slots[i]] >= 0, VD_E_STATE, "a free slot");
+}
 
-void Engine::dialog_check_ask(const int32_t* ques_host, int Tq) const {
-  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session: call vd_dialog_begin");
-  VD_REQUIRE(dses.valid, VD_E_STATE, "the weights or the math mode changed since vd_dialog_begin");
-  VD_REQUIRE(dses.round < cfg.R, VD_E_STATE, "the session is full: all maxQuesCount rounds have been asked");
+// a freed slot's state is never read again; a later join overwrites what it reads
+void Engine::dialog_leave(const int32_t* slots, int64_t n) {
+  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session");
+  dialog_check_slots(slots, n);
+  for (int64_t i = 0; i < n; ++i) dses.round[slots[i]] = -1;
+}
+
+int Engine::dialog_lockstep_round() const {
+  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session");
+  const int r = dses.round[0];
+  for (int s = 0; s < dses.C; ++s)
+    VD_REQUIRE(dses.round[s] >= 0 && dses.round[s] == r, VD_E_STATE, "the session's slots are not all occupied at one round");
+  return r;
+}
+
+std::vector<int32_t> Engine::dialog_all_slots() const {
+  std::vector<int32_t> s(std::max(dses.C, 0));
+  for (int i = 0; i < dses.C; ++i) s[i] = i;
+  return s;
+}
+
+// the pool of b's B dialogs, all at round 0, sampling as vd_gen_dialog_sample's rows b*R + r
+void Engine::dialog_begin(const vd_batch* b, int W, int max_ans_len) {
+  VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0, VD_E_SHAPE, "session batch with B, Tq > 0");
+  if (cfg.useHist) {
+    VD_REQUIRE(b->hist && b->Th > 0, VD_E_SHAPE, "a history encoder's session needs the batch's round-0 history row");
+    VD_REQUIRE(W >= b->Th && W >= b->Tq && max_ans_len >= 1, VD_E_BADARG,
+               "hist_width >= the batch's Th and Tq, max_ans_len >= 1");
+  }
+  dialog_open(b->B, b->Tq, W, max_ans_len);
+  std::vector<int64_t> base(b->B);
+  for (int i = 0; i < b->B; ++i) base[i] = (int64_t)i * cfg.R;
+  std::vector<int32_t> slots(b->B);
+  try {
+    dialog_join(b, base.data(), slots.data());
+  } catch (...) { dses.open = dses.valid = false; throw; }
+}
+
+void Engine::dialog_end() { dses.open = dses.valid = false; dses.encOut = nullptr; dses.last_n = 0; }
+
+void Engine::dialog_check_ask(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq) const {
+  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session: call vd_dialog_open or vd_dialog_begin");
+  VD_REQUIRE(dses.valid, VD_E_STATE, "the weights or the math mode changed since the session was opened");
+  dialog_check_slots(slots, n);
+  for (int64_t i = 0; i < n; ++i)
+    VD_REQUIRE(dses.round[slots[i]] < cfg.R, VD_E_STATE, "a conversation that has had all maxQuesCount rounds");
   VD_REQUIRE(ques_host != nullptr, VD_E_BADARG, "null question rows");
   VD_REQUIRE(Tq >= 1 && Tq <= dses.Tq, VD_E_SHAPE, "question width in [1, the session's question width]");
-  for (int64_t i = 0; i < (int64_t)dses.B * Tq; ++i)
+  for (int64_t i = 0; i < n * Tq; ++i)
     VD_REQUIRE(ques_host[i] >= 0 && ques_host[i] <= cfg.V, VD_E_BADARG, "a question token outside [0, vocabSize]");
 }
 
-// Round r = dses.round of the B dialogs in eval mode: the question pair over the B new questions, the history pair over the
-// B history rows r, then the family block for round r over the cached state.  Leaves encOut = the session's (B, H) rows and
-// ques1 / ques2 = this pass's runs, which forward_connect() reads; the last encoder_forward is no longer current.
-void Engine::dialog_encode(const int32_t* ques_host, int Tq) {
+// The ask's rows in eval mode: row i is conversation slots[i] at its round r_i.  One upload of the rows, one gather launch
+// (questions into the cache and time-major ids, history row r_i, the slot's image product and dialog-LSTM state), the
+// question and history pairs over the n rows, then the family block with per-row attention over each slot's facts.  Leaves
+// encOut = the (n, H) rows and ques1 / ques2 = this pass's runs, which forward_connect() reads; the last encoder_forward is
+// no longer current.
+Engine::AskRows Engine::dialog_encode(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int64_t row_offset) {
   quiesce();
   refresh_shadows();
-  const int R = cfg.R, H = cfg.H, B = dses.B, Tw = dses.Tq, W = dses.W, r = dses.round;
-  std::vector<int32_t> q((size_t)B * Tw, 0);                // right-aligned into the session's width, as ques_fwd
-  for (int b = 0; b < B; ++b)
-    for (int t = 0; t < Tq; ++t) q[(size_t)b * Tw + Tw - Tq + t] = ques_host[(size_t)b * Tq + t];
-  int32_t* qd = arena.get<int32_t>((int64_t)B * Tw);
-  VD_CUDA_CHECK(cudaMemcpyAsync(qd, q.data(), q.size() * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpy2DAsync((int32_t*)dses.ques.p + (size_t)r * Tw, (size_t)R * Tw * sizeof(int32_t), qd,
-                                  (size_t)Tw * sizeof(int32_t), (size_t)Tw * sizeof(int32_t), (size_t)B, cudaMemcpyDeviceToDevice,
-                                  cx.stream));
-  ids_q = arena.get<int32_t>((int64_t)B * Tw);
-  transpose_ids(cx, qd, ids_q, B, Tw);
-  if (cfg.useHist) {                                        // history row r: fact r, or the concatenated row r
-    int32_t* hd = arena.get<int32_t>((int64_t)B * W);
-    VD_CUDA_CHECK(cudaMemcpy2DAsync(hd, (size_t)W * sizeof(int32_t), (const int32_t*)dses.hist.p + (size_t)r * W,
-                                    (size_t)R * W * sizeof(int32_t), (size_t)W * sizeof(int32_t), (size_t)B,
-                                    cudaMemcpyDeviceToDevice, cx.stream));
-    ids_h = arena.get<int32_t>((int64_t)B * W);
-    transpose_ids(cx, hd, ids_h, B, W);
+  const int R = cfg.R, H = cfg.H, Tw = dses.Tq, W = dses.W;
+  AskRows rows;
+  rows.n = n;
+  std::vector<int32_t> up((size_t)n * (2 + Tw), 0);          // slot, round, questions right-aligned into the session's width
+  std::vector<int64_t> draw(n);
+  bool any_state = false;
+  for (int64_t i = 0; i < n; ++i) {
+    const int s = slots[i], r = dses.round[s];
+    up[i] = s; up[n + i] = r;
+    draw[i] = row_offset + dses.draw_base[s] + r;
+    any_state |= r > 0;
+    rows.any_next |= r + 1 < R;
+    for (int t = 0; t < Tq; ++t) up[2 * n + i * Tw + Tw - Tq + t] = ques_host[i * Tq + t];
   }
-  encoder_lstms(B, Tw, W, cfg.img_in_q ? (const float*)dses.img_e.p : nullptr);
+  int64_t* draw_dev = arena.get<int64_t>(n);
+  int32_t* up_dev = arena.get<int32_t>((int64_t)up.size());
+  VD_CUDA_CHECK(cudaMemcpyAsync(draw_dev, draw.data(), draw.size() * sizeof(int64_t), cudaMemcpyHostToDevice, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(up_dev, up.data(), up.size() * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+  rows.slot = up_dev; rows.round = up_dev + n; rows.draw = draw_dev;
+  DialogGather g;
+  g.n = n; g.R = R; g.slot = rows.slot; g.round = rows.round;
+  g.q = up_dev + 2 * n; g.Tq = Tw; g.ques = (int32_t*)dses.ques.p; g.ids_q = ids_q = arena.get<int32_t>(n * Tw);
+  ids_h = nullptr;
+  if (cfg.useHist) { g.hist = (const int32_t*)dses.hist.p; g.W = W; g.ids_h = ids_h = arena.get<int32_t>(n * W); }
+  float* img = nullptr;
+  if (dses.img_cols) { g.img = (const float*)dses.img.p; g.img_cols = dses.img_cols; g.img_out = img = arena.get<float>(n * dses.img_cols); }
+  if (cfg.fam_hre) {
+    g.h = (const float*)dses.state[0].p; g.c = (const float*)dses.state[1].p; g.H = H;
+    g.h_out = arena.get<float>(n * H); g.c_out = arena.get<float>(n * H);
+  }
+  {
+    const double moved = 8.0 * n * (dses.img_cols + (cfg.fam_hre ? 2 * H : 0)) + 4.0 * n * (3 * Tw + W);
+    LaunchCtx::Scope sc(&cx, "dialog_gather", 0.0, moved);
+    dialog_gather(cx, g);
+  }
+  encoder_lstms(n, Tw, W, cfg.img_in_q ? img : nullptr);
   if (cfg.rnn_layers) {                  // the question LSTMs' last state, forward_connect's source, kept for vd_dialog_rnn_state
     const float* src[4] = {ques1.h_last(), ques1.c_last(), ques2.h_last(), ques2.c_last()};
     for (int i = 0; i < 4; ++i)
-      VD_CUDA_CHECK(cudaMemcpyAsync(dses.rnn[i].p, src[i], (size_t)B * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
+      VD_CUDA_CHECK(cudaMemcpyAsync(dses.rnn[i].p, src[i], (size_t)n * H * sizeof(float), cudaMemcpyDeviceToDevice, cx.stream));
   }
   const float* q3 = ques2.h_last();
   const float* h3 = cfg.useHist ? hist2.h_last() : nullptr;
@@ -2211,108 +2313,108 @@ void Engine::dialog_encode(const int32_t* ques_host, int Tq) {
   float* facts = (float*)dses.facts.p;
   const int64_t fpitch = (int64_t)R * H;
   if (cfg.fam_lf) {
-    lf_block_fwd(q3, (const float*)dses.fc7.p, (const float*)dses.t_img.p, h3, B, 1, out);
+    lf_block_fwd(q3, img, img, h3, (int)n, 1, out);
   } else if (cfg.fam_hre) {
-    float* j = arena.get<float>((int64_t)B * 2 * H);
-    if (cfg.hre_att) {
-      sq = arena.get<float>(B); sh = arena.get<float>(B);
+    float* j = arena.get<float>(n * 2 * H);
+    if (cfg.hre_att) {                   // the row's own fact and score are cached before its attention reads them
+      sq = arena.get<float>(n); sh = arena.get<float>(n);
       int sq_w = seg("att.q.weight"), sh_w = seg("att.h.weight");
-      rowdot_fwd(cx, sq, q3, Wp(sq_w), Wp(sq_w + 1), B, H);
-      rowdot_fwd(cx, sh, h3, Wp(sh_w), Wp(sh_w + 1), B, H);
-      dialog_cache_write(cx, facts, (float*)dses.shc.p, h3, sh, B, R, H, r);
-      hre_join_fwd(q3, facts, sq, (const float*)dses.shc.p, fpitch, B, r, r + 1, j);
-    } else {                             // [q | h]: round r's own fact, no cache
-      hre_join_fwd(q3, h3, nullptr, nullptr, fpitch, B, r, r + 1, j);
+      rowdot_fwd(cx, sq, q3, Wp(sq_w), Wp(sq_w + 1), n, H);
+      rowdot_fwd(cx, sh, h3, Wp(sh_w), Wp(sh_w + 1), n, H);
+      dialog_cache_write(cx, facts, (float*)dses.shc.p, h3, sh, n, R, H, 0, rows.slot, rows.round);
+      hre_join_fwd(q3, facts, sq, (const float*)dses.shc.p, fpitch, (int)n, 0, 1, j, rows.slot, rows.round);
+    } else {                             // [q | h]: the row's own fact, no cache
+      hre_join_fwd(q3, h3, nullptr, nullptr, fpitch, (int)n, 0, 1, j);
     }
-    // the dialog LSTM's state after round r-1 is state[r & 1] (none at round 0); round r's goes to the other pair
-    const int cur = r & 1, nxt = cur ^ 1;
-    hre_dialog_fwd(j, B, 1, r > 0 ? (const float*)dses.state[2 * cur].p : nullptr,
-                   r > 0 ? (const float*)dses.state[2 * cur + 1].p : nullptr, (float*)dses.state[2 * nxt].p,
-                   (float*)dses.state[2 * nxt + 1].p, out);
+    // A row at round 0 continues the zero state the gather wrote; when no row has state, the step runs without one, as the
+    // full forward's first step does.  Either way the new state goes back to the rows' slots.
+    hre_dialog_fwd(j, (int)n, 1, any_state ? g.h_out : nullptr, any_state ? g.c_out : nullptr, out);
+    dialog_cache_write(cx, nullptr, nullptr, nullptr, nullptr, n, R, H, 0, rows.slot, nullptr, (float*)dses.state[0].p,
+                       (float*)dses.state[1].p, dialog.h_last(), dialog.c_last());
   } else {
-    dialog_cache_write(cx, facts, nullptr, h3, nullptr, B, R, H, r);
-    mn_family_fwd(q3, (const float*)dses.fc7.p, (const float*)dses.t_img.p, facts, fpitch, B, r, r + 1, out);
+    dialog_cache_write(cx, facts, nullptr, h3, nullptr, n, R, H, 0, rows.slot, rows.round);
+    mn_family_fwd(q3, img, img, facts, fpitch, (int)n, 0, 1, out, rows.slot, rows.round);
   }
   encOut = out;
   dses.encOut = out;
+  dses.last_n = n;
   conn_dh_l1 = conn_dc_l1 = conn_dc_l2 = nullptr;
-  have_fwd = true;                       // for forward_connect(); dialog_finish drops it again
+  have_fwd = true;                       // for forward_connect(); run_ask drops it again
+  return rows;
 }
 
-void Engine::dialog_finish(const DialogAnswers& a) {
-  const int r = dses.round;
-  if (cfg.useHist && r + 1 < cfg.R)
-    hist_append(cx, (int32_t*)dses.hist.p, dses.B, cfg.R, dses.W, r, (const int32_t*)dses.ques.p, dses.Tq, a.tokens, a.ld, a.len,
-                a.max_tokens, a.end_token, dses.max_ans_len, cfg.fam_lf);
+void Engine::dialog_finish(const AskRows& rows, const DialogAnswers& a) {
+  if (cfg.useHist && rows.any_next)      // rows at round R-1 write nothing
+    hist_append(cx, (int32_t*)dses.hist.p, rows.n, cfg.R, dses.W, 0, (const int32_t*)dses.ques.p, dses.Tq, a.tokens, a.ld, a.len,
+                a.max_tokens, a.end_token, dses.max_ans_len, cfg.fam_lf, rows.slot, rows.round);
 }
 
-// runs one ask: the encoder pass, `answer` (which enqueues the answerer and its copies to the host and says where the answers
-// are), the history append, one synchronisation; eval mode throughout.  The round advances only when all of it succeeded.
+// runs one ask: the encoder pass, `answer(rows)` (which enqueues the answerer and its copies to the host and says where the
+// answers are), the history append, one synchronisation; eval mode throughout.  The rows' rounds advance only when all of
+// it succeeded.
 template <typename F>
-static void run_ask(Engine* e, const int32_t* ques_host, int Tq, F&& answer) {
+static void run_ask(Engine* e, const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int64_t row_offset, F&& answer) {
   const int saved_training = e->training;
   e->training = 0;
   try {
-    e->dialog_encode(ques_host, Tq);
-    const Engine::DialogAnswers a = answer();
-    e->dialog_finish(a);
+    const Engine::AskRows rows = e->dialog_encode(slots, n, ques_host, Tq, row_offset);
+    const Engine::DialogAnswers a = answer(rows);
+    e->dialog_finish(rows, a);
     VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
   } catch (...) { e->training = saved_training; e->have_fwd = false; throw; }
   e->training = saved_training;
   e->have_fwd = false;
-  e->dses.round += 1;
+  for (int64_t i = 0; i < n; ++i) e->dses.round[slots[i]] += 1;
 }
 
-void Engine::dialog_ask_beam(const int32_t* ques_host, int Tq, int k, int L, int start_token, int end_token, int32_t* answer_host,
-                             int32_t* length_host, double* score_host) {
+void Engine::dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int L, int start_token,
+                             int end_token, int32_t* answer_host, int32_t* length_host, double* score_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a beam-search ask needs the gen decoder");
   VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
   VD_REQUIRE(start_token >= 1 && start_token <= cfg.V && end_token >= 1 && end_token <= cfg.V, VD_E_BADARG,
              "start_token and end_token in [1, vocabSize]");
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
-  dialog_check_ask(ques_host, Tq);
-  const int64_t B = dses.B;
-  run_ask(this, ques_host, Tq, [&] {
-    const BeamResult res = beam_search_rows(B, 1, 0, k, L, start_token, end_token);
-    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)B * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-    VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.len, (size_t)B * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.score, (size_t)B * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  dialog_check_ask(slots, n, ques_host, Tq);
+  run_ask(this, slots, n, ques_host, Tq, 0, [&](const AskRows&) {
+    const BeamResult res = beam_search_rows(n, 1, 0, k, L, start_token, end_token);
+    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)n * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.len, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.score, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
     return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
   });
 }
 
-void Engine::dialog_ask_sample(const int32_t* ques_host, int Tq, int L, int start_token, int end_token, float temperature,
-                               uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host) {
+void Engine::dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int L, int start_token,
+                               int end_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
+                               float* logp_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a sampling ask needs the gen decoder");
   check_sample_args(L, start_token, temperature, row_offset);
   VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
-  dialog_check_ask(ques_host, Tq);
-  const int64_t B = dses.B;
-  const int R = cfg.R, r = dses.round;
-  run_ask(this, ques_host, Tq, [&] {
-    // row b draws as global round row_offset + b*R + r, as vd_gen_dialog_sample's round r does
-    const SampleResult res = sample_rows(B, 1, 0, L, start_token, temperature, seed, row_offset, R, r);
-    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)B * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  dialog_check_ask(slots, n, ques_host, Tq);
+  run_ask(this, slots, n, ques_host, Tq, row_offset, [&](const AskRows& rows) {
+    // row i draws as global round row_offset + draw_base[slot] + its round (vd_dialog_begin: vd_gen_dialog_sample's rows)
+    const SampleResult res = sample_rows(n, 1, 0, L, start_token, temperature, seed, 0, -1, 0, rows.draw);
+    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)n * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
     if (logp_host)
-      VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)B * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+      VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)n * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
     return DialogAnswers{res.ans + 1, L + 1, nullptr, L, end_token};
   });
 }
 
-void Engine::dialog_ask_pool(const int32_t* ques_host, int Tq, int k, int32_t* index_host, float* score_host) {
+void Engine::dialog_ask_pool(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int32_t* index_host,
+                             float* score_host) {
   check_pool(k);
   VD_REQUIRE(index_host && score_host, VD_E_BADARG, "null output pointer");
-  dialog_check_ask(ques_host, Tq);
-  const int64_t B = dses.B;
-  run_ask(this, ques_host, Tq, [&] {
-    float* tv = arena.get<float>(B * k);
-    int32_t* ti = arena.get<int32_t>(B * k);
-    pool_topk(encOut, cfg.H, B, (const float*)pool_emb.p, pool_m, cfg.H, k, tv, ti);
-    int32_t* words = arena.get<int32_t>(B * pool_w);
-    gather_pool_rows(cx, (const int32_t*)pool_tok.p, pool_w, ti, k, B, words);
-    VD_CUDA_CHECK(cudaMemcpyAsync(index_host, ti, (size_t)B * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, tv, (size_t)B * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
+  dialog_check_ask(slots, n, ques_host, Tq);
+  run_ask(this, slots, n, ques_host, Tq, 0, [&](const AskRows&) {
+    float* tv = arena.get<float>(n * k);
+    int32_t* ti = arena.get<int32_t>(n * k);
+    pool_topk(encOut, cfg.H, n, (const float*)pool_emb.p, pool_m, cfg.H, k, tv, ti);
+    int32_t* words = arena.get<int32_t>(n * pool_w);
+    gather_pool_rows(cx, (const int32_t*)pool_tok.p, pool_w, ti, k, n, words);
+    VD_CUDA_CHECK(cudaMemcpyAsync(index_host, ti, (size_t)n * k * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, tv, (size_t)n * k * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
     return DialogAnswers{words, pool_w, nullptr, pool_w, cfg.V};
   });
 }

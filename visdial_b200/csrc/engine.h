@@ -293,17 +293,20 @@ struct Engine {
   const float* mn_query_in = nullptr;                           // what enters the memory attention as the query (q3 or qi_proj)
   // The forward blocks run on rounds [r0, r1) (nr = r1 - r0 rounds) of B dialogs: the full forward passes [0, R), a dialog
   // session [r, r+1) over its cached facts and image products.
+  // A dialog pool's ask passes B = n rows, [0, 1) and per-row slot / round (device, n): row i is dialog slot[i] at round
+  // round[i], facts and hrea's sh read at slot[i] (mn_attention_rows_fwd's per-row form).
   // MM -> MaskSoftMax -> MM -> fact -> (+q) -> query; facts of dialog b: rows 0..r1-1 of facts + b*fpitch
-  void mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1);
+  void mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1,
+                    const int32_t* slot = nullptr, const int32_t* round = nullptr);
   void mn_block_bwd(const float* dout, const float* out, float* dqin, float* dh3);   // dqin / dh3 are overwritten
   void san_image(const float* pool5, int64_t B, float* t);      // t (B, S*S, H) = tanh(Linear(pool5)), once per dialog
   void san_block_fwd(const float* u0, const float* timg, int B, int nr, float* out);   // SAN hops + out layer -> out
   void lf_block_fwd(const float* q3, const float* fc7, const float* timg, const float* h3, int B, int nr, float* out);
   void hre_join_fwd(const float* q3, const float* facts, const float* sq, const float* sh, int64_t fpitch, int B, int r0, int r1,
-                    float* j);
-  void hre_dialog_fwd(const float* j, int B, int nr, const float* h0, const float* c0, float* h_out, float* c_out, float* out);
+                    float* j, const int32_t* slot = nullptr, const int32_t* round = nullptr);
+  void hre_dialog_fwd(const float* j, int B, int nr, const float* h0, const float* c0, float* out);
   void mn_family_fwd(const float* q3, const float* img, const float* timg, const float* facts, int64_t fpitch, int B, int r0,
-                     int r1, float* out);
+                     int r1, float* out, const int32_t* slot = nullptr, const int32_t* round = nullptr);
   void san_block_bwd(const float* dEnc, float* du0);            // du0 (overwritten) = gradient wrt u0
   void forward_connect();
   void decoder_forward();
@@ -333,8 +336,10 @@ struct Engine {
   // its sampling on n rounds as beam_search_rows takes them; row i draws as global round
   // row_offset + i * draw_stride + draw_off (draw_stride < 0: the state's stride and offset)
   struct SampleResult { int32_t* ans; float* logp; };                   // (n, L + 1), (n, L)
+  // (draw_rounds non-null, device (n): row i draws as global round draw_rounds[i] instead)
   SampleResult sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature, uint64_t seed,
-                           int64_t row_offset, int64_t draw_stride = -1, int64_t draw_off = 0);
+                           int64_t row_offset, int64_t draw_stride = -1, int64_t draw_off = 0,
+                           const int64_t* draw_rounds = nullptr);
   // dialogs on the model's own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample): R rounds of {encoder forward on
   // the engine-owned history, round r's search, the history append} on the device
   struct DialogAnswers {             // where round r's answers are, for the history append
@@ -361,28 +366,45 @@ struct Engine {
   void answer_pool_retrieve(const vd_batch* b, int k, int32_t* index_host, float* score_host);
   void answer_pool_dialog(const vd_batch* b, int k, int W, int max_ans_len, int32_t* index_host, float* score_host,
                           int32_t* hist_host);
-  // dialog session (DESIGN §19): B dialogs asked one round at a time.  Its state lives in engine-owned buffers, so any
-  // other call between two asks leaves it intact; an ask encodes round r's B rows only, over the cached facts, image
-  // products and dialog-LSTM state, then answers them and appends round r to the history.
+  // dialog sessions (DESIGN §19, §20): a pool of C conversation slots, each free or holding one conversation at its own
+  // round.  The state lives in engine-owned buffers indexed by slot, so any other call between two asks leaves it intact.
+  // An ask encodes one row per asked conversation at that conversation's round, over its slot's cached facts, image
+  // product and dialog-LSTM state, then answers the rows and appends each to its slot's history.  vd_dialog_begin is the
+  // pool of C = B slots all joined at once, its lockstep asks the asks of slots 0..B-1.
   struct DialogSession {
     bool open = false, valid = false;  // valid drops when the weights or the math mode change
-    int B = 0, Tq = 0, W = 0, max_ans_len = 0, round = 0;
-    // state: the dialog-LSTM's {h, c} x 2 (ping-pong, hre / hrea); facts: mn, hrea; rnn: the last ask's question-LSTM
-    // {h1, c1, h2, c2} (encoders with .rnnLayers), the decoder start state besides encOut
-    GrowBuf hist, ques, fc7, img_e, t_img, facts, shc, state[4], rnn[4], enc;
-    const float* encOut = nullptr;   // the last ask's (B, H) encoding
+    int C = 0, Tq = 0, W = 0, max_ans_len = 0;
+    int64_t img_cols = 0;              // the per-slot image product: SAN t_img (S*S*H), img.embed(fc7) (IE) or fc7 (F); 0: none
+    std::vector<int> round;            // per slot: the next round to be asked, -1 while free
+    std::vector<int64_t> draw_base;    // per slot: the global round its round 0 draws as, for sampling asks
+    // per slot: history (C, R, W), asked questions (C, R, Tq), image product (C, img_cols), facts (C, R, H) (mn, hrea), sh
+    // (C, R) (hrea), dialog-LSTM {h, c} (C, H) (hre / hrea).  The last ask's question-LSTM {h1, c1, h2, c2} (encoders with
+    // .rnnLayers) and encoding, n rows in the ask's order: the decoder start state.
+    GrowBuf hist, ques, img, facts, shc, state[2], rnn[4], enc;
+    const float* encOut = nullptr;     // the last ask's (n, H) encoding
+    int64_t last_n = 0;
   } dses;
+  void dialog_open(int C, int Tq, int W, int max_ans_len);
+  // joins b's B dialogs into the lowest free slots (their ids into slots_host); draw_base (B) or null (all 0)
+  void dialog_join(const vd_batch* b, const int64_t* draw_base, int32_t* slots_host);
+  void dialog_leave(const int32_t* slots, int64_t n);
   void dialog_begin(const vd_batch* b, int W, int max_ans_len);
   void dialog_end();
-  void dialog_check_ask(const int32_t* ques_host, int Tq) const;
-  // the ask's encoder pass on round dses.round (questions already checked): encOut and the decoder start state on B rows
-  void dialog_encode(const int32_t* ques_host, int Tq);
-  void dialog_finish(const DialogAnswers& a);   // round r's history append, the round counter
-  void dialog_ask_beam(const int32_t* ques_host, int Tq, int k, int L, int start_token, int end_token, int32_t* answer_host,
-                       int32_t* length_host, double* score_host);
-  void dialog_ask_sample(const int32_t* ques_host, int Tq, int L, int start_token, int end_token, float temperature, uint64_t seed,
-                         int64_t row_offset, int32_t* answer_host, float* logp_host);
-  void dialog_ask_pool(const int32_t* ques_host, int Tq, int k, int32_t* index_host, float* score_host);
+  void dialog_check_slots(const int32_t* slots, int64_t n) const;   // in [0, C), distinct, occupied
+  int dialog_lockstep_round() const;    // every slot occupied and at one round: that round; else VD_E_STATE
+  void dialog_check_ask(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq) const;
+  // the ask's encoder pass over rows (slots[i], round of slots[i]) (checked): encOut and the decoder start state on n rows
+  struct AskRows { int64_t n = 0; const int32_t *slot = nullptr, *round = nullptr; const int64_t* draw = nullptr; bool any_next = false; };
+  AskRows dialog_encode(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int64_t row_offset);
+  void dialog_finish(const AskRows& rows, const DialogAnswers& a);   // the rows' history append
+  void dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int L, int start_token,
+                       int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
+  // row i draws as global round row_offset + draw_base[slots[i]] + its round
+  void dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int L, int start_token, int end_token,
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host);
+  void dialog_ask_pool(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int32_t* index_host,
+                       float* score_host);
+  std::vector<int32_t> dialog_all_slots() const;   // 0..C-1: the lockstep asks' rows
   void clamp_adam_step(float lr);
   void allreduce_grads();
   // Overlapped gradient sync (world > 1): dW is all-reduced in buckets on `comm_stream` as soon as each bucket's last

@@ -278,7 +278,7 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         // lower class.  N % 4 == 0 and 8-column groups: element (row, n0 + c) starts a Philox quadruple.
         float bkey = -INFINITY, bx = 0.f;
         int bcls = 0x7fffffff;
-        const uint64_t ebase = MODE == MODE_SAMPLE ? (uint64_t)(p.smp.row_offset + row * p.smp.row_stride) * (uint64_t)p.N : 0;
+        const uint64_t ebase = (MODE == MODE_SAMPLE && row_ok) ? (uint64_t)sample_round(p.smp, row) * (uint64_t)p.N : 0;
 #pragma unroll 1
         for (int c = half * (BN / NH); c < (half + 1) * (BN / NH); c += 8) {
           if (n0 + c >= p.N) break;                 // warp-uniform

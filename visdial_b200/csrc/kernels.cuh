@@ -91,20 +91,44 @@ void rowdot_bwd(LaunchCtx& cx, const float* ds, const float* x, const float* w, 
 // mn-att-ques-im-hist.lua:48-62 + MaskSoftMax.lua (mask j>i generated in-kernel, model.lua:281-288)
 void mn_attention_fwd(LaunchCtx& cx, const float* q, const float* h, float* probs, float* hAtt, int B, int R, int H);
 // rounds [r0, r1) only (a dialog session: [r, r+1)): q / hAtt (B*(r1-r0), H), the facts of dialog b rows 0..r1-1 of
-// h + b*hpitch, probs (B, r1-r0, R); row r of the full form's output, bit for bit
+// h + b*hpitch, probs (B, r1-r0, R); row r of the full form's output, bit for bit.  slot / round (device, B; a dialog
+// pool's ask): row b alone at round round[b] over the facts of dialog slot[b] (h + slot[b]*hpitch), probs (B, 1, R); r0, r1
+// are not read
 void mn_attention_rows_fwd(LaunchCtx& cx, const float* q, const float* h, int64_t hpitch, float* probs, float* hAtt, int B,
-                           int R, int H, int r0, int r1);
+                           int R, int H, int r0, int r1, const int32_t* slot = nullptr, const int32_t* round = nullptr);
 void mn_attention_bwd(LaunchCtx& cx, const float* q, const float* h, const float* probs, const float* dhAtt,
                       float* dq, float* dh, int B, int R, int H);
 // hrea-ques-im-hist.lua:89-129 + MaskFuture.lua + ReplaceZero.lua
 void hrea_attention_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, float* probs, float* att,
                         int B, int R, int H);
-// rounds [r0, r1) as mn_attention_rows_fwd: sq / att rows B*(r1-r0), sh (B, R), Hs rows of dialog b at Hs + b*hpitch
+// rounds [r0, r1) as mn_attention_rows_fwd: sq / att rows B*(r1-r0), sh (B, R), Hs rows of dialog b at Hs + b*hpitch;
+// slot / round as there (sh then has a row per dialog, read at slot[b])
 void hrea_attention_rows_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, int64_t hpitch, float* probs,
-                             float* att, int B, int R, int H, int r0, int r1);
-// a dialog session's cache write of round r: h3 (B, H) -> row r of facts (B, R, H); sh (B) -> column r of shc (B, R)
-// (both null unless hrea)
-void dialog_cache_write(LaunchCtx& cx, float* facts, float* shc, const float* h3, const float* sh, int64_t B, int R, int H, int r);
+                             float* att, int B, int R, int H, int r0, int r1, const int32_t* slot = nullptr,
+                             const int32_t* round = nullptr);
+// a dialog session's cache write, one launch for every piece given (each destination null with its source):
+//   h3 (B, H) -> facts (dialogs, R, H) at row (slot[b], round[b]); sh (B) -> shc (dialogs, R) at the same place;
+//   hn / cn (B, H) -> st_h / st_c (dialogs, H) at row slot[b] (the dialog LSTM's carried state).
+// slot null: dialog b; round null: round r.
+void dialog_cache_write(LaunchCtx& cx, float* facts, float* shc, const float* h3, const float* sh, int64_t B, int R, int H, int r,
+                        const int32_t* slot = nullptr, const int32_t* round = nullptr, float* st_h = nullptr, float* st_c = nullptr,
+                        const float* hn = nullptr, const float* cn = nullptr);
+// A dialog pool's ask gather, one launch: asked row b is conversation slot[b] at its round round[b] (device, n).
+//   q (n, Tq) right-aligned questions -> the question cache ques (slots, R, Tq) at (slot, round), and ids_q (Tq, n);
+//   the history cache hist (slots, R, W) at (slot, round) -> ids_h (W, n) (ids_h null: no history);
+//   img (slots, img_cols) -> img_out (n, img_cols) (img_out null: no image product);
+//   the dialog-LSTM state h / c (slots, H) -> h_out / c_out (n, H), zeros where round is 0 (h_out null: none).
+struct DialogGather {
+  int64_t n = 0; int R = 0;
+  const int32_t *slot = nullptr, *round = nullptr;
+  const int32_t* q = nullptr; int Tq = 0; int32_t *ques = nullptr, *ids_q = nullptr;
+  const int32_t* hist = nullptr; int W = 0; int32_t* ids_h = nullptr;
+  const float* img = nullptr; int64_t img_cols = 0; float* img_out = nullptr;
+  const float *h = nullptr, *c = nullptr; int H = 0; float *h_out = nullptr, *c_out = nullptr;
+};
+void dialog_gather(LaunchCtx& cx, const DialogGather& g);
+// dst row slot[i] <- src row i (n, cols): a join's image products into the joined slots
+void scatter_rows(LaunchCtx& cx, float* dst, const float* src, const int32_t* slot, int64_t n, int64_t cols);
 void hrea_attention_bwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, const float* probs,
                         const float* datt, float* dsq, float* dsh, float* dHs, int B, int R, int H);
 // MaskTime.lua:12-28 + JoinTable(-1) (hrea-ques-im-hist.lua:52-55,67-69)
@@ -180,8 +204,12 @@ void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, in
 // max_ans_len non-pad words of ans + b*ans_ld before the first end_token, of ans_len[b] - 2 words (ans_len null: ans_max);
 // an empty Q empties A.  Per-round: Q ++ A; concat: row r ++ <END> ++ Q ++ A; the rightmost W words.  An empty row r leaves
 // row r+1 empty (rightAlign's break, utils.lua:20-22).
+// slot (device, B; a dialog pool): CTA b writes dialog slot[b] of hist (and reads its question row slot[b]*R + round);
+// r < 0 (a join) still reads src row b*R.  round (device, B): CTA b appends at round round[b] (r is then any value >= 0),
+// and writes nothing at round R-1.
 void hist_append(LaunchCtx& cx, int32_t* hist, int64_t B, int R, int W, int r, const int32_t* src, int src_w, const int32_t* ans,
-                 int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat);
+                 int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat,
+                 const int32_t* slot = nullptr, const int32_t* round = nullptr);
 
 // ---- optimiser (model.lua:96-99, optim_updates.lua:62-91) ------------------------------------------
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1,

@@ -356,14 +356,20 @@ __global__ void k_repeat_rows(float* __restrict__ dst, const float* __restrict__
   dst[i] = src[(n / R) * lds + c];
 }
 
-// the dialog loop's history rows (hist_append in kernels.cuh), one CTA per dialog
+// the dialog loop's history rows (hist_append in kernels.cuh), one CTA per dialog, or per asked row of a dialog pool
+// (slot non-null: row b writes dialog slot[b], at round round[b] unless r < 0)
 __global__ void k_hist_append(int32_t* __restrict__ hist, int R, int W, int r, const int32_t* __restrict__ src, int src_w,
                               const int32_t* __restrict__ ans, int64_t ans_ld, const int32_t* __restrict__ ans_len, int ans_max,
-                              int end_token, int max_ans_len, int concat) {
+                              int end_token, int max_ans_len, int concat, const int32_t* __restrict__ slot,
+                              const int32_t* __restrict__ round) {
   extern __shared__ int32_t a_s[];                        // the answer's kept words (max_ans_len)
   __shared__ int s_len[3];
-  const int64_t b = blockIdx.x;
-  int32_t* rows = hist + b * R * W;
+  const int64_t b = blockIdx.x, d = slot ? slot[b] : b;
+  int32_t* rows = hist + d * R * W;
+  if (r >= 0 && round) {
+    r = round[b];
+    if (r >= R - 1) return;                                 // the conversation's last round: there is no row r + 1
+  }
   if (r < 0) {
     const int32_t* s = src + b * R * src_w;
     for (int j = threadIdx.x; j < R * W; j += blockDim.x) {
@@ -373,7 +379,7 @@ __global__ void k_hist_append(int32_t* __restrict__ hist, int R, int W, int r, c
     return;
   }
   const int32_t* prev = rows + (int64_t)r * W;
-  const int32_t* q = src + (b * R + r) * src_w;
+  const int32_t* q = src + (d * R + r) * src_w;
   if (threadIdx.x == 0) {
     int lp = 0, lq = 0, la = 0;                            // rows are pads then words: count the words from the right
     while (lp < W && prev[W - 1 - lp] != 0) ++lp;
@@ -470,15 +476,20 @@ __global__ void k_rowdot_bwd(const float* __restrict__ ds, const float* __restri
 // history attention; one block per dialog, dynamic smem = (2 or 3)*R*H + R*R floats.  The forwards take a round range
 // [r0, r1): the query / output rows are rounds r0..r1-1 of each dialog (B*(r1-r0) rows), the facts of dialog b are rows
 // 0..r1-1 of h + b*hpitch, probs is (B, r1-r0, R).  The full forward passes [0, R) and hpitch = R*H; a dialog session
-// passes [r, r+1) over its cached facts.  Each output element is reduced in the same order whatever the range.
+// passes [r, r+1) over its cached facts.  With slot / round non-null (a dialog pool's ask) block b is query row b alone, at
+// round round[b] over the facts of dialog slot[b]: r0, r1 are ignored.  Each output element is reduced in the same order
+// whatever the range.
 __global__ void k_mn_att_fwd(const float* __restrict__ q, const float* __restrict__ h, float* __restrict__ probs,
-                             float* __restrict__ hAtt, int R, int H, int r0, int r1, int64_t hpitch) {
+                             float* __restrict__ hAtt, int R, int H, int r0, int r1, int64_t hpitch,
+                             const int32_t* __restrict__ slot, const int32_t* __restrict__ round) {
   extern __shared__ float sm[];
+  const int b = blockIdx.x, tid = threadIdx.x, nw = blockDim.x >> 5, w = tid >> 5, l = tid & 31;
+  const int64_t d = slot ? slot[b] : b;
+  if (slot) { r0 = round[b]; r1 = r0 + 1; }
   const int nr = r1 - r0;
   float* sq = sm; float* shh = sm + nr * H; float* S = shh + r1 * H;
-  const int b = blockIdx.x, tid = threadIdx.x, nw = blockDim.x >> 5, w = tid >> 5, l = tid & 31;
   for (int i = tid; i < nr * H; i += blockDim.x) sq[i] = q[(int64_t)b * nr * H + i];
-  for (int i = tid; i < r1 * H; i += blockDim.x) shh[i] = h[(int64_t)b * hpitch + i];
+  for (int i = tid; i < r1 * H; i += blockDim.x) shh[i] = h[d * hpitch + i];
   __syncthreads();
   for (int p = w; p < nr * R; p += nw) {
     int i = r0 + p / R, j = p % R;
@@ -546,20 +557,24 @@ __global__ void k_mn_att_bwd(const float* __restrict__ q, const float* __restric
 
 // rounds [r0, r1) as k_mn_att_fwd: sq (B*(r1-r0)), sh (B, R) with only columns j <= i read, Hs rows 0..r1-1 of
 // Hs + b*hpitch.  The weighted sum runs over j <= i: a masked probability is exactly 0, so the terms j > i the sum skips
-// add exact zeros (for finite facts) and the full forward keeps its bits.
+// add exact zeros (for finite facts) and the full forward keeps its bits.  slot / round as k_mn_att_fwd's (sh then
+// (slots, R)).
 __global__ void k_hrea_att_fwd(const float* __restrict__ sq, const float* __restrict__ sh, const float* __restrict__ Hs,
-                               float* __restrict__ probs, float* __restrict__ att, int R, int H, int r0, int r1, int64_t hpitch) {
+                               float* __restrict__ probs, float* __restrict__ att, int R, int H, int r0, int r1, int64_t hpitch,
+                               const int32_t* __restrict__ slot, const int32_t* __restrict__ round) {
   extern __shared__ float sm[];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int64_t d = slot ? slot[b] : b;
+  if (slot) { r0 = round[b]; r1 = r0 + 1; }
   const int nr = r1 - r0;
   float* shh = sm; float* S = shh + r1 * H;
-  const int b = blockIdx.x, tid = threadIdx.x;
-  for (int i = tid; i < r1 * H; i += blockDim.x) shh[i] = Hs[(int64_t)b * hpitch + i];
+  for (int i = tid; i < r1 * H; i += blockDim.x) shh[i] = Hs[d * hpitch + i];
   if (tid < nr) {
     int i = r0 + tid;
     float row[32];
     float mx = -INFINITY;
     for (int j = 0; j < R; ++j) {
-      float v = (j > i) ? 0.f : sq[b * nr + tid] + sh[b * R + j];  // MaskFuture.lua:17-19
+      float v = (j > i) ? 0.f : sq[b * nr + tid] + sh[d * R + j];  // MaskFuture.lua:17-19
       if (v == 0.f) v = -INFINITY;                                  // ReplaceZero.lua:13-18
       row[j] = v; mx = fmaxf(mx, v);
     }
@@ -577,18 +592,76 @@ __global__ void k_hrea_att_fwd(const float* __restrict__ sq, const float* __rest
   }
 }
 
-// a dialog session's round-r cache write: fact h3 (B, H) into row r of facts (B, R, H) and, for hrea, its score sh (B)
-// into column r of shc (B, R), in one launch
+// a dialog session's cache write (dialog_cache_write in kernels.cuh), one thread per element of every piece present:
+// facts, then shc, then the dialog-LSTM state's h and c
 __global__ void k_dialog_cache_write(float* __restrict__ facts, float* __restrict__ shc, const float* __restrict__ h3,
-                                     const float* __restrict__ sh, int64_t B, int R, int H, int r) {
+                                     const float* __restrict__ sh, int64_t B, int R, int H, int r, const int32_t* __restrict__ slot,
+                                     const int32_t* __restrict__ round, float* __restrict__ st_h, float* __restrict__ st_c,
+                                     const float* __restrict__ hn, const float* __restrict__ cn) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < B * H) {
-    const int64_t b = i / H;
-    facts[(b * R + r) * H + i % H] = h3[i];
-  } else if (shc && i < B * H + B) {
-    const int64_t b = i - B * H;
-    shc[b * R + r] = sh[b];
+  const int64_t nf = facts ? B * H : 0, ns = shc ? B : 0;
+  if (i < nf) {
+    const int64_t b = i / H, d = slot ? slot[b] : b, rr = round ? round[b] : r;
+    facts[(d * R + rr) * H + i % H] = h3[i];
+    return;
   }
+  i -= nf;
+  if (i < ns) {
+    const int64_t d = slot ? slot[i] : i, rr = round ? round[i] : r;
+    shc[d * R + rr] = sh[i];
+    return;
+  }
+  i -= ns;
+  if (st_h && i < 2 * B * H) {
+    const bool is_c = i >= B * H;
+    const int64_t e = is_c ? i - B * H : i, b = e / H, d = slot ? slot[b] : b;
+    (is_c ? st_c : st_h)[d * H + e % H] = (is_c ? cn : hn)[e];
+  }
+}
+
+// a dialog pool's ask gather (dialog_gather in kernels.cuh): blockIdx.y picks the piece, threads stride over its elements
+__global__ void k_dialog_gather(DialogGather g) {
+  const int64_t n = g.n, stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  switch (blockIdx.y) {
+    case 0:                                                    // questions: the cache row, and time-major ids
+      for (int64_t i = i0; i < n * g.Tq; i += stride) {
+        const int64_t b = i / g.Tq, t = i % g.Tq;
+        const int32_t v = g.q[i];
+        g.ques[((int64_t)g.slot[b] * g.R + g.round[b]) * g.Tq + t] = v;
+        g.ids_q[t * n + b] = v;
+      }
+      break;
+    case 1:                                                    // history row round[b] of slot[b], time-major
+      if (g.ids_h)
+        for (int64_t i = i0; i < n * g.W; i += stride) {
+          const int64_t b = i / g.W, t = i % g.W;
+          g.ids_h[t * n + b] = g.hist[((int64_t)g.slot[b] * g.R + g.round[b]) * g.W + t];
+        }
+      break;
+    case 2:                                                    // the slot's image product
+      if (g.img_out)
+        for (int64_t i = i0; i < n * g.img_cols; i += stride) {
+          const int64_t b = i / g.img_cols;
+          g.img_out[i] = g.img[(int64_t)g.slot[b] * g.img_cols + i % g.img_cols];
+        }
+      break;
+    default:                                                   // the dialog-LSTM state; zeros for a conversation's round 0
+      if (g.h_out)
+        for (int64_t i = i0; i < n * g.H; i += stride) {
+          const int64_t b = i / g.H, src = (int64_t)g.slot[b] * g.H + i % g.H;
+          const bool first = g.round[b] == 0;
+          g.h_out[i] = first ? 0.f : g.h[src];
+          g.c_out[i] = first ? 0.f : g.c[src];
+        }
+      break;
+  }
+}
+
+__global__ void k_scatter_rows(float* __restrict__ dst, const float* __restrict__ src, const int32_t* __restrict__ slot,
+                               int64_t n, int64_t cols) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n * cols) dst[(int64_t)slot[i / cols] * cols + i % cols] = src[i];
 }
 
 __global__ void k_hrea_att_bwd(const float* __restrict__ Hs, const float* __restrict__ probs, const float* __restrict__ datt,
@@ -1058,7 +1131,7 @@ __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __r
   const int64_t r = blockIdx.x;
   const float* row = x + r * V;
   const float lse = row_lse(row, V, red);
-  const uint64_t base = (uint64_t)(smp.row_offset + r * smp.row_stride) * (uint64_t)V;
+  const uint64_t base = (uint64_t)sample_round(smp, r) * (uint64_t)V;
   const uint64_t q0 = base >> 2, q1 = (base + V - 1) >> 2;
   float bk = -INFINITY;
   int bc = 0x7fffffff;
@@ -1417,12 +1490,14 @@ void repeat_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, 
   L1D(k_repeat_rows, B * R * cols, dst, src, B, R, cols, lds < 0 ? cols : lds);
 }
 void hist_append(LaunchCtx& cx, int32_t* hist, int64_t B, int R, int W, int r, const int32_t* src, int src_w, const int32_t* ans,
-                 int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat) {
+                 int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat,
+                 const int32_t* slot, const int32_t* round) {
   VD_REQUIRE(W >= src_w && src_w > 0 && r < R - 1 && (r < 0 || max_ans_len >= 1), VD_E_BADARG, "hist_append: widths / round");
+  VD_REQUIRE(round == nullptr || slot != nullptr, VD_E_BADARG, "hist_append: per-row rounds need per-row slots");
   if (B <= 0) return;
   const int cap = r < 0 ? 0 : (int)std::min<int64_t>(max_ans_len, ans_ld);   // an answer row holds at most ans_ld words
   k_hist_append<<<(unsigned)B, 128, (size_t)cap * sizeof(int32_t), cx.stream>>>(hist, R, W, r, src, src_w, ans, ans_ld, ans_len,
-                                                                               ans_max, end_token, cap, concat ? 1 : 0);
+                                                                               ans_max, end_token, cap, concat ? 1 : 0, slot, round);
   check_launch(cx, "k_hist_append");
 }
 void sum_repeated_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols) {
@@ -1449,11 +1524,14 @@ void mn_attention_fwd(LaunchCtx& cx, const float* q, const float* h, float* prob
   mn_attention_rows_fwd(cx, q, h, (int64_t)R * H, probs, hAtt, B, R, H, 0, R);
 }
 void mn_attention_rows_fwd(LaunchCtx& cx, const float* q, const float* h, int64_t hpitch, float* probs, float* hAtt, int B,
-                           int R, int H, int r0, int r1) {
+                           int R, int H, int r0, int r1, const int32_t* slot, const int32_t* round) {
+  VD_REQUIRE((slot == nullptr) == (round == nullptr), VD_E_BADARG, "mn_attention: per-row slots and rounds go together");
+  if (slot) { r0 = 0; r1 = R; }                   // one row per block; shared memory for the deepest round
   VD_REQUIRE(0 <= r0 && r0 < r1 && r1 <= R && hpitch >= (int64_t)r1 * H, VD_E_BADARG, "mn_attention: round range / fact pitch");
-  size_t smem = (size_t)((r1 - r0) * H + r1 * H + (r1 - r0) * R) * sizeof(float);
+  const int nr = slot ? 1 : r1 - r0;
+  size_t smem = (size_t)(nr * H + r1 * H + nr * R) * sizeof(float);
   set_smem(k_mn_att_fwd, smem);
-  k_mn_att_fwd<<<B, 256, smem, cx.stream>>>(q, h, probs, hAtt, R, H, r0, r1, hpitch);
+  k_mn_att_fwd<<<B, 256, smem, cx.stream>>>(q, h, probs, hAtt, R, H, r0, r1, hpitch, slot, round);
   check_launch(cx, "mn_attention_fwd");
 }
 void mn_attention_bwd(LaunchCtx& cx, const float* q, const float* h, const float* probs, const float* dhAtt, float* dq,
@@ -1468,17 +1546,36 @@ void hrea_attention_fwd(LaunchCtx& cx, const float* sq, const float* sh, const f
   hrea_attention_rows_fwd(cx, sq, sh, Hs, (int64_t)R * H, probs, att, B, R, H, 0, R);
 }
 void hrea_attention_rows_fwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, int64_t hpitch, float* probs,
-                             float* att, int B, int R, int H, int r0, int r1) {
+                             float* att, int B, int R, int H, int r0, int r1, const int32_t* slot, const int32_t* round) {
   VD_REQUIRE(R <= 32, -2, "maxQuesCount must be <= 32");
+  VD_REQUIRE((slot == nullptr) == (round == nullptr), VD_E_BADARG, "hrea_attention: per-row slots and rounds go together");
+  if (slot) { r0 = 0; r1 = R; }
   VD_REQUIRE(0 <= r0 && r0 < r1 && r1 <= R && hpitch >= (int64_t)r1 * H, VD_E_BADARG, "hrea_attention: round range / fact pitch");
-  size_t smem = (size_t)(r1 * H + (r1 - r0) * R) * sizeof(float);
+  const int nr = slot ? 1 : r1 - r0;
+  size_t smem = (size_t)(r1 * H + nr * R) * sizeof(float);
   set_smem(k_hrea_att_fwd, smem);
-  k_hrea_att_fwd<<<B, 256, smem, cx.stream>>>(sq, sh, Hs, probs, att, R, H, r0, r1, hpitch);
+  k_hrea_att_fwd<<<B, 256, smem, cx.stream>>>(sq, sh, Hs, probs, att, R, H, r0, r1, hpitch, slot, round);
   check_launch(cx, "hrea_attention_fwd");
 }
-void dialog_cache_write(LaunchCtx& cx, float* facts, float* shc, const float* h3, const float* sh, int64_t B, int R, int H, int r) {
-  VD_REQUIRE(0 <= r && r < R && (shc == nullptr) == (sh == nullptr), VD_E_BADARG, "dialog_cache_write: round / sh pair");
-  L1D(k_dialog_cache_write, B * H + (shc ? B : 0), facts, shc, h3, sh, B, R, H, r);
+void dialog_cache_write(LaunchCtx& cx, float* facts, float* shc, const float* h3, const float* sh, int64_t B, int R, int H, int r,
+                        const int32_t* slot, const int32_t* round, float* st_h, float* st_c, const float* hn, const float* cn) {
+  VD_REQUIRE(0 <= r && r < R && (shc == nullptr) == (sh == nullptr) && (facts == nullptr) == (h3 == nullptr) &&
+             (st_h == nullptr) == (hn == nullptr) && (st_c == nullptr) == (cn == nullptr) && (st_h == nullptr) == (st_c == nullptr),
+             VD_E_BADARG, "dialog_cache_write: round / (destination, source) pairs");
+  VD_REQUIRE((round == nullptr || slot != nullptr) && (slot == nullptr || round != nullptr || (!facts && !shc)), VD_E_BADARG,
+             "dialog_cache_write: per-row rounds need per-row slots, and the facts need per-row rounds");
+  L1D(k_dialog_cache_write, (facts ? B * H : 0) + (shc ? B : 0) + (st_h ? 2 * B * H : 0), facts, shc, h3, sh, B, R, H, r, slot, round,
+      st_h, st_c, hn, cn);
+}
+void dialog_gather(LaunchCtx& cx, const DialogGather& g) {
+  if (g.n <= 0) return;
+  const int64_t most = std::max({g.n * g.Tq, g.n * g.W, g.n * g.img_cols, g.n * (int64_t)g.H});
+  const unsigned gx = (unsigned)std::min<int64_t>(blocks_for(most, 256), 2048);
+  k_dialog_gather<<<dim3(gx, 4), 256, 0, cx.stream>>>(g);
+  check_launch(cx, "dialog_gather");
+}
+void scatter_rows(LaunchCtx& cx, float* dst, const float* src, const int32_t* slot, int64_t n, int64_t cols) {
+  L1D(k_scatter_rows, n * cols, dst, src, slot, n, cols);
 }
 void hrea_attention_bwd(LaunchCtx& cx, const float* sq, const float* sh, const float* Hs, const float* probs,
                         const float* datt, float* dsq, float* dsh, float* dHs, int B, int R, int H) {

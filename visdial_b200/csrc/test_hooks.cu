@@ -55,6 +55,39 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        dialog_cache_write(e->cx, F(0), F(1), CF(2), CF(3), I[0], IN(1), IN(2), IN(3));
      }},
+    // per-row forms (a dialog pool's ask): ptrs as above, then slot, round (device, n); ints n, R, H, fact pitch
+    {"mn_attention_slots_fwd", 6, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       mn_attention_rows_fwd(e->cx, CF(0), CF(1), I[3], F(2), F(3), IN(0), IN(1), IN(2), 0, 1, CI32(4), CI32(5));
+     }},
+    {"hrea_attention_slots_fwd", 7, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       hrea_attention_rows_fwd(e->cx, CF(0), CF(1), CF(2), I[3], F(3), F(4), IN(0), IN(1), IN(2), 0, 1, CI32(5), CI32(6));
+     }},
+    // facts, shc, h3, sh, slot, round, st_h, st_c, hn, cn (each pair may be null); ints n, R, H
+    {"dialog_cache_write_slots", 10, 3, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       dialog_cache_write(e->cx, F(0), F(1), CF(2), CF(3), I[0], IN(1), IN(2), 0, CI32(4), CI32(5), F(6), F(7), CF(8), CF(9));
+     }},
+    // slot, round, q, ques, ids_q, hist, ids_h, img, img_out, h, c, h_out, c_out; ints n, R, Tq, W, img_cols, H
+    {"dialog_gather", 13, 6, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       DialogGather g;
+       g.n = I[0]; g.R = IN(1); g.slot = CI32(0); g.round = CI32(1); g.q = CI32(2); g.Tq = IN(2); g.ques = I32(3); g.ids_q = I32(4);
+       g.hist = CI32(5); g.W = IN(3); g.ids_h = I32(6); g.img = CF(7); g.img_cols = I[4]; g.img_out = F(8);
+       g.h = CF(9); g.c = CF(10); g.H = IN(5); g.h_out = F(11); g.c_out = F(12);
+       dialog_gather(e->cx, g);
+     }},
+    // dst, src, slot; ints n, cols
+    {"scatter_rows", 3, 2, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) { scatter_rows(e->cx, F(0), CF(1), CI32(2), I[0], I[1]); }},
+    // hist, src, ans, ans_len (or null), slot, round (or null); ints B, R, W, r, src_w, ans_ld, ans_max, end_token,
+    // max_ans_len, concat
+    {"hist_append_slots", 6, 10, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       hist_append(e->cx, I32(0), I[0], IN(1), IN(2), IN(3), CI32(1), IN(4), CI32(2), I[5], CI32(3), IN(6), IN(7), IN(8), I[9] != 0,
+                   CI32(4), CI32(5));
+     }},
     // ---- SAN: ints as the launcher's, the dropout site last; reals p
     {"san_expand_dropout", 2, 5, 1,
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {
@@ -130,6 +163,15 @@ const Entry TABLE[] = {
        s.temperature = (float)X[0]; s.row_offset = I[5]; s.row_stride = I[6];
        logsoftmax_sample_rows(e->cx, CF(0), I[0], IN(1), s, IN(2), I32(1), I32(2), F(3));
      }},
+    // as logsoftmax_sample_rows, and a fifth pointer: the per-row global rounds (SampleCfg::row_round)
+    {"logsoftmax_sample_rows_drawn", 5, 7, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       SampleCfg s;
+       s.seed_lo = (uint32_t)(uint64_t)I[3]; s.seed_hi = (uint32_t)((uint64_t)I[3] >> 32); s.step = (uint32_t)I[4];
+       s.temperature = (float)X[0]; s.row_offset = I[5]; s.row_stride = I[6];
+       s.row_round = static_cast<const int64_t*>(P[4]);
+       logsoftmax_sample_rows(e->cx, CF(0), I[0], IN(1), s, IN(2), I32(1), I32(2), F(3));
+     }},
     // ptrs logits, lse, tgt, mask_ids, scale, dlogits (may alias logits); ints rows, V
     {"nll_bwd_scaled", 6, 2, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
@@ -158,6 +200,16 @@ const Entry TABLE[] = {
        SampleCfg s;
        s.seed_lo = (uint32_t)(uint64_t)I[5]; s.seed_hi = (uint32_t)((uint64_t)I[5] >> 32); s.step = (uint32_t)I[6];
        s.temperature = (float)X[0]; s.row_offset = I[7]; s.row_stride = I[8];
+       VD_REQUIRE(vocab_sample_tc(e->cx, IN(0), IN(1), IN(2), CF(0), I[3], CF(1), I[4], CF(2), s, F(3), F(4), F(5), I32(6), F(7)),
+                  VD_E_SHAPE, "vocab_sample_tc: shape refused");
+     }},
+    // as vocab_sample_tc, and a ninth pointer: the per-row global rounds (SampleCfg::row_round)
+    {"vocab_sample_tc_drawn", 9, 9, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       SampleCfg s;
+       s.seed_lo = (uint32_t)(uint64_t)I[5]; s.seed_hi = (uint32_t)((uint64_t)I[5] >> 32); s.step = (uint32_t)I[6];
+       s.temperature = (float)X[0]; s.row_offset = I[7]; s.row_stride = I[8];
+       s.row_round = static_cast<const int64_t*>(P[8]);
        VD_REQUIRE(vocab_sample_tc(e->cx, IN(0), IN(1), IN(2), CF(0), I[3], CF(1), I[4], CF(2), s, F(3), F(4), F(5), I32(6), F(7)),
                   VD_E_SHAPE, "vocab_sample_tc: shape refused");
      }},

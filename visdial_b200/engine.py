@@ -498,6 +498,7 @@ class Engine:
         self._enc_rows = None
         check(self.lib.vd_dialog_ask_beam(self.h, q.ctypes.data, int(q.shape[1]), int(k), int(L), int(start), int(end),
                                           ans.ctypes.data, length.ctypes.data, score.ctypes.data))
+        self._dialog_rows = B
         return ans, length, score
 
     def dialog_ask_sample(self, ques, L: int, start: int, end: int, temperature: float, seed: int, row_offset: int):
@@ -511,6 +512,7 @@ class Engine:
         check(self.lib.vd_dialog_ask_sample(self.h, q.ctypes.data, int(q.shape[1]), int(L), int(start), int(end),
                                             float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset),
                                             ans.ctypes.data, logp.ctypes.data))
+        self._dialog_rows = B
         return ans, logp
 
     def dialog_ask_pool(self, ques, k: int = 1):
@@ -522,6 +524,7 @@ class Engine:
         self._enc_rows = None
         check(self.lib.vd_dialog_ask_pool(self.h, q.ctypes.data, int(q.shape[1]), int(k), index.ctypes.data,
                                           score.ctypes.data))
+        self._dialog_rows = B
         return index, score
 
     def dialog_round(self):
@@ -538,8 +541,8 @@ class Engine:
         return hist
 
     def dialog_encoding(self) -> DeviceTensor:
-        """The last ask's encoder output (B, rnnHiddenSize) on the device (vd_dialog_encoding)."""
-        _, B = self.dialog_round()
+        """The last ask's encoder output (rows, rnnHiddenSize) on the device, in the ask's row order (vd_dialog_encoding)."""
+        B = getattr(self, "_dialog_rows", 0)
         p = C.c_void_p()
         check(self.lib.vd_dialog_encoding(self.h, C.byref(p)))
         return DeviceTensor(self, p.value, (B, self.params["rnnHiddenSize"]))
@@ -547,7 +550,7 @@ class Engine:
     def dialog_rnn_state(self, level: int):
         """encoder_rnn_state for the last ask (vd_dialog_rnn_state): question-LSTM layer `level`'s (h, c) as (B, H) device
         tensors, or (None, None) for encoders without .rnnLayers."""
-        _, B = self.dialog_round()
+        B = getattr(self, "_dialog_rows", 0)
         hp, cp = C.c_void_p(), C.c_void_p()
         check(self.lib.vd_dialog_rnn_state(self.h, int(level), C.byref(hp), C.byref(cp)))
         if not hp.value:
@@ -558,6 +561,96 @@ class Engine:
     def dialog_end(self):
         """Close the session (vd_dialog_end)."""
         check(self.lib.vd_dialog_end(self.h))
+
+    # ---- dialog pools (DESIGN §20): conversations that join, are asked and leave on their own, each at its own round
+    def dialog_open(self, capacity: int, Tq: int, hist_width: int, max_ans_len: int):
+        """Open a pool of `capacity` free slots (vd_dialog_open); replaces any session."""
+        self._dialog_rows = 0
+        check(self.lib.vd_dialog_open(self.h, int(capacity), int(Tq), int(hist_width), int(max_ans_len)))
+
+    def dialog_join(self, batch: Batch, draw_base=None) -> np.ndarray:
+        """Join the batch's B dialogs (their image rows and round-0 history rows) into free slots (vd_dialog_join);
+        draw_base (B) is each one's global round of round 0 for sampling (None: 0).  Returns the slot ids (B)."""
+        B = int(batch.c.B)
+        slots = np.zeros(B, dtype=np.int32)
+        base = None
+        if draw_base is not None:
+            base = np.ascontiguousarray(draw_base, dtype=np.int64)
+            if base.shape != (B,):
+                raise ValueError("one draw base per joined dialog")
+        self._enc_rows = None
+        check(self.lib.vd_dialog_join(self.h, C.byref(batch.c), base.ctypes.data if base is not None else None,
+                                      slots.ctypes.data))
+        return slots
+
+    def dialog_leave(self, slots):
+        """Free the slots (vd_dialog_leave)."""
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        check(self.lib.vd_dialog_leave(self.h, s.ctypes.data, int(s.size)))
+
+    @staticmethod
+    def _slot_rows(slots, ques):
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        q = np.ascontiguousarray(ques, dtype=np.int32)
+        if q.ndim != 2 or q.shape[0] != s.size:
+            raise ValueError("one question row per asked slot: %d slots, question rows of shape %s" % (s.size, q.shape))
+        return s, q
+
+    def dialog_ask_beam_slots(self, slots, ques, k: int, L: int, start: int, end: int):
+        """Ask slots (n) one question each (vd_dialog_ask_beam_slots), each at its own round: (answer (n, L), length (n),
+        score (n)) in row order."""
+        s, q = self._slot_rows(slots, ques)
+        n = s.size
+        ans = np.zeros((n, int(L)), dtype=np.int32)
+        length = np.zeros(n, dtype=np.int32)
+        score = np.zeros(n, dtype=np.float64)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_beam_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(k), int(L),
+                                                int(start), int(end), ans.ctypes.data, length.ctypes.data, score.ctypes.data))
+        self._dialog_rows = n
+        return ans, length, score
+
+    def dialog_ask_sample_slots(self, slots, ques, L: int, start: int, end: int, temperature: float, seed: int,
+                                row_offset: int = 0):
+        """vd_dialog_ask_sample_slots: (answer (n, L+1), logp (n, L)); row i draws as global round row_offset +
+        draw_base[slot] + the slot's round."""
+        s, q = self._slot_rows(slots, ques)
+        n = s.size
+        ans = np.zeros((n, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((n, int(L)), dtype=np.float32)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_sample_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(L), int(start),
+                                                  int(end), float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset),
+                                                  ans.ctypes.data, logp.ctypes.data))
+        self._dialog_rows = n
+        return ans, logp
+
+    def dialog_ask_pool_slots(self, slots, ques, k: int = 1):
+        """vd_dialog_ask_pool_slots: (index (n, k) 0-based pool rows, score (n, k))."""
+        s, q = self._slot_rows(slots, ques)
+        n = s.size
+        index = np.zeros((n, int(k)), dtype=np.int32)
+        score = np.zeros((n, int(k)), dtype=np.float32)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_pool_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(k),
+                                                index.ctypes.data, score.ctypes.data))
+        self._dialog_rows = n
+        return index, score
+
+    def dialog_slots(self) -> np.ndarray:
+        """Each slot's next round, -1 when free (vd_dialog_slots); its length is the capacity."""
+        cap = C.c_int32()
+        check(self.lib.vd_dialog_slots(self.h, None, C.byref(cap)))
+        rounds = np.zeros(cap.value, dtype=np.int32)
+        check(self.lib.vd_dialog_slots(self.h, rounds.ctypes.data, C.byref(cap)))
+        return rounds
+
+    def dialog_slot_history(self, slots, hist_width: int) -> np.ndarray:
+        """The history rows (n, maxQuesCount, hist_width) of the slots (vd_dialog_slot_history)."""
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        hist = np.zeros((s.size, self.params["maxQuesCount"], int(hist_width)), dtype=np.int32)
+        check(self.lib.vd_dialog_slot_history(self.h, s.ctypes.data, int(s.size), hist.ctypes.data))
+        return hist
 
     def upload(self, dev_ptr: int, a: np.ndarray):
         a = np.ascontiguousarray(a, dtype=np.float32)

@@ -370,6 +370,12 @@ class Model:
         sampleWords / temperature for gen models, retrieveAnswers' topK for disc ones."""
         return DialogSession(self, dataloader, dtype, inds, params or {})
 
+    def openDialogPool(self, dataloader, dtype="val", capacity=128, params=None) -> "DialogPool":
+        """A dialog pool (DESIGN §20) of `capacity` conversations on the images and captions of split `dtype`: they join
+        (DialogPool.join), are asked (DialogPool.ask) and leave on their own, each at its own round.  `params` as
+        openDialogs'."""
+        return DialogPool(self, dataloader, dtype, params or {}, capacity=capacity)
+
     # ---- checkpoints (train.lua:33-34,78-80,99-102,120-121; evaluate.lua:58-91) -------------------------------
     def save(self, path: str, final: bool = False):
         """torch.save(path, {modelW, optims, modelParams}) — `final` = the model_final.t7 form (float weights, no optims)."""
@@ -384,15 +390,15 @@ class Model:
         return ck
 
 
-class DialogSession:
-    """Dialogs that are asked one question per round, each round answered before the next is asked (vd_dialog_*, DESIGN
-    §19).  The session opens on the dataset's images and captions; its questions come from `ask`.  The history rule, the
-    widths and the answers are generateAnswers' / retrieveAnswers' with `history = "generated"`: fed the dataset's
-    questions, a session answers as they do."""
+class DialogPool:
+    """Conversations about the dataset's images that join, are asked and leave on their own, each at its own round
+    (vd_dialog_open / join / ask_*_slots / leave, DESIGN §20).  A conversation is one dataset dialog's image and caption,
+    asked its questions one at a time; the history rule, the widths and the answers are generateAnswers' /
+    retrieveAnswers' with `history = "generated"`, and a sampled conversation draws as generateAnswers does for that
+    dialog.  Fed the same questions, a conversation's answers do not depend on the others asked with it."""
 
-    def __init__(self, model, dataloader, dtype, inds, params):
-        self.model, self.dl, self.eng = model, dataloader, model.engine
-        self.inds = np.asarray(list(inds), dtype=np.int64)
+    def __init__(self, model, dataloader, dtype, params, capacity=None):
+        self.model, self.dl, self.eng, self.dtype = model, dataloader, model.engine, dtype
         self.R = model.params["maxQuesCount"]
         self.disc = model.params["decoder"] == "disc"
         self.sampleWords = int(params.get("sampleWords", 0)) == 1
@@ -401,27 +407,101 @@ class DialogSession:
         self.topK = int(params.get("topK", 1))
         self.start, self.end = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]
         self.width = dataloader.maxQuesLen
-        maxAnsLen = dataloader.maxAnsLen
+        self.maxAnsLen = dataloader.maxAnsLen
         self.histWidth = 0
         if model.params.get("useHistory"):
             self.histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
-                min(dataloader.maxQuesLen + maxAnsLen, dataloader.maxHistoryLen)
-        offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
-        self.rowOffset = (offset + int(self.inds[0])) * self.R      # sampled draws as generateAnswers' for consecutive inds
-        img = getattr(dataloader, "unique_img_" + dtype, None)
-        self.image_ids = [_image_id(img[offset + int(i)]) if img is not None else offset + int(i) for i in self.inds]
-        batch = dataloader.getIndexData(self.inds, model.params, dtype)
-        # the session reads the images and round-0 history rows; questions are asked at the corpus's full width
-        host = {"ques_fwd": np.zeros((len(self.inds), self.R, self.width), np.int32)}
-        for k in ("hist", "img_feat"):
-            if k in batch:
-                host[k] = np.ascontiguousarray(batch[k])
+                min(dataloader.maxQuesLen + self.maxAnsLen, dataloader.maxHistoryLen)
+        self.offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) \
+            else 0
+        self.rowOffset = 0                   # sampling: a slot draws as global round draw_base + its round
+        self.words = getattr(dataloader, "ind2word", None)
         if self.disc:
             self.pool = dataloader.answerPool(dtype)
             self.eng.answer_pool_encode(self.pool)
-        self.eng.dialog_begin(Batch(host), self.histWidth, maxAnsLen)
+        if capacity is not None:
+            self.eng.dialog_open(int(capacity), self.width, self.histWidth, self.maxAnsLen)
+
+    def _batch(self, inds) -> dict:
+        """what a join reads of dialogs `inds`: images and round-0 history rows; questions are asked at the full width"""
+        batch = self.dl.getIndexData(np.asarray(inds, dtype=np.int64), self.model.params, self.dtype)
+        host = {"ques_fwd": np.zeros((len(inds), self.R, self.width), np.int32)}
+        for k in ("hist", "img_feat"):
+            if k in batch:
+                host[k] = np.ascontiguousarray(batch[k])
+        return host
+
+    def join(self, inds) -> list:
+        """Joins dialogs `inds` (0-based, of the split) as new conversations at round 0; returns their slots.  Raises
+        VdError (VD_E_STATE) and joins none when fewer slots are free."""
+        inds = [int(i) for i in inds]
+        host = self._batch(inds)
+        base = np.asarray([(self.offset + i) * self.R for i in inds], np.int64)
+        return self.eng.dialog_join(Batch(host), base).tolist()
+
+    def ask(self, questions: dict) -> dict:
+        """Asks each slot of `questions` ({slot: question}, text or token ids) its next round, all in one device call.
+        Returns {slot: entry} with DialogSession.ask's entries."""
+        from .utils import question_ids
+        slots = [int(s) for s in questions]
+        q = np.stack([question_ids(questions[s], self.dl.word2ind, self.width) for s in slots])
+        return dict(zip(slots, self._ask(slots, q)))
+
+    def _ask(self, slots, q) -> list:
+        from .utils import idToWords
+        text = (lambda ids: idToWords(ids, self.words)) if self.words else None
+        out = []
+        if self.disc:
+            index, score = self.eng.dialog_ask_pool_slots(slots, q, self.topK)
+            for b in range(len(q)):
+                a = [int(t) for t in self.pool[index[b, 0]] if t != 0]
+                out.append({"question": [int(t) for t in q[b] if t], "answer": a, "index": int(index[b, 0]),
+                            "score": float(score[b, 0]),
+                            "topK": [{"index": int(i), "score": float(v),
+                                      "answer": [int(t) for t in self.pool[i] if t != 0]} for i, v in zip(index[b], score[b])]})
+        elif self.sampleWords:
+            ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature, self.seed,
+                                                      self.rowOffset)
+            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
+        else:
+            ans, length, score = self.eng.dialog_ask_beam_slots(slots, q, self.beamSize, self.beamLen, self.start, self.end)
+            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist(), "score": float(score[b]),
+                    "length": int(length[b])} if length[b] > 0 else None for b in range(len(q))]
+        if text:
+            for e in out:
+                if e is not None:
+                    e["question_text"], e["answer_text"] = text(e["question"]), text(e["answer"])
+        return out
+
+    def leave(self, slots):
+        self.eng.dialog_leave([int(s) for s in slots])
+
+    def round(self, slot: int) -> int:
+        """The slot's next round to be asked (R once it has had maxQuesCount), -1 when free."""
+        return int(self.eng.dialog_slots()[int(slot)])
+
+    def history(self, slots) -> np.ndarray:
+        """The history rows the encoder reads, (len(slots), maxQuesCount, width)."""
+        return self.eng.dialog_slot_history([int(s) for s in slots], self.histWidth)
+
+    def close(self):
+        self.eng.dialog_end()
+
+
+class DialogSession(DialogPool):
+    """Dialogs that are asked one question per round, each round answered before the next is asked (vd_dialog_begin,
+    DESIGN §19): the pool whose slots 0..B-1 are dialogs `inds`, all asked at every round.  Fed the dataset's questions, a
+    session answers as generateAnswers / retrieveAnswers with `history = "generated"` do."""
+
+    def __init__(self, model, dataloader, dtype, inds, params):
+        super().__init__(model, dataloader, dtype, params)
+        self.inds = np.asarray(list(inds), dtype=np.int64)
+        self.rowOffset = (self.offset + int(self.inds[0])) * self.R      # draws as generateAnswers' for consecutive inds
+        img = getattr(dataloader, "unique_img_" + dtype, None)
+        self.image_ids = [_image_id(img[self.offset + int(i)]) if img is not None else self.offset + int(i) for i in self.inds]
+        host = self._batch(self.inds)
+        self.eng.dialog_begin(Batch(host), self.histWidth, self.maxAnsLen)
         self.caption = host["hist"][:, 0] if "hist" in host else None      # round 0's history row
-        self.words = getattr(dataloader, "ind2word", None)
 
     @property
     def round(self) -> int:
@@ -431,37 +511,12 @@ class DialogSession:
         """Asks the next round: one question per dialog, text (utils.question_words, unknown words as UNK) or token ids.
         Returns one entry per dialog as generateAnswers' (question, answer token lists, score / length for the beam, and
         their text), or retrieveAnswers' for disc models; None where no beam reached <END>."""
-        from .utils import idToWords, question_ids
+        from .utils import question_ids
         if len(questions) != len(self.inds):
             raise ValueError("one question per dialog: %d dialogs, %d questions" % (len(self.inds), len(questions)))
         q = np.stack([question_ids(x, self.dl.word2ind, self.width) for x in questions])
-        text = (lambda ids: idToWords(ids, self.words)) if self.words else None
-        out = []
-        if self.disc:
-            index, score = self.eng.dialog_ask_pool(q, self.topK)
-            for b in range(len(q)):
-                a = [int(t) for t in self.pool[index[b, 0]] if t != 0]
-                out.append({"question": [int(t) for t in q[b] if t], "answer": a, "index": int(index[b, 0]),
-                            "score": float(score[b, 0]),
-                            "topK": [{"index": int(i), "score": float(v),
-                                      "answer": [int(t) for t in self.pool[i] if t != 0]} for i, v in zip(index[b], score[b])]})
-        elif self.sampleWords:
-            ans, _ = self.eng.dialog_ask_sample(q, self.beamLen, self.start, self.end, self.temperature, self.seed,
-                                                self.rowOffset)
-            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
-        else:
-            ans, length, score = self.eng.dialog_ask_beam(q, self.beamSize, self.beamLen, self.start, self.end)
-            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist(), "score": float(score[b]),
-                    "length": int(length[b])} if length[b] > 0 else None for b in range(len(q))]
-        if text:
-            for e in out:
-                if e is not None:
-                    e["question_text"], e["answer_text"] = text(e["question"]), text(e["answer"])
-        return out
+        return self._ask(list(range(len(q))), q)
 
     def history(self) -> np.ndarray:
         """The history rows the encoder reads, (dialogs, maxQuesCount, width)."""
         return self.eng.dialog_history(self.histWidth)
-
-    def close(self):
-        self.eng.dialog_end()
