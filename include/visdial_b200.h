@@ -321,6 +321,24 @@ int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, cons
 int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
 int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
 
+/* ---- resuming conversations in a dialog pool (DESIGN §21) ------------------------------------ */
+/* vd_dialog_join_rounds: batch b's B dialogs join the open pool in the free slots slots[i] (HOST, an input: a reopened
+ * pool puts each conversation back in its own slot), at rounds[i] in [0, maxQuesCount-1] (HOST), with the rounds
+ * 0..rounds[i]-1 they already had: the image row and round-0 history row as vd_dialog_join reads them; questions 0..r-1
+ * from b->ques_fwd, right-aligned into the pool's width as asks do; answers (B, maxQuesCount, Ta) HOST word ids, row j
+ * the answer to question j, left-aligned and zero-padded (zeros are not words; <END> = vocabSize ends one).  draw_base as
+ * vd_dialog_join's, or NULL.  Afterwards a slot's history rows 0..r, question cache, facts and sh of rounds < r, dialog-LSTM
+ * (h, c) after round r-1, round (r) and draw base are those of a conversation that joined at round 0 and was asked
+ * q_0..q_{r-1} with the pool's answers replaced by a_0..a_{r-1} (in VD_MATH_FP32 bit for bit); round r's fact comes with
+ * the next ask.  One encoder pass over the sum of the rounds' rows, one synchronisation.  lf-ques / lf-ques-im: only the
+ * questions and the round are set, and answers may be NULL.
+ * Refusals, before any state changes: VD_E_STATE for no pool, a stale pool or an occupied target slot; VD_E_BADARG for a
+ * round outside [0, maxQuesCount-1], a slot outside [0, capacity) or named twice, Ta < 1, answer or question tokens
+ * outside [0, vocabSize], null answers for a history encoder, hist_width < b->Th; VD_E_SHAPE for b->Tq above the pool's
+ * question width. */
+int vd_dialog_join_rounds(vd_engine* e, const vd_batch* b, const int32_t* rounds, const int32_t* answers, int32_t Ta,
+                          const int64_t* draw_base, const int32_t* slots);
+
 /* ---- optimiser step (model.lua:96-105 + optim_updates.lua:62-91) ---------------------------- */
 /* all-reduce(SUM)/world of dW when a communicator is attached, then clamp(-5,5), then adam.
  * The LR decay (model.lua:102-105) stays with the caller, as in the reference. */

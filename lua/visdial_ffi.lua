@@ -80,6 +80,8 @@ int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, cons
                              int32_t* index, float* score);
 int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
 int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
+int vd_dialog_join_rounds(vd_engine* e, const vd_batch* b, const int32_t* rounds, const int32_t* answers, int32_t Ta,
+                          const int64_t* draw_base, const int32_t* slots);
 int vd_clamp_adam_step(vd_engine* e, float learning_rate);
 int vd_comm_unique_id(void* id_out);
 int vd_comm_init(vd_engine* e, const void* id, int32_t rank, int32_t world);

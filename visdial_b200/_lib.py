@@ -142,6 +142,7 @@ SIGNATURES = {
     "vd_dialog_end": [_H],
     "vd_dialog_open": [_H, C.c_int32, C.c_int32, C.c_int32, C.c_int32],
     "vd_dialog_join": [_H, _P(vd_batch), C.c_void_p, C.c_void_p],
+    "vd_dialog_join_rounds": [_H, _P(vd_batch), C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p],
     "vd_dialog_leave": [_H, C.c_void_p, C.c_int32],
     "vd_dialog_ask_beam_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.c_void_p, C.c_void_p, C.c_void_p],

@@ -14,10 +14,12 @@ from stdin and prints each answer.  One GPU only.
 With `-serve 1` it serves many conversations at once from a dialog pool of `-capacity` slots (Model.openDialogPool,
 DESIGN §20), reading JSON lines on stdin and writing JSON lines on stdout:
   in:  {"id": "u1", "image_id": 185565, "question": "is it sunny?"}   (the first line of an id joins it, with its image)
+       {"id": "u2", "image_id": 185565, "history": [["is it sunny?", "yes"]], "question": "any people?"}
+            (a first line may carry the rounds the conversation already had: it joins at round len(history); DESIGN §21)
        {"id": "u1", "leave": true}
   out: {"id", "round", "question", "answer", ...} for each answer; {"id", "error"} for a refused line (an unknown image, a
-       full pool, an unknown id).  A conversation that has had maxQuesCount answers is left, its last answer with
-       "done": true.
+       full pool, an unknown id, a malformed history, one of maxQuesCount rounds or more, or one for an open id).  A
+       conversation that has had maxQuesCount answers is left, its last answer with "done": true.
 The server reads every line available without blocking, applies its joins and leaves in arrival order, then asks every
 conversation with a pending question its oldest one, all in one device call (serve_step)."""
 from __future__ import annotations
@@ -38,18 +40,38 @@ def _image_index(dl, split: str) -> dict:
     return {image_id(x): i for i, x in enumerate(img)}
 
 
-def serve_step(lines, convs: dict, queues: dict, free: int, images) -> tuple:
+def _history_ok(h) -> bool:
+    """a join line's "history": a list of [question, answer] pairs, each text or a list of token ids"""
+    def turn(x):
+        return isinstance(x, str) or (isinstance(x, list) and all(isinstance(t, int) and not isinstance(t, bool) for t in x))
+    return isinstance(h, list) and all(isinstance(p, (list, tuple)) and len(p) == 2 and turn(p[0]) and turn(p[1]) for p in h)
+
+
+def serve_step(lines, convs: dict, queues: dict, free: int, images, max_rounds: int = 10) -> tuple:
     """One step of the serve loop, without the device.  lines: the JSON objects read since the last ask, in arrival order;
     convs: the open conversations' ids (each mapped to its slot; None for one joined in this step); queues: {id: [pending
-    question, ...]}; free: the free slots; images: the image ids conversations may join with.  Updates convs and queues and
-    returns (joins [(id, image_id)] new conversations to join, leaves [slot] the slots to free, errors [(id, message)],
-    asks [(id, question)]: each conversation with a pending question, with its oldest)."""
+    question, ...]}; free: the free slots; images: the image ids conversations may join with; max_rounds: maxQuesCount.
+    Updates convs and queues and returns (joins: the new conversations to join, (id, image_id), or (id, image_id,
+    history) for a join line with a "history" of earlier rounds; leaves [slot] the slots to free; errors [(id, message)];
+    asks [(id, question)]: each conversation with a pending question, with its oldest).  A line whose history is
+    malformed, has max_rounds rounds or more, or names an open id is refused and changes nothing."""
     joins, leaves, errors = [], [], []
     for obj in lines:
         cid = obj.get("id") if isinstance(obj, dict) else None
         if cid is None:
             errors.append((None, "a line needs an id"))
             continue
+        if "history" in obj:
+            h = obj["history"]
+            if cid in convs:
+                errors.append((cid, "a history only comes with a conversation's first line"))
+                continue
+            if not _history_ok(h):
+                errors.append((cid, "a history is a list of [question, answer] pairs"))
+                continue
+            if len(h) >= max_rounds:
+                errors.append((cid, "a history of %d rounds or more leaves nothing to ask" % max_rounds))
+                continue
         if obj.get("leave"):
             if cid not in convs:
                 errors.append((cid, "unknown id"))
@@ -74,7 +96,8 @@ def serve_step(lines, convs: dict, queues: dict, free: int, images) -> tuple:
                 continue
             free -= 1
             convs[cid] = None
-            joins.append((cid, obj["image_id"]))
+            joins.append((cid, obj["image_id"], [list(p) for p in obj["history"]]) if "history" in obj else
+                         (cid, obj["image_id"]))
         if obj.get("question") is not None:
             queues.setdefault(cid, []).append(obj["question"])
     asks = [(cid, q.pop(0)) for cid, q in queues.items() if q]
@@ -105,6 +128,7 @@ class _Lines:
 
 def serve(model, dl, split: str, index: dict, params: dict, capacity: int, out=sys.stdout):
     """The -serve loop: JSON lines on stdin, answers as JSON lines on `out`, until stdin ends and nothing is pending."""
+    from ._lib import VdError
     from .utils import idToWords
     pool = model.openDialogPool(dl, split, capacity, params)
     R = model.params["maxQuesCount"]
@@ -126,14 +150,23 @@ def serve(model, dl, split: str, index: dict, params: dict, capacity: int, out=s
                     objs.append(json.loads(line))
                 except ValueError:
                     objs.append({"id": None})
-            joins, leaves, errors, asks = serve_step(objs, convs, queues, free, index)
+            joins, leaves, errors, asks = serve_step(objs, convs, queues, free, index, R)
             for cid, msg in errors:
                 emit({"id": cid, "error": msg})
             if leaves:
                 pool.leave(leaves)
-            if joins:
-                for (cid, _), s in zip(joins, pool.join([index[img] for _, img in joins])):
+            fresh = [j for j in joins if len(j) == 2]
+            if fresh:
+                for (cid, _), s in zip(fresh, pool.join([index[img] for _, img in fresh])):
                     convs[cid] = s
+            for cid, img, history in (j for j in joins if len(j) == 3):    # joins at round len(history)
+                try:
+                    convs[cid] = pool.resume(index[img], history)
+                except (ValueError, VdError) as e:                          # a word outside the vocabulary, a bad token id
+                    del convs[cid]
+                    queues.pop(cid, None)
+                    emit({"id": cid, "error": str(e)})
+            asks = [(cid, q) for cid, q in asks if cid in convs]
             free = capacity - len(convs)
             if not asks:
                 continue

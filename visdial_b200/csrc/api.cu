@@ -384,6 +384,10 @@ int vd_dialog_open(vd_engine* h, int32_t capacity, int32_t Tq, int32_t hist_widt
 int vd_dialog_join(vd_engine* h, const vd_batch* b, const int64_t* draw_base, int32_t* slots) {
   VD_TRY({ ENG(h)->dialog_join(b, draw_base, slots); })
 }
+int vd_dialog_join_rounds(vd_engine* h, const vd_batch* b, const int32_t* rounds, const int32_t* answers, int32_t Ta,
+                          const int64_t* draw_base, const int32_t* slots) {
+  VD_TRY({ ENG(h)->dialog_join_rounds(b, rounds, answers, Ta, draw_base, slots); })
+}
 int vd_dialog_leave(vd_engine* h, const int32_t* slots, int32_t n) { VD_TRY({ ENG(h)->dialog_leave(slots, n); }) }
 int vd_dialog_ask_beam_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
                              int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length,

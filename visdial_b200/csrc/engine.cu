@@ -4,6 +4,7 @@
 #include <string.h>
 #include <math.h>
 #include <cmath>
+#include <algorithm>
 
 namespace vd {
 
@@ -993,7 +994,7 @@ void Engine::quiesce() {
 
 // The question and history LSTM pairs over `rows` rows of time-major ids ids_q (Tq, rows) / ids_h (Th, rows).  img_rows
 // (rows, IE): the image embedding MaskTime joins to the question LSTM's input (img_in_q), else null.
-void Engine::encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows) {
+void Engine::encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows, bool ques_pair) {
   const int E = cfg.E, H = cfg.H;
   const int64_t N = rows;
   const DropCfg d05 = dropcfg(0.5f), dnone = dropcfg(0.f);
@@ -1012,6 +1013,7 @@ void Engine::encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows) 
     if (serial_pairs()) { join_side(); lstm_pair_forward(hist1, hist2, main_chain); }
     else { lstm_pair_forward(hist1, hist2, side_chain); back_to_main(); }
   }
+  if (!ques_pair) { join_side(); return; }
   // question branch
   xq = arena.get<float>(N * Tq * E);
   embed_rows(cx, xq, Wp(0), ids_q, N * Tq, E, embdrop ? d05 : dnone, SITE_QEMBED);
@@ -2166,12 +2168,23 @@ void Engine::dialog_join(const vd_batch* b, const int64_t* draw_base, int32_t* s
     if (dses.round[s] < 0) slots.push_back(s);
   VD_REQUIRE((int)slots.size() == B, VD_E_STATE, "the pool has fewer free slots than dialogs to join");
   const vd_batch eb = encoder_only(b);
+  dialog_join_images(&eb, slots.data());
+  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  for (int i = 0; i < B; ++i) {
+    dses.round[slots[i]] = 0;
+    dses.draw_base[slots[i]] = draw_base ? draw_base[i] : 0;
+    slots_host[i] = slots[i];
+  }
+}
+
+const int32_t* Engine::dialog_join_images(const vd_batch* b, const int32_t* slots) {
+  const int B = b->B;
   quiesce();
-  stage_batch(&eb);
+  stage_batch(b);
   refresh_shadows();
   wait_img();
   int32_t* sd = arena.get<int32_t>(B);
-  VD_CUDA_CHECK(cudaMemcpyAsync(sd, slots.data(), (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(sd, slots, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
   if (cfg.useHist)                   // round 0 <- the caption row
     hist_append(cx, (int32_t*)dses.hist.p, B, cfg.R, dses.W, -1, db.hist, db.Th, nullptr, 0, nullptr, 0, 0, 0, false, sd);
   float* img = (float*)dses.img.p;
@@ -2187,11 +2200,151 @@ void Engine::dialog_join(const vd_batch* b, const int64_t* draw_base, int32_t* s
     scatter_rows(cx, img, db.img, sd, B, cfg.F);
   }
   release_img();
-  VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  return sd;
+}
+
+// b's dialogs resumed in slots[i] at rounds[i] (DESIGN §21).  A conversation's cached state at round r depends only on its
+// caption, image and rounds 0..r-1 (§17's causality), so it comes from one eval-mode pass over the P = sum r_i rows
+// (slot s_i, round j < r_i).  The rows are packed time-major by round over the dialogs sorted by r descending: round j's
+// rows are then a prefix block of the dialogs still going, so one dialog-LSTM step per round runs on a contiguous prefix
+// and continues the previous step's rows.
+void Engine::dialog_join_rounds(const vd_batch* b, const int32_t* rounds, const int32_t* answers, int Ta, const int64_t* draw_base,
+                                const int32_t* slots) {
+  VD_REQUIRE(dses.open, VD_E_STATE, "no dialog session: call vd_dialog_open");
+  VD_REQUIRE(dses.valid, VD_E_STATE, "the weights or the math mode changed since the session was opened");
+  VD_REQUIRE(b != nullptr && b->B > 0 && b->Tq > 0 && b->ques_fwd, VD_E_SHAPE, "resume batch with B, Tq > 0 and its questions");
+  VD_REQUIRE(b->Tq <= dses.Tq, VD_E_SHAPE, "the batch's question width is above the session's");
+  VD_REQUIRE(rounds != nullptr && slots != nullptr, VD_E_BADARG, "null rounds or slots");
+  VD_REQUIRE(Ta >= 1, VD_E_BADARG, "answer width Ta >= 1");
+  if (cfg.useHist) {
+    VD_REQUIRE(b->hist && b->Th > 0, VD_E_SHAPE, "a history encoder's join needs the batch's round-0 history row");
+    VD_REQUIRE(dses.W >= b->Th, VD_E_BADARG, "hist_width >= the batch's Th");
+    VD_REQUIRE(answers != nullptr, VD_E_BADARG, "a history encoder's resume needs the answers");
+  }
+  const int B = b->B, R = cfg.R, H = cfg.H, Tq = b->Tq, Tw = dses.Tq, W = dses.W, V = cfg.V;
+  std::vector<char> seen(dses.C, 0);
   for (int i = 0; i < B; ++i) {
-    dses.round[slots[i]] = 0;
+    VD_REQUIRE(slots[i] >= 0 && slots[i] < dses.C, VD_E_BADARG, "a slot id outside [0, capacity)");
+    VD_REQUIRE(!seen[slots[i]], VD_E_BADARG, "a slot named twice");
+    seen[slots[i]] = 1;
+    VD_REQUIRE(rounds[i] >= 0 && rounds[i] < R, VD_E_BADARG, "a round outside [0, maxQuesCount - 1]");
+    if (draw_base) VD_REQUIRE(draw_base[i] >= 0, VD_E_BADARG, "draw_base >= 0");
+  }
+  std::vector<int32_t> ques((size_t)B * R * Tq);       // checked and packed on the host
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  if (b->on_device)
+    VD_CUDA_CHECK(cudaMemcpy(ques.data(), b->ques_fwd, ques.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  else
+    std::copy_n(b->ques_fwd, ques.size(), ques.data());
+  for (int i = 0; i < B; ++i)
+    for (int j = 0; j < rounds[i]; ++j) {
+      for (int t = 0; t < Tq; ++t) {
+        const int32_t v = ques[((size_t)i * R + j) * Tq + t];
+        VD_REQUIRE(v >= 0 && v <= V, VD_E_BADARG, "a question token outside [0, vocabSize]");
+      }
+      if (cfg.useHist)
+        for (int t = 0; t < Ta; ++t) {
+          const int32_t v = answers[((size_t)i * R + j) * Ta + t];
+          VD_REQUIRE(v >= 0 && v <= V, VD_E_BADARG, "an answer token outside [0, vocabSize]");
+        }
+    }
+  for (int i = 0; i < B; ++i) VD_REQUIRE(dses.round[slots[i]] < 0, VD_E_STATE, "an occupied slot");
+
+  // sorted dialog i is batch row order[i]; round j has cnt[j] rows, from packed row row0[j] on
+  std::vector<int> order(B);
+  for (int i = 0; i < B; ++i) order[i] = i;
+  std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return rounds[x] > rounds[y]; });
+  const int rmax = rounds[order[0]];
+  std::vector<int32_t> cnt(R, 0), row0(R, 0);
+  for (int i = 0; i < B; ++i)
+    for (int j = 0; j < rounds[i]; ++j) ++cnt[j];
+  for (int j = 1; j < R; ++j) row0[j] = row0[j - 1] + cnt[j - 1];
+  const int64_t P = row0[R - 1] + cnt[R - 1];
+  // upload: per packed row slot, round and question (right-aligned into the session's width); per sorted dialog slot and
+  // round; row0; per sorted dialog its answers
+  const int64_t o_round = P, o_q = 2 * P, o_sd = o_q + P * Tw, o_sr = o_sd + B, o_row0 = o_sr + B, o_ans = o_row0 + R;
+  std::vector<int32_t> up((size_t)(o_ans + (cfg.useHist ? (int64_t)B * R * Ta : 0)), 0);
+  for (int i = 0; i < B; ++i) {
+    const int d = order[i];
+    up[o_sd + i] = slots[d];
+    up[o_sr + i] = rounds[d];
+    for (int j = 0; j < rounds[d]; ++j) {
+      const int64_t p = row0[j] + i;
+      up[p] = slots[d];
+      up[o_round + p] = j;
+      std::copy_n(&ques[((size_t)d * R + j) * Tq], Tq, &up[o_q + p * Tw + Tw - Tq]);
+    }
+    if (cfg.useHist) std::copy_n(answers + (size_t)d * R * Ta, (size_t)R * Ta, &up[o_ans + (int64_t)i * R * Ta]);
+  }
+  std::copy(row0.begin(), row0.end(), &up[o_row0]);
+
+  const int saved_training = training;
+  training = 0;
+  try {
+    const vd_batch eb = encoder_only(b);
+    dialog_join_images(&eb, slots);
+    int32_t* u = arena.get<int32_t>((int64_t)up.size());
+    VD_CUDA_CHECK(cudaMemcpyAsync(u, up.data(), up.size() * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+    const int32_t *slot_rows = u, *round_rows = u + o_round;
+    if (cfg.useHist)                 // rows 1..r_i by §17's rule, before the gather reads them
+      hist_prefill(cx, (int32_t*)dses.hist.p, B, R, W, u + o_sd, u + o_sr, u + o_row0, u + o_q, Tw, u + o_ans, Ta, V,
+                   dses.max_ans_len, cfg.fam_lf);
+    if (P > 0) {
+      // hre / hrea's dialog LSTM reads q; mn caches facts only; late fusion re-reads the whole row at each ask
+      const bool need_h = cfg.useHist && !cfg.fam_lf, need_q = cfg.fam_hre;
+      DialogGather g;
+      g.n = P; g.R = R; g.slot = slot_rows; g.round = round_rows;
+      g.q = u + o_q; g.Tq = Tw; g.ques = (int32_t*)dses.ques.p; g.ids_q = ids_q = arena.get<int32_t>(P * Tw);
+      ids_h = nullptr;
+      if (need_h) { g.hist = (const int32_t*)dses.hist.p; g.W = W; g.ids_h = ids_h = arena.get<int32_t>(P * W); }
+      float* img = nullptr;
+      if (need_q && cfg.img_in_q) {
+        g.img = (const float*)dses.img.p; g.img_cols = dses.img_cols; g.img_out = img = arena.get<float>(P * dses.img_cols);
+      }
+      {
+        const double moved = 8.0 * P * (need_q && cfg.img_in_q ? dses.img_cols : 0) + 4.0 * P * (3 * Tw + (need_h ? W : 0));
+        LaunchCtx::Scope sc(&cx, "dialog_gather", 0.0, moved);
+        dialog_gather(cx, g);
+      }
+      if (need_h) {
+        encoder_lstms(P, Tw, W, img, need_q);
+        const float* h3 = hist2.h_last();
+        float* facts = (float*)dses.facts.p;
+        const int64_t fpitch = (int64_t)R * H;
+        if (cfg.fam_mn) {
+          dialog_cache_write(cx, facts, nullptr, h3, nullptr, P, R, H, 0, slot_rows, round_rows);
+        } else {
+          const float* q3 = ques2.h_last();
+          float* j = arena.get<float>(P * 2 * H);
+          if (cfg.hre_att) {         // every row's fact and score are cached before any attention reads them
+            sq = arena.get<float>(P); sh = arena.get<float>(P);
+            int sq_w = seg("att.q.weight"), sh_w = seg("att.h.weight");
+            rowdot_fwd(cx, sq, q3, Wp(sq_w), Wp(sq_w + 1), P, H);
+            rowdot_fwd(cx, sh, h3, Wp(sh_w), Wp(sh_w + 1), P, H);
+            dialog_cache_write(cx, facts, (float*)dses.shc.p, h3, sh, P, R, H, 0, slot_rows, round_rows);
+            hre_join_fwd(q3, facts, sq, (const float*)dses.shc.p, fpitch, (int)P, 0, 1, j, slot_rows, round_rows);
+          } else {
+            hre_join_fwd(q3, h3, nullptr, nullptr, fpitch, (int)P, 0, 1, j);
+          }
+          // round j's step continues the first cnt[j] rows of step j-1 (step 0 without state, as a full forward's first
+          // step); each step's (h, c) go to its rows' slots, so a slot keeps the state of its last round r_i - 1
+          float* out = arena.get<float>(P * H);
+          const float *hp = nullptr, *cp = nullptr;
+          for (int t = 0; t < rmax; ++t) {
+            hre_dialog_fwd(j + (int64_t)row0[t] * 2 * H, cnt[t], 1, hp, cp, out + (int64_t)row0[t] * H);
+            hp = dialog.h_last(); cp = dialog.c_last();
+            dialog_cache_write(cx, nullptr, nullptr, nullptr, nullptr, cnt[t], R, H, 0, slot_rows + row0[t], nullptr,
+                               (float*)dses.state[0].p, (float*)dses.state[1].p, hp, cp);
+          }
+        }
+      }
+    }
+    VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  } catch (...) { training = saved_training; throw; }
+  training = saved_training;
+  for (int i = 0; i < B; ++i) {
+    dses.round[slots[i]] = rounds[i];
     dses.draw_base[slots[i]] = draw_base ? draw_base[i] : 0;
-    slots_host[i] = slots[i];
   }
 }
 

@@ -286,7 +286,8 @@ struct Engine {
 
   void quiesce();                    // drains what an abandoned call left pending, resets the arena; no forward is current
   void encoder_forward(const vd_batch* b);
-  void encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows);   // the question and history LSTM pairs
+  // the question and history LSTM pairs (ques_pair false: the history pair only, for a resume whose cache needs no q)
+  void encoder_lstms(int64_t rows, int Tq, int Th, const float* img_rows, bool ques_pair = true);
   void encoder_backward(const float* dEnc);
   // blocks shared by several encoder graphs
   float *qi_join = nullptr, *qi_proj = nullptr;                 // mn-ques-im-hist: [q | fc7] and tanh(Linear(.))
@@ -387,6 +388,14 @@ struct Engine {
   void dialog_open(int C, int Tq, int W, int max_ans_len);
   // joins b's B dialogs into the lowest free slots (their ids into slots_host); draw_base (B) or null (all 0)
   void dialog_join(const vd_batch* b, const int64_t* draw_base, int32_t* slots_host);
+  // a join's device work, not synchronised: stages b, writes the captions into round 0 of slots (B, host; uploaded here,
+  // the device copy returned) and the image products into their slots
+  const int32_t* dialog_join_images(const vd_batch* b, const int32_t* slots);
+  // b's B dialogs into the free slots slots[i] at rounds[i] (DESIGN §21): the history, question cache, facts, sh and
+  // dialog-LSTM state a join at round 0 followed by rounds[i] asks with answers (B, R, Ta) (HOST) would have left, from
+  // one encoder pass over the sum of rounds[i] rows
+  void dialog_join_rounds(const vd_batch* b, const int32_t* rounds, const int32_t* answers, int Ta, const int64_t* draw_base,
+                          const int32_t* slots);
   void dialog_leave(const int32_t* slots, int64_t n);
   void dialog_begin(const vd_batch* b, int W, int max_ans_len);
   void dialog_end();

@@ -210,6 +210,13 @@ void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, in
 void hist_append(LaunchCtx& cx, int32_t* hist, int64_t B, int R, int W, int r, const int32_t* src, int src_w, const int32_t* ans,
                  int64_t ans_ld, const int32_t* ans_len, int ans_max, int end_token, int max_ans_len, bool concat,
                  const int32_t* slot = nullptr, const int32_t* round = nullptr);
+// a dialog pool's resume (Engine::dialog_join_rounds): CTA i writes rows 1..rounds[i] of dialog slot[i] of hist, in order,
+// by hist_append's rule from row 0 on.  Round j's question is row row0[j] + i of q (rows, src_w) (rows packed time-major,
+// round j's a prefix block of the dialogs still going); its answer is row (i, j) of ans (n, R, Ta), left-aligned, pads not
+// words, cut at end_token (hist_append's ans_len-null form).
+void hist_prefill(LaunchCtx& cx, int32_t* hist, int64_t n, int R, int W, const int32_t* slot, const int32_t* rounds,
+                  const int32_t* row0, const int32_t* q, int src_w, const int32_t* ans, int Ta, int end_token, int max_ans_len,
+                  bool concat);
 
 // ---- optimiser (model.lua:96-99, optim_updates.lua:62-91) ------------------------------------------
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1,

@@ -356,6 +356,44 @@ __global__ void k_repeat_rows(float* __restrict__ dst, const float* __restrict__
   dst[i] = src[(n / R) * lds + c];
 }
 
+// The history rule (DESIGN §17), the one place it lives on the device: row `prev` (W, right-aligned) -> the next row `out`
+// from the question row q (src_w, right-aligned) and the answer tokens a, of which the first a_len[0] - 2 (a_len null:
+// a_max) are read, cut at end_token, pads skipped, at most max_ans_len kept.  Every thread of the CTA calls it; a_s holds
+// max_ans_len words.  The CTA synchronises once inside, before the writes; a caller that reads `out` next syncs again.
+__device__ __forceinline__ void hist_next_row(const int32_t* __restrict__ prev, int32_t* __restrict__ out, int W,
+                                              const int32_t* __restrict__ q, int src_w, const int32_t* __restrict__ a,
+                                              const int32_t* __restrict__ a_len, int a_max, int end_token, int max_ans_len,
+                                              int concat, int32_t* a_s, int* s_len) {
+  if (threadIdx.x == 0) {
+    int lp = 0, lq = 0, la = 0;                            // rows are pads then words: count the words from the right
+    while (lp < W && prev[W - 1 - lp] != 0) ++lp;
+    while (lq < src_w && q[src_w - 1 - lq] != 0) ++lq;
+    if (lp > 0 && lq > 0) {
+      const int n = a_len ? max(a_len[0] - 2, 0) : a_max;
+      for (int i = 0; i < n && la < max_ans_len; ++i) {
+        const int32_t t = a[i];
+        if (t == end_token) break;
+        if (t != 0) a_s[la++] = t;                          // a pad a stale beam column carried is not a word
+      }
+    }
+    s_len[0] = lp; s_len[1] = lq; s_len[2] = la;
+  }
+  __syncthreads();
+  const int lp = s_len[0], lq = s_len[1], la = s_len[2];
+  const int keep = concat ? lp + 1 : 0;                    // row r ++ <END>
+  const int total = lp == 0 ? 0 : keep + lq + la;
+  for (int j = threadIdx.x; j < W; j += blockDim.x) {
+    const int s = total - W + j;                           // position in the unbounded row; the rightmost W are kept
+    int32_t t = 0;
+    if (s >= 0) {
+      if (s < keep) t = s < lp ? prev[W - lp + s] : end_token;
+      else if (s < keep + lq) t = q[src_w - lq + (s - keep)];
+      else t = a_s[s - keep - lq];
+    }
+    out[j] = t;
+  }
+}
+
 // the dialog loop's history rows (hist_append in kernels.cuh), one CTA per dialog, or per asked row of a dialog pool
 // (slot non-null: row b writes dialog slot[b], at round round[b] unless r < 0)
 __global__ void k_hist_append(int32_t* __restrict__ hist, int R, int W, int r, const int32_t* __restrict__ src, int src_w,
@@ -378,37 +416,24 @@ __global__ void k_hist_append(int32_t* __restrict__ hist, int R, int W, int r, c
     }
     return;
   }
-  const int32_t* prev = rows + (int64_t)r * W;
-  const int32_t* q = src + (d * R + r) * src_w;
-  if (threadIdx.x == 0) {
-    int lp = 0, lq = 0, la = 0;                            // rows are pads then words: count the words from the right
-    while (lp < W && prev[W - 1 - lp] != 0) ++lp;
-    while (lq < src_w && q[src_w - 1 - lq] != 0) ++lq;
-    if (lp > 0 && lq > 0) {
-      const int32_t* a = ans + b * ans_ld;
-      const int n = ans_len ? max(ans_len[b] - 2, 0) : ans_max;
-      for (int i = 0; i < n && la < max_ans_len; ++i) {
-        const int32_t t = a[i];
-        if (t == end_token) break;
-        if (t != 0) a_s[la++] = t;                          // a pad a stale beam column carried is not a word
-      }
-    }
-    s_len[0] = lp; s_len[1] = lq; s_len[2] = la;
-  }
-  __syncthreads();
-  const int lp = s_len[0], lq = s_len[1], la = s_len[2];
-  const int keep = concat ? lp + 1 : 0;                    // row r ++ <END>
-  const int total = lp == 0 ? 0 : keep + lq + la;
-  int32_t* out = rows + (int64_t)(r + 1) * W;
-  for (int j = threadIdx.x; j < W; j += blockDim.x) {
-    const int s = total - W + j;                           // position in the unbounded row; the rightmost W are kept
-    int32_t t = 0;
-    if (s >= 0) {
-      if (s < keep) t = s < lp ? prev[W - lp + s] : end_token;
-      else if (s < keep + lq) t = q[src_w - lq + (s - keep)];
-      else t = a_s[s - keep - lq];
-    }
-    out[j] = t;
+  hist_next_row(rows + (int64_t)r * W, rows + (int64_t)(r + 1) * W, W, src + (d * R + r) * src_w, src_w, ans + b * ans_ld,
+                ans_len ? ans_len + b : nullptr, ans_max, end_token, max_ans_len, concat, a_s, s_len);
+}
+
+// a resumed conversation's history rows 1..rounds[i] (hist_prefill in kernels.cuh): CTA i builds them in order, each from
+// the one before, with the rule above
+__global__ void k_hist_prefill(int32_t* __restrict__ hist, int R, int W, const int32_t* __restrict__ slot,
+                               const int32_t* __restrict__ rounds, const int32_t* __restrict__ row0, const int32_t* __restrict__ q,
+                               int src_w, const int32_t* __restrict__ ans, int Ta, int end_token, int max_ans_len, int concat) {
+  extern __shared__ int32_t a_s[];
+  __shared__ int s_len[3];
+  const int64_t i = blockIdx.x;
+  int32_t* rows = hist + (int64_t)slot[i] * R * W;
+  const int r = rounds[i];
+  for (int j = 0; j < r; ++j) {
+    hist_next_row(rows + (int64_t)j * W, rows + (int64_t)(j + 1) * W, W, q + (row0[j] + i) * src_w, src_w,
+                  ans + (i * R + j) * Ta, nullptr, Ta, end_token, max_ans_len, concat, a_s, s_len);
+    __syncthreads();                                       // row j + 1 is the next row's `prev`; a_s and s_len are reused
   }
 }
 __global__ void k_sum_repeated_rows(float* __restrict__ dst, const float* __restrict__ src, int64_t B, int R, int64_t cols) {
@@ -1499,6 +1524,16 @@ void hist_append(LaunchCtx& cx, int32_t* hist, int64_t B, int R, int W, int r, c
   k_hist_append<<<(unsigned)B, 128, (size_t)cap * sizeof(int32_t), cx.stream>>>(hist, R, W, r, src, src_w, ans, ans_ld, ans_len,
                                                                                ans_max, end_token, cap, concat ? 1 : 0, slot, round);
   check_launch(cx, "k_hist_append");
+}
+void hist_prefill(LaunchCtx& cx, int32_t* hist, int64_t n, int R, int W, const int32_t* slot, const int32_t* rounds,
+                  const int32_t* row0, const int32_t* q, int src_w, const int32_t* ans, int Ta, int end_token, int max_ans_len,
+                  bool concat) {
+  VD_REQUIRE(W >= src_w && src_w > 0 && Ta >= 1 && max_ans_len >= 1, VD_E_BADARG, "hist_prefill: widths");
+  if (n <= 0) return;
+  const int cap = std::min(max_ans_len, Ta);
+  k_hist_prefill<<<(unsigned)n, 128, (size_t)cap * sizeof(int32_t), cx.stream>>>(hist, R, W, slot, rounds, row0, q, src_w, ans, Ta,
+                                                                              end_token, cap, concat ? 1 : 0);
+  check_launch(cx, "k_hist_prefill");
 }
 void sum_repeated_rows(LaunchCtx& cx, float* dst, const float* src, int64_t B, int R, int64_t cols) {
   L1D(k_sum_repeated_rows, B * cols, dst, src, B, R, cols);

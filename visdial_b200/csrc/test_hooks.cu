@@ -88,6 +88,12 @@ const Entry TABLE[] = {
        hist_append(e->cx, I32(0), I[0], IN(1), IN(2), IN(3), CI32(1), IN(4), CI32(2), I[5], CI32(3), IN(6), IN(7), IN(8), I[9] != 0,
                    CI32(4), CI32(5));
      }},
+    // hist, slot, rounds, row0, q, ans; ints n, R, W, src_w, Ta, end_token, max_ans_len, concat
+    {"hist_prefill", 6, 8, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       hist_prefill(e->cx, I32(0), I[0], IN(1), IN(2), CI32(1), CI32(2), CI32(3), CI32(4), IN(3), CI32(5), IN(4), IN(5), IN(6),
+                    I[7] != 0);
+     }},
     // ---- SAN: ints as the launcher's, the dropout site last; reals p
     {"san_expand_dropout", 2, 5, 1,
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {

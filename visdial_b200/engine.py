@@ -583,6 +583,30 @@ class Engine:
                                       slots.ctypes.data))
         return slots
 
+    def dialog_join_rounds(self, batch: Batch, rounds, answers, slots, draw_base=None):
+        """Resume the batch's B dialogs in the free slots `slots` (B) at `rounds` (B) (vd_dialog_join_rounds, DESIGN §21):
+        their questions 0..r-1 are the batch's ques_fwd rows, their answers `answers` (B, maxQuesCount, Ta) left-aligned
+        word ids (None for the encoders without history); draw_base as dialog_join's."""
+        B, R = int(batch.c.B), self.params["maxQuesCount"]
+        r = np.ascontiguousarray(rounds, dtype=np.int32).ravel()
+        s = np.ascontiguousarray(slots, dtype=np.int32).ravel()
+        if r.shape != (B,) or s.shape != (B,):
+            raise ValueError("one round and one slot per joined dialog")
+        a, Ta = None, 1
+        if answers is not None:
+            a = np.ascontiguousarray(answers, dtype=np.int32)
+            if a.ndim != 3 or a.shape[:2] != (B, R):
+                raise ValueError("answers must be (B, maxQuesCount, Ta)")
+            Ta = a.shape[2]
+        base = None
+        if draw_base is not None:
+            base = np.ascontiguousarray(draw_base, dtype=np.int64)
+            if base.shape != (B,):
+                raise ValueError("one draw base per joined dialog")
+        self._enc_rows = None
+        check(self.lib.vd_dialog_join_rounds(self.h, C.byref(batch.c), r.ctypes.data, a.ctypes.data if a is not None else None,
+                                             int(Ta), base.ctypes.data if base is not None else None, s.ctypes.data))
+
     def dialog_leave(self, slots):
         """Free the slots (vd_dialog_leave)."""
         s = np.ascontiguousarray(slots, dtype=np.int32).ravel()

@@ -390,12 +390,49 @@ class Model:
         return ck
 
 
+def history_answer(row, end: int, length=None) -> list:
+    """The words of an answer as the history rule reads them (DESIGN §17).  With `length`: a beam hypothesis (<START>
+    first) of that many tokens, its words between <START> and <END>, none when length is 0.  Without: the words before
+    the first <END> of `row` (a sample row without its <START> column, a pool row or a corpus answer).  Pads are not
+    words."""
+    if length is not None:
+        return [int(t) for t in row[1:max(int(length) - 1, 1)] if t != 0] if length > 0 else []
+    out = []
+    for t in row:
+        if int(t) == end:
+            break
+        if int(t) != 0:
+            out.append(int(t))
+    return out
+
+
+def transcript_arrays(transcripts, R: int, width: int):
+    """What vd_dialog_join_rounds reads for conversations given as transcripts, each a pair (question rows (width,)
+    right-aligned, answer word lists) of equal length r < R: rounds (B), ques_fwd (B, R, width) and answers (B, R, Ta)
+    left-aligned and zero-padded, Ta the longest answer (at least 1)."""
+    B = len(transcripts)
+    rounds = np.asarray([len(q) for q, _ in transcripts], np.int32)
+    if any(len(q) != len(a) for q, a in transcripts) or (rounds >= R).any():
+        raise ValueError("a transcript has one answer per question and fewer than maxQuesCount rounds")
+    Ta = max([1] + [len(w) for _, a in transcripts for w in a])
+    ques = np.zeros((B, R, width), np.int32)
+    ans = np.zeros((B, R, Ta), np.int32)
+    for i, (q, a) in enumerate(transcripts):
+        for j in range(len(q)):
+            ques[i, j] = q[j]
+            ans[i, j, :len(a[j])] = a[j]
+    return rounds, ques, ans
+
+
 class DialogPool:
     """Conversations about the dataset's images that join, are asked and leave on their own, each at its own round
     (vd_dialog_open / join / ask_*_slots / leave, DESIGN §20).  A conversation is one dataset dialog's image and caption,
     asked its questions one at a time; the history rule, the widths and the answers are generateAnswers' /
     retrieveAnswers' with `history = "generated"`, and a sampled conversation draws as generateAnswers does for that
-    dialog.  Fed the same questions, a conversation's answers do not depend on the others asked with it."""
+    dialog.  Fed the same questions, a conversation's answers do not depend on the others asked with it.
+    The pool keeps each conversation's transcript (its dialog index, draw base, questions and the answers it was given or
+    gave), so that conversations can join at any round (join with rounds, resume; DESIGN §21) and a pool can be reopened
+    with every conversation in its own slot after a weight or math-mode change (reopen)."""
 
     def __init__(self, model, dataloader, dtype, params, capacity=None):
         self.model, self.dl, self.eng, self.dtype = model, dataloader, model.engine, dtype
@@ -416,28 +453,90 @@ class DialogPool:
             else 0
         self.rowOffset = 0                   # sampling: a slot draws as global round draw_base + its round
         self.words = getattr(dataloader, "ind2word", None)
+        self.convs = {}                      # slot -> {"ind", "base", "ques": [rows], "ans": [word lists]}
         if self.disc:
             self.pool = dataloader.answerPool(dtype)
             self.eng.answer_pool_encode(self.pool)
+        self.capacity = capacity
         if capacity is not None:
             self.eng.dialog_open(int(capacity), self.width, self.histWidth, self.maxAnsLen)
 
-    def _batch(self, inds) -> dict:
-        """what a join reads of dialogs `inds`: images and round-0 history rows; questions are asked at the full width"""
+    def _batch(self, inds, gt=False) -> dict:
+        """what a join reads of dialogs `inds`: images and round-0 history rows; questions are asked at the full width.
+        gt: also the dialogs' own questions (right-aligned into the full width) and answers (corpus rows)."""
         batch = self.dl.getIndexData(np.asarray(inds, dtype=np.int64), self.model.params, self.dtype)
         host = {"ques_fwd": np.zeros((len(inds), self.R, self.width), np.int32)}
         for k in ("hist", "img_feat"):
             if k in batch:
                 host[k] = np.ascontiguousarray(batch[k])
+        if gt:
+            q = np.asarray(batch["ques_fwd"])
+            host["ques_fwd"][:, :, self.width - q.shape[2]:] = q
+            host["answer_out"] = np.asarray(batch["answer_out"])
         return host
 
-    def join(self, inds) -> list:
-        """Joins dialogs `inds` (0-based, of the split) as new conversations at round 0; returns their slots.  Raises
-        VdError (VD_E_STATE) and joins none when fewer slots are free."""
-        inds = [int(i) for i in inds]
+    def _free_slots(self, n: int) -> list:
+        from ._lib import VD_E_STATE, VdError
+        free = [s for s, r in enumerate(self.eng.dialog_slots()) if r < 0]
+        if len(free) < n:
+            raise VdError(VD_E_STATE, "the pool has fewer free slots than dialogs to join")
+        return free[:n]
+
+    def _join_rounds(self, inds, transcripts, slots, bases):
+        """conversations on dialogs `inds`' images and captions, each resumed from its transcript in its slot"""
         host = self._batch(inds)
+        rounds, host["ques_fwd"], ans = transcript_arrays(transcripts, self.R, self.width)
+        self.eng.dialog_join_rounds(Batch(host), rounds, ans if self.histWidth else None, slots, bases)
+        for i, s in enumerate(slots):
+            q, a = transcripts[i]
+            self.convs[int(s)] = {"ind": int(inds[i]), "base": int(bases[i]), "ques": list(q), "ans": list(a)}
+
+    def join(self, inds, rounds=None) -> list:
+        """Joins dialogs `inds` (0-based, of the split) as new conversations; returns their slots.  At round 0 by default;
+        with `rounds` (one per dialog, each below maxQuesCount) dialog i continues from round rounds[i] on its own
+        questions and ground-truth answers of the earlier rounds, in one device pass.  Raises VdError (VD_E_STATE) and
+        joins none when fewer slots are free."""
+        inds = [int(i) for i in inds]
         base = np.asarray([(self.offset + i) * self.R for i in inds], np.int64)
-        return self.eng.dialog_join(Batch(host), base).tolist()
+        if rounds is None:
+            slots = self.eng.dialog_join(Batch(self._batch(inds)), base).tolist()
+            for i, s, b in zip(inds, slots, base):
+                self.convs[s] = {"ind": i, "base": int(b), "ques": [], "ans": []}
+            return slots
+        if len(rounds) != len(inds):
+            raise ValueError("one round per joined dialog")
+        gt = self._batch(inds, gt=True)
+        transcripts = [([gt["ques_fwd"][d, j] for j in range(int(r))],
+                        [history_answer(gt["answer_out"][d, j], self.end) for j in range(int(r))])
+                       for d, r in enumerate(rounds)]
+        slots = self._free_slots(len(inds))
+        self._join_rounds(inds, transcripts, slots, base)
+        return slots
+
+    def resume(self, ind: int, transcript) -> int:
+        """A conversation about dialog `ind`'s image and caption that already had the rounds of `transcript`, a list of
+        (question, answer) pairs, each text (utils.question_ids / answer_ids) or token ids, fewer than maxQuesCount: it
+        joins at round len(transcript) with them as its history.  Returns its slot."""
+        from .utils import answer_ids, question_ids
+        q = [question_ids(x, self.dl.word2ind, self.width) for x, _ in transcript]
+        a = [[int(t) for t in answer_ids(y, self.dl.word2ind, self.maxAnsLen) if t] for _, y in transcript]
+        slot = self._free_slots(1)
+        self._join_rounds([int(ind)], [(q, a)], slot, [(self.offset + int(ind)) * self.R])
+        return slot[0]
+
+    def reopen(self):
+        """After Model.load / set_parameters / a math-mode change, which leave the engine's pool stale: reopens it at the
+        same capacity and rejoins every live conversation in its own slot, at its round, with its draw base, in one
+        device pass (a disc model's answer pool is encoded again).  A conversation that has had maxQuesCount rounds has
+        nothing left to ask and is not rejoined."""
+        if self.disc:
+            self.eng.answer_pool_encode(self.pool)
+        self.eng.dialog_open(int(self.capacity), self.width, self.histWidth, self.maxAnsLen)
+        live = sorted(s for s, c in self.convs.items() if len(c["ques"]) < self.R)
+        self.convs = {s: c for s, c in self.convs.items() if s in live}
+        if live:
+            c = [self.convs[s] for s in live]
+            self._join_rounds([x["ind"] for x in c], [(x["ques"], x["ans"]) for x in c], live, [x["base"] for x in c])
 
     def ask(self, questions: dict) -> dict:
         """Asks each slot of `questions` ({slot: question}, text or token ids) its next round, all in one device call.
@@ -453,6 +552,7 @@ class DialogPool:
         out = []
         if self.disc:
             index, score = self.eng.dialog_ask_pool_slots(slots, q, self.topK)
+            given = [history_answer(self.pool[index[b, 0]], self.end) for b in range(len(q))]
             for b in range(len(q)):
                 a = [int(t) for t in self.pool[index[b, 0]] if t != 0]
                 out.append({"question": [int(t) for t in q[b] if t], "answer": a, "index": int(index[b, 0]),
@@ -462,11 +562,17 @@ class DialogPool:
         elif self.sampleWords:
             ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature, self.seed,
                                                       self.rowOffset)
+            given = [history_answer(ans[b, 1:], self.end) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
         else:
             ans, length, score = self.eng.dialog_ask_beam_slots(slots, q, self.beamSize, self.beamLen, self.start, self.end)
+            given = [history_answer(ans[b], self.end, length[b]) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist(), "score": float(score[b]),
                     "length": int(length[b])} if length[b] > 0 else None for b in range(len(q))]
+        for s, row, a in zip(slots, q, given):            # the transcript a later resume or reopen replays
+            if s in self.convs:
+                self.convs[s]["ques"].append(np.array(row, np.int32))
+                self.convs[s]["ans"].append(a)
         if text:
             for e in out:
                 if e is not None:
@@ -475,6 +581,8 @@ class DialogPool:
 
     def leave(self, slots):
         self.eng.dialog_leave([int(s) for s in slots])
+        for s in slots:
+            self.convs.pop(int(s), None)
 
     def round(self, slot: int) -> int:
         """The slot's next round to be asked (R once it has had maxQuesCount), -1 when free."""
@@ -501,6 +609,8 @@ class DialogSession(DialogPool):
         self.image_ids = [_image_id(img[self.offset + int(i)]) if img is not None else self.offset + int(i) for i in self.inds]
         host = self._batch(self.inds)
         self.eng.dialog_begin(Batch(host), self.histWidth, self.maxAnsLen)
+        self.capacity = len(self.inds)
+        self.convs = {b: {"ind": int(i), "base": b * self.R, "ques": [], "ans": []} for b, i in enumerate(self.inds)}
         self.caption = host["hist"][:, 0] if "hist" in host else None      # round 0's history row
 
     @property

@@ -54,6 +54,26 @@ def question_ids(question, word2ind: dict, width: int) -> np.ndarray:
     return row
 
 
+def answer_ids(answer, word2ind: dict, width: int) -> np.ndarray:
+    """One answer row as the corpus's `ans` holds it: (width,) int32, left-aligned, zero-padded.  `answer` is text,
+    split by question_words' rules without the trailing '?' (words missing from word2ind become UNK; unverified against
+    nltk), or a list of token ids (pads dropped); either is cut to its first `width` tokens, as prepro.py cuts answers to
+    maxAnsLen."""
+    if isinstance(answer, str):
+        unk = word2ind.get("UNK")
+        ids = []
+        for w in question_words(answer)[:-1]:
+            if w not in word2ind and unk is None:
+                raise ValueError("%r is not in the vocabulary, which has no UNK" % w)
+            ids.append(word2ind.get(w, unk))
+    else:
+        ids = [int(t) for t in answer if int(t) != 0]
+    ids = ids[:width]
+    row = np.zeros(width, np.int32)
+    row[:len(ids)] = ids
+    return row
+
+
 def image_id(x):
     """dataloader.lua:42-44: `tonumber(string.match(name, '000%d+'))` on the json image names; ints pass through."""
     if isinstance(x, (int, np.integer)):
