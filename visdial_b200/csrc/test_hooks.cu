@@ -1,6 +1,7 @@
 // vd_test_kernel: the kernels.cuh launchers of pointwise.cu, lstm16.cu's streaming helpers, enc_lstm.cu's persistent
 // encoder LSTM pair and gemm_tc.cu's fused vocabulary projections, called by name on caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory
-// attribute and route are the engine's own.  The table below is the whole surface: name, pointer / int / real counts, and the call.
+// attribute and route are the engine's own; and whole SeqLSTM runs through the engine's own LSTM driver (seq_lstm, seq_lstm_pair).
+// The table below is the whole surface: name, pointer / int / real counts, and the call.
 //   dropout:  p = reals[0], the site an int; the factors are Engine::dropcfg(p)'s (identity unless training == 1).
 //   sampling: SampleCfg from ints (seed, step, row_offset, row_stride) and reals (temperature).
 // Pointers may be null where the launcher accepts null (mask ids, gt, inv_scale, ...).
@@ -24,6 +25,88 @@ struct Entry {
 #define CH16(i) (static_cast<const __half*>(P[i]))
 #define IN(i) ((int)I[i])
 #define DROP(k) e->dropcfg((float)X[k])
+
+// ---- whole SeqLSTM runs: the engine's own route decision and driver on caller buffers.  The run's state lives in the arena
+// and is copied out before the arena is rewound to where the call found it.
+struct ArenaRewind {
+  Arena& a;
+  Arena::Mark m;
+  ~ArenaRewind() { a.rewind(m); }
+};
+
+void copy_out(Engine* e, void* dst, const void* src, size_t bytes) {
+  if (dst && src) VD_CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, e->cx.stream));
+}
+
+void route_out(Engine* e, int32_t* dst, const LstmRoute* rt, int n) {
+  if (!dst) return;
+  int32_t v[10];
+  for (int k = 0; k < n; ++k) {
+    const int32_t r[5] = {(int32_t)rt[k].fwd, (int32_t)rt[k].bwd, rt[k].table_grad, rt[k].wave_fwd, rt[k].wave_bwd};
+    memcpy(v + 5 * k, r, sizeof(r));
+  }
+  VD_CUDA_CHECK(cudaMemcpyAsync(dst, v, 5 * n * sizeof(int32_t), cudaMemcpyHostToDevice, e->cx.stream));
+  VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+}
+
+// a SeqLSTM on weight segment wseg (bias = wseg + 1), D and H from the segment's (D + H, 4H) shape
+LstmRun test_run(Engine* e, int wseg, int T, int64_t R, const float* x, const int32_t* gather, const int32_t* mask) {
+  VD_REQUIRE(wseg >= 0 && wseg + 1 < (int)e->lay.segs.size() && e->lay.segs[wseg].init == VD_INIT_LSTM_W, VD_E_BADARG,
+             "seq_lstm: wseg is not an LSTM weight segment");
+  VD_REQUIRE(T >= 1 && R >= 1 && !(x && gather), VD_E_BADARG, "seq_lstm: T, R, or both x and gather");
+  const Seg& s = e->lay.segs[wseg];
+  LstmRun r;
+  r.T = T; r.R = R; r.H = (int)(s.cols / 4); r.D = (int)(s.rows - s.cols / 4); r.wseg = wseg;
+  r.x = x; r.gather = gather; r.mask = mask;
+  return r;
+}
+
+void seq_lstm_hook(Engine* e, void* const* P, const int64_t* I) {
+  e->refresh_shadows();
+  ArenaRewind rw{e->arena, e->arena.mark()};
+  const bool train = I[3] != 0;
+  VD_REQUIRE(P[0] || P[1], VD_E_BADARG, "seq_lstm: x or gather");
+  VD_REQUIRE(train || !(P[5] || P[6] || P[7] || P[10] || P[11] || P[12] || P[13] || P[14] || P[15] || P[16]), VD_E_BADARG,
+             "seq_lstm: a forward-only run has no saved gates and no gradients");
+  LstmRun r = test_run(e, IN(0), IN(1), I[2], CF(0), CI32(1), CI32(2));
+  r.h0 = CF(3); r.c0 = CF(4);
+  r.demb_out = F(15);
+  e->lstm_forward(r, train);
+  if (train) e->lstm_backward(r, CF(5), CF(6), CF(7), F(12), F(13), F(14));
+  const bool f16 = r.route.fwd == LstmPath::Opt16;
+  const size_t RH = (size_t)r.R * r.H, TRH = (size_t)r.T * RH, el = f16 ? sizeof(__half) : sizeof(float);
+  if (train) {
+    copy_out(e, P[8], f16 ? (const void*)r.h16 : r.h, TRH * el);
+    copy_out(e, P[9], r.c, TRH * sizeof(float));
+    copy_out(e, P[10], f16 ? (const void*)r.gates16 : r.gates, 4 * TRH * el);
+    copy_out(e, P[11], f16 ? (const void*)r.da16 : r.da, 4 * TRH * el);
+    copy_out(e, P[16], r.scale2, 2 * sizeof(float));
+  } else {
+    copy_out(e, P[8], r.h_last(), RH * sizeof(float));
+    copy_out(e, P[9], r.c_last(), RH * sizeof(float));
+  }
+  route_out(e, I32(17), &r.route, 1);
+  VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+}
+
+void seq_lstm_pair_hook(Engine* e, void* const* P, const int64_t* I) {
+  e->refresh_shadows();
+  ArenaRewind rw{e->arena, e->arena.mark()};
+  VD_REQUIRE(P[0], VD_E_BADARG, "seq_lstm_pair: x");
+  LstmRun l[2] = {test_run(e, IN(0), IN(2), I[3], CF(0), nullptr, CI32(1)), test_run(e, IN(1), IN(2), I[3], nullptr, nullptr, CI32(1))};
+  VD_REQUIRE(l[1].D == l[0].H, VD_E_BADARG, "seq_lstm_pair: layer 2's input is layer 1's h");
+  e->route_lstm_pair(l[0], l[1]);
+  e->lstm_pair_forward(l[0], l[1], e->main_chain);
+  e->lstm_pair_backward(l[0], l[1], CF(2), CF(3), CF(4), CF(5), F(10), e->main_chain);
+  const size_t TRH = (size_t)l[0].T * l[0].R * l[0].H * sizeof(float);
+  copy_out(e, P[6], l[0].h, TRH);
+  copy_out(e, P[7], l[0].c, TRH);
+  copy_out(e, P[8], l[1].h, TRH);
+  copy_out(e, P[9], l[1].c, TRH);
+  const LstmRoute rt[2] = {l[0].route, l[1].route};
+  route_out(e, I32(11), rt, 2);
+  VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+}
 
 const Entry TABLE[] = {
     // ---- history attention: (ptrs), ints B, R, H
@@ -296,6 +379,17 @@ const Entry TABLE[] = {
        VD_CUDA_CHECK(cudaMemcpyAsync(P[0], &n, sizeof(n), cudaMemcpyHostToDevice, e->cx.stream));
        VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
      }},
+    // ---- whole SeqLSTM runs (Engine::lstm_forward / lstm_backward, routed by route_lstm) on weight segment wseg.  ptrs x (T R, D)
+    // or null, gather ids (T R) or null, mask ids (T R), h0, c0, dh_all (T R, H), dh_last, dc_last (R, H); outputs h, c, gates, da,
+    // dx, dh0, dc0, demb_out ((V+1, E), overwritten; null: the embedding gradient goes to dW), scale, info; any of them may be
+    // null.  ints wseg, T, R, train.  train = 1: a saved run and its BPTT, h / c / gates / da of all T steps (Opt16: its fp16 h,
+    // gates and da, da times s; scale {s, 1/s}); train = 0: a run without saved state, h / c of the last step.  info int32
+    // {fwd path, bwd path, table_grad, wave_fwd, wave_bwd} (LstmPath values).  Weight and bias gradients accumulate into dW.
+    {"seq_lstm", 18, 4, 0, [](Engine* e, void* const* P, const int64_t* I, const double*) { seq_lstm_hook(e, P, I); }},
+    // two stacked runs routed by route_lstm_pair on the main chain's streams, forward and BPTT.  ptrs x (T R, D1), mask,
+    // dh_last2, dc_last2, dh_last1, dc_last1 (each may be null); outputs h1, c1, h2, c2 (T R, H), dx1 (T R, D1), info (two
+    // layers' five ints as seq_lstm's).  ints wseg1, wseg2, T, R
+    {"seq_lstm_pair", 12, 4, 0, [](Engine* e, void* const* P, const int64_t* I, const double*) { seq_lstm_pair_hook(e, P, I); }},
     // ---- answer-pool top-k (DESIGN §18), routed as the engine routes it: ptrs Q, E, topv, topi; ints rows, ldq, m, H, k
     {"answer_pool_topk", 4, 5, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
