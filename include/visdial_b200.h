@@ -189,6 +189,22 @@ int vd_gen_decoder_step(vd_engine* e, int32_t rows, const int32_t* tokens_host, 
  * and beam_len >= 2. */
 int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
                        int32_t* answer_host, int32_t* length_host, double* score_host);
+/* Diverse beam search (Vijayakumar et al., arXiv:1610.02424; DESIGN §22): vd_gen_beam_search's search with its beam_size
+ * = k columns split into `groups` G groups of w = k / G, group g owning columns [g*w, (g+1)*w).  Each step fills the
+ * groups in order; a candidate of group g is penalised by diversity * (the number of columns of groups < g filled at this
+ * step with its token) (Hamming diversity; unfilled columns and finished hypotheses do not count, so end_token never
+ * is).  Each explored column of group g takes its w best classes under the penalty; <END> candidates compete for the
+ * group's best finished hypothesis by their unpenalised score, the others fill the group's columns by their penalised
+ * score, and a column stores the unpenalised score, so every reported score is a log-probability.  At step 1 only each
+ * group's first column is explored.  G = 1 is vd_gen_beam_search bit for bit; diversity 0 makes every group a search of
+ * width w.  The decoder work is that of vd_gen_beam_search at beam_size k.
+ * answer_host (N, G, beam_len), length_host (N, G), score_host (N, G): each group's best finished hypothesis as
+ * vd_gen_beam_search's (length 0: none).  A round's pick (what a dialog's history takes) is the best of its G by (score
+ * desc, group asc) among groups of length > 0.
+ * Refusals as vd_gen_beam_search's, and VD_E_BADARG unless groups >= 1 divides beam_size and diversity is finite and >= 0. */
+int vd_gen_diverse_beam_search(vd_engine* e, int32_t beam_size, int32_t groups, float diversity, int32_t beam_len,
+                               int32_t start_token, int32_t end_token, int32_t* answer_host, int32_t* length_host,
+                               double* score_host);
 /* Model:generateAnswers' sampling (model.lua:581-602, sampleWords = 1) for EVERY round of the last vd_encoder_forward (N =
  * B * maxQuesCount rows), entirely on the device, the decoder fed its own samples (gen.lua:63-68).  One synchronisation, at
  * the end.  Draw rule (Gumbel-max over x / temperature, counter-based Philox; see DESIGN §14): the token of step t of row r
@@ -220,6 +236,13 @@ int vd_gen_dialog_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size
 int vd_gen_dialog_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
                          float temperature, uint64_t seed, int64_t row_offset, int32_t hist_width, int32_t max_ans_len,
                          int32_t* answer_host, float* logp_host, int32_t* hist_host);
+/* vd_gen_dialog_beam_search's loop with vd_gen_diverse_beam_search's search: round r's history row takes the round's
+ * pick.  Outputs (N, G, beam_len), (N, G), (N, G) for the N = B * maxQuesCount rounds; hist_host and refusals as
+ * vd_gen_dialog_beam_search's and vd_gen_diverse_beam_search's. */
+int vd_gen_dialog_diverse_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size, int32_t groups, float diversity,
+                                      int32_t beam_len, int32_t start_token, int32_t end_token, int32_t hist_width,
+                                      int32_t max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
+                                      int32_t* hist_host);
 
 /* ---- answer-pool retrieval: disc models answer (DESIGN §18) --------------------------------------------------------
  * A disc model answers a question by retrieval: it scores every answer of the split's answer pool (opt_list_<split>, every
@@ -318,6 +341,12 @@ int vd_dialog_ask_sample_slots(vd_engine* e, const int32_t* slots, int32_t n, co
                                int32_t* answer, float* logp);
 int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t k,
                              int32_t* index, float* score);
+/* vd_dialog_ask_beam_slots with vd_gen_diverse_beam_search's search (DESIGN §22): answer (n, G, beam_len), length (n, G),
+ * score (n, G) in row order; each slot's history takes its row's pick.  A vd_dialog_begin session is the pool of slots
+ * 0..B-1.  Refusals, before any state changes, as vd_dialog_ask_beam_slots' and vd_gen_diverse_beam_search's. */
+int vd_dialog_ask_diverse_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                                int32_t groups, float diversity, int32_t beam_len, int32_t start_token, int32_t end_token,
+                                int32_t* answer, int32_t* length, double* score);
 int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
 int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
 

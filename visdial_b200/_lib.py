@@ -120,11 +120,15 @@ SIGNATURES = {
                     C.c_int64],
     "vd_set_lazy_decout": [_H, C.c_int32],
     "vd_gen_beam_search": [_H, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_gen_diverse_beam_search": [_H, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                   C.c_void_p, C.c_void_p],
     "vd_gen_sample": [_H, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p],
     "vd_gen_dialog_beam_search": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gen_dialog_sample": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_int32,
                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_gen_dialog_diverse_beam_search": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32,
+                                          C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_answer_pool_encode": [_H, C.c_void_p, C.c_int64, C.c_int32],
     "vd_answer_pool": [_H, _P(C.c_void_p), _P(C.c_int64)],
     "vd_answer_pool_retrieve": [_H, _P(vd_batch), C.c_int32, C.c_void_p, C.c_void_p],
@@ -149,6 +153,8 @@ SIGNATURES = {
     "vd_dialog_ask_sample_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                    C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p],
     "vd_dialog_ask_pool_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p],
+    "vd_dialog_ask_diverse_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
+                                    C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_dialog_slots": [_H, C.c_void_p, _P(C.c_int32)],
     "vd_dialog_slot_history": [_H, C.c_void_p, C.c_int32, C.c_void_p],
     "vd_gemm_atb16": [_H, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,

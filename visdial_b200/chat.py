@@ -3,7 +3,8 @@
 Reads the model and data as `generate` does and opens a dialog session (Model.openDialogs) on the chosen images of
 `-split`: their features and captions; each question is answered before the next is asked, and the model's own answers
 become the history the next question is answered with.  Gen models answer with generate's beam search (`-beamSize`,
-`-beamLen`) or, with `-sampleWords 1`, by sampling; disc models with the best answer of the split's answer pool.
+`-beamLen`; diverse with `-beamGroups` > 1 and `-diversity`, DESIGN §22) or, with `-sampleWords 1`, by sampling; disc
+models with the best answer of the split's answer pool.
 
 With `-questions file.json` ({image_id: [question, ...]}, at most maxQuesCount per image; a question is text or a list of
 token ids) every image of the file (or of `-imageIds`) is asked its questions, round by round, and
@@ -17,7 +18,8 @@ DESIGN §20), reading JSON lines on stdin and writing JSON lines on stdout:
        {"id": "u2", "image_id": 185565, "history": [["is it sunny?", "yes"]], "question": "any people?"}
             (a first line may carry the rounds the conversation already had: it joins at round len(history); DESIGN §21)
        {"id": "u1", "leave": true}
-  out: {"id", "round", "question", "answer", ...} for each answer; {"id", "error"} for a refused line (an unknown image, a
+  out: {"id", "round", "question", "answer", ...} for each answer (with -beamGroups > 1 also "alternatives": every group's
+       finished answer as {"answer", "score"}, best first, the first being "answer"); {"id", "error"} for a refused line (an unknown image, a
        full pool, an unknown id, a malformed history, one of maxQuesCount rounds or more, or one for an open id).  A
        conversation that has had maxQuesCount answers is left, its last answer with "done": true.
 The server reads every line available without blocking, applies its joins and leaves in arrival order, then asks every
@@ -129,6 +131,7 @@ class _Lines:
 def serve(model, dl, split: str, index: dict, params: dict, capacity: int, out=sys.stdout):
     """The -serve loop: JSON lines on stdin, answers as JSON lines on `out`, until stdin ends and nothing is pending."""
     from ._lib import VdError
+    from .model import ranked_groups
     from .utils import idToWords
     pool = model.openDialogPool(dl, split, capacity, params)
     R = model.params["maxQuesCount"]
@@ -180,6 +183,9 @@ def serve(model, dl, split: str, index: dict, params: dict, capacity: int, out=s
                         "answer": idToWords(e["answer"], dl.ind2word).strip() if e else None}
                 if e and "score" in e:
                     line["score"] = e["score"]
+                if e and "groups" in e:
+                    line["alternatives"] = [{"answer": idToWords(g["answer"], dl.ind2word).strip(), "score": g["score"]}
+                                            for g in ranked_groups(e)]
                 if r == R:
                     line["done"] = True
                     done.append(cid)
@@ -220,7 +226,7 @@ def main(opt: dict, rank: int = 0, world: int = 1):
         missing = [i for i in ids if i not in index]
         if missing:
             raise SystemExit("image ids not in split %s: %s" % (split, missing))
-        params = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature")}
+        params = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "beamGroups", "diversity")}
         R = model.params["maxQuesCount"]
         if opt["serve"]:
             serve(model, dl, split, index, params, opt["capacity"])
@@ -254,7 +260,7 @@ def main(opt: dict, rank: int = 0, world: int = 1):
                                        "answer": idToWords(e["answer"], dl.ind2word)})
         session.close()
         path = os.path.join(opt["resultPath"], "results.json")
-        cli.write_json(path, {"opts": opt, "data": [{"image_id": i, "dialog": d} for i, d in zip(ids, dialogs)]})
+        cli.write_json(path, {"opts": cli.written_opts(opt), "data": [{"image_id": i, "dialog": d} for i, d in zip(ids, dialogs)]})
         print("Writing the results to " + path, flush=True)
     finally:
         dl.close()

@@ -4,6 +4,7 @@ given alone flips its default), the checkpoint hand-over, the engine set-up and 
 from __future__ import annotations
 
 import json
+import math
 import os
 import socket
 import sys
@@ -79,14 +80,20 @@ GENERATE_OPTIONS = [
     ("backend", "cudnn", "nn|cudnn (accepted, no effect)"),
     ("dialogsPerCall", 1, "Dialogs per encoder forward and device search call (1 = the reference's per-dialog loop)"),
 ]
-# the generate command's table: generate.lua's options above, and which history each round is answered with
+# diverse beam search (DESIGN §22): several distinct answers per question from one search
+DIVERSE_OPTIONS = [
+    ("beamGroups", 1, "Diverse beam search: groups the beam is split into (1 = plain beam search; must divide beamSize)"),
+    ("diversity", 0.5, "Diverse beam search: penalty per earlier group's column that chose the same token"),
+]
+# the generate command's table: generate.lua's options above, diverse beam search, and which history each round is
+# answered with
 HISTORY_MODES = ("gt", "generated")
-GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + [
+GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + [
     ("history", "gt", "History each round is answered with: gt (the dataset's) | generated (the dialog's own answers)"),
 ]
 
-# the chat command: generate's options, and which images are talked about with which questions
-CHAT_OPTIONS = GENERATE_OPTIONS + [
+# the chat command: generate's options, diverse beam search, and which images are talked about with which questions
+CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + [
     ("split", "val", "Split the images and captions come from"),
     ("imageIds", "", "Comma-separated COCO image ids of the split (default: the -questions file's, else its first image)"),
     ("questions", "", "JSON {image_id: [question, ...]}: ask these and write results.json; else read stdin, one per line"),
@@ -144,6 +151,11 @@ def parse(options, argv=None, prog=None) -> dict:
         fail("-math is one of %s" % "|".join(MATH_MODES))
     if "history" in opt and opt["history"] not in HISTORY_MODES:
         fail("-history is one of %s" % "|".join(HISTORY_MODES))
+    if "beamGroups" in opt:
+        if opt["beamGroups"] < 1 or opt["beamSize"] % opt["beamGroups"] != 0:
+            fail("-beamGroups must be at least 1 and divide -beamSize")
+        if not math.isfinite(opt["diversity"]) or opt["diversity"] < 0:
+            fail("-diversity must be finite and >= 0")
     if opt["gpus"] < 1:
         fail("-gpus must be at least 1")
     if opt["gpuid"] < 0:
@@ -162,6 +174,13 @@ def train_opts(argv=None, now=None, options=TRAIN_OPTIONS, prog="python -m visdi
     if "att" in opt["encoder"] and opt["inputImg"] == "data/data_img.h5":           # :62-65 (conv features)
         opt["inputImg"] = "data/data_img_pool5.h5"
     return opt
+
+
+def written_opts(opt: dict) -> dict:
+    """The options a results.json records: the diverse beam search options only when they change the search
+    (-beamGroups > 1), so that a plain beam search writes the file it wrote before they existed."""
+    plain = opt.get("beamGroups", 1) == 1
+    return {k: v for k, v in opt.items() if not (plain and k in ("beamGroups", "diversity"))}
 
 
 def model_params(opt: dict) -> dict:

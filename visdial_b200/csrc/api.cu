@@ -271,7 +271,15 @@ int vd_gen_decoder_step(vd_engine* h, int32_t rows, const int32_t* tokens_host, 
 
 int vd_gen_beam_search(vd_engine* h, int32_t beam_size, int32_t beam_len, int32_t start_token, int32_t end_token,
                        int32_t* answer_host, int32_t* length_host, double* score_host) {
-  VD_TRY({ ENG(h)->gen_beam_search(beam_size, beam_len, start_token, end_token, answer_host, length_host, score_host); })
+  VD_TRY({ ENG(h)->gen_beam_search(beam_size, 1, 0.f, beam_len, start_token, end_token, answer_host, length_host, score_host); })
+}
+
+int vd_gen_diverse_beam_search(vd_engine* h, int32_t beam_size, int32_t groups, float diversity, int32_t beam_len,
+                               int32_t start_token, int32_t end_token, int32_t* answer_host, int32_t* length_host,
+                               double* score_host) {
+  VD_TRY({
+    ENG(h)->gen_beam_search(beam_size, groups, diversity, beam_len, start_token, end_token, answer_host, length_host, score_host);
+  })
 }
 
 int vd_gen_sample(vd_engine* h, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
@@ -282,8 +290,16 @@ int vd_gen_sample(vd_engine* h, int32_t beam_len, int32_t start_token, float tem
 int vd_gen_dialog_beam_search(vd_engine* h, const vd_batch* b, int32_t beam_size, int32_t beam_len, int32_t start_token,
                               int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
                               int32_t* length_host, double* score_host, int32_t* hist_host) {
-  VD_TRY({ ENG(h)->gen_dialog_beam_search(b, beam_size, beam_len, start_token, end_token, hist_width, max_ans_len, answer_host,
-                                          length_host, score_host, hist_host); })
+  VD_TRY({ ENG(h)->gen_dialog_beam_search(b, beam_size, 1, 0.f, beam_len, start_token, end_token, hist_width, max_ans_len,
+                                          answer_host, length_host, score_host, hist_host); })
+}
+
+int vd_gen_dialog_diverse_beam_search(vd_engine* h, const vd_batch* b, int32_t beam_size, int32_t groups, float diversity,
+                                      int32_t beam_len, int32_t start_token, int32_t end_token, int32_t hist_width,
+                                      int32_t max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
+                                      int32_t* hist_host) {
+  VD_TRY({ ENG(h)->gen_dialog_beam_search(b, beam_size, groups, diversity, beam_len, start_token, end_token, hist_width,
+                                          max_ans_len, answer_host, length_host, score_host, hist_host); })
 }
 
 int vd_gen_dialog_sample(vd_engine* h, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
@@ -320,7 +336,8 @@ int vd_dialog_ask_beam(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t be
   VD_TRY({
     Engine* e = ENG(h);
     const std::vector<int32_t> s = e->dialog_all_slots();
-    e->dialog_ask_beam(s.data(), (int64_t)s.size(), ques, Tq, beam_size, beam_len, start_token, end_token, answer, length, score);
+    e->dialog_ask_beam(s.data(), (int64_t)s.size(), ques, Tq, beam_size, 1, 0.f, beam_len, start_token, end_token, answer, length,
+                       score);
   })
 }
 int vd_dialog_ask_sample(vd_engine* h, const int32_t* ques, int32_t Tq, int32_t beam_len, int32_t start_token, int32_t end_token,
@@ -392,7 +409,15 @@ int vd_dialog_leave(vd_engine* h, const int32_t* slots, int32_t n) { VD_TRY({ EN
 int vd_dialog_ask_beam_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
                              int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length,
                              double* score) {
-  VD_TRY({ ENG(h)->dialog_ask_beam(slots, n, ques, Tq, beam_size, beam_len, start_token, end_token, answer, length, score); })
+  VD_TRY({ ENG(h)->dialog_ask_beam(slots, n, ques, Tq, beam_size, 1, 0.f, beam_len, start_token, end_token, answer, length, score); })
+}
+int vd_dialog_ask_diverse_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                                int32_t groups, float diversity, int32_t beam_len, int32_t start_token, int32_t end_token,
+                                int32_t* answer, int32_t* length, double* score) {
+  VD_TRY({
+    ENG(h)->dialog_ask_beam(slots, n, ques, Tq, beam_size, groups, diversity, beam_len, start_token, end_token, answer, length,
+                            score);
+  })
 }
 int vd_dialog_ask_sample_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_len,
                                int32_t start_token, int32_t end_token, float temperature, uint64_t seed, int64_t row_offset,

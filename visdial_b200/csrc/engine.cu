@@ -1737,29 +1737,37 @@ void Engine::gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float
   lstm_forward(gstep2, true);
 }
 
-// Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once.
-void Engine::gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
-                             double* score_host) {
+// Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once; with G > 1
+// groups, diverse beam search (DESIGN §22).
+void Engine::gen_beam_search(int k, int G, float lam, int L, int start_token, int end_token, int32_t* answer_host,
+                             int32_t* length_host, double* score_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_search needs the gen decoder after encoder_forward");
-  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  check_beam_args(k, G, lam, L);
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
-  const int64_t N = db.N;
-  const BeamResult res = beam_search_rows(N, 1, 0, k, L, start_token, end_token);
-  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  const int64_t NG = db.N * G;
+  const BeamResult res = beam_search_rows(db.N, 1, 0, k, G, lam, L, start_token, end_token);
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.gans, (size_t)NG * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.glen, (size_t)NG * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.gscore, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+void Engine::check_beam_args(int k, int G, float lam, int L) const {
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  VD_REQUIRE(G >= 1 && k % G == 0, VD_E_BADARG, "groups >= 1 and a divisor of beam_size");
+  VD_REQUIRE(std::isfinite(lam) && lam >= 0.f, VD_E_BADARG, "diversity finite and >= 0");
 }
 
 // The search itself, enqueued on cx.stream, for n rounds whose start state is row i * stride + off of the last encoder
 // forward (i < n; stride 1, off 0: every round): row i*k + j is hypothesis j of round i.  Every step runs on device-resident
 // tokens and parents: the state gather, the decoder step of gen_decoder_step_logits, the fused log-softmax + top-k and the
-// candidate merge, which writes the next step's tokens and parents.  Returns each round's best finished hypothesis in the
-// arena (n rows), valid until the next encoder forward.
-Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int L, int start_token,
-                                            int end_token) {
+// candidate merge, which writes the next step's tokens and parents.  The merge fills G groups of k / G columns in order,
+// penalising the tokens earlier groups chose (DESIGN §22); its top-k input is the same k per row at any G.  Returns each
+// group's best finished hypothesis and each round's pick in the arena, valid until the next encoder forward.
+Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int G, float lam, int L,
+                                            int start_token, int end_token) {
   forward_connect();
   const int H = cfg.H;
   const int64_t N = n, rows = N * k;
@@ -1775,12 +1783,16 @@ Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t o
   int32_t* parent = arena.get<int32_t>(rows);
   float* tv = arena.get<float>(rows * k);
   int32_t* ti = arena.get<int32_t>(rows * k);
-  int32_t* ans = arena.get<int32_t>(N * L);
-  int32_t* ans_len = arena.get<int32_t>(N);
-  double* ans_score = arena.get<double>(N);
-  VD_CUDA_CHECK(cudaMemsetAsync(ans, 0, (size_t)N * L * sizeof(int32_t), cx.stream));
-  VD_CUDA_CHECK(cudaMemsetAsync(ans_len, 0, (size_t)N * sizeof(int32_t), cx.stream));
-  VD_CUDA_CHECK(cudaMemsetAsync(ans_score, 0, (size_t)N * sizeof(double), cx.stream));
+  int32_t* ans = arena.get<int32_t>(N * G * L);
+  int32_t* ans_len = arena.get<int32_t>(N * G);
+  double* ans_score = arena.get<double>(N * G);
+  VD_CUDA_CHECK(cudaMemsetAsync(ans, 0, (size_t)N * G * L * sizeof(int32_t), cx.stream));
+  VD_CUDA_CHECK(cudaMemsetAsync(ans_len, 0, (size_t)N * G * sizeof(int32_t), cx.stream));
+  VD_CUDA_CHECK(cudaMemsetAsync(ans_score, 0, (size_t)N * G * sizeof(double), cx.stream));
+  // G > 1: the last step's merge also writes each round's pick
+  BeamResult res = {ans, ans_len, ans_score, ans, ans_len, ans_score};
+  if (G > 1) { res.ans = arena.get<int32_t>(N * L); res.len = arena.get<int32_t>(N); res.score = arena.get<double>(N); }
+  int32_t* pick_ans = G > 1 ? res.ans : nullptr;
   // model.lua:478-503: h = {layer-1 h at Tq, encOut}, c = {layer-1 c, layer-2 c}, each round's row repeated k times.  Encoders
   // without .rnnLayers feed explicit zero rows, not "no initial state": the first step's kernels differ between the two.
   const float* init[4] = {gen_h0[0], gen_h0[1], gen_c0[0], gen_c0[1]};
@@ -1802,10 +1814,12 @@ Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t o
     gen_decoder_step_logits(rows, tok, h, c);
     logsoftmax_topk_rows(cx, gstep_logp, tok, rows, cfg.V, k, tv, ti);
     const int a = (stp - 1) & 1;
-    beam_merge(cx, N, stp, k, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, ans, ans_len,
-               ans_score);
+    // the top-k lists, the scores and beams in and out
+    LaunchCtx::Scope sc(&cx, "beam_merge", 0.0, 8.0 * rows * k + 16.0 * rows + 8.0 * rows * (stp + 1));
+    beam_merge(cx, N, stp, k, G, lam, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, ans,
+               ans_len, ans_score, pick_ans, pick_ans ? res.len : nullptr, pick_ans ? res.score : nullptr);
   }
-  return {ans, ans_len, ans_score};
+  return res;
 }
 
 // Model:generateAnswers' sampling (model.lua:581-602) for all N rounds of the last encoder forward at once, on the device.
@@ -1946,28 +1960,29 @@ static void scatter_round(cudaStream_t s, void* dst, const void* src, size_t byt
                                   cudaMemcpyDeviceToDevice, s));
 }
 
-void Engine::gen_dialog_beam_search(const vd_batch* b, int k, int L, int start_token, int end_token, int W, int max_ans_len,
-                                    int32_t* answer_host, int32_t* length_host, double* score_host, int32_t* hist_host) {
+void Engine::gen_dialog_beam_search(const vd_batch* b, int k, int G, float lam, int L, int start_token, int end_token, int W,
+                                    int max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
+                                    int32_t* hist_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_beam_search needs the gen decoder");
-  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  check_beam_args(k, G, lam, L);
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
   const int R = cfg.R;
-  const int64_t B = b->B, N = B * R;
-  int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)N * L * sizeof(int32_t));
-  int32_t* len = (int32_t*)dialog_out[1].ensure((size_t)N * sizeof(int32_t));
-  double* score = (double*)dialog_out[2].ensure((size_t)N * sizeof(double));
+  const int64_t B = b->B, NG = B * R * G;
+  int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)NG * L * sizeof(int32_t));
+  int32_t* len = (int32_t*)dialog_out[1].ensure((size_t)NG * sizeof(int32_t));
+  double* score = (double*)dialog_out[2].ensure((size_t)NG * sizeof(double));
   gen_dialog(b, W, max_ans_len, [&](int r) {
-    const BeamResult res = beam_search_rows(B, R, r, k, L, start_token, end_token);
-    scatter_round(cx.stream, ans, res.ans, (size_t)L * sizeof(int32_t), R, r, B);
-    scatter_round(cx.stream, len, res.len, sizeof(int32_t), R, r, B);
-    scatter_round(cx.stream, score, res.score, sizeof(double), R, r, B);
-    // the tokens between <START> and the hypothesis' <END>
+    const BeamResult res = beam_search_rows(B, R, r, k, G, lam, L, start_token, end_token);
+    scatter_round(cx.stream, ans, res.gans, (size_t)G * L * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, len, res.glen, (size_t)G * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, score, res.gscore, (size_t)G * sizeof(double), R, r, B);
+    // the pick's tokens between <START> and the hypothesis' <END>
     return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
   }, hist_host);
-  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)N * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, len, (size_t)N * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, score, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)NG * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(length_host, len, (size_t)NG * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+  VD_CUDA_CHECK(cudaMemcpyAsync(score_host, score, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
@@ -2520,19 +2535,20 @@ static void run_ask(Engine* e, const int32_t* slots, int64_t n, const int32_t* q
   for (int64_t i = 0; i < n; ++i) e->dses.round[slots[i]] += 1;
 }
 
-void Engine::dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int L, int start_token,
-                             int end_token, int32_t* answer_host, int32_t* length_host, double* score_host) {
+void Engine::dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int G, float lam, int L,
+                             int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a beam-search ask needs the gen decoder");
-  VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
+  check_beam_args(k, G, lam, L);
   VD_REQUIRE(start_token >= 1 && start_token <= cfg.V && end_token >= 1 && end_token <= cfg.V, VD_E_BADARG,
              "start_token and end_token in [1, vocabSize]");
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   dialog_check_ask(slots, n, ques_host, Tq);
   run_ask(this, slots, n, ques_host, Tq, 0, [&](const AskRows&) {
-    const BeamResult res = beam_search_rows(n, 1, 0, k, L, start_token, end_token);
-    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)n * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-    VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.len, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
-    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.score, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+    const BeamResult res = beam_search_rows(n, 1, 0, k, G, lam, L, start_token, end_token);
+    const size_t nG = (size_t)n * G;
+    VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.gans, nG * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.glen, nG * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
+    VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.gscore, nG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
     return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
   });
 }

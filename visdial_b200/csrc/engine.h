@@ -323,11 +323,16 @@ struct Engine {
   void gen_decoder_step(int64_t rows, const int32_t* tokens_host, const float* const* h_prev, const float* const* c_prev);
   // its core on device-resident tokens, up to the vocabulary projection: gstep_logp holds the LOGITS on return
   void gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
-  // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device
-  void gen_beam_search(int k, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
-  // its search on n rounds whose start state is row i * stride + off of the last encoder forward; results in the arena
-  struct BeamResult { int32_t* ans; int32_t* len; double* score; };     // (n, L), (n), (n)
-  BeamResult beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int L, int start_token, int end_token);
+  // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device; G groups of
+  // k / G with diversity lam (DESIGN §22; G = 1: the reference's search).  Outputs (N, G, L), (N, G), (N, G).
+  void gen_beam_search(int k, int G, float lam, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
+                       double* score_host);
+  void check_beam_args(int k, int G, float lam, int L) const;
+  // its search on n rounds whose start state is row i * stride + off of the last encoder forward; results in the arena:
+  // the pick (n, L), (n), (n) (the best group's answer) and every group's (n, G, L), (n, G), (n, G); G = 1: the same arrays
+  struct BeamResult { int32_t* ans; int32_t* len; double* score; int32_t* gans; int32_t* glen; double* gscore; };
+  BeamResult beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int G, float lam, int L, int start_token,
+                              int end_token);
   // the decoder step up to the second LSTM layer (gstep1 / gstep2 hold the new state on return)
   void gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // Model:generateAnswers' sampling for every round of the last encoder forward, entirely on the device
@@ -351,8 +356,9 @@ struct Engine {
   };
   GrowBuf dialog_hist, dialog_out[4];   // (B, R, W) history; answers, lengths, scores / log-probabilities of all rounds
   void gen_dialog(const vd_batch* b, int W, int max_ans_len, const std::function<DialogAnswers(int)>& search, int32_t* hist_host);
-  void gen_dialog_beam_search(const vd_batch* b, int k, int L, int start_token, int end_token, int W, int max_ans_len,
-                              int32_t* answer_host, int32_t* length_host, double* score_host, int32_t* hist_host);
+  void gen_dialog_beam_search(const vd_batch* b, int k, int G, float lam, int L, int start_token, int end_token, int W,
+                              int max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
+                              int32_t* hist_host);
   void gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
                          int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host, int32_t* hist_host);
   // answer pool (DESIGN §18): a disc model answers by retrieval from the split's answer pool.  pool_tok (m, w) are the pool's
@@ -406,8 +412,8 @@ struct Engine {
   struct AskRows { int64_t n = 0; const int32_t *slot = nullptr, *round = nullptr; const int64_t* draw = nullptr; bool any_next = false; };
   AskRows dialog_encode(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int64_t row_offset);
   void dialog_finish(const AskRows& rows, const DialogAnswers& a);   // the rows' history append
-  void dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int L, int start_token,
-                       int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
+  void dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int G, float lam, int L,
+                       int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
   // row i draws as global round row_offset + draw_base[slots[i]] + its round
   void dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int L, int start_token, int end_token,
                          float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host);

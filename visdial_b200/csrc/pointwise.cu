@@ -1198,88 +1198,147 @@ __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __r
   }
 }
 
-// The candidate merge of one beam-search step (model.lua:529-569 as model.py restates it), one warp per round n.  Row
-// n*k + w is hypothesis (column) w of round n; candidate q = w*k + j is the j-th best class of row n*k + w, scored
-// scores[w] + topv in fp64.  At step 1 only column 0 is explored.  Candidates whose token is end_token compete for the
-// round's best finished hypothesis (strictly greater replaces: the first maximum in (step, q) order wins, as the
-// reference's stable sort keeps it); the others are ranked by (score desc, q asc) and the first min(#, k) fill columns
-// 0.. from the PRE-merge beams.  A column left unfilled keeps its beam and score, and is fed next step the state it was
-// fed this step (parent -1 - row) and its beam's next position (a pad, 0).  beams: (N, k, L) token histories.
-__global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int L, int end_token, const float* __restrict__ topv,
-                                                   const int32_t* __restrict__ topi, const double* __restrict__ sc_in,
-                                                   double* __restrict__ sc_out, const int32_t* __restrict__ beams_in,
-                                                   int32_t* __restrict__ beams_out, int32_t* __restrict__ tokens,
-                                                   int32_t* __restrict__ parent, int32_t* __restrict__ ans, int32_t* __restrict__ ans_len,
-                                                   double* __restrict__ ans_score) {
-  __shared__ int win_q[32];
+// The candidate merge of one beam-search step (model.lua:529-569 as model.py restates it), generalised to diverse beam
+// search (DESIGN §22), one warp per round n.  Row n*k + c is hypothesis (column) c of round n.  The k columns form G
+// groups of w = k / G; group g owns columns [g*w, (g+1)*w) and the groups are merged in order g = 0 .. G-1.
+//  - Explored columns: all w of the group (only its first at step 1).  Explored column e of group g takes its w best
+//    classes from its k top-k entries by (augmented desc, top-k position asc), augmented = (double)logp - lam * n_g(v),
+//    n_g(v) = the columns of groups < g filled at this step with token v.  Group 0 has no penalties: its explored set is
+//    the first w entries.  Candidate q = e*w + j is the j-th of them (G = 1: q = c*k + j, the reference's order).
+//  - Candidates whose token is end_token compete for group g's best finished hypothesis, unpenalised score
+//    s = scores[c] + logp in fp64 (strictly greater replaces: the first maximum in (step, q) order wins, as the
+//    reference's stable sort keeps it).
+//  - The others are ranked by (a desc, q asc), a = s - lam * n_g(v), and the first min(#, w) fill the group's columns
+//    from the PRE-merge beams; a column stores the unpenalised s.  A column left unfilled keeps its beam and score, and
+//    is fed next step the state it was fed this step (parent -1 - row) and its beam's next position (a pad, 0).
+// Penalties only lower a score and group g's penalised tokens number at most g*w, so the w best classes of a row under
+// the penalty lie inside its unpenalised top k: the decoder's top-k list holds every class DBS could pick.  The products
+// lam * n are __dmul_rn so that no fused multiply-add changes a's rounding.  beams: (N, k, L) token histories; ans
+// (N, G, L), ans_len / ans_score (N, G).  pick_* (N, L), (N), (N), or null: at the last step (stp == L - 1) the best of
+// the G answers by (score desc, group asc), groups without a finished hypothesis skipped (pick_len 0 when none).
+__global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float lam, int L, int end_token,
+                                                   const float* __restrict__ topv, const int32_t* __restrict__ topi,
+                                                   const double* __restrict__ sc_in, double* __restrict__ sc_out,
+                                                   const int32_t* __restrict__ beams_in, int32_t* __restrict__ beams_out,
+                                                   int32_t* __restrict__ tokens, int32_t* __restrict__ parent,
+                                                   int32_t* __restrict__ ans, int32_t* __restrict__ ans_len,
+                                                   double* __restrict__ ans_score, int32_t* __restrict__ pick_ans,
+                                                   int32_t* __restrict__ pick_len, double* __restrict__ pick_score) {
+  // per column: the filling candidate's source column, its token (0: unfilled) and its stored score
+  __shared__ int win_c[32], win_t[32];
   __shared__ double win_s[32];
+  // groups g > 0 (w <= 16): per explored entry its augmented value and penalty count; per candidate its top-k position
+  // and penalty count
+  __shared__ double e_aug[16 * 32];
+  __shared__ unsigned char e_cnt[16 * 32], c_pos[16 * 16], c_cnt[16 * 16];
   const int n = blockIdx.x, lane = threadIdx.x;
-  const int ncand = (stp == 1 ? 1 : k) * k;
-  const float* tv = topv + (int64_t)n * k * k;          // rows n*k .. n*k+k-1, k entries each: index q
+  const int w = k / G;
+  const int ne = stp == 1 ? 1 : w;                       // explored columns per group
+  const int ncand = ne * w;
+  const double lamd = (double)lam;
+  const float* tv = topv + (int64_t)n * k * k;          // rows n*k .. n*k+k-1, k entries each
   const int32_t* ti = topi + (int64_t)n * k * k;
   const double* sc = sc_in + (int64_t)n * k;
   const int32_t* bin = beams_in + (int64_t)n * k * L;
-  // finished hypotheses of this step: the first maximum, then against the round's best so far
-  bool fnd = false; double fs = 0.0; int fq = 0x7fffffff;
-  for (int q = lane; q < ncand; q += 32) {
-    if (ti[q] + 1 != end_token) continue;
-    const double s = sc[q / k] + (double)tv[q];
-    if (!fnd || s > fs) { fnd = true; fs = s; fq = q; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const bool of = __shfl_xor_sync(FULL, fnd, o);
-    const double os = __shfl_xor_sync(FULL, fs, o);
-    const int oq = __shfl_xor_sync(FULL, fq, o);
-    if (of && (!fnd || os > fs || (os == fs && oq < fq))) { fnd = true; fs = os; fq = oq; }
-  }
-  const bool better = fnd && (ans_len[n] == 0 || fs > ans_score[n]);    // warp-uniform
-  __syncwarp();                                            // every lane has read the best so far before lane 0 replaces it
-  if (better) {
-    const int w = fq / k;
-    for (int p = lane; p < stp; p += 32) ans[(int64_t)n * L + p] = bin[(int64_t)w * L + p];
-    if (lane == 0) { ans[(int64_t)n * L + stp] = end_token; ans_len[n] = stp + 1; ans_score[n] = fs; }
-  }
-  // the k best other candidates: round j takes the best one strictly after round j-1's winner
-  int nfill = 0;
-  double ps = INFINITY; int pq = -1;
-  for (int j = 0; j < k; ++j) {
-    bool ok = false; double bs = 0.0; int bq = 0x7fffffff;
+  for (int g = 0; g < G; ++g) {
+    const int c0 = g * w;
+    if (g > 0) {
+      for (int i = lane; i < ne * k; i += 32) {
+        const int t = ti[c0 * k + i] + 1;
+        int cnt = 0;
+        for (int c = 0; c < c0; ++c) cnt += win_t[c] == t;
+        e_cnt[i] = (unsigned char)cnt;
+        e_aug[i] = (double)tv[c0 * k + i] - __dmul_rn(lamd, (double)cnt);
+      }
+      __syncwarp();
+      for (int i = lane; i < ne * k; i += 32) {
+        const int e = i / k, p = i % k;
+        const double a = e_aug[i];
+        int rank = 0;
+        for (int p2 = 0; p2 < k; ++p2) {
+          const double a2 = e_aug[e * k + p2];
+          rank += a2 > a || (a2 == a && p2 < p);
+        }
+        if (rank < w) { c_pos[e * w + rank] = (unsigned char)p; c_cnt[e * w + rank] = e_cnt[i]; }
+      }
+      __syncwarp();
+    }
+    // candidate q of group g: its top-k entry (column c0 + q / w), and its penalty count
+    const auto entry = [&](int q) { return (c0 + q / w) * k + (g ? (int)c_pos[q] : q % w); };
+    const auto count = [&](int q) { return g ? (int)c_cnt[q] : 0; };
+    // finished hypotheses of this step: the first maximum, then against the group's best so far
+    bool fnd = false; double fs = 0.0; int fq = 0x7fffffff;
     for (int q = lane; q < ncand; q += 32) {
-      if (ti[q] + 1 == end_token) continue;
-      const double s = sc[q / k] + (double)tv[q];
-      if (!(s < ps || (s == ps && q > pq))) continue;
-      if (!ok || s > bs) { ok = true; bs = s; bq = q; }
+      const int idx = entry(q);
+      if (ti[idx] + 1 != end_token) continue;
+      const double s = sc[idx / k] + (double)tv[idx];
+      if (!fnd || s > fs) { fnd = true; fs = s; fq = q; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-      const bool of = __shfl_xor_sync(FULL, ok, o);
-      const double os = __shfl_xor_sync(FULL, bs, o);
-      const int oq = __shfl_xor_sync(FULL, bq, o);
-      if (of && (!ok || os > bs || (os == bs && oq < bq))) { ok = true; bs = os; bq = oq; }
+      const bool of = __shfl_xor_sync(FULL, fnd, o);
+      const double os = __shfl_xor_sync(FULL, fs, o);
+      const int oq = __shfl_xor_sync(FULL, fq, o);
+      if (of && (!fnd || os > fs || (os == fs && oq < fq))) { fnd = true; fs = os; fq = oq; }
     }
-    if (!ok) break;                                        // warp-uniform
-    if (lane == 0) { win_q[j] = bq; win_s[j] = bs; }
-    nfill = j + 1; ps = bs; pq = bq;
+    const int64_t ng = (int64_t)n * G + g;
+    const bool better = fnd && (ans_len[ng] == 0 || fs > ans_score[ng]);    // warp-uniform
+    __syncwarp();                                          // every lane has read the best so far before lane 0 replaces it
+    if (better) {
+      const int c = c0 + fq / w;
+      for (int p = lane; p < stp; p += 32) ans[ng * L + p] = bin[(int64_t)c * L + p];
+      if (lane == 0) { ans[ng * L + stp] = end_token; ans_len[ng] = stp + 1; ans_score[ng] = fs; }
+    }
+    // the w best other candidates: round j takes the best one strictly after round j-1's winner
+    int nfill = 0;
+    double ps = INFINITY; int pq = -1;
+    for (int j = 0; j < w; ++j) {
+      bool ok = false; double bs = 0.0; int bq = 0x7fffffff;
+      for (int q = lane; q < ncand; q += 32) {
+        const int idx = entry(q);
+        if (ti[idx] + 1 == end_token) continue;
+        double s = sc[idx / k] + (double)tv[idx];
+        if (const int cnt = count(q)) s -= __dmul_rn(lamd, (double)cnt);
+        if (!(s < ps || (s == ps && q > pq))) continue;
+        if (!ok || s > bs) { ok = true; bs = s; bq = q; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const bool of = __shfl_xor_sync(FULL, ok, o);
+        const double os = __shfl_xor_sync(FULL, bs, o);
+        const int oq = __shfl_xor_sync(FULL, bq, o);
+        if (of && (!ok || os > bs || (os == bs && oq < bq))) { ok = true; bs = os; bq = oq; }
+      }
+      if (!ok) break;                                      // warp-uniform
+      if (lane == 0) {
+        const int idx = entry(bq);
+        win_c[c0 + j] = idx / k; win_t[c0 + j] = ti[idx] + 1; win_s[c0 + j] = sc[idx / k] + (double)tv[idx];
+      }
+      nfill = j + 1; ps = bs; pq = bq;
+    }
+    for (int j = nfill + lane; j < w; j += 32) { win_c[c0 + j] = c0 + j; win_t[c0 + j] = 0; win_s[c0 + j] = sc[c0 + j]; }
+    __syncwarp();                                          // the next group counts this one's tokens
   }
-  __syncwarp();
   const int row0 = n * k;
   for (int i = lane; i < k * (stp + 1); i += 32) {
     const int c = i / (stp + 1), p = i % (stp + 1);
-    int32_t t;
-    if (c < nfill) {
-      const int q = win_q[c];
-      t = p < stp ? bin[(int64_t)(q / k) * L + p] : ti[q] + 1;
-    } else {
-      t = p < stp ? bin[(int64_t)c * L + p] : 0;
-    }
+    const int32_t t = p < stp ? bin[(int64_t)win_c[c] * L + p] : win_t[c];
     beams_out[((int64_t)row0 + c) * L + p] = t;
     if (p == stp) tokens[row0 + c] = t;
   }
   for (int c = lane; c < k; c += 32) {
-    const bool f = c < nfill;
-    sc_out[row0 + c] = f ? win_s[c] : sc[c];
-    parent[row0 + c] = f ? row0 + win_q[c] / k : -1 - (row0 + c);
+    sc_out[row0 + c] = win_s[c];
+    parent[row0 + c] = win_t[c] ? row0 + win_c[c] : -1 - (row0 + c);
+  }
+  if (pick_ans && stp == L - 1) {
+    int best = -1; double bsc = 0.0;                       // warp-uniform
+    for (int g = 0; g < G; ++g) {
+      const int64_t ng = (int64_t)n * G + g;
+      if (ans_len[ng] > 0 && (best < 0 || ans_score[ng] > bsc)) { best = g; bsc = ans_score[ng]; }
+    }
+    const int64_t nb = (int64_t)n * G + (best < 0 ? 0 : best);
+    for (int p = lane; p < L; p += 32) pick_ans[(int64_t)n * L + p] = best < 0 ? 0 : ans[nb * L + p];
+    if (lane == 0) { pick_len[n] = best < 0 ? 0 : ans_len[nb]; pick_score[n] = bsc; }
   }
 }
 
@@ -1760,13 +1819,17 @@ void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mas
 void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* beams, int32_t* tokens, double* scores) {
   L1D(k_beam_init, rows * L, rows, L, start_token, beams, tokens, scores);
 }
-void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int L, int end_token, const float* topv, const int32_t* topi,
-                const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out, int32_t* tokens,
-                int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score) {
+void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int L, int end_token, const float* topv,
+                const int32_t* topi, const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out,
+                int32_t* tokens, int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score, int32_t* pick_ans,
+                int32_t* pick_len, double* pick_score) {
   VD_REQUIRE(k >= 1 && k <= 32 && stp >= 1 && stp < L, VD_E_BADARG, "beam_merge: k / step");
+  VD_REQUIRE(G >= 1 && k % G == 0 && std::isfinite(lam) && lam >= 0.f, VD_E_BADARG, "beam_merge: groups / diversity");
+  VD_REQUIRE(!pick_ans == !pick_len && !pick_ans == !pick_score, VD_E_BADARG, "beam_merge: all pick outputs or none");
   if (N == 0) return;
-  k_beam_merge<<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, L, end_token, topv, topi, scores_in, scores_out, beams_in, beams_out,
-                                                  tokens, parent, ans, ans_len, ans_score);
+  k_beam_merge<<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, G, lam, L, end_token, topv, topi, scores_in, scores_out, beams_in,
+                                                  beams_out, tokens, parent, ans, ans_len, ans_score, pick_ans, pick_len,
+                                                  pick_score);
   check_launch(cx, "k_beam_merge");
 }
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1, float beta2,

@@ -244,6 +244,15 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        logsoftmax_topk_rows(e->cx, CF(0), CI32(1), I[0], IN(1), IN(2), F(2), I32(3));
      }},
+    // the beam-search merge of one step (DESIGN §22).  ptrs topv, topi, scores_in, scores_out, beams_in, beams_out, tokens,
+    // parent, ans, ans_len, ans_score, pick_ans, pick_len, pick_score (the three pick pointers all null or none); ints N, stp,
+    // k, G, L, end_token; reals diversity
+    {"beam_merge", 14, 6, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       beam_merge(e->cx, I[0], IN(1), IN(2), IN(3), (float)X[0], IN(4), IN(5), CF(0), CI32(1), static_cast<const double*>(P[2]),
+                  static_cast<double*>(P[3]), CI32(4), I32(5), I32(6), I32(7), I32(8), I32(9), static_cast<double*>(P[10]), I32(11),
+                  I32(12), static_cast<double*>(P[13]));
+     }},
     // ptrs logits, tokens, answer, logp; ints rows, V, L, seed, step, row_offset, row_stride; reals temperature
     {"logsoftmax_sample_rows", 4, 7, 1,
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {

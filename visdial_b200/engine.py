@@ -390,6 +390,21 @@ class Engine:
                                           score.ctypes.data))
         return ans, length, score
 
+    def gen_diverse_beam_search(self, k: int, G: int, diversity: float, L: int, start: int, end: int):
+        """Diverse beam search for every round of the last encoder forward (vd_gen_diverse_beam_search, DESIGN §22): k
+        columns in G groups of k / G, Hamming diversity `diversity`.  Returns each group's best finished hypothesis as
+        (answer (N, G, L) int32, length (N, G) int32 — 0 where the group finished none — and score (N, G) float64)."""
+        N = self._enc_rows
+        if N is None:
+            raise _lib.VdError(_lib.VD_E_STATE, "gen_diverse_beam_search before encoder_forward")
+        G = int(G)                         # buffers for G >= 1; the library refuses a G it cannot take
+        ans = np.zeros((N, max(G, 1), int(L)), dtype=np.int32)
+        length = np.zeros((N, max(G, 1)), dtype=np.int32)
+        score = np.zeros((N, max(G, 1)), dtype=np.float64)
+        check(self.lib.vd_gen_diverse_beam_search(self.h, int(k), G, float(diversity), int(L), int(start), int(end),
+                                                  ans.ctypes.data, length.ctypes.data, score.ctypes.data))
+        return ans, length, score
+
     def gen_sample(self, L: int, start: int, temperature: float, seed: int, row_offset: int = 0):
         """Ancestral sampling for every round of the last encoder forward on the device (vd_gen_sample).  Returns (answer
         (N, L+1) int32 — column 0 = `start` — and logp (N, L) float32, each sample's un-tempered log-probability).  Row r's
@@ -416,6 +431,24 @@ class Engine:
         check(self.lib.vd_gen_dialog_beam_search(self.h, C.byref(batch.c), int(k), int(L), int(start), int(end),
                                                  int(hist_width), int(max_ans_len), ans.ctypes.data, length.ctypes.data,
                                                  score.ctypes.data, hist.ctypes.data))
+        self._enc_rows = B * R
+        return ans, length, score, hist
+
+    def gen_dialog_diverse_beam_search(self, batch: Batch, k: int, G: int, diversity: float, L: int, start: int, end: int,
+                                       hist_width: int, max_ans_len: int):
+        """Dialogs on the model's own answers with diverse beam search (vd_gen_dialog_diverse_beam_search): round r's
+        history takes each round's pick.  Returns (answer (N, G, L), length (N, G), score (N, G), history rows (B,
+        maxQuesCount, hist_width))."""
+        B, R, G = batch.c.B, self.params["maxQuesCount"], int(G)
+        ans = np.zeros((B * R, max(G, 1), int(L)), dtype=np.int32)
+        length = np.zeros((B * R, max(G, 1)), dtype=np.int32)
+        score = np.zeros((B * R, max(G, 1)), dtype=np.float64)
+        hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
+        self._enc_rows = None
+        check(self.lib.vd_gen_dialog_diverse_beam_search(self.h, C.byref(batch.c), int(k), G, float(diversity), int(L),
+                                                         int(start), int(end), int(hist_width), int(max_ans_len),
+                                                         ans.ctypes.data, length.ctypes.data, score.ctypes.data,
+                                                         hist.ctypes.data))
         self._enc_rows = B * R
         return ans, length, score, hist
 
@@ -631,6 +664,21 @@ class Engine:
         self._enc_rows = None
         check(self.lib.vd_dialog_ask_beam_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(k), int(L),
                                                 int(start), int(end), ans.ctypes.data, length.ctypes.data, score.ctypes.data))
+        self._dialog_rows = n
+        return ans, length, score
+
+    def dialog_ask_diverse_slots(self, slots, ques, k: int, G: int, diversity: float, L: int, start: int, end: int):
+        """Ask slots (n) one question each with diverse beam search (vd_dialog_ask_diverse_slots): (answer (n, G, L),
+        length (n, G), score (n, G)) in row order; each slot's history takes its row's pick."""
+        s, q = self._slot_rows(slots, ques)
+        n, G = s.size, int(G)
+        ans = np.zeros((n, max(G, 1), int(L)), dtype=np.int32)
+        length = np.zeros((n, max(G, 1)), dtype=np.int32)
+        score = np.zeros((n, max(G, 1)), dtype=np.float64)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_diverse_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(k), G,
+                                                   float(diversity), int(L), int(start), int(end), ans.ctypes.data,
+                                                   length.ctypes.data, score.ctypes.data))
         self._dialog_rows = n
         return ans, length, score
 

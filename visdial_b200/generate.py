@@ -7,7 +7,9 @@ utils.idToWords, which is what vis/static/main.js shows.  A round where no beam 
 anything is written (the reference dies there too, model.lua:575).  `-dialogsPerCall D` searches D dialogs per device
 call; 1 (the default) is the reference's per-dialog loop.  `-history generated` answers every round with the dialog's own
 earlier answers in its history instead of the dataset's (`-history gt`, the default and the reference's behaviour; DESIGN
-§17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.  A disc checkpoint answers every round with the
+§17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.  `-beamGroups G` (> 1, dividing `-beamSize`) runs
+diverse beam search with penalty `-diversity` (DESIGN §22): each round's answer is the best group's, and the round also
+lists `"answers"`, the text of every group that finished an answer, best first (the first is the round's answer).  A disc checkpoint answers every round with the
 best answer of the split's answer pool (Model.retrieveAnswers, DESIGN §18); the beam and sampling options do not apply
 to it, and its answer text is the pool row's words.
 
@@ -23,19 +25,25 @@ from . import cli
 def rank_share(model, dl, opt: dict) -> list:
     """This rank's share of the first `maxThreads` val dialogs as results.json entries (an empty list when the share is
     empty): generateAnswers' token lists turned into utils.idToWords text."""
+    from .model import ranked_groups
     from .utils import idToWords
     dl.restrict("val", max(0, opt["maxThreads"]))                                   # model.lua:455 over the ranks
     sampleParams = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "dialogsPerCall")}   # :88-94
     sampleParams["history"] = opt.get("history", "gt")
+    sampleParams.update({k: opt[k] for k in ("beamGroups", "diversity") if k in opt})
     if model.params["decoder"] == "disc":
         # a disc model answers by retrieval from the split's answer pool (DESIGN §18); model.lua:434-437 stops here
         answers = model.retrieveAnswers(dl, "val", {k: sampleParams[k] for k in ("dialogsPerCall", "history")})
     else:
         answers = model.generateAnswers(dl, "val", sampleParams)                    # :96
     words = dl.ind2word
-    return [{"image_id": a["image_id"],
-             "dialog": [{"question": idToWords(r["question"], words), "answer": idToWords(r["answer"], words)}
-                        for r in a["dialog"]]} for a in answers]
+
+    def turn(r):
+        t = {"question": idToWords(r["question"], words), "answer": idToWords(r["answer"], words)}
+        if "groups" in r:
+            t["answers"] = [idToWords(g["answer"], words) for g in ranked_groups(r)]
+        return t
+    return [{"image_id": a["image_id"], "dialog": [turn(r) for r in a["dialog"]]} for a in answers]
 
 
 def main(opt: dict, rank: int = 0, world: int = 1):
@@ -51,7 +59,7 @@ def main(opt: dict, rank: int = 0, world: int = 1):
         data = vdist.gather_objects(data, world)
     if rank == 0:
         # the file says what was generated, not how the run was spread over GPUs: 1- and N-GPU runs write the same bytes
-        opts = {k: v for k, v in opt.items() if k != "gpus"}
+        opts = {k: v for k, v in cli.written_opts(opt).items() if k != "gpus"}
         path = os.path.join(opt["resultPath"], "results.json")                      # :97-103
         cli.write_json(path, {"opts": opts, "data": data})
         say("Writing the results to " + path)

@@ -226,7 +226,13 @@ class Model:
         `history`: "gt" (the default, the reference's behaviour) answers every round with the dataset's history;
         "generated" runs each dialog on its own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample, DESIGN §17):
         round r's history holds the answers generated for rounds < r.  Encoders without history have nothing to feed back
-        and answer as with "gt"."""
+        and answer as with "gt".
+
+        `beamGroups` G > 1 (default 1) runs diverse beam search (vd_gen_diverse_beam_search, DESIGN §22): the beamSize
+        columns in G groups, each group's candidates penalised by `diversity` (default 0.5) per column of an earlier group
+        that chose the same token at that step.  Each round's answer / score / length are then the pick (the best group by
+        score, the lower group on ties; what the "generated" history takes), and "groups" lists the G groups' entries
+        (None for a group that finished no hypothesis).  `strict` raises only when every group is empty."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
@@ -242,6 +248,8 @@ class Model:
         sampleWords = bool(params.get("sampleWords", 0) == 1)                           # :443
         temperature, seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
         beamSize, beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
+        groups, diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
+        diverse = groups > 1 and not sampleWords
         startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
         numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
         dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
@@ -269,6 +277,9 @@ class Model:
                 if sampleWords:
                     answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
                                                                  rowOffset, histWidth, maxAnsLen)
+                elif diverse:
+                    answer, length, score, _ = self.engine.gen_dialog_diverse_beam_search(
+                        batch, beamSize, groups, diversity, beamLen, startToken, endToken, histWidth, maxAnsLen)
                 else:
                     answer, length, score, _ = self.engine.gen_dialog_beam_search(batch, beamSize, beamLen, startToken,
                                                                                   endToken, histWidth, maxAnsLen)
@@ -276,23 +287,31 @@ class Model:
                 self.forwardBackward(batch, True, True)                                 # :467
                 if sampleWords:                                                         # :582-594
                     answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
+                elif diverse:
+                    answer, length, score = self.engine.gen_diverse_beam_search(beamSize, groups, diversity, beamLen,
+                                                                                startToken, endToken)
                 else:                                                                   # :472-579
                     answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
+            R = self.params["maxQuesCount"]
             if not sampleWords:
-                length, score = length.reshape(len(inds), -1), score.reshape(len(inds), -1)
+                length, score = length.reshape(len(inds), R, -1), score.reshape(len(inds), R, -1)
             ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
             Tq = ques.shape[2]
-            answer = answer.reshape(len(inds), -1, answer.shape[1])
+            answer = answer.reshape(len(inds), R, -1, answer.shape[-1])
             self.wrapper.training()                                                     # :605
             for d, convId in enumerate(inds):
                 w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
                 threadAnswers = []
                 for it in range(ques.shape[1]):
-                    q, a = ques[d, it, Tq - w:], answer[d, it]
+                    q = ques[d, it, Tq - w:]
                     if sampleWords:
-                        threadAnswers.append(entry(q, a))
-                    elif length[d, it] > 0:
-                        threadAnswers.append(entry(q, a, score=float(score[d, it]), length=int(length[d, it])))
+                        threadAnswers.append(entry(q, answer[d, it, 0]))
+                        continue
+                    gs = [entry(q, answer[d, it, g], score=float(score[d, it, g]), length=int(length[d, it, g]))
+                          if length[d, it, g] > 0 else None for g in range(length.shape[2])]
+                    best = pick_group(length[d, it], score[d, it])
+                    if best >= 0:
+                        threadAnswers.append(dict(gs[best], groups=gs) if diverse else gs[best])
                     elif strict:
                         raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
                     else:
@@ -390,6 +409,22 @@ class Model:
         return ck
 
 
+def pick_group(length, score) -> int:
+    """A diverse search's pick (DESIGN §22): the group of the best finished hypothesis by (score desc, group asc), -1 when
+    no group finished one."""
+    best = -1
+    for g in range(len(length)):
+        if length[g] > 0 and (best < 0 or score[g] > score[best]):
+            best = g
+    return best
+
+
+def ranked_groups(entry) -> list:
+    """The finished groups of a diverse entry ("groups"), best first by (score desc, group asc): the pick is the first."""
+    done = [e for e in entry.get("groups", [entry]) if e is not None]
+    return sorted(done, key=lambda e: -e["score"])
+
+
 def history_answer(row, end: int, length=None) -> list:
     """The words of an answer as the history rule reads them (DESIGN §17).  With `length`: a beam hypothesis (<START>
     first) of that many tokens, its words between <START> and <END>, none when length is 0.  Without: the words before
@@ -441,6 +476,7 @@ class DialogPool:
         self.sampleWords = int(params.get("sampleWords", 0)) == 1
         self.temperature, self.seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
         self.beamSize, self.beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
+        self.groups, self.diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
         self.topK = int(params.get("topK", 1))
         self.start, self.end = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]
         self.width = dataloader.maxQuesLen
@@ -564,6 +600,16 @@ class DialogPool:
                                                       self.rowOffset)
             given = [history_answer(ans[b, 1:], self.end) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
+        elif self.groups > 1:
+            ans, length, score = self.eng.dialog_ask_diverse_slots(slots, q, self.beamSize, self.groups, self.diversity,
+                                                                   self.beamLen, self.start, self.end)
+            given = []
+            for b in range(len(q)):
+                gs = [{"answer": ans[b, g].tolist(), "score": float(score[b, g]), "length": int(length[b, g])}
+                      if length[b, g] > 0 else None for g in range(self.groups)]
+                best = pick_group(length[b], score[b])
+                given.append(history_answer(ans[b, best], self.end, length[b, best]) if best >= 0 else [])
+                out.append(dict(gs[best], question=[int(t) for t in q[b] if t], groups=gs) if best >= 0 else None)
         else:
             ans, length, score = self.eng.dialog_ask_beam_slots(slots, q, self.beamSize, self.beamLen, self.start, self.end)
             given = [history_answer(ans[b], self.end, length[b]) for b in range(len(q))]
@@ -577,6 +623,9 @@ class DialogPool:
             for e in out:
                 if e is not None:
                     e["question_text"], e["answer_text"] = text(e["question"]), text(e["answer"])
+                    for x in e.get("groups", ()):
+                        if x is not None:
+                            x["answer_text"] = text(x["answer"])
         return out
 
     def leave(self, slots):
