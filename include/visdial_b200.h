@@ -243,6 +243,22 @@ int vd_gen_dialog_diverse_beam_search(vd_engine* e, const vd_batch* b, int32_t b
                                       int32_t beam_len, int32_t start_token, int32_t end_token, int32_t hist_width,
                                       int32_t max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
                                       int32_t* hist_host);
+/* Truncated sampling (DESIGN §23): vd_gen_sample / vd_gen_dialog_sample with the draw restricted, at every step of every
+ * row, to a prefix of the classes in the order (y desc, class asc), y = logit / temperature: the first top_k of them
+ * (top_k = 0: all), then of those the shortest prefix holding top_p of their softmax mass (top_p = 1: all), measured in
+ * integer masses rint(exp(y - max y) 2^32) so that the boundary does not depend on summation order.  The token is the
+ * Gumbel-max argmax of vd_gen_sample's keys over the prefix: an exact draw from the renormalised truncated softmax, equal
+ * to vd_gen_sample's token whenever that token is in the prefix.  logp stays the un-tempered, untruncated LogSoftMax's.
+ * Truncation is active when 1 <= top_k < vocabSize or top_p < 1; inactive, the calls are vd_gen_sample /
+ * vd_gen_dialog_sample bit for bit.  Outputs as theirs.
+ * Refusals, before any state changes: those of vd_gen_sample / vd_gen_dialog_sample, and VD_E_BADARG for top_k < 0, top_p
+ * outside (0, 1] or not finite, and active truncation with vocabSize > 49152 (a row is staged in shared memory). */
+int vd_gen_truncated_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed,
+                            int64_t row_offset, int32_t top_k, float top_p, int32_t* answer_host, float* logp_host);
+int vd_gen_dialog_truncated_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
+                                   float temperature, uint64_t seed, int64_t row_offset, int32_t top_k, float top_p,
+                                   int32_t hist_width, int32_t max_ans_len, int32_t* answer_host, float* logp_host,
+                                   int32_t* hist_host);
 
 /* ---- answer-pool retrieval: disc models answer (DESIGN §18) --------------------------------------------------------
  * A disc model answers a question by retrieval: it scores every answer of the split's answer pool (opt_list_<split>, every
@@ -347,6 +363,12 @@ int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, cons
 int vd_dialog_ask_diverse_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
                                 int32_t groups, float diversity, int32_t beam_len, int32_t start_token, int32_t end_token,
                                 int32_t* answer, int32_t* length, double* score);
+/* vd_dialog_ask_sample_slots with vd_gen_truncated_sample's draw (DESIGN §23): answer (n, beam_len + 1), logp (n, beam_len)
+ * or NULL in row order.  A vd_dialog_begin session is the pool of slots 0..B-1.  Refusals, before any state changes, as
+ * vd_dialog_ask_sample_slots' and vd_gen_truncated_sample's. */
+int vd_dialog_ask_truncated_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq,
+                                  int32_t beam_len, int32_t start_token, int32_t end_token, float temperature, uint64_t seed,
+                                  int64_t row_offset, int32_t top_k, float top_p, int32_t* answer, float* logp);
 int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
 int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
 

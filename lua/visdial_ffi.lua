@@ -58,6 +58,12 @@ int vd_gen_dialog_diverse_beam_search(vd_engine* e, const vd_batch* b, int32_t b
                                       int32_t beam_len, int32_t start_token, int32_t end_token, int32_t hist_width,
                                       int32_t max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
                                       int32_t* hist_host);
+int vd_gen_truncated_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed,
+                            int64_t row_offset, int32_t top_k, float top_p, int32_t* answer_host, float* logp_host);
+int vd_gen_dialog_truncated_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
+                                   float temperature, uint64_t seed, int64_t row_offset, int32_t top_k, float top_p,
+                                   int32_t hist_width, int32_t max_ans_len, int32_t* answer_host, float* logp_host,
+                                   int32_t* hist_host);
 int vd_answer_pool_encode(vd_engine* e, const int32_t* tokens_host, int64_t m, int32_t width);
 int vd_answer_pool(vd_engine* e, const float** emb_dev, int64_t* m);
 int vd_answer_pool_retrieve(vd_engine* e, const vd_batch* b, int32_t k, int32_t* index_host, float* score_host);
@@ -88,6 +94,9 @@ int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, cons
 int vd_dialog_ask_diverse_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
                                 int32_t groups, float diversity, int32_t beam_len, int32_t start_token, int32_t end_token,
                                 int32_t* answer, int32_t* length, double* score);
+int vd_dialog_ask_truncated_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq,
+                                  int32_t beam_len, int32_t start_token, int32_t end_token, float temperature, uint64_t seed,
+                                  int64_t row_offset, int32_t top_k, float top_p, int32_t* answer, float* logp);
 int vd_dialog_slots(vd_engine* e, int32_t* rounds, int32_t* capacity);
 int vd_dialog_slot_history(vd_engine* e, const int32_t* slots, int32_t n, int32_t* hist);
 int vd_dialog_join_rounds(vd_engine* e, const vd_batch* b, const int32_t* rounds, const int32_t* answers, int32_t Ta,

@@ -129,6 +129,10 @@ SIGNATURES = {
                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gen_dialog_diverse_beam_search": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32,
                                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_gen_truncated_sample": [_H, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_int32, C.c_float, C.c_void_p,
+                                C.c_void_p],
+    "vd_gen_dialog_truncated_sample": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64,
+                                       C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_answer_pool_encode": [_H, C.c_void_p, C.c_int64, C.c_int32],
     "vd_answer_pool": [_H, _P(C.c_void_p), _P(C.c_int64)],
     "vd_answer_pool_retrieve": [_H, _P(vd_batch), C.c_int32, C.c_void_p, C.c_void_p],
@@ -155,6 +159,8 @@ SIGNATURES = {
     "vd_dialog_ask_pool_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p],
     "vd_dialog_ask_diverse_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_dialog_ask_truncated_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_float, C.c_uint64, C.c_int64, C.c_int32, C.c_float, C.c_void_p, C.c_void_p],
     "vd_dialog_slots": [_H, C.c_void_p, _P(C.c_int32)],
     "vd_dialog_slot_history": [_H, C.c_void_p, C.c_int32, C.c_void_p],
     "vd_gemm_atb16": [_H, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,

@@ -3,8 +3,9 @@
 Reads the model and data as `generate` does and opens a dialog session (Model.openDialogs) on the chosen images of
 `-split`: their features and captions; each question is answered before the next is asked, and the model's own answers
 become the history the next question is answered with.  Gen models answer with generate's beam search (`-beamSize`,
-`-beamLen`; diverse with `-beamGroups` > 1 and `-diversity`, DESIGN §22) or, with `-sampleWords 1`, by sampling; disc
-models with the best answer of the split's answer pool.
+`-beamLen`; diverse with `-beamGroups` > 1 and `-diversity`, DESIGN §22) or, with `-sampleWords 1`, by sampling
+(truncated to the top `-topK` words and the top `-topP` of the probability, DESIGN §23); disc models with the best answer
+of the split's answer pool.
 
 With `-questions file.json` ({image_id: [question, ...]}, at most maxQuesCount per image; a question is text or a list of
 token ids) every image of the file (or of `-imageIds`) is asked its questions, round by round, and
@@ -227,6 +228,8 @@ def main(opt: dict, rank: int = 0, world: int = 1):
         if missing:
             raise SystemExit("image ids not in split %s: %s" % (split, missing))
         params = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "beamGroups", "diversity")}
+        if model.params["decoder"] == "gen":         # a disc pool's topK is its retrieval list: the truncation is gen's
+            params.update({k: opt[k] for k in ("topK", "topP") if k in opt})
         R = model.params["maxQuesCount"]
         if opt["serve"]:
             serve(model, dl, split, index, params, opt["capacity"])

@@ -85,15 +85,21 @@ DIVERSE_OPTIONS = [
     ("beamGroups", 1, "Diverse beam search: groups the beam is split into (1 = plain beam search; must divide beamSize)"),
     ("diversity", 0.5, "Diverse beam search: penalty per earlier group's column that chose the same token"),
 ]
-# the generate command's table: generate.lua's options above, diverse beam search, and which history each round is
-# answered with
+# truncated sampling (DESIGN §23): -sampleWords 1 draws from the top-k / top-p prefix of each step's distribution
+TRUNCATION_OPTIONS = [
+    ("topK", 0, "Sampling: draw from the topK most likely words only (0 = all)"),
+    ("topP", 1.0, "Sampling: draw from the fewest most likely words holding topP of the probability (1 = all)"),
+]
+# the generate command's table: generate.lua's options above, diverse beam search, truncated sampling, and which history
+# each round is answered with
 HISTORY_MODES = ("gt", "generated")
-GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + [
+GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + TRUNCATION_OPTIONS + [
     ("history", "gt", "History each round is answered with: gt (the dataset's) | generated (the dialog's own answers)"),
 ]
 
-# the chat command: generate's options, diverse beam search, and which images are talked about with which questions
-CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + [
+# the chat command: generate's options, diverse beam search, truncated sampling, and which images are talked about with
+# which questions
+CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + TRUNCATION_OPTIONS + [
     ("split", "val", "Split the images and captions come from"),
     ("imageIds", "", "Comma-separated COCO image ids of the split (default: the -questions file's, else its first image)"),
     ("questions", "", "JSON {image_id: [question, ...]}: ask these and write results.json; else read stdin, one per line"),
@@ -156,6 +162,13 @@ def parse(options, argv=None, prog=None) -> dict:
             fail("-beamGroups must be at least 1 and divide -beamSize")
         if not math.isfinite(opt["diversity"]) or opt["diversity"] < 0:
             fail("-diversity must be finite and >= 0")
+    if "topK" in opt:
+        if opt["topK"] < 0:
+            fail("-topK must be >= 0")
+        if not (0.0 < opt["topP"] <= 1.0):
+            fail("-topP must be in (0, 1]")
+        if not truncated_sampling(opt):         # options that change nothing leave the run's options as they were
+            del opt["topK"], opt["topP"]
     if opt["gpus"] < 1:
         fail("-gpus must be at least 1")
     if opt["gpuid"] < 0:
@@ -176,11 +189,19 @@ def train_opts(argv=None, now=None, options=TRAIN_OPTIONS, prog="python -m visdi
     return opt
 
 
+def truncated_sampling(opt: dict) -> bool:
+    """-sampleWords 1 with a truncating -topK (> 0) or -topP (< 1)"""
+    return opt.get("sampleWords", 0) == 1 and (opt.get("topK", 0) > 0 or opt.get("topP", 1.0) < 1.0)
+
+
 def written_opts(opt: dict) -> dict:
     """The options a results.json records: the diverse beam search options only when they change the search
-    (-beamGroups > 1), so that a plain beam search writes the file it wrote before they existed."""
+    (-beamGroups > 1), and the truncation options only when they truncate a sampling run (-sampleWords 1 with -topK > 0 or
+    -topP < 1), so that every run without them writes the file it wrote before they existed."""
     plain = opt.get("beamGroups", 1) == 1
-    return {k: v for k, v in opt.items() if not (plain and k in ("beamGroups", "diversity"))}
+    untruncated = not truncated_sampling(opt)
+    return {k: v for k, v in opt.items()
+            if not (plain and k in ("beamGroups", "diversity")) and not (untruncated and k in ("topK", "topP"))}
 
 
 def model_params(opt: dict) -> dict:

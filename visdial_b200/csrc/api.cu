@@ -309,6 +309,25 @@ int vd_gen_dialog_sample(vd_engine* h, const vd_batch* b, int32_t beam_len, int3
                                      answer_host, logp_host, hist_host); })
 }
 
+static vd::TruncCfg trunc_cfg(int32_t top_k, float top_p) {
+  vd::TruncCfg t;
+  t.top_k = top_k;
+  t.top_p = top_p;
+  return t;
+}
+int vd_gen_truncated_sample(vd_engine* h, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed,
+                            int64_t row_offset, int32_t top_k, float top_p, int32_t* answer_host, float* logp_host) {
+  VD_TRY({ ENG(h)->gen_sample(beam_len, start_token, temperature, seed, row_offset, answer_host, logp_host, trunc_cfg(top_k, top_p)); })
+}
+
+int vd_gen_dialog_truncated_sample(vd_engine* h, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
+                                   float temperature, uint64_t seed, int64_t row_offset, int32_t top_k, float top_p,
+                                   int32_t hist_width, int32_t max_ans_len, int32_t* answer_host, float* logp_host,
+                                   int32_t* hist_host) {
+  VD_TRY({ ENG(h)->gen_dialog_sample(b, beam_len, start_token, end_token, temperature, seed, row_offset, hist_width, max_ans_len,
+                                     answer_host, logp_host, hist_host, trunc_cfg(top_k, top_p)); })
+}
+
 int vd_answer_pool_encode(vd_engine* h, const int32_t* tokens_host, int64_t m, int32_t width) {
   VD_TRY({ ENG(h)->answer_pool_encode(tokens_host, m, width); })
 }
@@ -424,6 +443,14 @@ int vd_dialog_ask_sample_slots(vd_engine* h, const int32_t* slots, int32_t n, co
                                int32_t* answer, float* logp) {
   VD_TRY({
     ENG(h)->dialog_ask_sample(slots, n, ques, Tq, beam_len, start_token, end_token, temperature, seed, row_offset, answer, logp);
+  })
+}
+int vd_dialog_ask_truncated_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq,
+                                  int32_t beam_len, int32_t start_token, int32_t end_token, float temperature, uint64_t seed,
+                                  int64_t row_offset, int32_t top_k, float top_p, int32_t* answer, float* logp) {
+  VD_TRY({
+    ENG(h)->dialog_ask_sample(slots, n, ques, Tq, beam_len, start_token, end_token, temperature, seed, row_offset, answer, logp,
+                              trunc_cfg(top_k, top_p));
   })
 }
 int vd_dialog_ask_pool_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t k,

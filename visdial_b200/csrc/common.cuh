@@ -127,6 +127,27 @@ __device__ __forceinline__ void sample_words(const SampleCfg& s, uint64_t q, uin
 // (key, class) beats (key2, class2): key descending, class ascending
 __device__ __forceinline__ bool sample_before(float k, int c, float k2, int c2) { return k > k2 || (k == k2 && c < c2); }
 
+// Truncated sampling (DESIGN §23): the draw above restricted to a prefix of the classes in the order
+// (y desc, class asc), y_j = x_j / T (the key's own fp32 division).  Active when 1 <= top_k < V or top_p < 1.
+//  1. top-k: the first top_k classes (all V when top_k is 0 or >= V).
+//  2. top-p over the classes step 1 kept: m = max y, w_j = expf(y_j - m), integer mass q_j = rint(w_j 2^32) (uint64),
+//     S = the kept classes' sum of q, tau = (uint64)ceil((double)top_p * (double)S); keep the shortest prefix whose
+//     cumulative q reaches tau (at least the first class).  Integer masses make S and every prefix sum independent of the
+//     summation order.  top_p = 1 skips the step.
+//  3. the token is 1 + argmax of y_j + g_j over the kept classes, g_j the SAME Philox Gumbel value as the untruncated draw
+//     (idx, SITE_SAMPLE, step): an exact draw from the renormalised truncated softmax, and equal to the untruncated draw
+//     whenever that draw's class is kept.  logp stays x_tok - lse of the untempered, untruncated LogSoftMax.
+// The numpy twin is tests/truncation_twin.py.
+struct TruncCfg {
+  int32_t top_k = 0;        // 0: no top-k
+  float top_p = 1.f;        // in (0, 1]; 1: no top-p
+};
+__host__ __device__ __forceinline__ bool trunc_active(const TruncCfg& t, int V) {
+  return (t.top_k >= 1 && t.top_k < V) || t.top_p < 1.f;
+}
+// the widest vocabulary whose row (4 V bytes of y) fits the truncated sampler's shared-memory stage beside its histograms
+constexpr int TRUNC_MAX_V = 49152;
+
 // ---------------------------------------------------------------------------------------------
 // Launch context: stream + launch accounting + optional per-class event bracketing.
 // ---------------------------------------------------------------------------------------------

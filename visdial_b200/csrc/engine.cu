@@ -1824,23 +1824,27 @@ Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t o
 
 // Model:generateAnswers' sampling (model.lua:581-602) for all N rounds of the last encoder forward at once, on the device.
 void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
-                        float* logp_host) {
+                        float* logp_host, const TruncCfg& tr) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_sample needs the gen decoder after encoder_forward");
-  check_sample_args(L, start_token, temperature, row_offset);
+  check_sample_args(L, start_token, temperature, row_offset, tr);
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
   const int64_t N = db.N;
-  const SampleResult res = sample_rows(N, 1, 0, L, start_token, temperature, seed, row_offset);
+  const SampleResult res = sample_rows(N, 1, 0, L, start_token, temperature, seed, row_offset, -1, 0, nullptr, tr);
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)N * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   if (logp_host)
     VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)N * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
-void Engine::check_sample_args(int L, int start_token, float temperature, int64_t row_offset) const {
+void Engine::check_sample_args(int L, int start_token, float temperature, int64_t row_offset, const TruncCfg& tr) const {
   VD_REQUIRE(L >= 1 && std::isfinite(temperature) && temperature > 0.f && row_offset >= 0 && start_token >= 1 &&
              start_token <= cfg.V, VD_E_BADARG, "beam_len >= 1, finite temperature > 0, row_offset >= 0, start_token in [1, V]");
+  VD_REQUIRE(tr.top_k >= 0 && std::isfinite(tr.top_p) && tr.top_p > 0.f && tr.top_p <= 1.f, VD_E_BADARG,
+             "top_k >= 0, top_p in (0, 1]");
+  VD_REQUIRE(!trunc_active(tr, cfg.V) || cfg.V <= TRUNC_MAX_V, VD_E_BADARG,
+             "truncated sampling stages a vocabulary row in shared memory: vocabSize <= 49152");
 }
 
 // The sampling itself, enqueued on cx.stream, for n rounds whose start state is row i * stride + off of the last encoder
@@ -1851,7 +1855,7 @@ void Engine::check_sample_args(int L, int start_token, float temperature, int64_
 // (n, L + 1) and log-probabilities (n, L) in the arena, valid until the next encoder forward.
 Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature,
                                          uint64_t seed, int64_t row_offset, int64_t draw_stride, int64_t draw_off,
-                                         const int64_t* draw_rounds) {
+                                         const int64_t* draw_rounds, const TruncCfg& tr) {
   forward_connect();
   const int H = cfg.H, V = cfg.V;
   const int64_t N = n;
@@ -1865,7 +1869,9 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
   const int nparts = vocab_lse_nparts(V);
   float *pm = nullptr, *ps = nullptr, *pk = nullptr, *px = nullptr;
   int32_t* pc = nullptr;
-  if (tcmode()) {
+  // active truncation needs each row's boundaries before its draw, which the fused epilogue cannot have: the rows route
+  const bool trunc = trunc_active(tr, V);
+  if (tcmode() && !trunc) {
     pm = arena.get<float>(N * nparts); ps = arena.get<float>(N * nparts); pk = arena.get<float>(N * nparts);
     px = arena.get<float>(N * nparts); pc = arena.get<int32_t>(N * nparts);
   }
@@ -1897,7 +1903,7 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
     gen_decoder_step_lstm(N, tok, h, c);
     smp.step = (uint32_t)stp;
     bool took = false;
-    if (tcmode() && (stp == 1 || fused)) {
+    if (tcmode() && !trunc && (stp == 1 || fused)) {
       LaunchCtx::Scope sc(&cx, "vocab_sample", 2.0 * N * V * H, 4.0 * (N * (double)H + (double)V * H + 5.0 * N * nparts));
       took = vocab_sample_tc(cx, (int)N, V, H, gstep2.h, H, Wp(wo), H, Wp(wo + 1), smp, pm, ps, pk, pc, px);
       if (took) vocab_sample_finish(cx, pm, ps, pk, pc, px, nparts, N, stp, L, tok, ans, lp);
@@ -1905,11 +1911,14 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
     if (stp == 1) fused = took;
     VD_REQUIRE(took == fused, VD_E_STATE, "vocab_sample_tc changed its mind between steps");
     if (!fused) {
-      // logits written once, read by the row's lse (two passes) and the draw
-      LaunchCtx::Scope sc(&cx, "sample_rows", 2.0 * N * V * H, 4.0 * (N * (double)H + (double)V * H + 2.0 * N * V));
+      // logits written once, read by the row's lse (two passes) and the draw (truncated: the lse and the row's staging in
+      // shared memory, which the selection and the draw read)
+      LaunchCtx::Scope sc(&cx, trunc ? "truncated_sample" : "sample_rows", 2.0 * N * V * H,
+                          4.0 * (N * (double)H + (double)V * H + (trunc ? 4.0 : 2.0) * N * V));
       float* logits = arena.get<float>(N * V);
       linear_fwd(wo, gstep2.h, N, logits, 0);
-      logsoftmax_sample_rows(cx, logits, N, V, smp, L, tok, ans, lp);
+      if (trunc) truncated_sample_rows(cx, logits, N, V, smp, tr, L, tok, ans, lp);
+      else logsoftmax_sample_rows(cx, logits, N, V, smp, L, tok, ans, lp);
     }
     h[0] = gstep1.h; h[1] = gstep2.h;
     c[0] = gstep1.c; c[1] = gstep2.c;
@@ -1988,9 +1997,9 @@ void Engine::gen_dialog_beam_search(const vd_batch* b, int k, int G, float lam, 
 
 void Engine::gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
                                int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host,
-                               int32_t* hist_host) {
+                               int32_t* hist_host, const TruncCfg& tr) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_sample needs the gen decoder");
-  check_sample_args(L, start_token, temperature, row_offset);
+  check_sample_args(L, start_token, temperature, row_offset, tr);
   VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
@@ -1999,7 +2008,7 @@ void Engine::gen_dialog_sample(const vd_batch* b, int L, int start_token, int en
   int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)N * (L + 1) * sizeof(int32_t));
   float* lp = (float*)dialog_out[3].ensure((size_t)N * L * sizeof(float));
   gen_dialog(b, W, max_ans_len, [&](int r) {
-    const SampleResult res = sample_rows(B, R, r, L, start_token, temperature, seed, row_offset);
+    const SampleResult res = sample_rows(B, R, r, L, start_token, temperature, seed, row_offset, -1, 0, nullptr, tr);
     scatter_round(cx.stream, ans, res.ans, (size_t)(L + 1) * sizeof(int32_t), R, r, B);
     scatter_round(cx.stream, lp, res.logp, (size_t)L * sizeof(float), R, r, B);
     // the samples before the first <END>
@@ -2555,15 +2564,15 @@ void Engine::dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* que
 
 void Engine::dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int L, int start_token,
                                int end_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
-                               float* logp_host) {
+                               float* logp_host, const TruncCfg& tr) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a sampling ask needs the gen decoder");
-  check_sample_args(L, start_token, temperature, row_offset);
+  check_sample_args(L, start_token, temperature, row_offset, tr);
   VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   dialog_check_ask(slots, n, ques_host, Tq);
   run_ask(this, slots, n, ques_host, Tq, row_offset, [&](const AskRows& rows) {
     // row i draws as global round row_offset + draw_base[slot] + its round (vd_dialog_begin: vd_gen_dialog_sample's rows)
-    const SampleResult res = sample_rows(n, 1, 0, L, start_token, temperature, seed, 0, -1, 0, rows.draw);
+    const SampleResult res = sample_rows(n, 1, 0, L, start_token, temperature, seed, 0, -1, 0, rows.draw, tr);
     VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)n * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
     if (logp_host)
       VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)n * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));

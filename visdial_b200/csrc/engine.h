@@ -336,16 +336,18 @@ struct Engine {
   // the decoder step up to the second LSTM layer (gstep1 / gstep2 hold the new state on return)
   void gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // Model:generateAnswers' sampling for every round of the last encoder forward, entirely on the device
+  // (tr: top-k / top-p truncation, DESIGN §23; the default truncates nothing)
   void gen_sample(int L, int start_token, float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host,
-                  float* logp_host);
-  void check_sample_args(int L, int start_token, float temperature, int64_t row_offset) const;
+                  float* logp_host, const TruncCfg& tr = {});
+  void check_sample_args(int L, int start_token, float temperature, int64_t row_offset, const TruncCfg& tr = {}) const;
   // its sampling on n rounds as beam_search_rows takes them; row i draws as global round
   // row_offset + i * draw_stride + draw_off (draw_stride < 0: the state's stride and offset)
   struct SampleResult { int32_t* ans; float* logp; };                   // (n, L + 1), (n, L)
-  // (draw_rounds non-null, device (n): row i draws as global round draw_rounds[i] instead)
+  // (draw_rounds non-null, device (n): row i draws as global round draw_rounds[i] instead).  Active truncation takes the
+  // rows route in every math mode.
   SampleResult sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature, uint64_t seed,
                            int64_t row_offset, int64_t draw_stride = -1, int64_t draw_off = 0,
-                           const int64_t* draw_rounds = nullptr);
+                           const int64_t* draw_rounds = nullptr, const TruncCfg& tr = {});
   // dialogs on the model's own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample): R rounds of {encoder forward on
   // the engine-owned history, round r's search, the history append} on the device
   struct DialogAnswers {             // where round r's answers are, for the history append
@@ -360,7 +362,8 @@ struct Engine {
                               int max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
                               int32_t* hist_host);
   void gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
-                         int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host, int32_t* hist_host);
+                         int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host, int32_t* hist_host,
+                         const TruncCfg& tr = {});
   // answer pool (DESIGN §18): a disc model answers by retrieval from the split's answer pool.  pool_tok (m, w) are the pool's
   // token rows, pool_emb (m, H) opt.lstm's h_T of each; pool_valid drops when the weights or the math mode change.
   GrowBuf pool_tok, pool_emb, pool_scratch;
@@ -416,7 +419,8 @@ struct Engine {
                        int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
   // row i draws as global round row_offset + draw_base[slots[i]] + its round
   void dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int L, int start_token, int end_token,
-                         float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host);
+                         float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host,
+                         const TruncCfg& tr = {});
   void dialog_ask_pool(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int32_t* index_host,
                        float* score_host);
   std::vector<int32_t> dialog_all_slots() const;   // 0..C-1: the lockstep asks' rows

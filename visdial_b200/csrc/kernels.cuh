@@ -201,6 +201,11 @@ void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int 
 // the bits it would give), the Gumbel-max draw of common.cuh; writes as vocab_sample_finish
 void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,
                             int32_t* answer, float* logp);
+// its truncated form (common.cuh's TruncCfg rule, DESIGN §23): the same draw over the top-k / top-p prefix of each row, logp
+// still logsoftmax_rows' bits.  V <= TRUNC_MAX_V (the row is staged in shared memory); VD_E_BADARG otherwise, or for
+// top_k < 0 or top_p outside (0, 1].
+void truncated_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, const TruncCfg& tr,
+                           int L, int32_t* tokens, int32_t* answer, float* logp);
 // the dialog loop's history (Engine::gen_dialog), one CTA per dialog b of hist (B, R, W), right-aligned rows.
 // r < 0: row 0 <- row b*R of src (B*R, src_w), right-aligned into W >= src_w; rows 1.. <- pads.
 // r >= 0: row r+1 <- round r's write (DESIGN §17): Q = the words of question row b*R + r of src (B*R, src_w), A = the first

@@ -1144,18 +1144,12 @@ __global__ void __launch_bounds__(256) k_logsoftmax_topk_rows(const float* __res
   }
 }
 
-// The sampling step from materialised logits, one block per row.  The lse comes from row_lse, so x_tok - lse is the
-// log-probability k_logsoftmax_rows would write.  Each thread takes Philox quadruples (4 consecutive element indices, one
-// call) strided over the row, keeps its best (key, class), and the block reduces them with the same order.
-__global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __restrict__ x, int V, SampleCfg smp, int L,
-                                                                int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
-                                                                float* __restrict__ logp) {
-  __shared__ float red[33];
-  __shared__ float sk[8];
-  __shared__ int sc[8];
-  const int64_t r = blockIdx.x;
-  const float* row = x + r * V;
-  const float lse = row_lse(row, V, red);
+// The Gumbel-max draw of common.cuh over row r's classes, by the whole block: y_of(j, y) gives class j's y = x_j / T and
+// says whether j takes part.  Each thread takes Philox quadruples (4 consecutive element indices, one call) strided over
+// the row, keeps its best (key, class), and the block reduces them with the same order.  The winning class is returned on
+// thread 0.
+template <typename Y>
+__device__ __forceinline__ int row_gumbel_argmax(const SampleCfg& smp, int64_t r, int V, Y y_of, float* sk, int* sc) {
   const uint64_t base = (uint64_t)sample_round(smp, r) * (uint64_t)V;
   const uint64_t q0 = base >> 2, q1 = (base + V - 1) >> 2;
   float bk = -INFINITY;
@@ -1163,11 +1157,13 @@ __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __r
   for (uint64_t q = q0 + threadIdx.x; q <= q1; q += blockDim.x) {
     const int64_t j0 = (int64_t)(q * 4 - base);                 // class of word 0 (< 0 or >= V outside the row)
     float y[4];
+    bool in[4];
     float ymax = -INFINITY;
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int64_t j = j0 + e;
-      y[e] = (j >= 0 && j < V) ? row[j] / smp.temperature : -INFINITY;
+      in[e] = j >= 0 && j < V && y_of((int)j, y[e]);
+      if (!in[e]) y[e] = -INFINITY;
       ymax = fmaxf(ymax, y[e]);
     }
     if (ymax + GUMBEL_MAX < bk) continue;                        // no key of the quadruple can reach the best one
@@ -1175,10 +1171,10 @@ __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __r
     sample_words(smp, q, o);
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      const int64_t j = j0 + e;
-      if (j < 0 || j >= V) continue;
+      if (!in[e]) continue;
+      const int j = (int)(j0 + e);
       const float key = y[e] + gumbel_of_word(o[e]);
-      if (sample_before(key, (int)j, bk, bc)) { bk = key; bc = (int)j; }
+      if (sample_before(key, j, bk, bc)) { bk = key; bc = j; }
     }
   }
 #pragma unroll
@@ -1189,9 +1185,170 @@ __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __r
   }
   if ((threadIdx.x & 31) == 0) { sk[threadIdx.x >> 5] = bk; sc[threadIdx.x >> 5] = bc; }
   __syncthreads();
-  if (threadIdx.x == 0) {
+  if (threadIdx.x == 0)
     for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
       if (sample_before(sk[w], sc[w], bk, bc)) { bk = sk[w]; bc = sc[w]; }
+  return bc;
+}
+
+// The sampling step from materialised logits, one block per row.  The lse comes from row_lse, so x_tok - lse is the
+// log-probability k_logsoftmax_rows would write.
+__global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __restrict__ x, int V, SampleCfg smp, int L,
+                                                                int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
+                                                                float* __restrict__ logp) {
+  __shared__ float red[33];
+  __shared__ float sk[8];
+  __shared__ int sc[8];
+  const int64_t r = blockIdx.x;
+  const float* row = x + r * V;
+  const float lse = row_lse(row, V, red);
+  const int bc = row_gumbel_argmax(smp, r, V, [&](int j, float& y) { y = row[j] / smp.temperature; return true; }, sk, sc);
+  if (threadIdx.x == 0) {
+    tokens[r] = bc + 1;
+    answer[r * (L + 1) + smp.step] = bc + 1;
+    if (logp) logp[r * L + smp.step - 1] = row[bc] - lse;
+  }
+}
+
+// ---- truncated sampling (common.cuh's rule, DESIGN §23) ------------------------------------------------------------
+// Order-preserving 32-bit key of y: key(a) > key(b) <=> a > b, with -0 and +0 one key (they are equal y).
+__device__ __forceinline__ uint32_t trunc_key(float y) {
+  const uint32_t u = __float_as_uint(y == 0.f ? 0.f : y);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float trunc_y(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+// integer mass q = rint(expf(y - m) 2^32) (2^32 at the maximum; the scaling by 2^32 is exact)
+__device__ __forceinline__ unsigned long long trunc_mass(float y, float m) { return __float2ull_rn(expf(y - m) * 0x1p32f); }
+
+struct TruncShared {
+  unsigned long long hist[8][256];   // per-warp radix histograms: logits crowd into a few high digits
+  unsigned long long scan[8];
+  unsigned long long sel_excl;
+  uint32_t sel_digit;
+  int sel_class;
+  float red[33];
+  float sk[8];
+  int sc[8];
+};
+
+// inclusive prefix sum over the 256 threads in thread order; sh holds >= 8 T
+template <typename T>
+__device__ __forceinline__ T block_incl_scan(T v, T* sh) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T n = __shfl_up_sync(FULL, v, o);
+    if (lane >= o) v += n;
+  }
+  __syncthreads();
+  if (lane == 31) sh[w] = v;
+  __syncthreads();
+  for (int i = 0; i < w; ++i) v += sh[i];
+  return v;
+}
+
+// Radix select over the staged y, 8 bits per pass from the top: the key t with W(key > t) < need <= W(key >= t), W the sum
+// of weight(j, key) (0: j takes no part), and above = W(key > t).  need must be in [1, W(all)].
+struct TruncSel { uint32_t key; unsigned long long above; };
+template <typename Wt>
+__device__ __forceinline__ TruncSel trunc_radix_select(const float* ys, int V, unsigned long long need, Wt weight, TruncShared& s) {
+  const int w = threadIdx.x >> 5;
+  uint32_t prefix = 0;
+  unsigned long long acc = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = threadIdx.x; i < 8 * 256; i += blockDim.x) (&s.hist[0][0])[i] = 0;
+    __syncthreads();
+    const uint32_t hmask = shift == 24 ? 0u : 0xffffffffu << (shift + 8);
+    for (int j = threadIdx.x; j < V; j += blockDim.x) {
+      const uint32_t k = trunc_key(ys[j]);
+      if ((k & hmask) != prefix) continue;
+      const unsigned long long wt = weight(j, k);
+      if (wt) atomicAdd(&s.hist[w][(k >> shift) & 255u], wt);
+    }
+    __syncthreads();
+    const uint32_t d = 255u - threadIdx.x;                       // thread t: digit 255 - t, so the scan runs key-descending
+    unsigned long long tot = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) tot += s.hist[i][d];
+    const unsigned long long incl = block_incl_scan(tot, s.scan), rem = need - acc;
+    if (incl - tot < rem && rem <= incl) { s.sel_digit = d; s.sel_excl = incl - tot; }
+    __syncthreads();
+    prefix |= s.sel_digit << shift;
+    acc += s.sel_excl;
+  }
+  return {prefix, acc};
+}
+
+// the class of the n-th (1-based) class of key t in class order: each thread counts a contiguous chunk, a block scan
+// finds the chunk, its thread walks it
+__device__ __forceinline__ int trunc_nth_of_key(const float* ys, int V, uint32_t t, uint32_t n, TruncShared& s) {
+  const int per = (V + blockDim.x - 1) / blockDim.x, b = threadIdx.x * per, e = min(V, b + per);
+  uint32_t c = 0;
+  for (int j = b; j < e; ++j) c += trunc_key(ys[j]) == t;
+  const uint32_t incl = block_incl_scan(c, reinterpret_cast<uint32_t*>(s.scan));
+  if (incl - c < n && n <= incl) {
+    uint32_t seen = incl - c;
+    for (int j = b; j < e; ++j)
+      if (trunc_key(ys[j]) == t && ++seen == n) { s.sel_class = j; break; }
+  }
+  __syncthreads();
+  return s.sel_class;
+}
+
+// The truncated sampling step from materialised logits, one 256-thread block per row (so row_lse reduces in
+// k_logsoftmax_rows' order and logp is its bits).  y = x / T is staged in dynamic shared memory (4 V bytes).  The kept
+// classes are a prefix of (y desc, class asc), held as its last element (tk, tc): key > tk, or key == tk and class <= tc.
+// top-k and top-p each find their boundary key by radix select (counts, then integer masses over the top-k prefix) and
+// the boundary class among that key's ties by a block scan in class order; the draw is row_gumbel_argmax over the prefix.
+__global__ void __launch_bounds__(256) k_truncated_sample_rows(const float* __restrict__ x, int V, SampleCfg smp, TruncCfg tr,
+                                                               int L, int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
+                                                               float* __restrict__ logp) {
+  extern __shared__ float ys[];
+  __shared__ TruncShared s;
+  const int64_t r = blockIdx.x;
+  const float* row = x + r * V;
+  float m = -INFINITY;
+  for (int j = threadIdx.x; j < V; j += blockDim.x) {
+    const float y = row[j] / smp.temperature;
+    ys[j] = y;
+    m = fmaxf(m, y);
+  }
+  m = block_max(m, s.red);                                       // its barriers also publish ys
+  uint32_t tk = 0;                                               // key 0 is below every y: all classes kept
+  int tc = 0x7fffffff;
+  if (tr.top_k >= 1 && tr.top_k < V) {
+    const TruncSel k = trunc_radix_select(ys, V, (unsigned long long)tr.top_k, [](int, uint32_t) { return 1ull; }, s);
+    tk = k.key;
+    tc = trunc_nth_of_key(ys, V, tk, (uint32_t)(tr.top_k - k.above), s);
+  }
+  if (tr.top_p < 1.f) {
+    const uint32_t k0 = tk;
+    const int c0 = tc;
+    auto mass = [&](int j, uint32_t k) { return (k > k0 || (k == k0 && j <= c0)) ? trunc_mass(ys[j], m) : 0ull; };
+    unsigned long long S = 0;
+    for (int j = threadIdx.x; j < V; j += blockDim.x) S += mass(j, trunc_key(ys[j]));
+    S = block_incl_scan(S, s.scan);
+    if (threadIdx.x == blockDim.x - 1) s.sel_excl = S;
+    __syncthreads();
+    S = s.sel_excl;
+    const unsigned long long tau = (unsigned long long)ceil((double)tr.top_p * (double)S);
+    const TruncSel p = trunc_radix_select(ys, V, tau, mass, s);
+    tk = p.key;
+    const unsigned long long qt = trunc_mass(trunc_y(tk), m);    // every tie of tk has this mass (> 0: it was selected)
+    // the ties it takes: the least n with above + n qt >= tau (a double quotient, corrected in integers)
+    const unsigned long long rem = tau - p.above;
+    unsigned long long n = (unsigned long long)((double)rem / (double)qt);
+    while (n * qt < rem) ++n;
+    while (n > 1 && (n - 1) * qt >= rem) --n;
+    tc = trunc_nth_of_key(ys, V, tk, (uint32_t)n, s);
+  }
+  const int bc = row_gumbel_argmax(smp, r, V, [&](int j, float& y) {
+    y = ys[j];
+    const uint32_t k = trunc_key(y);
+    return k > tk || (k == tk && j <= tc);
+  }, s.sk, s.sc);
+  const float lse = row_lse(row, V, s.red);                      // last: nothing long-lived across the selection
+  if (threadIdx.x == 0) {
     tokens[r] = bc + 1;
     answer[r * (L + 1) + smp.step] = bc + 1;
     if (logp) logp[r * L + smp.step - 1] = row[bc] - lse;
@@ -1801,6 +1958,18 @@ void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, in
   if (rows <= 0) return;
   k_logsoftmax_sample_rows<<<(unsigned)rows, 256, 0, cx.stream>>>(logits, V, smp, L, tokens, answer, logp);
   check_launch(cx, "k_logsoftmax_sample_rows");
+}
+void truncated_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, const TruncCfg& tr,
+                           int L, int32_t* tokens, int32_t* answer, float* logp) {
+  VD_REQUIRE(V >= 1 && V <= TRUNC_MAX_V, VD_E_BADARG, "truncated_sample_rows: V must be in [1, 49152] (the staged row)");
+  VD_REQUIRE(tr.top_k >= 0 && std::isfinite(tr.top_p) && tr.top_p > 0.f && tr.top_p <= 1.f, VD_E_BADARG,
+             "truncated_sample_rows: top_k >= 0, top_p in (0, 1]");
+  if (rows <= 0) return;
+  // the dynamic stage beside the static histograms passes the 48 KB default from V = 8 121 on: always opted in
+  const size_t smem = (size_t)V * sizeof(float);
+  VD_CUDA_CHECK(cudaFuncSetAttribute(k_truncated_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k_truncated_sample_rows<<<(unsigned)rows, 256, smem, cx.stream>>>(logits, V, smp, tr, L, tokens, answer, logp);
+  check_launch(cx, "k_truncated_sample_rows");
 }
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H) {
   L1D(k_beam_gather, rows * H, dst, out_prev, in_prev, parent, rows, H);

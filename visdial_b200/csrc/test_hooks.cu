@@ -270,6 +270,18 @@ const Entry TABLE[] = {
        s.row_round = static_cast<const int64_t*>(P[4]);
        logsoftmax_sample_rows(e->cx, CF(0), I[0], IN(1), s, IN(2), I32(1), I32(2), F(3));
      }},
+    // as logsoftmax_sample_rows, a fifth pointer (the per-row global rounds, or null: the affine rule), an eighth int top_k
+    // and a second real top_p (DESIGN §23)
+    {"truncated_sample_rows", 5, 8, 2,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       SampleCfg s;
+       s.seed_lo = (uint32_t)(uint64_t)I[3]; s.seed_hi = (uint32_t)((uint64_t)I[3] >> 32); s.step = (uint32_t)I[4];
+       s.temperature = (float)X[0]; s.row_offset = I[5]; s.row_stride = I[6];
+       s.row_round = static_cast<const int64_t*>(P[4]);
+       TruncCfg t;
+       t.top_k = IN(7); t.top_p = (float)X[1];
+       truncated_sample_rows(e->cx, CF(0), I[0], IN(1), s, t, IN(2), I32(1), I32(2), F(3));
+     }},
     // ptrs logits, lse, tgt, mask_ids, scale, dlogits (may alias logits); ints rows, V
     {"nll_bwd_scaled", 6, 2, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) {

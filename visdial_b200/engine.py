@@ -418,6 +418,20 @@ class Engine:
                                      int(row_offset), ans.ctypes.data, logp.ctypes.data))
         return ans, logp
 
+    def gen_truncated_sample(self, L: int, start: int, temperature: float, seed: int, row_offset: int = 0, top_k: int = 0,
+                             top_p: float = 1.0):
+        """gen_sample with top-k / top-p truncation (vd_gen_truncated_sample, DESIGN §23): each step draws from the first
+        `top_k` classes by (logit desc, class asc) (0: all), then the shortest prefix of those holding `top_p` of their mass
+        (1: all), with gen_sample's Philox draws.  Returns (answer (N, L+1), logp (N, L)) as gen_sample's."""
+        N = self._enc_rows
+        if N is None:
+            raise _lib.VdError(_lib.VD_E_STATE, "gen_truncated_sample before encoder_forward")
+        ans = np.zeros((N, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((N, int(L)), dtype=np.float32)
+        check(self.lib.vd_gen_truncated_sample(self.h, int(L), int(start), float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                               int(row_offset), int(top_k), float(top_p), ans.ctypes.data, logp.ctypes.data))
+        return ans, logp
+
     def gen_dialog_beam_search(self, batch: Batch, k: int, L: int, start: int, end: int, hist_width: int, max_ans_len: int):
         """Dialogs on the model's own answers with the beam search (vd_gen_dialog_beam_search): every round of `batch`,
         round r's encoder reading the answers generated for rounds < r.  Returns (answer (N, L), length (N), score (N),
@@ -464,6 +478,22 @@ class Engine:
         check(self.lib.vd_gen_dialog_sample(self.h, C.byref(batch.c), int(L), int(start), int(end), float(temperature),
                                             int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset), int(hist_width), int(max_ans_len),
                                             ans.ctypes.data, logp.ctypes.data, hist.ctypes.data))
+        self._enc_rows = B * R
+        return ans, logp, hist
+
+    def gen_dialog_truncated_sample(self, batch: Batch, L: int, start: int, end: int, temperature: float, seed: int,
+                                    row_offset: int, hist_width: int, max_ans_len: int, top_k: int = 0, top_p: float = 1.0):
+        """gen_dialog_sample with gen_truncated_sample's draw (vd_gen_dialog_truncated_sample): (answer (N, L+1), logp (N, L),
+        history rows (B, maxQuesCount, hist_width))."""
+        B, R = batch.c.B, self.params["maxQuesCount"]
+        ans = np.zeros((B * R, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((B * R, int(L)), dtype=np.float32)
+        hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
+        self._enc_rows = None
+        check(self.lib.vd_gen_dialog_truncated_sample(self.h, C.byref(batch.c), int(L), int(start), int(end), float(temperature),
+                                                      int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset), int(top_k), float(top_p),
+                                                      int(hist_width), int(max_ans_len), ans.ctypes.data, logp.ctypes.data,
+                                                      hist.ctypes.data))
         self._enc_rows = B * R
         return ans, logp, hist
 
@@ -694,6 +724,22 @@ class Engine:
         check(self.lib.vd_dialog_ask_sample_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(L), int(start),
                                                   int(end), float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, int(row_offset),
                                                   ans.ctypes.data, logp.ctypes.data))
+        self._dialog_rows = n
+        return ans, logp
+
+    def dialog_ask_truncated_slots(self, slots, ques, L: int, start: int, end: int, temperature: float, seed: int,
+                                   row_offset: int = 0, top_k: int = 0, top_p: float = 1.0):
+        """dialog_ask_sample_slots with gen_truncated_sample's draw (vd_dialog_ask_truncated_slots): (answer (n, L+1),
+        logp (n, L)) in row order."""
+        s, q = self._slot_rows(slots, ques)
+        n = s.size
+        ans = np.zeros((n, int(L) + 1), dtype=np.int32)
+        logp = np.zeros((n, int(L)), dtype=np.float32)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_truncated_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(L),
+                                                     int(start), int(end), float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF,
+                                                     int(row_offset), int(top_k), float(top_p), ans.ctypes.data,
+                                                     logp.ctypes.data))
         self._dialog_rows = n
         return ans, logp
 

@@ -9,7 +9,10 @@ call; 1 (the default) is the reference's per-dialog loop.  `-history generated` 
 earlier answers in its history instead of the dataset's (`-history gt`, the default and the reference's behaviour; DESIGN
 §17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.  `-beamGroups G` (> 1, dividing `-beamSize`) runs
 diverse beam search with penalty `-diversity` (DESIGN §22): each round's answer is the best group's, and the round also
-lists `"answers"`, the text of every group that finished an answer, best first (the first is the round's answer).  A disc checkpoint answers every round with the
+lists `"answers"`, the text of every group that finished an answer, best first (the first is the round's answer).
+`-topK K` and `-topP P` truncate `-sampleWords 1`'s draws to the K most likely words and then to the fewest of those
+holding P of the probability (DESIGN §23); they combine with `-history`, `-dialogsPerCall` and `-gpus`, and
+results.json records them only when they truncate.  A disc checkpoint answers every round with the
 best answer of the split's answer pool (Model.retrieveAnswers, DESIGN §18); the beam and sampling options do not apply
 to it, and its answer text is the pool row's words.
 
@@ -30,7 +33,7 @@ def rank_share(model, dl, opt: dict) -> list:
     dl.restrict("val", max(0, opt["maxThreads"]))                                   # model.lua:455 over the ranks
     sampleParams = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "dialogsPerCall")}   # :88-94
     sampleParams["history"] = opt.get("history", "gt")
-    sampleParams.update({k: opt[k] for k in ("beamGroups", "diversity") if k in opt})
+    sampleParams.update({k: opt[k] for k in ("beamGroups", "diversity", "topK", "topP") if k in opt})
     if model.params["decoder"] == "disc":
         # a disc model answers by retrieval from the split's answer pool (DESIGN §18); model.lua:434-437 stops here
         answers = model.retrieveAnswers(dl, "val", {k: sampleParams[k] for k in ("dialogsPerCall", "history")})

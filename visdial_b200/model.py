@@ -232,7 +232,12 @@ class Model:
         columns in G groups, each group's candidates penalised by `diversity` (default 0.5) per column of an earlier group
         that chose the same token at that step.  Each round's answer / score / length are then the pick (the best group by
         score, the lower group on ties; what the "generated" history takes), and "groups" lists the G groups' entries
-        (None for a group that finished no hypothesis).  `strict` raises only when every group is empty."""
+        (None for a group that finished no hypothesis).  `strict` raises only when every group is empty.
+
+        With `sampleWords`, `topK` K (default 0, off) and `topP` P (default 1, off) truncate every draw (DESIGN §23): to the
+        first K classes by (logit desc, class asc), then to the shortest prefix of those holding P of their softmax mass
+        (vd_gen_truncated_sample / vd_gen_dialog_truncated_sample).  When neither truncates (K = 0 or K >= vocabSize, and
+        P = 1) the calls are the untruncated ones.  Beam search ignores both."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
@@ -250,6 +255,8 @@ class Model:
         beamSize, beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
         groups, diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
         diverse = groups > 1 and not sampleWords
+        topK, topP = int(params.get("topK", 0)), float(params.get("topP", 1.0))
+        truncated = sampleWords and truncates(topK, topP, self.params["vocabSize"])
         startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
         numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
         dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
@@ -274,7 +281,10 @@ class Model:
             batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
             rowOffset = (offset + first) * self.params["maxQuesCount"]
             if generated:
-                if sampleWords:
+                if truncated:
+                    answer, _, _ = self.engine.gen_dialog_truncated_sample(batch, beamLen, startToken, endToken, temperature,
+                                                                           seed, rowOffset, histWidth, maxAnsLen, topK, topP)
+                elif sampleWords:
                     answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
                                                                  rowOffset, histWidth, maxAnsLen)
                 elif diverse:
@@ -285,7 +295,9 @@ class Model:
                                                                                   endToken, histWidth, maxAnsLen)
             else:
                 self.forwardBackward(batch, True, True)                                 # :467
-                if sampleWords:                                                         # :582-594
+                if truncated:
+                    answer, _ = self.engine.gen_truncated_sample(beamLen, startToken, temperature, seed, rowOffset, topK, topP)
+                elif sampleWords:                                                       # :582-594
                     answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
                 elif diverse:
                     answer, length, score = self.engine.gen_diverse_beam_search(beamSize, groups, diversity, beamLen,
@@ -386,7 +398,7 @@ class Model:
     def openDialogs(self, dataloader, dtype="val", inds=(0,), params=None) -> "DialogSession":
         """A dialog session (DESIGN §19) on dialogs `inds` (0-based) of split `dtype`: their images and captions, and
         questions asked one round at a time with DialogSession.ask.  `params` are generateAnswers' beamSize / beamLen /
-        sampleWords / temperature for gen models, retrieveAnswers' topK for disc ones."""
+        sampleWords / temperature / topK / topP for gen models, retrieveAnswers' topK for disc ones."""
         return DialogSession(self, dataloader, dtype, inds, params or {})
 
     def openDialogPool(self, dataloader, dtype="val", capacity=128, params=None) -> "DialogPool":
@@ -407,6 +419,11 @@ class Model:
         ck = load_checkpoint(path, permutation)
         restore(self, ck, restore_adam_state)
         return ck
+
+
+def truncates(topK: int, topP: float, V: int) -> bool:
+    """whether top-k / top-p truncation changes a draw over V classes (DESIGN §23): 1 <= topK < V or topP < 1"""
+    return 1 <= topK < V or topP < 1.0
 
 
 def pick_group(length, score) -> int:
@@ -477,7 +494,11 @@ class DialogPool:
         self.temperature, self.seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
         self.beamSize, self.beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
         self.groups, self.diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
-        self.topK = int(params.get("topK", 1))
+        # topK: a disc model's retrieval list length (default 1); a gen model's top-k truncation of sampling asks (default
+        # 0, off), with topP (DESIGN §23)
+        self.topK = int(params.get("topK", 1 if self.disc else 0))
+        self.topP = float(params.get("topP", 1.0))
+        self.truncated = not self.disc and self.sampleWords and truncates(self.topK, self.topP, model.params["vocabSize"])
         self.start, self.end = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]
         self.width = dataloader.maxQuesLen
         self.maxAnsLen = dataloader.maxAnsLen
@@ -596,8 +617,12 @@ class DialogPool:
                             "topK": [{"index": int(i), "score": float(v),
                                       "answer": [int(t) for t in self.pool[i] if t != 0]} for i, v in zip(index[b], score[b])]})
         elif self.sampleWords:
-            ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature, self.seed,
-                                                      self.rowOffset)
+            if self.truncated:
+                ans, _ = self.eng.dialog_ask_truncated_slots(slots, q, self.beamLen, self.start, self.end, self.temperature,
+                                                             self.seed, self.rowOffset, self.topK, self.topP)
+            else:
+                ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature,
+                                                          self.seed, self.rowOffset)
             given = [history_answer(ans[b, 1:], self.end) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
         elif self.groups > 1:
