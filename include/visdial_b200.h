@@ -205,6 +205,21 @@ int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_
 int vd_gen_diverse_beam_search(vd_engine* e, int32_t beam_size, int32_t groups, float diversity, int32_t beam_len,
                                int32_t start_token, int32_t end_token, int32_t* answer_host, int32_t* length_host,
                                double* score_host);
+/* n-best lists with length normalisation (DESIGN §24): vd_gen_diverse_beam_search's search (groups = 1: vd_gen_beam_search's)
+ * with each group keeping its nbest best finished hypotheses instead of one.  A finished hypothesis of `length` tokens
+ * (<START> .. <END>) has l = length - 1 generated tokens and norm = score / lp(l), lp(l) = ((5 + l) / 6)^length_penalty
+ * (GNMT, Wu et al., arXiv:1609.08144), lp computed in fp64 with the host's pow and the division in IEEE fp64; score stays
+ * the summed log-probability.  A group's list holds its n best of all the <END> candidates the search met, by (norm desc,
+ * step asc, candidate asc).  Live beams, their scores and the decoder work are those of the search without lists.  A
+ * round's pick (what a dialog's history takes) is the best list head by (norm desc, group asc) among groups that finished
+ * a hypothesis.  nbest = 1 and length_penalty = 0 is vd_gen_diverse_beam_search bit for bit.
+ * answer_host (N, G, nbest, beam_len), length_host (N, G, nbest) (0: an entry never filled), score_host (N, G, nbest) and
+ * norm_host (N, G, nbest) or NULL, each list best first.
+ * Refusals as vd_gen_diverse_beam_search's, and VD_E_BADARG unless 1 <= nbest <= 32 and length_penalty is finite and
+ * >= 0. */
+int vd_gen_nbest_beam_search(vd_engine* e, int32_t beam_size, int32_t groups, float diversity, float length_penalty,
+                             int32_t nbest, int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer_host,
+                             int32_t* length_host, double* score_host, double* norm_host);
 /* Model:generateAnswers' sampling (model.lua:581-602, sampleWords = 1) for EVERY round of the last vd_encoder_forward (N =
  * B * maxQuesCount rows), entirely on the device, the decoder fed its own samples (gen.lua:63-68).  One synchronisation, at
  * the end.  Draw rule (Gumbel-max over x / temperature, counter-based Philox; see DESIGN §14): the token of step t of row r
@@ -243,6 +258,13 @@ int vd_gen_dialog_diverse_beam_search(vd_engine* e, const vd_batch* b, int32_t b
                                       int32_t beam_len, int32_t start_token, int32_t end_token, int32_t hist_width,
                                       int32_t max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
                                       int32_t* hist_host);
+/* vd_gen_dialog_beam_search's loop with vd_gen_nbest_beam_search's search: round r's history row takes the round's pick.
+ * Outputs (N, G, nbest, beam_len), (N, G, nbest) three times for the N = B * maxQuesCount rounds; hist_host and refusals as
+ * vd_gen_dialog_beam_search's and vd_gen_nbest_beam_search's. */
+int vd_gen_dialog_nbest_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size, int32_t groups, float diversity,
+                                    float length_penalty, int32_t nbest, int32_t beam_len, int32_t start_token,
+                                    int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
+                                    int32_t* length_host, double* score_host, double* norm_host, int32_t* hist_host);
 /* Truncated sampling (DESIGN §23): vd_gen_sample / vd_gen_dialog_sample with the draw restricted, at every step of every
  * row, to a prefix of the classes in the order (y desc, class asc), y = logit / temperature: the first top_k of them
  * (top_k = 0: all), then of those the shortest prefix holding top_p of their softmax mass (top_p = 1: all), measured in
@@ -363,6 +385,14 @@ int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, cons
 int vd_dialog_ask_diverse_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
                                 int32_t groups, float diversity, int32_t beam_len, int32_t start_token, int32_t end_token,
                                 int32_t* answer, int32_t* length, double* score);
+/* vd_dialog_ask_beam_slots with vd_gen_nbest_beam_search's search (DESIGN §24): answer (n, G, nbest, beam_len), length,
+ * score and norm (n, G, nbest) (norm may be NULL) in row order; each slot's history takes its row's pick.  A
+ * vd_dialog_begin session is the pool of slots 0..B-1.  Refusals, before any state changes, as vd_dialog_ask_beam_slots'
+ * and vd_gen_nbest_beam_search's. */
+int vd_dialog_ask_nbest_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                              int32_t groups, float diversity, float length_penalty, int32_t nbest, int32_t beam_len,
+                              int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length, double* score,
+                              double* norm);
 /* vd_dialog_ask_sample_slots with vd_gen_truncated_sample's draw (DESIGN §23): answer (n, beam_len + 1), logp (n, beam_len)
  * or NULL in row order.  A vd_dialog_begin session is the pool of slots 0..B-1.  Refusals, before any state changes, as
  * vd_dialog_ask_sample_slots' and vd_gen_truncated_sample's. */

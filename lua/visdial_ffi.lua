@@ -46,6 +46,9 @@ int vd_gen_beam_search(vd_engine* e, int32_t beam_size, int32_t beam_len, int32_
 int vd_gen_diverse_beam_search(vd_engine* e, int32_t beam_size, int32_t groups, float diversity, int32_t beam_len,
                                int32_t start_token, int32_t end_token, int32_t* answer_host, int32_t* length_host,
                                double* score_host);
+int vd_gen_nbest_beam_search(vd_engine* e, int32_t beam_size, int32_t groups, float diversity, float length_penalty,
+                             int32_t nbest, int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer_host,
+                             int32_t* length_host, double* score_host, double* norm_host);
 int vd_gen_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
                   int32_t* answer_host, float* logp_host);
 int vd_gen_dialog_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size, int32_t beam_len, int32_t start_token,
@@ -58,6 +61,10 @@ int vd_gen_dialog_diverse_beam_search(vd_engine* e, const vd_batch* b, int32_t b
                                       int32_t beam_len, int32_t start_token, int32_t end_token, int32_t hist_width,
                                       int32_t max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
                                       int32_t* hist_host);
+int vd_gen_dialog_nbest_beam_search(vd_engine* e, const vd_batch* b, int32_t beam_size, int32_t groups, float diversity,
+                                    float length_penalty, int32_t nbest, int32_t beam_len, int32_t start_token,
+                                    int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
+                                    int32_t* length_host, double* score_host, double* norm_host, int32_t* hist_host);
 int vd_gen_truncated_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed,
                             int64_t row_offset, int32_t top_k, float top_p, int32_t* answer_host, float* logp_host);
 int vd_gen_dialog_truncated_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
@@ -94,6 +101,10 @@ int vd_dialog_ask_pool_slots(vd_engine* e, const int32_t* slots, int32_t n, cons
 int vd_dialog_ask_diverse_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
                                 int32_t groups, float diversity, int32_t beam_len, int32_t start_token, int32_t end_token,
                                 int32_t* answer, int32_t* length, double* score);
+int vd_dialog_ask_nbest_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                              int32_t groups, float diversity, float length_penalty, int32_t nbest, int32_t beam_len,
+                              int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length, double* score,
+                              double* norm);
 int vd_dialog_ask_truncated_slots(vd_engine* e, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq,
                                   int32_t beam_len, int32_t start_token, int32_t end_token, float temperature, uint64_t seed,
                                   int64_t row_offset, int32_t top_k, float top_p, int32_t* answer, float* logp);

@@ -122,6 +122,8 @@ SIGNATURES = {
     "vd_gen_beam_search": [_H, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gen_diverse_beam_search": [_H, C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                    C.c_void_p, C.c_void_p],
+    "vd_gen_nbest_beam_search": [_H, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gen_sample": [_H, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_void_p, C.c_void_p],
     "vd_gen_dialog_beam_search": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
@@ -129,6 +131,9 @@ SIGNATURES = {
                              C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_gen_dialog_diverse_beam_search": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_float, C.c_int32, C.c_int32, C.c_int32,
                                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_gen_dialog_nbest_beam_search": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_int32, C.c_int32,
+                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p],
     "vd_gen_truncated_sample": [_H, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64, C.c_int32, C.c_float, C.c_void_p,
                                 C.c_void_p],
     "vd_gen_dialog_truncated_sample": [_H, _P(vd_batch), C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_uint64, C.c_int64,
@@ -159,6 +164,8 @@ SIGNATURES = {
     "vd_dialog_ask_pool_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p],
     "vd_dialog_ask_diverse_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p],
+    "vd_dialog_ask_nbest_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float,
+                                  C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     "vd_dialog_ask_truncated_slots": [_H, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_float, C.c_uint64, C.c_int64, C.c_int32, C.c_float, C.c_void_p, C.c_void_p],
     "vd_dialog_slots": [_H, C.c_void_p, _P(C.c_int32)],

@@ -3,7 +3,8 @@
 Reads the model and data as `generate` does and opens a dialog session (Model.openDialogs) on the chosen images of
 `-split`: their features and captions; each question is answered before the next is asked, and the model's own answers
 become the history the next question is answered with.  Gen models answer with generate's beam search (`-beamSize`,
-`-beamLen`; diverse with `-beamGroups` > 1 and `-diversity`, DESIGN §22) or, with `-sampleWords 1`, by sampling
+`-beamLen`; diverse with `-beamGroups` > 1 and `-diversity`, DESIGN §22; n-best lists ranked by length-normalised score
+with `-nBest` and `-lengthPenalty`, DESIGN §24) or, with `-sampleWords 1`, by sampling
 (truncated to the top `-topK` words and the top `-topP` of the probability, DESIGN §23); disc models with the best answer
 of the split's answer pool.
 
@@ -20,7 +21,9 @@ DESIGN §20), reading JSON lines on stdin and writing JSON lines on stdout:
             (a first line may carry the rounds the conversation already had: it joins at round len(history); DESIGN §21)
        {"id": "u1", "leave": true}
   out: {"id", "round", "question", "answer", ...} for each answer (with -beamGroups > 1 also "alternatives": every group's
-       finished answer as {"answer", "score"}, best first, the first being "answer"); {"id", "error"} for a refused line (an unknown image, a
+       finished answer as {"answer", "score"}, best first, the first being "answer"; with -nBest or -lengthPenalty also
+       "normScore", and with -nBest > 1 "nbest": every group's finished answers as {"answer", "score", "normScore"}, best
+       first, the first being "answer"); {"id", "error"} for a refused line (an unknown image, a
        full pool, an unknown id, a malformed history, one of maxQuesCount rounds or more, or one for an open id).  A
        conversation that has had maxQuesCount answers is left, its last answer with "done": true.
 The server reads every line available without blocking, applies its joins and leaves in arrival order, then asks every
@@ -184,6 +187,11 @@ def serve(model, dl, split: str, index: dict, params: dict, capacity: int, out=s
                         "answer": idToWords(e["answer"], dl.ind2word).strip() if e else None}
                 if e and "score" in e:
                     line["score"] = e["score"]
+                if e and "normScore" in e:
+                    line["normScore"] = e["normScore"]
+                if e and "nbest" in e:
+                    line["nbest"] = [{"answer": idToWords(x["answer"], dl.ind2word).strip(), "score": x["score"],
+                                      "normScore": x["normScore"]} for x in e["nbest"]]
                 if e and "groups" in e:
                     line["alternatives"] = [{"answer": idToWords(g["answer"], dl.ind2word).strip(), "score": g["score"]}
                                             for g in ranked_groups(e)]
@@ -228,6 +236,7 @@ def main(opt: dict, rank: int = 0, world: int = 1):
         if missing:
             raise SystemExit("image ids not in split %s: %s" % (split, missing))
         params = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "beamGroups", "diversity")}
+        params.update({k: opt[k] for k in ("lengthPenalty", "nBest") if k in opt})
         if model.params["decoder"] == "gen":         # a disc pool's topK is its retrieval list: the truncation is gen's
             params.update({k: opt[k] for k in ("topK", "topP") if k in opt})
         R = model.params["maxQuesCount"]

@@ -85,21 +85,26 @@ DIVERSE_OPTIONS = [
     ("beamGroups", 1, "Diverse beam search: groups the beam is split into (1 = plain beam search; must divide beamSize)"),
     ("diversity", 0.5, "Diverse beam search: penalty per earlier group's column that chose the same token"),
 ]
+# n-best lists (DESIGN §24): the beam search keeps each group's nBest best finished answers, ranked by length-normalised score
+NBEST_OPTIONS = [
+    ("lengthPenalty", 0.0, "Beam search: rank finished answers by score / ((5 + l) / 6)^lengthPenalty, l their tokens (0 = by score)"),
+    ("nBest", 1, "Beam search: finished answers each group keeps and reports, best first (1 to 32)"),
+]
 # truncated sampling (DESIGN §23): -sampleWords 1 draws from the top-k / top-p prefix of each step's distribution
 TRUNCATION_OPTIONS = [
     ("topK", 0, "Sampling: draw from the topK most likely words only (0 = all)"),
     ("topP", 1.0, "Sampling: draw from the fewest most likely words holding topP of the probability (1 = all)"),
 ]
-# the generate command's table: generate.lua's options above, diverse beam search, truncated sampling, and which history
-# each round is answered with
+# the generate command's table: generate.lua's options above, diverse beam search, n-best lists, truncated sampling, and
+# which history each round is answered with
 HISTORY_MODES = ("gt", "generated")
-GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + TRUNCATION_OPTIONS + [
+GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + NBEST_OPTIONS + TRUNCATION_OPTIONS + [
     ("history", "gt", "History each round is answered with: gt (the dataset's) | generated (the dialog's own answers)"),
 ]
 
-# the chat command: generate's options, diverse beam search, truncated sampling, and which images are talked about with
-# which questions
-CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + TRUNCATION_OPTIONS + [
+# the chat command: generate's options, diverse beam search, n-best lists, truncated sampling, and which images are talked
+# about with which questions
+CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + NBEST_OPTIONS + TRUNCATION_OPTIONS + [
     ("split", "val", "Split the images and captions come from"),
     ("imageIds", "", "Comma-separated COCO image ids of the split (default: the -questions file's, else its first image)"),
     ("questions", "", "JSON {image_id: [question, ...]}: ask these and write results.json; else read stdin, one per line"),
@@ -162,6 +167,13 @@ def parse(options, argv=None, prog=None) -> dict:
             fail("-beamGroups must be at least 1 and divide -beamSize")
         if not math.isfinite(opt["diversity"]) or opt["diversity"] < 0:
             fail("-diversity must be finite and >= 0")
+    if "nBest" in opt:
+        if not math.isfinite(opt["lengthPenalty"]) or opt["lengthPenalty"] < 0:
+            fail("-lengthPenalty must be finite and >= 0")
+        if not 1 <= opt["nBest"] <= 32:
+            fail("-nBest must be in [1, 32]")
+        if opt["lengthPenalty"] == 0 and opt["nBest"] == 1:   # options that change nothing leave the run's options as they were
+            del opt["lengthPenalty"], opt["nBest"]
     if "topK" in opt:
         if opt["topK"] < 0:
             fail("-topK must be >= 0")
@@ -196,12 +208,15 @@ def truncated_sampling(opt: dict) -> bool:
 
 def written_opts(opt: dict) -> dict:
     """The options a results.json records: the diverse beam search options only when they change the search
-    (-beamGroups > 1), and the truncation options only when they truncate a sampling run (-sampleWords 1 with -topK > 0 or
-    -topP < 1), so that every run without them writes the file it wrote before they existed."""
+    (-beamGroups > 1), the n-best options only when one differs from its default (-lengthPenalty 0, -nBest 1), and the
+    truncation options only when they truncate a sampling run (-sampleWords 1 with -topK > 0 or -topP < 1), so that every
+    run without them writes the file it wrote before they existed."""
     plain = opt.get("beamGroups", 1) == 1
     untruncated = not truncated_sampling(opt)
+    unlisted = all(opt.get(n, d) == d for n, d, _ in NBEST_OPTIONS)
     return {k: v for k, v in opt.items()
-            if not (plain and k in ("beamGroups", "diversity")) and not (untruncated and k in ("topK", "topP"))}
+            if not (plain and k in ("beamGroups", "diversity")) and not (untruncated and k in ("topK", "topP"))
+            and not (unlisted and k in ("lengthPenalty", "nBest"))}
 
 
 def model_params(opt: dict) -> dict:

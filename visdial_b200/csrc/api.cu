@@ -282,6 +282,22 @@ int vd_gen_diverse_beam_search(vd_engine* h, int32_t beam_size, int32_t groups, 
   })
 }
 
+static vd::NBestCfg nbest_cfg(float length_penalty, int32_t nbest, double* norm_host) {
+  vd::NBestCfg c;
+  c.alpha = length_penalty;
+  c.nbest = nbest;
+  c.norm_host = norm_host;
+  return c;
+}
+int vd_gen_nbest_beam_search(vd_engine* h, int32_t beam_size, int32_t groups, float diversity, float length_penalty,
+                             int32_t nbest, int32_t beam_len, int32_t start_token, int32_t end_token, int32_t* answer_host,
+                             int32_t* length_host, double* score_host, double* norm_host) {
+  VD_TRY({
+    ENG(h)->gen_beam_search(beam_size, groups, diversity, beam_len, start_token, end_token, answer_host, length_host, score_host,
+                            nbest_cfg(length_penalty, nbest, norm_host));
+  })
+}
+
 int vd_gen_sample(vd_engine* h, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed, int64_t row_offset,
                   int32_t* answer_host, float* logp_host) {
   VD_TRY({ ENG(h)->gen_sample(beam_len, start_token, temperature, seed, row_offset, answer_host, logp_host); })
@@ -300,6 +316,15 @@ int vd_gen_dialog_diverse_beam_search(vd_engine* h, const vd_batch* b, int32_t b
                                       int32_t* hist_host) {
   VD_TRY({ ENG(h)->gen_dialog_beam_search(b, beam_size, groups, diversity, beam_len, start_token, end_token, hist_width,
                                           max_ans_len, answer_host, length_host, score_host, hist_host); })
+}
+
+int vd_gen_dialog_nbest_beam_search(vd_engine* h, const vd_batch* b, int32_t beam_size, int32_t groups, float diversity,
+                                    float length_penalty, int32_t nbest, int32_t beam_len, int32_t start_token,
+                                    int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
+                                    int32_t* length_host, double* score_host, double* norm_host, int32_t* hist_host) {
+  VD_TRY({ ENG(h)->gen_dialog_beam_search(b, beam_size, groups, diversity, beam_len, start_token, end_token, hist_width,
+                                          max_ans_len, answer_host, length_host, score_host, hist_host,
+                                          nbest_cfg(length_penalty, nbest, norm_host)); })
 }
 
 int vd_gen_dialog_sample(vd_engine* h, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,
@@ -436,6 +461,15 @@ int vd_dialog_ask_diverse_slots(vd_engine* h, const int32_t* slots, int32_t n, c
   VD_TRY({
     ENG(h)->dialog_ask_beam(slots, n, ques, Tq, beam_size, groups, diversity, beam_len, start_token, end_token, answer, length,
                             score);
+  })
+}
+int vd_dialog_ask_nbest_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_size,
+                              int32_t groups, float diversity, float length_penalty, int32_t nbest, int32_t beam_len,
+                              int32_t start_token, int32_t end_token, int32_t* answer, int32_t* length, double* score,
+                              double* norm) {
+  VD_TRY({
+    ENG(h)->dialog_ask_beam(slots, n, ques, Tq, beam_size, groups, diversity, beam_len, start_token, end_token, answer, length,
+                            score, nbest_cfg(length_penalty, nbest, norm));
   })
 }
 int vd_dialog_ask_sample_slots(vd_engine* h, const int32_t* slots, int32_t n, const int32_t* ques, int32_t Tq, int32_t beam_len,

@@ -214,6 +214,7 @@ Engine::~Engine() {
   for (auto& g : stage) g.release();
   for (auto& g : dense_buf) g.release();
   dialog_hist.release();
+  beam_lp.release();
   for (auto& g : dialog_out) g.release();
   if (copy_stream) {
     cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream);
@@ -1738,26 +1739,43 @@ void Engine::gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float
 }
 
 // Model:generateAnswers' beam search (model.lua:472-579) for all N rounds of the last encoder forward at once; with G > 1
-// groups, diverse beam search (DESIGN §22).
+// groups, diverse beam search (DESIGN §22); with nc, n-best lists (DESIGN §24).
 void Engine::gen_beam_search(int k, int G, float lam, int L, int start_token, int end_token, int32_t* answer_host,
-                             int32_t* length_host, double* score_host) {
+                             int32_t* length_host, double* score_host, const NBestCfg& nc) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_search needs the gen decoder after encoder_forward");
-  check_beam_args(k, G, lam, L);
+  check_beam_args(k, G, lam, L, nc);
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
-  const int64_t NG = db.N * G;
-  const BeamResult res = beam_search_rows(db.N, 1, 0, k, G, lam, L, start_token, end_token);
+  const int64_t NG = db.N * G * nc.nbest;
+  const double* lp = length_penalty_table(nc.alpha, L);
+  const BeamResult res = beam_search_rows(db.N, 1, 0, k, G, lam, L, start_token, end_token, nc.nbest, lp);
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.gans, (size_t)NG * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.glen, (size_t)NG * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.gscore, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  if (nc.norm_host)
+    VD_CUDA_CHECK(cudaMemcpyAsync(nc.norm_host, res.gnorm, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
-void Engine::check_beam_args(int k, int G, float lam, int L) const {
+void Engine::check_beam_args(int k, int G, float lam, int L, const NBestCfg& nc) const {
+  VD_REQUIRE(nc.nbest >= 1 && nc.nbest <= 32, VD_E_BADARG, "nbest in [1, 32]");
+  VD_REQUIRE(std::isfinite(nc.alpha) && nc.alpha >= 0.f, VD_E_BADARG, "length_penalty finite and >= 0");
   VD_REQUIRE(k >= 1 && k <= 32 && k <= cfg.V && L >= 2, VD_E_BADARG, "beam_size in [1, min(32, vocabSize)], beam_len >= 2");
   VD_REQUIRE(G >= 1 && k % G == 0, VD_E_BADARG, "groups >= 1 and a divisor of beam_size");
   VD_REQUIRE(std::isfinite(lam) && lam >= 0.f, VD_E_BADARG, "diversity finite and >= 0");
+}
+
+// lp(l) = ((5 + l) / 6)^alpha (Wu et al., arXiv:1609.08144) for l = 0 .. L-1, in fp64 with the C library's pow, so that a
+// host twin calling the same pow gets the same bits; the device never calls pow.  The copy is from pageable memory: it
+// has left `t` when cudaMemcpyAsync returns.  alpha 0: null, every lp is exactly 1.
+const double* Engine::length_penalty_table(float alpha, int L) {
+  if (alpha == 0.f) return nullptr;
+  std::vector<double> t(L);
+  for (int l = 0; l < L; ++l) t[l] = std::pow((5.0 + l) / 6.0, (double)alpha);
+  double* d = (double*)beam_lp.ensure((size_t)L * sizeof(double));
+  VD_CUDA_CHECK(cudaMemcpyAsync(d, t.data(), (size_t)L * sizeof(double), cudaMemcpyHostToDevice, cx.stream));
+  return d;
 }
 
 // The search itself, enqueued on cx.stream, for n rounds whose start state is row i * stride + off of the last encoder
@@ -1765,9 +1783,10 @@ void Engine::check_beam_args(int k, int G, float lam, int L) const {
 // tokens and parents: the state gather, the decoder step of gen_decoder_step_logits, the fused log-softmax + top-k and the
 // candidate merge, which writes the next step's tokens and parents.  The merge fills G groups of k / G columns in order,
 // penalising the tokens earlier groups chose (DESIGN §22); its top-k input is the same k per row at any G.  Returns each
-// group's best finished hypothesis and each round's pick in the arena, valid until the next encoder forward.
+// group's list of its nbest best finished hypotheses by norm (lp: the length-penalty table, DESIGN §24) and each round's
+// pick in the arena, valid until the next encoder forward.
 Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int G, float lam, int L,
-                                            int start_token, int end_token) {
+                                            int start_token, int end_token, int nbest, const double* lp) {
   forward_connect();
   const int H = cfg.H;
   const int64_t N = n, rows = N * k;
@@ -1783,16 +1802,30 @@ Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t o
   int32_t* parent = arena.get<int32_t>(rows);
   float* tv = arena.get<float>(rows * k);
   int32_t* ti = arena.get<int32_t>(rows * k);
-  int32_t* ans = arena.get<int32_t>(N * G * L);
-  int32_t* ans_len = arena.get<int32_t>(N * G);
-  double* ans_score = arena.get<double>(N * G);
-  VD_CUDA_CHECK(cudaMemsetAsync(ans, 0, (size_t)N * G * L * sizeof(int32_t), cx.stream));
-  VD_CUDA_CHECK(cudaMemsetAsync(ans_len, 0, (size_t)N * G * sizeof(int32_t), cx.stream));
-  VD_CUDA_CHECK(cudaMemsetAsync(ans_score, 0, (size_t)N * G * sizeof(double), cx.stream));
-  // G > 1: the last step's merge also writes each round's pick
-  BeamResult res = {ans, ans_len, ans_score, ans, ans_len, ans_score};
-  if (G > 1) { res.ans = arena.get<int32_t>(N * L); res.len = arena.get<int32_t>(N); res.score = arena.get<double>(N); }
-  int32_t* pick_ans = G > 1 ? res.ans : nullptr;
+  // the lists' slots (a slot's tokens past its length stay 0); the norms and the order are read only where filled
+  const int64_t NL = N * G * nbest;
+  BeamLists lists;
+  lists.nbest = nbest;
+  lists.lp = lp;
+  lists.ans = arena.get<int32_t>(NL * L);
+  lists.len = arena.get<int32_t>(NL);
+  lists.score = arena.get<double>(NL);
+  VD_CUDA_CHECK(cudaMemsetAsync(lists.ans, 0, (size_t)NL * L * sizeof(int32_t), cx.stream));
+  VD_CUDA_CHECK(cudaMemsetAsync(lists.len, 0, (size_t)NL * sizeof(int32_t), cx.stream));
+  VD_CUDA_CHECK(cudaMemsetAsync(lists.score, 0, (size_t)NL * sizeof(double), cx.stream));
+  if (lp || nbest > 1) lists.norm = arena.get<double>(NL);
+  BeamResult res = {lists.ans, lists.len, lists.score, lists.ans, lists.len, lists.score, lists.norm ? lists.norm : lists.score};
+  if (nbest > 1) {                                 // the last step's merge writes the lists in order
+    lists.ord = arena.get<int32_t>(NL);
+    res.gans = lists.out_ans = arena.get<int32_t>(NL * L);
+    res.glen = lists.out_len = arena.get<int32_t>(NL);
+    res.gscore = lists.out_score = arena.get<double>(NL);
+    res.gnorm = lists.out_norm = arena.get<double>(NL);
+  }
+  // G > 1 or nbest > 1: the last step's merge also writes each round's pick
+  const bool pick = G > 1 || nbest > 1;
+  if (pick) { res.ans = arena.get<int32_t>(N * L); res.len = arena.get<int32_t>(N); res.score = arena.get<double>(N); }
+  int32_t* pick_ans = pick ? res.ans : nullptr;
   // model.lua:478-503: h = {layer-1 h at Tq, encOut}, c = {layer-1 c, layer-2 c}, each round's row repeated k times.  Encoders
   // without .rnnLayers feed explicit zero rows, not "no initial state": the first step's kernels differ between the two.
   const float* init[4] = {gen_h0[0], gen_h0[1], gen_c0[0], gen_c0[1]};
@@ -1816,8 +1849,8 @@ Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t o
     const int a = (stp - 1) & 1;
     // the top-k lists, the scores and beams in and out
     LaunchCtx::Scope sc(&cx, "beam_merge", 0.0, 8.0 * rows * k + 16.0 * rows + 8.0 * rows * (stp + 1));
-    beam_merge(cx, N, stp, k, G, lam, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, ans,
-               ans_len, ans_score, pick_ans, pick_ans ? res.len : nullptr, pick_ans ? res.score : nullptr);
+    beam_merge(cx, N, stp, k, G, lam, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, lists,
+               pick_ans, pick_ans ? res.len : nullptr, pick_ans ? res.score : nullptr);
   }
   return res;
 }
@@ -1971,27 +2004,34 @@ static void scatter_round(cudaStream_t s, void* dst, const void* src, size_t byt
 
 void Engine::gen_dialog_beam_search(const vd_batch* b, int k, int G, float lam, int L, int start_token, int end_token, int W,
                                     int max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
-                                    int32_t* hist_host) {
+                                    int32_t* hist_host, const NBestCfg& nc) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_beam_search needs the gen decoder");
-  check_beam_args(k, G, lam, L);
+  check_beam_args(k, G, lam, L, nc);
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
   const int R = cfg.R;
-  const int64_t B = b->B, NG = B * R * G;
+  const int64_t Gn = (int64_t)G * nc.nbest;        // list entries per round
+  const int64_t B = b->B, NG = B * R * Gn;
   int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)NG * L * sizeof(int32_t));
   int32_t* len = (int32_t*)dialog_out[1].ensure((size_t)NG * sizeof(int32_t));
   double* score = (double*)dialog_out[2].ensure((size_t)NG * sizeof(double));
+  double* norm = nc.norm_host ? (double*)dialog_out[3].ensure((size_t)NG * sizeof(double)) : nullptr;
+  VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+  cx.stream = main_stream;
+  const double* lp = length_penalty_table(nc.alpha, L);
   gen_dialog(b, W, max_ans_len, [&](int r) {
-    const BeamResult res = beam_search_rows(B, R, r, k, G, lam, L, start_token, end_token);
-    scatter_round(cx.stream, ans, res.gans, (size_t)G * L * sizeof(int32_t), R, r, B);
-    scatter_round(cx.stream, len, res.glen, (size_t)G * sizeof(int32_t), R, r, B);
-    scatter_round(cx.stream, score, res.gscore, (size_t)G * sizeof(double), R, r, B);
+    const BeamResult res = beam_search_rows(B, R, r, k, G, lam, L, start_token, end_token, nc.nbest, lp);
+    scatter_round(cx.stream, ans, res.gans, (size_t)Gn * L * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, len, res.glen, (size_t)Gn * sizeof(int32_t), R, r, B);
+    scatter_round(cx.stream, score, res.gscore, (size_t)Gn * sizeof(double), R, r, B);
+    if (norm) scatter_round(cx.stream, norm, res.gnorm, (size_t)Gn * sizeof(double), R, r, B);
     // the pick's tokens between <START> and the hypothesis' <END>
     return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
   }, hist_host);
   VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, ans, (size_t)NG * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(length_host, len, (size_t)NG * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(score_host, score, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+  if (norm) VD_CUDA_CHECK(cudaMemcpyAsync(nc.norm_host, norm, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
 }
 
@@ -2545,19 +2585,23 @@ static void run_ask(Engine* e, const int32_t* slots, int64_t n, const int32_t* q
 }
 
 void Engine::dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int G, float lam, int L,
-                             int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host) {
+                             int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host,
+                             const NBestCfg& nc) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a beam-search ask needs the gen decoder");
-  check_beam_args(k, G, lam, L);
+  check_beam_args(k, G, lam, L, nc);
   VD_REQUIRE(start_token >= 1 && start_token <= cfg.V && end_token >= 1 && end_token <= cfg.V, VD_E_BADARG,
              "start_token and end_token in [1, vocabSize]");
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   dialog_check_ask(slots, n, ques_host, Tq);
   run_ask(this, slots, n, ques_host, Tq, 0, [&](const AskRows&) {
-    const BeamResult res = beam_search_rows(n, 1, 0, k, G, lam, L, start_token, end_token);
-    const size_t nG = (size_t)n * G;
+    const BeamResult res = beam_search_rows(n, 1, 0, k, G, lam, L, start_token, end_token, nc.nbest,
+                                            length_penalty_table(nc.alpha, L));
+    const size_t nG = (size_t)n * G * nc.nbest;
     VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.gans, nG * L * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
     VD_CUDA_CHECK(cudaMemcpyAsync(length_host, res.glen, nG * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
     VD_CUDA_CHECK(cudaMemcpyAsync(score_host, res.gscore, nG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
+    if (nc.norm_host)
+      VD_CUDA_CHECK(cudaMemcpyAsync(nc.norm_host, res.gnorm, nG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
     return DialogAnswers{res.ans + 1, L, res.len, 0, end_token};
   });
 }

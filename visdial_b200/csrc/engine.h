@@ -130,6 +130,11 @@ struct GrowBuf {
   void release();
 };
 
+// a beam search's n-best lists (DESIGN §24): each group keeps its nbest best finished hypotheses by score / lp(length - 1),
+// lp(l) = ((5 + l) / 6)^alpha; the default (0, 1) is the best finished hypothesis by score.  norm_host: the norms' copy,
+// or null.
+struct NBestCfg { float alpha = 0.f; int nbest = 1; double* norm_host = nullptr; };
+
 struct Engine {
   Cfg cfg;
   Layout lay;
@@ -324,15 +329,19 @@ struct Engine {
   // its core on device-resident tokens, up to the vocabulary projection: gstep_logp holds the LOGITS on return
   void gen_decoder_step_logits(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // Model:generateAnswers' beam search for every round of the last encoder forward, entirely on the device; G groups of
-  // k / G with diversity lam (DESIGN §22; G = 1: the reference's search).  Outputs (N, G, L), (N, G), (N, G).
+  // k / G with diversity lam (DESIGN §22; G = 1: the reference's search).  Outputs (N, G, nbest, L), (N, G, nbest) twice.
   void gen_beam_search(int k, int G, float lam, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
-                       double* score_host);
-  void check_beam_args(int k, int G, float lam, int L) const;
+                       double* score_host, const NBestCfg& nc = {});
+  void check_beam_args(int k, int G, float lam, int L, const NBestCfg& nc = {}) const;
+  // lp[0 .. L-1] on the device, computed with the host's pow once per call (null for alpha 0: every lp is 1)
+  GrowBuf beam_lp;
+  const double* length_penalty_table(float alpha, int L);
   // its search on n rounds whose start state is row i * stride + off of the last encoder forward; results in the arena:
-  // the pick (n, L), (n), (n) (the best group's answer) and every group's (n, G, L), (n, G), (n, G); G = 1: the same arrays
-  struct BeamResult { int32_t* ans; int32_t* len; double* score; int32_t* gans; int32_t* glen; double* gscore; };
+  // the pick (n, L), (n), (n) (the best list head's answer) and every group's ordered list (n, G, nbest, L), (n, G, nbest)
+  // three times (gnorm is gscore when lp is null and nbest is 1); G = 1 and nbest = 1: the pick is the list
+  struct BeamResult { int32_t* ans; int32_t* len; double* score; int32_t* gans; int32_t* glen; double* gscore; double* gnorm; };
   BeamResult beam_search_rows(int64_t n, int64_t stride, int64_t off, int k, int G, float lam, int L, int start_token,
-                              int end_token);
+                              int end_token, int nbest = 1, const double* lp = nullptr);
   // the decoder step up to the second LSTM layer (gstep1 / gstep2 hold the new state on return)
   void gen_decoder_step_lstm(int64_t rows, const int32_t* tok, const float* const* h_prev, const float* const* c_prev);
   // Model:generateAnswers' sampling for every round of the last encoder forward, entirely on the device
@@ -360,7 +369,7 @@ struct Engine {
   void gen_dialog(const vd_batch* b, int W, int max_ans_len, const std::function<DialogAnswers(int)>& search, int32_t* hist_host);
   void gen_dialog_beam_search(const vd_batch* b, int k, int G, float lam, int L, int start_token, int end_token, int W,
                               int max_ans_len, int32_t* answer_host, int32_t* length_host, double* score_host,
-                              int32_t* hist_host);
+                              int32_t* hist_host, const NBestCfg& nc = {});
   void gen_dialog_sample(const vd_batch* b, int L, int start_token, int end_token, float temperature, uint64_t seed,
                          int64_t row_offset, int W, int max_ans_len, int32_t* answer_host, float* logp_host, int32_t* hist_host,
                          const TruncCfg& tr = {});
@@ -416,7 +425,8 @@ struct Engine {
   AskRows dialog_encode(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int64_t row_offset);
   void dialog_finish(const AskRows& rows, const DialogAnswers& a);   // the rows' history append
   void dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int k, int G, float lam, int L,
-                       int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host);
+                       int start_token, int end_token, int32_t* answer_host, int32_t* length_host, double* score_host,
+                       const NBestCfg& nc = {});
   // row i draws as global round row_offset + draw_base[slots[i]] + its round
   void dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* ques_host, int Tq, int L, int start_token, int end_token,
                          float temperature, uint64_t seed, int64_t row_offset, int32_t* answer_host, float* logp_host,

@@ -189,14 +189,26 @@ void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mas
                           int32_t* topi);
 // the whole search on the device (Engine::gen_beam_search): beams (rows, L) = <start> then pads, tokens = <start>, scores = 0
 void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* beams, int32_t* tokens, double* scores);
+// Each group's list of its n best finished hypotheses (DESIGN §24), ordered by (norm desc, step asc, candidate asc), norm =
+// score / lp(length - 1).  The merge keeps the entries in slots: ans (N, G, n, L), len (N, G, n) (0: never filled; slots
+// fill in order 0, 1, ..), score (N, G, n), norm (N, G, n), and ord (N, G, n) the slot at each list position.  At the last
+// step it writes the lists in order to out_* (N, G, n, ...).  n = 1: the slot is the list, ord and out_* are null.
+struct BeamLists {
+  int nbest = 1;
+  const double* lp = nullptr;     // lp[l], l = 0 .. L-1, or null: every lp is 1 (length penalty 0)
+  int32_t* ans = nullptr; int32_t* len = nullptr; double* score = nullptr;
+  double* norm = nullptr;         // null (only with lp null): the norm is the score
+  int32_t* ord = nullptr;
+  int32_t* out_ans = nullptr; int32_t* out_len = nullptr; double* out_score = nullptr; double* out_norm = nullptr;
+};
 // the candidate merge of step stp for N rounds of k hypotheses in G groups of k / G (model.lua:529-569; diverse beam search
-// with Hamming diversity lam for G > 1, DESIGN §22): next beams / scores / tokens / parents, and each group's best finished
-// hypothesis (ans (N, G, L), ans_len (N, G) = 0 while there is none, ans_score (N, G)).  pick_* (N, L), (N), (N) or all
-// null: at the last step (stp == L - 1), the best of each round's G answers by (score desc, group asc)
+// with Hamming diversity lam for G > 1, DESIGN §22): next beams / scores / tokens / parents, and each group's list of
+// finished hypotheses (DESIGN §24; n = 1, lp null: its best finished hypothesis, len 0 while there is none).  pick_* (N, L),
+// (N), (N) or all null: at the last step (stp == L - 1), the best of each round's G list heads by (norm desc, group asc)
 void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int L, int end_token, const float* topv,
                 const int32_t* topi, const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out,
-                int32_t* tokens, int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score, int32_t* pick_ans,
-                int32_t* pick_len, double* pick_score);
+                int32_t* tokens, int32_t* parent, const BeamLists& lists, int32_t* pick_ans, int32_t* pick_len,
+                double* pick_score);
 // the sampling step from materialised logits, one block per row: lse from the same row_lse as logsoftmax_rows (so logp is
 // the bits it would give), the Gumbel-max draw of common.cuh; writes as vocab_sample_finish
 void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,

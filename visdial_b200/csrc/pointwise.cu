@@ -1362,25 +1362,29 @@ __global__ void __launch_bounds__(256) k_truncated_sample_rows(const float* __re
 //    classes from its k top-k entries by (augmented desc, top-k position asc), augmented = (double)logp - lam * n_g(v),
 //    n_g(v) = the columns of groups < g filled at this step with token v.  Group 0 has no penalties: its explored set is
 //    the first w entries.  Candidate q = e*w + j is the j-th of them (G = 1: q = c*k + j, the reference's order).
-//  - Candidates whose token is end_token compete for group g's best finished hypothesis, unpenalised score
-//    s = scores[c] + logp in fp64 (strictly greater replaces: the first maximum in (step, q) order wins, as the
-//    reference's stable sort keeps it).
+//  - Candidates whose token is end_token enter group g's list of finished hypotheses (DESIGN §24) by their norm
+//    x = s / lp[stp] (IEEE fp64 division; lp null: x = s), s = scores[c] + logp in fp64 unpenalised: the list keeps the n
+//    best by (x desc, step asc, q asc).  Rounds take the step's finished candidates best first by (x desc, q asc), each
+//    strictly after the last round's; a ballot over the list (lane i holds position i) gives a candidate's position, and the
+//    rounds stop at the first that would land at position >= n.  A new entry's tokens go to a free slot or to the slot of
+//    the evicted n-th entry, which is from an earlier step (so shorter, every token overwritten): no row moves, and only
+//    the order array ord changes.  n = 1 with lp null is the reference's rule: the first maximum in (step, q) order.
 //  - The others are ranked by (a desc, q asc), a = s - lam * n_g(v), and the first min(#, w) fill the group's columns
 //    from the PRE-merge beams; a column stores the unpenalised s.  A column left unfilled keeps its beam and score, and
 //    is fed next step the state it was fed this step (parent -1 - row) and its beam's next position (a pad, 0).
 // Penalties only lower a score and group g's penalised tokens number at most g*w, so the w best classes of a row under
 // the penalty lie inside its unpenalised top k: the decoder's top-k list holds every class DBS could pick.  The products
-// lam * n are __dmul_rn so that no fused multiply-add changes a's rounding.  beams: (N, k, L) token histories; ans
-// (N, G, L), ans_len / ans_score (N, G).  pick_* (N, L), (N), (N), or null: at the last step (stp == L - 1) the best of
-// the G answers by (score desc, group asc), groups without a finished hypothesis skipped (pick_len 0 when none).
-__global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float lam, int L, int end_token,
+// lam * n are __dmul_rn so that no fused multiply-add changes a's rounding.  beams: (N, k, L) token histories; lists as
+// BeamLists says.  At the last step (stp == L - 1) the lists are written in order to out_* (n > 1), and pick_* (N, L),
+// (N), (N), or null, take the best of the G list heads by (x desc, group asc), groups without a finished hypothesis skipped
+// (pick_len 0 when none).
+__global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float lam, int L, int end_token, const BeamLists lst,
                                                    const float* __restrict__ topv, const int32_t* __restrict__ topi,
                                                    const double* __restrict__ sc_in, double* __restrict__ sc_out,
                                                    const int32_t* __restrict__ beams_in, int32_t* __restrict__ beams_out,
                                                    int32_t* __restrict__ tokens, int32_t* __restrict__ parent,
-                                                   int32_t* __restrict__ ans, int32_t* __restrict__ ans_len,
-                                                   double* __restrict__ ans_score, int32_t* __restrict__ pick_ans,
-                                                   int32_t* __restrict__ pick_len, double* __restrict__ pick_score) {
+                                                   int32_t* __restrict__ pick_ans, int32_t* __restrict__ pick_len,
+                                                   double* __restrict__ pick_score) {
   // per column: the filling candidate's source column, its token (0: unfilled) and its stored score
   __shared__ int win_c[32], win_t[32];
   __shared__ double win_s[32];
@@ -1388,7 +1392,12 @@ __global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float 
   // and penalty count
   __shared__ double e_aug[16 * 32];
   __shared__ unsigned char e_cnt[16 * 32], c_pos[16 * 16], c_cnt[16 * 16];
+  __shared__ int s_ord[32];                                // the last step: a list's slot at each position
   const int n = blockIdx.x, lane = threadIdx.x;
+  const int nb = lst.nbest;
+  const double lpv = lst.lp ? lst.lp[stp] : 1.0;         // every candidate of this step has l = stp generated tokens
+  const bool last = stp == L - 1;
+  int best = -1, bslot = 0; double bnorm = 0.0;          // the pick so far (warp-uniform)
   const int w = k / G;
   const int ne = stp == 1 ? 1 : w;                       // explored columns per group
   const int ncand = ne * w;
@@ -1423,28 +1432,72 @@ __global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float 
     // candidate q of group g: its top-k entry (column c0 + q / w), and its penalty count
     const auto entry = [&](int q) { return (c0 + q / w) * k + (g ? (int)c_pos[q] : q % w); };
     const auto count = [&](int q) { return g ? (int)c_cnt[q] : 0; };
-    // finished hypotheses of this step: the first maximum, then against the group's best so far
-    bool fnd = false; double fs = 0.0; int fq = 0x7fffffff;
-    for (int q = lane; q < ncand; q += 32) {
-      const int idx = entry(q);
-      if (ti[idx] + 1 != end_token) continue;
-      const double s = sc[idx / k] + (double)tv[idx];
-      if (!fnd || s > fs) { fnd = true; fs = s; fq = q; }
+    // finished hypotheses of this step into the group's list: lane i holds position i's slot and norm, m positions are
+    // filled (slots fill in order, so slots 0 .. m-1 are the filled ones)
+    const int64_t lb = ((int64_t)n * G + g) * nb;          // the group's first slot
+    int m = __popc(__ballot_sync(FULL, lane < nb && lst.len[lb + lane] > 0));
+    int pslot = 0; double pnorm = 0.0;
+    if (lane < m) {
+      pslot = lst.ord ? lst.ord[lb + lane] : lane;
+      pnorm = lst.norm ? lst.norm[lb + pslot] : lst.score[lb + pslot];
     }
+    __syncwarp();                                          // every lane has read the list before a round writes it
+    double xn = INFINITY; int xq = -1;                     // the last round's candidate
+    for (;;) {
+      bool fnd = false; double fx = 0.0, fs = 0.0; int fq = 0x7fffffff;
+      for (int q = lane; q < ncand; q += 32) {
+        const int idx = entry(q);
+        if (ti[idx] + 1 != end_token) continue;
+        const double s = sc[idx / k] + (double)tv[idx];
+        const double x = __ddiv_rn(s, lpv);
+        if (!(x < xn || (x == xn && q > xq))) continue;
+        if (!fnd || x > fx) { fnd = true; fx = x; fs = s; fq = q; }
+      }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const bool of = __shfl_xor_sync(FULL, fnd, o);
-      const double os = __shfl_xor_sync(FULL, fs, o);
-      const int oq = __shfl_xor_sync(FULL, fq, o);
-      if (of && (!fnd || os > fs || (os == fs && oq < fq))) { fnd = true; fs = os; fq = oq; }
-    }
-    const int64_t ng = (int64_t)n * G + g;
-    const bool better = fnd && (ans_len[ng] == 0 || fs > ans_score[ng]);    // warp-uniform
-    __syncwarp();                                          // every lane has read the best so far before lane 0 replaces it
-    if (better) {
+      for (int o = 16; o > 0; o >>= 1) {
+        const bool of = __shfl_xor_sync(FULL, fnd, o);
+        const double ox = __shfl_xor_sync(FULL, fx, o);
+        const double os = __shfl_xor_sync(FULL, fs, o);
+        const int oq = __shfl_xor_sync(FULL, fq, o);
+        if (of && (!fnd || ox > fx || (ox == fx && oq < fq))) { fnd = true; fx = ox; fs = os; fq = oq; }
+      }
+      if (!fnd) break;                                     // warp-uniform
+      // after every entry of an earlier step, or of an earlier round, whose norm is not below it
+      const int pos = __popc(__ballot_sync(FULL, lane < m && pnorm >= fx));
+      if (pos >= nb) break;
+      const int slot = m < nb ? m : __shfl_sync(FULL, pslot, nb - 1);
+      const int us = __shfl_up_sync(FULL, pslot, 1);
+      const double un = __shfl_up_sync(FULL, pnorm, 1);
+      if (lane > pos) { pslot = us; pnorm = un; }
+      if (lane == pos) { pslot = slot; pnorm = fx; }
+      m = min(m + 1, nb);
       const int c = c0 + fq / w;
-      for (int p = lane; p < stp; p += 32) ans[ng * L + p] = bin[(int64_t)c * L + p];
-      if (lane == 0) { ans[ng * L + stp] = end_token; ans_len[ng] = stp + 1; ans_score[ng] = fs; }
+      int32_t* dst = lst.ans + (lb + slot) * L;
+      for (int p = lane; p < stp; p += 32) dst[p] = bin[(int64_t)c * L + p];
+      if (lane == 0) {
+        dst[stp] = end_token; lst.len[lb + slot] = stp + 1; lst.score[lb + slot] = fs;
+        if (lst.norm) lst.norm[lb + slot] = fx;
+      }
+      if (pos == nb - 1) break;                            // the next candidate would land at position n
+      xn = fx; xq = fq;
+    }
+    if (lst.ord && lane < m) lst.ord[lb + lane] = pslot;
+    const double hn = __shfl_sync(FULL, pnorm, 0);
+    const int hs = __shfl_sync(FULL, pslot, 0);
+    if (m > 0 && (best < 0 || hn > bnorm)) { best = g; bnorm = hn; bslot = hs; }
+    if (last && lst.out_ans) {                             // the list in order
+      s_ord[lane] = pslot;
+      __syncwarp();                                        // the order, and the slots' tokens other lanes wrote
+      for (int i = lane; i < nb * L; i += 32) {
+        const int ps = i / L, p = i % L;
+        lst.out_ans[(lb + ps) * L + p] = ps < m ? lst.ans[(lb + s_ord[ps]) * L + p] : 0;
+      }
+      if (lane < nb) {
+        lst.out_len[lb + lane] = lane < m ? lst.len[lb + pslot] : 0;
+        lst.out_score[lb + lane] = lane < m ? lst.score[lb + pslot] : 0.0;
+        lst.out_norm[lb + lane] = lane < m ? pnorm : 0.0;
+      }
+      __syncwarp();                                        // s_ord is the next group's
     }
     // the w best other candidates: round j takes the best one strictly after round j-1's winner
     int nfill = 0;
@@ -1487,15 +1540,10 @@ __global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float 
     sc_out[row0 + c] = win_s[c];
     parent[row0 + c] = win_t[c] ? row0 + win_c[c] : -1 - (row0 + c);
   }
-  if (pick_ans && stp == L - 1) {
-    int best = -1; double bsc = 0.0;                       // warp-uniform
-    for (int g = 0; g < G; ++g) {
-      const int64_t ng = (int64_t)n * G + g;
-      if (ans_len[ng] > 0 && (best < 0 || ans_score[ng] > bsc)) { best = g; bsc = ans_score[ng]; }
-    }
-    const int64_t nb = (int64_t)n * G + (best < 0 ? 0 : best);
-    for (int p = lane; p < L; p += 32) pick_ans[(int64_t)n * L + p] = best < 0 ? 0 : ans[nb * L + p];
-    if (lane == 0) { pick_len[n] = best < 0 ? 0 : ans_len[nb]; pick_score[n] = bsc; }
+  if (pick_ans && last) {
+    const int64_t src = ((int64_t)n * G + (best < 0 ? 0 : best)) * nb + bslot;
+    for (int p = lane; p < L; p += 32) pick_ans[(int64_t)n * L + p] = best < 0 ? 0 : lst.ans[src * L + p];
+    if (lane == 0) { pick_len[n] = best < 0 ? 0 : lst.len[src]; pick_score[n] = best < 0 ? 0.0 : lst.score[src]; }
   }
 }
 
@@ -1990,15 +2038,20 @@ void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* bea
 }
 void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int L, int end_token, const float* topv,
                 const int32_t* topi, const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out,
-                int32_t* tokens, int32_t* parent, int32_t* ans, int32_t* ans_len, double* ans_score, int32_t* pick_ans,
-                int32_t* pick_len, double* pick_score) {
+                int32_t* tokens, int32_t* parent, const BeamLists& lists, int32_t* pick_ans, int32_t* pick_len,
+                double* pick_score) {
   VD_REQUIRE(k >= 1 && k <= 32 && stp >= 1 && stp < L, VD_E_BADARG, "beam_merge: k / step");
   VD_REQUIRE(G >= 1 && k % G == 0 && std::isfinite(lam) && lam >= 0.f, VD_E_BADARG, "beam_merge: groups / diversity");
   VD_REQUIRE(!pick_ans == !pick_len && !pick_ans == !pick_score, VD_E_BADARG, "beam_merge: all pick outputs or none");
+  const BeamLists& b = lists;
+  VD_REQUIRE(b.nbest >= 1 && b.nbest <= 32 && b.ans && b.len && b.score && (b.norm || !b.lp), VD_E_BADARG,
+             "beam_merge: n in [1, 32], the list slots, and norms with a length-penalty table");
+  const bool many = b.nbest > 1;
+  VD_REQUIRE(!b.ord == !many && !b.out_ans == !many && !b.out_len == !many && !b.out_score == !many && !b.out_norm == !many &&
+             (!many || b.norm), VD_E_BADARG, "beam_merge: n > 1 takes norms, the order and every ordered output");
   if (N == 0) return;
-  k_beam_merge<<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, G, lam, L, end_token, topv, topi, scores_in, scores_out, beams_in,
-                                                  beams_out, tokens, parent, ans, ans_len, ans_score, pick_ans, pick_len,
-                                                  pick_score);
+  k_beam_merge<<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, G, lam, L, end_token, b, topv, topi, scores_in, scores_out, beams_in,
+                                                  beams_out, tokens, parent, pick_ans, pick_len, pick_score);
   check_launch(cx, "k_beam_merge");
 }
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1, float beta2,

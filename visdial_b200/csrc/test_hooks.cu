@@ -249,9 +249,23 @@ const Entry TABLE[] = {
     // k, G, L, end_token; reals diversity
     {"beam_merge", 14, 6, 1,
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       BeamLists b;
+       b.ans = I32(8); b.len = I32(9); b.score = static_cast<double*>(P[10]);
        beam_merge(e->cx, I[0], IN(1), IN(2), IN(3), (float)X[0], IN(4), IN(5), CF(0), CI32(1), static_cast<const double*>(P[2]),
-                  static_cast<double*>(P[3]), CI32(4), I32(5), I32(6), I32(7), I32(8), I32(9), static_cast<double*>(P[10]), I32(11),
-                  I32(12), static_cast<double*>(P[13]));
+                  static_cast<double*>(P[3]), CI32(4), I32(5), I32(6), I32(7), b, I32(11), I32(12), static_cast<double*>(P[13]));
+     }},
+    // as beam_merge with n-best lists (DESIGN §24): ans / ans_len / ans_score are the list slots (N, G, n, ...), and seven
+    // more ptrs: lp (L, or null), norm, ord, out_ans, out_len, out_score, out_norm (the last five null for n = 1); a seventh
+    // int n
+    {"beam_merge_nbest", 21, 7, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       BeamLists b;
+       b.nbest = IN(6);
+       b.ans = I32(8); b.len = I32(9); b.score = static_cast<double*>(P[10]);
+       b.lp = static_cast<const double*>(P[14]); b.norm = static_cast<double*>(P[15]); b.ord = I32(16);
+       b.out_ans = I32(17); b.out_len = I32(18); b.out_score = static_cast<double*>(P[19]); b.out_norm = static_cast<double*>(P[20]);
+       beam_merge(e->cx, I[0], IN(1), IN(2), IN(3), (float)X[0], IN(4), IN(5), CF(0), CI32(1), static_cast<const double*>(P[2]),
+                  static_cast<double*>(P[3]), CI32(4), I32(5), I32(6), I32(7), b, I32(11), I32(12), static_cast<double*>(P[13]));
      }},
     // ptrs logits, tokens, answer, logp; ints rows, V, L, seed, step, row_offset, row_stride; reals temperature
     {"logsoftmax_sample_rows", 4, 7, 1,

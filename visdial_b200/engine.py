@@ -405,6 +405,26 @@ class Engine:
                                                   ans.ctypes.data, length.ctypes.data, score.ctypes.data))
         return ans, length, score
 
+    def gen_nbest_beam_search(self, k: int, G: int, diversity: float, length_penalty: float, nbest: int, L: int, start: int,
+                              end: int):
+        """n-best lists of a (diverse) beam search for every round of the last encoder forward (vd_gen_nbest_beam_search,
+        DESIGN §24): each group's `nbest` best finished hypotheses by norm = score / ((5 + l) / 6)^length_penalty, l = length
+        - 1.  Returns (answer (N, G, nbest, L) int32, length (N, G, nbest) int32 — 0 for an entry never filled — score and
+        norm (N, G, nbest) float64), each list best first."""
+        N = self._enc_rows
+        if N is None:
+            raise _lib.VdError(_lib.VD_E_STATE, "gen_nbest_beam_search before encoder_forward")
+        G, nb = int(G), int(nbest)         # buffers for G, nbest >= 1; the library refuses what it cannot take
+        shape = (N, max(G, 1), max(nb, 1))
+        ans = np.zeros(shape + (int(L),), dtype=np.int32)
+        length = np.zeros(shape, dtype=np.int32)
+        score = np.zeros(shape, dtype=np.float64)
+        norm = np.zeros(shape, dtype=np.float64)
+        check(self.lib.vd_gen_nbest_beam_search(self.h, int(k), G, float(diversity), float(length_penalty), nb, int(L),
+                                                int(start), int(end), ans.ctypes.data, length.ctypes.data, score.ctypes.data,
+                                                norm.ctypes.data))
+        return ans, length, score, norm
+
     def gen_sample(self, L: int, start: int, temperature: float, seed: int, row_offset: int = 0):
         """Ancestral sampling for every round of the last encoder forward on the device (vd_gen_sample).  Returns (answer
         (N, L+1) int32 — column 0 = `start` — and logp (N, L) float32, each sample's un-tempered log-probability).  Row r's
@@ -465,6 +485,26 @@ class Engine:
                                                          hist.ctypes.data))
         self._enc_rows = B * R
         return ans, length, score, hist
+
+    def gen_dialog_nbest_beam_search(self, batch: Batch, k: int, G: int, diversity: float, length_penalty: float, nbest: int,
+                                     L: int, start: int, end: int, hist_width: int, max_ans_len: int):
+        """Dialogs on the model's own answers with n-best lists (vd_gen_dialog_nbest_beam_search): round r's history takes
+        each round's pick.  Returns (answer (N, G, nbest, L), length, score, norm (N, G, nbest), history rows (B,
+        maxQuesCount, hist_width))."""
+        B, R, G, nb = batch.c.B, self.params["maxQuesCount"], int(G), int(nbest)
+        shape = (B * R, max(G, 1), max(nb, 1))
+        ans = np.zeros(shape + (int(L),), dtype=np.int32)
+        length = np.zeros(shape, dtype=np.int32)
+        score = np.zeros(shape, dtype=np.float64)
+        norm = np.zeros(shape, dtype=np.float64)
+        hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
+        self._enc_rows = None
+        check(self.lib.vd_gen_dialog_nbest_beam_search(self.h, C.byref(batch.c), int(k), G, float(diversity),
+                                                       float(length_penalty), nb, int(L), int(start), int(end),
+                                                       int(hist_width), int(max_ans_len), ans.ctypes.data, length.ctypes.data,
+                                                       score.ctypes.data, norm.ctypes.data, hist.ctypes.data))
+        self._enc_rows = B * R
+        return ans, length, score, norm, hist
 
     def gen_dialog_sample(self, batch: Batch, L: int, start: int, end: int, temperature: float, seed: int, row_offset: int,
                           hist_width: int, max_ans_len: int):
@@ -711,6 +751,24 @@ class Engine:
                                                    length.ctypes.data, score.ctypes.data))
         self._dialog_rows = n
         return ans, length, score
+
+    def dialog_ask_nbest_slots(self, slots, ques, k: int, G: int, diversity: float, length_penalty: float, nbest: int, L: int,
+                               start: int, end: int):
+        """Ask slots (n) one question each with n-best lists (vd_dialog_ask_nbest_slots): (answer (n, G, nbest, L), length,
+        score, norm (n, G, nbest)) in row order; each slot's history takes its row's pick."""
+        s, q = self._slot_rows(slots, ques)
+        n, G, nb = s.size, int(G), int(nbest)
+        shape = (n, max(G, 1), max(nb, 1))
+        ans = np.zeros(shape + (int(L),), dtype=np.int32)
+        length = np.zeros(shape, dtype=np.int32)
+        score = np.zeros(shape, dtype=np.float64)
+        norm = np.zeros(shape, dtype=np.float64)
+        self._enc_rows = None
+        check(self.lib.vd_dialog_ask_nbest_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(k), G,
+                                                 float(diversity), float(length_penalty), nb, int(L), int(start), int(end),
+                                                 ans.ctypes.data, length.ctypes.data, score.ctypes.data, norm.ctypes.data))
+        self._dialog_rows = n
+        return ans, length, score, norm
 
     def dialog_ask_sample_slots(self, slots, ques, L: int, start: int, end: int, temperature: float, seed: int,
                                 row_offset: int = 0):

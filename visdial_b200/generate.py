@@ -10,6 +10,9 @@ earlier answers in its history instead of the dataset's (`-history gt`, the defa
 §17); it combines with `-sampleWords`, `-dialogsPerCall` and `-gpus`.  `-beamGroups G` (> 1, dividing `-beamSize`) runs
 diverse beam search with penalty `-diversity` (DESIGN §22): each round's answer is the best group's, and the round also
 lists `"answers"`, the text of every group that finished an answer, best first (the first is the round's answer).
+`-nBest n` keeps each group's n best finished answers and the round also lists `"nbest"`, their text best first (the
+first is the round's answer); `-lengthPenalty a` ranks finished answers by score / ((5 + l) / 6)^a, l their tokens
+(DESIGN §24).  results.json records the two only when they differ from their defaults (1 and 0).
 `-topK K` and `-topP P` truncate `-sampleWords 1`'s draws to the K most likely words and then to the fewest of those
 holding P of the probability (DESIGN §23); they combine with `-history`, `-dialogsPerCall` and `-gpus`, and
 results.json records them only when they truncate.  A disc checkpoint answers every round with the
@@ -33,7 +36,7 @@ def rank_share(model, dl, opt: dict) -> list:
     dl.restrict("val", max(0, opt["maxThreads"]))                                   # model.lua:455 over the ranks
     sampleParams = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "dialogsPerCall")}   # :88-94
     sampleParams["history"] = opt.get("history", "gt")
-    sampleParams.update({k: opt[k] for k in ("beamGroups", "diversity", "topK", "topP") if k in opt})
+    sampleParams.update({k: opt[k] for k in ("beamGroups", "diversity", "lengthPenalty", "nBest", "topK", "topP") if k in opt})
     if model.params["decoder"] == "disc":
         # a disc model answers by retrieval from the split's answer pool (DESIGN §18); model.lua:434-437 stops here
         answers = model.retrieveAnswers(dl, "val", {k: sampleParams[k] for k in ("dialogsPerCall", "history")})
@@ -45,6 +48,8 @@ def rank_share(model, dl, opt: dict) -> list:
         t = {"question": idToWords(r["question"], words), "answer": idToWords(r["answer"], words)}
         if "groups" in r:
             t["answers"] = [idToWords(g["answer"], words) for g in ranked_groups(r)]
+        if "nbest" in r:
+            t["nbest"] = [idToWords(x["answer"], words) for x in r["nbest"]]
         return t
     return [{"image_id": a["image_id"], "dialog": [turn(r) for r in a["dialog"]]} for a in answers]
 

@@ -234,6 +234,13 @@ class Model:
         score, the lower group on ties; what the "generated" history takes), and "groups" lists the G groups' entries
         (None for a group that finished no hypothesis).  `strict` raises only when every group is empty.
 
+        `lengthPenalty` alpha (default 0) and `nBest` n (default 1) keep each group's n best finished hypotheses by norm =
+        score / ((5 + l) / 6)^alpha, l = length - 1 (vd_gen_nbest_beam_search / vd_gen_dialog_nbest_beam_search, DESIGN
+        §24).  At the defaults the calls are the ones above.  Otherwise each round's answer / score / length are the pick's
+        (the best group head by normScore, the lower group on ties), every entry carries "normScore", "groups" (G > 1)
+        lists the group heads, and with n > 1 "nbest" lists every finished hypothesis of every group by (normScore desc,
+        group asc, list position asc).  Sampling ignores both.
+
         With `sampleWords`, `topK` K (default 0, off) and `topP` P (default 1, off) truncate every draw (DESIGN §23): to the
         first K classes by (logit desc, class asc), then to the shortest prefix of those holding P of their softmax mass
         (vd_gen_truncated_sample / vd_gen_dialog_truncated_sample).  When neither truncates (K = 0 or K >= vocabSize, and
@@ -255,6 +262,8 @@ class Model:
         beamSize, beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
         groups, diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
         diverse = groups > 1 and not sampleWords
+        lengthPenalty, nBest = float(params.get("lengthPenalty", 0.0)), int(params.get("nBest", 1))
+        listed = not sampleWords and (lengthPenalty != 0.0 or nBest != 1)
         topK, topP = int(params.get("topK", 0)), float(params.get("topP", 1.0))
         truncated = sampleWords and truncates(topK, topP, self.params["vocabSize"])
         startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
@@ -287,6 +296,10 @@ class Model:
                 elif sampleWords:
                     answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
                                                                  rowOffset, histWidth, maxAnsLen)
+                elif listed:
+                    answer, length, score, norm, _ = self.engine.gen_dialog_nbest_beam_search(
+                        batch, beamSize, groups, diversity, lengthPenalty, nBest, beamLen, startToken, endToken, histWidth,
+                        maxAnsLen)
                 elif diverse:
                     answer, length, score, _ = self.engine.gen_dialog_diverse_beam_search(
                         batch, beamSize, groups, diversity, beamLen, startToken, endToken, histWidth, maxAnsLen)
@@ -299,17 +312,24 @@ class Model:
                     answer, _ = self.engine.gen_truncated_sample(beamLen, startToken, temperature, seed, rowOffset, topK, topP)
                 elif sampleWords:                                                       # :582-594
                     answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
+                elif listed:
+                    answer, length, score, norm = self.engine.gen_nbest_beam_search(beamSize, groups, diversity, lengthPenalty,
+                                                                                    nBest, beamLen, startToken, endToken)
                 elif diverse:
                     answer, length, score = self.engine.gen_diverse_beam_search(beamSize, groups, diversity, beamLen,
                                                                                 startToken, endToken)
                 else:                                                                   # :472-579
                     answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
             R = self.params["maxQuesCount"]
-            if not sampleWords:
+            if listed:
+                answer, length = answer.reshape(len(inds), R, groups, nBest, -1), length.reshape(len(inds), R, groups, nBest)
+                score, norm = score.reshape(length.shape), norm.reshape(length.shape)
+            elif not sampleWords:
                 length, score = length.reshape(len(inds), R, -1), score.reshape(len(inds), R, -1)
             ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
             Tq = ques.shape[2]
-            answer = answer.reshape(len(inds), R, -1, answer.shape[-1])
+            if not listed:
+                answer = answer.reshape(len(inds), R, -1, answer.shape[-1])
             self.wrapper.training()                                                     # :605
             for d, convId in enumerate(inds):
                 w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
@@ -318,6 +338,13 @@ class Model:
                     q = ques[d, it, Tq - w:]
                     if sampleWords:
                         threadAnswers.append(entry(q, answer[d, it, 0]))
+                        continue
+                    if listed:
+                        e = listed_entry(answer[d, it], length[d, it], score[d, it], norm[d, it],
+                                         lambda a, **sc: entry(q, a, **sc))
+                        if e is None and strict:
+                            raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
+                        threadAnswers.append(e)
                         continue
                     gs = [entry(q, answer[d, it, g], score=float(score[d, it, g]), length=int(length[d, it, g]))
                           if length[d, it, g] > 0 else None for g in range(length.shape[2])]
@@ -437,9 +464,32 @@ def pick_group(length, score) -> int:
 
 
 def ranked_groups(entry) -> list:
-    """The finished groups of a diverse entry ("groups"), best first by (score desc, group asc): the pick is the first."""
+    """The finished groups of a diverse entry ("groups"), best first by (score desc, group asc), or by (normScore desc,
+    group asc) when the entries carry one (DESIGN §24): the pick is the first."""
     done = [e for e in entry.get("groups", [entry]) if e is not None]
-    return sorted(done, key=lambda e: -e["score"])
+    return sorted(done, key=lambda e: -e.get("normScore", e["score"]))
+
+
+def listed_entry(answer, length, score, norm, make):
+    """A round's entry from its n-best lists (DESIGN §24): answer (G, n, L), length / score / norm (G, n).  `make(answer,
+    score=, length=, normScore=)` builds one hypothesis' entry.  Returns the pick's entry (the best group head by
+    (normScore desc, group asc)) with "groups" (the G heads, None for a group that finished nothing) when G > 1 and
+    "nbest" (every finished hypothesis by (normScore desc, group asc, list position asc)) when n > 1; None when no group
+    finished a hypothesis."""
+    G, n = length.shape
+    lists = [[make(answer[g, i], score=float(score[g, i]), length=int(length[g, i]), normScore=float(norm[g, i]))
+              for i in range(n) if length[g, i] > 0] for g in range(G)]
+    best = pick_group(length[:, 0], norm[:, 0])
+    if best < 0:
+        return None
+    e = dict(lists[best][0])
+    if G > 1:
+        e["groups"] = [x[0] if x else None for x in lists]
+    if n > 1:
+        ranked = sorted(((x["normScore"], g, i) for g, xs in enumerate(lists) for i, x in enumerate(xs)),
+                        key=lambda t: (-t[0], t[1], t[2]))
+        e["nbest"] = [lists[g][i] for _, g, i in ranked]
+    return e
 
 
 def history_answer(row, end: int, length=None) -> list:
@@ -494,6 +544,7 @@ class DialogPool:
         self.temperature, self.seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
         self.beamSize, self.beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
         self.groups, self.diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
+        self.lengthPenalty, self.nBest = float(params.get("lengthPenalty", 0.0)), int(params.get("nBest", 1))
         # topK: a disc model's retrieval list length (default 1); a gen model's top-k truncation of sampling asks (default
         # 0, off), with topP (DESIGN §23)
         self.topK = int(params.get("topK", 1 if self.disc else 0))
@@ -625,6 +676,16 @@ class DialogPool:
                                                           self.seed, self.rowOffset)
             given = [history_answer(ans[b, 1:], self.end) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
+        elif self.lengthPenalty != 0.0 or self.nBest != 1:
+            ans, length, score, norm = self.eng.dialog_ask_nbest_slots(slots, q, self.beamSize, self.groups, self.diversity,
+                                                                       self.lengthPenalty, self.nBest, self.beamLen,
+                                                                       self.start, self.end)
+            given = []
+            for b in range(len(q)):
+                e = listed_entry(ans[b], length[b], score[b], norm[b],
+                                 lambda a, **sc: dict(answer=a.tolist(), **sc))
+                given.append(history_answer(e["answer"], self.end, e["length"]) if e else [])
+                out.append(dict(e, question=[int(t) for t in q[b] if t]) if e else None)
         elif self.groups > 1:
             ans, length, score = self.eng.dialog_ask_diverse_slots(slots, q, self.beamSize, self.groups, self.diversity,
                                                                    self.beamLen, self.start, self.end)
@@ -648,7 +709,7 @@ class DialogPool:
             for e in out:
                 if e is not None:
                     e["question_text"], e["answer_text"] = text(e["question"]), text(e["answer"])
-                    for x in e.get("groups", ()):
+                    for x in list(e.get("groups", ())) + list(e.get("nbest", ())):
                         if x is not None:
                             x["answer_text"] = text(x["answer"])
         return out
