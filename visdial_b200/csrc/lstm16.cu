@@ -10,11 +10,14 @@
 // and c_t, dc, every accumulator, the weight gradients and the final h_T that meets the encoder stay fp32.
 //
 //   k_lstm16<0>    : gates = h_{t-1} Wh^T (wgmma, 128x128 tiles) + P16[token] + bias -> pointwise -> fp16 gates,
-//                    fp32 c_t, fp16 h_t (+ fp32 h_T on the last step)
-//   k_lstm16<1>    : dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t, fp32 dc carry
-//   Both run their pointwise epilogue on the accumulator registers (no shared-memory accumulator tile), which leaves room
-//   for a 5-stage (forward) / 4-stage (backward) operand ring of 32 KB stages; the epilogue inputs are fetched by cp.async
-//   before the tile's contraction (the backward: those of its first 32 hidden units).
+//                    fp32 c_t, fp16 h_t (+ fp32 h_T on the last step).  Each CTA keeps one 128-row column slice of Wh
+//                    resident in shared memory (128 KB at H = 512) and streams only h_{t-1}; its two consumer warpgroups
+//                    contract their 64-row halves and take turns, so that one's main loop runs under the other's
+//                    epilogue; one 5-stage ring carries both halves' h_{t-1} rows in the order of the turns.
+//   k_lstm16<1>    : dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t, fp32 dc carry; a 4-stage ring of 32 KB
+//                    (A and B) stages shared by both consumer warpgroups.
+//   Both run their pointwise epilogue on the accumulator registers (no shared-memory accumulator tile); the epilogue inputs
+//   are fetched by cp.async before the tile's contraction (the backward: those of its first 32 hidden units).
 //   k_atb16        : dWh += inv_scale * h^T da  (both operands MN-major fp16, 128 x 256 tiles, stream-K, red.global.add)
 //   k_lstm16_first / k_lstm16_bwd_last / k_segsum16 / k_cvt16 / k_amax / k_pick_scale : streaming helpers
 #include <cuda.h>
@@ -122,17 +125,41 @@ struct Lstm16Params {
 struct Lstm16Maps { CUtensorMap g16, c, h16; };   // [R,4H] fp16 gates / da ; [R,H] fp32 c / dc ; [R,H] fp16 h: 16 x 32 boxes
 
 // ------------------------------------------------------------------------------------------------
-// MODE 0 = forward step, MODE 1 = backward step.  Persistent over the tile list; warpgroup 0 = TMA producer (one thread),
-// warpgroups 1-2 = consumers (64 rows each).  Each consumer warp runs the pointwise epilogue of its 16 rows straight from
-// its accumulator registers, 32 hidden units at a time, with the inputs staged by cp.async in the T16 / T32 tiles above.
-template <int MODE>
-struct Cfg16 {
+// MODE 0 = forward step, MODE 1 = backward step; warpgroup 0 = TMA producers, warpgroups 1-2 = consumers (64 rows each).
+// Each consumer warp runs the pointwise epilogue of its 16 rows straight from its accumulator registers, 32 hidden units at a
+// time, with the inputs staged by cp.async in the T16 / T32 tiles above.
+template <int MODE> struct Cfg16;
+
+// Forward: each CTA owns one column slice (32 hidden units x 4 gates = 128 rows of Wh, all H of K) for the whole launch and
+// keeps it resident in shared memory; only h_{t-1} streams.  The two consumer warpgroups each contract their own 64-row half of
+// a 128-row block against the whole slice and take turns (named-barrier token): one warpgroup's main loop runs while the other
+// runs its epilogue.  The turns fix the order in which the halves are consumed, so one ring of 64-row stages carries both,
+// in that order, and keeps four stages in flight across the hand-over from one warpgroup to the other.
+template <>
+struct Cfg16<0> {
   static constexpr int THREADS = 128 + 32 * EW16;
-  // per-warp staging: forward {4 gate tiles T16, c tile T32, h tile T16} = 7 KB (the inputs, x-projection rows and c_prev,
-  // land in the gate and c tiles; the outputs overwrite them in place); backward {4 gate tiles T16, c_prev, c_t, dc T32} = 10 KB
-  static constexpr int STG_PER_WARP = MODE == 0 ? (5 * T16_BYTES + T32_BYTES) : (4 * T16_BYTES + 3 * T32_BYTES);
+  static constexpr int KB_MAX = 512 / BK16;                       // k-blocks of the slice at the largest H (lstm16_shape_ok)
+  static constexpr int SLICE_KB = 4 * 32 * BK16 * 2;              // one k-block of the slice: 4 gate boxes of 32 rows = 16 KB
+  static constexpr int RES_BYTES = KB_MAX * SLICE_KB;             // 128 KB
+  static constexpr int A_STAGE = 64 * BK16 * 2;                   // 64 rows of h_{t-1} x one k-block = 8 KB
+  static constexpr int A_STAGES = 5;                              // as many as fit beside the slice and the staging
+  // per-warp staging {4 gate tiles T16, h tile T16, c tile T32} = 7 KB: the inputs, x-projection rows and c_prev, land in the
+  // gate and c tiles; the outputs overwrite them in place
+  static constexpr int STG_PER_WARP = 5 * T16_BYTES + T32_BYTES;
+  static constexpr int STG_BYTES = EW16 * STG_PER_WARP;           // 56 KB
+  static constexpr int BAR_BYTES = 8 * (KB_MAX + 2 * A_STAGES);
+  static constexpr int TOTAL = RES_BYTES + A_STAGES * A_STAGE + STG_BYTES + BAR_BYTES + 1024;   // + alignment slack
+  static_assert(TOTAL <= 232448, "k_lstm16<0>: shared memory");
+};
+
+// Backward: persistent over the tile list, one producer thread, a ring of 32 KB stages (A and B) shared by both consumers.
+template <>
+struct Cfg16<1> {
+  static constexpr int THREADS = 128 + 32 * EW16;
+  // per-warp staging: {4 gate tiles T16, c_prev, c_t, dc T32} = 10 KB
+  static constexpr int STG_PER_WARP = 4 * T16_BYTES + 3 * T32_BYTES;
   static constexpr int STG_BYTES = EW16 * STG_PER_WARP;
-  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES) / STAGE16;      // fwd 5, bwd 4
+  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES) / STAGE16;      // 4
   static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + 1024 + 256;
 };
 
@@ -140,6 +167,7 @@ template <int MODE>
 __global__ void __launch_bounds__(Cfg16<MODE>::THREADS, 1)
 k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
          const __grid_constant__ Lstm16Maps em, const Lstm16Params p) {
+  static_assert(MODE == 1, "the forward step is the k_lstm16<0> specialisation below");
   using C = Cfg16<MODE>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -151,9 +179,9 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int H = p.H;
   const int num_m = (p.R + BM16 - 1) / BM16;
-  const int num_n = MODE == 0 ? H / 32 : H / BN16;
+  const int num_n = H / BN16;
   const int num_tiles = num_m * num_n;
-  const int num_kb = (MODE == 0 ? H : 4 * H) / BK16;
+  const int num_kb = 4 * H / BK16;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
@@ -174,13 +202,7 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
           uint8_t* sb = sa + 16384;
           mbar_expect_tx(&full[s], STAGE16);
           tma_load_2d(sa, &tmA, &full[s], kb * BK16, m0);
-          if (MODE == 0) {
-            // tile columns = [i | f | o | g] of 32 hidden units
-#pragma unroll
-            for (int g = 0; g < 4; ++g) tma_load_2d(sb + g * 4096, &tmB, &full[s], kb * BK16, g * H + nt * 32);
-          } else {
-            tma_load_2d(sb, &tmB, &full[s], kb * BK16, nt * BN16);
-          }
+          tma_load_2d(sb, &tmB, &full[s], kb * BK16, nt * BN16);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
@@ -214,156 +236,264 @@ k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtens
       wgmma_hold(d);
       if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
     };
-    if constexpr (MODE == 0) {
-      // ---- forward.  Tile columns [i | f | o | g] x 32 hidden units, so the thread holding column 8jj + fu of gate i holds
-      // the same unit of f, o and g in fragments jj + 4, jj + 8, jj + 12: the pointwise step runs where the accumulators are.
-      uint8_t* sG = stg; uint8_t* sH = stg + 4 * T16_BYTES; uint8_t* sC = sH + T16_BYTES;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n) * BM16;
-        const int nt = tile % num_n;
-        const int r0 = m0 + wg * 64 + (cw & 3) * 16;          // first of the warp's 16 rows
-        const int j0 = nt * 32;                                // first hidden unit of the tile
-        const int64_t row = (int64_t)r0 + (lane & 15);         // lanes l and l + 16 both describe row l % 16
-        const bool row_ok = row < p.R;
-        const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
-        // A pad token's x-projection is exactly zero (LookupTableMaskZero: embedding row 0 is zero, and the table carries no
-        // bias), so finished sequences skip the gather: at late time steps most of the 100 x 20-token options have ended, and
-        // every row would otherwise read the same 4 KB of L2
-        const int32_t tk = row_ok ? __ldg(p.tok + row) : 0;
-        const __half* prow = tk != 0 ? p.ptable + (int64_t)tk * 4 * H + j0 : nullptr;
-        const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H + j0 : nullptr;
-        if (lane == 0) bulk_wait_read0();                      // the previous tile's TMA stores have read the staging tiles
+    // ---- backward: 128 hidden units per tile = 4 groups of 32; fragment columns are hidden units, so the thread reads the
+    // gates / c / dc of exactly the units its accumulators hold.  The first group's inputs are fetched before the contraction.
+    uint8_t* sG = stg; uint8_t* sCP = stg + 4 * T16_BYTES; uint8_t* sCC = sCP + T32_BYTES; uint8_t* sDC = sCC + T32_BYTES;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m0 = (tile / num_n) * BM16;
+      const int nt = tile % num_n;
+      const int r0 = m0 + wg * 64 + (cw & 3) * 16;
+      const int64_t row = (int64_t)r0 + (lane & 15);
+      const bool row_ok = row < p.R;
+      const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
+      const __half* grow = row_ok ? p.gsave + row * 4 * H : nullptr;
+      const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H : nullptr;
+      const float* ccrow = row_ok ? p.c_cur + row * H : nullptr;
+      const float* dcrow = row_ok ? p.dc_carry + row * H : nullptr;
+      auto fetch = [&](int j) {                              // inputs of hidden units j .. j + 31 -> staging
+        if (lane == 0) bulk_wait_read0();
         __syncwarp();
 #pragma unroll
-        for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, prow ? prow + g * H : nullptr, lane);
-        t32_load(sC, cprow, lane);
-        float d[BN16 / 2];
-        contract(d);                                           // the loads fly while the MMAs of this tile run
+        for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, grow ? grow + g * H + j : nullptr, lane);
+        t32_load(sCP, cprow ? cprow + j : nullptr, lane);
+        t32_load(sCC, ccrow ? ccrow + j : nullptr, lane);
+        t32_load(sDC, dcrow ? dcrow + j : nullptr, lane);
+      };
+      fetch(nt * BN16);
+      float d[BN16 / 2];
+      contract(d);
+#pragma unroll
+      for (int grp = 0; grp < BN16 / 32; ++grp) {
+        const int j = nt * BN16 + grp * 32;
+        if (grp > 0) fetch(j);
         cp_wait_all();
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           const int r = fr + 8 * hh;
-          const float kp = __shfl_sync(0xffffffffu, keep, r);
-          const int64_t grow = (int64_t)r0 + r;
+          const float keep_r = __shfl_sync(0xffffffffu, keep, r);
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj) {
             const int u = 8 * jj + fu;
-            float a[4][2], cp[2], hn[2];
+            float g[4][2], cp[2], cc[2], dc[2], out[4][2], dcn[2];
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const float2 x = ld_h2(t16_at(sG + g * T16_BYTES, r, u));
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + g * H + j0 + u));
-              a[g][0] = d[4 * (jj + 4 * g) + 2 * hh] + (x.x + b.x);
-              a[g][1] = d[4 * (jj + 4 * g) + 2 * hh + 1] + (x.y + b.y);
+            for (int gg = 0; gg < 4; ++gg) {
+              const float2 x = ld_h2(t16_at(sG + gg * T16_BYTES, r, u));
+              g[gg][0] = x.x; g[gg][1] = x.y;
             }
-            const float2 c2 = *reinterpret_cast<const float2*>(t32_at(sC, r, u));
-            cp[0] = c2.x; cp[1] = c2.y;
+            const float2 cp2 = *reinterpret_cast<const float2*>(t32_at(sCP, r, u));
+            const float2 cc2 = *reinterpret_cast<const float2*>(t32_at(sCC, r, u));
+            const float2 dc2 = *reinterpret_cast<const float2*>(t32_at(sDC, r, u));
+            cp[0] = cp2.x; cp[1] = cp2.y; cc[0] = cc2.x; cc[1] = cc2.y; dc[0] = dc2.x; dc[1] = dc2.y;
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-              const float gi = sig16(a[0][e]), gf = sig16(a[1][e]), go = sig16(a[2][e]), gg = tanh16(a[3][e]);
-              const float c_ = (gf * cp[e] + gi * gg) * kp;
-              a[0][e] = gi * kp; a[1][e] = gf * kp; a[2][e] = go * kp; a[3][e] = gg * kp;
-              cp[e] = c_; hn[e] = go * tanh16(c_) * kp;
+              const float dh = d[4 * (4 * grp + jj) + 2 * hh + e];
+              const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
+              const float tcv = tanh16(cc[e]);
+              const float dd = (dc[e] + dh * go * (1.f - tcv * tcv)) * keep_r;
+              const float dhe = dh * keep_r;
+              out[0][e] = dd * gg_ * gi * (1.f - gi);
+              out[1][e] = dd * cp[e] * gf * (1.f - gf);
+              out[2][e] = dhe * tcv * go * (1.f - go);
+              out[3][e] = dd * gi * (1.f - gg_ * gg_);
+              dcn[e] = dd * gf;
             }
 #pragma unroll
-            for (int g = 0; g < 4; ++g) st_h2(t16_at(sG + g * T16_BYTES, r, u), a[g][0], a[g][1]);
-            *reinterpret_cast<float2*>(t32_at(sC, r, u)) = make_float2(cp[0], cp[1]);
-            st_h2(t16_at(sH, r, u), hn[0], hn[1]);
-            if (p.h32_out && grow < p.R)                  // last step only: the fp32 h that meets the encoder output
-              *reinterpret_cast<float2*>(p.h32_out + grow * H + j0 + u) = make_float2(hn[0], hn[1]);
+            for (int gg = 0; gg < 4; ++gg) st_h2(t16_at(sG + gg * T16_BYTES, r, u), out[gg][0], out[gg][1]);
+            *reinterpret_cast<float2*>(t32_at(sDC, r, u)) = make_float2(dcn[0], dcn[1]);
           }
         }
         fence_proxy_async_smem();
         __syncwarp();
         if (lane == 0) {
-          if (p.save_gates) {
 #pragma unroll
-            for (int g = 0; g < 4; ++g) tma_store_2d(&em.g16, sG + g * T16_BYTES, g * H + j0, r0);
-          }
-          tma_store_2d(&em.c, sC, j0, r0);
-          tma_store_2d(&em.h16, sH, j0, r0);
+          for (int gg = 0; gg < 4; ++gg) tma_store_2d(&em.g16, sG + gg * T16_BYTES, gg * H + j, r0);
+          tma_store_2d(&em.c, sDC, j, r0);
           bulk_commit();
         }
         __syncwarp();
       }
-    } else {
-      // ---- backward: 128 hidden units per tile = 4 groups of 32; fragment columns are hidden units, so the thread reads the
-      // gates / c / dc of exactly the units its accumulators hold.  The first group's inputs are fetched before the contraction.
-      uint8_t* sG = stg; uint8_t* sCP = stg + 4 * T16_BYTES; uint8_t* sCC = sCP + T32_BYTES; uint8_t* sDC = sCC + T32_BYTES;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n) * BM16;
-        const int nt = tile % num_n;
-        const int r0 = m0 + wg * 64 + (cw & 3) * 16;
-        const int64_t row = (int64_t)r0 + (lane & 15);
-        const bool row_ok = row < p.R;
-        const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
-        const __half* grow = row_ok ? p.gsave + row * 4 * H : nullptr;
-        const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H : nullptr;
-        const float* ccrow = row_ok ? p.c_cur + row * H : nullptr;
-        const float* dcrow = row_ok ? p.dc_carry + row * H : nullptr;
-        auto fetch = [&](int j) {                              // inputs of hidden units j .. j + 31 -> staging
-          if (lane == 0) bulk_wait_read0();
-          __syncwarp();
+    }
+    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
+  }
+}
+
+// Forward step.  CTA b owns the column slice nt = b % num_n and walks the 128-row blocks b / num_n, + P, + 2P, ... (P =
+// gridDim.x / num_n CTAs per slice).  Thread 0 loads the slice once (one barrier per k-block, so the first contraction starts
+// on the first 16 KB) and then streams h_{t-1} through the ring.  Warpgroup w contracts rows 64w .. 64w + 63 of each block
+// with the m64n128k16 instructions, operands and k order of a 128 x 128 tile: the accumulators are bit for bit those of a
+// kernel that streams both operands.  The turn is a token on two named barriers of the 256 consumer
+// threads: warpgroup 1 runs its main loop, arrives on barrier 2 (warpgroup 2's main loop may start) and runs its epilogue;
+// warpgroup 2 arrives on barrier 1 after its main loop, except after its last block, so that every barrier phase that is
+// arrived on is also waited on.  Without the token the two start together and stay in lockstep.
+template <>
+__global__ void __launch_bounds__(Cfg16<0>::THREADS, 1)
+k_lstm16<0>(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+            const __grid_constant__ Lstm16Maps em, const Lstm16Params p) {
+  using C = Cfg16<0>;
+  constexpr int AS = C::A_STAGES;
+  constexpr int TOKEN_WG1 = 1, TOKEN_WG2 = 2;                 // named barriers (0 is __syncthreads')
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  uint8_t* slice = smem;                                      // [k-block][gate i f o g][32 rows][64 halves], 128B swizzle
+  uint8_t* ring = slice + C::RES_BYTES;                       // [stage][64 rows][64 halves], 128B swizzle
+  uint8_t* stg_all = ring + AS * C::A_STAGE;
+  uint64_t* wfull = (uint64_t*)(stg_all + C::STG_BYTES);      // [k-block]: that k-block of the slice has landed
+  uint64_t* full = wfull + C::KB_MAX;                         // [stage]
+  uint64_t* empty = full + AS;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int H = p.H;
+  const int num_m = (p.R + BM16 - 1) / BM16;
+  const int num_n = H / 32;
+  const int num_kb = H / BK16;
+  const int nt = blockIdx.x % num_n, per = gridDim.x / num_n;   // this CTA's slice; CTAs per slice
+  const int mb0 = blockIdx.x / num_n;                           // this CTA's first row block (none if >= num_m)
+
+  if (threadIdx.x == 0) {
+    for (int kb = 0; kb < num_kb; ++kb) mbar_init(&wfull[kb], 1);
+    for (int s = 0; s < AS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    if (threadIdx.x == 0 && mb0 < num_m) {
+      // ===== TMA producer: the slice once, then per row block warpgroup 1's 64 rows of A, k-block by k-block, then
+      // warpgroup 2's: the order of the turns
+      for (int kb = 0; kb < num_kb; ++kb) {
+        uint8_t* sb = slice + kb * C::SLICE_KB;
+        mbar_expect_tx(&wfull[kb], C::SLICE_KB);
+        // slice rows = [i | f | o | g] of 32 hidden units
 #pragma unroll
-          for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, grow ? grow + g * H + j : nullptr, lane);
-          t32_load(sCP, cprow ? cprow + j : nullptr, lane);
-          t32_load(sCC, ccrow ? ccrow + j : nullptr, lane);
-          t32_load(sDC, dcrow ? dcrow + j : nullptr, lane);
-        };
-        fetch(nt * BN16);
-        float d[BN16 / 2];
-        contract(d);
-#pragma unroll
-        for (int grp = 0; grp < BN16 / 32; ++grp) {
-          const int j = nt * BN16 + grp * 32;
-          if (grp > 0) fetch(j);
-          cp_wait_all();
-#pragma unroll
-          for (int hh = 0; hh < 2; ++hh) {
-            const int r = fr + 8 * hh;
-            const float keep_r = __shfl_sync(0xffffffffu, keep, r);
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const int u = 8 * jj + fu;
-              float g[4][2], cp[2], cc[2], dc[2], out[4][2], dcn[2];
-#pragma unroll
-              for (int gg = 0; gg < 4; ++gg) {
-                const float2 x = ld_h2(t16_at(sG + gg * T16_BYTES, r, u));
-                g[gg][0] = x.x; g[gg][1] = x.y;
-              }
-              const float2 cp2 = *reinterpret_cast<const float2*>(t32_at(sCP, r, u));
-              const float2 cc2 = *reinterpret_cast<const float2*>(t32_at(sCC, r, u));
-              const float2 dc2 = *reinterpret_cast<const float2*>(t32_at(sDC, r, u));
-              cp[0] = cp2.x; cp[1] = cp2.y; cc[0] = cc2.x; cc[1] = cc2.y; dc[0] = dc2.x; dc[1] = dc2.y;
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const float dh = d[4 * (4 * grp + jj) + 2 * hh + e];
-                const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
-                const float tcv = tanh16(cc[e]);
-                const float dd = (dc[e] + dh * go * (1.f - tcv * tcv)) * keep_r;
-                const float dhe = dh * keep_r;
-                out[0][e] = dd * gg_ * gi * (1.f - gi);
-                out[1][e] = dd * cp[e] * gf * (1.f - gf);
-                out[2][e] = dhe * tcv * go * (1.f - go);
-                out[3][e] = dd * gi * (1.f - gg_ * gg_);
-                dcn[e] = dd * gf;
-              }
-#pragma unroll
-              for (int gg = 0; gg < 4; ++gg) st_h2(t16_at(sG + gg * T16_BYTES, r, u), out[gg][0], out[gg][1]);
-              *reinterpret_cast<float2*>(t32_at(sDC, r, u)) = make_float2(dcn[0], dcn[1]);
-            }
+        for (int g = 0; g < 4; ++g) tma_load_2d(sb + g * 4096, &tmB, &wfull[kb], kb * BK16, g * H + nt * 32);
+      }
+      int s = 0; uint32_t ph = 0;
+      for (int mb = mb0; mb < num_m; mb += per) {
+        for (int w = 0; w < 2; ++w) {
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&empty[s], ph ^ 1);
+            mbar_expect_tx(&full[s], C::A_STAGE);
+            tma_load_2d(ring + s * C::A_STAGE, &tmA, &full[s], kb * BK16, mb * BM16 + w * 64);
+            if (++s == AS) { s = 0; ph ^= 1; }
           }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-#pragma unroll
-            for (int gg = 0; gg < 4; ++gg) tma_store_2d(&em.g16, sG + gg * T16_BYTES, gg * H + j, r0);
-            tma_store_2d(&em.c, sDC, j, r0);
-            bulk_commit();
-          }
-          __syncwarp();
         }
       }
+    }
+  } else {
+    const int cw = warp - 4, wg = cw >> 2;
+    uint8_t* stg = stg_all + cw * C::STG_PER_WARP;
+    // fragment rows of this thread within the warp's 16, and the unit pair within a group of 8 columns
+    const int fr = lane >> 2, fu = 2 * (lane & 3);
+    // main loop of one row block: this warpgroup's 64 rows x 128 columns against the resident slice.  Its k-blocks take
+    // ring positions (2 j + wg) num_kb .. + num_kb - 1 in its j-th turn; (s, ph) = the ring position of the next one.
+    int s = 0; uint32_t ph = 0;
+    auto skip = [&](int n) {                                   // the other warpgroup's turn
+      for (s += n; s >= AS; s -= AS) ph ^= 1;
+    };
+    skip(wg * num_kb);
+    auto contract = [&](float (&d)[BN16 / 2], bool first) {
+#pragma unroll
+      for (int i = 0; i < BN16 / 2; ++i) d[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        if (first) mbar_wait(&wfull[kb], 0);
+        mbar_wait(&full[s], ph);
+        const uint64_t adesc = make_desc(smem_u32(ring + s * C::A_STAGE), 16, 1024),
+                       bdesc = make_desc(smem_u32(slice + kb * C::SLICE_KB), 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK16 / UK16; ++k)
+          wgmma_f16_n128(d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == AS) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+      skip(num_kb);
+    };
+    // Tile columns [i | f | o | g] x 32 hidden units, so the thread holding column 8jj + fu of gate i holds the same unit of
+    // f, o and g in fragments jj + 4, jj + 8, jj + 12: the pointwise step runs where the accumulators are.
+    uint8_t* sG = stg; uint8_t* sH = stg + 4 * T16_BYTES; uint8_t* sC = sH + T16_BYTES;
+    for (int mb = mb0; mb < num_m; mb += per) {
+      // first hidden unit of the slice.  Opaque to the compiler, so that the bias and output addresses derived from it are
+      // formed in the epilogue instead of being hoisted out of the loop, where they would spill
+      int j0 = nt * 32;
+      asm volatile("" : "+r"(j0));
+      const int r0 = mb * BM16 + wg * 64 + (cw & 3) * 16;      // first of the warp's 16 rows
+      const int64_t row = (int64_t)r0 + (lane & 15);           // lanes l and l + 16 both describe row l % 16
+      const bool row_ok = row < p.R;
+      const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
+      // A pad token's x-projection is exactly zero (LookupTableMaskZero: embedding row 0 is zero, and the table carries no
+      // bias), so finished sequences skip the gather: at late time steps most of the 100 x 20-token options have ended, and
+      // every row would otherwise read the same 4 KB of L2
+      const int32_t tk = row_ok ? __ldg(p.tok + row) : 0;
+      const __half* prow = tk != 0 ? p.ptable + (int64_t)tk * 4 * H + j0 : nullptr;
+      const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H + j0 : nullptr;
+      if (lane == 0) bulk_wait_read0();                        // the previous block's TMA stores have read the staging tiles
+      __syncwarp();
+#pragma unroll
+      for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, prow ? prow + g * H : nullptr, lane);
+      t32_load(sC, cprow, lane);
+      const bool first = mb == mb0;
+      if (wg == 0) {
+        if (!first) bar_named(TOKEN_WG1, 256);                 // warpgroup 2's main loop is done
+      } else {
+        bar_named(TOKEN_WG2, 256);                             // warpgroup 1's main loop is done
+      }
+      float d[BN16 / 2];
+      contract(d, first);                                      // the loads fly while the MMAs of this block run
+      if (wg == 0) bar_arrive_named(TOKEN_WG2, 256);
+      else if (mb + per < num_m) bar_arrive_named(TOKEN_WG1, 256);
+      cp_wait_all();
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = fr + 8 * hh;
+        const float kp = __shfl_sync(0xffffffffu, keep, r);
+        const int64_t grow = (int64_t)r0 + r;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+          const int u = 8 * jj + fu;
+          float a[4][2], cp[2], hn[2];
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            const float2 x = ld_h2(t16_at(sG + g * T16_BYTES, r, u));
+            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + g * H + j0 + u));
+            a[g][0] = d[4 * (jj + 4 * g) + 2 * hh] + (x.x + b.x);
+            a[g][1] = d[4 * (jj + 4 * g) + 2 * hh + 1] + (x.y + b.y);
+          }
+          const float2 c2 = *reinterpret_cast<const float2*>(t32_at(sC, r, u));
+          cp[0] = c2.x; cp[1] = c2.y;
+#pragma unroll
+          for (int e2 = 0; e2 < 2; ++e2) {
+            const float gi = sig16(a[0][e2]), gf = sig16(a[1][e2]), go = sig16(a[2][e2]), gg = tanh16(a[3][e2]);
+            const float c_ = (gf * cp[e2] + gi * gg) * kp;
+            a[0][e2] = gi * kp; a[1][e2] = gf * kp; a[2][e2] = go * kp; a[3][e2] = gg * kp;
+            cp[e2] = c_; hn[e2] = go * tanh16(c_) * kp;
+          }
+#pragma unroll
+          for (int g = 0; g < 4; ++g) st_h2(t16_at(sG + g * T16_BYTES, r, u), a[g][0], a[g][1]);
+          *reinterpret_cast<float2*>(t32_at(sC, r, u)) = make_float2(cp[0], cp[1]);
+          st_h2(t16_at(sH, r, u), hn[0], hn[1]);
+          if (p.h32_out && grow < p.R)                    // last step only: the fp32 h that meets the encoder output
+            *reinterpret_cast<float2*>(p.h32_out + grow * H + j0 + u) = make_float2(hn[0], hn[1]);
+        }
+      }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) {
+        if (p.save_gates) {
+#pragma unroll
+          for (int g = 0; g < 4; ++g) tma_store_2d(&em.g16, sG + g * T16_BYTES, g * H + j0, r0);
+        }
+        tma_store_2d(&em.c, sC, j0, r0);
+        tma_store_2d(&em.h16, sH, j0, r0);
+        bulk_commit();
+      }
+      __syncwarp();
     }
     if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
   }
@@ -702,19 +832,18 @@ static CUtensorMap tmap_f(const float* base, int64_t rows, int64_t cols, int64_t
   return make_tmap16(base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, rows, cols, ld, box_rows, box_cols, swz);
 }
 
+// persistent, balanced waves (see gemm_tc.cu::launch): the fewest workers, at most pmax, that take cdiv(n, pmax) items each
+static int balanced_workers(int n, int pmax) { return n <= pmax ? n : cdiv(n, cdiv(n, pmax)); }
+
 template <int MODE>
 static void launch16(LaunchCtx& cx, const CUtensorMap& tA, const CUtensorMap& tB, const Lstm16Maps& em, const Lstm16Params& p,
-                     int num_tiles) {
+                     int grid) {
   using C = Cfg16<MODE>;
   static bool attr_set = false;
   if (!attr_set) {
     VD_CUDA_CHECK(cudaFuncSetAttribute(k_lstm16<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::TOTAL));
     attr_set = true;
   }
-  // persistent, balanced waves (see gemm_tc.cu::launch)
-  const int pmax = cx.sms();
-  int grid = num_tiles;
-  if (num_tiles > pmax) { const int rounds = cdiv(num_tiles, pmax); grid = cdiv(num_tiles, rounds); }
   k_lstm16<MODE><<<grid, C::THREADS, C::TOTAL, cx.stream>>>(tA, tB, em, p);
   check_launch(cx, "k_lstm16");
 }
@@ -731,14 +860,16 @@ void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, co
   Lstm16Params p = {};
   p.R = (int)R; p.H = H; p.ptable = ptable16; p.tok = tok; p.bias = bias; p.c_prev = c_prev; p.mask_ids = mask_ids;
   p.h32_out = h32_out; p.save_gates = gates16 != nullptr;
-  CUtensorMap tA = tmap_h(h_prev16, R, H, H, BM16, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
+  CUtensorMap tA = tmap_h(h_prev16, R, H, H, 64, BK16, CU_TENSOR_MAP_SWIZZLE_128B);       // one warpgroup's 64 rows
   CUtensorMap tB = tmap_h(Wh16, 4 * (int64_t)H, H, H, 32, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
   Lstm16Maps em;
   em.g16 = gates16 ? tmap_h(gates16, R, 4 * (int64_t)H, 4 * (int64_t)H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B)
                    : tmap_h(h16_out, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
   em.c = tmap_f(c_out, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_128B);
   em.h16 = tmap_h(h16_out, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
-  launch16<0>(cx, tA, tB, em, p, cdiv(R, BM16) * (H / 32));
+  // each of the H / 32 column slices gets the same number of CTAs, which split its 128-row blocks evenly
+  const int slices = H / 32;
+  launch16<0>(cx, tA, tB, em, p, slices * balanced_workers(cdiv(R, BM16), std::max(1, cx.sms() / slices)));
 }
 
 void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, const __half* Whb16, const __half* gates16,
@@ -753,7 +884,7 @@ void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, c
   em.g16 = tmap_h(da16, R, 4 * (int64_t)H, 4 * (int64_t)H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
   em.c = tmap_f(dc_carry, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_128B);
   em.h16 = em.c;
-  launch16<1>(cx, tA, tB, em, p, cdiv(R, BM16) * (H / BN16));
+  launch16<1>(cx, tA, tB, em, p, balanced_workers(cdiv(R, BM16) * (H / BN16), cx.sms()));
 }
 
 void lstm16_first_step(LaunchCtx& cx, int64_t R, int H, const __half* ptable16, const int32_t* tok, const float* bias,

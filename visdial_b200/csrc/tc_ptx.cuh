@@ -44,6 +44,7 @@ template <int NR> __device__ __forceinline__ void wgmma_hold(float (&d)[NR]) {  
   for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ void bar_named(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void bar_arrive_named(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // shared-memory matrix descriptor (sm_90 GMMA): 128-byte swizzle.  K-major tiles: rows of 128 bytes, 8-row atoms SBO = 1024
 // apart (LBO unused); MN-major (16-bit types only): 64-element groups LBO apart, 8-k-row atoms SBO apart.
