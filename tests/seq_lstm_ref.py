@@ -8,10 +8,14 @@ Two modes.  Free-running: the whole sequence from the inputs.  Teacher-forced (t
 saved at t-1, and in the BPTT the recurrent gradient of step t is da_{t+1} of the device, while the cell-gradient carry runs free.
 Each step then carries one step's error only.  The gradients (weight_grads, table_grads) are contractions of whatever operands they
 are given: the reference's own, or the device's saved h / da.  Every function also returns the contraction of the absolute values,
-sum_k |a_k b_k|, the scale of an accumulated contraction's rounding error."""
+sum_k |a_k b_k|, the scale of an accumulated contraction's rounding error.  bptt_bound is the per-element error bound of a
+BPTT computed in fp32 from given gates, c and recurrent gradients (test_seq_lstm_gpu.py, test_lstm16_bwd_step_gpu.py)."""
 import numpy as np
 
 from helpers import lstm_step_bwd_ref, lstm_step_fwd_ref
+
+U = 2.0 ** -24
+TINY = 2.0 ** -149           # fp32's smallest subnormal: the absolute rounding of results that underflow
 
 
 def _f64(a):
@@ -66,6 +70,32 @@ def backward(W, gates, c, c0=None, mask=None, dh_all=None, dh_last=None, dc_last
         cp = c[t - 1] if t else _f64(c0)
         da[t], dc = lstm_step_bwd_ref(gates[t], cp, c[t], dh[t], dc, None if mask is None else mask[t])
     return da, dh, Sdh, dc
+
+
+def bptt_bound(gates, c, c0, mask, dh, e_dh, dc_last, act):
+    """the teacher-forced BPTT's per-element bound on da and the bound of the free-running cell-gradient carry past step 0"""
+    T, R, G = gates.shape
+    H = G // 4
+    eda = np.zeros_like(gates)
+    dc = np.zeros((R, H)) if dc_last is None else np.asarray(dc_last, np.float64)
+    edc = np.zeros((R, H))
+    for t in reversed(range(T)):
+        a, ct = gates[t], c[t]
+        cp = c[t - 1] if t else (np.zeros((R, H)) if c0 is None else c0)
+        i, f, o, g = a[:, :H], a[:, H:2 * H], a[:, 2 * H:3 * H], a[:, 3 * H:]
+        tc = np.tanh(ct)
+        d = dc + dh[t] * o * (1 - tc * tc)
+        ed = edc + e_dh[t] * o * (1 - tc * tc) + np.abs(dh[t]) * o * 2 * np.abs(tc) * act + 3 * U * (np.abs(dc) + np.abs(d))
+        eda[t] = np.concatenate([ed * np.abs(g * i * (1 - i)), ed * np.abs(cp * f * (1 - f)),
+                                 e_dh[t] * np.abs(tc * o * (1 - o)) + np.abs(dh[t]) * o * (1 - o) * act,
+                                 ed * np.abs(i * (1 - g * g))], 1) + TINY
+        edc = ed * f + U * np.abs(d) * f
+        dc = d * f
+        if mask is not None:
+            edc[mask[t]] = 0
+            dc[mask[t]] = 0
+            eda[t][mask[t]] = 0
+    return eda, edc
 
 
 def weight_grads(W, x, h, da, h0=None):

@@ -37,7 +37,6 @@ pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
 TF32 = 2.0 ** -9
 ACT = 5e-7
-TINY = 2.0 ** -149           # fp32's smallest subnormal: the absolute rounding of results that underflow
 SIMT, TC, OPT16, PAIR16 = 0, 1, 2, 3
 FREE = {VD_MATH_FP32: 1e-5, VD_MATH_TF32: 3e-2, VD_MATH_F16: 3e-2}
 MODES = {"fp32": VD_MATH_FP32, "tf32": VD_MATH_TF32, "f16": VD_MATH_F16}
@@ -212,32 +211,6 @@ def cell_bounds(a, cp, c, dz, act):
     return ea, ec, eh
 
 
-def bptt_bound(gates, c, c0, mask, dh, e_dh, dc_last, act):
-    """the teacher-forced BPTT's per-element bound on da and the bound of the free-running cell-gradient carry past step 0"""
-    T, R, G = gates.shape
-    H = G // 4
-    eda = np.zeros_like(gates)
-    dc = np.zeros((R, H)) if dc_last is None else np.asarray(dc_last, np.float64)
-    edc = np.zeros((R, H))
-    for t in reversed(range(T)):
-        a, ct = gates[t], c[t]
-        cp = c[t - 1] if t else (np.zeros((R, H)) if c0 is None else c0)
-        i, f, o, g = a[:, :H], a[:, H:2 * H], a[:, 2 * H:3 * H], a[:, 3 * H:]
-        tc = np.tanh(ct)
-        d = dc + dh[t] * o * (1 - tc * tc)
-        ed = edc + e_dh[t] * o * (1 - tc * tc) + np.abs(dh[t]) * o * 2 * np.abs(tc) * act + 3 * U * (np.abs(dc) + np.abs(d))
-        eda[t] = np.concatenate([ed * np.abs(g * i * (1 - i)), ed * np.abs(cp * f * (1 - f)),
-                                 e_dh[t] * np.abs(tc * o * (1 - o)) + np.abs(dh[t]) * o * (1 - o) * act,
-                                 ed * np.abs(i * (1 - g * g))], 1) + TINY
-        edc = ed * f + U * np.abs(d) * f
-        dc = d * f
-        if mask is not None:
-            edc[mask[t]] = 0
-            dc[mask[t]] = 0
-            eda[t][mask[t]] = 0
-    return eda, edc
-
-
 def gemm_factor(mode, K, exact_operands=False):
     return (K + 2) * U + (TF32 if mode != VD_MATH_FP32 and not exact_operands else 0.0)
 
@@ -270,10 +243,10 @@ def check_saved(tag, mode, rt, W, b, emb, x, tok, mask, h0, c0, dh_all, dh_last,
     da, dh, Sdh, dc0 = S.backward(W, got["gates"], got["c"], c0, m, dh_all, dh_last, dc_last, tf_da=da_dev)
     if opt16:
         e_dh = (2.0 ** -11 + (G + 2) * U) * Sdh
-        eda, _ = bptt_bound(got["gates"], got["c"], c0, m, dh, e_dh, dc_last, 2.0 ** -10)
+        eda, _ = S.bptt_bound(got["gates"], got["c"], c0, m, dh, e_dh, dc_last, 2.0 ** -10)
         eda += 2.0 ** -11 * np.abs(da) + 2.0 ** -25 / s
     else:
-        eda, edc = bptt_bound(got["gates"], got["c"], c0, m, dh, gemm_factor(mode, G) * Sdh, dc_last, ACT)
+        eda, edc = S.bptt_bound(got["gates"], got["c"], c0, m, dh, gemm_factor(mode, G) * Sdh, dc_last, ACT)
         eda += 4 * U * np.abs(da)
     close(da_dev, da, eda, tag, "da")
     if m is not None:
