@@ -19,10 +19,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 # option-stream phases, by kernel-name substring (first match wins)
-PHASES = [("opt_fwd_step", "k_lstm16<0>"), ("opt_fwd_first", "k_lstm16_first"), ("opt_bptt_step", "k_lstm16<1>"),
+PHASES = [("opt_fwd_step", "k_lstm16<0>"), ("opt_fwd_first", "k_lstm16_first"), ("opt_bptt_step", "k_lstm16_bptt"),
           ("opt_bptt_last", "k_lstm16_bwd_last"), ("wgrad_atb16", "k_atb16"), ("token_sort", "k_tok_"),
           ("segsum16", "k_segsum16"), ("colsum", "colsum"), ("dP_gemm", "k_tc_"), ("dP_gemm", "gemm")]
-PERSISTENT = ("k_lstm16<", "k_atb16", "k_enc_pair")
+PERSISTENT = ("k_lstm16<", "k_lstm16_bptt", "k_atb16", "k_enc_pair")
 
 
 def short(name):
@@ -66,7 +66,7 @@ def analyse(ks, lines, verbose):
     by_stream = collections.defaultdict(list)
     for k in ks:
         by_stream[k["stream"]].append(k)
-    opt = max(by_stream, key=lambda s: sum(1 for k in by_stream[s] if "k_lstm16<1>" in k["name"]))
+    opt = max(by_stream, key=lambda s: sum(1 for k in by_stream[s] if "k_lstm16_bptt" in k["name"]))
     step_end = max(k["e"] for k in ks)
     r = {"step_ms": step_end}
     if verbose:
@@ -85,7 +85,7 @@ def analyse(ks, lines, verbose):
         q[0] = min(q[0], k["s"]); q[1] = max(q[1], k["e"]); q[2] += k["e"] - k["s"]; q[3] += 1
     for p, (a, b, d, c) in ph.items():
         r["opt." + p] = d
-    bptt_end = max((k["e"] for k in by_stream[opt] if "k_lstm16<1>" in k["name"]), default=0.0)
+    bptt_end = max((k["e"] for k in by_stream[opt] if "k_lstm16_bptt" in k["name"]), default=0.0)
     opt_end = by_stream[opt][-1]["e"]
     r["opt_tail_ms"] = opt_end - bptt_end          # last BPTT step -> last kernel of the option stream
     # the other streams' last kernel that ends before the option stream does, and who waits for the option stream

@@ -622,13 +622,10 @@ void Engine::lstm_backward_step(LstmRun& r, int t) {
   if (r.route.bwd == LstmPath::Opt16) {
     const __half* g16 = r.gates16 + t * RG;
     __half* da16_t = r.da16 + t * RG;
-    if (last) {
-      LaunchCtx::Scope sc(&cx, "lstm_step_bwd_last", 0.0, R * (2.0 * G + 2.0 * G + 16.0 * H));
-      lstm16_bwd_last(cx, R, H, g16, cp, r.c + t * RH, r.bw_dh_last, r.scale2, mk, r.dc_carry, da16_t);
-    } else {
-      LaunchCtx::Scope sc(&cx, "lstm_step_bwd", 2.0 * R * G * H, R * (3.0 * 2.0 * G + 16.0 * H));
-      lstm16_step_bwd(cx, R, H, r.da16 + (t + 1) * RG, r.Whb16, g16, cp, r.c + t * RH, r.dc_carry, mk, da16_t);
-    }
+    // steps T - 2 .. 0 run in lstm_backward, all in one lstm16_bptt call
+    VD_REQUIRE(last, VD_E_STATE, "fp16 BPTT: lstm_backward runs the steps before the last one");
+    LaunchCtx::Scope sc(&cx, "lstm_step_bwd_last", 0.0, R * (2.0 * G + 2.0 * G + 16.0 * H));
+    lstm16_bwd_last(cx, R, H, g16, cp, r.c + t * RH, r.bw_dh_last, r.scale2, mk, r.dc_carry, da16_t);
     return;
   }
   LstmBwdStep s;
@@ -702,7 +699,20 @@ void Engine::lstm_backward_end(LstmRun& r, float* dx_out, float* dh0_out, float*
 void Engine::lstm_backward(LstmRun& r, const float* dh_all, const float* dh_last, const float* dc_last, float* dx_out,
                            float* dh0_out, float* dc0_out) {
   lstm_backward_begin(r, dh_all, dh_last, dc_last);
-  for (int t = r.T - 1; t >= 0; --t) lstm_backward_step(r, t);
+  if (r.route.bwd == LstmPath::Opt16) {
+    lstm_backward_step(r, r.T - 1);
+    if (r.T > 1) {
+      // every 128-row block runs steps T - 2 .. 0 in one launch, with its dc carry on chip: per row and step the HBM bytes
+      // are the fp16 gates in and da out and the fp32 c_{t-1} and c_t in (12 KB at H = 512), plus the carry in and out once
+      // (the block's da_{t+1} is read back from L2, where the cluster wrote it the step before)
+      const int H = r.H, G = 4 * r.H, S = r.T - 1;
+      const double R = (double)r.R;
+      LaunchCtx::Scope sc(&cx, "lstm_step_bwd", S * 2.0 * R * G * H, S * R * (2.0 * G + 2.0 * G + 8.0 * H) + R * 8.0 * H);
+      lstm16_bptt(cx, r.R, H, r.T, r.da16, r.Whb16, r.gates16, r.c, r.c0, r.mask, r.dc_carry);
+    }
+  } else {
+    for (int t = r.T - 1; t >= 0; --t) lstm_backward_step(r, t);
+  }
   lstm_backward_end(r, dx_out, dh0_out, dc0_out);
 }
 

@@ -271,8 +271,18 @@ bool lstm16_shape_ok(int64_t R, int H);
 void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, const __half* Wh16, const __half* ptable16,
                      const int32_t* tok, const float* bias, const float* c_prev, const int32_t* mask_ids, __half* gates16,
                      float* c_out, __half* h16_out, float* h32_out);
+// one BPTT step t < T - 1 (k_lstm16_bptt over one step): dc_carry is read and overwritten in place
 void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, const __half* Whb16, const __half* gates16,
                      const float* c_prev, const float* c_cur, float* dc_carry, const int32_t* mask_ids, __half* da16);
+// BPTT steps T - 2 .. 0 of a saved run (da16: T slices of (R, 4H), slice T - 1 written by lstm16_bwd_last; gates16 likewise;
+// c: T slices of (R, H); c0 the initial cell state or null; mask: T slices of R ids or null), in waves of clusters that each
+// run one 128-row block through every step with the dc carry on chip
+void lstm16_bptt(LaunchCtx& cx, int64_t R, int H, int T, __half* da16, const __half* Whb16, const __half* gates16, const float* c,
+                 const float* c0, const int32_t* mask, float* dc_carry);
+// its launch plan: clusters of csize = H / 128 CTAs, one per row block; `clusters` row blocks per launch (the last launch may
+// take fewer), `waves` launches
+struct Bptt16Plan { int csize, clusters, waves; };
+Bptt16Plan lstm16_bptt_plan(LaunchCtx& cx, int64_t R, int H);
 void lstm16_first_step(LaunchCtx& cx, int64_t R, int H, const __half* ptable16, const int32_t* tok, const float* bias,
                        const float* c_prev, const int32_t* mask_ids, __half* gates16, float* c_out, __half* h16_out, float* h32_out);
 void lstm16_bwd_last(LaunchCtx& cx, int64_t R, int H, const __half* gates16, const float* c_prev, const float* c_cur,

@@ -14,10 +14,18 @@
 //                    resident in shared memory (128 KB at H = 512) and streams only h_{t-1}; its two consumer warpgroups
 //                    contract their 64-row halves and take turns, so that one's main loop runs under the other's
 //                    epilogue; one 5-stage ring carries both halves' h_{t-1} rows in the order of the turns.
-//   k_lstm16<1>    : dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t, fp32 dc carry; a 4-stage ring of 32 KB
-//                    (A and B) stages shared by both consumer warpgroups.
+//   k_lstm16_bptt  : BPTT steps t_hi .. 0 in one launch: dh = da_{t+1} Wh (wgmma) -> backward pointwise -> fp16 da_t.  One
+//                    cluster of H / 128 CTAs per 128-row block (CTA u: hidden units 128u .. 128u + 127), a cluster barrier
+//                    between the steps (da_t of the whole block, written by the cluster, is the next step's A operand, read
+//                    back from L2); the fp32 dc carry stays on chip for all steps (half in registers, half in shared
+//                    memory).  A 4-stage ring of 32 KB (A and B) stages shared by both consumer warpgroups; 8 KB of
+//                    staging per consumer warp; 32 KB of carry: 224 KB of shared memory, 168 registers, no spills.
+//                    Launched in waves of as many clusters as fit in the SM budget (lstm16_bptt_plan); a one-step launch
+//                    is the step test hook.  Per row and step it moves 12 KB of HBM at H = 512 (gates in, da out, c_{t-1}
+//                    and c_t in) where one launch per step moved 20 KB (also da_{t+1} in and the carry in and out).
 //   Both run their pointwise epilogue on the accumulator registers (no shared-memory accumulator tile); the epilogue inputs
-//   are fetched by cp.async before the tile's contraction (the backward: those of its first 32 hidden units).
+//   are fetched by cp.async before the tile's contraction (the backward: those of its first 32 hidden units, during the
+//   cluster barrier before the step).
 //   k_atb16        : dWh += inv_scale * h^T da  (both operands MN-major fp16, 128 x 256 tiles, stream-K, red.global.add)
 //   k_lstm16_first / k_lstm16_bwd_last / k_segsum16 / k_cvt16 / k_amax / k_pick_scale : streaming helpers
 #include <cuda.h>
@@ -119,13 +127,11 @@ struct Lstm16Params {
   const int32_t* mask_ids;                     // maskzero ids or null
   float* h32_out;                              // optional fp32 copy of h (the step whose h meets fp32 consumers)
   int save_gates;
-  // backward
-  const __half* gsave; const float* c_cur; float* dc_carry;
 };
 struct Lstm16Maps { CUtensorMap g16, c, h16; };   // [R,4H] fp16 gates / da ; [R,H] fp32 c / dc ; [R,H] fp16 h: 16 x 32 boxes
 
 // ------------------------------------------------------------------------------------------------
-// MODE 0 = forward step, MODE 1 = backward step; warpgroup 0 = TMA producers, warpgroups 1-2 = consumers (64 rows each).
+// MODE 0 = forward step (the only specialisation); warpgroup 0 = TMA producers, warpgroups 1-2 = consumers (64 rows each).
 // Each consumer warp runs the pointwise epilogue of its 16 rows straight from its accumulator registers, 32 hidden units at a
 // time, with the inputs staged by cp.async in the T16 / T32 tiles above.
 template <int MODE> struct Cfg16;
@@ -152,170 +158,10 @@ struct Cfg16<0> {
   static_assert(TOTAL <= 232448, "k_lstm16<0>: shared memory");
 };
 
-// Backward: persistent over the tile list, one producer thread, a ring of 32 KB stages (A and B) shared by both consumers.
-template <>
-struct Cfg16<1> {
-  static constexpr int THREADS = 128 + 32 * EW16;
-  // per-warp staging: {4 gate tiles T16, c_prev, c_t, dc T32} = 10 KB
-  static constexpr int STG_PER_WARP = 4 * T16_BYTES + 3 * T32_BYTES;
-  static constexpr int STG_BYTES = EW16 * STG_PER_WARP;
-  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES) / STAGE16;      // 4
-  static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + 1024 + 256;
-};
-
+// The forward step is the k_lstm16<0> specialisation below; the BPTT runs k_lstm16_bptt.
 template <int MODE>
-__global__ void __launch_bounds__(Cfg16<MODE>::THREADS, 1)
-k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-         const __grid_constant__ Lstm16Maps em, const Lstm16Params p) {
-  static_assert(MODE == 1, "the forward step is the k_lstm16<0> specialisation below");
-  using C = Cfg16<MODE>;
-  constexpr int STAGES = C::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint8_t* stg_all = smem + STAGES * STAGE16;
-  uint64_t* full = (uint64_t*)(stg_all + C::STG_BYTES);
-  uint64_t* empty = full + STAGES;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int H = p.H;
-  const int num_m = (p.R + BM16 - 1) / BM16;
-  const int num_n = H / BN16;
-  const int num_tiles = num_m * num_n;
-  const int num_kb = 4 * H / BK16;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    if (threadIdx.x == 0) {
-      // ===== TMA producer: 128 rows of A, 128 rows of B per k-block
-      int s = 0; uint32_t ph = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m0 = (tile / num_n) * BM16;
-        const int nt = tile % num_n;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* sa = smem + s * STAGE16;
-          uint8_t* sb = sa + 16384;
-          mbar_expect_tx(&full[s], STAGE16);
-          tma_load_2d(sa, &tmA, &full[s], kb * BK16, m0);
-          tma_load_2d(sb, &tmB, &full[s], kb * BK16, nt * BN16);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else {
-    const int cw = warp - 4, wg = cw >> 2;
-    uint8_t* stg = stg_all + cw * C::STG_PER_WARP;
-    // fragment rows of this thread within the warp's 16, and the unit pair within a group of 8 columns
-    const int fr = lane >> 2, fu = 2 * (lane & 3);
-    int s = 0; uint32_t ph = 0;
-    // main loop of one tile: this warpgroup's 64 rows x 128 columns, accumulated in registers
-    auto contract = [&](float (&d)[BN16 / 2]) {
-#pragma unroll
-      for (int i = 0; i < BN16 / 2; ++i) d[i] = 0.f;
-      int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], ph);
-        const uint32_t sa = smem_u32(smem + s * STAGE16);
-        const uint64_t adesc = make_desc(sa + wg * 64 * 128, 16, 1024), bdesc = make_desc(sa + 16384, 16, 1024);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK16 / UK16; ++k)
-          wgmma_f16_n128(d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
-        prev = s;
-        if (++s == STAGES) { s = 0; ph ^= 1; }
-      }
-      wgmma_wait<0>();
-      wgmma_hold(d);
-      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
-    };
-    // ---- backward: 128 hidden units per tile = 4 groups of 32; fragment columns are hidden units, so the thread reads the
-    // gates / c / dc of exactly the units its accumulators hold.  The first group's inputs are fetched before the contraction.
-    uint8_t* sG = stg; uint8_t* sCP = stg + 4 * T16_BYTES; uint8_t* sCC = sCP + T32_BYTES; uint8_t* sDC = sCC + T32_BYTES;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m0 = (tile / num_n) * BM16;
-      const int nt = tile % num_n;
-      const int r0 = m0 + wg * 64 + (cw & 3) * 16;
-      const int64_t row = (int64_t)r0 + (lane & 15);
-      const bool row_ok = row < p.R;
-      const float keep = (row_ok && p.mask_ids && p.mask_ids[row] == 0) ? 0.f : 1.f;
-      const __half* grow = row_ok ? p.gsave + row * 4 * H : nullptr;
-      const float* cprow = (row_ok && p.c_prev) ? p.c_prev + row * H : nullptr;
-      const float* ccrow = row_ok ? p.c_cur + row * H : nullptr;
-      const float* dcrow = row_ok ? p.dc_carry + row * H : nullptr;
-      auto fetch = [&](int j) {                              // inputs of hidden units j .. j + 31 -> staging
-        if (lane == 0) bulk_wait_read0();
-        __syncwarp();
-#pragma unroll
-        for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, grow ? grow + g * H + j : nullptr, lane);
-        t32_load(sCP, cprow ? cprow + j : nullptr, lane);
-        t32_load(sCC, ccrow ? ccrow + j : nullptr, lane);
-        t32_load(sDC, dcrow ? dcrow + j : nullptr, lane);
-      };
-      fetch(nt * BN16);
-      float d[BN16 / 2];
-      contract(d);
-#pragma unroll
-      for (int grp = 0; grp < BN16 / 32; ++grp) {
-        const int j = nt * BN16 + grp * 32;
-        if (grp > 0) fetch(j);
-        cp_wait_all();
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int r = fr + 8 * hh;
-          const float keep_r = __shfl_sync(0xffffffffu, keep, r);
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const int u = 8 * jj + fu;
-            float g[4][2], cp[2], cc[2], dc[2], out[4][2], dcn[2];
-#pragma unroll
-            for (int gg = 0; gg < 4; ++gg) {
-              const float2 x = ld_h2(t16_at(sG + gg * T16_BYTES, r, u));
-              g[gg][0] = x.x; g[gg][1] = x.y;
-            }
-            const float2 cp2 = *reinterpret_cast<const float2*>(t32_at(sCP, r, u));
-            const float2 cc2 = *reinterpret_cast<const float2*>(t32_at(sCC, r, u));
-            const float2 dc2 = *reinterpret_cast<const float2*>(t32_at(sDC, r, u));
-            cp[0] = cp2.x; cp[1] = cp2.y; cc[0] = cc2.x; cc[1] = cc2.y; dc[0] = dc2.x; dc[1] = dc2.y;
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const float dh = d[4 * (4 * grp + jj) + 2 * hh + e];
-              const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
-              const float tcv = tanh16(cc[e]);
-              const float dd = (dc[e] + dh * go * (1.f - tcv * tcv)) * keep_r;
-              const float dhe = dh * keep_r;
-              out[0][e] = dd * gg_ * gi * (1.f - gi);
-              out[1][e] = dd * cp[e] * gf * (1.f - gf);
-              out[2][e] = dhe * tcv * go * (1.f - go);
-              out[3][e] = dd * gi * (1.f - gg_ * gg_);
-              dcn[e] = dd * gf;
-            }
-#pragma unroll
-            for (int gg = 0; gg < 4; ++gg) st_h2(t16_at(sG + gg * T16_BYTES, r, u), out[gg][0], out[gg][1]);
-            *reinterpret_cast<float2*>(t32_at(sDC, r, u)) = make_float2(dcn[0], dcn[1]);
-          }
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-#pragma unroll
-          for (int gg = 0; gg < 4; ++gg) tma_store_2d(&em.g16, sG + gg * T16_BYTES, gg * H + j, r0);
-          tma_store_2d(&em.c, sDC, j, r0);
-          bulk_commit();
-        }
-        __syncwarp();
-      }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
-  }
-}
+__global__ void k_lstm16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                         const __grid_constant__ Lstm16Maps em, const Lstm16Params p);
 
 // Forward step.  CTA b owns the column slice nt = b % num_n and walks the 128-row blocks b / num_n, + P, + 2P, ... (P =
 // gridDim.x / num_n CTAs per slice).  Thread 0 loads the slice once (one barrier per k-block, so the first contraction starts
@@ -494,6 +340,240 @@ k_lstm16<0>(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         bulk_commit();
       }
       __syncwarp();
+    }
+    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Backward (BPTT): one cluster of H / 128 CTAs per 128-row block runs the block's whole time loop, t = t_hi .. 0, in one
+// launch.  CTA u of the cluster owns hidden units 128u .. 128u + 127 of the block (its tile: dh = da_{t+1} Whb[units]^T over
+// all 4H of k), so the cluster's CTAs together write all 4H columns of the block's da_t, which is what every one of them reads
+// as its A operand at step t - 1: a cluster barrier between the steps is the only coupling (option rows are independent
+// sequences), clusters never wait on each other.  The fp32 cell-gradient carry dc stays on chip for the whole loop, in the
+// accumulator-fragment layout (64 floats per consumer thread: 32 in registers beside the 64 accumulators, 32 in shared
+// memory): it is read once before the first step and written once after the last.
+//
+// Visibility of da_t to the next step's TMA loads (async proxy -> global -> async proxy, across the CTAs of the cluster):
+//   1. every consumer warp waits until its bulk stores of da_t are complete (cp.async.bulk.wait_group 0 — not .read, which
+//      only says that the staging tiles may be reused);
+//   2. fence.proxy.async.global orders them against the generic-proxy release that follows;
+//   3. barrier.cluster.arrive.release by every thread, barrier.cluster.wait.acquire by every thread;
+//   4. only then does the producer thread, after one more fence.proxy.async.global, issue the TMA loads of da_t.
+// The producer may run ahead of its consumers into the next step's loads only as far as this barrier.
+struct Bptt16 {
+  static constexpr int THREADS = 128 + 32 * EW16;
+  // per-warp staging: {4 gate tiles T16 (the inputs, overwritten by da), c_{t-1}, c_t T32} = 8 KB
+  static constexpr int STG_PER_WARP = 4 * T16_BYTES + 2 * T32_BYTES;
+  static constexpr int STG_BYTES = EW16 * STG_PER_WARP;                       // 64 KB
+  static constexpr int DCS_BYTES = 256 * (BN16 / 4) * 4;                    // half of the dc carry: 32 KB
+  static constexpr int STAGES = (232448 - 1024 - 256 - STG_BYTES - DCS_BYTES) / STAGE16;   // 4
+  static constexpr int TOTAL = STAGES * STAGE16 + STG_BYTES + DCS_BYTES + 1024 + 256;    // + alignment slack + barriers
+  static_assert(STAGES >= 4 && TOTAL <= 232448, "k_lstm16_bptt: shared memory");
+  // the producer warpgroup hands registers to the consumers (128 x 40 + 256 x 232 <= 64 K): without it the consumers spill
+  static constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+};
+struct Bptt16Params {
+  int R, H;
+  int mb0;                                 // row block of cluster 0; cluster c runs block mb0 + c
+  int t_hi;                                // steps t_hi, t_hi - 1, ..., 0
+  const __half* gates; int64_t g_step;     // saved fp16 gates of step t at gates + t g_step, (R, 4H)
+  const float* c; int64_t c_step;          // c_t at c + t c_step, (R, H); c_{t-1} likewise, and c0 (null: zeros) for t = 0
+  const float* c0;
+  const int32_t* mask; int64_t m_step;     // maskzero ids of step t at mask + t m_step, or null
+  float* dc_carry;                         // (R, H) fp32: the carry into step t_hi in, the carry out of step 0 out
+};
+
+__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+
+// tmA: da_{t+1} of step t as slice z = t of an (R, 4H) x z tensor, 128 x 64 boxes; tmB: Whb (H, 4H), 128 x 64 boxes;
+// tmD: da_t as slice z = t, 16 x 32 boxes (SWIZZLE_64B, the T16 staging tiles)
+__global__ void __launch_bounds__(Bptt16::THREADS, 1)
+k_lstm16_bptt(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+              const __grid_constant__ CUtensorMap tmD, const Bptt16Params p) {
+  using C = Bptt16;
+  constexpr int STAGES = C::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+  uint8_t* stg_all = smem + STAGES * STAGE16;
+  uint64_t* full = (uint64_t*)(stg_all + C::STG_BYTES + C::DCS_BYTES);
+  uint64_t* empty = full + STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int H = p.H;
+  const int num_n = H / BN16;                                  // = the cluster size (a 1-D grid of 1-D clusters)
+  const int nt = blockIdx.x % num_n;
+  const int m0 = (p.mb0 + blockIdx.x / num_n) * BM16;
+  const int num_kb = 4 * H / BK16;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(C::PRODUCER_REGS));
+    // ===== TMA producer: 128 rows of A, 128 rows of B per k-block.  Every thread of the warpgroup takes part in the
+    // cluster barrier between the steps; thread 0 issues the loads.
+    int s = 0; uint32_t ph = 0;
+    for (int t = p.t_hi; t >= 0; --t) {
+      if (t < p.t_hi) { cluster_arrive_release(); cluster_wait_acquire(); }   // da_t of step t + 1 is in global memory
+      if (threadIdx.x == 0) {
+        if (t < p.t_hi) fence_proxy_async_global();
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[s], ph ^ 1);
+          uint8_t* sa = smem + s * STAGE16;
+          uint8_t* sb = sa + 16384;
+          mbar_expect_tx(&full[s], STAGE16);
+          tma_load_3d(sa, &tmA, &full[s], kb * BK16, m0, t);
+          tma_load_2d(sb, &tmB, &full[s], kb * BK16, nt * BN16);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(C::CONSUMER_REGS));
+    const int cw = warp - 4, wg = cw >> 2;
+    uint8_t* stg = stg_all + cw * C::STG_PER_WARP;
+    // fragment rows of this thread within the warp's 16, and the unit pair within a group of 8 columns
+    const int fr = lane >> 2, fu = 2 * (lane & 3);
+    int s = 0; uint32_t ph = 0;
+    // main loop of one step: this warpgroup's 64 rows x 128 columns, accumulated in registers
+    auto contract = [&](float (&d)[BN16 / 2]) {
+#pragma unroll
+      for (int i = 0; i < BN16 / 2; ++i) d[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[s], ph);
+        const uint32_t sa = smem_u32(smem + s * STAGE16);
+        const uint64_t adesc = make_desc(sa + wg * 64 * 128, 16, 1024), bdesc = make_desc(sa + 16384, 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK16 / UK16; ++k)
+          wgmma_f16_n128(d, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+    };
+    // 128 hidden units per tile = 4 groups of 32; fragment columns are hidden units, so the thread reads the gates / c of
+    // exactly the units its accumulators (and its dc carry) hold
+    uint8_t* sG = stg; uint8_t* sCP = stg + 4 * T16_BYTES; uint8_t* sCC = sCP + T32_BYTES;
+    const int r0 = m0 + wg * 64 + (cw & 3) * 16;               // first of the warp's 16 rows
+    const int64_t row = (int64_t)r0 + (lane & 15);             // lanes l and l + 16 both describe row l % 16
+    const bool row_ok = row < p.R;
+    const int j0 = nt * BN16;
+    // the dc carry in d's layout: element i = 4 jb + 2 hh + e is dc of row r0 + fr + 8 hh, unit j0 + 8 jb + fu + e.  The
+    // first two groups' (i < 32) live in registers, the last two's in shared memory, [i - 32][consumer thread] (a warp's
+    // accesses are 32 consecutive words): all 64 beside the 64 accumulators do not fit in the 168 registers of a thread.
+    float dcr[BN16 / 4];
+    float* dcs = reinterpret_cast<float*>(stg_all + C::STG_BYTES) + (threadIdx.x - 128);
+    auto dc_at = [&](int i) -> float& { return i < BN16 / 4 ? dcr[i] : dcs[(i - BN16 / 4) * 256]; };
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int64_t rr = (int64_t)r0 + fr + 8 * hh;
+#pragma unroll
+      for (int jb = 0; jb < BN16 / 8; ++jb) {
+        const float2 v = rr < p.R ? *reinterpret_cast<const float2*>(p.dc_carry + rr * H + j0 + 8 * jb + fu) : make_float2(0.f, 0.f);
+        dc_at(4 * jb + 2 * hh) = v.x; dc_at(4 * jb + 2 * hh + 1) = v.y;
+      }
+    }
+    // inputs of step t, hidden units j .. j + 31 -> staging.  The row is made opaque to the compiler, so that the addresses
+    // derived from it are formed here instead of being hoisted out of the step loop, where they would spill
+    auto fetch = [&](int t, int j) {
+      int64_t row = (int64_t)r0 + (lane & 15);
+      asm volatile("" : "+l"(row));
+      const __half* grow = row_ok ? p.gates + t * p.g_step + row * 4 * H : nullptr;
+      const float* cpbase = t > 0 ? p.c + (t - 1) * p.c_step : p.c0;
+      const float* cprow = (row_ok && cpbase) ? cpbase + row * H : nullptr;
+      const float* ccrow = row_ok ? p.c + t * p.c_step + row * H : nullptr;
+      if (lane == 0) bulk_wait_read0();
+      __syncwarp();
+#pragma unroll
+      for (int g = 0; g < 4; ++g) t16_load(sG + g * T16_BYTES, grow ? grow + g * H + j : nullptr, lane);
+      t32_load(sCP, cprow ? cprow + j : nullptr, lane);
+      t32_load(sCC, ccrow ? ccrow + j : nullptr, lane);
+    };
+    fetch(p.t_hi, j0);
+    for (int t = p.t_hi; t >= 0; --t) {
+      const float keep = (row_ok && p.mask && p.mask[t * p.m_step + row] == 0) ? 0.f : 1.f;
+      float d[BN16 / 2];
+      contract(d);
+#pragma unroll
+      for (int grp = 0; grp < BN16 / 32; ++grp) {
+        const int j = j0 + grp * 32;
+        if (grp > 0) fetch(t, j);
+        cp_wait_all();
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = fr + 8 * hh;
+          const float keep_r = __shfl_sync(0xffffffffu, keep, r);
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int u = 8 * jj + fu;
+            float g[4][2], cp[2], cc[2], out[4][2];
+#pragma unroll
+            for (int gg = 0; gg < 4; ++gg) {
+              const float2 x = ld_h2(t16_at(sG + gg * T16_BYTES, r, u));
+              g[gg][0] = x.x; g[gg][1] = x.y;
+            }
+            const float2 cp2 = *reinterpret_cast<const float2*>(t32_at(sCP, r, u));
+            const float2 cc2 = *reinterpret_cast<const float2*>(t32_at(sCC, r, u));
+            cp[0] = cp2.x; cp[1] = cp2.y; cc[0] = cc2.x; cc[1] = cc2.y;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int i = 4 * (4 * grp + jj) + 2 * hh + e;
+              const float dh = d[i];
+              const float gi = g[0][e], gf = g[1][e], go = g[2][e], gg_ = g[3][e];
+              const float tcv = tanh16(cc[e]);
+              const float dd = (dc_at(i) + dh * go * (1.f - tcv * tcv)) * keep_r;
+              const float dhe = dh * keep_r;
+              out[0][e] = dd * gg_ * gi * (1.f - gi);
+              out[1][e] = dd * cp[e] * gf * (1.f - gf);
+              out[2][e] = dhe * tcv * go * (1.f - go);
+              out[3][e] = dd * gi * (1.f - gg_ * gg_);
+              dc_at(i) = dd * gf;
+            }
+#pragma unroll
+            for (int gg = 0; gg < 4; ++gg) st_h2(t16_at(sG + gg * T16_BYTES, r, u), out[gg][0], out[gg][1]);
+          }
+        }
+        fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+#pragma unroll
+          for (int gg = 0; gg < 4; ++gg) tma_store_3d(&tmD, sG + gg * T16_BYTES, gg * H + j, r0, t);
+          bulk_commit();
+        }
+        __syncwarp();
+      }
+      if (t > 0) {
+        if (lane == 0) {
+          asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // this warp's da_t is in global memory
+          fence_proxy_async_global();
+        }
+        __syncwarp();
+        cluster_arrive_release();
+        fetch(t - 1, j0);                                      // the next step's first inputs fly across the barrier
+        cluster_wait_acquire();                                // (pairs the arrive; nothing here reads da_t)
+      }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int64_t rr = (int64_t)r0 + fr + 8 * hh;
+      if (rr < p.R) {
+#pragma unroll
+        for (int jb = 0; jb < BN16 / 8; ++jb)
+          *reinterpret_cast<float2*>(p.dc_carry + rr * H + j0 + 8 * jb + fu) = make_float2(dc_at(4 * jb + 2 * hh), dc_at(4 * jb + 2 * hh + 1));
+      }
     }
     if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all TMA stores performed
   }
@@ -850,7 +930,8 @@ static void launch16(LaunchCtx& cx, const CUtensorMap& tA, const CUtensorMap& tB
 
 }  // namespace tc
 
-bool lstm16_shape_ok(int64_t R, int H) { return H % 256 == 0 && H <= 512 && R >= 1024; }
+// H = 256 or 512: the BPTT's clusters are H / 128 = 2 or 4 CTAs
+bool lstm16_shape_ok(int64_t R, int H) { return (H == 256 || H == 512) && R >= 1024; }
 
 void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, const __half* Wh16, const __half* ptable16,
                      const int32_t* tok, const float* bias, const float* c_prev, const int32_t* mask_ids, __half* gates16,
@@ -872,19 +953,92 @@ void lstm16_step_fwd(LaunchCtx& cx, int64_t R, int H, const __half* h_prev16, co
   launch16<0>(cx, tA, tB, em, p, slices * balanced_workers(cdiv(R, BM16), std::max(1, cx.sms() / slices)));
 }
 
+Bptt16Plan lstm16_bptt_plan(LaunchCtx& cx, int64_t R, int H) {
+  using namespace tc;
+  VD_REQUIRE(lstm16_shape_ok(R, H), VD_E_STATE, "lstm16_bptt_plan: shape");
+  const int csize = H / BN16;
+  // clusters of k_lstm16_bptt the device can hold at once, per cluster size (the kernel's shared memory gives one CTA per SM)
+  static std::mutex mu;
+  static std::map<std::pair<int, int>, int> fit;
+  int dev = 0;
+  VD_CUDA_CHECK(cudaGetDevice(&dev));
+  int maxc = 0;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    int& f = fit[{dev, csize}];
+    if (f == 0) {
+      VD_CUDA_CHECK(cudaFuncSetAttribute(k_lstm16_bptt, cudaFuncAttributeMaxDynamicSharedMemorySize, Bptt16::TOTAL));
+      cudaLaunchConfig_t cfg = {};
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = csize; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+      cfg.gridDim = dim3(csize * std::max(1, cx.sm_count / csize)); cfg.blockDim = dim3(Bptt16::THREADS); cfg.dynamicSmemBytes = Bptt16::TOTAL;
+      cfg.attrs = attr; cfg.numAttrs = 1;
+      VD_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&f, k_lstm16_bptt, &cfg));
+      VD_REQUIRE(f >= 1, VD_E_STATE, "k_lstm16_bptt: no cluster fits on the device");
+    }
+    maxc = f;
+  }
+  // as many clusters as fit and as the SM budget allows, balanced over the waves
+  const int num_m = cdiv(R, BM16);
+  Bptt16Plan pl;
+  pl.csize = csize;
+  pl.clusters = balanced_workers(num_m, std::max(1, std::min(maxc, cx.sms() / csize)));
+  pl.waves = cdiv(num_m, pl.clusters);
+  return pl;
+}
+
+// steps t_hi .. 0 of every row block, a wave of clusters per launch.  The tensors of step t: da_{t+1} = slice t of da_in
+// (z slices of (R, 4H)), da_t -> slice t of da_out, gates / c / mask at base + t step.
+static void lstm16_bptt_run(LaunchCtx& cx, int64_t R, int H, int t_hi, const __half* da_in, __half* da_out, const __half* Whb16,
+                            const __half* gates16, int64_t g_step, const float* c, int64_t c_step, const float* c0,
+                            const int32_t* mask, int64_t m_step, float* dc_carry) {
+  using namespace tc;
+  const Bptt16Plan pl = lstm16_bptt_plan(cx, R, H);
+  const int64_t G = 4 * (int64_t)H;
+  auto map3 = [&](const __half* base, int box_rows, int box_cols, CUtensorMapSwizzle swz) {
+    CUtensorMap tm;
+    cuuint64_t dims[3] = {(cuuint64_t)G, (cuuint64_t)R, (cuuint64_t)(t_hi + 1)};
+    cuuint64_t strides[2] = {(cuuint64_t)G * 2, (cuuint64_t)(R * G * 2)};
+    cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = get_encode()(&tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)base, dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) throw CudaError(-3, "cuTensorMapEncodeTiled (lstm16 bptt) failed (" + std::to_string((int)r) + ")");
+    return tm;
+  };
+  const CUtensorMap tA = map3(da_in, BM16, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
+  const CUtensorMap tB = tmap_h(Whb16, H, G, G, 128, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
+  const CUtensorMap tD = map3(da_out, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
+  Bptt16Params p = {};
+  p.R = (int)R; p.H = H; p.t_hi = t_hi;
+  p.gates = gates16; p.g_step = g_step; p.c = c; p.c_step = c_step; p.c0 = c0; p.mask = mask; p.m_step = m_step;
+  p.dc_carry = dc_carry;
+  const int num_m = cdiv(R, BM16);
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = pl.csize; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  for (int mb0 = 0; mb0 < num_m; mb0 += pl.clusters) {
+    p.mb0 = mb0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(pl.csize * std::min(pl.clusters, num_m - mb0)); cfg.blockDim = dim3(Bptt16::THREADS);
+    cfg.dynamicSmemBytes = Bptt16::TOTAL; cfg.stream = cx.stream; cfg.attrs = attr; cfg.numAttrs = 1;
+    VD_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_lstm16_bptt, tA, tB, tD, p));
+    check_launch(cx, "k_lstm16_bptt");
+  }
+}
+
 void lstm16_step_bwd(LaunchCtx& cx, int64_t R, int H, const __half* da_next16, const __half* Whb16, const __half* gates16,
                      const float* c_prev, const float* c_cur, float* dc_carry, const int32_t* mask_ids, __half* da16) {
-  using namespace tc;
   VD_REQUIRE(lstm16_shape_ok(R, H), VD_E_STATE, "lstm16_step_bwd: shape");
-  Lstm16Params p = {};
-  p.R = (int)R; p.H = H; p.gsave = gates16; p.c_prev = c_prev; p.c_cur = c_cur; p.dc_carry = dc_carry; p.mask_ids = mask_ids;
-  CUtensorMap tA = tmap_h(da_next16, R, 4 * (int64_t)H, 4 * (int64_t)H, BM16, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
-  CUtensorMap tB = tmap_h(Whb16, H, 4 * (int64_t)H, 4 * (int64_t)H, 128, BK16, CU_TENSOR_MAP_SWIZZLE_128B);
-  Lstm16Maps em;
-  em.g16 = tmap_h(da16, R, 4 * (int64_t)H, 4 * (int64_t)H, 16, 32, CU_TENSOR_MAP_SWIZZLE_64B);
-  em.c = tmap_f(dc_carry, R, H, H, 16, 32, CU_TENSOR_MAP_SWIZZLE_128B);
-  em.h16 = em.c;
-  launch16<1>(cx, tA, tB, em, p, balanced_workers(cdiv(R, BM16) * (H / BN16), cx.sms()));
+  lstm16_bptt_run(cx, R, H, 0, da_next16, da16, Whb16, gates16, 0, c_cur, 0, c_prev, mask_ids, 0, dc_carry);
+}
+
+void lstm16_bptt(LaunchCtx& cx, int64_t R, int H, int T, __half* da16, const __half* Whb16, const __half* gates16, const float* c,
+                 const float* c0, const int32_t* mask, float* dc_carry) {
+  VD_REQUIRE(lstm16_shape_ok(R, H) && T >= 2, VD_E_STATE, "lstm16_bptt: shape");
+  const int64_t RG = R * 4 * H;
+  lstm16_bptt_run(cx, R, H, T - 2, da16 + RG, da16, Whb16, gates16, RG, c, R * H, c0, mask, R, dc_carry);
 }
 
 void lstm16_first_step(LaunchCtx& cx, int64_t R, int H, const __half* ptable16, const int32_t* tok, const float* bias,

@@ -33,6 +33,11 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
 // ---- warpgroup MMA (wgmma, sm_90a).  A warpgroup = 4 consecutive warps starting at a multiple of 4; each wgmma
 // computes a 64-row slab, fp32 accumulators in registers: thread (warp w, lane l) holds rows 16(w%4) + l/4 (+8) and
 // columns 8j + 2(l%4) (+1) as d[4j + {0,1,2,3}] = {(r,c), (r,c+1), (r+8,c), (r+8,c+1)}.
@@ -143,6 +148,10 @@ __device__ __forceinline__ const float* shfl_ptr(const float* p, int src_lane) {
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* tm, const void* smem_src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }

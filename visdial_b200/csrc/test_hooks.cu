@@ -390,6 +390,22 @@ const Entry TABLE[] = {
          VD_CUDA_CHECK(cudaStreamDestroy(cs[1].stream));
        }
      }},
+    // ---- the fp16 option-LSTM BPTT (lstm16.cu, k_lstm16_bptt) over steps T - 2 .. 0 in waves of clusters.  ptrs da16 (T slices
+    // of (R, 4H); slice T - 1 is the input), Whb16 (H, 4H), gates16 (T slices of (R, 4H)), c (T slices of (R, H)), c0 (R, H) or
+    // null, mask ids (T slices of R) or null, dc_carry (R, H, in and out), plan (3 int64: cluster size, row blocks per launch,
+    // launches; may be null).  ints R, H, T, SM budget (0: all SMs)
+    {"lstm16_bptt", 8, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       LaunchCtx cx;
+       cx.sm_count = e->cx.sm_count; cx.sm_budget = IN(3); cx.stream = e->cx.stream;
+       lstm16_bptt(cx, I[0], IN(1), IN(2), H16(0), CH16(1), CH16(2), CF(3), CF(4), CI32(5), F(6));
+       if (P[7]) {
+         const Bptt16Plan pl = lstm16_bptt_plan(cx, I[0], IN(1));
+         const int64_t v[3] = {pl.csize, pl.clusters, pl.waves};
+         VD_CUDA_CHECK(cudaMemcpyAsync(P[7], v, sizeof(v), cudaMemcpyHostToDevice, e->cx.stream));
+         VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+       }
+     }},
     {"segsum_rows16", 5, 3, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        segsum_rows16(e->cx, static_cast<const __half*>(P[0]), I[0], CI32(1), CI32(2), I[1], F(3), IN(2), CF(4));
