@@ -116,6 +116,30 @@ int vd_set_dropout_seed(vd_engine* e, uint64_t seed, uint64_t iteration);
 #define VD_MATH_F16 2         /* TF32 mode + the many-row option LSTM (disc.lua:4-20) with fp16 operands and fp16 saved state
                                  (h, gates, da, x-projection table), fp32 accumulation, fp32 cell state and gradients */
 int vd_set_math_mode(vd_engine* e, int32_t mode);
+/* Answer rules (DESIGN §25): classes barred from every token choice of a gen model's answering calls, beam search (plain,
+ * diverse, n-best) and sampling (plain, truncated), for whole splits, dialogs and dialog asks alike, until changed.  At step
+ * t the answer so far has t - 1 words w[1 .. t-1] (the row's own earlier tokens; a beam's pads are 0):
+ *  - min_words m >= 0: end_token is barred while t <= m, so every finished answer has at least m words;
+ *  - no_repeat_ngram n >= 0 (0 = off): a word is barred if it would complete an n-gram already in w (a window holding a pad
+ *    matches nothing, <START> is in no n-gram, end_token is never barred by this rule); n = 1 bars every word already used;
+ *  - banned: n_banned <= 1024 ids in [1, vocabSize], never chosen.
+ * If a row's barred set would cover every class, end_token is allowed.  Scores and log-probabilities stay the unconstrained
+ * LogSoftMax's.  A beam row with fewer allowed classes than the beam lists what it has; sampling draws from the allowed
+ * classes with the same keys, so a draw is unchanged whenever its unconstrained token is allowed.  Active rules send
+ * sampling through the materialised-logits route in every math mode.  vd_gen_sample and vd_gen_truncated_sample take no
+ * end_token: their <END> is vocabSize (the dataloader's).
+ * r = NULL turns the rules off (the default: every call is then exactly what it is without them).  Refused with VD_E_BADARG,
+ * keeping the old rules: a negative count, n_banned > 1024, banned NULL with n_banned > 0, an id outside [1, vocabSize], or
+ * active rules with vocabSize > 49152 (a row's barred set is a bit mask in shared memory).  While active, an answering call
+ * is refused with VD_E_BADARG, before any state changes, when its end_token is banned, or when min_words > beam_len - 2
+ * (beam search) / beam_len - 1 (sampling).  Disc retrieval, training, evaluation and vd_gen_decoder_step ignore them. */
+typedef struct vd_answer_rules {
+  int32_t min_words;
+  int32_t no_repeat_ngram;
+  int32_t n_banned;
+  const int32_t* banned; /* HOST, n_banned ids; copied by the call */
+} vd_answer_rules;
+int vd_set_answer_rules(vd_engine* e, const vd_answer_rules* r);
 /* gen decoder: on = 1 lets vd_decoder_forward keep the (rows, vocabSize) log-probabilities on chip when the caller only
  * passes decOut on to the criterion (decoder:forward -> criterion:forward, model.lua:313-314): decOut_dev is then NULL, the
  * projection's epilogue keeps the softmax statistics and the target log-probability, and vd_criterion_backward recomputes the

@@ -65,6 +65,10 @@ int vd_gen_dialog_nbest_beam_search(vd_engine* e, const vd_batch* b, int32_t bea
                                     float length_penalty, int32_t nbest, int32_t beam_len, int32_t start_token,
                                     int32_t end_token, int32_t hist_width, int32_t max_ans_len, int32_t* answer_host,
                                     int32_t* length_host, double* score_host, double* norm_host, int32_t* hist_host);
+typedef struct vd_answer_rules {
+  int32_t min_words; int32_t no_repeat_ngram; int32_t n_banned; const int32_t* banned;
+} vd_answer_rules;
+int vd_set_answer_rules(vd_engine* e, const vd_answer_rules* r);
 int vd_gen_truncated_sample(vd_engine* e, int32_t beam_len, int32_t start_token, float temperature, uint64_t seed,
                             int64_t row_offset, int32_t top_k, float top_p, int32_t* answer_host, float* logp_host);
 int vd_gen_dialog_truncated_sample(vd_engine* e, const vd_batch* b, int32_t beam_len, int32_t start_token, int32_t end_token,

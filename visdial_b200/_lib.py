@@ -57,6 +57,11 @@ class vd_corpus_desc(C.Structure):
             "img_pos", "num_rounds", "images")])
 
 
+class vd_answer_rules(C.Structure):
+    _fields_ = [("min_words", C.c_int32), ("no_repeat_ngram", C.c_int32), ("n_banned", C.c_int32),
+                ("banned", C.POINTER(C.c_int32))]
+
+
 _P = C.POINTER
 _H = C.c_void_p  # vd_engine*
 
@@ -78,6 +83,7 @@ SIGNATURES = {
     "vd_set_training": [_H, C.c_int32],
     "vd_set_dropout_seed": [_H, C.c_uint64, C.c_uint64],
     "vd_set_math_mode": [_H, C.c_int32],
+    "vd_set_answer_rules": [_H, _P(vd_answer_rules)],
     "vd_set_option_overlap": [_H, C.c_int32, C.c_int32],
     "vd_encoder_forward": [_H, _P(vd_batch), _P(C.c_void_p)],
     "vd_forward_connect": [_H],

@@ -239,6 +239,7 @@ def main(opt: dict, rank: int = 0, world: int = 1):
         params.update({k: opt[k] for k in ("lengthPenalty", "nBest") if k in opt})
         if model.params["decoder"] == "gen":         # a disc pool's topK is its retrieval list: the truncation is gen's
             params.update({k: opt[k] for k in ("topK", "topP") if k in opt})
+            params.update(cli.answer_rule_params(opt))
         R = model.params["maxQuesCount"]
         if opt["serve"]:
             serve(model, dl, split, index, params, opt["capacity"])

@@ -95,16 +95,22 @@ TRUNCATION_OPTIONS = [
     ("topK", 0, "Sampling: draw from the topK most likely words only (0 = all)"),
     ("topP", 1.0, "Sampling: draw from the fewest most likely words holding topP of the probability (1 = all)"),
 ]
-# the generate command's table: generate.lua's options above, diverse beam search, n-best lists, truncated sampling, and
-# which history each round is answered with
+# answer rules (DESIGN §25): words barred from every beam-search or sampling step of a gen model's answers
+ANSWER_RULE_OPTIONS = [
+    ("minWords", 0, "Answers: <END> is barred until the answer has minWords words"),
+    ("noRepeatNgram", 0, "Answers: no n-gram of this many words occurs twice in an answer (0 = off)"),
+    ("bannedWords", "", "Answers: comma-separated words never generated (e.g. UNK)"),
+]
+# the generate command's table: generate.lua's options above, diverse beam search, n-best lists, truncated sampling, answer
+# rules, and which history each round is answered with
 HISTORY_MODES = ("gt", "generated")
-GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + NBEST_OPTIONS + TRUNCATION_OPTIONS + [
+GENERATE_COMMAND_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + NBEST_OPTIONS + TRUNCATION_OPTIONS + ANSWER_RULE_OPTIONS + [
     ("history", "gt", "History each round is answered with: gt (the dataset's) | generated (the dialog's own answers)"),
 ]
 
-# the chat command: generate's options, diverse beam search, n-best lists, truncated sampling, and which images are talked
-# about with which questions
-CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + NBEST_OPTIONS + TRUNCATION_OPTIONS + [
+# the chat command: generate's options, diverse beam search, n-best lists, truncated sampling, answer rules, and which images
+# are talked about with which questions
+CHAT_OPTIONS = GENERATE_OPTIONS + DIVERSE_OPTIONS + NBEST_OPTIONS + TRUNCATION_OPTIONS + ANSWER_RULE_OPTIONS + [
     ("split", "val", "Split the images and captions come from"),
     ("imageIds", "", "Comma-separated COCO image ids of the split (default: the -questions file's, else its first image)"),
     ("questions", "", "JSON {image_id: [question, ...]}: ask these and write results.json; else read stdin, one per line"),
@@ -181,6 +187,11 @@ def parse(options, argv=None, prog=None) -> dict:
             fail("-topP must be in (0, 1]")
         if not truncated_sampling(opt):         # options that change nothing leave the run's options as they were
             del opt["topK"], opt["topP"]
+    if "minWords" in opt:
+        if opt["minWords"] < 0 or opt["noRepeatNgram"] < 0:
+            fail("-minWords and -noRepeatNgram must be >= 0")
+        if not answer_rules_active(opt):        # options that change nothing leave the run's options as they were
+            del opt["minWords"], opt["noRepeatNgram"], opt["bannedWords"]
     if opt["gpus"] < 1:
         fail("-gpus must be at least 1")
     if opt["gpuid"] < 0:
@@ -206,17 +217,36 @@ def truncated_sampling(opt: dict) -> bool:
     return opt.get("sampleWords", 0) == 1 and (opt.get("topK", 0) > 0 or opt.get("topP", 1.0) < 1.0)
 
 
+def banned_words(opt: dict) -> list:
+    """-bannedWords as a list of words (empty entries dropped)"""
+    return [w.strip() for w in opt.get("bannedWords", "").split(",") if w.strip()]
+
+
+def answer_rules_active(opt: dict) -> bool:
+    """-minWords > 0, -noRepeatNgram > 0 or a -bannedWords word"""
+    return opt.get("minWords", 0) > 0 or opt.get("noRepeatNgram", 0) > 0 or bool(banned_words(opt))
+
+
+def answer_rule_params(opt: dict) -> dict:
+    """the answer rules as generateAnswers / DialogPool params (none when inactive)"""
+    if not answer_rules_active(opt):
+        return {}
+    return {"minWords": opt.get("minWords", 0), "noRepeatNgram": opt.get("noRepeatNgram", 0), "bannedWords": banned_words(opt)}
+
+
 def written_opts(opt: dict) -> dict:
     """The options a results.json records: the diverse beam search options only when they change the search
     (-beamGroups > 1), the n-best options only when one differs from its default (-lengthPenalty 0, -nBest 1), and the
     truncation options only when they truncate a sampling run (-sampleWords 1 with -topK > 0 or -topP < 1), so that every
-    run without them writes the file it wrote before they existed."""
+    run without them writes the file it wrote before they existed.  The answer rules likewise, only when active."""
     plain = opt.get("beamGroups", 1) == 1
+    unruled = not answer_rules_active(opt)
     untruncated = not truncated_sampling(opt)
     unlisted = all(opt.get(n, d) == d for n, d, _ in NBEST_OPTIONS)
     return {k: v for k, v in opt.items()
             if not (plain and k in ("beamGroups", "diversity")) and not (untruncated and k in ("topK", "topP"))
-            and not (unlisted and k in ("lengthPenalty", "nBest"))}
+            and not (unlisted and k in ("lengthPenalty", "nBest"))
+            and not (unruled and k in ("minWords", "noRepeatNgram", "bannedWords"))}
 
 
 def model_params(opt: dict) -> dict:

@@ -171,6 +171,13 @@ int vd_set_math_mode(vd_engine* h, int32_t mode) {
     e->math_mode = mode;
   })
 }
+int vd_set_answer_rules(vd_engine* h, const vd_answer_rules* r) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    if (r) e->set_answer_rules(r->min_words, r->no_repeat_ngram, r->n_banned, r->banned);
+    else e->set_answer_rules(0, 0, 0, nullptr);
+  })
+}
 
 int vd_encoder_forward(vd_engine* h, const vd_batch* b, const float** encOut) {
   VD_TRY({ Engine* e = ENG(h); e->encoder_forward(b); if (encOut) *encOut = e->encOut; })

@@ -148,6 +148,29 @@ __host__ __device__ __forceinline__ bool trunc_active(const TruncCfg& t, int V) 
 // the widest vocabulary whose row (4 V bytes of y) fits the truncated sampler's shared-memory stage beside its histograms
 constexpr int TRUNC_MAX_V = 49152;
 
+// Answer rules (DESIGN §25): classes barred from a generation step's choice, in beam search and sampling alike.  At step stp
+// of row r, t[1 .. stp-1] are the row's own earlier tokens (t[0] = <START>), read from hist + r * ld.
+//  1. banned: the n_banned ids in [1, V] are never candidates.
+//  2. min_words m: end_token is barred while stp <= m (the answer so far has stp - 1 words).
+//  3. no_repeat_ngram n (0 = off): w is barred if for some j >= 1 with j + n - 1 <= stp - 1, t[j .. j+n-2] equals
+//     t[stp-n+1 .. stp-1] and t[j+n-1] == w; a window holding a 0 (a pad) matches nothing; end_token is never barred here.
+//     n = 1 bars every token already in the answer.
+//  4. fallback: if every class is barred, end_token is allowed.
+// Scores are untouched: logp stays the unconstrained LogSoftMax.  The numpy twin is tests/answer_rules_twin.py.
+struct AnswerRules {
+  int32_t min_words = 0, no_repeat_ngram = 0, n_banned = 0;
+  const int32_t* banned = nullptr;   // device (n_banned)
+  int32_t end_token = 0;
+  int32_t step = 0;
+  const int32_t* hist = nullptr;     // device: row r's tokens at hist + r * ld (beam search: the pre-merge beams (rows, L);
+  int64_t ld = 0;                    // sampling: the answer (rows, L + 1))
+};
+__host__ __device__ __forceinline__ bool rules_active(int32_t min_words, int32_t no_repeat_ngram, int32_t n_banned) {
+  return min_words > 0 || no_repeat_ngram > 0 || n_banned > 0;
+}
+// one bit per class: the barred set of a row lives in shared memory
+constexpr int RULES_MASK_WORDS = TRUNC_MAX_V / 32;
+
 // ---------------------------------------------------------------------------------------------
 // Launch context: stream + launch accounting + optional per-class event bracketing.
 // ---------------------------------------------------------------------------------------------

@@ -215,6 +215,7 @@ Engine::~Engine() {
   for (auto& g : dense_buf) g.release();
   dialog_hist.release();
   beam_lp.release();
+  rules_banned.release();
   for (auto& g : dialog_out) g.release();
   if (copy_stream) {
     cudaStreamSynchronize(copy_stream); cudaStreamDestroy(copy_stream);
@@ -1754,6 +1755,7 @@ void Engine::gen_beam_search(int k, int G, float lam, int L, int start_token, in
                              int32_t* length_host, double* score_host, const NBestCfg& nc) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_beam_search needs the gen decoder after encoder_forward");
   check_beam_args(k, G, lam, L, nc);
+  check_rules(L, end_token, true);
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
@@ -1766,6 +1768,41 @@ void Engine::gen_beam_search(int k, int G, float lam, int L, int start_token, in
   if (nc.norm_host)
     VD_CUDA_CHECK(cudaMemcpyAsync(nc.norm_host, res.gnorm, (size_t)NG * sizeof(double), cudaMemcpyDeviceToHost, cx.stream));
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+}
+
+void Engine::set_answer_rules(int32_t min_words, int32_t no_repeat_ngram, int32_t n_banned, const int32_t* banned_host) {
+  VD_REQUIRE(min_words >= 0 && no_repeat_ngram >= 0 && n_banned >= 0, VD_E_BADARG, "answer rules: counts must be >= 0");
+  VD_REQUIRE(n_banned <= 1024, VD_E_BADARG, "answer rules: at most 1024 banned ids");
+  VD_REQUIRE(banned_host || n_banned == 0, VD_E_BADARG, "answer rules: null banned ids");
+  for (int i = 0; i < n_banned; ++i)
+    VD_REQUIRE(banned_host[i] >= 1 && banned_host[i] <= cfg.V, VD_E_BADARG, "answer rules: a banned id outside [1, vocabSize]");
+  const bool active = rules_active(min_words, no_repeat_ngram, n_banned);
+  VD_REQUIRE(!active || cfg.V <= TRUNC_MAX_V, VD_E_BADARG, "answer rules keep a row's barred set in shared memory: vocabSize <= 49152");
+  if (n_banned > 0) {
+    VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
+    int32_t* d = (int32_t*)rules_banned.ensure((size_t)n_banned * sizeof(int32_t));
+    VD_CUDA_CHECK(cudaMemcpy(d, banned_host, (size_t)n_banned * sizeof(int32_t), cudaMemcpyHostToDevice));
+  }
+  rules.min_words = min_words;
+  rules.no_repeat_ngram = no_repeat_ngram;
+  rules.banned.assign(banned_host, banned_host + n_banned);
+  rules.active = active;
+}
+
+void Engine::check_rules(int L, int end_token, bool beam) const {
+  if (!rules.active) return;
+  VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "answer rules: end_token in [1, vocabSize]");
+  for (int32_t b : rules.banned) VD_REQUIRE(b != end_token, VD_E_BADARG, "answer rules: end_token is banned");
+  VD_REQUIRE(rules.min_words <= (beam ? L - 2 : L - 1), VD_E_BADARG,
+             beam ? "answer rules: min_words > beam_len - 2 (no answer could finish)" : "answer rules: min_words > beam_len - 1");
+}
+
+AnswerRules Engine::answer_rules(int end_token, int step, const int32_t* hist, int64_t ld) const {
+  AnswerRules a;
+  a.min_words = rules.min_words; a.no_repeat_ngram = rules.no_repeat_ngram; a.n_banned = (int32_t)rules.banned.size();
+  a.banned = a.n_banned ? (const int32_t*)rules_banned.p : nullptr;
+  a.end_token = end_token; a.step = step; a.hist = hist; a.ld = ld;
+  return a;
 }
 
 void Engine::check_beam_args(int k, int G, float lam, int L, const NBestCfg& nc) const {
@@ -1855,12 +1892,14 @@ Engine::BeamResult Engine::beam_search_rows(int64_t n, int64_t stride, int64_t o
     const float* h[2] = {fed[0], fed[1]};
     const float* c[2] = {fed[2], fed[3]};
     gen_decoder_step_logits(rows, tok, h, c);
-    logsoftmax_topk_rows(cx, gstep_logp, tok, rows, cfg.V, k, tv, ti);
     const int a = (stp - 1) & 1;
+    // the answer rules read each row's pre-merge beam: positions 1 .. stp-1 are its words so far
+    const AnswerRules ar = answer_rules(end_token, stp, beams[a], L);
+    logsoftmax_topk_rows(cx, gstep_logp, tok, rows, cfg.V, k, tv, ti, rules.active ? &ar : nullptr);
     // the top-k lists, the scores and beams in and out
     LaunchCtx::Scope sc(&cx, "beam_merge", 0.0, 8.0 * rows * k + 16.0 * rows + 8.0 * rows * (stp + 1));
     beam_merge(cx, N, stp, k, G, lam, L, end_token, tv, ti, scores[a], scores[a ^ 1], beams[a], beams[a ^ 1], tok, parent, lists,
-               pick_ans, pick_ans ? res.len : nullptr, pick_ans ? res.score : nullptr);
+               pick_ans, pick_ans ? res.len : nullptr, pick_ans ? res.score : nullptr, rules.active);
   }
   return res;
 }
@@ -1870,6 +1909,7 @@ void Engine::gen_sample(int L, int start_token, float temperature, uint64_t seed
                         float* logp_host, const TruncCfg& tr) {
   VD_REQUIRE(cfg.dec == DEC_GEN && have_fwd, VD_E_STATE, "gen_sample needs the gen decoder after encoder_forward");
   check_sample_args(L, start_token, temperature, row_offset, tr);
+  check_rules(L, cfg.V, false);                    // no end_token argument: <END> is vocabSize, the dataloader's
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   cx.stream = main_stream;
@@ -1898,7 +1938,7 @@ void Engine::check_sample_args(int L, int start_token, float temperature, int64_
 // (n, L + 1) and log-probabilities (n, L) in the arena, valid until the next encoder forward.
 Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature,
                                          uint64_t seed, int64_t row_offset, int64_t draw_stride, int64_t draw_off,
-                                         const int64_t* draw_rounds, const TruncCfg& tr) {
+                                         const int64_t* draw_rounds, const TruncCfg& tr, int end_token) {
   forward_connect();
   const int H = cfg.H, V = cfg.V;
   const int64_t N = n;
@@ -1912,9 +1952,10 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
   const int nparts = vocab_lse_nparts(V);
   float *pm = nullptr, *ps = nullptr, *pk = nullptr, *px = nullptr;
   int32_t* pc = nullptr;
-  // active truncation needs each row's boundaries before its draw, which the fused epilogue cannot have: the rows route
-  const bool trunc = trunc_active(tr, V);
-  if (tcmode() && !trunc) {
+  // active truncation needs each row's boundaries before its draw, and active answer rules its barred set, which the fused
+  // epilogue cannot have: the rows route
+  const bool trunc = trunc_active(tr, V), rows_route = trunc || rules.active;
+  if (tcmode() && !rows_route) {
     pm = arena.get<float>(N * nparts); ps = arena.get<float>(N * nparts); pk = arena.get<float>(N * nparts);
     px = arena.get<float>(N * nparts); pc = arena.get<int32_t>(N * nparts);
   }
@@ -1946,7 +1987,7 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
     gen_decoder_step_lstm(N, tok, h, c);
     smp.step = (uint32_t)stp;
     bool took = false;
-    if (tcmode() && !trunc && (stp == 1 || fused)) {
+    if (tcmode() && !rows_route && (stp == 1 || fused)) {
       LaunchCtx::Scope sc(&cx, "vocab_sample", 2.0 * N * V * H, 4.0 * (N * (double)H + (double)V * H + 5.0 * N * nparts));
       took = vocab_sample_tc(cx, (int)N, V, H, gstep2.h, H, Wp(wo), H, Wp(wo + 1), smp, pm, ps, pk, pc, px);
       if (took) vocab_sample_finish(cx, pm, ps, pk, pc, px, nparts, N, stp, L, tok, ans, lp);
@@ -1960,8 +2001,11 @@ Engine::SampleResult Engine::sample_rows(int64_t n, int64_t stride, int64_t off,
                           4.0 * (N * (double)H + (double)V * H + (trunc ? 4.0 : 2.0) * N * V));
       float* logits = arena.get<float>(N * V);
       linear_fwd(wo, gstep2.h, N, logits, 0);
-      if (trunc) truncated_sample_rows(cx, logits, N, V, smp, tr, L, tok, ans, lp);
-      else logsoftmax_sample_rows(cx, logits, N, V, smp, L, tok, ans, lp);
+      // the answer rules read each row's answer so far: positions 1 .. stp-1
+      const AnswerRules ar = answer_rules(end_token > 0 ? end_token : V, stp, ans, L + 1);
+      const AnswerRules* arp = rules.active ? &ar : nullptr;
+      if (trunc) truncated_sample_rows(cx, logits, N, V, smp, tr, L, tok, ans, lp, arp);
+      else logsoftmax_sample_rows(cx, logits, N, V, smp, L, tok, ans, lp, arp);
     }
     h[0] = gstep1.h; h[1] = gstep2.h;
     c[0] = gstep1.c; c[1] = gstep2.c;
@@ -2017,6 +2061,7 @@ void Engine::gen_dialog_beam_search(const vd_batch* b, int k, int G, float lam, 
                                     int32_t* hist_host, const NBestCfg& nc) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_beam_search needs the gen decoder");
   check_beam_args(k, G, lam, L, nc);
+  check_rules(L, end_token, true);
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
   VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
   const int R = cfg.R;
@@ -2051,6 +2096,7 @@ void Engine::gen_dialog_sample(const vd_batch* b, int L, int start_token, int en
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "gen_dialog_sample needs the gen decoder");
   check_sample_args(L, start_token, temperature, row_offset, tr);
   VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
+  check_rules(L, end_token, false);
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   VD_REQUIRE(b != nullptr && b->B > 0, VD_E_SHAPE, "batch B must be > 0");
   const int R = cfg.R;
@@ -2058,7 +2104,7 @@ void Engine::gen_dialog_sample(const vd_batch* b, int L, int start_token, int en
   int32_t* ans = (int32_t*)dialog_out[0].ensure((size_t)N * (L + 1) * sizeof(int32_t));
   float* lp = (float*)dialog_out[3].ensure((size_t)N * L * sizeof(float));
   gen_dialog(b, W, max_ans_len, [&](int r) {
-    const SampleResult res = sample_rows(B, R, r, L, start_token, temperature, seed, row_offset, -1, 0, nullptr, tr);
+    const SampleResult res = sample_rows(B, R, r, L, start_token, temperature, seed, row_offset, -1, 0, nullptr, tr, end_token);
     scatter_round(cx.stream, ans, res.ans, (size_t)(L + 1) * sizeof(int32_t), R, r, B);
     scatter_round(cx.stream, lp, res.logp, (size_t)L * sizeof(float), R, r, B);
     // the samples before the first <END>
@@ -2599,6 +2645,7 @@ void Engine::dialog_ask_beam(const int32_t* slots, int64_t n, const int32_t* que
                              const NBestCfg& nc) {
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a beam-search ask needs the gen decoder");
   check_beam_args(k, G, lam, L, nc);
+  check_rules(L, end_token, true);
   VD_REQUIRE(start_token >= 1 && start_token <= cfg.V && end_token >= 1 && end_token <= cfg.V, VD_E_BADARG,
              "start_token and end_token in [1, vocabSize]");
   VD_REQUIRE(answer_host && length_host && score_host, VD_E_BADARG, "null output pointer");
@@ -2622,11 +2669,12 @@ void Engine::dialog_ask_sample(const int32_t* slots, int64_t n, const int32_t* q
   VD_REQUIRE(cfg.dec == DEC_GEN, VD_E_STATE, "a sampling ask needs the gen decoder");
   check_sample_args(L, start_token, temperature, row_offset, tr);
   VD_REQUIRE(end_token >= 1 && end_token <= cfg.V, VD_E_BADARG, "end_token in [1, V]");
+  check_rules(L, end_token, false);
   VD_REQUIRE(answer_host, VD_E_BADARG, "null answer pointer");
   dialog_check_ask(slots, n, ques_host, Tq);
   run_ask(this, slots, n, ques_host, Tq, row_offset, [&](const AskRows& rows) {
     // row i draws as global round row_offset + draw_base[slot] + its round (vd_dialog_begin: vd_gen_dialog_sample's rows)
-    const SampleResult res = sample_rows(n, 1, 0, L, start_token, temperature, seed, 0, -1, 0, rows.draw, tr);
+    const SampleResult res = sample_rows(n, 1, 0, L, start_token, temperature, seed, 0, -1, 0, rows.draw, tr, end_token);
     VD_CUDA_CHECK(cudaMemcpyAsync(answer_host, res.ans, (size_t)n * (L + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, cx.stream));
     if (logp_host)
       VD_CUDA_CHECK(cudaMemcpyAsync(logp_host, res.logp, (size_t)n * L * sizeof(float), cudaMemcpyDeviceToHost, cx.stream));

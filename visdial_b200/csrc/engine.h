@@ -333,6 +333,16 @@ struct Engine {
   void gen_beam_search(int k, int G, float lam, int L, int start_token, int end_token, int32_t* answer_host, int32_t* length_host,
                        double* score_host, const NBestCfg& nc = {});
   void check_beam_args(int k, int G, float lam, int L, const NBestCfg& nc = {}) const;
+  // answer rules (DESIGN §25): barred classes in every beam search and sampling step while active; off by default.  The
+  // banned ids live on the device (rules_banned) and on the host (for the refusals).
+  struct Rules { int32_t min_words = 0, no_repeat_ngram = 0; std::vector<int32_t> banned; bool active = false; } rules;
+  GrowBuf rules_banned;
+  void set_answer_rules(int32_t min_words, int32_t no_repeat_ngram, int32_t n_banned, const int32_t* banned_host);
+  // refuses (VD_E_BADARG) a call the active rules cannot serve: end_token banned, or min_words > L - 2 (beam search: a
+  // finished answer needs step min_words + 1 <= L - 1) / L - 1 (sampling)
+  void check_rules(int L, int end_token, bool beam) const;
+  // the rules of step `step` over row histories hist (row pitch ld)
+  AnswerRules answer_rules(int end_token, int step, const int32_t* hist, int64_t ld) const;
   // lp[0 .. L-1] on the device, computed with the host's pow once per call (null for alpha 0: every lp is 1)
   GrowBuf beam_lp;
   const double* length_penalty_table(float alpha, int L);
@@ -352,11 +362,11 @@ struct Engine {
   // its sampling on n rounds as beam_search_rows takes them; row i draws as global round
   // row_offset + i * draw_stride + draw_off (draw_stride < 0: the state's stride and offset)
   struct SampleResult { int32_t* ans; float* logp; };                   // (n, L + 1), (n, L)
-  // (draw_rounds non-null, device (n): row i draws as global round draw_rounds[i] instead).  Active truncation takes the
-  // rows route in every math mode.
+  // (draw_rounds non-null, device (n): row i draws as global round draw_rounds[i] instead).  Active truncation and active
+  // answer rules take the rows route in every math mode.  end_token: the rules' <END> (0: vocabSize, the dataloader's).
   SampleResult sample_rows(int64_t n, int64_t stride, int64_t off, int L, int start_token, float temperature, uint64_t seed,
                            int64_t row_offset, int64_t draw_stride = -1, int64_t draw_off = 0,
-                           const int64_t* draw_rounds = nullptr, const TruncCfg& tr = {});
+                           const int64_t* draw_rounds = nullptr, const TruncCfg& tr = {}, int end_token = 0);
   // dialogs on the model's own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample): R rounds of {encoder forward on
   // the engine-owned history, round r's search, the history append} on the device
   struct DialogAnswers {             // where round r's answers are, for the history append

@@ -185,8 +185,9 @@ void scale_copy(LaunchCtx& cx, float* dst, const float* src, int64_t n, float al
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H);
 // the k <= 32 best log-probabilities per row and their classes (value desc, class asc), never writing the log-probabilities:
 // lse from the same row_lse as logsoftmax_rows, so the values are logsoftmax_rows' bits
+// ar (DESIGN §25): the answer rules' barred classes take no part; entries past a row's allowed count are (-inf, -1)
 void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
-                          int32_t* topi);
+                          int32_t* topi, const AnswerRules* ar = nullptr);
 // the whole search on the device (Engine::gen_beam_search): beams (rows, L) = <start> then pads, tokens = <start>, scores = 0
 void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* beams, int32_t* tokens, double* scores);
 // Each group's list of its n best finished hypotheses (DESIGN §24), ordered by (norm desc, step asc, candidate asc), norm =
@@ -208,16 +209,17 @@ struct BeamLists {
 void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int L, int end_token, const float* topv,
                 const int32_t* topi, const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out,
                 int32_t* tokens, int32_t* parent, const BeamLists& lists, int32_t* pick_ans, int32_t* pick_len,
-                double* pick_score);
+                double* pick_score, bool skip_empty = false);   // skip_empty: -inf entries are no candidates (DESIGN §25)
 // the sampling step from materialised logits, one block per row: lse from the same row_lse as logsoftmax_rows (so logp is
 // the bits it would give), the Gumbel-max draw of common.cuh; writes as vocab_sample_finish
+// ar (DESIGN §25): the answer rules' barred classes take no part in the draw
 void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,
-                            int32_t* answer, float* logp);
+                            int32_t* answer, float* logp, const AnswerRules* ar = nullptr);
 // its truncated form (common.cuh's TruncCfg rule, DESIGN §23): the same draw over the top-k / top-p prefix of each row, logp
 // still logsoftmax_rows' bits.  V <= TRUNC_MAX_V (the row is staged in shared memory); VD_E_BADARG otherwise, or for
 // top_k < 0 or top_p outside (0, 1].
 void truncated_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, const TruncCfg& tr,
-                           int L, int32_t* tokens, int32_t* answer, float* logp);
+                           int L, int32_t* tokens, int32_t* answer, float* logp, const AnswerRules* ar = nullptr);
 // the dialog loop's history (Engine::gen_dialog), one CTA per dialog b of hist (B, R, W), right-aligned rows.
 // r < 0: row 0 <- row b*R of src (B*R, src_w), right-aligned into W >= src_w; rows 1.. <- pads.
 // r >= 0: row r+1 <- round r's write (DESIGN §17): Q = the words of question row b*R + r of src (B*R, src_w), A = the first

@@ -1080,6 +1080,41 @@ __global__ void k_logsoftmax_rows(float* __restrict__ x, const int32_t* __restri
   for (int c = threadIdx.x; c < V; c += blockDim.x) row[c] -= lse;
 }
 
+// ---- answer rules (common.cuh's AnswerRules, DESIGN §25) ------------------------------------------------------------
+__device__ __forceinline__ bool is_barred(const uint32_t* bar, int c) { return (bar[c >> 5] >> (c & 31)) & 1u; }
+__device__ __forceinline__ void set_barred(uint32_t* bar, int c) { atomicOr(&bar[c >> 5], 1u << (c & 31)); }
+
+// Row r's barred set as a V-bit mask in shared memory (bit c: class c, token c + 1), built by the whole block: banned ids,
+// <END> while stp <= min_words, the n-gram scan (start j = 1 .. stp-n per thread, n - 1 compares each), the fallback.
+// Returns the number of allowed classes (>= 1) on every thread.  red: block_sum's 33 floats (exact: counts < 2^24).
+__device__ __forceinline__ int build_barred(const AnswerRules& ar, int64_t r, int V, uint32_t* bar, float* red) {
+  const int nw = (V + 31) >> 5, stp = ar.step, n = ar.no_repeat_ngram;
+  for (int i = threadIdx.x; i < nw; i += blockDim.x) bar[i] = 0u;
+  __syncthreads();
+  for (int i = threadIdx.x; i < ar.n_banned; i += blockDim.x) set_barred(bar, ar.banned[i] - 1);
+  if (threadIdx.x == 0 && stp <= ar.min_words) set_barred(bar, ar.end_token - 1);
+  if (n > 0) {
+    const int32_t* t = ar.hist + r * ar.ld;
+    for (int j = 1 + (int)threadIdx.x; j <= stp - n; j += blockDim.x) {
+      bool match = true;
+      for (int i = 0; i < n - 1 && match; ++i) {
+        const int32_t a = t[j + i];
+        match = a != 0 && a == t[stp - n + 1 + i];
+      }
+      const int32_t w = t[j + n - 1];
+      if (match && w != ar.end_token && (unsigned)(w - 1) < (unsigned)V) set_barred(bar, w - 1);
+    }
+  }
+  __syncthreads();
+  int cnt = 0;
+  for (int i = threadIdx.x; i < nw; i += blockDim.x) cnt += __popc(bar[i]);
+  const int allowed = V - (int)block_sum((float)cnt, red);
+  if (allowed > 0) return allowed;
+  if (threadIdx.x == 0) { const int c = ar.end_token - 1; bar[c >> 5] &= ~(1u << (c & 31)); }   // the fallback
+  __syncthreads();
+  return 1;
+}
+
 // (v, c) precedes (w, d) in torch.topk's order with the pinned tie rule: value descending, class ascending
 __device__ __forceinline__ bool topk_before(float v, int c, float w, int d) { return v > w || (v == w && c < d); }
 
@@ -1089,24 +1124,42 @@ __device__ __forceinline__ bool topk_before(float v, int c, float w, int d) { re
 // Each thread keeps the KMAX best (x - lse, class) pairs of its strided columns, sorted, in registers; the block then pops
 // k winners from the thread heads.  A row whose mask id is 0 is all zeros in k_logsoftmax_rows (MaskZero): its top k is
 // classes 0..k-1 with value 0.
-template <int KMAX>
+// RULES: the answer rules' barred classes (ar, DESIGN §25) take no part; the list is the k best allowed classes, its entries
+// past the allowed count (-inf, -1), and a pad row lists the first k allowed classes with value 0.
+template <int KMAX, bool RULES>
 __global__ void __launch_bounds__(256) k_logsoftmax_topk_rows(const float* __restrict__ x, const int32_t* __restrict__ mask_ids,
-                                                              int V, int k, float* __restrict__ topv, int32_t* __restrict__ topi) {
+                                                              int V, int k, float* __restrict__ topv, int32_t* __restrict__ topi,
+                                                              AnswerRules ar) {
   __shared__ float red[33];
   __shared__ float sv[8];
   __shared__ int si[8];
   __shared__ int win;
+  __shared__ uint32_t bar[RULES ? RULES_MASK_WORDS : 1];
   const int64_t r = blockIdx.x;
   if (mask_ids && mask_ids[r] == 0) {
-    for (int j = threadIdx.x; j < k; j += blockDim.x) { topv[r * k + j] = 0.f; topi[r * k + j] = j; }
+    if constexpr (RULES) {
+      build_barred(ar, r, V, bar, red);
+      if (threadIdx.x == 0) {
+        int j = 0;
+        for (int w = 0; w * 32 < V && j < k; ++w) {
+          uint32_t f = ~bar[w] & (V - w * 32 >= 32 ? 0xffffffffu : (1u << (V - w * 32)) - 1u);   // allowed classes
+          for (; f && j < k; f &= f - 1, ++j) { topv[r * k + j] = 0.f; topi[r * k + j] = w * 32 + __ffs(f) - 1; }
+        }
+        for (; j < k; ++j) { topv[r * k + j] = -INFINITY; topi[r * k + j] = -1; }
+      }
+    } else {
+      for (int j = threadIdx.x; j < k; j += blockDim.x) { topv[r * k + j] = 0.f; topi[r * k + j] = j; }
+    }
     return;
   }
   const float* row = x + r * V;
   const float lse = row_lse(row, V, red);
+  if constexpr (RULES) build_barred(ar, r, V, bar, red);
   float lv[KMAX]; int lc[KMAX];
 #pragma unroll
   for (int i = 0; i < KMAX; ++i) { lv[i] = -INFINITY; lc[i] = 0x7fffffff; }
   for (int c = threadIdx.x; c < V; c += blockDim.x) {
+    if (RULES && is_barred(bar, c)) continue;
     float v = row[c] - lse;
     if (!topk_before(v, c, lv[KMAX - 1], lc[KMAX - 1])) continue;
     int ci = c;
@@ -1131,7 +1184,8 @@ __global__ void __launch_bounds__(256) k_logsoftmax_topk_rows(const float* __res
     if (threadIdx.x == 0) {
       for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
         if (topk_before(sv[w], si[w], bv, bi)) { bv = sv[w]; bi = si[w]; }
-      topv[r * k + j] = bv; topi[r * k + j] = bi;
+      const bool none = RULES && bi == 0x7fffffff;           // fewer than k allowed classes
+      topv[r * k + j] = none ? -INFINITY : bv; topi[r * k + j] = none ? -1 : bi;
       win = bi;
     }
     __syncthreads();
@@ -1192,17 +1246,24 @@ __device__ __forceinline__ int row_gumbel_argmax(const SampleCfg& smp, int64_t r
 }
 
 // The sampling step from materialised logits, one block per row.  The lse comes from row_lse, so x_tok - lse is the
-// log-probability k_logsoftmax_rows would write.
+// log-probability k_logsoftmax_rows would write.  RULES: the answer rules' barred classes (ar, DESIGN §25) take no part in
+// the draw; the allowed classes' keys are unchanged.
+template <bool RULES>
 __global__ void __launch_bounds__(256) k_logsoftmax_sample_rows(const float* __restrict__ x, int V, SampleCfg smp, int L,
                                                                 int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
-                                                                float* __restrict__ logp) {
+                                                                float* __restrict__ logp, AnswerRules ar) {
   __shared__ float red[33];
   __shared__ float sk[8];
   __shared__ int sc[8];
+  __shared__ uint32_t bar[RULES ? RULES_MASK_WORDS : 1];
   const int64_t r = blockIdx.x;
   const float* row = x + r * V;
   const float lse = row_lse(row, V, red);
-  const int bc = row_gumbel_argmax(smp, r, V, [&](int j, float& y) { y = row[j] / smp.temperature; return true; }, sk, sc);
+  if constexpr (RULES) build_barred(ar, r, V, bar, red);
+  const int bc = row_gumbel_argmax(smp, r, V, [&](int j, float& y) {
+    y = row[j] / smp.temperature;
+    return !RULES || !is_barred(bar, j);
+  }, sk, sc);
   if (threadIdx.x == 0) {
     tokens[r] = bc + 1;
     answer[r * (L + 1) + smp.step] = bc + 1;
@@ -1279,17 +1340,18 @@ __device__ __forceinline__ TruncSel trunc_radix_select(const float* ys, int V, u
   return {prefix, acc};
 }
 
-// the class of the n-th (1-based) class of key t in class order: each thread counts a contiguous chunk, a block scan
-// finds the chunk, its thread walks it
-__device__ __forceinline__ int trunc_nth_of_key(const float* ys, int V, uint32_t t, uint32_t n, TruncShared& s) {
+// the class of the n-th (1-based) class of key t in class order among the classes in(j) admits: each thread counts a
+// contiguous chunk, a block scan finds the chunk, its thread walks it
+template <typename In>
+__device__ __forceinline__ int trunc_nth_of_key(const float* ys, int V, uint32_t t, uint32_t n, TruncShared& s, In in) {
   const int per = (V + blockDim.x - 1) / blockDim.x, b = threadIdx.x * per, e = min(V, b + per);
   uint32_t c = 0;
-  for (int j = b; j < e; ++j) c += trunc_key(ys[j]) == t;
+  for (int j = b; j < e; ++j) c += trunc_key(ys[j]) == t && in(j);
   const uint32_t incl = block_incl_scan(c, reinterpret_cast<uint32_t*>(s.scan));
   if (incl - c < n && n <= incl) {
     uint32_t seen = incl - c;
     for (int j = b; j < e; ++j)
-      if (trunc_key(ys[j]) == t && ++seen == n) { s.sel_class = j; break; }
+      if (trunc_key(ys[j]) == t && in(j) && ++seen == n) { s.sel_class = j; break; }
   }
   __syncthreads();
   return s.sel_class;
@@ -1300,31 +1362,39 @@ __device__ __forceinline__ int trunc_nth_of_key(const float* ys, int V, uint32_t
 // classes are a prefix of (y desc, class asc), held as its last element (tk, tc): key > tk, or key == tk and class <= tc.
 // top-k and top-p each find their boundary key by radix select (counts, then integer masses over the top-k prefix) and
 // the boundary class among that key's ties by a block scan in class order; the draw is row_gumbel_argmax over the prefix.
+// RULES: the answer rules' barred classes (ar, DESIGN §25) are out of the row before truncation: they count in neither
+// top-k nor the masses, m is the allowed classes' maximum, and the draw skips them.  Their bit mask follows ys in the stage.
+template <bool RULES>
 __global__ void __launch_bounds__(256) k_truncated_sample_rows(const float* __restrict__ x, int V, SampleCfg smp, TruncCfg tr,
                                                                int L, int32_t* __restrict__ tokens, int32_t* __restrict__ answer,
-                                                               float* __restrict__ logp) {
+                                                               float* __restrict__ logp, AnswerRules ar) {
   extern __shared__ float ys[];
   __shared__ TruncShared s;
   const int64_t r = blockIdx.x;
   const float* row = x + r * V;
+  uint32_t* bar = reinterpret_cast<uint32_t*>(ys + V);
+  int nal = V;                                                   // allowed classes
+  if constexpr (RULES) nal = build_barred(ar, r, V, bar, s.red);
+  const auto in = [&](int j) { return !RULES || !is_barred(bar, j); };
   float m = -INFINITY;
   for (int j = threadIdx.x; j < V; j += blockDim.x) {
     const float y = row[j] / smp.temperature;
     ys[j] = y;
-    m = fmaxf(m, y);
+    if (in(j)) m = fmaxf(m, y);
   }
   m = block_max(m, s.red);                                       // its barriers also publish ys
   uint32_t tk = 0;                                               // key 0 is below every y: all classes kept
   int tc = 0x7fffffff;
-  if (tr.top_k >= 1 && tr.top_k < V) {
-    const TruncSel k = trunc_radix_select(ys, V, (unsigned long long)tr.top_k, [](int, uint32_t) { return 1ull; }, s);
+  if (tr.top_k >= 1 && tr.top_k < nal) {
+    const TruncSel k = trunc_radix_select(ys, V, (unsigned long long)tr.top_k,
+                                          [&](int j, uint32_t) { return in(j) ? 1ull : 0ull; }, s);
     tk = k.key;
-    tc = trunc_nth_of_key(ys, V, tk, (uint32_t)(tr.top_k - k.above), s);
+    tc = trunc_nth_of_key(ys, V, tk, (uint32_t)(tr.top_k - k.above), s, in);
   }
   if (tr.top_p < 1.f) {
     const uint32_t k0 = tk;
     const int c0 = tc;
-    auto mass = [&](int j, uint32_t k) { return (k > k0 || (k == k0 && j <= c0)) ? trunc_mass(ys[j], m) : 0ull; };
+    auto mass = [&](int j, uint32_t k) { return (in(j) && (k > k0 || (k == k0 && j <= c0))) ? trunc_mass(ys[j], m) : 0ull; };
     unsigned long long S = 0;
     for (int j = threadIdx.x; j < V; j += blockDim.x) S += mass(j, trunc_key(ys[j]));
     S = block_incl_scan(S, s.scan);
@@ -1340,12 +1410,12 @@ __global__ void __launch_bounds__(256) k_truncated_sample_rows(const float* __re
     unsigned long long n = (unsigned long long)((double)rem / (double)qt);
     while (n * qt < rem) ++n;
     while (n > 1 && (n - 1) * qt >= rem) --n;
-    tc = trunc_nth_of_key(ys, V, tk, (uint32_t)n, s);
+    tc = trunc_nth_of_key(ys, V, tk, (uint32_t)n, s, in);
   }
   const int bc = row_gumbel_argmax(smp, r, V, [&](int j, float& y) {
     y = ys[j];
     const uint32_t k = trunc_key(y);
-    return k > tk || (k == tk && j <= tc);
+    return in(j) && (k > tk || (k == tk && j <= tc));
   }, s.sk, s.sc);
   const float lse = row_lse(row, V, s.red);                      // last: nothing long-lived across the selection
   if (threadIdx.x == 0) {
@@ -1378,6 +1448,8 @@ __global__ void __launch_bounds__(256) k_truncated_sample_rows(const float* __re
 // BeamLists says.  At the last step (stp == L - 1) the lists are written in order to out_* (n > 1), and pick_* (N, L),
 // (N), (N), or null, take the best of the G list heads by (x desc, group asc), groups without a finished hypothesis skipped
 // (pick_len 0 when none).
+// SKIP (the answer rules, DESIGN §25): a top-k entry of value -inf is no candidate; it finishes nothing and fills no column.
+template <bool SKIP>
 __global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float lam, int L, int end_token, const BeamLists lst,
                                                    const float* __restrict__ topv, const int32_t* __restrict__ topi,
                                                    const double* __restrict__ sc_in, double* __restrict__ sc_out,
@@ -1449,6 +1521,7 @@ __global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float 
         const int idx = entry(q);
         if (ti[idx] + 1 != end_token) continue;
         const double s = sc[idx / k] + (double)tv[idx];
+        if (SKIP && s == -INFINITY) continue;                // scores are finite: only a -inf entry gives -inf
         const double x = __ddiv_rn(s, lpv);
         if (!(x < xn || (x == xn && q > xq))) continue;
         if (!fnd || x > fx) { fnd = true; fx = x; fs = s; fq = q; }
@@ -1508,6 +1581,7 @@ __global__ void __launch_bounds__(32) k_beam_merge(int stp, int k, int G, float 
         const int idx = entry(q);
         if (ti[idx] + 1 == end_token) continue;
         double s = sc[idx / k] + (double)tv[idx];
+        if (SKIP && s == -INFINITY) continue;
         if (const int cnt = count(q)) s -= __dmul_rn(lamd, (double)cnt);
         if (!(s < ps || (s == ps && q > pq))) continue;
         if (!ok || s > bs) { ok = true; bs = s; bq = q; }
@@ -2001,36 +2075,60 @@ void vocab_sample_finish(LaunchCtx& cx, const float* part_max, const float* part
                          const float* part_x, int nparts, int64_t rows, int step, int L, int32_t* tokens, int32_t* answer, float* logp) {
   L1D(k_vocab_sample_finish, rows, part_max, part_sum, part_key, part_cls, part_x, nparts, rows, step, L, tokens, answer, logp);
 }
+static void check_rules(const AnswerRules* ar, int V) {
+  if (!ar) return;
+  VD_REQUIRE(V >= 1 && V <= TRUNC_MAX_V, VD_E_BADARG, "answer rules need V in [1, 49152] (the row's bit mask)");
+  VD_REQUIRE(ar->min_words >= 0 && ar->no_repeat_ngram >= 0 && ar->n_banned >= 0 && ar->n_banned <= 1024 &&
+             (ar->banned || ar->n_banned == 0) && ar->end_token >= 1 && ar->end_token <= V && ar->step >= 1 &&
+             (ar->hist || ar->no_repeat_ngram == 0) && ar->ld > 0,
+             VD_E_BADARG, "answer rules: counts, banned ids, end_token, step or history");
+}
 void logsoftmax_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, int L, int32_t* tokens,
-                            int32_t* answer, float* logp) {
+                            int32_t* answer, float* logp, const AnswerRules* ar) {
+  check_rules(ar, V);
   if (rows <= 0) return;
-  k_logsoftmax_sample_rows<<<(unsigned)rows, 256, 0, cx.stream>>>(logits, V, smp, L, tokens, answer, logp);
+  if (ar) k_logsoftmax_sample_rows<true><<<(unsigned)rows, 256, 0, cx.stream>>>(logits, V, smp, L, tokens, answer, logp, *ar);
+  else k_logsoftmax_sample_rows<false><<<(unsigned)rows, 256, 0, cx.stream>>>(logits, V, smp, L, tokens, answer, logp, {});
   check_launch(cx, "k_logsoftmax_sample_rows");
 }
 void truncated_sample_rows(LaunchCtx& cx, const float* logits, int64_t rows, int V, const SampleCfg& smp, const TruncCfg& tr,
-                           int L, int32_t* tokens, int32_t* answer, float* logp) {
+                           int L, int32_t* tokens, int32_t* answer, float* logp, const AnswerRules* ar) {
   VD_REQUIRE(V >= 1 && V <= TRUNC_MAX_V, VD_E_BADARG, "truncated_sample_rows: V must be in [1, 49152] (the staged row)");
   VD_REQUIRE(tr.top_k >= 0 && std::isfinite(tr.top_p) && tr.top_p > 0.f && tr.top_p <= 1.f, VD_E_BADARG,
              "truncated_sample_rows: top_k >= 0, top_p in (0, 1]");
+  check_rules(ar, V);
   if (rows <= 0) return;
-  // the dynamic stage beside the static histograms passes the 48 KB default from V = 8 121 on: always opted in
-  const size_t smem = (size_t)V * sizeof(float);
-  VD_CUDA_CHECK(cudaFuncSetAttribute(k_truncated_sample_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k_truncated_sample_rows<<<(unsigned)rows, 256, smem, cx.stream>>>(logits, V, smp, tr, L, tokens, answer, logp);
+  // the dynamic stage beside the static histograms passes the 48 KB default from V = 8 121 on: always opted in.  With the
+  // rules the row's barred bits follow it (6 KB at V = 49 152: 198 KB beside 16.3 KB static, within a CTA's 227 KB)
+  const size_t smem = (size_t)V * sizeof(float) + (ar ? (size_t)((V + 31) / 32) * sizeof(uint32_t) : 0);
+  if (ar) {
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_truncated_sample_rows<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_truncated_sample_rows<true><<<(unsigned)rows, 256, smem, cx.stream>>>(logits, V, smp, tr, L, tokens, answer, logp, *ar);
+  } else {
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_truncated_sample_rows<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k_truncated_sample_rows<false><<<(unsigned)rows, 256, smem, cx.stream>>>(logits, V, smp, tr, L, tokens, answer, logp, {});
+  }
   check_launch(cx, "k_truncated_sample_rows");
 }
 void beam_gather(LaunchCtx& cx, float* dst, const float* out_prev, const float* in_prev, const int32_t* parent, int64_t rows, int H) {
   L1D(k_beam_gather, rows * H, dst, out_prev, in_prev, parent, rows, H);
 }
-void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
-                          int32_t* topi) {
-  VD_REQUIRE(k >= 1 && k <= 32 && k <= V, VD_E_BADARG, "logsoftmax_topk_rows: k");
-  if (rows == 0) return;
+template <bool RULES>
+static void launch_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
+                             int32_t* topi, const AnswerRules& ar) {
   const unsigned g = (unsigned)rows;
-  if (k <= 4) k_logsoftmax_topk_rows<4><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
-  else if (k <= 8) k_logsoftmax_topk_rows<8><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
-  else if (k <= 16) k_logsoftmax_topk_rows<16><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
-  else k_logsoftmax_topk_rows<32><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi);
+  if (k <= 4) k_logsoftmax_topk_rows<4, RULES><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi, ar);
+  else if (k <= 8) k_logsoftmax_topk_rows<8, RULES><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi, ar);
+  else if (k <= 16) k_logsoftmax_topk_rows<16, RULES><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi, ar);
+  else k_logsoftmax_topk_rows<32, RULES><<<g, 256, 0, cx.stream>>>(logits, mask_ids, V, k, topv, topi, ar);
+}
+void logsoftmax_topk_rows(LaunchCtx& cx, const float* logits, const int32_t* mask_ids, int64_t rows, int V, int k, float* topv,
+                          int32_t* topi, const AnswerRules* ar) {
+  VD_REQUIRE(k >= 1 && k <= 32 && k <= V, VD_E_BADARG, "logsoftmax_topk_rows: k");
+  check_rules(ar, V);
+  if (rows == 0) return;
+  if (ar) launch_topk_rows<true>(cx, logits, mask_ids, rows, V, k, topv, topi, *ar);
+  else launch_topk_rows<false>(cx, logits, mask_ids, rows, V, k, topv, topi, {});
   check_launch(cx, "k_logsoftmax_topk_rows");
 }
 void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* beams, int32_t* tokens, double* scores) {
@@ -2039,7 +2137,7 @@ void beam_init(LaunchCtx& cx, int64_t rows, int L, int start_token, int32_t* bea
 void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int L, int end_token, const float* topv,
                 const int32_t* topi, const double* scores_in, double* scores_out, const int32_t* beams_in, int32_t* beams_out,
                 int32_t* tokens, int32_t* parent, const BeamLists& lists, int32_t* pick_ans, int32_t* pick_len,
-                double* pick_score) {
+                double* pick_score, bool skip_empty) {
   VD_REQUIRE(k >= 1 && k <= 32 && stp >= 1 && stp < L, VD_E_BADARG, "beam_merge: k / step");
   VD_REQUIRE(G >= 1 && k % G == 0 && std::isfinite(lam) && lam >= 0.f, VD_E_BADARG, "beam_merge: groups / diversity");
   VD_REQUIRE(!pick_ans == !pick_len && !pick_ans == !pick_score, VD_E_BADARG, "beam_merge: all pick outputs or none");
@@ -2050,8 +2148,12 @@ void beam_merge(LaunchCtx& cx, int64_t N, int stp, int k, int G, float lam, int 
   VD_REQUIRE(!b.ord == !many && !b.out_ans == !many && !b.out_len == !many && !b.out_score == !many && !b.out_norm == !many &&
              (!many || b.norm), VD_E_BADARG, "beam_merge: n > 1 takes norms, the order and every ordered output");
   if (N == 0) return;
-  k_beam_merge<<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, G, lam, L, end_token, b, topv, topi, scores_in, scores_out, beams_in,
-                                                  beams_out, tokens, parent, pick_ans, pick_len, pick_score);
+  if (skip_empty)
+    k_beam_merge<true><<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, G, lam, L, end_token, b, topv, topi, scores_in, scores_out,
+                                                          beams_in, beams_out, tokens, parent, pick_ans, pick_len, pick_score);
+  else
+    k_beam_merge<false><<<(unsigned)N, 32, 0, cx.stream>>>(stp, k, G, lam, L, end_token, b, topv, topi, scores_in, scores_out,
+                                                           beams_in, beams_out, tokens, parent, pick_ans, pick_len, pick_score);
   check_launch(cx, "k_beam_merge");
 }
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1, float beta2,

@@ -108,6 +108,15 @@ void seq_lstm_pair_hook(Engine* e, void* const* P, const int64_t* I) {
   VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
 }
 
+// the answer rules of a *_rules hook: P = {hist, banned}, I = {step, ld, end_token, min_words, no_repeat_ngram, n_banned}
+AnswerRules hook_rules(void* const* P, const int64_t* I) {
+  AnswerRules a;
+  a.hist = static_cast<const int32_t*>(P[0]); a.banned = static_cast<const int32_t*>(P[1]);
+  a.step = (int32_t)I[0]; a.ld = I[1]; a.end_token = (int32_t)I[2];
+  a.min_words = (int32_t)I[3]; a.no_repeat_ngram = (int32_t)I[4]; a.n_banned = (int32_t)I[5];
+  return a;
+}
+
 const Entry TABLE[] = {
     // ---- history attention: (ptrs), ints B, R, H
     {"mn_attention_fwd", 4, 3, 0,
@@ -295,6 +304,51 @@ const Entry TABLE[] = {
        TruncCfg t;
        t.top_k = IN(7); t.top_p = (float)X[1];
        truncated_sample_rows(e->cx, CF(0), I[0], IN(1), s, t, IN(2), I32(1), I32(2), F(3));
+     }},
+    // ---- the answer rules (DESIGN §25) on the kernels above: each takes its hook's arguments plus the row histories hist
+    // (row pitch ld) and the banned ids (device, or null), and the ints ld, end_token, min_words, no_repeat_ngram, n_banned
+    // (the rules' step is the hook's step).  ptrs logits, mask_ids, topv, topi, hist, banned; ints rows, V, k, step, then
+    // the five
+    {"logsoftmax_topk_rows_rules", 6, 9, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       const AnswerRules ar = hook_rules(P + 4, I + 3);
+       logsoftmax_topk_rows(e->cx, CF(0), CI32(1), I[0], IN(1), IN(2), F(2), I32(3), &ar);
+     }},
+    // beam_merge_nbest's arguments; -inf top-k entries are no candidates
+    {"beam_merge_rules", 21, 7, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       BeamLists b;
+       b.nbest = IN(6);
+       b.ans = I32(8); b.len = I32(9); b.score = static_cast<double*>(P[10]);
+       b.lp = static_cast<const double*>(P[14]); b.norm = static_cast<double*>(P[15]); b.ord = I32(16);
+       b.out_ans = I32(17); b.out_len = I32(18); b.out_score = static_cast<double*>(P[19]); b.out_norm = static_cast<double*>(P[20]);
+       beam_merge(e->cx, I[0], IN(1), IN(2), IN(3), (float)X[0], IN(4), IN(5), CF(0), CI32(1), static_cast<const double*>(P[2]),
+                  static_cast<double*>(P[3]), CI32(4), I32(5), I32(6), I32(7), b, I32(11), I32(12), static_cast<double*>(P[13]), true);
+     }},
+    // logsoftmax_sample_rows_drawn's arguments (the fifth pointer may be null: the affine rule), then hist, banned; the
+    // seven ints, then the five
+    {"logsoftmax_sample_rows_rules", 7, 12, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       SampleCfg s;
+       s.seed_lo = (uint32_t)(uint64_t)I[3]; s.seed_hi = (uint32_t)((uint64_t)I[3] >> 32); s.step = (uint32_t)I[4];
+       s.temperature = (float)X[0]; s.row_offset = I[5]; s.row_stride = I[6];
+       s.row_round = static_cast<const int64_t*>(P[4]);
+       AnswerRules ar = hook_rules(P + 5, I + 6);
+       ar.step = IN(4);
+       logsoftmax_sample_rows(e->cx, CF(0), I[0], IN(1), s, IN(2), I32(1), I32(2), F(3), &ar);
+     }},
+    // truncated_sample_rows' arguments, then hist, banned; its eight ints, then the five
+    {"truncated_sample_rows_rules", 7, 13, 2,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       SampleCfg s;
+       s.seed_lo = (uint32_t)(uint64_t)I[3]; s.seed_hi = (uint32_t)((uint64_t)I[3] >> 32); s.step = (uint32_t)I[4];
+       s.temperature = (float)X[0]; s.row_offset = I[5]; s.row_stride = I[6];
+       s.row_round = static_cast<const int64_t*>(P[4]);
+       TruncCfg t;
+       t.top_k = IN(7); t.top_p = (float)X[1];
+       AnswerRules ar = hook_rules(P + 5, I + 7);
+       ar.step = IN(4);
+       truncated_sample_rows(e->cx, CF(0), I[0], IN(1), s, t, IN(2), I32(1), I32(2), F(3), &ar);
      }},
     // ptrs logits, lse, tgt, mask_ids, scale, dlogits (may alias logits); ints rows, V
     {"nll_bwd_scaled", 6, 2, 0,

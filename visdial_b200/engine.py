@@ -257,6 +257,18 @@ class Engine:
     def set_math_mode(self, mode: int):
         check(self.lib.vd_set_math_mode(self.h, mode))
 
+    def set_answer_rules(self, min_words: int = 0, no_repeat_ngram: int = 0, banned=()):
+        """The answer rules of every later beam search and sampling call (vd_set_answer_rules, DESIGN §25): <END> barred
+        while an answer has fewer than `min_words` words, no repeated `no_repeat_ngram`-gram (0 = off), and the `banned`
+        token ids never chosen.  All three at their defaults turn the rules off."""
+        ids = np.ascontiguousarray(np.asarray(list(banned), dtype=np.int64).astype(np.int32).ravel())
+        if min_words == 0 and no_repeat_ngram == 0 and ids.size == 0:
+            check(self.lib.vd_set_answer_rules(self.h, None))
+            return
+        r = _lib.vd_answer_rules(int(min_words), int(no_repeat_ngram), int(ids.size),
+                                 ids.ctypes.data_as(C.POINTER(C.c_int32)) if ids.size else None)
+        check(self.lib.vd_set_answer_rules(self.h, C.byref(r)))
+
     def set_lazy_decout(self, on: bool):
         check(self.lib.vd_set_lazy_decout(self.h, 1 if on else 0))
 

@@ -15,7 +15,9 @@ first is the round's answer); `-lengthPenalty a` ranks finished answers by score
 (DESIGN §24).  results.json records the two only when they differ from their defaults (1 and 0).
 `-topK K` and `-topP P` truncate `-sampleWords 1`'s draws to the K most likely words and then to the fewest of those
 holding P of the probability (DESIGN §23); they combine with `-history`, `-dialogsPerCall` and `-gpus`, and
-results.json records them only when they truncate.  A disc checkpoint answers every round with the
+results.json records them only when they truncate.  `-minWords m`, `-noRepeatNgram n` and `-bannedWords w1,w2` are the
+answer rules (DESIGN §25): no answer ends before m words, repeats an n-gram or uses a banned word, in beam search and
+sampling alike; results.json records them only when one is set.  A disc checkpoint answers every round with the
 best answer of the split's answer pool (Model.retrieveAnswers, DESIGN §18); the beam and sampling options do not apply
 to it, and its answer text is the pool row's words.
 
@@ -37,6 +39,7 @@ def rank_share(model, dl, opt: dict) -> list:
     sampleParams = {k: opt[k] for k in ("beamSize", "beamLen", "sampleWords", "temperature", "dialogsPerCall")}   # :88-94
     sampleParams["history"] = opt.get("history", "gt")
     sampleParams.update({k: opt[k] for k in ("beamGroups", "diversity", "lengthPenalty", "nBest", "topK", "topP") if k in opt})
+    sampleParams.update(cli.answer_rule_params(opt))
     if model.params["decoder"] == "disc":
         # a disc model answers by retrieval from the split's answer pool (DESIGN §18); model.lua:434-437 stops here
         answers = model.retrieveAnswers(dl, "val", {k: sampleParams[k] for k in ("dialogsPerCall", "history")})

@@ -4,6 +4,8 @@ read like the reference's own driver code.  `generateAnswers` (beam search / sam
 search and the sampling entirely on the device (vd_gen_beam_search, vd_gen_sample)."""
 from __future__ import annotations
 
+import contextlib
+
 import numpy as np
 
 from . import decoders, encoders
@@ -244,7 +246,12 @@ class Model:
         With `sampleWords`, `topK` K (default 0, off) and `topP` P (default 1, off) truncate every draw (DESIGN §23): to the
         first K classes by (logit desc, class asc), then to the shortest prefix of those holding P of their softmax mass
         (vd_gen_truncated_sample / vd_gen_dialog_truncated_sample).  When neither truncates (K = 0 or K >= vocabSize, and
-        P = 1) the calls are the untruncated ones.  Beam search ignores both."""
+        P = 1) the calls are the untruncated ones.  Beam search ignores both.
+
+        `minWords` (default 0), `noRepeatNgram` (default 0, off) and `bannedWords` (a list of words, default none) are the
+        answer rules (vd_set_answer_rules, DESIGN §25), in beam search and sampling alike: no answer ends before minWords
+        words, repeats a noRepeatNgram-gram or uses a banned word.  They are set for this call's engine calls only; at their
+        defaults nothing is set.  An unknown banned word raises ValueError."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
         params = params or {}
@@ -267,6 +274,7 @@ class Model:
         topK, topP = int(params.get("topK", 0)), float(params.get("topP", 1.0))
         truncated = sampleWords and truncates(topK, topP, self.params["vocabSize"])
         startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
+        rules = answer_rules(params, dataloader.word2ind)
         numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
         dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
         ind2word = getattr(dataloader, "ind2word", None)
@@ -289,37 +297,38 @@ class Model:
             self.wrapper.evaluate()                                                     # :460
             batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
             rowOffset = (offset + first) * self.params["maxQuesCount"]
-            if generated:
-                if truncated:
-                    answer, _, _ = self.engine.gen_dialog_truncated_sample(batch, beamLen, startToken, endToken, temperature,
-                                                                           seed, rowOffset, histWidth, maxAnsLen, topK, topP)
-                elif sampleWords:
-                    answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
-                                                                 rowOffset, histWidth, maxAnsLen)
-                elif listed:
-                    answer, length, score, norm, _ = self.engine.gen_dialog_nbest_beam_search(
-                        batch, beamSize, groups, diversity, lengthPenalty, nBest, beamLen, startToken, endToken, histWidth,
-                        maxAnsLen)
-                elif diverse:
-                    answer, length, score, _ = self.engine.gen_dialog_diverse_beam_search(
-                        batch, beamSize, groups, diversity, beamLen, startToken, endToken, histWidth, maxAnsLen)
+            with rules_set(self.engine, rules):
+                if generated:
+                    if truncated:
+                        answer, _, _ = self.engine.gen_dialog_truncated_sample(batch, beamLen, startToken, endToken, temperature,
+                                                                               seed, rowOffset, histWidth, maxAnsLen, topK, topP)
+                    elif sampleWords:
+                        answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
+                                                                     rowOffset, histWidth, maxAnsLen)
+                    elif listed:
+                        answer, length, score, norm, _ = self.engine.gen_dialog_nbest_beam_search(
+                            batch, beamSize, groups, diversity, lengthPenalty, nBest, beamLen, startToken, endToken, histWidth,
+                            maxAnsLen)
+                    elif diverse:
+                        answer, length, score, _ = self.engine.gen_dialog_diverse_beam_search(
+                            batch, beamSize, groups, diversity, beamLen, startToken, endToken, histWidth, maxAnsLen)
+                    else:
+                        answer, length, score, _ = self.engine.gen_dialog_beam_search(batch, beamSize, beamLen, startToken,
+                                                                                      endToken, histWidth, maxAnsLen)
                 else:
-                    answer, length, score, _ = self.engine.gen_dialog_beam_search(batch, beamSize, beamLen, startToken,
-                                                                                  endToken, histWidth, maxAnsLen)
-            else:
-                self.forwardBackward(batch, True, True)                                 # :467
-                if truncated:
-                    answer, _ = self.engine.gen_truncated_sample(beamLen, startToken, temperature, seed, rowOffset, topK, topP)
-                elif sampleWords:                                                       # :582-594
-                    answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
-                elif listed:
-                    answer, length, score, norm = self.engine.gen_nbest_beam_search(beamSize, groups, diversity, lengthPenalty,
-                                                                                    nBest, beamLen, startToken, endToken)
-                elif diverse:
-                    answer, length, score = self.engine.gen_diverse_beam_search(beamSize, groups, diversity, beamLen,
-                                                                                startToken, endToken)
-                else:                                                                   # :472-579
-                    answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
+                    self.forwardBackward(batch, True, True)                                 # :467
+                    if truncated:
+                        answer, _ = self.engine.gen_truncated_sample(beamLen, startToken, temperature, seed, rowOffset, topK, topP)
+                    elif sampleWords:                                                       # :582-594
+                        answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
+                    elif listed:
+                        answer, length, score, norm = self.engine.gen_nbest_beam_search(beamSize, groups, diversity, lengthPenalty,
+                                                                                        nBest, beamLen, startToken, endToken)
+                    elif diverse:
+                        answer, length, score = self.engine.gen_diverse_beam_search(beamSize, groups, diversity, beamLen,
+                                                                                    startToken, endToken)
+                    else:                                                                   # :472-579
+                        answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
             R = self.params["maxQuesCount"]
             if listed:
                 answer, length = answer.reshape(len(inds), R, groups, nBest, -1), length.reshape(len(inds), R, groups, nBest)
@@ -448,6 +457,34 @@ class Model:
         return ck
 
 
+def answer_rules(params: dict, word2ind: dict):
+    """The answer rules of `params` (DESIGN §25) as Engine.set_answer_rules' (min_words, no_repeat_ngram, banned ids):
+    `minWords` (default 0), `noRepeatNgram` (default 0, off) and `bannedWords` (words, mapped through word2ind).  None when
+    all three are at their defaults.  Raises ValueError for a banned word the vocabulary does not have."""
+    minWords, noRepeat = int(params.get("minWords", 0)), int(params.get("noRepeatNgram", 0))
+    words = list(params.get("bannedWords", ()) or ())
+    unknown = [w for w in words if w not in word2ind]
+    if unknown:
+        raise ValueError("bannedWords not in the vocabulary: %s" % ", ".join(map(str, unknown)))
+    if minWords == 0 and noRepeat == 0 and not words:
+        return None
+    return minWords, noRepeat, [int(word2ind[w]) for w in words]
+
+
+@contextlib.contextmanager
+def rules_set(engine, rules):
+    """`rules` (answer_rules' value) on `engine` for the calls inside, cleared after them even when one raises, so that they
+    never reach another caller of the engine; None sets nothing."""
+    if rules is None:
+        yield
+        return
+    engine.set_answer_rules(*rules)
+    try:
+        yield
+    finally:
+        engine.set_answer_rules()
+
+
 def truncates(topK: int, topP: float, V: int) -> bool:
     """whether top-k / top-p truncation changes a draw over V classes (DESIGN §23): 1 <= topK < V or topP < 1"""
     return 1 <= topK < V or topP < 1.0
@@ -550,6 +587,8 @@ class DialogPool:
         self.topK = int(params.get("topK", 1 if self.disc else 0))
         self.topP = float(params.get("topP", 1.0))
         self.truncated = not self.disc and self.sampleWords and truncates(self.topK, self.topP, model.params["vocabSize"])
+        # the answer rules (DESIGN §25) of this pool's asks, set around each ask only; a disc pool retrieves without them
+        self.rules = None if self.disc else answer_rules(params, dataloader.word2ind)
         self.start, self.end = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]
         self.width = dataloader.maxQuesLen
         self.maxAnsLen = dataloader.maxAnsLen
@@ -669,17 +708,21 @@ class DialogPool:
                                       "answer": [int(t) for t in self.pool[i] if t != 0]} for i, v in zip(index[b], score[b])]})
         elif self.sampleWords:
             if self.truncated:
-                ans, _ = self.eng.dialog_ask_truncated_slots(slots, q, self.beamLen, self.start, self.end, self.temperature,
-                                                             self.seed, self.rowOffset, self.topK, self.topP)
+                with rules_set(self.eng, self.rules):
+                    ans, _ = self.eng.dialog_ask_truncated_slots(slots, q, self.beamLen, self.start, self.end,
+                                                                 self.temperature, self.seed, self.rowOffset, self.topK,
+                                                                 self.topP)
             else:
-                ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature,
-                                                          self.seed, self.rowOffset)
+                with rules_set(self.eng, self.rules):
+                    ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature,
+                                                              self.seed, self.rowOffset)
             given = [history_answer(ans[b, 1:], self.end) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
         elif self.lengthPenalty != 0.0 or self.nBest != 1:
-            ans, length, score, norm = self.eng.dialog_ask_nbest_slots(slots, q, self.beamSize, self.groups, self.diversity,
-                                                                       self.lengthPenalty, self.nBest, self.beamLen,
-                                                                       self.start, self.end)
+            with rules_set(self.eng, self.rules):
+                ans, length, score, norm = self.eng.dialog_ask_nbest_slots(slots, q, self.beamSize, self.groups,
+                                                                           self.diversity, self.lengthPenalty, self.nBest,
+                                                                           self.beamLen, self.start, self.end)
             given = []
             for b in range(len(q)):
                 e = listed_entry(ans[b], length[b], score[b], norm[b],
@@ -687,8 +730,9 @@ class DialogPool:
                 given.append(history_answer(e["answer"], self.end, e["length"]) if e else [])
                 out.append(dict(e, question=[int(t) for t in q[b] if t]) if e else None)
         elif self.groups > 1:
-            ans, length, score = self.eng.dialog_ask_diverse_slots(slots, q, self.beamSize, self.groups, self.diversity,
-                                                                   self.beamLen, self.start, self.end)
+            with rules_set(self.eng, self.rules):
+                ans, length, score = self.eng.dialog_ask_diverse_slots(slots, q, self.beamSize, self.groups, self.diversity,
+                                                                       self.beamLen, self.start, self.end)
             given = []
             for b in range(len(q)):
                 gs = [{"answer": ans[b, g].tolist(), "score": float(score[b, g]), "length": int(length[b, g])}
@@ -697,7 +741,9 @@ class DialogPool:
                 given.append(history_answer(ans[b, best], self.end, length[b, best]) if best >= 0 else [])
                 out.append(dict(gs[best], question=[int(t) for t in q[b] if t], groups=gs) if best >= 0 else None)
         else:
-            ans, length, score = self.eng.dialog_ask_beam_slots(slots, q, self.beamSize, self.beamLen, self.start, self.end)
+            with rules_set(self.eng, self.rules):
+                ans, length, score = self.eng.dialog_ask_beam_slots(slots, q, self.beamSize, self.beamLen, self.start,
+                                                                    self.end)
             given = [history_answer(ans[b], self.end, length[b]) for b in range(len(q))]
             out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist(), "score": float(score[b]),
                     "length": int(length[b])} if length[b] > 0 else None for b in range(len(q))]
