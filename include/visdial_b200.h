@@ -56,6 +56,8 @@ typedef struct vd_params {
   int32_t numOptions;           /* 100 */
   float dropout;                /* 0.5; used by the LF graphs, MN/att/HREA hard-code 0.5 */
   int32_t gpuid;                /* CUDA device ordinal */
+  int32_t imgRegions;           /* 0: img_feat is the imgSpatialSize^2 grid; P > 0: P detector region rows of imgFeatureSize
+                                   channels per image (DESIGN §26), att encoders only */
 } vd_params;
 
 /* A batch as produced by dataloader:getTrainBatch / getTestBatch (dataloader.lua:324-478),
@@ -65,7 +67,7 @@ typedef struct vd_batch {
   int32_t Tq, Th, Ta, To;       /* trimmed question / history / answer(+1) / option widths */
   const int32_t* ques_fwd;      /* (B,10,Tq) right-aligned */
   const int32_t* hist;          /* (B,10,Th) right-aligned */
-  const float* img_feat;        /* (B,F) fc7 or (B,S,S,C) NHWC pool5 — one row per dialog */
+  const float* img_feat;        /* (B,F) fc7, (B,S,S,C) NHWC pool5 or (B,P,C) regions — one row per dialog */
   const int32_t* options;       /* disc: (N,100,To) left-aligned raw option tokens */
   const int32_t* answer_ind;    /* (N) 1-based ground-truth option */
   const int32_t* answer_in;     /* gen: (B,10,Ta) <START> a.. 0.. */
@@ -73,6 +75,9 @@ typedef struct vd_batch {
   const int32_t* option_in;     /* gen eval: (B,10,100,To) */
   const int32_t* option_out;    /* gen eval: (B,10,100,To) */
   int32_t on_device;            /* 0: host pointers (staged + copied H2D by the engine), 1: device */
+  const int32_t* img_count;     /* (B) regions present per dialog's image, each in [1, imgRegions] (checked when staged from
+                                   the host; a precondition for device batches); NULL = all present.  Region engines only:
+                                   the SAN attends over rows 0 .. count-1 and the rest never affect a result (DESIGN §26) */
 } vd_batch;
 
 /* ---- parameter layout: host-only, needs no GPU --------------------------------------------- */
@@ -558,9 +563,10 @@ typedef struct vd_corpus_desc {
   int32_t useIm;
   int32_t maxHistoryLen;        /* opt.maxHistoryLen (60) — overwritten by min(R*(Lq+La),300) when concatHistory (:142,:217) */
   int32_t imgNorm;              /* 1: L2-normalise over dim 2 at load                      (:64-68) */
-  int32_t imgAtt;               /* 1: images are (N,C,S,S) and are stored (N,S,S,C)        (:70-72) */
+  int32_t imgAtt;               /* 1: images are (N,C,S,S) and are stored (N,S,S,C)        (:70-72);
+                                   2: region features (N,P,C), stored as given (DESIGN §26) */
   int32_t imgChannels;          /* C (pool5 512) or F (fc7 4096)                                   */
-  int32_t imgSpatial;           /* S (14); ignored unless imgAtt                                   */
+  int32_t imgSpatial;           /* S (14) for imgAtt 1, P (regions per image) for imgAtt 2; ignored unless imgAtt */
   int32_t startToken, endToken; /* word2ind['<START>'], word2ind['<END>']                  (:17-22) */
   const int32_t* ques;          /* (n,R,Lq) left-aligned  'ques_<split>'                           */
   const int32_t* ques_len;      /* (n,R)                  'ques_length_<split>'                    */
@@ -574,7 +580,7 @@ typedef struct vd_corpus_desc {
   const int32_t* ans_index;     /* (n,R) 1-based gt option 'ans_index_<split>' (NULL for test)     */
   const int32_t* img_pos;       /* (n) 0-based row of images as stored ('img_pos_<split>'; the +1 of :76-77 is Lua indexing) */
   const int32_t* num_rounds;    /* (n)                    'num_rounds_<split>' (may be NULL)       */
-  const float* images;          /* (N,F) or (N,C,S,S) fp32 'images_<split>' of the image h5 (NULL unless useIm) */
+  const float* images;          /* (N,F), (N,C,S,S) or (N,P,C) fp32 'images_<split>' of the image h5 (NULL unless useIm) */
 } vd_corpus_desc;
 
 /* dataloader:initialize tensors -> HBM + dataloader:prepareDataset on the device.  Host pointers. */
@@ -591,6 +597,12 @@ int vd_corpus_get_batch(vd_corpus* c, const int64_t* inds, int32_t n, int32_t de
  * "opt_in","opt_out","img_fv"}, or "opt_list": the raw (numOptList, maxAnsLen) answer pool as uploaded, which the host no
  * longer keeps (the pool vd_answer_pool_encode takes); *elems receives the element count (call with host_dst = NULL to size). */
 int vd_corpus_read(vd_corpus* c, const char* name, void* host_dst, int64_t* elems);
+/* Region corpora (imgAtt = 2): counts_host (numImages) = 'num_boxes_<split>', each image's region count in [1, P].  Checks
+ * every count (VD_E_BADARG, corpus unchanged, if one is outside), uploads them and zeroes every pad row (rows >= count) of
+ * the resident features.  Later batches carry img_count[b] = counts[img_pos[inds[b]]], gathered on the device.  Without
+ * this call every region is present.  Once per corpus: the pad rows are zeroed in place, so a second call is VD_E_STATE,
+ * as is a corpus without region features. */
+int vd_corpus_region_counts(vd_corpus* c, const int32_t* counts_host, int64_t numImages);
 /* bytes the last vd_corpus_get_batch read + wrote in HBM (algorithmic) and the number of kernels it launched */
 int vd_corpus_batch_bytes(vd_corpus* c, int64_t* bytes, int32_t* launches);
 

@@ -10,12 +10,14 @@ typedef struct vd_params {
   int32_t vocabSize, embedSize, rnnHiddenSize, numLayers, imgFeatureSize, imgSpatialSize, imgEmbedSize,
           commonEmbeddingSize, numAttentionLayers, maxQuesCount, numOptions;
   float dropout; int32_t gpuid;
+  int32_t imgRegions;            /* 0: the S x S grid; P > 0: P region rows per image (att encoders) */
 } vd_params;
 typedef struct vd_batch {
   int32_t B, Tq, Th, Ta, To;
   const int32_t* ques_fwd; const int32_t* hist; const float* img_feat; const int32_t* options;
   const int32_t* answer_ind; const int32_t* answer_in; const int32_t* answer_out;
   const int32_t* option_in; const int32_t* option_out; int32_t on_device;
+  const int32_t* img_count;      /* (B) region counts in [1, imgRegions], NULL = every region present */
 } vd_batch;
 const char* vd_last_error(void);
 int vd_create(const vd_params* p, vd_engine** out);

@@ -33,7 +33,7 @@ class vd_params(C.Structure):
         ("numLayers", C.c_int32), ("imgFeatureSize", C.c_int32), ("imgSpatialSize", C.c_int32),
         ("imgEmbedSize", C.c_int32), ("commonEmbeddingSize", C.c_int32),
         ("numAttentionLayers", C.c_int32), ("maxQuesCount", C.c_int32), ("numOptions", C.c_int32),
-        ("dropout", C.c_float), ("gpuid", C.c_int32),
+        ("dropout", C.c_float), ("gpuid", C.c_int32), ("imgRegions", C.c_int32),
     ]
 
 
@@ -43,7 +43,7 @@ class vd_batch(C.Structure):
         ("ques_fwd", C.c_void_p), ("hist", C.c_void_p), ("img_feat", C.c_void_p),
         ("options", C.c_void_p), ("answer_ind", C.c_void_p), ("answer_in", C.c_void_p),
         ("answer_out", C.c_void_p), ("option_in", C.c_void_p), ("option_out", C.c_void_p),
-        ("on_device", C.c_int32),
+        ("on_device", C.c_int32), ("img_count", C.c_void_p),
     ]
 
 
@@ -192,6 +192,7 @@ SIGNATURES = {
     "vd_corpus_get_batch": [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _P(vd_batch)],
     "vd_corpus_read": [C.c_void_p, C.c_char_p, C.c_void_p, _P(C.c_int64)],
     "vd_corpus_batch_bytes": [C.c_void_p, _P(C.c_int64), _P(C.c_int32)],
+    "vd_corpus_region_counts": [C.c_void_p, C.c_void_p, C.c_int64],
 }
 
 _lib = None

@@ -275,6 +275,31 @@ def vocab_size(opt: dict) -> int:
         return len(json.load(f)["word2ind"]) + 2
 
 
+def set_image_regions(mp: dict, opt: dict, subsets):
+    """imgRegions from the image features file (DESIGN §26): P when its images_<split> is a 3-D (numImages, P, C) region
+    file, and no entry for a grid or fc7 file, so that those runs record the modelParams they recorded before.  A region
+    file needs an att encoder and imgFeatureSize = C."""
+    from .dataloader import image_regions
+    mp.pop("imgRegions", None)
+    if not opt.get("useIm") or not subsets:
+        return mp
+    found = {s: image_regions(opt["inputImg"], s) for s in subsets}
+    if len(set(found.values())) > 1:
+        raise ValueError("the splits of %s hold different image features (%s); one run needs one layout (regions, "
+                         "channels)" % (opt["inputImg"], ", ".join("%s: %s" % kv for kv in sorted(found.items()))))
+    P, C = found[subsets[0]]
+    if P == 0:
+        return mp
+    if "att" not in mp["encoder"]:
+        raise ValueError("%s holds region features, which only the att encoders read, not %s"
+                         % (opt["inputImg"], mp["encoder"]))
+    if int(mp.get("imgFeatureSize", 4096)) != C:
+        raise ValueError("%s holds region features of %d channels but the model has imgFeatureSize = %d (pass "
+                         "-imgFeatureSize %d to train on it)" % (opt["inputImg"], C, int(mp.get("imgFeatureSize", 4096)), C))
+    mp["imgRegions"] = P
+    return mp
+
+
 def build(mp: dict, opt: dict, rank: int, world: int, subsets, ck=None):
     """Model on GPU gpuid + rank in the requested math mode (with the checkpoint's weights and learning rate when `ck` is
     given), and its device dataloader over `subsets` read from opt's files.  Returns (model, dataloader)."""
@@ -283,6 +308,7 @@ def build(mp: dict, opt: dict, rank: int, world: int, subsets, ck=None):
     from .dataloader import Dataloader
     from .model import Model
     mp = dict(mp, gpuid=opt["gpuid"] + rank)
+    set_image_regions(mp, opt, subsets)
     model = Model(mp, seed=SEED)
     model.engine.set_math_mode({"fp32": VD_MATH_FP32, "tf32": VD_MATH_TF32, "f16": VD_MATH_F16}[opt["math"]])
     if ck is not None:

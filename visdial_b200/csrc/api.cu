@@ -14,6 +14,7 @@ void corpus_destroy(Corpus* c);
 void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd_batch* out);
 void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems);
 void corpus_batch_bytes(Corpus* c, int64_t* bytes, int32_t* launches);
+void corpus_region_counts(Corpus* c, const int32_t* counts_host, int64_t numImages);
 void test_kernel(Engine* e, const char* name, void* const* ptrs, int n_ptrs, const int64_t* ints, int n_ints, const double* reals,
                  int n_reals);
 }  // namespace vd
@@ -770,6 +771,9 @@ int vd_corpus_get_batch(vd_corpus* h, const int64_t* inds, int32_t n, int32_t de
 }
 int vd_corpus_read(vd_corpus* h, const char* name, void* host_dst, int64_t* elems) {
   VD_TRY({ vd::corpus_read(CORP(h), name, host_dst, elems); })
+}
+int vd_corpus_region_counts(vd_corpus* h, const int32_t* counts_host, int64_t numImages) {
+  VD_TRY({ vd::corpus_region_counts(CORP(h), counts_host, numImages); })
 }
 int vd_corpus_batch_bytes(vd_corpus* h, int64_t* bytes, int32_t* launches) {
   VD_TRY({ vd::corpus_batch_bytes(CORP(h), bytes, launches); })

@@ -7,6 +7,7 @@
 //   dataloader:processHistory              :202-278
 //   dataloader:processOptions              :281-321
 //   image L2 norm + NCHW->NHWC permute     :59-73
+//   region features and their counts       DESIGN §26 (no reference counterpart)
 //   getTrainBatch / getTestBatch           :324-375
 //   getIndexData / getIndexOption          :378-478
 // Everything here is int32/fp32 HBM-bound gather work: one thread per output element (or 16 B vector), fully
@@ -186,11 +187,23 @@ __global__ void __launch_bounds__(256) k_gather_tokens(const GatherJobs jobs, co
   }
 }
 
-// img_feat[b] = img_fv[img_pos[ind[b]]] (:394-398); 4 independent 16 B loads in flight per thread
+// region features: every row at or past its image's count of a (nimg, P, C4 float4) volume <- 0, once, so that the gathered
+// batches hold exact zeros there
+__global__ void k_zero_pad_regions(float4* __restrict__ x, const int32_t* __restrict__ cnt, int64_t total4, int P, int64_t C4) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total4) return;
+  const int64_t row = i / C4;
+  if ((int)(row % P) >= cnt[row / P]) x[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+// img_feat[b] = img_fv[img_pos[ind[b]]] (:394-398); 4 independent 16 B loads in flight per thread.  Region corpora with
+// counts: img_count[b] = counts[img_pos[ind[b]]] as well
 __global__ void __launch_bounds__(256) k_gather_img(const float4* __restrict__ src, const int32_t* __restrict__ img_pos,
                                                     const int32_t* __restrict__ ind, float4* __restrict__ dst,
-                                                    int64_t elems4) {
+                                                    int64_t elems4, const int32_t* __restrict__ counts,
+                                                    int32_t* __restrict__ count_out) {
   const int64_t b = blockIdx.y;
+  if (counts && blockIdx.x == 0 && threadIdx.x == 0) count_out[b] = counts[img_pos[ind[b]]];
   const float4* s = src + (int64_t)img_pos[ind[b]] * elems4;
   float4* d = dst + b * elems4;
   int64_t base = (int64_t)blockIdx.x * blockDim.x * 4 + threadIdx.x;
@@ -210,6 +223,8 @@ struct Corpus {
   int n = 0, R = 0, Lq = 0, La = 0, Lc = 0, K = 0, m = 0, Wh = 0, nimg = 0;
   int useHist = 0, concat = 0, useIm = 0, maxHistoryLen = 0, start_tok = 0, end_tok = 0;
   int64_t img_elems = 0;
+  int regions = 0;               // P of a region corpus (imgAtt 2), else 0
+  int32_t* img_count = nullptr;  // (nimg) region counts, null = every region present
   bool has_ans_index = false;
   // raw (device)
   int32_t *ques = nullptr, *ques_len = nullptr, *ans = nullptr, *ans_len = nullptr, *cap = nullptr, *cap_len = nullptr,
@@ -222,7 +237,7 @@ struct Corpus {
   std::vector<int32_t> h_ques_len, h_hist_len, h_ans_len1, h_opt_maxlen;
   std::vector<void*> owned;
   // two alternating output sets
-  struct OutSet { GrowBuf ques, hist, ans_in, ans_out, ans_ind, options, opt_in, opt_out, img, ind; } out[2];
+  struct OutSet { GrowBuf ques, hist, ans_in, ans_out, ans_ind, options, opt_in, opt_out, img, ind, cnt; } out[2];
   int32_t* h_ind[2] = {nullptr, nullptr}; int h_ind_cap[2] = {0, 0};
   cudaEvent_t ind_free[2] = {nullptr, nullptr};
   int cur = 0;
@@ -244,7 +259,8 @@ struct Corpus {
     for (void* p : owned) cudaFree(p);
     for (int s = 0; s < 2; ++s) {
       OutSet& o = out[s];
-      GrowBuf* bs[] = {&o.ques, &o.hist, &o.ans_in, &o.ans_out, &o.ans_ind, &o.options, &o.opt_in, &o.opt_out, &o.img, &o.ind};
+      GrowBuf* bs[] = {&o.ques, &o.hist, &o.ans_in, &o.ans_out, &o.ans_ind, &o.options, &o.opt_in, &o.opt_out, &o.img, &o.ind,
+                       &o.cnt};
       for (GrowBuf* b : bs) b->release();
       if (h_ind[s]) cudaFreeHost(h_ind[s]);
       if (ind_free[s]) cudaEventDestroy(ind_free[s]);
@@ -350,14 +366,21 @@ Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d) {
     VD_REQUIRE(d->images && d->img_pos && d->numImages > 0 && d->imgChannels > 0, VD_E_BADARG, "useIm: images / img_pos missing");
     check_lengths(d->img_pos, n, 0, d->numImages - 1, "img_pos");
     c->img_pos = c->upload(d->img_pos, n);
-    const int C = d->imgChannels, P = d->imgAtt ? d->imgSpatial * d->imgSpatial : 1;
+    VD_REQUIRE(d->imgAtt >= 0 && d->imgAtt <= 2, VD_E_BADARG, "imgAtt must be 0, 1 or 2");
+    const bool region = d->imgAtt == 2;
+    const int C = d->imgChannels, P = region ? d->imgSpatial : d->imgAtt ? d->imgSpatial * d->imgSpatial : 1;
     VD_REQUIRE(!d->imgAtt || d->imgSpatial > 0, VD_E_SHAPE, "imgSpatial");
+    VD_REQUIRE(!region || !d->imgNorm, VD_E_BADARG, "region features are not L2-normalised (imgNorm = 0)");
+    VD_REQUIRE(!region || C % 4 == 0, VD_E_SHAPE, "region feature channels must be a multiple of 4");
+    VD_REQUIRE(!eng->cfg.useIm || region == (eng->cfg.regions > 0), VD_E_SHAPE,
+               "region features need an engine with imgRegions = P, grid features one with imgRegions = 0");
+    c->regions = region ? P : 0;
     c->img_elems = (int64_t)C * P;
     VD_REQUIRE(c->img_elems % 4 == 0, VD_E_SHAPE, "image feature row must be a multiple of 4 floats");
-    const int64_t want = eng->cfg.att ? (int64_t)eng->cfg.S * eng->cfg.S * eng->cfg.F : (int64_t)eng->cfg.F;
+    const int64_t want = eng->cfg.att ? (int64_t)eng->cfg.P * eng->cfg.F : (int64_t)eng->cfg.F;
     VD_REQUIRE(!eng->cfg.useIm || c->img_elems == want, VD_E_SHAPE, "image feature size != params");
     c->img_fv = c->dalloc<float>((int64_t)c->nimg * c->img_elems);
-    if (!d->imgAtt) {
+    if (d->imgAtt != 1) {                       // fc7 rows, or region rows (N, P, C) as stored
       VD_CUDA_CHECK(cudaMemcpyAsync(c->img_fv, d->images, (size_t)c->nimg * c->img_elems * 4, cudaMemcpyHostToDevice, st));
       if (d->imgNorm) { k_img_norm_rows<<<c->nimg, 256, 0, st>>>(c->img_fv, C); check_launch(cx, "k_img_norm_rows"); }
     } else {
@@ -469,11 +492,14 @@ void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd
     if (c->useIm) {
       float* img = (float*)o.img.ensure((size_t)n * c->img_elems * 4);
       const int64_t e4 = c->img_elems / 4;
-      k_gather_img<<<dim3(cdiv(e4, 1024), n), 256, 0, st>>>((const float4*)c->img_fv, c->img_pos, ind, (float4*)img, e4);
+      int32_t* cnt = c->img_count ? (int32_t*)o.cnt.ensure((size_t)n * 4) : nullptr;
+      k_gather_img<<<dim3(cdiv(e4, 1024), n), 256, 0, st>>>((const float4*)c->img_fv, c->img_pos, ind, (float4*)img, e4,
+                                                              c->img_count, cnt);
       check_launch(cx, "k_gather_img");
       ++launches;
       out->img_feat = img;
-      bytes += (int64_t)n * c->img_elems * 8 + (int64_t)n * 4;
+      out->img_count = cnt;
+      bytes += (int64_t)n * c->img_elems * 8 + (int64_t)n * 4 + (cnt ? (int64_t)n * 8 : 0);
     }
   }
   out->on_device = 1;
@@ -502,6 +528,28 @@ void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems) {
     VD_CUDA_CHECK(cudaStreamSynchronize(c->eng->main_stream));
     VD_CUDA_CHECK(cudaMemcpy(host_dst, p, (size_t)cnt * 4, cudaMemcpyDeviceToHost));
   }
+}
+
+void corpus_region_counts(Corpus* c, const int32_t* counts_host, int64_t numImages) {
+  VD_REQUIRE(c->regions > 0 && c->img_fv, VD_E_STATE, "region counts need a corpus of region features (imgAtt = 2)");
+  // the pad rows are zeroed in place: counts set once could not be raised later without the rows they zeroed
+  VD_REQUIRE(c->img_count == nullptr, VD_E_STATE, "region counts are set once per corpus");
+  VD_REQUIRE(counts_host != nullptr, VD_E_BADARG, "counts is null");
+  VD_REQUIRE(numImages == c->nimg, VD_E_BADARG, "counts must hold one entry per image (numImages)");
+  for (int64_t i = 0; i < numImages; ++i)
+    if (counts_host[i] < 1 || counts_host[i] > c->regions) {
+      char buf[160];
+      snprintf(buf, sizeof(buf), "num_boxes[%lld] = %d outside [1, %d]", (long long)i, counts_host[i], c->regions);
+      throw CudaError(VD_E_BADARG, buf);
+    }
+  VD_CUDA_CHECK(cudaSetDevice(c->gpuid));
+  cudaStream_t st = c->eng->main_stream;
+  c->img_count = c->dalloc<int32_t>(c->nimg);
+  VD_CUDA_CHECK(cudaMemcpyAsync(c->img_count, counts_host, (size_t)c->nimg * 4, cudaMemcpyHostToDevice, st));
+  const int64_t C4 = c->img_elems / c->regions / 4, total4 = (int64_t)c->nimg * c->img_elems / 4;
+  k_zero_pad_regions<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>((float4*)c->img_fv, c->img_count, total4, c->regions, C4);
+  check_launch(c->eng->cx, "k_zero_pad_regions");
+  VD_CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
 void corpus_batch_bytes(Corpus* c, int64_t* bytes, int32_t* launches) {

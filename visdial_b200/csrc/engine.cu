@@ -28,6 +28,7 @@ Cfg parse_cfg(const vd_params* p) {
   else VD_REQUIRE(false, VD_E_BADARG, "unknown decoder (disc | gen)");
   c.V = p->vocabSize; c.E = p->embedSize; c.H = p->rnnHiddenSize; c.L = p->numLayers; c.F = p->imgFeatureSize;
   c.S = p->imgSpatialSize; c.IE = p->imgEmbedSize; c.Cm = p->commonEmbeddingSize; c.hops = p->numAttentionLayers;
+  c.regions = p->imgRegions;
   c.R = p->maxQuesCount; c.K = p->numOptions; c.dropout = p->dropout; c.gpuid = p->gpuid;
   // opts.lua:55-59,62
   c.useHist = c.encoder.find("hist") != std::string::npos;
@@ -43,6 +44,12 @@ Cfg parse_cfg(const vd_params* p) {
   c.mn_qi = c.enc == ENC_MN_QIH;
   c.embdrop = c.fam_mn || c.enc == ENC_LF_ATT;
   c.rnn_layers = (c.fam_lf && !c.att) || c.fam_hre;
+  VD_REQUIRE(c.regions >= 0 && c.regions <= 4096, VD_E_BADARG, "imgRegions must be in [0, 4096]");
+  VD_REQUIRE(c.regions == 0 || c.att, VD_E_BADARG, "region features (imgRegions > 0) are for the att encoders only");
+  c.P = c.regions > 0 ? c.regions : c.S * c.S;
+  // k_san_att_bwd stages a dialog round's du, p and dp rows in (H + 2P + 33) floats of shared memory (48 KB without opt-in)
+  VD_REQUIRE(!c.san || (int64_t)c.H + 2 * (int64_t)c.P + 33 <= 12288, VD_E_BADARG,
+             "attention positions too many for rnnHiddenSize: rnnHiddenSize + 2 * positions must be <= 12255");
   if (c.enc == ENC_LF_ATT) c.hops = 1;           // hard-wired upstream: lf-att-ques-im-hist.lua:49 does not read params.numAttentionLayers
   VD_REQUIRE(c.V > 2 && c.E > 0 && c.H > 0, VD_E_BADARG, "vocabSize / embedSize / rnnHiddenSize must be positive");
   VD_REQUIRE(c.L == 2, VD_E_BADARG, "numLayers must be 2");
@@ -298,7 +305,19 @@ void Engine::stage_batch(const vd_batch* b) {
   VD_REQUIRE(b->ques_fwd && b->Tq > 0, VD_E_SHAPE, "ques_fwd / Tq missing");
   if (cfg.useHist) VD_REQUIRE(b->hist && b->Th > 0, VD_E_SHAPE, "encoder uses history: hist / Th missing");
   if (cfg.useIm) VD_REQUIRE(b->img_feat, VD_E_SHAPE, "encoder uses the image: img_feat missing");
-  int64_t img_elems = cfg.att ? (int64_t)b->B * cfg.S * cfg.S * cfg.F : (int64_t)b->B * cfg.F;
+  int64_t img_elems = cfg.att ? (int64_t)b->B * cfg.P * cfg.F : (int64_t)b->B * cfg.F;
+  if (b->img_count) {
+    VD_REQUIRE(cfg.regions > 0, VD_E_BADARG, "img_count is for region engines (imgRegions > 0) only");
+    if (b->on_device) {
+      db.img_count = b->img_count;             // [1, P] is the caller's precondition (a corpus checked its counts)
+    } else {
+      for (int i = 0; i < b->B; ++i)
+        VD_REQUIRE(b->img_count[i] >= 1 && b->img_count[i] <= cfg.P, VD_E_BADARG, "img_count outside [1, imgRegions]");
+      int32_t* d = (int32_t*)stage_cnt.ensure((size_t)b->B * sizeof(int32_t));
+      VD_CUDA_CHECK(cudaMemcpyAsync(d, b->img_count, (size_t)b->B * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
+      db.img_count = d;
+    }
+  }
   struct Item { const void* src; size_t bytes; const void** dst; } items[9] = {
       {b->ques_fwd, (size_t)db.N * b->Tq * 4, (const void**)&db.ques},
       {cfg.useHist ? b->hist : nullptr, (size_t)db.N * b->Th * 4, (const void**)&db.hist},
@@ -834,12 +853,14 @@ void Engine::mn_block_bwd(const float* dout, const float* out, float* dqin, floa
 // acts on the repeated tensor; hops of {img_common + ques_common -> tanh -> dropout -> score -> softmax -> weighted sum + u}
 void Engine::san_image(const float* pool5, int64_t B, float* t) {
   wait_img();
-  linear_fwd(seg("san.img.weight"), pool5, B * cfg.S * cfg.S, t, 1);
+  linear_fwd(seg("san.img.weight"), pool5, B * cfg.P, t, 1);
 }
+// Region engines (DESIGN §26): san_cnt holds the B dialogs' counts (null: all present); the GEMMs run over all P rows, the
+// attention kernels skip the pad rows and give them zero probability and zero gradients.
 void Engine::san_block_fwd(const float* u0, const float* timg, int B, int nr, float* out) {
   const int H = cfg.H;
   const int64_t N = (int64_t)B * nr;
-  const int P = cfg.S * cfg.S, Cm = cfg.Cm;
+  const int P = cfg.P, Cm = cfg.Cm;
   const DropCfg d05 = dropcfg(0.5f);
   t_img = const_cast<float*>(timg);
   img_tr = arena.get<float>(N * P * H);
@@ -856,10 +877,11 @@ void Engine::san_block_fwd(const float* u0, const float* timg, int B, int nr, fl
     ques_common[hop] = arena.get<float>(N * Cm);
     linear_fwd(w_qc, u_hop[hop], N, ques_common[hop], 0);
     sc[hop] = arena.get<float>(N * P);
-    san_score_fwd(cx, img_common[hop], ques_common[hop], Wp(w_s), Wp(w_s + 1), sc[hop], N, P, Cm, d05, SITE_HOP0 + hop);
+    san_score_fwd(cx, img_common[hop], ques_common[hop], Wp(w_s), Wp(w_s + 1), sc[hop], N, P, Cm, d05, SITE_HOP0 + hop, san_cnt,
+                  nr);
     pr[hop] = arena.get<float>(N * P);
     u_hop[hop + 1] = arena.get<float>(N * H);
-    san_softmax_att_fwd(cx, sc[hop], pr[hop], img_tr, u_hop[hop], u_hop[hop + 1], N, P, H);
+    san_softmax_att_fwd(cx, sc[hop], pr[hop], img_tr, u_hop[hop], u_hop[hop + 1], N, P, H, san_cnt, nr);
   }
   u_d = arena.get<float>(N * H);
   dropout_apply(cx, u_d, u_hop[cfg.hops], N * H, d05, SITE_U_OUT);
@@ -868,7 +890,7 @@ void Engine::san_block_fwd(const float* u0, const float* timg, int B, int nr, fl
 void Engine::san_block_bwd(const float* dEnc, float* du) {
   const int H = cfg.H, R = cfg.R, B = db.B;
   const int64_t N = db.N;
-  const int P = cfg.S * cfg.S, Cm = cfg.Cm;
+  const int P = cfg.P, Cm = cfg.Cm;
   const DropCfg d05 = dropcfg(0.5f);
   float* dpre = arena.get<float>(N * H);
   tanh_bwd(cx, dpre, dEnc, encOut, N * H);
@@ -883,19 +905,19 @@ void Engine::san_block_bwd(const float* dEnc, float* du) {
     int w_ic = seg((pre + "img_common.weight").c_str()), w_qc = seg((pre + "ques_common.weight").c_str()),
         w_s = seg((pre + "score.weight").c_str());
     if (hop == cfg.hops - 1) {
-      san_att_bwd(cx, du, pr[hop], img_tr, ds, dimg_tr, N, P, H);
+      san_att_bwd(cx, du, pr[hop], img_tr, ds, dimg_tr, N, P, H, san_cnt, R);
     } else {
       float* tmp = arena.get<float>(N * P * H);
-      san_att_bwd(cx, du, pr[hop], img_tr, ds, tmp, N, P, H);
+      san_att_bwd(cx, du, pr[hop], img_tr, ds, tmp, N, P, H, san_cnt, R);
       add_inplace(cx, dimg_tr, tmp, N * P * H);
     }
     san_score_bwd(cx, ds, img_common[hop], ques_common[hop], Wp(w_s), dic, dqc, dWp(w_s), dWp(w_s + 1), N, P, Cm, d05,
-                  SITE_HOP0 + hop);
+                  SITE_HOP0 + hop, san_cnt, R);
     linear_bwd(w_ic, img_tr, dic, N * P, dimg_tr, 1.f);
     linear_bwd(w_qc, u_hop[hop], dqc, N, du, 1.f);          // du now = grad wrt u_hop[hop]
   }
   float* dt_pre = arena.get<float>((int64_t)B * P * H);
-  san_collapse_bwd(cx, dimg_tr, t_img, dt_pre, B, R, P, H, d05, SITE_IMG_TR);
+  san_collapse_bwd(cx, dimg_tr, t_img, dt_pre, B, R, P, H, d05, SITE_IMG_TR, san_cnt);
   linear_bwd(seg("san.img.weight"), db.img, dt_pre, (int64_t)B * P, nullptr, 0.f);
   release_img();                                   // last reader of this step's image staging buffer
 }
@@ -1080,9 +1102,10 @@ void Engine::encoder_forward(const vd_batch* b) {
 
   const float* timg = nullptr;
   if (cfg.san) {
-    float* t = arena.get<float>((int64_t)B * cfg.S * cfg.S * H);
+    float* t = arena.get<float>((int64_t)B * cfg.P * H);
     san_image(db.img, B, t);
     timg = t;
+    san_cnt = db.img_count;
   }
   if (cfg.fam_lf) {
     lf_block_fwd(q3, db.img, timg, h3, B, R, encOut);
@@ -2037,6 +2060,7 @@ void Engine::gen_dialog(const vd_batch* b, int W, int max_ans_len, const std::fu
     hist_append(cx, hist, B, R, W, -1, db.hist, db.Th, nullptr, 0, nullptr, 0, 0, 0, false);   // round 0 <- the caption row
     vd_batch rb = {};
     rb.B = B; rb.Tq = db.Tq; rb.Th = W; rb.ques_fwd = db.ques; rb.hist = hist; rb.img_feat = db.img; rb.on_device = 1;
+    rb.img_count = db.img_count;
     for (int r = 0; r < R; ++r) {
       encoder_forward(&rb);
       const DialogAnswers a = search(r);
@@ -2250,7 +2274,7 @@ void Engine::dialog_open(int C, int Tq, int W, int max_ans_len) {
   VD_CUDA_CHECK(cudaSetDevice(cfg.gpuid));
   const int R = cfg.R, H = cfg.H;
   if (!cfg.useHist) W = 0;
-  dses.img_cols = cfg.san ? (int64_t)cfg.S * cfg.S * H : cfg.img_in_q ? cfg.IE : cfg.useIm ? cfg.F : 0;
+  dses.img_cols = cfg.san ? (int64_t)cfg.P * H : cfg.img_in_q ? cfg.IE : cfg.useIm ? cfg.F : 0;
   if (cfg.useHist) {
     dses.hist.ensure((size_t)C * R * W * sizeof(int32_t));
     if (cfg.fam_mn || cfg.hre_att) dses.facts.ensure((size_t)C * R * H * sizeof(float));   // the attention's facts
@@ -2266,6 +2290,7 @@ void Engine::dialog_open(int C, int Tq, int W, int max_ans_len) {
   dses.C = C; dses.Tq = Tq; dses.W = W; dses.max_ans_len = max_ans_len;
   dses.round.assign(C, -1);
   dses.draw_base.assign(C, 0);
+  dses.count.assign(cfg.regions > 0 ? C : 0, cfg.P);
   dses.open = dses.valid = true;
 }
 
@@ -2290,11 +2315,26 @@ void Engine::dialog_join(const vd_batch* b, const int64_t* draw_base, int32_t* s
   const vd_batch eb = encoder_only(b);
   dialog_join_images(&eb, slots.data());
   VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
+  const std::vector<int32_t> counts = batch_counts_host(b);
   for (int i = 0; i < B; ++i) {
+    if (!counts.empty()) dses.count[slots[i]] = counts[i];
     dses.round[slots[i]] = 0;
     dses.draw_base[slots[i]] = draw_base ? draw_base[i] : 0;
     slots_host[i] = slots[i];
   }
+}
+
+std::vector<int32_t> Engine::batch_counts_host(const vd_batch* b) {
+  std::vector<int32_t> c;
+  if (cfg.regions <= 0) return c;
+  c.assign(b->B, cfg.P);
+  if (b->img_count && b->on_device) {
+    VD_CUDA_CHECK(cudaStreamSynchronize(main_stream));   // a corpus batch's counts are gathered on the main stream
+    VD_CUDA_CHECK(cudaMemcpy(c.data(), b->img_count, (size_t)b->B * sizeof(int32_t), cudaMemcpyDeviceToHost));
+  }
+  else if (b->img_count)
+    std::copy_n(b->img_count, b->B, c.data());
+  return c;
 }
 
 const int32_t* Engine::dialog_join_images(const vd_batch* b, const int32_t* slots) {
@@ -2462,7 +2502,9 @@ void Engine::dialog_join_rounds(const vd_batch* b, const int32_t* rounds, const 
     VD_CUDA_CHECK(cudaStreamSynchronize(cx.stream));
   } catch (...) { training = saved_training; throw; }
   training = saved_training;
+  const std::vector<int32_t> counts = batch_counts_host(b);
   for (int i = 0; i < B; ++i) {
+    if (!counts.empty()) dses.count[slots[i]] = counts[i];
     dses.round[slots[i]] = rounds[i];
     dses.draw_base[slots[i]] = draw_base ? draw_base[i] : 0;
   }
@@ -2542,7 +2584,9 @@ Engine::AskRows Engine::dialog_encode(const int32_t* slots, int64_t n, const int
   const int R = cfg.R, H = cfg.H, Tw = dses.Tq, W = dses.W;
   AskRows rows;
   rows.n = n;
-  std::vector<int32_t> up((size_t)n * (2 + Tw), 0);          // slot, round, questions right-aligned into the session's width
+  // slot, round, questions right-aligned into the session's width, then (region engines) the slot's region count
+  const int64_t o_cnt = n * (2 + Tw);
+  std::vector<int32_t> up((size_t)(o_cnt + (cfg.regions > 0 ? n : 0)), 0);
   std::vector<int64_t> draw(n);
   bool any_state = false;
   for (int64_t i = 0; i < n; ++i) {
@@ -2552,12 +2596,14 @@ Engine::AskRows Engine::dialog_encode(const int32_t* slots, int64_t n, const int
     any_state |= r > 0;
     rows.any_next |= r + 1 < R;
     for (int t = 0; t < Tq; ++t) up[2 * n + i * Tw + Tw - Tq + t] = ques_host[i * Tq + t];
+    if (cfg.regions > 0) up[o_cnt + i] = dses.count[s];
   }
   int64_t* draw_dev = arena.get<int64_t>(n);
   int32_t* up_dev = arena.get<int32_t>((int64_t)up.size());
   VD_CUDA_CHECK(cudaMemcpyAsync(draw_dev, draw.data(), draw.size() * sizeof(int64_t), cudaMemcpyHostToDevice, cx.stream));
   VD_CUDA_CHECK(cudaMemcpyAsync(up_dev, up.data(), up.size() * sizeof(int32_t), cudaMemcpyHostToDevice, cx.stream));
   rows.slot = up_dev; rows.round = up_dev + n; rows.draw = draw_dev;
+  san_cnt = cfg.regions > 0 ? up_dev + o_cnt : nullptr;
   DialogGather g;
   g.n = n; g.R = R; g.slot = rows.slot; g.round = rows.round;
   g.q = up_dev + 2 * n; g.Tq = Tw; g.ques = (int32_t*)dses.ques.p; g.ids_q = ids_q = arena.get<int32_t>(n * Tw);

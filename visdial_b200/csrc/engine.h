@@ -17,6 +17,8 @@ struct Cfg {
   std::string encoder, decoder;
   int enc = 0, dec = 0;
   int V = 0, E = 300, H = 512, L = 2, F = 4096, S = 14, IE = 300, Cm = 512, hops = 1, R = 10, K = 100;
+  int regions = 0;          // imgRegions: 0 = the S x S grid, > 0 = region rows (DESIGN §26)
+  int P = 196;              // SAN positions per image: S * S, or regions
   float dropout = 0.5f;
   int gpuid = 0;
   bool useIm = false, useHist = false, att = false;
@@ -122,6 +124,7 @@ struct DevBatch {
   const int32_t* options = nullptr; const int32_t* answer_ind = nullptr;
   const int32_t* answer_in = nullptr; const int32_t* answer_out = nullptr;
   const int32_t* option_in = nullptr; const int32_t* option_out = nullptr;
+  const int32_t* img_count = nullptr;   // (B) region counts, null = all present
 };
 
 struct GrowBuf {
@@ -192,6 +195,8 @@ struct Engine {
   // mn-att
   float *hAtt = nullptr, *hAtt_d = nullptr, *hAttTr = nullptr, *sum1 = nullptr, *qh2 = nullptr, *t_img = nullptr,
         *img_tr = nullptr, *u_d = nullptr;
+  const int32_t* san_cnt = nullptr;  // region counts of the SAN's dialogs (one per san_block_fwd dialog), null = all present
+  GrowBuf stage_cnt;                 // a host batch's img_count, staged
   std::vector<float*> img_common, ques_common, sc, pr, u_hop;   // per hop; u_hop[0] = qh2
   // decoder
   float *scores = nullptr, *dscores = nullptr, *row_loss = nullptr, *logp = nullptr, *dlogits = nullptr,
@@ -305,7 +310,7 @@ struct Engine {
   void mn_block_fwd(const float* qin, const float* facts, int64_t fpitch, float* out, int B, int r0, int r1,
                     const int32_t* slot = nullptr, const int32_t* round = nullptr);
   void mn_block_bwd(const float* dout, const float* out, float* dqin, float* dh3);   // dqin / dh3 are overwritten
-  void san_image(const float* pool5, int64_t B, float* t);      // t (B, S*S, H) = tanh(Linear(pool5)), once per dialog
+  void san_image(const float* pool5, int64_t B, float* t);      // t (B, P, H) = tanh(Linear(pool5)), once per dialog
   void san_block_fwd(const float* u0, const float* timg, int B, int nr, float* out);   // SAN hops + out layer -> out
   void lf_block_fwd(const float* q3, const float* fc7, const float* timg, const float* h3, int B, int nr, float* out);
   void hre_join_fwd(const float* q3, const float* facts, const float* sq, const float* sh, int64_t fpitch, int B, int r0, int r1,
@@ -403,9 +408,10 @@ struct Engine {
   struct DialogSession {
     bool open = false, valid = false;  // valid drops when the weights or the math mode change
     int C = 0, Tq = 0, W = 0, max_ans_len = 0;
-    int64_t img_cols = 0;              // the per-slot image product: SAN t_img (S*S*H), img.embed(fc7) (IE) or fc7 (F); 0: none
+    int64_t img_cols = 0;              // the per-slot image product: SAN t_img (P*H), img.embed(fc7) (IE) or fc7 (F); 0: none
     std::vector<int> round;            // per slot: the next round to be asked, -1 while free
     std::vector<int64_t> draw_base;    // per slot: the global round its round 0 draws as, for sampling asks
+    std::vector<int32_t> count;        // per slot: its image's region count (region engines, DESIGN §26)
     // per slot: history (C, R, W), asked questions (C, R, Tq), image product (C, img_cols), facts (C, R, H) (mn, hrea), sh
     // (C, R) (hrea), dialog-LSTM {h, c} (C, H) (hre / hrea).  The last ask's question-LSTM {h1, c1, h2, c2} (encoders with
     // .rnnLayers) and encoding, n rows in the ask's order: the decoder start state.
@@ -425,6 +431,8 @@ struct Engine {
   void dialog_join_rounds(const vd_batch* b, const int32_t* rounds, const int32_t* answers, int Ta, const int64_t* draw_base,
                           const int32_t* slots);
   void dialog_leave(const int32_t* slots, int64_t n);
+  // b's B region counts on the host (cfg.P each when b carries none); empty for a grid engine
+  std::vector<int32_t> batch_counts_host(const vd_batch* b);
   void dialog_begin(const vd_batch* b, int W, int max_ans_len);
   void dialog_end();
   void dialog_check_slots(const int32_t* slots, int64_t n) const;   // in [0, C), distinct, occupied

@@ -138,18 +138,20 @@ void masktime_bwd(LaunchCtx& cx, const float* dx, int64_t ldx, int off, const in
                   int T, int64_t N, int I);
 
 // ---- SAN spatial attention (mn-att-ques-im-hist.lua:67-106) ---------------------------------------
+// cnt (region features, DESIGN §26): null = every position attended; else (N / R) per-dialog counts c in [1, P], row n
+// attends over positions 0 .. cnt[n / R] - 1 and the pad positions' outputs are zeros (san_collapse_bwd: cnt (B)).
 void san_expand_dropout(LaunchCtx& cx, float* img_tr, const float* t, int B, int R, int P, int H, DropCfg d, uint32_t site);
 void san_score_fwd(LaunchCtx& cx, const float* img_common, const float* ques_common, const float* w, const float* b,
-                   float* s, int64_t N, int P, int Cm, DropCfg d, uint32_t site);
+                   float* s, int64_t N, int P, int Cm, DropCfg d, uint32_t site, const int32_t* cnt = nullptr, int R = 1);
 void san_softmax_att_fwd(LaunchCtx& cx, const float* s, float* p, const float* img_tr, const float* u_in, float* u_out,
-                         int64_t N, int P, int H);
+                         int64_t N, int P, int H, const int32_t* cnt = nullptr, int R = 1);
 void san_att_bwd(LaunchCtx& cx, const float* du, const float* p, const float* img_tr, float* ds, float* dimg_tr,
-                 int64_t N, int P, int H);
+                 int64_t N, int P, int H, const int32_t* cnt = nullptr, int R = 1);
 void san_score_bwd(LaunchCtx& cx, const float* ds, const float* img_common, const float* ques_common, const float* w,
                    float* d_img_common, float* d_ques_common, float* dw, float* db, int64_t N, int P, int Cm,
-                   DropCfg d, uint32_t site);
+                   DropCfg d, uint32_t site, const int32_t* cnt = nullptr, int R = 1);
 void san_collapse_bwd(LaunchCtx& cx, const float* dimg_tr, const float* t, float* dt_pre, int B, int R, int P, int H,
-                      DropCfg d, uint32_t site);
+                      DropCfg d, uint32_t site, const int32_t* cnt = nullptr);
 
 // ---- decoders / criterions / ranks ---------------------------------------------------------------
 // disc.lua:22-29  scores[n,k] = feat[n,k,:] . encOut[n,:]

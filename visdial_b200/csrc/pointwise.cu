@@ -767,13 +767,23 @@ __device__ __forceinline__ float tanh_e(float x) {
   const float e = __expf(-2.f * fabsf(x));
   return copysignf(__fdividef(1.f - e, 1.f + e), x);
 }
+// Region features (DESIGN §26): with MASK, row n of the SAN kernels below attends over positions 0 .. cnt[n / R] - 1 only.
+// Positions at or past the count are never loaded; their outputs (score, probability, ds, dic, dimg_tr, dt_pre) are written as
+// zeros.  The count arguments come last so that the MASK = false instantiations keep the parameter offsets they had.
+
 // warp per (n,p)
+template <bool MASK>
 __global__ void k_san_score_fwd(const float* __restrict__ ic, const float* __restrict__ qc, const float* __restrict__ w,
-                                const float* __restrict__ b, float* __restrict__ s, int64_t NP, int P, int Cm, DropCfg d, uint32_t site) {
+                                const float* __restrict__ b, float* __restrict__ s, int64_t NP, int P, int Cm, DropCfg d, uint32_t site,
+                                const int32_t* __restrict__ cnt, int R) {
   int64_t row = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   int l = threadIdx.x & 31;
   if (row >= NP) return;
   int64_t n = row / P;
+  if (MASK && (int)(row - n * P) >= cnt[n / R]) {
+    if (l == 0) s[row] = 0.f;
+    return;
+  }
   float acc = 0.f;
   for (int c4 = l; c4 < (Cm >> 2); c4 += 32) {
     float4 a = reinterpret_cast<const float4*>(ic + row * Cm)[c4];
@@ -793,19 +803,24 @@ __global__ void k_san_score_fwd(const float* __restrict__ ic, const float* __res
 
 // grid (N, 2 halves of H), block 256: softmax over the P scores (recomputed per half: P is 196), then u_out = p . img_tr + u_in for the
 // half's columns — thread = float4 column piece x position group, groups combined in shared memory
+template <bool MASK>
 __global__ void __launch_bounds__(256) k_san_softmax_att_fwd(const float* __restrict__ s, float* __restrict__ p, const float* __restrict__ img_tr,
-                                                             const float* __restrict__ u_in, float* __restrict__ u_out, int P, int H) {
+                                                             const float* __restrict__ u_in, float* __restrict__ u_out, int P, int H,
+                                                             const int32_t* __restrict__ cnt, int R) {
   extern __shared__ float sm[];          // P floats + 33 + 256 float4
   float* sp = sm; float* red = sm + P;
   float4* part = reinterpret_cast<float4*>(sm + ((P + 33 + 3) & ~3));
   const int64_t n = blockIdx.x;
+  const int c = MASK ? cnt[n / R] : P;   // positions attended
   float mx = -INFINITY;
-  for (int i = threadIdx.x; i < P; i += blockDim.x) { float v = s[n * P + i]; sp[i] = v; mx = fmaxf(mx, v); }
+  for (int i = threadIdx.x; i < c; i += blockDim.x) { float v = s[n * P + i]; sp[i] = v; mx = fmaxf(mx, v); }
   mx = block_max(mx, red);
   float sum = 0.f;
-  for (int i = threadIdx.x; i < P; i += blockDim.x) { float e = expf(sp[i] - mx); sp[i] = e; sum += e; }
+  for (int i = threadIdx.x; i < c; i += blockDim.x) { float e = expf(sp[i] - mx); sp[i] = e; sum += e; }
   sum = block_sum(sum, red);
-  for (int i = threadIdx.x; i < P; i += blockDim.x) { float v = sp[i] / sum; sp[i] = v; if (blockIdx.y == 0) p[n * P + i] = v; }
+  for (int i = threadIdx.x; i < c; i += blockDim.x) { float v = sp[i] / sum; sp[i] = v; if (blockIdx.y == 0) p[n * P + i] = v; }
+  if (MASK && blockIdx.y == 0)
+    for (int i = c + threadIdx.x; i < P; i += blockDim.x) p[n * P + i] = 0.f;
   __syncthreads();
   const int H4 = H >> 2, half = (H4 + 1) >> 1;
   const int c_lo = blockIdx.y * half, c_hi = min(H4, c_lo + half);
@@ -817,14 +832,14 @@ __global__ void __launch_bounds__(256) k_san_softmax_att_fwd(const float* __rest
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (pg < npg && c4 < c_hi) {
       int i = pg;
-      for (; i + 3 * npg < P; i += 4 * npg) {
+      for (; i + 3 * npg < c; i += 4 * npg) {
         const float4 a = base[(int64_t)i * H4 + c4], b = base[(int64_t)(i + npg) * H4 + c4];
-        const float4 c = base[(int64_t)(i + 2 * npg) * H4 + c4], e = base[(int64_t)(i + 3 * npg) * H4 + c4];
+        const float4 g = base[(int64_t)(i + 2 * npg) * H4 + c4], e = base[(int64_t)(i + 3 * npg) * H4 + c4];
         const float w0 = sp[i], w1 = sp[i + npg], w2 = sp[i + 2 * npg], w3 = sp[i + 3 * npg];
-        acc.x += w0 * a.x + w1 * b.x + w2 * c.x + w3 * e.x; acc.y += w0 * a.y + w1 * b.y + w2 * c.y + w3 * e.y;
-        acc.z += w0 * a.z + w1 * b.z + w2 * c.z + w3 * e.z; acc.w += w0 * a.w + w1 * b.w + w2 * c.w + w3 * e.w;
+        acc.x += w0 * a.x + w1 * b.x + w2 * g.x + w3 * e.x; acc.y += w0 * a.y + w1 * b.y + w2 * g.y + w3 * e.y;
+        acc.z += w0 * a.z + w1 * b.z + w2 * g.z + w3 * e.z; acc.w += w0 * a.w + w1 * b.w + w2 * g.w + w3 * e.w;
       }
-      for (; i < P; i += npg) {
+      for (; i < c; i += npg) {
         const float4 a = base[(int64_t)i * H4 + c4]; const float w0 = sp[i];
         acc.x += w0 * a.x; acc.y += w0 * a.y; acc.z += w0 * a.z; acc.w += w0 * a.w;
       }
@@ -841,18 +856,21 @@ __global__ void __launch_bounds__(256) k_san_softmax_att_fwd(const float* __rest
 }
 
 // block per n (512 threads): dp = du . img_tr ; ds = p*(dp - sum p dp) ; dimg_tr = p * du
+template <bool MASK>
 __global__ void __launch_bounds__(512) k_san_att_bwd(const float* __restrict__ du, const float* __restrict__ p, const float* __restrict__ img_tr,
-                                                     float* __restrict__ ds, float* __restrict__ dimg_tr, int P, int H) {
+                                                     float* __restrict__ ds, float* __restrict__ dimg_tr, int P, int H,
+                                                     const int32_t* __restrict__ cnt, int R) {
   extern __shared__ float sm[];          // H + P + P + 33
   float* sdu = sm; float* sp = sdu + H; float* sdp = sp + P; float* red = sdp + P;
   const int64_t n = blockIdx.x;
   const int tid = threadIdx.x, nw = blockDim.x >> 5, w = tid >> 5, l = tid & 31;
   const int H4 = H >> 2;
+  const int cn = MASK ? cnt[n / R] : P;  // positions attended
   for (int c = tid; c < H; c += blockDim.x) sdu[c] = du[n * H + c];
-  for (int i = tid; i < P; i += blockDim.x) sp[i] = p[n * P + i];
+  for (int i = tid; i < cn; i += blockDim.x) sp[i] = p[n * P + i];
   __syncthreads();
   const float4* sdu4 = reinterpret_cast<const float4*>(sdu);
-  for (int i = w; i < P; i += nw) {
+  for (int i = w; i < cn; i += nw) {
     const float4* row = reinterpret_cast<const float4*>(img_tr) + (n * P + i) * H4;
     float acc = 0.f;
 #pragma unroll 4
@@ -862,11 +880,17 @@ __global__ void __launch_bounds__(512) k_san_att_bwd(const float* __restrict__ d
   }
   __syncthreads();
   float part = 0.f;
-  for (int i = tid; i < P; i += blockDim.x) part += sp[i] * sdp[i];
+  for (int i = tid; i < cn; i += blockDim.x) part += sp[i] * sdp[i];
   float dot = block_sum(part, red);
-  for (int i = tid; i < P; i += blockDim.x) ds[n * P + i] = sp[i] * (sdp[i] - dot);
+  for (int i = tid; i < cn; i += blockDim.x) ds[n * P + i] = sp[i] * (sdp[i] - dot);
+  if (MASK)
+    for (int i = cn + tid; i < P; i += blockDim.x) ds[n * P + i] = 0.f;
   float4* out = reinterpret_cast<float4*>(dimg_tr) + n * P * H4;
   for (int i = w; i < P; i += nw) {
+    if (MASK && i >= cn) {
+      for (int c = l; c < H4; c += 32) out[(int64_t)i * H4 + c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      continue;
+    }
     const float pi = sp[i];
     for (int c = l; c < H4; c += 32) { const float4 b = sdu4[c]; out[(int64_t)i * H4 + c] = make_float4(pi * b.x, pi * b.y, pi * b.z, pi * b.w); }
   }
@@ -875,14 +899,17 @@ __global__ void __launch_bounds__(512) k_san_att_bwd(const float* __restrict__ d
 // grid (N, column slices), block 256: thread = float4 column piece x position group; a block walks ALL P positions of its columns, the
 // position groups are combined in shared memory in a fixed order, so dqc — an intermediate gradient that flows on into the encoder — is
 // written once and deterministically (only the leaf gradients dw, db use atomics).  Recomputes y = tanh(ic + qc) and the dropout factor.
+template <bool MASK>
 __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__ ds, const float* __restrict__ ic, const float* __restrict__ qc,
                                                        const float* __restrict__ w, float* __restrict__ dic, float* __restrict__ dqc,
-                                                       float* __restrict__ dw, float* __restrict__ db, int P, int Cm, DropCfg d, uint32_t site) {
+                                                       float* __restrict__ dw, float* __restrict__ db, int P, int Cm, DropCfg d, uint32_t site,
+                                                       const int32_t* __restrict__ cnt, int R) {
   extern __shared__ float sm[];          // P floats (ds row), then 2 x 256 float4
   float4* part_q = reinterpret_cast<float4*>(sm + ((P + 3) & ~3));
   float4* part_w = part_q + 256;
   const int64_t n = blockIdx.x;
-  for (int i = threadIdx.x; i < P; i += blockDim.x) sm[i] = ds[n * P + i];
+  const int cn = MASK ? cnt[n / R] : P;  // positions attended
+  for (int i = threadIdx.x; i < cn; i += blockDim.x) sm[i] = ds[n * P + i];
   __syncthreads();
   const int C4 = Cm >> 2, per = (C4 + gridDim.y - 1) / gridDim.y;
   const int c_lo = blockIdx.y * per, c_hi = min(C4, c_lo + per);
@@ -896,7 +923,7 @@ __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__
     if (pg < npg && c4 < c_hi) {
       const float4 q = reinterpret_cast<const float4*>(qc)[n * C4 + c4], wc = reinterpret_cast<const float4*>(w)[c4];
 #pragma unroll 4
-      for (int i = pg; i < P; i += npg) {
+      for (int i = pg; i < cn; i += npg) {
         const int64_t idx4 = (n * P + i) * C4 + c4;
         const float4 a = ic4[idx4];
         float f[4];
@@ -909,6 +936,8 @@ __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__
         aq.x += o.x; aq.y += o.y; aq.z += o.z; aq.w += o.w;
         aw.x += g0 * y0; aw.y += g1 * y1; aw.z += g2 * y2; aw.w += g3 * y3;
       }
+      if (MASK)
+        for (int i = cn + pg; i < P; i += npg) dic4[(n * P + i) * C4 + c4] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     part_q[threadIdx.x] = aq; part_w[threadIdx.x] = aw;
     __syncthreads();
@@ -926,17 +955,24 @@ __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__
   // db: the scores of a row enter a softmax, so sum_i ds[n, i] is zero up to rounding — summed in a fixed order by one thread
   if (blockIdx.y == 0 && threadIdx.x == 0) {
     float acc = 0.f;
-    for (int i = 0; i < P; ++i) acc += sm[i];
+    for (int i = 0; i < cn; ++i) acc += sm[i];
     atomicAdd(db, acc);
   }
 }
 
-// thread = float4 of (B,P,H): sum over the R rounds that share the image (dropout factor recomputed), times tanh'
+// thread = float4 of (B,P,H): sum over the R rounds that share the image (dropout factor recomputed), times tanh'.  With
+// MASK, dialog b's positions at or past cnt[b] (H4 float4 per position) are written as zeros.
+template <bool MASK>
 __global__ void k_san_collapse_bwd(const float* __restrict__ dimg_tr, const float* __restrict__ t, float* __restrict__ dt_pre,
-                                   int64_t total4, int R, int64_t PH4, DropCfg d, uint32_t site) {
+                                   int64_t total4, int R, int64_t PH4, DropCfg d, uint32_t site, const int32_t* __restrict__ cnt,
+                                   int64_t H4) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;    // float4 index into (B,P,H)
   if (i >= total4) return;
   int64_t b = i / PH4, rem = i % PH4;
+  if (MASK && rem / H4 >= cnt[b]) {
+    reinterpret_cast<float4*>(dt_pre)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 5
   for (int r = 0; r < R; ++r) {
@@ -1973,42 +2009,51 @@ void san_expand_dropout(LaunchCtx& cx, float* img_tr, const float* t, int B, int
   L1D(k_san_expand_dropout, total4, img_tr, t, total4, R, PH4, d, site);
 }
 void san_score_fwd(LaunchCtx& cx, const float* img_common, const float* ques_common, const float* w, const float* b, float* s,
-                   int64_t N, int P, int Cm, DropCfg d, uint32_t site) {
+                   int64_t N, int P, int Cm, DropCfg d, uint32_t site, const int32_t* cnt, int R) {
   VD_REQUIRE(Cm % 4 == 0, -1, "commonEmbeddingSize % 4");
-  L1D(k_san_score_fwd, N * P * 32, img_common, ques_common, w, b, s, N * P, P, Cm, d, site);
+  if (N * P <= 0) return;
+  auto k = cnt ? k_san_score_fwd<true> : k_san_score_fwd<false>;
+  k<<<blocks_for(N * P * 32, 256), 256, 0, cx.stream>>>(img_common, ques_common, w, b, s, N * P, P, Cm, d, site, cnt, R);
+  check_launch(cx, "k_san_score_fwd");
 }
 void san_softmax_att_fwd(LaunchCtx& cx, const float* s, float* p, const float* img_tr, const float* u_in, float* u_out,
-                         int64_t N, int P, int H) {
+                         int64_t N, int P, int H, const int32_t* cnt, int R) {
   if (N <= 0) return;
   VD_REQUIRE(H % 4 == 0, -1, "H % 4");
   size_t smem = (size_t)(((P + 33 + 3) & ~3) + 256 * 4) * sizeof(float);
-  k_san_softmax_att_fwd<<<dim3((unsigned)N, 2), 256, smem, cx.stream>>>(s, p, img_tr, u_in, u_out, P, H);
+  auto k = cnt ? k_san_softmax_att_fwd<true> : k_san_softmax_att_fwd<false>;
+  k<<<dim3((unsigned)N, 2), 256, smem, cx.stream>>>(s, p, img_tr, u_in, u_out, P, H, cnt, R);
   check_launch(cx, "san_softmax_att_fwd");
 }
 void san_att_bwd(LaunchCtx& cx, const float* du, const float* p, const float* img_tr, float* ds, float* dimg_tr, int64_t N,
-                 int P, int H) {
+                 int P, int H, const int32_t* cnt, int R) {
   if (N <= 0) return;
   VD_REQUIRE(H % 4 == 0, -1, "H % 4");
   size_t smem = (size_t)(H + 2 * P + 33) * sizeof(float);
-  k_san_att_bwd<<<(int)N, 512, smem, cx.stream>>>(du, p, img_tr, ds, dimg_tr, P, H);
+  auto k = cnt ? k_san_att_bwd<true> : k_san_att_bwd<false>;
+  k<<<(int)N, 512, smem, cx.stream>>>(du, p, img_tr, ds, dimg_tr, P, H, cnt, R);
   check_launch(cx, "san_att_bwd");
 }
 void san_score_bwd(LaunchCtx& cx, const float* ds, const float* img_common, const float* ques_common, const float* w,
                    float* d_img_common, float* d_ques_common, float* dw, float* db, int64_t N, int P, int Cm, DropCfg d,
-                   uint32_t site) {
+                   uint32_t site, const int32_t* cnt, int R) {
   if (N <= 0) return;
   VD_REQUIRE(Cm % 4 == 0, -1, "commonEmbeddingSize % 4");
   const int CS = Cm >= 512 ? 4 : 1;                      // column slices per dialog round
   const size_t smem = (size_t)(((P + 3) & ~3) + 2 * 256 * 4) * sizeof(float);
-  k_san_score_bwd<<<dim3((unsigned)N, CS), 256, smem, cx.stream>>>(ds, img_common, ques_common, w, d_img_common, d_ques_common, dw, db, P,
-                                                                    Cm, d, site);
+  auto k = cnt ? k_san_score_bwd<true> : k_san_score_bwd<false>;
+  k<<<dim3((unsigned)N, CS), 256, smem, cx.stream>>>(ds, img_common, ques_common, w, d_img_common, d_ques_common, dw, db, P, Cm, d,
+                                                      site, cnt, R);
   check_launch(cx, "san_score_bwd");
 }
 void san_collapse_bwd(LaunchCtx& cx, const float* dimg_tr, const float* t, float* dt_pre, int B, int R, int P, int H,
-                      DropCfg d, uint32_t site) {
+                      DropCfg d, uint32_t site, const int32_t* cnt) {
   VD_REQUIRE(H % 4 == 0, -1, "H % 4");
   int64_t PH4 = (int64_t)P * H / 4, total4 = (int64_t)B * PH4;
-  L1D(k_san_collapse_bwd, total4, dimg_tr, t, dt_pre, total4, R, PH4, d, site);
+  if (total4 <= 0) return;
+  auto k = cnt ? k_san_collapse_bwd<true> : k_san_collapse_bwd<false>;
+  k<<<blocks_for(total4, 256), 256, 0, cx.stream>>>(dimg_tr, t, dt_pre, total4, R, PH4, d, site, cnt, (int64_t)H / 4);
+  check_launch(cx, "k_san_collapse_bwd");
 }
 
 void disc_scores_fwd(LaunchCtx& cx, const float* feat, const float* encOut, float* scores, int64_t N, int K, int H) {

@@ -211,6 +211,29 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {
        san_collapse_bwd(e->cx, CF(0), CF(1), F(2), IN(0), IN(1), IN(2), IN(3), DROP(0), (uint32_t)I[4]);
      }},
+    // masked SAN (region features, DESIGN §26): the pointer after the unmasked entry's is the count array; ints as the
+    // unmasked entry's, then R (rows per count; san_collapse_bwd's counts are per dialog)
+    {"san_score_fwd_masked", 6, 5, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       san_score_fwd(e->cx, CF(0), CF(1), CF(2), CF(3), F(4), I[0], IN(1), IN(2), DROP(0), (uint32_t)I[3], CI32(5), IN(4));
+     }},
+    {"san_softmax_att_fwd_masked", 6, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       san_softmax_att_fwd(e->cx, CF(0), F(1), CF(2), CF(3), F(4), I[0], IN(1), IN(2), CI32(5), IN(3));
+     }},
+    {"san_att_bwd_masked", 6, 4, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       san_att_bwd(e->cx, CF(0), CF(1), CF(2), F(3), F(4), I[0], IN(1), IN(2), CI32(5), IN(3));
+     }},
+    {"san_score_bwd_masked", 9, 5, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       san_score_bwd(e->cx, CF(0), CF(1), CF(2), CF(3), F(4), F(5), F(6), F(7), I[0], IN(1), IN(2), DROP(0), (uint32_t)I[3],
+                     CI32(8), IN(4));
+     }},
+    {"san_collapse_bwd_masked", 4, 5, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       san_collapse_bwd(e->cx, CF(0), CF(1), F(2), IN(0), IN(1), IN(2), IN(3), DROP(0), (uint32_t)I[4], CI32(3));
+     }},
     // ---- option scores, criteria, ranks
     {"disc_scores_fwd", 3, 3, 0,
      [](Engine* e, void* const* P, const int64_t* I, const double*) { disc_scores_fwd(e->cx, CF(0), CF(1), F(2), I[0], IN(1), IN(2)); }},

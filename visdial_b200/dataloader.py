@@ -13,7 +13,7 @@ There is no CPU path: without libvisdial_b200.so and a GPU every call raises.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 
@@ -37,6 +37,7 @@ class DeviceBatch(Batch):
         "answer_in": lambda b, R, K: (b.B, R, b.Ta), "answer_out": lambda b, R, K: (b.B, R, b.Ta),
         "answer_ind": lambda b, R, K: (b.B, R), "options": lambda b, R, K: (b.B * R, K, b.To),
         "option_in": lambda b, R, K: (b.B, R, K, b.To), "option_out": lambda b, R, K: (b.B, R, K, b.To),
+        "img_count": lambda b, R, K: (b.B,),
     }
 
     def __init__(self, eng: Engine, c: vd_batch, R: int, K: int, img_shape, num_answer_tokens: int,
@@ -76,6 +77,23 @@ class DeviceBatch(Batch):
         return self
 
 
+def read_num_boxes(path: str, dtype: str) -> Optional[np.ndarray]:
+    """num_boxes_<dtype> of an image features file, or None when the file has none (every region present)."""
+    from . import h5lite
+    try:
+        return h5lite.read(path, ["num_boxes_" + dtype])["num_boxes_" + dtype]
+    except h5lite.H5Error:
+        return None
+
+
+def image_regions(path: str, dtype: str) -> Tuple[int, int]:
+    """(P, C) of a region features file's images_<dtype> (numImages, P, C); (0, C) for a grid or fc7 file.  Reads the
+    dataset's header only."""
+    from . import h5lite
+    shape = h5lite.shapes(path, ["images_" + dtype])["images_" + dtype]
+    return (int(shape[1]), int(shape[2])) if len(shape) == 3 else (0, int(shape[1]))
+
+
 class Corpus:
     """One split resident in HBM (vd_corpus handle)."""
 
@@ -101,10 +119,21 @@ class Corpus:
         d.imgNorm = int(opt.get("imgNorm", 1))          # opts.lua:15 default 1; opts.lua:66 (derive_flags) sets 0 for 'att' encoders
         att = "att" in opt.get("encoder", "")                                       # :70
         d.imgAtt = int(att)
+        # region features (DESIGN §26): a 3-D images_<split> (numImages, P, C), stored as given, with optional per-image
+        # counts num_boxes_<split>; the grid's is 4-D (N, C, S, S)
+        region = d.useIm and r["images"].ndim == 3
+        if region:
+            if not att:
+                raise ValueError("region features (a 3-D images dataset) are for the att encoders only, not %s"
+                                 % opt.get("encoder"))
+            d.imgAtt, d.imgNorm = 2, 0
         if d.useIm:
             im = r["images"]
-            d.numImages, d.imgChannels = im.shape[0], im.shape[1]
-            d.imgSpatial = im.shape[2] if att else 0
+            if region:
+                d.numImages, d.imgSpatial, d.imgChannels = im.shape
+            else:
+                d.numImages, d.imgChannels = im.shape[0], im.shape[1]
+                d.imgSpatial = im.shape[2] if att else 0
         d.startToken, d.endToken = start, end
         for field, key in (("ques", "ques"), ("ques_len", "ques_length"), ("ans", "ans"), ("ans_len", "ans_length"),
                            ("cap", "cap"), ("cap_len", "cap_length"), ("opt", "opt"), ("opt_list", "opt_list"),
@@ -118,13 +147,21 @@ class Corpus:
         h = C.c_void_p()
         check(eng.lib.vd_corpus_create(eng.h, C.byref(d), C.byref(h)))
         self.h = h
+        if region and raw.get("num_boxes") is not None:
+            counts = np.ascontiguousarray(raw["num_boxes"], dtype=np.int32).reshape(-1)
+            try:
+                check(eng.lib.vd_corpus_region_counts(h, counts.ctypes.data, len(counts)))
+            except Exception:
+                eng.lib.vd_corpus_destroy(h)
+                raise
         self.numThreads = int(d.numThreads)
         self.R, self.K = int(d.numRounds), int(d.numOptions)
         self.ans_len1 = r["ans_length"].astype(np.int64) + 1                        # :196
         self.num_rounds = r.get("num_rounds")
         if d.useIm:
             im = r["images"]
-            self.img_shape = (im.shape[2], im.shape[3], im.shape[1]) if att else (im.shape[1],)
+            self.img_shape = tuple(im.shape[1:]) if region else (im.shape[2], im.shape[3], im.shape[1]) if att else \
+                (im.shape[1],)
         else:
             self.img_shape = None
         # the host copies of the big arrays are not needed after the upload
@@ -251,6 +288,10 @@ class Dataloader:
                     d["images"] = h5lite.read(opt["inputImg"], ["images_" + dtype])["images_" + dtype]
                 except h5lite.H5Error as e:
                     raise ValueError("no 'images_%s' in %s (%s)" % (dtype, opt["inputImg"], e))
+                if d["images"].ndim == 3:                                           # region features (DESIGN §26)
+                    nb = read_num_boxes(opt["inputImg"], dtype)
+                    if nb is not None:
+                        d["num_boxes"] = nb
             data[dtype] = d
         return self.initialize(dict(opt, vocabSize=n_words + 2), subsets, data, vocab_size_no_specials=n_words)
 

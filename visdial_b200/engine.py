@@ -39,6 +39,7 @@ def to_c_params(params: dict) -> vd_params:
               "imgEmbedSize", "commonEmbeddingSize", "numAttentionLayers", "maxQuesCount", "numOptions", "gpuid"):
         setattr(p, k, int(params.get(k, DEFAULT_PARAMS[k])))
     p.dropout = float(params.get("dropout", 0.5))
+    p.imgRegions = int(params.get("imgRegions", 0))     # 0: the grid; P > 0: region rows (DESIGN §26)
     return p
 
 
@@ -124,9 +125,11 @@ def _ptr(a: Optional[np.ndarray]):
 
 class Batch:
     """Keeps the numpy arrays alive and exposes the vd_batch struct.  Arrays are the dataloader's batch
-    table (SURVEY.md Appendix A): int32 ids, float32 features, C-contiguous."""
+    table (SURVEY.md Appendix A): int32 ids, float32 features, C-contiguous.  Region engines (imgRegions > 0) also take
+    `img_count` (B,), each image's region count (DESIGN §26); without it every region is present."""
 
-    KEYS_I32 = ("ques_fwd", "hist", "options", "answer_ind", "answer_in", "answer_out", "option_in", "option_out")
+    KEYS_I32 = ("ques_fwd", "hist", "options", "answer_ind", "answer_in", "answer_out", "option_in", "option_out",
+                "img_count")
 
     def __init__(self, arrays: Dict[str, np.ndarray]):
         self.arrays = {}

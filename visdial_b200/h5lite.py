@@ -183,6 +183,13 @@ class _Reader:
             out.append((fid, cd))
         return out
 
+    def shape(self, hdr: int) -> Tuple[int, ...]:
+        """a dataset's dimensions from its dataspace message, without reading its data"""
+        msgs = {t: (d, sz) for t, d, sz in self.messages(hdr)}
+        if 0x0001 not in msgs:
+            raise H5Error("object is not a simple dataset")
+        return self._shape(msgs[0x0001][0])
+
     def read(self, hdr: int) -> np.ndarray:
         msgs = {t: (d, sz) for t, d, sz in self.messages(hdr)}
         if 0x0001 not in msgs or 0x0003 not in msgs or 0x0008 not in msgs:
@@ -273,6 +280,28 @@ class _Reader:
                 out[sl] = chunk[tuple(slice(0, s.stop - s.start) for s in sl)]
         walk(btree)
         return out
+
+
+def _open(path: str):
+    with open(path, "rb") as f:
+        try:
+            return mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_READ)
+        except ValueError:                                         # an empty file cannot be mapped
+            raise H5Error("not an HDF5 file (empty)")
+
+
+def shapes(path: str, names: Optional[List[str]] = None) -> Dict[str, Tuple[int, ...]]:
+    """The dimensions of all (or the named) datasets of an HDF5 file, read from their headers only: no dataset is
+    read or decoded.  A named dataset that is not in the file is an H5Error."""
+    with _open(path) as buf:
+        r = _Reader(buf, path)
+        table = r.walk()
+        if names is not None:
+            missing = [n for n in names if n.lstrip("/") not in table]
+            if missing:
+                raise H5Error("datasets not in file: %s" % ", ".join(missing))
+            table = {n.lstrip("/"): table[n.lstrip("/")] for n in names}
+        return {k: r.shape(v) for k, v in table.items()}
 
 
 def read(path: str, names: Optional[List[str]] = None) -> Dict[str, np.ndarray]:

@@ -613,7 +613,7 @@ class DialogPool:
         gt: also the dialogs' own questions (right-aligned into the full width) and answers (corpus rows)."""
         batch = self.dl.getIndexData(np.asarray(inds, dtype=np.int64), self.model.params, self.dtype)
         host = {"ques_fwd": np.zeros((len(inds), self.R, self.width), np.int32)}
-        for k in ("hist", "img_feat"):
+        for k in ("hist", "img_feat", "img_count"):
             if k in batch:
                 host[k] = np.ascontiguousarray(batch[k])
         if gt:

@@ -66,7 +66,10 @@ def make_batch(params: dict, B: int, seed: int = 1234, max_ques_len: int = 20, m
         out["hist"] = _right_align(rows, Th).reshape(B, R, Th)
 
     if "im" in enc:
-        if "att" in enc:                                                   # pool5 NHWC, un-normalised (opts.lua:66)
+        if int(params.get("imgRegions", 0)) > 0:                           # region rows with adaptive counts (DESIGN §26)
+            out["img_feat"], out["img_count"] = region_features(rng, B, int(params["imgRegions"]),
+                                                                int(params["imgFeatureSize"]), adaptive=True)
+        elif "att" in enc:                                                 # pool5 NHWC, un-normalised (opts.lua:66)
             S, Cc = int(params["imgSpatialSize"]), int(params["imgFeatureSize"])
             out["img_feat"] = np.maximum(rng.standard_normal((B, S, S, Cc), dtype=np.float32), 0)
         else:                                                              # fc7, L2-normalised (dataloader.lua:64-68)
@@ -132,14 +135,43 @@ class SyntheticDataloader:
                           gen_eval=params.get("decoder") == "gen")
 
 
+def region_features(rng, n: int, P: int, C: int, adaptive: bool = True, lo: int = 1):
+    """Detector region features as a v1.0 features file holds them: (n, P, C) float32 rows, and with `adaptive` the
+    per-image counts (n,) int32 in [lo, P] (the first image has P regions and, for n >= 2, the second has lo), else None
+    (a fixed P boxes per image).  Rows at or past an image's count hold nonzero junk, as a file's padding may."""
+    feats = (np.maximum(rng.standard_normal((n, P, C), dtype=np.float32), 0) + 0.01).astype(np.float32)
+    if not adaptive:
+        return feats, None
+    counts = rng.integers(lo, P + 1, size=n).astype(np.int32)
+    counts[0] = P
+    if n >= 2:
+        counts[1] = lo
+    pad = np.arange(P)[None, :] >= counts[:, None]
+    feats[pad] = rng.uniform(-3.0, 3.0, size=(int(pad.sum()), C)).astype(np.float32)
+    return feats, counts
+
+
+def write_region_features(path: str, splits: Dict[str, tuple]):
+    """An image features h5 of region features: {split: (images (n, P, C), counts (n,) or None)} as images_<split> and,
+    when counts are given, num_boxes_<split>."""
+    from . import h5lite
+    data = {}
+    for split, (feats, counts) in splits.items():
+        data["images_" + split] = np.ascontiguousarray(feats, dtype=np.float32)
+        if counts is not None:
+            data["num_boxes_" + split] = np.ascontiguousarray(counts, dtype=np.int32)
+    h5lite.write(path, data)
+
+
 def make_corpus(params: dict, num_threads: int = 64, num_opt_list: int = 512, seed: int = 4321, max_ques_len: int = 20,
                 max_ans_len: int = 20, max_cap_len: int = 40, ques_len_cap: int = None, ans_len_cap: int = None,
-                edge_cases: bool = True, num_images: int = None) -> Dict[str, np.ndarray]:
+                edge_cases: bool = True, num_images: int = None, region_adaptive: bool = True) -> Dict[str, np.ndarray]:
     """One split of visdial_data.h5 + data_img.h5 in the layout data/prepro.py:105-183 writes (dataset names without
     the `_<split>` suffix): left-aligned zero-padded token matrices with separate length arrays, 1-based option rows
     into `opt_list`, 1-based `ans_index`, 0-based `img_pos`.  `edge_cases` plants what the reference's loops treat
     specially: an empty question / empty answer round in the middle of a dialog (utils.lua:20-22 `break`), an empty
-    caption, an empty option, and one dialog with every sequence at full length."""
+    caption, an empty option, and one dialog with every sequence at full length.  With params' imgRegions = P > 0 the
+    images are region features (numImages, P, imgFeatureSize) with `num_boxes` (region_features; region_adaptive)."""
     rng = np.random.default_rng(seed)
     V = int(params["vocabSize"])
     R = int(params.get("maxQuesCount", 10))
@@ -183,7 +215,12 @@ def make_corpus(params: dict, num_threads: int = 64, num_opt_list: int = 512, se
         nimg = int(num_images or n)
         out["img_pos"] = rng.permutation(nimg)[:n].astype(np.int32) if nimg >= n else \
             rng.integers(0, nimg, size=n).astype(np.int32)
-        if "att" in enc:                                                          # pool5 as stored: N x C x S x S
+        if int(params.get("imgRegions", 0)) > 0:                                  # region rows N x P x C (DESIGN §26)
+            out["images"], nb = region_features(rng, nimg, int(params["imgRegions"]), int(params["imgFeatureSize"]),
+                                                adaptive=region_adaptive)
+            if nb is not None:
+                out["num_boxes"] = nb
+        elif "att" in enc:                                                        # pool5 as stored: N x C x S x S
             S, Cc = int(params["imgSpatialSize"]), int(params["imgFeatureSize"])
             out["images"] = np.maximum(rng.standard_normal((nimg, Cc, S, S), dtype=np.float32), 0) + 0.01
         else:
