@@ -2,11 +2,10 @@
 
 GEMM primitives (vd_gemm_tn / vd_gemm_atb / vd_gemm_atb16): shapes on both sides of every routing predicate and tile
 edge, strided and offset operands, NaN guard bands around C (padding columns and rows past M must come back untouched,
-and with beta = 0 the NaN inside C must never be read).  The route is asserted, not only the result: a Python mirror of
-the acceptance predicate says "tensor cores" or "CUDA cores", and the error class must agree.  The natural error scale of
-an output element is s = sqrt(sum_k (a_k b_k)^2) (times tanh' after act = 1); TF32 operands (10-bit mantissa) leave a
-normalised rms error rms(err) / rms(s) of about 3e-4, an fp32 contraction about 1e-7, so 1e-5 separates the classes.  The
-bounds of test_tensorcore_gpu.py hold on top: rms <= 1.5e-3 sqrt(K), max <= 8e-3 sqrt(K) for unit-variance operands.
+and with beta = 0 the NaN inside C must never be read).  The route is asserted from the launch counters against the
+Python mirror of the acceptance predicates in tests/gemm_ref.py, and every element of C is held to gemm_ref's bound:
+(n + 3) U (sum_k |a_k b_k| + |bias| + |beta C0|), plus 2^-9 sum_k |a_k b_k| on the tensor cores (fp32 operands meet
+TF32), through tanh' for act = 1 (test_gemm_gpu.py covers the engine's own shapes the same way).
 
 SeqLSTM step hooks (vd_lstm_step_fwd / _bwd): per element against the numpy step of tests/helpers.py, which
 test_oracle_units.py pins to the oracle.  Inputs are O(1) (x-projection and bias ~ N(0, 0.5^2), h in (-1, 1), weights
@@ -22,6 +21,7 @@ import numpy as np
 import pytest
 import torch
 
+import gemm_ref as G
 from helpers import (Buf, _image, _view, lstm_step_bwd_ref, lstm_step_fwd_ref, seg_slices, small_params, torch_batch,
                      torch_params)
 from oracle import philox
@@ -33,10 +33,6 @@ from visdial_b200.synthetic import make_batch
 pytestmark = pytest.mark.gpu
 
 
-def _aligned(off, ld):
-    return off % 4 == 0 and ld % 4 == 0        # cudaMalloc bases are 256-byte aligned: 16 bytes <=> off % 4 == 0
-
-
 def _r4(x):
     return (x + 3) // 4 * 4
 
@@ -45,6 +41,7 @@ def _r4(x):
 def eng():
     e = Engine(small_params("lf-ques", "disc"))
     e.set_math_mode(VD_MATH_TF32)
+    e.profile(True)                       # the GEMM cases read their route from the launch counters
     yield e
     e.close()
 
@@ -54,19 +51,35 @@ def sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-def _check_class(err, scale, K, tc, what):
+GEMM_KERNELS = ("k_tc_gemm", "gemm_tn_simt", "k_tc_atb", "gemm_atb_simt")
+
+
+def _launches(eng):
+    return {n: eng.kernel_stats(n)["launches"] for n in GEMM_KERNELS}
+
+
+def _assert_route(eng, before, want, what):
+    d = {n: v - before[n] for n, v in _launches(eng).items()}
+    assert d == {n: int(n == want) for n in GEMM_KERNELS}, (what, "expected one launch of " + want, d)
+
+
+def _check_class(res, K, what):
+    """res = (err, bound, scale, tc) from _run_tn / _run_atb, which asserted the route: every element within its bound, and
+    the error class of the route.  scale = sqrt(sum_k (a_k b_k)^2) (times tanh' after act = 1): TF32 operands leave a
+    normalised rms error rms(err) / rms(scale) of about 3e-4, an fp32 contraction about 1e-7; for unit-variance operands
+    also rms <= 1.5e-3 sqrt(K), max <= 8e-3 sqrt(K) as in test_tensorcore_gpu.py"""
+    err, bound, scale, tc = res
+    r = float((np.abs(err) / bound).max())
+    assert r <= 1, (what, r)
     rms = float(np.sqrt(np.mean(err ** 2)))
     norm = rms / max(float(np.sqrt(np.mean(scale ** 2))), 1e-30)
     assert rms <= 1.5e-3 * np.sqrt(K) and float(np.abs(err).max()) <= 8e-3 * np.sqrt(K), (what, rms, float(np.abs(err).max()))
-    if tc:
-        assert norm > 1e-5, ("expected the TF32 tensor-core route", what, norm)
-        assert norm < 3e-3, (what, norm)
-    else:
-        assert norm < 1e-5, ("expected the fp32 CUDA-core route", what, norm)
+    assert (1e-5 < norm < 3e-3) if tc else norm < 1e-5, (what, tc, norm)
 
 
 # ---------------------------------------------------------------------------------------------- C = act(beta C + bias + A B^T)
-def _run_tn(eng, M, N, K, beta=0.0, bias=False, act=0, offA=0, lda=None, offB=0, ldb=None, offC=0, ldc=None, seed=0):
+def _run_tn(eng, M, N, K, beta=0.0, bias=False, act=0, offA=0, lda=None, offB=0, ldb=None, offC=0, ldc=None, seed=0,
+            tcmode=True):
     lda = lda or _r4(K)
     ldb = ldb or _r4(K)
     ldc = ldc or _r4(N) + 4
@@ -81,14 +94,19 @@ def _run_tn(eng, M, N, K, beta=0.0, bias=False, act=0, offA=0, lda=None, offB=0,
     if bias:
         bufs.append(Buf(eng, bv))
     dA, dB, dC = bufs[:3]
+    tc = G.tn_takes_tc(tcmode, M, N, K, None, G.aligned(offA, lda), G.aligned(offB, ldb), G.aligned(offC, ldc))
+    before = _launches(eng)
     check(eng.lib.vd_gemm_tn(eng.h, M, N, K, dA.ptr(offA), lda, dB.ptr(offB), ldb, dC.ptr(offC), ldc, beta,
                              bufs[3].ptr() if bias else None, act))
+    _assert_route(eng, before, "k_tc_gemm" if tc else "gemm_tn_simt", (M, N, K))
     out = dC.get()
     for b in bufs:
         b.free()
     A64, B64 = A.astype(np.float64), B.astype(np.float64)
     pre = A64 @ B64.T + (bv[None, :] if bias else 0) + (beta * C0.astype(np.float64) if beta != 0 else 0)
     ref = np.tanh(pre) if act else pre
+    extra = (np.abs(bv)[None, :] if bias else 0) + (abs(beta) * np.abs(C0.astype(np.float64)) if beta != 0 else 0)
+    bound = G.bound(K, np.abs(A64) @ np.abs(B64).T, extra, tc, False, act, ref)
     scale = np.sqrt((A64 ** 2) @ (B64 ** 2).T)
     if act:
         scale = scale * (1 - ref ** 2)
@@ -97,8 +115,7 @@ def _run_tn(eng, M, N, K, beta=0.0, bias=False, act=0, offA=0, lda=None, offB=0,
     guard = out.copy()
     _view(guard, offC, M, N, ldc)[:] = np.nan
     assert np.isnan(guard).all(), "vd_gemm_tn wrote outside C[0:M, 0:N]"
-    tc = M >= 64 and N >= 16 and N % 4 == 0 and K >= 32 and _aligned(offA, lda) and _aligned(offB, ldb) and _aligned(offC, ldc)
-    return got - ref, scale, tc
+    return got - ref, bound, scale, tc
 
 
 TN_M = [63, 64, 65, 127, 128, 129, 257]
@@ -114,15 +131,15 @@ def test_gemm_tn_tile_edges(eng, M):
         i = TN_M.index(M) * len(TN_N) + j
         K = TN_K[i % len(TN_K)]
         beta, bias, act = (0.0, 1.0, 0.5)[i % 3], (i // 3) % 2 == 1, int(i % 5 == 0)
-        err, scale, tc = _run_tn(eng, M, N, K, beta=beta, bias=bias, act=act, seed=i)
-        _check_class(err, scale, K, tc, (M, N, K, beta, bias, act))
+        res = _run_tn(eng, M, N, K, beta=beta, bias=bias, act=act, seed=i)
+        _check_class(res, K, (M, N, K, beta, bias, act))
 
 
 @pytest.mark.parametrize("N", [17, 20, 68, 132])
 def test_gemm_tn_k_edges(eng, N):
     for K in TN_K:
-        err, scale, tc = _run_tn(eng, 129, N, K, beta=0.5, bias=True, seed=K)
-        _check_class(err, scale, K, tc, (129, N, K))
+        res = _run_tn(eng, 129, N, K, beta=0.5, bias=True, seed=K)
+        _check_class(res, K, (129, N, K))
 
 
 # (offA, lda+, offB, ldb+, offC, ldc+): pitches are round_up(K or N, 4) + the extra
@@ -136,23 +153,23 @@ def test_gemm_tn_strided_views(eng, M, N, K, strides):
     """offset / strided operands: 16-byte aligned ones stay on the tensor cores, misaligned ones (offset 1 float or
     ld % 4 != 0) go to the CUDA cores; either way C's padding columns and the rows past M stay untouched"""
     oA, eA, oB, eB, oC, eC = strides
-    err, scale, tc = _run_tn(eng, M, N, K, beta=1.0, bias=True, offA=oA, lda=_r4(K) + eA, offB=oB, ldb=_r4(K) + eB,
-                             offC=oC, ldc=_r4(N) + eC, seed=sum(strides))
-    _check_class(err, scale, K, tc, (M, N, K, strides))
+    res = _run_tn(eng, M, N, K, beta=1.0, bias=True, offA=oA, lda=_r4(K) + eA, offB=oB, ldb=_r4(K) + eB,
+                  offC=oC, ldc=_r4(N) + eC, seed=sum(strides))
+    _check_class(res, K, (M, N, K, strides))
 
 
 def test_gemm_tn_fp32_mode_never_takes_the_tensor_cores(eng):
     eng.set_math_mode(VD_MATH_FP32)
     try:
         for M, N, K in ((128, 128, 64), (257, 65, 300)):
-            err, scale, _ = _run_tn(eng, M, N, K, beta=1.0, bias=True)
-            _check_class(err, scale, K, False, (M, N, K))
+            res = _run_tn(eng, M, N, K, beta=1.0, bias=True, tcmode=False)
+            _check_class(res, K, (M, N, K))
     finally:
         eng.set_math_mode(VD_MATH_TF32)
 
 
 # ---------------------------------------------------------------------------------------------- C += A^T B  (weight gradients)
-def _run_atb(eng, M, N, K, offA=0, lda=None, offB=0, ldb=None, offC=0, ldc=None, seed=0):
+def _run_atb(eng, M, N, K, offA=0, lda=None, offB=0, ldb=None, offC=0, ldc=None, seed=0, sms=132):
     lda = lda or _r4(M)
     ldb = ldb or _r4(N)
     ldc = ldc or _r4(N) + 4
@@ -161,7 +178,10 @@ def _run_atb(eng, M, N, K, offA=0, lda=None, offB=0, ldb=None, offC=0, ldc=None,
     B = rng.standard_normal((K, N)).astype(np.float32)
     C0 = rng.standard_normal((M, N)).astype(np.float32)
     dA, dB, dC = Buf(eng, _image(A, offA, lda)), Buf(eng, _image(B, offB, ldb)), Buf(eng, _image(C0, offC, ldc, rows_extra=3))
+    tc = G.atb_takes_tc(True, M, N, K, None, G.aligned(offA, lda), G.aligned(offB, ldb))
+    before = _launches(eng)
     check(eng.lib.vd_gemm_atb(eng.h, M, N, K, dA.ptr(offA), lda, dB.ptr(offB), ldb, dC.ptr(offC), ldc))
+    _assert_route(eng, before, "k_tc_atb" if tc else "gemm_atb_simt", (M, N, K))
     out = dC.get()
     for b in (dA, dB, dC):
         b.free()
@@ -172,8 +192,9 @@ def _run_atb(eng, M, N, K, offA=0, lda=None, offB=0, ldb=None, offC=0, ldc=None,
     guard = out.copy()
     _view(guard, offC, M, N, ldc)[:] = np.nan
     assert np.isnan(guard).all(), "vd_gemm_atb wrote outside C[0:M, 0:N]"
-    tc = M >= 32 and N >= 32 and K >= 64 and _aligned(offA, lda) and _aligned(offB, ldb)
-    return got - ref, np.sqrt((A64 ** 2).T @ (B64 ** 2)), tc
+    n = G.chain("atb", K, tc, M, N, sms)
+    bound = G.bound(n, np.abs(A64).T @ np.abs(B64), np.abs(C0.astype(np.float64)), tc, False)
+    return got - ref, bound, np.sqrt((A64 ** 2).T @ (B64 ** 2)), tc
 
 
 ATB_MN = [31, 32, 33, 127, 128, 129]
@@ -181,25 +202,25 @@ ATB_K = [63, 64, 65, 255, 256, 257, 1000]
 
 
 @pytest.mark.parametrize("M", ATB_MN)
-def test_gemm_atb_tile_and_split_edges(eng, M):
+def test_gemm_atb_tile_and_split_edges(eng, sms, M):
     """M, N around the 32 threshold and the 128-wide tile, K around the 64 threshold, the 32-row k-block and the
     K / 128 split-K steps (one 128 x 128 tile: the split count is K // 128 up to two waves)"""
     for j, N in enumerate(ATB_MN):
         K = ATB_K[(ATB_MN.index(M) * len(ATB_MN) + j) % len(ATB_K)]
-        err, scale, tc = _run_atb(eng, M, N, K)
-        _check_class(err, scale, K, tc, (M, N, K))
+        res = _run_atb(eng, M, N, K, sms=sms)
+        _check_class(res, K, (M, N, K))
     for K in ATB_K:
-        err, scale, tc = _run_atb(eng, M, 129, K, seed=1)
-        _check_class(err, scale, K, tc, (M, 129, K))
+        res = _run_atb(eng, M, 129, K, seed=1, sms=sms)
+        _check_class(res, K, (M, 129, K))
 
 
 @pytest.mark.parametrize("strides", [(4, 4, 4, 8, 1, 3), (1, 0, 0, 0, 0, 0), (0, 0, 0, 1, 0, 0), (0, 2, 0, 0, 4, 8)])
 @pytest.mark.parametrize("M,N,K", [(129, 65, 257), (33, 128, 64)])
-def test_gemm_atb_strided_views(eng, M, N, K, strides):
+def test_gemm_atb_strided_views(eng, sms, M, N, K, strides):
     """the tensor-core weight gradient needs aligned A and B only: C may sit anywhere (it is reduced with atomics)"""
     oA, eA, oB, eB, oC, eC = strides
-    err, scale, tc = _run_atb(eng, M, N, K, offA=oA, lda=_r4(M) + eA, offB=oB, ldb=_r4(N) + eB, offC=oC, ldc=_r4(N) + eC)
-    _check_class(err, scale, K, tc, (M, N, K, strides))
+    res = _run_atb(eng, M, N, K, offA=oA, lda=_r4(M) + eA, offB=oB, ldb=_r4(N) + eB, offC=oC, ldc=_r4(N) + eC, sms=sms)
+    _check_class(res, K, (M, N, K, strides))
 
 
 @pytest.mark.parametrize("M,N,K,offA,offB,offC,ldc_extra", [(64, 64, 64, 0, 0, 0, 4), (64, 128, 65, 4, 8, 1, 3),

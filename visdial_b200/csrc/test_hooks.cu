@@ -1,5 +1,5 @@
 // vd_test_kernel: the kernels.cuh launchers of pointwise.cu, lstm16.cu's streaming helpers, enc_lstm.cu's persistent
-// encoder LSTM pair and gemm_tc.cu's fused vocabulary projections, called by name on caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory
+// encoder LSTM pair, gemm_tc.cu's fused vocabulary projections and the engine's two dense contractions, called by name on caller-provided DEVICE buffers on the engine's LaunchCtx, so that grid, shared-memory
 // attribute and route are the engine's own; and whole SeqLSTM runs through the engine's own LSTM driver (seq_lstm, seq_lstm_pair).
 // The table below is the whole surface: name, pointer / int / real counts, and the call.
 //   dropout:  p = reals[0], the site an int; the factors are Engine::dropcfg(p)'s (identity unless training == 1).
@@ -32,6 +32,13 @@ struct ArenaRewind {
   Arena& a;
   Arena::Mark m;
   ~ArenaRewind() { a.rewind(m); }
+};
+
+// an SM budget set for one call, restored however the call ends
+struct BudgetRestore {
+  LaunchCtx& cx;
+  int budget;
+  ~BudgetRestore() { cx.sm_budget = budget; }
 };
 
 void copy_out(Engine* e, void* dst, const void* src, size_t bytes) {
@@ -466,6 +473,21 @@ const Entry TABLE[] = {
          VD_CUDA_CHECK(cudaEventDestroy(ev));
          VD_CUDA_CHECK(cudaStreamDestroy(cs[1].stream));
        }
+     }},
+    // ---- the dense contractions as the engine routes them in its current math mode (Engine::gemm_tn / gemm_atb: the
+    // tensor-core kernel where gemm_tn_tc / gemm_atb_tc take the shape, the CUDA-core one otherwise).
+    // ptrs A, gather (or null), B, C, bias (or null); ints M, N, K, lda, ldb, ldc, act; reals beta
+    {"gemm_tn", 5, 7, 1,
+     [](Engine* e, void* const* P, const int64_t* I, const double* X) {
+       e->gemm_tn(IN(0), IN(1), IN(2), CF(0), I[3], CI32(1), CF(2), I[4], F(3), I[5], (float)X[0], CF(4), IN(6));
+     }},
+    // ptrs A, gather (or null), B, C; ints M, N, K, lda, ldb, ldc, SM budget (0: the engine's own, as it stands), which holds
+    // for this call only
+    {"gemm_atb", 4, 7, 0,
+     [](Engine* e, void* const* P, const int64_t* I, const double*) {
+       BudgetRestore br{e->cx, e->cx.sm_budget};
+       if (I[6] > 0) e->cx.sm_budget = IN(6);
+       e->gemm_atb(IN(0), IN(1), I[2], CF(0), I[3], CI32(1), CF(2), I[4], F(3), I[5]);
      }},
     // ---- the fp16 option-LSTM BPTT (lstm16.cu, k_lstm16_bptt) over steps T - 2 .. 0 in waves of clusters.  ptrs da16 (T slices
     // of (R, 4H); slice T - 1 is the input), Whb16 (H, 4H), gates16 (T slices of (R, 4H)), c (T slices of (R, H)), c0 (R, H) or
