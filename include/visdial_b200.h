@@ -157,6 +157,14 @@ int vd_set_lazy_decout(vd_engine* e, int32_t on);
  * value) to the encoder's chains.  on = 0: the reference's order (encoder, then decoder) on one timeline — used by
  * bench.py to time the option-LSTM step kernel alone for the roofline. */
 int vd_set_option_overlap(vd_engine* e, int32_t on, int32_t reserve_sms);
+/* Deterministic training (DESIGN §27).  on = 1: every output of a training step (vd_forward_backward, _dense, _dense_gen and
+ * the fine-grained backward calls: the loss and dW; W, m and v after vd_clamp_adam_step) is a function of the parameters,
+ * math mode, W, optimiser state, batch and dropout seed / iteration only — bit for bit the same on every run, whatever the
+ * GPU's SM count, vd_set_option_overlap's setting or the streams' timing.  The gradient reductions then take routes without
+ * float atomics (partial sums in fixed slots, added in a fixed order), at some cost in speed.  Default 0: the atomic routes.
+ * May be set between steps.  VD_E_BADARG unless on is 0 or 1; VD_E_STATE for on = 1 on an engine with a communicator of
+ * world > 1 (vd_comm_init with world > 1 is likewise refused on a deterministic engine). */
+int vd_set_deterministic(vd_engine* e, int32_t on);
 
 /* ---- fine-grained module protocol (what Model:forwardBackward calls, model.lua:297-337) ----- */
 int vd_encoder_forward(vd_engine* e, const vd_batch* b, const float** encOut_dev);       /* encoder:forward(inputs), :297 */

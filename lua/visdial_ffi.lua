@@ -29,6 +29,7 @@ int vd_get_parameters(vd_engine* e, float* host_dst, int64_t n);
 int vd_zero_grad(vd_engine* e);
 int vd_set_training(vd_engine* e, int32_t training);
 int vd_set_dropout_seed(vd_engine* e, uint64_t seed, uint64_t iteration);
+int vd_set_deterministic(vd_engine* e, int32_t on);   /* 1: training steps repeat bit for bit (DESIGN §27); one GPU */
 int vd_encoder_forward(vd_engine* e, const vd_batch* b, const float** encOut_dev);
 int vd_forward_connect(vd_engine* e);
 int vd_decoder_forward(vd_engine* e, const vd_batch* b, const float** decOut_dev);

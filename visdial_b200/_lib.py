@@ -85,6 +85,7 @@ SIGNATURES = {
     "vd_set_math_mode": [_H, C.c_int32],
     "vd_set_answer_rules": [_H, _P(vd_answer_rules)],
     "vd_set_option_overlap": [_H, C.c_int32, C.c_int32],
+    "vd_set_deterministic": [_H, C.c_int32],
     "vd_encoder_forward": [_H, _P(vd_batch), _P(C.c_void_p)],
     "vd_forward_connect": [_H],
     "vd_decoder_forward": [_H, _P(vd_batch), _P(C.c_void_p)],

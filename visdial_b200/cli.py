@@ -123,6 +123,7 @@ MATH_MODES = ("fp32", "tf32", "f16")
 RUN_OPTIONS = [
     ("gpus", 1, "Number of GPUs (one process each, on gpuid .. gpuid+gpus-1)"),
     ("math", "tf32", "Tensor-core math mode: fp32 (rank-exact evaluation) | tf32 | f16"),
+    ("deterministic", 0, "1: training steps repeat bit for bit (gradient sums in a fixed order, one GPU; DESIGN §27) | 0"),
 ]
 
 SEED = 1234                                                   # torch.manualSeed(1234), train.lua:12 / evaluate.lua:41
@@ -194,6 +195,12 @@ def parse(options, argv=None, prog=None) -> dict:
             del opt["minWords"], opt["noRepeatNgram"], opt["bannedWords"]
     if opt["gpus"] < 1:
         fail("-gpus must be at least 1")
+    if opt["deterministic"] not in (0, 1):
+        fail("-deterministic is 0 or 1")
+    if opt["deterministic"] == 1 and opt["gpus"] != 1:
+        fail("-deterministic 1 runs on one GPU (-gpus 1)")
+    if opt["deterministic"] == 0:               # the default changes nothing: the run's options stay as they were
+        del opt["deterministic"]
     if opt["gpuid"] < 0:
         fail("-gpuid must be >= 0: visdial_b200 has no CPU path")
     return opt
@@ -311,6 +318,8 @@ def build(mp: dict, opt: dict, rank: int, world: int, subsets, ck=None):
     set_image_regions(mp, opt, subsets)
     model = Model(mp, seed=SEED)
     model.engine.set_math_mode({"fp32": VD_MATH_FP32, "tf32": VD_MATH_TF32, "f16": VD_MATH_F16}[opt["math"]])
+    if opt.get("deterministic", 0):
+        model.engine.set_deterministic(True)
     if ck is not None:
         restore(model, ck)
     dl = Dataloader(model.engine, seed=SEED, rank=rank, world=world).initialize_from_files(opt, subsets)

@@ -163,6 +163,15 @@ int vd_set_option_overlap(vd_engine* h, int32_t on, int32_t reserve_sms) {
     }
   })
 }
+int vd_set_deterministic(vd_engine* h, int32_t on) {
+  VD_TRY({
+    Engine* e = ENG(h);
+    VD_REQUIRE(on == 0 || on == 1, VD_E_BADARG, "deterministic must be 0 or 1");
+    VD_REQUIRE(on == 0 || e->world == 1, VD_E_STATE, "deterministic mode runs on one GPU (world 1)");
+    e->join_options_backward();        // a pending option backward finishes on the routes it was issued with
+    e->cx.deterministic = on != 0;
+  })
+}
 int vd_set_math_mode(vd_engine* h, int32_t mode) {
   VD_TRY({
     VD_REQUIRE(mode == VD_MATH_TF32 || mode == VD_MATH_FP32 || mode == VD_MATH_F16, VD_E_BADARG, "unknown math mode");
@@ -527,7 +536,11 @@ int vd_clamp_adam_step(vd_engine* h, float lr) { VD_TRY({ ENG(h)->clamp_adam_ste
 
 int vd_comm_unique_id(void* id_out) { VD_TRY({ NOTNULL(id_out); vd::comm_unique_id(id_out); }) }
 int vd_comm_init(vd_engine* h, const void* id, int32_t rank, int32_t world) {
-  VD_TRY({ VD_REQUIRE(id != nullptr || world == 1, VD_E_BADARG, "id is null"); vd::comm_init(ENG(h), id, rank, world); })
+  VD_TRY({
+    VD_REQUIRE(id != nullptr || world == 1, VD_E_BADARG, "id is null");
+    VD_REQUIRE(world == 1 || !ENG(h)->cx.deterministic, VD_E_STATE, "deterministic mode runs on one GPU (world 1)");
+    vd::comm_init(ENG(h), id, rank, world);
+  })
 }
 int vd_comm_allreduce_grads(vd_engine* h) { VD_TRY({ ENG(h)->allreduce_grads(); }) }
 

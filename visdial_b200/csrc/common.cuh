@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <functional>
 #include <string>
 #include <stdexcept>
 #include <vector>
@@ -189,6 +190,15 @@ struct LaunchCtx {
   int sm_budget = 0;          // > 0: persistent / single-wave kernels size their grids to this many SMs (the rest stay free
                               // for a concurrent higher-priority stream); 0 = all of them
   int sms() const { return sm_budget > 0 ? sm_budget : sm_count; }
+  // deterministic mode (DESIGN §27): the launchers of the gradient reductions take their routes without float atomics, whose
+  // split counts and chunkings follow from the shapes alone; their partial sums live in `scratch` (device memory that stays
+  // valid until the engine's next forward) and are added in a fixed order
+  bool deterministic = false;
+  std::function<void*(size_t)> scratch;
+  template <typename T> T* scratch_get(int64_t n) {
+    VD_REQUIRE(scratch, -3, "deterministic route without a scratch allocator");
+    return static_cast<T*>(scratch((size_t)n * sizeof(T)));
+  }
   std::map<std::string, KStat> stats;
   std::vector<cudaEvent_t> free_events;
 

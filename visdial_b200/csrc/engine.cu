@@ -170,6 +170,7 @@ Engine::Engine(const vd_params* p) {
   VD_CUDA_CHECK(cudaGetDeviceProperties(&prop, cfg.gpuid));
   VD_REQUIRE(prop.major == 9 && prop.minor == 0, VD_E_CUDA, "visdial_b200 is built for sm_90a (H100) only");
   cx.sm_count = prop.multiProcessorCount;
+  cx.scratch = [this](size_t bytes) { return arena.alloc(bytes); };
   // the encoder's chains of small dependent kernels get the highest priority, the option LSTM's SM-filling launches
   // the lowest: a freed SM goes to the latency-bound chain first
   int prio_lo = 0, prio_hi = 0;
@@ -757,7 +758,8 @@ void Engine::lstm_pair_backward(LstmRun& l1, LstmRun& l2, const float* dh_last2,
     cvt_f32_to_f16(cx, B1cat + G, 2 * G, Wp(l1.wseg) + (int64_t)l1.D * G, G, H, G);         // [... | Wh1]
     int* flags = arena.get<int>(enc_pair_bwd_flag_ints(T, R, H));
     float* dh1 = nullptr; float* dh2 = nullptr;
-    if (enc_pair_gate_split(H)) { dh1 = arena.get<float>(TR * H); dh2 = arena.get<float>(TR * H); }
+    // the gate split sums its partial products with float atomics: deterministic mode takes the unit split
+    if (enc_pair_gate_split(H) && !cx.deterministic) { dh1 = arena.get<float>(TR * H); dh2 = arena.get<float>(TR * H); }
     l1.scale2 = l2.scale2 = arena.get<float>(2);       // da16 of both layers = fp16(s da); the weight gradients take 1/s
     {
       LaunchCtx::Scope sc2(&cx, "enc_pair_bwd", 2.0 * T * R * (double)H * 3.0 * G, 4.0 * T * R * (4.0 * G + 4.0 * H));
@@ -1022,6 +1024,7 @@ void Engine::quiesce() {
     VD_CUDA_CHECK(cudaStreamSynchronize(opt_stream));
     opt_fwd_pending = opt_bwd_pending = false;
   }
+  opt_demb = nullptr; opt_dx = nullptr;          // an abandoned step's option gradients are not folded in later
   arena.reset();
   have_fwd = false;
 }
@@ -1203,15 +1206,18 @@ void Engine::encoder_backward(const float* dEnc) {
   }
 
   // question LSTMs (+ gradients handed back by the gen decoder, gen.lua:45-60); the history chain's BPTT runs
-  // concurrently on the side stream (disjoint weight segments; the shared embedding gradient is atomics-only)
+  // concurrently on the side stream (disjoint weight segments; the shared embedding gradient is atomics-only).  Deterministic
+  // mode: the history's embedding gradient is added after the join, behind the question's (its route adds without atomics)
   const bool embdrop = cfg.embdrop;
+  const float* hist_dx = nullptr;
   if (cfg.useHist) {
     if (serial_pairs()) join_side(); else fork_side();
     const PairStreams& hs = serial_pairs() ? main_chain : side_chain;
     float* dx1 = arena.get<float>(N * db.Th * E);
     lstm_pair_backward(hist1, hist2, dh3, nullptr, nullptr, nullptr, dx1, hs);
     reduce_segments(seg("hist.lstm1.weight"), seg("hist.lstm2.weight") + 1, hs.a);              // bucket 2
-    embed_scatter_add(cx, dWp(0), dx1, E, ids_h, N * db.Th, E, embdrop ? d05 : dnone, SITE_HEMBED);
+    if (cx.deterministic) hist_dx = dx1;
+    else embed_scatter_add(cx, dWp(0), dx1, E, ids_h, N * db.Th, E, embdrop ? d05 : dnone, SITE_HEMBED, cfg.V + 1);
     back_to_main();
   }
   {
@@ -1219,7 +1225,7 @@ void Engine::encoder_backward(const float* dEnc) {
     float* dx1 = arena.get<float>(N * db.Tq * D1);
     lstm_pair_backward(ques1, ques2, dq3, conn_dc_l2, conn_dh_l1, conn_dc_l1, dx1, main_chain);
     reduce_segments(seg("ques.lstm1.weight"), seg("ques.lstm2.weight") + 1, main_stream);       // bucket 3
-    embed_scatter_add(cx, dWp(0), dx1, D1, ids_q, N * db.Tq, E, embdrop ? d05 : dnone, SITE_QEMBED);
+    embed_scatter_add(cx, dWp(0), dx1, D1, ids_q, N * db.Tq, E, embdrop ? d05 : dnone, SITE_QEMBED, cfg.V + 1);
     if (cfg.img_in_q) {
       float* die = arena.get<float>(N * cfg.IE);
       masktime_bwd(cx, dx1, D1, E, ids_q, die, db.Tq, N, cfg.IE);
@@ -1227,6 +1233,7 @@ void Engine::encoder_backward(const float* dEnc) {
     }
   }
   join_side();
+  if (hist_dx) embed_scatter_add(cx, dWp(0), hist_dx, E, ids_h, N * db.Th, E, embdrop ? d05 : dnone, SITE_HEMBED, cfg.V + 1);
   // what is left — the option LSTM's weights (final when the option stream ends, i.e. now), the word embedding, which every
   // branch writes, and the small layers not covered above — goes in clamp_adam_step
   // (opt.lstm, final at the same moment, goes out with the embedding in the grouped launch of reduce_remaining)
@@ -1292,13 +1299,14 @@ void Engine::options_forward_async() {
 }
 
 void Engine::join_options_backward() {
-  if (!opt_bwd_pending) return;
-  opt_bwd_pending = false;
+  if (!opt_bwd_pending && !opt_demb && !opt_dx) return;
   cudaStream_t prev = cx.stream;
   cx.stream = main_stream;
-  VD_CUDA_CHECK(cudaStreamWaitEvent(main_stream, ev_opt_done, 0));
+  if (opt_bwd_pending) VD_CUDA_CHECK(cudaStreamWaitEvent(main_stream, ev_opt_done, 0));
+  opt_bwd_pending = false;
   if (opt_demb) add_inplace(cx, dWp(0), opt_demb, (int64_t)(cfg.V + 1) * cfg.E);
-  opt_demb = nullptr;
+  if (opt_dx) embed_scatter_add(cx, dWp(0), opt_dx, cfg.E, ids_o, opt.R * db.To, cfg.E, dropcfg(0.f), 0, cfg.V + 1);
+  opt_demb = nullptr; opt_dx = nullptr;
   cx.stream = prev;
 }
 
@@ -1419,7 +1427,7 @@ void Engine::decoder_backward() {
     lstm_backward(dec2, do2, nullptr, nullptr, dx2, gen_dh0[1], gen_dc0[1]);
     float* dx1 = arena.get<float>(N * db.Ta * E);
     lstm_backward(dec1, dx2, nullptr, nullptr, dx1, gen_dh0[0], gen_dc0[0]);
-    embed_scatter_add(cx, dWp(0), dx1, E, ids_ai, N * db.Ta, E, dropcfg(0.f), 0);
+    embed_scatter_add(cx, dWp(0), dx1, E, ids_ai, N * db.Ta, E, dropcfg(0.f), 0, cfg.V + 1);
   }
 }
 
@@ -1434,15 +1442,18 @@ void Engine::options_backward(const float* dfeat) {
     cx.stream = opt_stream;
     cx.sm_budget = cx.sm_count - opt_reserve_sms;
   }
+  // Deterministic mode: with or without the overlap, the option LSTM's embedding gradient is added to dW(wordEmbed) in
+  // join_options_backward, after the encoder's (its routes add without atomics)
   if (opt.route.table_grad) {
     // embedding gradient in projected space; written to a private (V+1,E) buffer when overlapped, because the
     // encoder's embedding gradients accumulate into dW(wordEmbed) with atomics at the same time
-    opt.demb_out = opt_overlap ? (opt_demb = arena.get<float>((int64_t)(cfg.V + 1) * E)) : nullptr;
+    opt.demb_out = opt_overlap || cx.deterministic ? (opt_demb = arena.get<float>((int64_t)(cfg.V + 1) * E)) : nullptr;
     lstm_backward(opt, nullptr, dfeat, nullptr, nullptr, nullptr, nullptr);
   } else {
     float* dx = arena.get<float>(opt.R * db.To * E);
     lstm_backward(opt, nullptr, dfeat, nullptr, dx, nullptr, nullptr);
-    embed_scatter_add(cx, dWp(0), dx, E, ids_o, opt.R * db.To, E, dropcfg(0.f), 0);   // atomics: safe next to the encoder's
+    if (cx.deterministic) opt_dx = dx;
+    else embed_scatter_add(cx, dWp(0), dx, E, ids_o, opt.R * db.To, E, dropcfg(0.f), 0, cfg.V + 1);   // atomics: safe next to the encoder's
   }
   if (opt_overlap) {
     VD_CUDA_CHECK(cudaEventRecord(ev_opt_done, opt_stream));
@@ -1637,7 +1648,7 @@ float Engine::forward_backward_dense_gen(const vd_batch* b, const int32_t* round
   lstm_backward(l2, dh2, nullptr, nullptr, dx2, dst[1], dst[3]);
   float* dx1 = arena.get<float>(TR * E);
   lstm_backward(l1, dx2, nullptr, nullptr, dx1, dst[0], dst[2]);
-  embed_scatter_add(cx, dWp(0), dx1, E, oi, TR, E, dropcfg(0.f), 0);
+  embed_scatter_add(cx, dWp(0), dx1, E, oi, TR, E, dropcfg(0.f), 0, cfg.V + 1);
   // the K options' initial-state gradients summed per dialog (fixed k order, no atomics), onto the annotated round
   float** gout[4] = {&gen_dh0[0], &gen_dh0[1], &gen_dc0[0], &gen_dc0[1]};
   for (int i = 0; i < 4; ++i) {

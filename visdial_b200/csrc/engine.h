@@ -271,6 +271,7 @@ struct Engine {
   bool opt_overlap = true, opt_fwd_pending = false, opt_bwd_pending = false;
   int opt_reserve_sms = 16;         // SMs the option stream's persistent kernels leave free while they overlap the encoder
   float* opt_demb = nullptr;
+  const float* opt_dx = nullptr;     // deterministic mode: the option LSTM's input gradient, added to dW(wordEmbed) at the join
   void options_forward_async();
   void options_backward(const float* dfeat);   // the option BPTT from d(h_T) (opt.R, H), on opt_stream when overlapped
   void join_options_backward();      // main stream waits for the option BPTT and folds its embedding gradient in

@@ -91,6 +91,8 @@ __global__ void __launch_bounds__(NT) k_gemm_tn(int M, int N, int K, const float
 }
 
 // C[m,n] += sum_k A[row(k), m] * B[k, n];  grid.z splits K.
+// SLOT (deterministic mode): split z stores its partial tile into slot z of C (slots of M x N, ldc = N), for slot_reduce
+template <bool SLOT>
 __global__ void __launch_bounds__(NT) k_gemm_atb(int M, int N, int64_t K, int64_t k_per_split,
                                                  const float* __restrict__ A, int64_t lda,
                                                  const int32_t* __restrict__ a_gather,
@@ -152,7 +154,8 @@ __global__ void __launch_bounds__(NT) k_gemm_atb(int M, int N, int64_t K, int64_
     for (int j = 0; j < TN; ++j) {
       int n = n0 + tx * TN + j;
       if (n >= N) continue;
-      atomicAdd(C + (int64_t)m * ldc + n, acc[i][j]);
+      if constexpr (SLOT) C[(int64_t)blockIdx.z * M * ldc + (int64_t)m * ldc + n] = acc[i][j];
+      else atomicAdd(C + (int64_t)m * ldc + n, acc[i][j]);
     }
   }
 }
@@ -173,11 +176,24 @@ void gemm_atb_simt(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64
   int vec = (M % 4 == 0 && N % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 &&
              ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0)) ? 1 : 0;
   int tiles = cdiv(N, BN) * cdiv(M, BM);
+  if (cx.deterministic) {
+    // the split count from the shape alone (about four waves of a 132-SM H100, at most 32 partial tiles), each split's
+    // partial tile stored in its own slot and the slots added to C in split order
+    int64_t splits = std::max<int64_t>(1, std::min<int64_t>({(528LL + tiles - 1) / tiles, (K + 511) / 512, 32LL}));
+    const int64_t kps = ((K + splits - 1) / splits + BK - 1) / BK * BK;
+    splits = (K + kps - 1) / kps;
+    float* ws = cx.scratch_get<float>(splits * M * N);
+    k_gemm_atb<true><<<dim3(cdiv(N, BN), cdiv(M, BM), (unsigned)splits), NT, 0, cx.stream>>>(M, N, K, kps, A, lda, a_gather, B, ldb,
+                                                                                             ws, N, vec);
+    check_launch(cx, "gemm_atb_simt");
+    slot_reduce(cx, C, ldc, ws, (int)splits, M, N);
+    return;
+  }
   int splits = (int)std::max<int64_t>(1, std::min<int64_t>((4LL * cx.sm_count + tiles - 1) / tiles, (K + 511) / 512));
   int64_t kps = ((K + splits - 1) / splits + BK - 1) / BK * BK;
   splits = (int)((K + kps - 1) / kps);
   dim3 grid(cdiv(N, BN), cdiv(M, BM), splits);
-  k_gemm_atb<<<grid, NT, 0, cx.stream>>>(M, N, K, kps, A, lda, a_gather, B, ldb, C, ldc, vec);
+  k_gemm_atb<false><<<grid, NT, 0, cx.stream>>>(M, N, K, kps, A, lda, a_gather, B, ldb, C, ldc, vec);
   check_launch(cx, "gemm_atb_simt");
 }
 

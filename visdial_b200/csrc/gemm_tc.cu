@@ -513,12 +513,14 @@ k_tc_gemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 // index of the activations in HBM), and wgmma takes tf32 operands K-major only: the two consumer warpgroups load each
 // k-block (32 rows of A and B) from global memory and transpose it into the K-major 128B-swizzled layout while storing
 // it (double-buffered: the next k-block's loads fly while the current one's MMAs run).  One (tile, K-split) per CTA; the
-// fp32 partial sums are reduced into C with red.global.add.
+// fp32 partial sums are reduced into C with red.global.add.  SLOT (deterministic mode): split s stores its partial tile
+// into slot s of C instead (slots of M x N, row pitch ldc = N), for slot_reduce.
 constexpr int ATB_KB = 32;       // k-rows per k-block (4 MMAs)
 constexpr int ATB_BN = 128;
 constexpr int ATB_THREADS = 256;
 constexpr int ATB_OP_BYTES = 128 * ATB_KB * 4;            // one operand tile: 128 rows of 128 B
 constexpr int ATB_SMEM = 2 * 2 * ATB_OP_BYTES + 1024;
+constexpr int ATB_DET_CTAS = 264, ATB_DET_SPLITS = 32;   // deterministic mode's split plan
 struct AtbParams { int M, N; int64_t K, k_per_split; const float* A; int64_t lda; const float* B; int64_t ldb; float* C; int64_t ldc; };
 
 // thread's share of a k-block of one operand: 32 k-rows x 128 columns = 1024 chunks of (4 consecutive k, one column), 4 per
@@ -546,6 +548,7 @@ __device__ __forceinline__ void atb_store(uint8_t* tile, const float4 (&r)[4]) {
   }
 }
 
+template <bool SLOT>
 __global__ void __launch_bounds__(ATB_THREADS, 1)
 k_tc_atb(const AtbParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -590,18 +593,24 @@ k_tc_atb(const AtbParams p) {
     wgmma_hold(d);
     __syncthreads();
   }
-  // fragment -> red.add into C
+  // fragment -> red.add into C (SLOT: stores into the split's slot)
   const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const int r0 = m0 + wg * 64 + 16 * w + (lane >> 2), c0 = n0 + 2 * (lane & 3);
+  float* const C = SLOT ? p.C + (int64_t)blockIdx.y * p.M * p.ldc : p.C;
 #pragma unroll
   for (int j = 0; j < ATB_BN / 8; ++j) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int m = r0 + 8 * h, n = c0 + 8 * j;
       if (m < p.M) {
-        float* crow = p.C + (int64_t)m * p.ldc + n;
-        if (n < p.N) atomicAdd(crow, d[4 * j + 2 * h]);
-        if (n + 1 < p.N) atomicAdd(crow + 1, d[4 * j + 2 * h + 1]);
+        float* crow = C + (int64_t)m * p.ldc + n;
+        if constexpr (SLOT) {
+          if (n < p.N) crow[0] = d[4 * j + 2 * h];
+          if (n + 1 < p.N) crow[1] = d[4 * j + 2 * h + 1];
+        } else {
+          if (n < p.N) atomicAdd(crow, d[4 * j + 2 * h]);
+          if (n + 1 < p.N) atomicAdd(crow + 1, d[4 * j + 2 * h + 1]);
+        }
       }
     }
   }
@@ -705,6 +714,25 @@ bool gemm_atb_tc(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t
   if (M < 32 || N < 32 || K < 64) return false;
   if (!tma_ok(A, lda) || !tma_ok(B, ldb)) return false;
   const int tiles = cdiv(M, BM) * cdiv(N, ATB_BN);
+  static bool attr_set = false;
+  if (!attr_set) {
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_atb<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATB_SMEM));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_atb<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATB_SMEM));
+    attr_set = true;
+  }
+  if (cx.deterministic) {
+    // the split count from the shape alone (about two waves of a 132-SM H100, at most ATB_DET_SPLITS partial tiles), each
+    // split's partial tile stored in its own slot and the slots added to C in split order
+    int64_t splits = std::max<int64_t>(1, std::min<int64_t>({(int64_t)ATB_DET_CTAS / tiles, K / (ATB_KB * 4), (int64_t)ATB_DET_SPLITS}));
+    const int64_t kps = ((K + splits - 1) / splits + ATB_KB - 1) / ATB_KB * ATB_KB;
+    splits = (K + kps - 1) / kps;
+    float* ws = cx.scratch_get<float>(splits * M * N);
+    AtbParams p = {M, N, K, kps, A, lda, B, ldb, ws, N};
+    k_tc_atb<true><<<dim3(tiles, (unsigned)splits), ATB_THREADS, ATB_SMEM, cx.stream>>>(p);
+    check_launch(cx, "k_tc_atb");
+    slot_reduce(cx, C, ldc, ws, (int)splits, M, N);
+    return true;
+  }
   // whole waves: the largest split count with tiles * splits <= 2 * #SM
   // (under an SM budget — the option stream sharing the GPU with the encoder's chains — a single wave of budget CTAs, so
   // that the reserved SMs really stay free: a second wave would be placed on them)
@@ -713,13 +741,8 @@ bool gemm_atb_tc(LaunchCtx& cx, int M, int N, int64_t K, const float* A, int64_t
   int64_t kps = ((K + splits - 1) / splits + ATB_KB - 1) / ATB_KB * ATB_KB;
   splits = (K + kps - 1) / kps;
   AtbParams p = {M, N, K, kps, A, lda, B, ldb, C, ldc};
-  static bool attr_set = false;
-  if (!attr_set) {
-    VD_CUDA_CHECK(cudaFuncSetAttribute(k_tc_atb, cudaFuncAttributeMaxDynamicSharedMemorySize, ATB_SMEM));
-    attr_set = true;
-  }
   dim3 grid(tiles, (unsigned)splits);
-  k_tc_atb<<<grid, ATB_THREADS, ATB_SMEM, cx.stream>>>(p);
+  k_tc_atb<false><<<grid, ATB_THREADS, ATB_SMEM, cx.stream>>>(p);
   check_launch(cx, "k_tc_atb");
   return true;
 }

@@ -53,9 +53,10 @@ void scatter_round_rows(LaunchCtx& cx, const float* src, const int32_t* round, f
 // nn.LookupTableMaskZero forward (+ the nn.Dropout that follows it in mn-att-ques-im-hist.lua:24-25)
 void embed_rows(LaunchCtx& cx, float* out, const float* emb, const int32_t* ids, int64_t rows, int E,
                 DropCfg d, uint32_t site);
-// LookupTable accGradParameters: demb[ids[r],:] += dx[r,0:E] * dropfactor; pad rows privatised per block.
+// LookupTable accGradParameters: demb[ids[r],:] += dx[r,0:E] * dropfactor; pad rows privatised per block.  Deterministic
+// mode: group_rows_by_token's stable sort of the ids (in [0, nv)) and a segmented sum in row order, without atomics.
 void embed_scatter_add(LaunchCtx& cx, float* demb, const float* dx, int64_t ldx, const int32_t* ids,
-                       int64_t rows, int E, DropCfg d, uint32_t site);
+                       int64_t rows, int E, DropCfg d, uint32_t site, int nv);
 
 // ---- SeqLSTM pointwise halves (the GEMM halves are gemm_tn) --------------------------------------
 // gates (R,4H) holds pre-activations without bias on entry, activated [i f o g] on exit.
@@ -246,9 +247,13 @@ void hist_prefill(LaunchCtx& cx, int32_t* hist, int64_t n, int R, int W, const i
 void clamp_adam(LaunchCtx& cx, float* W, float* dW, float* m, float* v, int64_t n, float step, float beta1,
                 float beta2, float eps, float grad_scale);
 void fill_l2_flush(LaunchCtx& cx, float* buf, int64_t n);
+// deterministic mode (DESIGN §27): C[m, n] (row pitch ldc) += the sum over s = 0 .. S-1, in that order, of ws[s][m][n]
+// (S slots of M x N, row pitch N) — the second pass of every reduction whose partial sums the first pass wrote to slots
+void slot_reduce(LaunchCtx& cx, float* C, int64_t ldc, const float* ws, int S, int64_t M, int N);
 // counting sort of rows by token id (perm = row indices grouped by token, sorted_tok = their ids) and the
 // segmented row sum out[tok,:] += sum_{rows with that token} X[row,:]   (LookupTable accGradParameters in
-// projected space: the embedding gradient of the option LSTM without a 640k x 300 x 2048 contraction)
+// projected space: the embedding gradient of the option LSTM without a 640k x 300 x 2048 contraction).
+// Deterministic mode: the sort is stable (a token's rows in index order) and the sum adds each token's rows in that order.
 void group_rows_by_token(LaunchCtx& cx, const int32_t* ids, int64_t n, int nv, int32_t* scratch3nv, int32_t* perm,
                          int32_t* sorted_tok);
 void segsum_rows(LaunchCtx& cx, const float* X, int64_t ldx, const int32_t* perm, const int32_t* sorted_tok, int64_t n,
@@ -298,6 +303,8 @@ void cvt_f32_to_f16(LaunchCtx& cx, __half* dst, int64_t ldd, const float* src, i
 void pick_grad_scale(LaunchCtx& cx, const float* x, int64_t n, uint32_t* bits, float* scale2);
 void segsum_rows16(LaunchCtx& cx, const __half* X, int64_t ldx, const int32_t* perm, const int32_t* sorted_tok, int64_t n,
                    float* out, int ncols, const float* inv_scale);
+void segsum_rows16_det(LaunchCtx& cx, const __half* X, int64_t ldx, const int32_t* perm, const int32_t* sorted_tok, int64_t n,
+                       float* out, int ncols, const float* inv_scale);   // segsum_rows16's deterministic route (pointwise.cu)
 void gemm_atb16(LaunchCtx& cx, int M, int N, int64_t K, const __half* A, int64_t lda, const __half* B, int64_t ldb, float* C,
                 int64_t ldc, const float* inv_scale);
 // persistent two-layer SeqLSTM of the few-row encoder LSTMs (enc_lstm.cu): one launch for both layers and all T steps

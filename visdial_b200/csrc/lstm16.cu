@@ -593,6 +593,9 @@ k_lstm16_bptt(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 // number; the consumers add each finished partial tile into C with red.global.add (C is accumulated with atomics anyway,
 // so no fix-up pass).  A CTA that starts late, behind kernels of other streams, claims fewer chunks.  The last CTA to
 // finish resets the counter, so one zeroed counter per stream serves every launch on it.
+// SLOT (deterministic mode): the chunk plan follows from the shape alone, and a chunk's partial tile is stored into the slot of
+// its k-range (ws: k-ranges x M x N) instead; slot_reduce then adds the slots to C in k-range order, so the sum does not depend
+// on which CTA claimed which chunk.
 constexpr int A16_KB = 64;                 // k-rows per stage (4 MMAs)
 constexpr int A16_BM = 128, A16_BN = 256;
 constexpr int A16_THREADS = 384;
@@ -608,9 +611,11 @@ struct Atb16Params {
   int chunk, num_chunks;                   // k-blocks per chunk, chunks (tiles x k-ranges)
   float* C; int64_t ldc; const float* inv_scale;
   int* counter;                            // [0] next chunk, [1] CTAs done; both zero between launches
+  float* ws;                               // SLOT: the k-range slots
 };
+constexpr int A16_DET_RANGES = 16;         // SLOT: k-ranges (partial tiles per tile) at most
 
-template <bool VEC4>   // C 16-byte aligned with ldc % 4 == 0: the partial tiles go out as red.global.add.v4
+template <bool VEC4, bool SLOT>   // VEC4: C 16-byte aligned with ldc % 4 == 0: the partial tiles go out as red.global.add.v4
 __global__ void __launch_bounds__(A16_THREADS, 1)
 k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Atb16Params p) {
   extern __shared__ uint8_t smem_raw[];
@@ -701,8 +706,11 @@ k_atb16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
           const float r0 = __shfl_xor_sync(0xffffffffu, s0, 1), r1 = __shfl_xor_sync(0xffffffffu, s1, 1);
           const int col = n0 + 8 * j - (odd ? 2 : 0);
           const float4 v = odd ? make_float4(r0 * sc, r1 * sc, k0 * sc, k1 * sc) : make_float4(k0 * sc, k1 * sc, r0 * sc, r1 * sc);
-          if (row < p.M && col < p.N)                  // M, N multiples of 64: a 4-column group is all in or all out
-            red_add_v4(p.C + (int64_t)row * p.ldc + col, v.x, v.y, v.z, v.w);
+          if (row < p.M && col < p.N) {                // M, N multiples of 64: a 4-column group is all in or all out
+            if constexpr (SLOT)
+              *reinterpret_cast<float4*>(p.ws + ((int64_t)(c / p.tiles) * p.M + row) * p.N + col) = v;
+            else red_add_v4(p.C + (int64_t)row * p.ldc + col, v.x, v.y, v.z, v.w);
+          }
         }
       } else {
 #pragma unroll
@@ -1080,6 +1088,7 @@ void segsum_rows16(LaunchCtx& cx, const __half* X, int64_t ldx, const int32_t* p
                    float* out, int ncols, const float* inv_scale) {
   VD_REQUIRE(ncols % 8 == 0 && ldx % 8 == 0, VD_E_STATE, "segsum_rows16: alignment");
   if (n == 0) return;
+  if (cx.deterministic) { segsum_rows16_det(cx, X, ldx, perm, sorted_tok, n, out, ncols, inv_scale); return; }
   tc::k_segsum16<<<(unsigned)((n + tc::SEG16_ROWS - 1) / tc::SEG16_ROWS), 256, 0, cx.stream>>>(X, ldx, perm, sorted_tok, n, out, ncols,
                                                                                                inv_scale);
   check_launch(cx, "k_segsum16");
@@ -1110,7 +1119,13 @@ void gemm_atb16(LaunchCtx& cx, int M, int N, int64_t K, const __half* A, int64_t
   VD_REQUIRE((K + A16_KB - 1) / A16_KB <= INT32_MAX, VD_E_STATE, "gemm_atb16: K");
   p.kbt = (int)((K + A16_KB - 1) / A16_KB);
   const int64_t sms = cx.sms(), total = (int64_t)p.tiles * p.kbt;
-  p.chunk = (int)std::min<int64_t>(p.kbt, std::max<int64_t>(A16_MIN_CHUNK, cdiv(total, sms * A16_CHUNKS_PER_CTA)));
+  if (cx.deterministic) {
+    const int ranges = std::max(1, std::min(A16_DET_RANGES, cdiv(p.kbt, A16_MIN_CHUNK)));
+    p.chunk = cdiv(p.kbt, ranges);
+    p.ws = cx.scratch_get<float>((int64_t)cdiv(p.kbt, p.chunk) * M * N);
+  } else {
+    p.chunk = (int)std::min<int64_t>(p.kbt, std::max<int64_t>(A16_MIN_CHUNK, cdiv(total, sms * A16_CHUNKS_PER_CTA)));
+  }
   p.num_chunks = p.tiles * cdiv(p.kbt, p.chunk);
   p.C = C; p.ldc = ldc; p.inv_scale = inv_scale;
   p.counter = atb16_counter(cx.stream);
@@ -1118,13 +1133,20 @@ void gemm_atb16(LaunchCtx& cx, int M, int N, int64_t K, const __half* A, int64_t
               tB = tmap_h(B, K, N, ldb, A16_KB, 64, CU_TENSOR_MAP_SWIZZLE_128B);
   static bool attr_set = false;
   if (!attr_set) {
-    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
-    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
+    VD_CUDA_CHECK(cudaFuncSetAttribute(k_atb16<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, A16_TOTAL));
     attr_set = true;
   }
   const unsigned grid = (unsigned)std::min<int64_t>(sms, p.num_chunks);
-  if (ldc % 4 == 0 && ((uintptr_t)C & 15) == 0) k_atb16<true><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
-  else k_atb16<false><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
+  if (cx.deterministic) {
+    k_atb16<true, true><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
+    check_launch(cx, "k_atb16");
+    slot_reduce(cx, C, ldc, p.ws, cdiv(p.kbt, p.chunk), M, N);
+    return;
+  }
+  if (ldc % 4 == 0 && ((uintptr_t)C & 15) == 0) k_atb16<true, false><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
+  else k_atb16<false, false><<<grid, A16_THREADS, A16_TOTAL, cx.stream>>>(tA, tB, p);
   check_launch(cx, "k_atb16");
 }
 

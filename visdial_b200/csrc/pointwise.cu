@@ -284,7 +284,9 @@ __global__ void k_vocab_sample_finish(const float* __restrict__ pm, const float*
 // ------------------------------------------------------------------------------------------------
 // out[c] += sum_r X[r, c] (bias gradients).  HBM-bound: a block covers 256 rows x 128 columns, a warp reads whole 512-byte row pieces
 // (float4 per lane) of every 8th row with 4 loads in flight, the 8 warps are combined in shared memory, then one atomicAdd per column.
+// SLOT (deterministic mode): the block's column sums go to its row of out (gridDim.y, cols) instead, for slot_reduce.
 constexpr int CS_ROWS = 256;
+template <bool SLOT>
 __global__ void __launch_bounds__(256) k_colsum_add4(float* __restrict__ out, const float* __restrict__ X, int64_t rows, int cols, int64_t ldx) {
   __shared__ float4 red[8][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -310,17 +312,24 @@ __global__ void __launch_bounds__(256) k_colsum_add4(float* __restrict__ out, co
   if (warp == 0 && c < cols) {
 #pragma unroll
     for (int w = 1; w < 8; ++w) { const float4 o = red[w][lane]; acc.x += o.x; acc.y += o.y; acc.z += o.z; acc.w += o.w; }
-    atomicAdd(out + c, acc.x); atomicAdd(out + c + 1, acc.y); atomicAdd(out + c + 2, acc.z); atomicAdd(out + c + 3, acc.w);
+    if constexpr (SLOT) {
+      float* o = out + (int64_t)blockIdx.y * cols + c;
+      o[0] = acc.x; o[1] = acc.y; o[2] = acc.z; o[3] = acc.w;
+    } else {
+      atomicAdd(out + c, acc.x); atomicAdd(out + c + 1, acc.y); atomicAdd(out + c + 2, acc.z); atomicAdd(out + c + 3, acc.w);
+    }
   }
 }
 // any shape (odd column counts, unaligned leading dimension): one thread per column
+template <bool SLOT>
 __global__ void k_colsum_add(float* __restrict__ out, const float* __restrict__ X, int64_t rows, int cols, int64_t ldx) {
   int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= cols) return;
   int64_t r0 = (int64_t)blockIdx.y * CS_ROWS, r1 = min(rows, r0 + CS_ROWS);
   float acc = 0.f;
   for (int64_t r = r0; r < r1; ++r) acc += X[r * ldx + c];
-  atomicAdd(out + c, acc);
+  if constexpr (SLOT) out[(int64_t)blockIdx.y * cols + c] = acc;
+  else atomicAdd(out + c, acc);
 }
 
 __global__ void k_dropout_apply(float* __restrict__ out, const float* __restrict__ in, int64_t n, DropCfg d, uint32_t site) {
@@ -476,7 +485,9 @@ __global__ void k_rowdot_fwd(float* __restrict__ out, const float* __restrict__ 
   acc = warp_sum(acc);
   if (l == 0) out[r] = acc + b[0];
 }
-// block per 32-row chunk; threads over columns
+// block per 32-row chunk; threads over columns.  SLOT (deterministic mode): the block's dw / db sums go to its row of dw
+// (gridDim.x, H) / its element of db (gridDim.x), for slot_reduce.
+template <bool SLOT>
 __global__ void k_rowdot_bwd(const float* __restrict__ ds, const float* __restrict__ x, const float* __restrict__ w,
                              float* __restrict__ dx, int accumulate_dx, float* __restrict__ dw, float* __restrict__ db,
                              int64_t rows, int H) {
@@ -488,12 +499,14 @@ __global__ void k_rowdot_bwd(const float* __restrict__ ds, const float* __restri
       acc += s * x[r * H + c];
       if (dx) { if (accumulate_dx) dx[r * H + c] += s * wc; else dx[r * H + c] = s * wc; }
     }
-    atomicAdd(dw + c, acc);
+    if constexpr (SLOT) dw[(int64_t)blockIdx.x * H + c] = acc;
+    else atomicAdd(dw + c, acc);
   }
   if (threadIdx.x == 0) {
     float acc = 0.f;
     for (int64_t r = r0; r < r1; ++r) acc += ds[r];
-    atomicAdd(db, acc);
+    if constexpr (SLOT) db[blockIdx.x] = acc;
+    else atomicAdd(db, acc);
   }
 }
 
@@ -899,7 +912,8 @@ __global__ void __launch_bounds__(512) k_san_att_bwd(const float* __restrict__ d
 // grid (N, column slices), block 256: thread = float4 column piece x position group; a block walks ALL P positions of its columns, the
 // position groups are combined in shared memory in a fixed order, so dqc — an intermediate gradient that flows on into the encoder — is
 // written once and deterministically (only the leaf gradients dw, db use atomics).  Recomputes y = tanh(ic + qc) and the dropout factor.
-template <bool MASK>
+// SLOT (deterministic mode): row n's dw / db sums go to row n of dw (N, Cm) / element n of db (N), for slot_reduce.
+template <bool MASK, bool SLOT>
 __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__ ds, const float* __restrict__ ic, const float* __restrict__ qc,
                                                        const float* __restrict__ w, float* __restrict__ dic, float* __restrict__ dqc,
                                                        float* __restrict__ dw, float* __restrict__ db, int P, int Cm, DropCfg d, uint32_t site,
@@ -948,7 +962,8 @@ __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__
         aw.x += ow.x; aw.y += ow.y; aw.z += ow.z; aw.w += ow.w;
       }
       reinterpret_cast<float4*>(dqc)[n * C4 + c4] = aq;
-      atomicAdd(dw + 4 * c4, aw.x); atomicAdd(dw + 4 * c4 + 1, aw.y); atomicAdd(dw + 4 * c4 + 2, aw.z); atomicAdd(dw + 4 * c4 + 3, aw.w);
+      if constexpr (SLOT) reinterpret_cast<float4*>(dw)[n * C4 + c4] = aw;
+      else { atomicAdd(dw + 4 * c4, aw.x); atomicAdd(dw + 4 * c4 + 1, aw.y); atomicAdd(dw + 4 * c4 + 2, aw.z); atomicAdd(dw + 4 * c4 + 3, aw.w); }
     }
     __syncthreads();
   }
@@ -956,7 +971,8 @@ __global__ void __launch_bounds__(256) k_san_score_bwd(const float* __restrict__
   if (blockIdx.y == 0 && threadIdx.x == 0) {
     float acc = 0.f;
     for (int i = 0; i < cn; ++i) acc += sm[i];
-    atomicAdd(db, acc);
+    if constexpr (SLOT) db[n] = acc;
+    else atomicAdd(db, acc);
   }
 }
 
@@ -1815,6 +1831,135 @@ __global__ void __launch_bounds__(256) k_segsum_rows(const float* __restrict__ X
   }
 }
 
+// ---- deterministic mode (DESIGN §27): reductions without float atomics ------------------------------------------------
+// C[m, n] += ws[0][m][n] + ws[1][m][n] + ... + ws[S-1][m][n], summed in slot order (S slots of M x N, row pitch N)
+__global__ void k_slot_reduce(float* __restrict__ C, int64_t ldc, const float* __restrict__ ws, int S, int64_t M, int N) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, MN = M * N;
+  if (i >= MN) return;
+  float acc = ws[i];
+  for (int s = 1; s < S; ++s) acc += ws[(int64_t)s * MN + i];
+  C[(i / N) * ldc + i % N] += acc;
+}
+
+// Stable counting sort of row ids by token: the rows are cut into blocks of TS_ROWS (from n alone), each walked in index order
+// by one warp.  hist[b][v] = rows of block b with token v; after k_tsort_scan it is the rank of block b's first such row among
+// the rows of token v, and total[v] their count.  Ranks inside a warp step come from match.any, so no cursor atomics: row i
+// lands at base[v] + (rows of token v before row i).
+constexpr int TS_ROWS = 2048;
+__global__ void __launch_bounds__(32) k_tsort_hist(const int32_t* __restrict__ ids, int64_t n, int nv, int32_t* __restrict__ hist) {
+  const int lane = threadIdx.x;
+  int32_t* h = hist + (int64_t)blockIdx.x * nv;
+  const int64_t r0 = (int64_t)blockIdx.x * TS_ROWS, r1 = min(n, r0 + TS_ROWS);
+  for (int64_t i0 = r0; i0 < r1; i0 += 32) {
+    const int64_t i = i0 + lane;
+    const int v = i < r1 ? ids[i] : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, v >= 0 ? v : -1 - lane);
+    if (v >= 0 && lane == __ffs(peers) - 1) h[v] += __popc(peers);
+    __syncwarp();
+  }
+}
+__global__ void k_tsort_scan(int32_t* __restrict__ hist, int nblk, int nv, int32_t* __restrict__ total) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= nv) return;
+  int32_t run = 0;
+  for (int b = 0; b < nblk; ++b) { const int32_t c = hist[(int64_t)b * nv + v]; hist[(int64_t)b * nv + v] = run; run += c; }
+  total[v] = run;
+}
+__global__ void __launch_bounds__(32) k_tsort_fill(const int32_t* __restrict__ ids, int64_t n, int nv, int32_t* __restrict__ hist,
+                                                   const int32_t* __restrict__ base, int32_t* __restrict__ perm,
+                                                   int32_t* __restrict__ sorted_tok) {
+  const int lane = threadIdx.x;
+  int32_t* cur = hist + (int64_t)blockIdx.x * nv;
+  const int64_t r0 = (int64_t)blockIdx.x * TS_ROWS, r1 = min(n, r0 + TS_ROWS);
+  const unsigned lt = (1u << lane) - 1u;
+  for (int64_t i0 = r0; i0 < r1; i0 += 32) {
+    const int64_t i = i0 + lane;
+    const int v = i < r1 ? ids[i] : -1;
+    const unsigned peers = __match_any_sync(0xffffffffu, v >= 0 ? v : -1 - lane);
+    const int leader = __ffs(peers) - 1;
+    int c = 0;
+    if (v >= 0 && lane == leader) c = cur[v];
+    c = __shfl_sync(0xffffffffu, c, leader);
+    if (v >= 0) {
+      const int pos = base[v] + c + __popc(peers & lt);
+      perm[pos] = (int32_t)i; sorted_tok[pos] = v;
+      if (lane == leader) cur[v] = c + __popc(peers);
+    }
+    __syncwarp();
+  }
+}
+
+// Segmented row sum without atomics: out[tok, :] += scale * sum of X[perm[p], :] over the positions p of each token, in p order.
+// Pass 1: block b owns positions [b SD_ROWS, (b+1) SD_ROWS) (from n alone).  A token whose positions all lie in the block is
+// added to out by the block; the part of a token that starts in an earlier block goes to head[b], that of a token that starts
+// in the block and goes on into the next one to tail[b].  Pass 2 (k_segsum_det_join): the block where such a token starts
+// adds tail[b] + head[b+1] + ... in block order.  T = float or __half (4 columns per thread); the dropout factor of element
+// (row, c) is drop_factor(d, site, row ncols + c) (an embedding gradient; d.thresh = 0: none).
+constexpr int SD_ROWS = 256;
+__device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
+__device__ __forceinline__ float4 ld4(const __half* p) {
+  const uint2 u = *reinterpret_cast<const uint2*>(p);
+  const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(a.x, a.y, b.x, b.y);
+}
+__device__ __forceinline__ void add_scaled4(float* o, const float4& a, float s) {
+  float4 v = *reinterpret_cast<float4*>(o);
+  v.x += s * a.x; v.y += s * a.y; v.z += s * a.z; v.w += s * a.w;
+  *reinterpret_cast<float4*>(o) = v;
+}
+__device__ __forceinline__ bool sd_cont_prev(const int32_t* tok, int64_t p0) { return p0 > 0 && tok[p0 - 1] == tok[p0]; }
+__device__ __forceinline__ bool sd_cont_next(const int32_t* tok, int64_t p1, int64_t n) { return p1 < n && tok[p1] == tok[p1 - 1]; }
+template <typename T>
+__global__ void __launch_bounds__(256) k_segsum_det(const T* __restrict__ X, int64_t ldx, const int32_t* __restrict__ perm,
+                                                    const int32_t* __restrict__ tok, int64_t n, float* __restrict__ out, int ncols,
+                                                    const float* __restrict__ scale, DropCfg d, uint32_t site,
+                                                    float* __restrict__ head, float* __restrict__ tail) {
+  const int64_t p0 = (int64_t)blockIdx.x * SD_ROWS, p1 = min(n, p0 + SD_ROWS);
+  const bool cprev = sd_cont_prev(tok, p0), cnext = sd_cont_next(tok, p1, n);
+  const float sc = scale ? __ldg(scale) : 1.f;
+  for (int c0 = threadIdx.x * 4; c0 < ncols; c0 += blockDim.x * 4) {
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    int cur = tok[p0];
+    bool first = true;
+    for (int64_t p = p0; p <= p1; ++p) {
+      const int t = p < p1 ? tok[p] : -1;
+      if (t != cur) {                      // the segment of `cur` ends at p (or the block ends)
+        if (first && cprev) *reinterpret_cast<float4*>(head + (int64_t)blockIdx.x * ncols + c0) = acc;
+        else if (p == p1 && cnext) *reinterpret_cast<float4*>(tail + (int64_t)blockIdx.x * ncols + c0) = acc;
+        else add_scaled4(out + (int64_t)cur * ncols + c0, acc, sc);
+        if (p == p1) break;
+        acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        cur = t; first = false;
+      }
+      const int64_t row = perm[p];
+      float4 v = ld4(X + row * ldx + c0);
+      float f[4];
+      drop_factor4(d, site, (uint64_t)(row * ncols + c0) >> 2, f);
+      acc.x += v.x * f[0]; acc.y += v.y * f[1]; acc.z += v.z * f[2]; acc.w += v.w * f[3];
+    }
+  }
+}
+__global__ void __launch_bounds__(256) k_segsum_det_join(const int32_t* __restrict__ tok, int64_t n, float* __restrict__ out, int ncols,
+                                                         const float* __restrict__ scale, const float* __restrict__ head,
+                                                         const float* __restrict__ tail) {
+  const int64_t nblk = (n + SD_ROWS - 1) / SD_ROWS, b = blockIdx.x;
+  const int64_t p0 = b * SD_ROWS, p1 = min(n, p0 + SD_ROWS);
+  // block b holds a tail when its last token goes on and did not come in from the block before as its only token
+  if (!sd_cont_next(tok, p1, n) || (sd_cont_prev(tok, p0) && tok[p0] == tok[p1 - 1])) return;
+  const int t = tok[p1 - 1];
+  const float sc = scale ? __ldg(scale) : 1.f;
+  for (int c0 = threadIdx.x * 4; c0 < ncols; c0 += blockDim.x * 4) {
+    float4 acc = ld4(tail + b * ncols + c0);
+    for (int64_t c = b + 1; c < nblk; ++c) {
+      const float4 h = ld4(head + c * ncols + c0);
+      acc.x += h.x; acc.y += h.y; acc.z += h.z; acc.w += h.w;
+      const int64_t q0 = c * SD_ROWS, q1 = min(n, q0 + SD_ROWS);
+      if (tok[q1 - 1] != t || !sd_cont_next(tok, q1, n)) break;   // the token ends in block c
+    }
+    add_scaled4(out + (int64_t)t * ncols + c0, acc, sc);
+  }
+}
+
 inline int blocks_for(int64_t n, int threads) { return (int)((n + threads - 1) / threads); }
 template <typename F>
 void set_smem(F f, size_t bytes) {
@@ -1829,6 +1974,19 @@ void set_smem(F f, size_t bytes) {
       check_launch(cx, #kern);                                                             \
     }                                                                                      \
   } while (0)
+
+template <typename T>
+static void segsum_det(LaunchCtx& cx, const T* X, int64_t ldx, const int32_t* perm, const int32_t* sorted_tok, int64_t n, float* out,
+                       int ncols, const float* scale, DropCfg d, uint32_t site) {
+  if (n <= 0) return;
+  const int nblk = cdiv(n, SD_ROWS);
+  float* head = cx.scratch_get<float>((int64_t)nblk * ncols);
+  float* tail = cx.scratch_get<float>((int64_t)nblk * ncols);
+  k_segsum_det<T><<<nblk, 256, 0, cx.stream>>>(X, ldx, perm, sorted_tok, n, out, ncols, scale, d, site, head, tail);
+  check_launch(cx, "k_segsum_det");
+  k_segsum_det_join<<<nblk, 256, 0, cx.stream>>>(sorted_tok, n, out, ncols, scale, head, tail);
+  check_launch(cx, "k_segsum_det_join");
+}
 
 void transpose_ids(LaunchCtx& cx, const int32_t* src, int32_t* dst, int64_t rows, int T) {
   L1D(k_transpose_ids, rows * T, src, dst, rows, T);
@@ -1848,9 +2006,18 @@ void embed_rows(LaunchCtx& cx, float* out, const float* emb, const int32_t* ids,
   L1D(k_embed_rows, rows * (E / 4), out, emb, ids, rows, E / 4, d, site);
 }
 void embed_scatter_add(LaunchCtx& cx, float* demb, const float* dx, int64_t ldx, const int32_t* ids, int64_t rows, int E,
-                       DropCfg d, uint32_t site) {
+                       DropCfg d, uint32_t site, int nv) {
   VD_REQUIRE(E <= SC_THREADS * SC_MAXACC, -1, "embedSize too large for embed_scatter_add");
   if (rows <= 0) return;
+  if (cx.deterministic) {
+    VD_REQUIRE(nv > 0 && E % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)dx & 15) == 0, -1, "embed_scatter_add: deterministic route shape");
+    int32_t* s3 = cx.scratch_get<int32_t>(3 * (int64_t)nv);
+    int32_t* perm = cx.scratch_get<int32_t>(rows);
+    int32_t* stok = cx.scratch_get<int32_t>(rows);
+    group_rows_by_token(cx, ids, rows, nv, s3, perm, stok);
+    segsum_det(cx, dx, ldx, perm, stok, rows, demb, E, nullptr, d, site);
+    return;
+  }
   k_embed_scatter_add<<<blocks_for(rows, SC_ROWS), SC_THREADS, 0, cx.stream>>>(demb, dx, ldx, ids, rows, E, d, site);
   check_launch(cx, "embed_scatter_add");
 }
@@ -1872,8 +2039,17 @@ void lstm_pointwise_bwd(LaunchCtx& cx, const float* gates, const float* c_prev, 
 void colsum_add(LaunchCtx& cx, float* out, const float* X, int64_t rows, int cols, int64_t ldx) {
   if (rows <= 0 || cols <= 0) return;
   dim3 grid(cdiv(cols, 128), cdiv(rows, CS_ROWS));
-  if (cols % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)X & 15) == 0) k_colsum_add4<<<grid, 256, 0, cx.stream>>>(out, X, rows, cols, ldx);
-  else k_colsum_add<<<grid, 128, 0, cx.stream>>>(out, X, rows, cols, ldx);
+  const bool vec = cols % 4 == 0 && ldx % 4 == 0 && ((uintptr_t)X & 15) == 0;
+  if (cx.deterministic) {
+    float* ws = cx.scratch_get<float>((int64_t)grid.y * cols);
+    if (vec) k_colsum_add4<true><<<grid, 256, 0, cx.stream>>>(ws, X, rows, cols, ldx);
+    else k_colsum_add<true><<<grid, 128, 0, cx.stream>>>(ws, X, rows, cols, ldx);
+    check_launch(cx, "colsum_add");
+    slot_reduce(cx, out, cols, ws, (int)grid.y, 1, cols);
+    return;
+  }
+  if (vec) k_colsum_add4<false><<<grid, 256, 0, cx.stream>>>(out, X, rows, cols, ldx);
+  else k_colsum_add<false><<<grid, 128, 0, cx.stream>>>(out, X, rows, cols, ldx);
   check_launch(cx, "colsum_add");
 }
 void dropout_apply(LaunchCtx& cx, float* out, const float* in, int64_t n, DropCfg d, uint32_t site) {
@@ -1925,7 +2101,16 @@ void rowdot_fwd(LaunchCtx& cx, float* out, const float* x, const float* w, const
 void rowdot_bwd(LaunchCtx& cx, const float* ds, const float* x, const float* w, float* dx, int accumulate_dx, float* dw,
                 float* db, int64_t rows, int H) {
   if (rows <= 0) return;
-  k_rowdot_bwd<<<blocks_for(rows, 32), 256, 0, cx.stream>>>(ds, x, w, dx, accumulate_dx, dw, db, rows, H);
+  const int nb = blocks_for(rows, 32);
+  if (cx.deterministic) {
+    float* ws = cx.scratch_get<float>((int64_t)nb * (H + 1));
+    k_rowdot_bwd<true><<<nb, 256, 0, cx.stream>>>(ds, x, w, dx, accumulate_dx, ws, ws + (int64_t)nb * H, rows, H);
+    check_launch(cx, "rowdot_bwd");
+    slot_reduce(cx, dw, H, ws, nb, 1, H);
+    slot_reduce(cx, db, 1, ws + (int64_t)nb * H, nb, 1, 1);
+    return;
+  }
+  k_rowdot_bwd<false><<<nb, 256, 0, cx.stream>>>(ds, x, w, dx, accumulate_dx, dw, db, rows, H);
   check_launch(cx, "rowdot_bwd");
 }
 
@@ -2041,7 +2226,17 @@ void san_score_bwd(LaunchCtx& cx, const float* ds, const float* img_common, cons
   VD_REQUIRE(Cm % 4 == 0, -1, "commonEmbeddingSize % 4");
   const int CS = Cm >= 512 ? 4 : 1;                      // column slices per dialog round
   const size_t smem = (size_t)(((P + 3) & ~3) + 2 * 256 * 4) * sizeof(float);
-  auto k = cnt ? k_san_score_bwd<true> : k_san_score_bwd<false>;
+  if (cx.deterministic) {
+    float* ws = cx.scratch_get<float>(N * (Cm + 1));
+    auto k = cnt ? k_san_score_bwd<true, true> : k_san_score_bwd<false, true>;
+    k<<<dim3((unsigned)N, CS), 256, smem, cx.stream>>>(ds, img_common, ques_common, w, d_img_common, d_ques_common, ws, ws + N * Cm, P,
+                                                        Cm, d, site, cnt, R);
+    check_launch(cx, "san_score_bwd");
+    slot_reduce(cx, dw, Cm, ws, (int)N, 1, Cm);
+    slot_reduce(cx, db, 1, ws + N * Cm, (int)N, 1, 1);
+    return;
+  }
+  auto k = cnt ? k_san_score_bwd<true, false> : k_san_score_bwd<false, false>;
   k<<<dim3((unsigned)N, CS), 256, smem, cx.stream>>>(ds, img_common, ques_common, w, d_img_common, d_ques_common, dw, db, P, Cm, d,
                                                       site, cnt, R);
   check_launch(cx, "san_score_bwd");
@@ -2210,6 +2405,20 @@ void group_rows_by_token(LaunchCtx& cx, const int32_t* ids, int64_t n, int nv, i
                          int32_t* sorted_tok) {
   if (n <= 0) return;
   int32_t *counts = scratch3nv, *offsets = scratch3nv + nv, *cursor = scratch3nv + 2 * (int64_t)nv;
+  if (cx.deterministic) {                  // stable: the rows of a token in index order
+    const int nblk = cdiv(n, TS_ROWS);
+    int32_t* hist = cx.scratch_get<int32_t>((int64_t)nblk * nv);
+    VD_CUDA_CHECK(cudaMemsetAsync(hist, 0, (size_t)nblk * nv * sizeof(int32_t), cx.stream));
+    k_tsort_hist<<<nblk, 32, 0, cx.stream>>>(ids, n, nv, hist);
+    check_launch(cx, "k_tsort_hist");
+    k_tsort_scan<<<cdiv(nv, 256), 256, 0, cx.stream>>>(hist, nblk, nv, counts);
+    check_launch(cx, "k_tsort_scan");
+    k_tok_scan<<<1, 1024, 0, cx.stream>>>(counts, offsets, cursor, nv);
+    check_launch(cx, "k_tok_scan");
+    k_tsort_fill<<<nblk, 32, 0, cx.stream>>>(ids, n, nv, hist, offsets, perm, sorted_tok);
+    check_launch(cx, "k_tsort_fill");
+    return;
+  }
   VD_CUDA_CHECK(cudaMemsetAsync(counts, 0, (size_t)nv * sizeof(int32_t), cx.stream));
   L1D(k_tok_hist, n, ids, n, counts);
   k_tok_scan<<<1, 1024, 0, cx.stream>>>(counts, offsets, cursor, nv);
@@ -2220,8 +2429,16 @@ void segsum_rows(LaunchCtx& cx, const float* X, int64_t ldx, const int32_t* perm
                  float* out, int ncols) {
   if (n <= 0) return;
   VD_REQUIRE(ncols % 4 == 0 && ldx % 4 == 0, -1, "segsum_rows: ncols, ldx must be multiples of 4");
+  if (cx.deterministic) { segsum_det(cx, X, ldx, perm, sorted_tok, n, out, ncols, nullptr, DropCfg{}, 0); return; }
   k_segsum_rows<<<blocks_for(n, SEG_ROWS), 256, 0, cx.stream>>>(X, ldx, perm, sorted_tok, n, out, ncols);
   check_launch(cx, "k_segsum_rows");
+}
+void segsum_rows16_det(LaunchCtx& cx, const __half* X, int64_t ldx, const int32_t* perm, const int32_t* sorted_tok, int64_t n,
+                       float* out, int ncols, const float* inv_scale) {
+  segsum_det(cx, X, ldx, perm, sorted_tok, n, out, ncols, inv_scale, DropCfg{}, 0);
+}
+void slot_reduce(LaunchCtx& cx, float* C, int64_t ldc, const float* ws, int S, int64_t M, int N) {
+  L1D(k_slot_reduce, M * N, C, ldc, ws, S, M, N);
 }
 void fill_l2_flush(LaunchCtx& cx, float* buf, int64_t n) {
   k_fill<<<cx.sm_count * 8, 256, 0, cx.stream>>>(buf, n, 0.f);

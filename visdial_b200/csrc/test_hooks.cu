@@ -433,7 +433,7 @@ const Entry TABLE[] = {
      }},
     {"embed_scatter_add", 3, 4, 1,
      [](Engine* e, void* const* P, const int64_t* I, const double* X) {
-       embed_scatter_add(e->cx, F(0), CF(1), I[0], CI32(2), I[1], IN(2), DROP(0), (uint32_t)I[3]);
+       embed_scatter_add(e->cx, F(0), CF(1), I[0], CI32(2), I[1], IN(2), DROP(0), (uint32_t)I[3], e->cfg.V + 1);
      }},
     // ptrs ids, scratch (3 nv int32), perm, sorted_tok; ints n, nv
     {"group_rows_by_token", 4, 2, 0,
@@ -456,7 +456,10 @@ const Entry TABLE[] = {
      [](Engine* e, void* const* P, const int64_t* I, const double*) {
        VD_REQUIRE(I[8] == 1 || I[8] == 2, VD_E_BADARG, "gemm_atb16: streams");
        LaunchCtx cs[2];
-       for (LaunchCtx& c : cs) { c.sm_count = e->cx.sm_count; c.sm_budget = IN(6); c.stream = e->cx.stream; }
+       for (LaunchCtx& c : cs) {
+         c.sm_count = e->cx.sm_count; c.sm_budget = IN(6); c.stream = e->cx.stream;
+         c.deterministic = e->cx.deterministic; c.scratch = e->cx.scratch;
+       }
        cudaEvent_t ev = nullptr;
        if (I[8] == 2) {
          VD_CUDA_CHECK(cudaStreamCreateWithFlags(&cs[1].stream, cudaStreamNonBlocking));
@@ -615,8 +618,10 @@ void test_kernel(Engine* e, const char* name, void* const* ptrs, int n_ptrs, con
     VD_REQUIRE(n_ptrs == t.n_ptrs && n_ints == t.n_ints && n_reals == t.n_reals, VD_E_BADARG, "vd_test_kernel: argument counts");
     VD_REQUIRE((n_ptrs == 0 || ptrs) && (n_ints == 0 || ints) && (n_reals == 0 || reals), VD_E_BADARG,
                "vd_test_kernel: null argument array");
+    const Arena::Mark mk = e->arena.mark();
     t.fn(e, ptrs, ints, reals);
     VD_CUDA_CHECK(cudaStreamSynchronize(e->cx.stream));
+    if (e->cx.deterministic) e->arena.rewind(mk);   // the deterministic routes' partial sums
     return;
   }
   throw CudaError(VD_E_BADARG, std::string("vd_test_kernel: unknown kernel ") + name);

@@ -278,6 +278,12 @@ class Engine:
     def set_option_overlap(self, on: bool, reserve_sms: int = -1):
         check(self.lib.vd_set_option_overlap(self.h, int(on), int(reserve_sms)))
 
+    def set_deterministic(self, on: bool):
+        """Deterministic training (vd_set_deterministic, DESIGN §27): every training step's loss, gradients and Adam update
+        repeat bit for bit for the same parameters, math mode, weights, optimiser state, batch and dropout seed, whatever
+        the GPU's SM count or the option stream's overlap.  Off by default; one GPU only."""
+        check(self.lib.vd_set_deterministic(self.h, 1 if on else 0))
+
     # ---- module protocol -----------------------------------------------------------------------
     def _N(self, batch: Batch) -> int:
         return batch.c.B * self.params["maxQuesCount"]
