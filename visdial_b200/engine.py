@@ -123,6 +123,12 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data
 
 
+def _norms(shape, length_penalty: float, nbest: int) -> Optional[np.ndarray]:
+    """The n-best calls' norm buffer, None at length_penalty = 0 and nbest = 1: there the norms are the scores, and the
+    call (passed NULL) copies none back, as the plain and diverse searches do not."""
+    return None if float(length_penalty) == 0.0 and int(nbest) == 1 else np.zeros(shape, dtype=np.float64)
+
+
 class Batch:
     """Keeps the numpy arrays alive and exposes the vd_batch struct.  Arrays are the dataloader's batch
     table (SURVEY.md Appendix A): int32 ids, float32 features, C-contiguous.  Region engines (imgRegions > 0) also take
@@ -431,7 +437,8 @@ class Engine:
         """n-best lists of a (diverse) beam search for every round of the last encoder forward (vd_gen_nbest_beam_search,
         DESIGN §24): each group's `nbest` best finished hypotheses by norm = score / ((5 + l) / 6)^length_penalty, l = length
         - 1.  Returns (answer (N, G, nbest, L) int32, length (N, G, nbest) int32 — 0 for an entry never filled — score and
-        norm (N, G, nbest) float64), each list best first."""
+        norm (N, G, nbest) float64), each list best first; at length_penalty = 0 and nbest = 1 the norm is the score
+        array."""
         N = self._enc_rows
         if N is None:
             raise _lib.VdError(_lib.VD_E_STATE, "gen_nbest_beam_search before encoder_forward")
@@ -440,11 +447,11 @@ class Engine:
         ans = np.zeros(shape + (int(L),), dtype=np.int32)
         length = np.zeros(shape, dtype=np.int32)
         score = np.zeros(shape, dtype=np.float64)
-        norm = np.zeros(shape, dtype=np.float64)
+        norm = _norms(shape, length_penalty, nb)
         check(self.lib.vd_gen_nbest_beam_search(self.h, int(k), G, float(diversity), float(length_penalty), nb, int(L),
                                                 int(start), int(end), ans.ctypes.data, length.ctypes.data, score.ctypes.data,
-                                                norm.ctypes.data))
-        return ans, length, score, norm
+                                                _ptr(norm)))
+        return ans, length, score, score if norm is None else norm
 
     def gen_sample(self, L: int, start: int, temperature: float, seed: int, row_offset: int = 0):
         """Ancestral sampling for every round of the last encoder forward on the device (vd_gen_sample).  Returns (answer
@@ -517,15 +524,15 @@ class Engine:
         ans = np.zeros(shape + (int(L),), dtype=np.int32)
         length = np.zeros(shape, dtype=np.int32)
         score = np.zeros(shape, dtype=np.float64)
-        norm = np.zeros(shape, dtype=np.float64)
+        norm = _norms(shape, length_penalty, nb)
         hist = np.zeros((B, R, int(hist_width)), dtype=np.int32)
         self._enc_rows = None
         check(self.lib.vd_gen_dialog_nbest_beam_search(self.h, C.byref(batch.c), int(k), G, float(diversity),
                                                        float(length_penalty), nb, int(L), int(start), int(end),
                                                        int(hist_width), int(max_ans_len), ans.ctypes.data, length.ctypes.data,
-                                                       score.ctypes.data, norm.ctypes.data, hist.ctypes.data))
+                                                       score.ctypes.data, _ptr(norm), hist.ctypes.data))
         self._enc_rows = B * R
-        return ans, length, score, norm, hist
+        return ans, length, score, score if norm is None else norm, hist
 
     def gen_dialog_sample(self, batch: Batch, L: int, start: int, end: int, temperature: float, seed: int, row_offset: int,
                           hist_width: int, max_ans_len: int):
@@ -783,13 +790,13 @@ class Engine:
         ans = np.zeros(shape + (int(L),), dtype=np.int32)
         length = np.zeros(shape, dtype=np.int32)
         score = np.zeros(shape, dtype=np.float64)
-        norm = np.zeros(shape, dtype=np.float64)
+        norm = _norms(shape, length_penalty, nb)
         self._enc_rows = None
         check(self.lib.vd_dialog_ask_nbest_slots(self.h, s.ctypes.data, n, q.ctypes.data, int(q.shape[1]), int(k), G,
                                                  float(diversity), float(length_penalty), nb, int(L), int(start), int(end),
-                                                 ans.ctypes.data, length.ctypes.data, score.ctypes.data, norm.ctypes.data))
+                                                 ans.ctypes.data, length.ctypes.data, score.ctypes.data, _ptr(norm)))
         self._dialog_rows = n
-        return ans, length, score, norm
+        return ans, length, score, score if norm is None else norm
 
     def dialog_ask_sample_slots(self, slots, ques, L: int, start: int, end: int, temperature: float, seed: int,
                                 row_offset: int = 0):

@@ -1,10 +1,12 @@
 """Mirror of the reference's `Model` class (/root/reference/model.lua:8-430) over the C engine.
 Same method names, argument meaning and call order as the Lua original, so that the parity tests
 read like the reference's own driver code.  `generateAnswers` (beam search / sampling, model.lua:432-613) runs the beam
-search and the sampling entirely on the device (vd_gen_beam_search, vd_gen_sample)."""
+search and the sampling entirely on the device; `answer_spec` decides, for it, retrieveAnswers and the dialog sessions
+and pools, which engine call answers and with which arguments."""
 from __future__ import annotations
 
 import contextlib
+import dataclasses
 
 import numpy as np
 
@@ -215,7 +217,8 @@ class Model:
     # ---- beam search / sampling (model.lua:432-613, generate.lua) ---------------------------------------------
     def generateAnswers(self, dataloader, dtype="val", params=None, strict=True):
         """Model:generateAnswers.  Beam search (the default) and sampling (`sampleWords = 1`) run entirely on the device
-        through vd_gen_beam_search / vd_gen_sample, for `params.dialogsPerCall` dialogs (default 1) per encoder forward and
+        through vd_gen_nbest_beam_search / vd_gen_truncated_sample (at their neutral arguments vd_gen_beam_search /
+        vd_gen_sample bit for bit; answer_spec), for `params.dialogsPerCall` dialogs (default 1) per encoder forward and
         engine call: every round of those dialogs is searched or sampled at once.  One dialog per call gives exactly the
         per-dialog trimming and kernel shapes of the reference's loop; more dialogs per call run wider kernels (in the
         tensor-core math modes their rounding can differ from per-dialog runs).  The draws of a sampled round depend only on
@@ -226,27 +229,28 @@ class Model:
         model.lua:575).
 
         `history`: "gt" (the default, the reference's behaviour) answers every round with the dataset's history;
-        "generated" runs each dialog on its own answers (vd_gen_dialog_beam_search / vd_gen_dialog_sample, DESIGN §17):
+        "generated" runs each dialog on its own answers (vd_gen_dialog_nbest_beam_search / vd_gen_dialog_truncated_sample,
+        DESIGN §17):
         round r's history holds the answers generated for rounds < r.  Encoders without history have nothing to feed back
         and answer as with "gt".
 
-        `beamGroups` G > 1 (default 1) runs diverse beam search (vd_gen_diverse_beam_search, DESIGN §22): the beamSize
+        `beamGroups` G > 1 (default 1) runs diverse beam search (DESIGN §22): the beamSize
         columns in G groups, each group's candidates penalised by `diversity` (default 0.5) per column of an earlier group
         that chose the same token at that step.  Each round's answer / score / length are then the pick (the best group by
         score, the lower group on ties; what the "generated" history takes), and "groups" lists the G groups' entries
         (None for a group that finished no hypothesis).  `strict` raises only when every group is empty.
 
         `lengthPenalty` alpha (default 0) and `nBest` n (default 1) keep each group's n best finished hypotheses by norm =
-        score / ((5 + l) / 6)^alpha, l = length - 1 (vd_gen_nbest_beam_search / vd_gen_dialog_nbest_beam_search, DESIGN
-        §24).  At the defaults the calls are the ones above.  Otherwise each round's answer / score / length are the pick's
+        score / ((5 + l) / 6)^alpha, l = length - 1 (DESIGN §24).  At the defaults nothing of this changes.  Otherwise
+        each round's answer / score / length are the pick's
         (the best group head by normScore, the lower group on ties), every entry carries "normScore", "groups" (G > 1)
         lists the group heads, and with n > 1 "nbest" lists every finished hypothesis of every group by (normScore desc,
         group asc, list position asc).  Sampling ignores both.
 
         With `sampleWords`, `topK` K (default 0, off) and `topP` P (default 1, off) truncate every draw (DESIGN §23): to the
-        first K classes by (logit desc, class asc), then to the shortest prefix of those holding P of their softmax mass
-        (vd_gen_truncated_sample / vd_gen_dialog_truncated_sample).  When neither truncates (K = 0 or K >= vocabSize, and
-        P = 1) the calls are the untruncated ones.  Beam search ignores both.
+        first K classes by (logit desc, class asc), then to the shortest prefix of those holding P of their softmax mass.
+        When neither truncates (K = 0 or K >= vocabSize, and P = 1) the draws are the untruncated ones.  Beam search
+        ignores both.
 
         `minWords` (default 0), `noRepeatNgram` (default 0, off) and `bannedWords` (a list of words, default none) are the
         answer rules (vd_set_answer_rules, DESIGN §25), in beam search and sampling alike: no answer ends before minWords
@@ -254,120 +258,7 @@ class Model:
         defaults nothing is set.  An unknown banned word raises ValueError."""
         if self.params["decoder"] == "disc":                                            # :434-437
             raise ValueError("Sampling/beam search only for generative model")
-        params = params or {}
-        history = params.get("history", "gt")
-        if history not in HISTORY_MODES:
-            raise ValueError("history is one of %s, not %r" % ("|".join(HISTORY_MODES), history))
-        generated = history == "generated" and bool(self.params.get("useHistory"))
-        if generated:
-            # the width the dataloader sizes history rows for (dataloader.lua:217-225, getIndexData's cut :387-392)
-            maxAnsLen = dataloader.maxAnsLen
-            histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
-                min(dataloader.maxQuesLen + maxAnsLen, dataloader.maxHistoryLen)
-        sampleWords = bool(params.get("sampleWords", 0) == 1)                           # :443
-        temperature, seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
-        beamSize, beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
-        groups, diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
-        diverse = groups > 1 and not sampleWords
-        lengthPenalty, nBest = float(params.get("lengthPenalty", 0.0)), int(params.get("nBest", 1))
-        listed = not sampleWords and (lengthPenalty != 0.0 or nBest != 1)
-        topK, topP = int(params.get("topK", 0)), float(params.get("topP", 1.0))
-        truncated = sampleWords and truncates(topK, topP, self.params["vocabSize"])
-        startToken, endToken = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]   # :453-454
-        rules = answer_rules(params, dataloader.word2ind)
-        numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
-        dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
-        ind2word = getattr(dataloader, "ind2word", None)
-        words = (lambda ids: " ".join(ind2word.get(int(t), "<UNK>") for t in ids if int(t) > 0)) if ind2word else None
-        img = getattr(dataloader, "unique_img_" + dtype, None)
-        # getIndexData hands out this rank's slice of the split: the image list and the sampled rounds' global indices
-        # count from the slice's first dialog
-        offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
-
-        def entry(q, answer, **scored):
-            e = {"question": q.tolist(), "answer": answer.tolist(), **scored}
-            if words:
-                e["question_text"], e["answer_text"] = words(q), words(answer)
-            return e
-
-        answerTable = []
-        ques_len = None
-        for first in range(0, numThreads, dialogsPerCall):
-            inds = np.arange(first, min(numThreads, first + dialogsPerCall))
-            self.wrapper.evaluate()                                                     # :460
-            batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
-            rowOffset = (offset + first) * self.params["maxQuesCount"]
-            with rules_set(self.engine, rules):
-                if generated:
-                    if truncated:
-                        answer, _, _ = self.engine.gen_dialog_truncated_sample(batch, beamLen, startToken, endToken, temperature,
-                                                                               seed, rowOffset, histWidth, maxAnsLen, topK, topP)
-                    elif sampleWords:
-                        answer, _, _ = self.engine.gen_dialog_sample(batch, beamLen, startToken, endToken, temperature, seed,
-                                                                     rowOffset, histWidth, maxAnsLen)
-                    elif listed:
-                        answer, length, score, norm, _ = self.engine.gen_dialog_nbest_beam_search(
-                            batch, beamSize, groups, diversity, lengthPenalty, nBest, beamLen, startToken, endToken, histWidth,
-                            maxAnsLen)
-                    elif diverse:
-                        answer, length, score, _ = self.engine.gen_dialog_diverse_beam_search(
-                            batch, beamSize, groups, diversity, beamLen, startToken, endToken, histWidth, maxAnsLen)
-                    else:
-                        answer, length, score, _ = self.engine.gen_dialog_beam_search(batch, beamSize, beamLen, startToken,
-                                                                                      endToken, histWidth, maxAnsLen)
-                else:
-                    self.forwardBackward(batch, True, True)                                 # :467
-                    if truncated:
-                        answer, _ = self.engine.gen_truncated_sample(beamLen, startToken, temperature, seed, rowOffset, topK, topP)
-                    elif sampleWords:                                                       # :582-594
-                        answer, _ = self.engine.gen_sample(beamLen, startToken, temperature, seed, rowOffset)
-                    elif listed:
-                        answer, length, score, norm = self.engine.gen_nbest_beam_search(beamSize, groups, diversity, lengthPenalty,
-                                                                                        nBest, beamLen, startToken, endToken)
-                    elif diverse:
-                        answer, length, score = self.engine.gen_diverse_beam_search(beamSize, groups, diversity, beamLen,
-                                                                                    startToken, endToken)
-                    else:                                                                   # :472-579
-                        answer, length, score = self.engine.gen_beam_search(beamSize, beamLen, startToken, endToken)
-            R = self.params["maxQuesCount"]
-            if listed:
-                answer, length = answer.reshape(len(inds), R, groups, nBest, -1), length.reshape(len(inds), R, groups, nBest)
-                score, norm = score.reshape(length.shape), norm.reshape(length.shape)
-            elif not sampleWords:
-                length, score = length.reshape(len(inds), R, -1), score.reshape(len(inds), R, -1)
-            ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
-            Tq = ques.shape[2]
-            if not listed:
-                answer = answer.reshape(len(inds), R, -1, answer.shape[-1])
-            self.wrapper.training()                                                     # :605
-            for d, convId in enumerate(inds):
-                w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
-                threadAnswers = []
-                for it in range(ques.shape[1]):
-                    q = ques[d, it, Tq - w:]
-                    if sampleWords:
-                        threadAnswers.append(entry(q, answer[d, it, 0]))
-                        continue
-                    if listed:
-                        e = listed_entry(answer[d, it], length[d, it], score[d, it], norm[d, it],
-                                         lambda a, **sc: entry(q, a, **sc))
-                        if e is None and strict:
-                            raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
-                        threadAnswers.append(e)
-                        continue
-                    gs = [entry(q, answer[d, it, g], score=float(score[d, it, g]), length=int(length[d, it, g]))
-                          if length[d, it, g] > 0 else None for g in range(length.shape[2])]
-                    best = pick_group(length[d, it], score[d, it])
-                    if best >= 0:
-                        threadAnswers.append(dict(gs[best], groups=gs) if diverse else gs[best])
-                    elif strict:
-                        raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
-                    else:
-                        threadAnswers.append(None)
-                gid = offset + int(convId)
-                answerTable.append({"image_id": _image_id(img[gid]) if img is not None else gid,
-                                    "dialog": threadAnswers})                           # :606
-        return answerTable
+        return self._answer_split(dataloader, dtype, params or {}, strict)
 
     def retrieveAnswers(self, dataloader, dtype="val", params=None):
         """What a disc model answers (DESIGN §18): every round of the first `maxThreads` dialogs of split `dtype` answered
@@ -380,55 +271,57 @@ class Model:
         `topK` list of {index, score, answer}; with text when the dataloader carries ind2word."""
         if self.params["decoder"] != "disc":
             raise ValueError("retrieveAnswers answers with the disc decoder; gen models use generateAnswers")
-        params = params or {}
+        return self._answer_split(dataloader, dtype, params or {}, True)
+
+    def _answer_split(self, dataloader, dtype, params, strict):
+        """generateAnswers' and retrieveAnswers' walk over the split: `dialogsPerCall` dialogs per engine call, every round
+        of them answered at once, on the dataset's history or on their own answers"""
         history = params.get("history", "gt")
         if history not in HISTORY_MODES:
             raise ValueError("history is one of %s, not %r" % ("|".join(HISTORY_MODES), history))
         generated = history == "generated" and bool(self.params.get("useHistory"))
-        maxAnsLen = dataloader.maxAnsLen
-        if generated:
-            histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
-                min(dataloader.maxQuesLen + maxAnsLen, dataloader.maxHistoryLen)
-        topK = int(params.get("topK", 1))
-        numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])
+        spec = answer_spec(params, self.params, dataloader, dtype)
+        gen = spec.family != "pool"
+        numThreads = int(params.get("maxThreads") or dataloader.numThreads[dtype])      # :455
         dialogsPerCall = max(1, int(params.get("dialogsPerCall", 1)))
-        pool = dataloader.answerPool(dtype)
-        self.engine.answer_pool_encode(pool)
         ind2word = getattr(dataloader, "ind2word", None)
         words = (lambda ids: " ".join(ind2word.get(int(t), "<UNK>") for t in ids if int(t) > 0)) if ind2word else None
         img = getattr(dataloader, "unique_img_" + dtype, None)
-        offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) else 0
-
-        def answer_of(j):
-            return np.array([t for t in pool[j] if t != 0], dtype=pool.dtype)
-
-        def entry(q, idx, sc):
-            a = answer_of(int(idx[0]))
-            e = {"question": q.tolist(), "answer": a.tolist(), "index": int(idx[0]), "score": float(sc[0]),
-                 "topK": [{"index": int(i), "score": float(v), "answer": answer_of(int(i)).tolist()} for i, v in zip(idx, sc)]}
-            if words:
-                e["question_text"], e["answer_text"] = words(q), words(a)
-            return e
-
+        pool = None if gen else dataloader.answerPool(dtype)
+        if pool is not None:
+            self.engine.answer_pool_encode(pool)
+        R = self.params["maxQuesCount"]
         answerTable = []
         ques_len = None
-        R = self.params["maxQuesCount"]
         for first in range(0, numThreads, dialogsPerCall):
             inds = np.arange(first, min(numThreads, first + dialogsPerCall))
-            batch = dataloader.getIndexData(inds, self.params, dtype)
-            if generated:
-                index, score, _ = self.engine.answer_pool_dialog(batch, topK, histWidth, maxAnsLen)
-            else:
-                index, score = self.engine.answer_pool_retrieve(batch, topK)
-            index, score = index.reshape(len(inds), R, topK), score.reshape(len(inds), R, topK)
-            ques = batch["ques_fwd"]
+            if gen:
+                self.wrapper.evaluate()                                                 # :460
+            batch = dataloader.getIndexData(inds, self.params, dtype)                   # :462-463
+            # the sampled rounds' global indices count from this rank's first dialog of the split
+            rowOffset = (spec.offset + first) * R
+            with rules_set(self.engine, spec.rules):
+                if generated:
+                    out = spec.dialogs(self.engine, batch, rowOffset)
+                else:
+                    if gen:
+                        self.forwardBackward(batch, True, True)                         # :467
+                    out = spec.split(self.engine, batch, rowOffset)
+            if gen:
+                self.wrapper.training()                                                 # :605
+            ques = batch["ques_fwd"]                                                    # (D, maxQuesCount, Tq)
             Tq = ques.shape[2]
             for d, convId in enumerate(inds):
                 w, ques_len = _question_width(dataloader, dtype, inds, convId, Tq, ques_len)
-                gid = offset + int(convId)
+                threadAnswers = []
+                for it in range(ques.shape[1]):
+                    e = spec.entry(out, d * R + it, ques[d, it, Tq - w:].tolist(), words, pool)
+                    if e is None and strict:
+                        raise IndexError("no beam reached <END> within beamLen (model.lua:575 indexes nil here)")
+                    threadAnswers.append(e)
+                gid = spec.offset + int(convId)
                 answerTable.append({"image_id": _image_id(img[gid]) if img is not None else gid,
-                                    "dialog": [entry(ques[d, it, Tq - w:], index[d, it], score[d, it])
-                                               for it in range(ques.shape[1])]})
+                                    "dialog": threadAnswers})                           # :606
         return answerTable
 
     def openDialogs(self, dataloader, dtype="val", inds=(0,), params=None) -> "DialogSession":
@@ -455,6 +348,121 @@ class Model:
         ck = load_checkpoint(path, permutation)
         restore(self, ck, restore_adam_state)
         return ck
+
+
+def answer_spec(params: dict, model_params: dict, dataloader, dtype: str) -> "AnswerSpec":
+    """How `params` answer the questions of a `model_params` model on split `dtype`, for the split (generateAnswers /
+    retrieveAnswers), the dialog loop (their `history = "generated"`) and the slot asks of sessions and pools.  A disc
+    model retrieves its `topK` (default 1) best rows of the split's answer pool and ignores the answer rules; a gen model
+    samples (`sampleWords = 1`) or runs the beam search.  An argument a call would not use takes its neutral value, the
+    one at which the general call is the narrow one bit for bit (DESIGN §22-§24): G = 1 and diversity 0 unless
+    beamGroups > 1 or the search is listed (lengthPenalty != 0 or nBest != 1); topK = 0 and topP = 1 unless they
+    truncate.  Raises ValueError for a banned word the vocabulary does not have."""
+    disc = model_params["decoder"] == "disc"
+    family = "pool" if disc else "sample" if int(params.get("sampleWords", 0)) == 1 else "beam"   # model.lua:443
+    k, G, lam = int(params.get("beamSize", 5)), int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
+    alpha, n = float(params.get("lengthPenalty", 0.0)), int(params.get("nBest", 1))
+    listed = alpha != 0.0 or n != 1
+    if not (G > 1 or listed):
+        G, lam = 1, 0.0
+    topK, topP = int(params.get("topK", 1 if disc else 0)), float(params.get("topP", 1.0))
+    top = (topK, topP) if truncates(topK, topP, model_params["vocabSize"]) else (0, 1.0)
+    histWidth = 0
+    if model_params.get("useHistory"):
+        # the width the dataloader sizes history rows for (dataloader.lua:217-225, getIndexData's cut :387-392)
+        histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
+            min(dataloader.maxQuesLen + dataloader.maxAnsLen, dataloader.maxHistoryLen)
+    return AnswerSpec(
+        family=family, beam=(k, G, lam, alpha if listed else 0.0, n), listed=listed, L=int(params.get("beamLen", 20)),
+        temperature=float(params.get("temperature", 1.0)), seed=int(params.get("seed", 1234)), top=top, pool_k=topK,
+        rules=None if disc else answer_rules(params, dataloader.word2ind),
+        start=dataloader.word2ind["<START>"], end=dataloader.word2ind["<END>"],              # model.lua:453-454
+        histWidth=histWidth, maxAnsLen=dataloader.maxAnsLen,
+        # getIndexData hands out this rank's slice of the split: the image list and the sampled rounds' global indices
+        # count from the slice's first dialog
+        offset=dataloader.part[dtype][0] if dtype in getattr(dataloader, "part", {}) else 0)
+
+
+@dataclasses.dataclass(frozen=True)
+class AnswerSpec:
+    """answer_spec's value, and the one engine call of its family for each scope: the n-best search (beam), the truncated
+    draw (sample) or the pool's retrieval (pool).  A search returns (answer (rows, G, nBest, L), length, score, and norm
+    when listed, else None: the search's norms are its scores), a draw its answer rows (rows, L + 1), a retrieval (index,
+    score) (rows, topK)."""
+    family: str                     # "beam", "sample" or "pool"
+    beam: tuple                     # (beamSize, G, diversity, lengthPenalty, nBest) as the n-best calls take them
+    listed: bool                    # lengthPenalty != 0 or nBest != 1: entries carry normScore
+    L: int                          # beamLen
+    temperature: float
+    seed: int
+    top: tuple                      # (topK, topP) of the truncated draw
+    pool_k: int                     # topK: a pool's list length
+    rules: tuple                    # answer_rules' value; None for none
+    start: int
+    end: int
+    histWidth: int                  # the history rows' width; 0 for encoders without history
+    maxAnsLen: int
+    offset: int                     # this rank's first dialog of the split
+
+    def split(self, eng, batch, rowOffset):
+        """every round of `batch`, after its encoder forward for a gen model"""
+        if self.family == "pool":
+            return eng.answer_pool_retrieve(batch, self.pool_k)
+        if self.family == "sample":
+            return eng.gen_truncated_sample(self.L, self.start, self.temperature, self.seed, rowOffset, *self.top)[0]
+        return self._lists(eng.gen_nbest_beam_search(*self.beam, self.L, self.start, self.end))
+
+    def dialogs(self, eng, batch, rowOffset):
+        """every round of `batch`'s dialogs on their own answers"""
+        if self.family == "pool":
+            return eng.answer_pool_dialog(batch, self.pool_k, self.histWidth, self.maxAnsLen)[:2]
+        if self.family == "sample":
+            return eng.gen_dialog_truncated_sample(batch, self.L, self.start, self.end, self.temperature, self.seed, rowOffset,
+                                                   self.histWidth, self.maxAnsLen, *self.top)[0]
+        return self._lists(eng.gen_dialog_nbest_beam_search(batch, *self.beam, self.L, self.start, self.end, self.histWidth,
+                                                            self.maxAnsLen)[:4])
+
+    def slots(self, eng, slots, q, rowOffset):
+        """the next round of each slot of a session or pool, question rows `q`"""
+        if self.family == "pool":
+            return eng.dialog_ask_pool_slots(slots, q, self.pool_k)
+        if self.family == "sample":
+            return eng.dialog_ask_truncated_slots(slots, q, self.L, self.start, self.end, self.temperature, self.seed,
+                                                  rowOffset, *self.top)[0]
+        return self._lists(eng.dialog_ask_nbest_slots(slots, q, *self.beam, self.L, self.start, self.end))
+
+    def _lists(self, out):
+        answer, length, score, norm = out
+        return answer, length, score, norm if self.listed else None
+
+    def entry(self, out, row: int, question: list, text, pool=None, make=None):
+        """Row `row`'s entry of an engine call's outputs `out`: question token list `question`, question_text /
+        answer_text by `text` (None: no text).  `make(answer, **scores)` builds a search's hypothesis entries (default:
+        the question, the answer and the scores, with their text)."""
+        if self.family == "pool":
+            return pool_entry(question, pool, out[0][row], out[1][row], text)
+        if self.family == "sample":
+            return _entry(question, out[row].tolist(), text)
+        answer, length, score, norm = out
+        return listed_entry(answer[row], length[row], score[row], None if norm is None else norm[row],
+                            make or (lambda a, **sc: _entry(question, a.tolist(), text, **sc)))
+
+
+def _entry(question: list, answer: list, text, **fields) -> dict:
+    """{question, answer, **fields} and, with a text helper, question_text and answer_text"""
+    e = {"question": question, "answer": answer, **fields}
+    if text:
+        e["question_text"], e["answer_text"] = text(question), text(answer)
+    return e
+
+
+def pool_entry(question: list, pool, index, score, text) -> dict:
+    """A retrieved round's entry: the top-1 pool row's non-pad words as the answer, its 0-based `index` and `score`, and
+    the `topK` list of {index, score, answer}"""
+    def answer(j):
+        return [int(t) for t in pool[int(j)] if t != 0]
+    return _entry(question, answer(index[0]), text, index=int(index[0]), score=float(score[0]),
+                  topK=[{"index": int(i), "score": float(v), "answer": answer(i)} for i, v in zip(index, score)])
 
 
 def answer_rules(params: dict, word2ind: dict):
@@ -508,15 +516,18 @@ def ranked_groups(entry) -> list:
 
 
 def listed_entry(answer, length, score, norm, make):
-    """A round's entry from its n-best lists (DESIGN §24): answer (G, n, L), length / score / norm (G, n).  `make(answer,
-    score=, length=, normScore=)` builds one hypothesis' entry.  Returns the pick's entry (the best group head by
-    (normScore desc, group asc)) with "groups" (the G heads, None for a group that finished nothing) when G > 1 and
-    "nbest" (every finished hypothesis by (normScore desc, group asc, list position asc)) when n > 1; None when no group
-    finished a hypothesis."""
+    """A round's entry from its search lists (DESIGN §22, §24): answer (G, n, L), length / score (G, n), and norm (G, n)
+    for n-best lists or None.  `make(answer, score=, length=[, normScore=])` builds one hypothesis' entry, normScore when
+    there are norms.  Returns the pick's entry (the best group head by (norm desc, group asc), the score standing in for
+    the norm without norms) with "groups" (the G heads, None for a group that finished nothing) when G > 1 and "nbest"
+    (every finished hypothesis by (normScore desc, group asc, list position asc)) when n > 1; None when no group finished
+    a hypothesis."""
     G, n = length.shape
-    lists = [[make(answer[g, i], score=float(score[g, i]), length=int(length[g, i]), normScore=float(norm[g, i]))
+    key = score if norm is None else norm
+    lists = [[make(answer[g, i], score=float(score[g, i]), length=int(length[g, i]),
+                   **({} if norm is None else {"normScore": float(norm[g, i])}))
               for i in range(n) if length[g, i] > 0] for g in range(G)]
-    best = pick_group(length[:, 0], norm[:, 0])
+    best = pick_group(length[:, 0], key[:, 0])
     if best < 0:
         return None
     e = dict(lists[best][0])
@@ -577,32 +588,16 @@ class DialogPool:
         self.model, self.dl, self.eng, self.dtype = model, dataloader, model.engine, dtype
         self.R = model.params["maxQuesCount"]
         self.disc = model.params["decoder"] == "disc"
-        self.sampleWords = int(params.get("sampleWords", 0)) == 1
-        self.temperature, self.seed = float(params.get("temperature", 1.0)), int(params.get("seed", 1234))
-        self.beamSize, self.beamLen = int(params.get("beamSize", 5)), int(params.get("beamLen", 20))
-        self.groups, self.diversity = int(params.get("beamGroups", 1)), float(params.get("diversity", 0.5))
-        self.lengthPenalty, self.nBest = float(params.get("lengthPenalty", 0.0)), int(params.get("nBest", 1))
-        # topK: a disc model's retrieval list length (default 1); a gen model's top-k truncation of sampling asks (default
-        # 0, off), with topP (DESIGN §23)
-        self.topK = int(params.get("topK", 1 if self.disc else 0))
-        self.topP = float(params.get("topP", 1.0))
-        self.truncated = not self.disc and self.sampleWords and truncates(self.topK, self.topP, model.params["vocabSize"])
-        # the answer rules (DESIGN §25) of this pool's asks, set around each ask only; a disc pool retrieves without them
-        self.rules = None if self.disc else answer_rules(params, dataloader.word2ind)
-        self.start, self.end = dataloader.word2ind["<START>"], dataloader.word2ind["<END>"]
-        self.width = dataloader.maxQuesLen
-        self.maxAnsLen = dataloader.maxAnsLen
-        self.histWidth = 0
-        if model.params.get("useHistory"):
-            self.histWidth = dataloader.maxHistoryLen if dataloader.concatHistory else \
-                min(dataloader.maxQuesLen + self.maxAnsLen, dataloader.maxHistoryLen)
-        self.offset = dataloader.part[dtype][0] if hasattr(dataloader, "part") and dtype in getattr(dataloader, "part", {}) \
-            else 0
+        # a disc pool's topK is its retrieval list (default 1), a gen pool's the truncation of sampling asks (default 0,
+        # off, with topP); the answer rules (DESIGN §25) are set around each gen ask only
+        self.spec = answer_spec(params, model.params, dataloader, dtype)
+        self.end, self.width = self.spec.end, dataloader.maxQuesLen
+        self.histWidth, self.maxAnsLen, self.offset = self.spec.histWidth, self.spec.maxAnsLen, self.spec.offset
         self.rowOffset = 0                   # sampling: a slot draws as global round draw_base + its round
         self.words = getattr(dataloader, "ind2word", None)
         self.convs = {}                      # slot -> {"ind", "base", "ques": [rows], "ans": [word lists]}
+        self.pool = dataloader.answerPool(dtype) if self.disc else None
         if self.disc:
-            self.pool = dataloader.answerPool(dtype)
             self.eng.answer_pool_encode(self.pool)
         self.capacity = capacity
         if capacity is not None:
@@ -696,57 +691,27 @@ class DialogPool:
     def _ask(self, slots, q) -> list:
         from .utils import idToWords
         text = (lambda ids: idToWords(ids, self.words)) if self.words else None
-        out = []
-        if self.disc:
-            index, score = self.eng.dialog_ask_pool_slots(slots, q, self.topK)
-            given = [history_answer(self.pool[index[b, 0]], self.end) for b in range(len(q))]
-            for b in range(len(q)):
-                a = [int(t) for t in self.pool[index[b, 0]] if t != 0]
-                out.append({"question": [int(t) for t in q[b] if t], "answer": a, "index": int(index[b, 0]),
-                            "score": float(score[b, 0]),
-                            "topK": [{"index": int(i), "score": float(v),
-                                      "answer": [int(t) for t in self.pool[i] if t != 0]} for i, v in zip(index[b], score[b])]})
-        elif self.sampleWords:
-            if self.truncated:
-                with rules_set(self.eng, self.rules):
-                    ans, _ = self.eng.dialog_ask_truncated_slots(slots, q, self.beamLen, self.start, self.end,
-                                                                 self.temperature, self.seed, self.rowOffset, self.topK,
-                                                                 self.topP)
+        spec = self.spec
+        with rules_set(self.eng, spec.rules):
+            got = spec.slots(self.eng, slots, q, self.rowOffset)
+        out, given = [], []
+        for b in range(len(q)):
+            question = [int(t) for t in q[b] if t]
+            # an ask's search hypotheses carry no question: the round's entry has it ahead of a plain pick's answer,
+            # after a diverse pick's scores and after n-best lists
+            e = spec.entry(got, b, question, None, self.pool, make=lambda a, **sc: dict(answer=a.tolist(), **sc))
+            if spec.family == "pool":
+                given.append(history_answer(self.pool[got[0][b, 0]], self.end))
+            elif spec.family == "sample":
+                given.append(history_answer(got[b, 1:], self.end))
             else:
-                with rules_set(self.eng, self.rules):
-                    ans, _ = self.eng.dialog_ask_sample_slots(slots, q, self.beamLen, self.start, self.end, self.temperature,
-                                                              self.seed, self.rowOffset)
-            given = [history_answer(ans[b, 1:], self.end) for b in range(len(q))]
-            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist()} for b in range(len(q))]
-        elif self.lengthPenalty != 0.0 or self.nBest != 1:
-            with rules_set(self.eng, self.rules):
-                ans, length, score, norm = self.eng.dialog_ask_nbest_slots(slots, q, self.beamSize, self.groups,
-                                                                           self.diversity, self.lengthPenalty, self.nBest,
-                                                                           self.beamLen, self.start, self.end)
-            given = []
-            for b in range(len(q)):
-                e = listed_entry(ans[b], length[b], score[b], norm[b],
-                                 lambda a, **sc: dict(answer=a.tolist(), **sc))
                 given.append(history_answer(e["answer"], self.end, e["length"]) if e else [])
-                out.append(dict(e, question=[int(t) for t in q[b] if t]) if e else None)
-        elif self.groups > 1:
-            with rules_set(self.eng, self.rules):
-                ans, length, score = self.eng.dialog_ask_diverse_slots(slots, q, self.beamSize, self.groups, self.diversity,
-                                                                       self.beamLen, self.start, self.end)
-            given = []
-            for b in range(len(q)):
-                gs = [{"answer": ans[b, g].tolist(), "score": float(score[b, g]), "length": int(length[b, g])}
-                      if length[b, g] > 0 else None for g in range(self.groups)]
-                best = pick_group(length[b], score[b])
-                given.append(history_answer(ans[b, best], self.end, length[b, best]) if best >= 0 else [])
-                out.append(dict(gs[best], question=[int(t) for t in q[b] if t], groups=gs) if best >= 0 else None)
-        else:
-            with rules_set(self.eng, self.rules):
-                ans, length, score = self.eng.dialog_ask_beam_slots(slots, q, self.beamSize, self.beamLen, self.start,
-                                                                    self.end)
-            given = [history_answer(ans[b], self.end, length[b]) for b in range(len(q))]
-            out = [{"question": [int(t) for t in q[b] if t], "answer": ans[b].tolist(), "score": float(score[b]),
-                    "length": int(length[b])} if length[b] > 0 else None for b in range(len(q))]
+                if e is not None and spec.listed:
+                    e = dict(e, question=question)
+                elif e is not None:
+                    groups = e.pop("groups", None)
+                    e = {"question": question, **e} if groups is None else dict(e, question=question, groups=groups)
+            out.append(e)
         for s, row, a in zip(slots, q, given):            # the transcript a later resume or reopen replays
             if s in self.convs:
                 self.convs[s]["ques"].append(np.array(row, np.int32))
