@@ -126,7 +126,21 @@ RUN_OPTIONS = [
     ("deterministic", 0, "1: training steps repeat bit for bit (gradient sums in a fixed order, one GPU; DESIGN §27) | 0"),
 ]
 
+# validation while training (DESIGN §28), parsed with train's, finetune's and finetune_gen's tables
+VALIDATION_OPTIONS = [
+    ("valIter", 0, "Rank the val split every valIter epochs, log val_log.json and keep model_best.t7 (0 = never)"),
+    ("valDenseAnnotations", "", "VisDial v1.0 val dense relevance annotations: the validations also compute NDCG, the "
+                                "selection metric (else MRR)"),
+    ("valPatience", 0, "Stop after valPatience validations in a row without a better selection metric (0 = never)"),
+]
+
 SEED = 1234                                                   # torch.manualSeed(1234), train.lua:12 / evaluate.lua:41
+
+
+def usage_error(prog: str, msg: str):
+    """Exit 2 with `msg`, as an argument parser refuses a command line."""
+    print("%s: error: %s (see -h)" % (prog, msg), file=sys.stderr)
+    raise SystemExit(2)
 
 
 def parse(options, argv=None, prog=None) -> dict:
@@ -137,8 +151,7 @@ def parse(options, argv=None, prog=None) -> dict:
     prog = prog or os.path.basename(sys.argv[0])
 
     def fail(msg):
-        print("%s: error: %s (see -h)" % (prog, msg), file=sys.stderr)
-        raise SystemExit(2)
+        usage_error(prog, msg)
 
     args = list(sys.argv[1:] if argv is None else argv)
     opt = dict(defaults)
@@ -193,6 +206,16 @@ def parse(options, argv=None, prog=None) -> dict:
             fail("-minWords and -noRepeatNgram must be >= 0")
         if not answer_rules_active(opt):        # options that change nothing leave the run's options as they were
             del opt["minWords"], opt["noRepeatNgram"], opt["bannedWords"]
+    if "valIter" in opt:
+        if opt["valIter"] < 0 or opt["valPatience"] < 0:
+            fail("-valIter and -valPatience must be >= 0")
+        if opt["valIter"] == 0 and opt["valPatience"] > 0:
+            fail("-valPatience needs -valIter")
+        if opt["valIter"] == 0 and opt["valDenseAnnotations"]:
+            fail("-valDenseAnnotations needs -valIter")
+        for n, d, _ in VALIDATION_OPTIONS:      # the defaults change nothing: the run's options stay as they were
+            if opt[n] == d:
+                del opt[n]
     if opt["gpus"] < 1:
         fail("-gpus must be at least 1")
     if opt["deterministic"] not in (0, 1):
@@ -207,8 +230,9 @@ def parse(options, argv=None, prog=None) -> dict:
 
 
 def train_opts(argv=None, now=None, options=TRAIN_OPTIONS, prog="python -m visdial_b200.train") -> dict:
-    """opts.lua:42-67: parsed options, the time-stamped default savePath and the flags derived from the encoder name."""
-    opt = parse(options, argv, prog)
+    """opts.lua:42-67: parsed options, the time-stamped default savePath and the flags derived from the encoder name.
+    `options` are parsed with VALIDATION_OPTIONS; a validating run's files are checked here (validation_data_problem)."""
+    opt = parse(options + VALIDATION_OPTIONS, argv, prog)
     if opt["savePath"] == "checkpoints/":                                           # :44-52
         t = now or time.localtime()
         opt["savePath"] = "checkpoints/model-%d-%d-%d-%d:%d:%d-%s-%s/" % (
@@ -216,7 +240,41 @@ def train_opts(argv=None, now=None, options=TRAIN_OPTIONS, prog="python -m visdi
     derive_flags(opt)                                                               # :55-59,66
     if "att" in opt["encoder"] and opt["inputImg"] == "data/data_img.h5":           # :62-65 (conv features)
         opt["inputImg"] = "data/data_img_pool5.h5"
+    if opt.get("valIter"):
+        problem = validation_data_problem(opt)
+        if problem:
+            usage_error(prog, problem)
     return opt
+
+
+def validation_data_problem(opt: dict):
+    """Why -valIter cannot run on opt's files, or None: the question file needs the val split, the json its
+    unique_img_val, and a -valDenseAnnotations file must read against them (visdial_b200.dense.read).  Host reads only (the
+    h5 headers, num_rounds_val, the json), so that a bad file is refused before any GPU work."""
+    from . import dense, h5lite
+    try:
+        shapes = h5lite.shapes(opt["inputQues"])
+    except (OSError, h5lite.H5Error) as e:
+        return "-valIter: cannot read %s (%s)" % (opt["inputQues"], e)
+    if "opt_val" not in shapes or "ans_index_val" not in shapes:
+        return "-valIter: %s has no val split (opt_val, ans_index_val)" % opt["inputQues"]
+    try:
+        with open(opt["inputJson"]) as f:
+            unique_img = json.load(f).get("unique_img_val")
+    except (OSError, ValueError) as e:
+        return "-valIter: cannot read %s (%s)" % (opt["inputJson"], e)
+    if unique_img is None or len(unique_img) != shapes["opt_val"][0]:
+        return "-valIter: %s needs unique_img_val, one entry per val dialog of %s" % (opt["inputJson"], opt["inputQues"])
+    if not opt.get("valDenseAnnotations"):
+        return None
+    num_rounds = h5lite.read(opt["inputQues"], ["num_rounds_val"])["num_rounds_val"] if "num_rounds_val" in shapes else None
+    try:
+        ann = dense.read(opt["valDenseAnnotations"], int(shapes["opt_val"][2]), unique_img=unique_img, num_rounds=num_rounds)
+    except (OSError, ValueError) as e:
+        return "-valDenseAnnotations: %s" % (e.args[0] if e.args else e)
+    if len(ann) == 0:
+        return "-valDenseAnnotations: %s has no usable annotated round" % opt["valDenseAnnotations"]
+    return None
 
 
 def truncated_sampling(opt: dict) -> bool:
@@ -257,8 +315,8 @@ def written_opts(opt: dict) -> dict:
 
 
 def model_params(opt: dict) -> dict:
-    """`modelParams = opt` (train.lua:27) without the options that only say how the run is launched."""
-    run_only = {n for n, _, _ in RUN_OPTIONS}
+    """`modelParams = opt` (train.lua:27) without the options that only say how the run is launched or validated."""
+    run_only = {n for n, _, _ in RUN_OPTIONS + VALIDATION_OPTIONS}
     return {k: v for k, v in opt.items() if k not in run_only}
 
 

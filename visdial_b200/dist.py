@@ -57,6 +57,14 @@ def gather_objects(local: list, world: int) -> list:
     return [x for part in objs for x in part]
 
 
+def broadcast_object(obj, rank: int):
+    """Rank 0's `obj` on every rank (a decision rank 0 took, such as ending training early)."""
+    import torch.distributed as dist
+    box = [obj if rank == 0 else None]
+    dist.broadcast_object_list(box, src=0)
+    return box[0]
+
+
 def mean_over_ranks(value: float, world: int) -> float:
     import torch
     import torch.distributed as dist

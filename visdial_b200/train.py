@@ -7,7 +7,11 @@ checkpoint's weights and learning rate with fresh Adam moments, as train.lua:78-
 
 `-gpus N` trains data-parallel on GPUs gpuid .. gpuid+N-1: each rank draws its own `batchSize` dialogs per iteration, the
 gradients are all-reduced inside the engine's Adam step (NCCL), an epoch is ceil(numTrainThreads / (N * batchSize))
-iterations, the printed loss is the mean of the ranks' running losses, and only rank 0 writes files."""
+iterations, the printed loss is the mean of the ranks' running losses, and only rank 0 writes files.
+
+`-valIter N` also ranks the val split every N epochs (visdial_b200.validation, DESIGN §28): `<savePath>/val_log.json`, a
+`[Val]` line, `<savePath>/model_best.t7` at each strict improvement of the selection metric, and with `-valPatience P` an
+early stop after P validations without one (model_final.t7 is written as at the normal end)."""
 from __future__ import annotations
 
 import hashlib
@@ -37,20 +41,30 @@ def main(opt: dict, rank: int = 0, world: int = 1, iteration=standard_iteration)
     else:
         mp = cli.model_params(opt)                                                  # :27
     mp["vocabSize"] = cli.vocab_size(opt)                                           # :55-59 (the dataloader's count)
-    model, dl = cli.build(mp, opt, rank, world, ["train"], ck)                      # :47-48,76-81
+    validating = opt.get("valIter", 0) > 0                                          # the val split is read for it only
+    model, dl = cli.build(mp, opt, rank, world, ["train", "val"] if validating else ["train"], ck)   # :47-48,76-81
     vdist.attach_engine(model.engine, rank, world)
     p = model.params
-    p.update({k: getattr(dl, k) for k in ("numTrainThreads", "numTestThreads", "numValThreads", "vocabSize",
+    # (numValThreads is not recorded: the val split is loaded only to validate, and the checkpoints' modelParams are
+    # those of a run without it)
+    p.update({k: getattr(dl, k) for k in ("numTrainThreads", "numTestThreads", "vocabSize",
                                           "maxQuesCount", "maxQuesLen", "maxAnsLen") if hasattr(dl, k)})
+    if validating:                              # the dataloader's widths are its last split's: record the train split's
+        p.update(maxQuesLen=int(dl.corpus["train"].desc.maxQuesLen), maxAnsLen=int(dl.corpus["train"].desc.maxAnsLen))
     p["gpuid"] = opt["gpuid"]
     savePath = opt["savePath"]                                                      # :62-65
     if rank == 0:
         os.makedirs(savePath, exist_ok=True)
     step, epoch_items = iteration(model, dl, opt, say)
+    validate = None
+    if validating:
+        from .validation import Validator
+        validate = Validator(model, dl, opt, rank, world, say)
     numIterPerEpoch = p["numIterPerEpoch"] = math.ceil(epoch_items / (world * p["batchSize"]))   # :68-69
     say("\n%d iter per epoch." % numIterPerEpoch)
     say("Training..")
     saveEvery = int(p["saveIter"]) * numIterPerEpoch
+    valEvery = int(opt.get("valIter", 0)) * numIterPerEpoch
     for it in range(1, int(p["numEpochs"]) * numIterPerEpoch + 1):                  # :90-117
         step()
         if saveEvery > 0 and it % saveEvery == 0 and rank == 0:
@@ -59,6 +73,10 @@ def main(opt: dict, rank: int = 0, world: int = 1, iteration=standard_iteration)
             loss = vdist.mean_over_ranks(model.runningLoss, world) if world > 1 else model.runningLoss
             say("[%s][Epoch:%.02f][Iter:%d][Loss:%.05f][lr:%f]" % (time.strftime("%c"), it / numIterPerEpoch, it, loss,
                                                                    model.optims["learningRate"]))
+        if valEvery > 0 and it % valEvery == 0 and validate(it, it // numIterPerEpoch):
+            break
+    if validate is not None:
+        validate.report_best()
     if world > 1:
         # every rank applied the same all-reduced gradient: a rank whose weights differ from rank 0's would mean that the
         # final checkpoint does not describe what was trained, so it is not written
