@@ -593,6 +593,11 @@ typedef struct vd_corpus_desc {
 
 /* dataloader:initialize tensors -> HBM + dataloader:prepareDataset on the device.  Host pointers. */
 int vd_corpus_create(vd_engine* e, const vd_corpus_desc* d, vd_corpus** out);
+/* vd_corpus_create with a limit: imgDeviceBytes is the most prepared image feature bytes (numImages x row x 4) the corpus
+ * keeps on the device, 0 = no limit (vd_corpus_create).  A split over it keeps them in one pinned host allocation
+ * (DESIGN §29), and each batch's rows are copied to the device by the copy engines; the batches are bit for bit the same.
+ * VD_E_OOM when the pinned allocation fails. */
+int vd_corpus_create_limited(vd_engine* e, const vd_corpus_desc* d, int64_t imgDeviceBytes, vd_corpus** out);
 int vd_corpus_destroy(vd_corpus* c);
 /* Assemble the batch of dialogs `inds` (HOST array of n 0-based dialog indices = Lua's inds - 1) on the engine's stream.
  *   decoder_gen = 0: getIndexData + getIndexOption('disc')  -> ques_fwd, hist, img_feat, answer_in/out, answer_ind, options
@@ -601,13 +606,23 @@ int vd_corpus_destroy(vd_corpus* c);
  * `out` receives DEVICE pointers (on_device = 1) into corpus-owned buffers that stay valid until the second-next
  * vd_corpus_get_batch on this corpus (two buffer sets, alternating). */
 int vd_corpus_get_batch(vd_corpus* c, const int64_t* inds, int32_t n, int32_t decoder_gen, vd_batch* out);
+/* Start copying the image rows of dialogs `inds` (HOST array of n 0-based indices) from a host-placed corpus's pinned
+ * features into a landing buffer outside the two buffer sets, on the corpus's copy stream, behind the work already on the
+ * engine's stream; returns without waiting.  The next vd_corpus_get_batch takes those rows when it is given the same n
+ * indices in the same order, and copies its rows itself otherwise; either way it ends the prefetch.  Batches keep their
+ * lifetime (until the second-next vd_corpus_get_batch).  Does nothing on a corpus whose features are on the device.
+ * VD_E_SHAPE for n < 1 or an index out of range. */
+int vd_corpus_prefetch(vd_corpus* c, const int64_t* inds, int32_t n);
+/* Where the prepared image features are: *on_host = 1 in pinned host memory, 0 on the device; *bytes = their size
+ * (0 without images).  Either pointer may be NULL. */
+int vd_corpus_image_memory(vd_corpus* c, int32_t* on_host, int64_t* bytes);
 /* Read one PREPARED tensor back to the host (parity tests): name in {"ques_fwd","hist","hist_len","ans_in","ans_out",
  * "opt_in","opt_out","img_fv"}, or "opt_list": the raw (numOptList, maxAnsLen) answer pool as uploaded, which the host no
  * longer keeps (the pool vd_answer_pool_encode takes); *elems receives the element count (call with host_dst = NULL to size). */
 int vd_corpus_read(vd_corpus* c, const char* name, void* host_dst, int64_t* elems);
 /* Region corpora (imgAtt = 2): counts_host (numImages) = 'num_boxes_<split>', each image's region count in [1, P].  Checks
  * every count (VD_E_BADARG, corpus unchanged, if one is outside), uploads them and zeroes every pad row (rows >= count) of
- * the resident features.  Later batches carry img_count[b] = counts[img_pos[inds[b]]], gathered on the device.  Without
+ * the resident features (on the host for a host-placed corpus, with the same +0.0f values).  Later batches carry img_count[b] = counts[img_pos[inds[b]]], gathered on the device.  Without
  * this call every region is present.  Once per corpus: the pad rows are zeroed in place, so a second call is VD_E_STATE,
  * as is a corpus without region features. */
 int vd_corpus_region_counts(vd_corpus* c, const int32_t* counts_host, int64_t numImages);

@@ -136,6 +136,8 @@ typedef struct vd_corpus_desc {
 int vd_corpus_create(vd_engine* e, const vd_corpus_desc* d, vd_corpus** out);
 int vd_corpus_destroy(vd_corpus* c);
 int vd_corpus_get_batch(vd_corpus* c, const int64_t* inds, int32_t n, int32_t decoder_gen, vd_batch* out);
+int vd_corpus_prefetch(vd_corpus* c, const int64_t* inds, int32_t n);
+int vd_corpus_image_memory(vd_corpus* c, int32_t* on_host, int64_t* bytes);
 ]]
 
 local M = {}

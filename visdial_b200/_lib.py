@@ -189,11 +189,14 @@ SIGNATURES = {
     "vd_profiler_range": [_H, C.c_int32],
     "vd_flush_l2": [_H],
     "vd_corpus_create": [_H, _P(vd_corpus_desc), _P(C.c_void_p)],
+    "vd_corpus_create_limited": [_H, _P(vd_corpus_desc), C.c_int64, _P(C.c_void_p)],
     "vd_corpus_destroy": [C.c_void_p],
     "vd_corpus_get_batch": [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, _P(vd_batch)],
     "vd_corpus_read": [C.c_void_p, C.c_char_p, C.c_void_p, _P(C.c_int64)],
     "vd_corpus_batch_bytes": [C.c_void_p, _P(C.c_int64), _P(C.c_int32)],
     "vd_corpus_region_counts": [C.c_void_p, C.c_void_p, C.c_int64],
+    "vd_corpus_prefetch": [C.c_void_p, C.c_void_p, C.c_int32],
+    "vd_corpus_image_memory": [C.c_void_p, _P(C.c_int32), _P(C.c_int64)],
 }
 
 _lib = None

@@ -365,6 +365,22 @@ def set_image_regions(mp: dict, opt: dict, subsets):
     return mp
 
 
+def host_memory_problem(opt: dict, subsets, world: int, gpuid: int):
+    """Why the image features this run keeps in pinned host memory (dataloader.image_placement; one copy per rank) would
+    not fit in the host's physical memory, or None.  Reads the features file's headers only."""
+    from .dataloader import device_memory, host_memory, image_placement, split_image_bytes
+    if not opt.get("useIm") or not subsets:
+        return None
+    sizes = split_image_bytes(opt["inputImg"], subsets)
+    place = image_placement(sizes, int(opt.get("batchSize", 40)), device_memory(gpuid))
+    pinned = sum(b for b, (on_host, _) in zip(sizes, place) if on_host)
+    if pinned == 0 or world * pinned <= host_memory():
+        return None
+    return ("the image features of %s do not fit on the GPU and take %.1f GB of pinned host memory per GPU: %d GPUs "
+            "need %.1f GB, more than the host's %.1f GB" % (opt["inputImg"], pinned / 1e9, world, world * pinned / 1e9,
+                                                            host_memory() / 1e9))
+
+
 def build(mp: dict, opt: dict, rank: int, world: int, subsets, ck=None):
     """Model on GPU gpuid + rank in the requested math mode (with the checkpoint's weights and learning rate when `ck` is
     given), and its device dataloader over `subsets` read from opt's files.  Returns (model, dataloader)."""
@@ -374,6 +390,9 @@ def build(mp: dict, opt: dict, rank: int, world: int, subsets, ck=None):
     from .model import Model
     mp = dict(mp, gpuid=opt["gpuid"] + rank)
     set_image_regions(mp, opt, subsets)
+    problem = host_memory_problem(opt, subsets, world, mp["gpuid"])
+    if problem:
+        usage_error(os.path.basename(sys.argv[0]), problem)
     model = Model(mp, seed=SEED)
     model.engine.set_math_mode({"fp32": VD_MATH_FP32, "tf32": VD_MATH_TF32, "f16": VD_MATH_F16}[opt["math"]])
     if opt.get("deterministic", 0):

@@ -9,12 +9,14 @@ void comm_unique_id(void* out);
 void comm_init(Engine* e, const void* idbytes, int rank, int world);
 void comm_destroy(Engine* e);
 struct Corpus;
-Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d);
+Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d, int64_t img_device_bytes);
 void corpus_destroy(Corpus* c);
 void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd_batch* out);
 void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems);
 void corpus_batch_bytes(Corpus* c, int64_t* bytes, int32_t* launches);
 void corpus_region_counts(Corpus* c, const int32_t* counts_host, int64_t numImages);
+void corpus_prefetch(Corpus* c, const int64_t* inds, int n);
+void corpus_image_memory(Corpus* c, int32_t* on_host, int64_t* bytes);
 void test_kernel(Engine* e, const char* name, void* const* ptrs, int n_ptrs, const int64_t* ints, int n_ints, const double* reals,
                  int n_reals);
 }  // namespace vd
@@ -765,14 +767,18 @@ int vd_flush_l2(vd_engine* h) {
 struct vd_corpus { vd::Corpus* c; };
 #define CORP(h) ((h) ? (h)->c : (throw vd::CudaError(VD_E_BADARG, "corpus handle is null"), (vd::Corpus*)nullptr))
 
-int vd_corpus_create(vd_engine* h, const vd_corpus_desc* d, vd_corpus** out) {
+int vd_corpus_create_limited(vd_engine* h, const vd_corpus_desc* d, int64_t imgDeviceBytes, vd_corpus** out) {
   VD_TRY({
     NOTNULL(out);
+    VD_REQUIRE(imgDeviceBytes >= 0, VD_E_BADARG, "imgDeviceBytes must be >= 0 (0 = no limit)");
     Engine* e = ENG(h);
     VD_CUDA_CHECK(cudaSetDevice(e->cfg.gpuid));
-    vd::Corpus* c = vd::corpus_create(e, d);
+    vd::Corpus* c = vd::corpus_create(e, d, imgDeviceBytes);
     *out = new vd_corpus{c};
   })
+}
+int vd_corpus_create(vd_engine* h, const vd_corpus_desc* d, vd_corpus** out) {
+  return vd_corpus_create_limited(h, d, 0, out);
 }
 int vd_corpus_destroy(vd_corpus* h) {
   VD_TRY({
@@ -781,6 +787,12 @@ int vd_corpus_destroy(vd_corpus* h) {
 }
 int vd_corpus_get_batch(vd_corpus* h, const int64_t* inds, int32_t n, int32_t decoder_gen, vd_batch* out) {
   VD_TRY({ vd::corpus_get_batch(CORP(h), inds, n, decoder_gen, out); })
+}
+int vd_corpus_prefetch(vd_corpus* h, const int64_t* inds, int32_t n) {
+  VD_TRY({ vd::corpus_prefetch(CORP(h), inds, n); })
+}
+int vd_corpus_image_memory(vd_corpus* h, int32_t* on_host, int64_t* bytes) {
+  VD_TRY({ vd::corpus_image_memory(CORP(h), on_host, bytes); })
 }
 int vd_corpus_read(vd_corpus* h, const char* name, void* host_dst, int64_t* elems) {
   VD_TRY({ vd::corpus_read(CORP(h), name, host_dst, elems); })

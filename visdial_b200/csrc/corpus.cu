@@ -233,6 +233,15 @@ struct Corpus {
   int32_t *ques_fwd = nullptr, *hist = nullptr, *hist_len = nullptr, *ans_in = nullptr, *ans_out = nullptr,
           *opt_in = nullptr, *opt_out = nullptr, *opt_maxlen = nullptr;
   float* img_fv = nullptr;
+  // host placement (DESIGN §29): the prepared features in one pinned allocation instead of img_fv; each batch's rows are
+  // copied from it by the copy engines on copy_stream, ordered against the engine stream by events.  A prefetch lands in
+  // `landing`, outside the two-slot ring, and the get-batch it was made for swaps that buffer into its slot.
+  float* img_host = nullptr;
+  std::vector<int32_t> h_img_pos, h_counts;
+  cudaStream_t copy_stream = nullptr;
+  cudaEvent_t ev_main = nullptr, ev_copied = nullptr, ev_prefetched = nullptr;
+  GrowBuf landing;
+  std::vector<int64_t> pf_inds; bool pf_live = false;
   // host metadata: the lengths getIndexData / getIndexOption take maxima over (:380-381,:388-389,:401-402,:443-444)
   std::vector<int32_t> h_ques_len, h_hist_len, h_ans_len1, h_opt_maxlen;
   std::vector<void*> owned;
@@ -256,7 +265,12 @@ struct Corpus {
   }
   ~Corpus() {
     cudaSetDevice(gpuid);
+    if (copy_stream) cudaStreamSynchronize(copy_stream);
     for (void* p : owned) cudaFree(p);
+    landing.release();
+    if (img_host) cudaFreeHost(img_host);
+    for (cudaEvent_t e : {ev_main, ev_copied, ev_prefetched}) if (e) cudaEventDestroy(e);
+    if (copy_stream) cudaStreamDestroy(copy_stream);
     for (int s = 0; s < 2; ++s) {
       OutSet& o = out[s];
       GrowBuf* bs[] = {&o.ques, &o.hist, &o.ans_in, &o.ans_out, &o.ans_ind, &o.options, &o.opt_in, &o.opt_out, &o.img, &o.ind,
@@ -277,7 +291,7 @@ static void check_lengths(const int32_t* len, int64_t cnt, int lo, int hi, const
     }
 }
 
-Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d) {
+Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d, int64_t img_device_bytes) {
   VD_REQUIRE(d != nullptr, VD_E_BADARG, "corpus descriptor is null");
   VD_REQUIRE(d->numThreads > 0 && d->numRounds > 0 && d->maxQuesLen > 0 && d->maxAnsLen > 0, VD_E_SHAPE, "corpus sizes");
   VD_REQUIRE(d->ques && d->ques_len && d->ans && d->ans_len, VD_E_BADARG, "ques / ans arrays missing");
@@ -379,31 +393,63 @@ Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d) {
     VD_REQUIRE(c->img_elems % 4 == 0, VD_E_SHAPE, "image feature row must be a multiple of 4 floats");
     const int64_t want = eng->cfg.att ? (int64_t)eng->cfg.P * eng->cfg.F : (int64_t)eng->cfg.F;
     VD_REQUIRE(!eng->cfg.useIm || c->img_elems == want, VD_E_SHAPE, "image feature size != params");
-    c->img_fv = c->dalloc<float>((int64_t)c->nimg * c->img_elems);
-    if (d->imgAtt != 1) {                       // fc7 rows, or region rows (N, P, C) as stored
+    const int64_t img_bytes = (int64_t)c->nimg * c->img_elems * 4;
+    const bool host = img_device_bytes > 0 && img_bytes > img_device_bytes;
+    if (host) {
+      if (cudaHostAlloc((void**)&c->img_host, (size_t)img_bytes, cudaHostAllocDefault) != cudaSuccess) {
+        (void)cudaGetLastError();
+        c->img_host = nullptr;
+        char buf[256];
+        snprintf(buf, sizeof(buf), "cannot pin %.2f GB of host memory for the image features of a split larger than "
+                 "imgDeviceBytes (%.2f GB)", img_bytes / 1e9, img_device_bytes / 1e9);
+        throw CudaError(VD_E_OOM, buf);
+      }
+      c->h_img_pos.assign(d->img_pos, d->img_pos + n);
+      VD_CUDA_CHECK(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
+      for (cudaEvent_t* e : {&c->ev_main, &c->ev_copied, &c->ev_prefetched})
+        VD_CUDA_CHECK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    } else {
+      c->img_fv = c->dalloc<float>((int64_t)c->nimg * c->img_elems);
+    }
+    if (!host && d->imgAtt != 1) {              // fc7 rows, or region rows (N, P, C) as stored
       VD_CUDA_CHECK(cudaMemcpyAsync(c->img_fv, d->images, (size_t)c->nimg * c->img_elems * 4, cudaMemcpyHostToDevice, st));
       if (d->imgNorm) { k_img_norm_rows<<<c->nimg, 256, 0, st>>>(c->img_fv, C); check_launch(cx, "k_img_norm_rows"); }
     } else {
-      // staged in chunks of <= 256 MB so a 33 GB feature file never needs a second full-size device buffer
+      // staged in chunks of <= 256 MB so a 33 GB feature file never needs a second full-size device buffer.  A host-placed
+      // split runs the device path's kernels on each chunk (they work row by row, so chunking changes no bit) and copies
+      // the prepared chunk back into the pinned array.
       const int chunk = (int)std::max<int64_t>(1, std::min<int64_t>(c->nimg, (256ll << 20) / (c->img_elems * 4)));
-      float* stage = nullptr; float* nm = nullptr;
+      float* stage = nullptr; float* nm = nullptr; float* nhwc = nullptr;
       VD_CUDA_CHECK(cudaMalloc(&stage, (size_t)chunk * c->img_elems * 4));
-      if (d->imgNorm) VD_CUDA_CHECK(cudaMalloc(&nm, (size_t)chunk * P * 4));
+      if (d->imgAtt == 1 && d->imgNorm) VD_CUDA_CHECK(cudaMalloc(&nm, (size_t)chunk * P * 4));
+      if (d->imgAtt == 1 && host) VD_CUDA_CHECK(cudaMalloc(&nhwc, (size_t)chunk * c->img_elems * 4));
       for (int i0 = 0; i0 < c->nimg; i0 += chunk) {
         const int cnt = std::min(chunk, c->nimg - i0);
         VD_CUDA_CHECK(cudaMemcpyAsync(stage, d->images + (int64_t)i0 * c->img_elems, (size_t)cnt * c->img_elems * 4,
                                       cudaMemcpyHostToDevice, st));
-        if (d->imgNorm) {
-          k_img_norm_pos<<<dim3(cdiv(P, 128), cnt), 128, 0, st>>>(stage, nm, C, P);
-          check_launch(cx, "k_img_norm_pos");
+        const float* prepared = stage;
+        if (d->imgAtt == 1) {
+          if (d->imgNorm) {
+            k_img_norm_pos<<<dim3(cdiv(P, 128), cnt), 128, 0, st>>>(stage, nm, C, P);
+            check_launch(cx, "k_img_norm_pos");
+          }
+          float* dst = host ? nhwc : c->img_fv + (int64_t)i0 * c->img_elems;
+          k_img_nchw_to_nhwc<<<dim3(cdiv(P, 32), cdiv(C, 32), cnt), dim3(32, 8), 0, st>>>(
+              stage, d->imgNorm ? nm : nullptr, dst, C, P);
+          check_launch(cx, "k_img_nchw_to_nhwc");
+          prepared = dst;
+        } else if (d->imgNorm) {
+          k_img_norm_rows<<<cnt, 256, 0, st>>>(stage, C);
+          check_launch(cx, "k_img_norm_rows");
         }
-        k_img_nchw_to_nhwc<<<dim3(cdiv(P, 32), cdiv(C, 32), cnt), dim3(32, 8), 0, st>>>(
-            stage, d->imgNorm ? nm : nullptr, c->img_fv + (int64_t)i0 * c->img_elems, C, P);
-        check_launch(cx, "k_img_nchw_to_nhwc");
+        if (host)
+          VD_CUDA_CHECK(cudaMemcpyAsync(c->img_host + (int64_t)i0 * c->img_elems, prepared, (size_t)cnt * c->img_elems * 4,
+                                        cudaMemcpyDeviceToHost, st));
       }
       VD_CUDA_CHECK(cudaStreamSynchronize(st));
       cudaFree(stage);
       if (nm) cudaFree(nm);
+      if (nhwc) cudaFree(nhwc);
     }
   }
   VD_CUDA_CHECK(cudaStreamSynchronize(st));
@@ -412,6 +458,35 @@ Corpus* corpus_create(Engine* eng, const vd_corpus_desc* d) {
 }
 
 void corpus_destroy(Corpus* c) { delete c; }
+
+// dst[b] = img_host[img_pos[inds[b]]] on the copy stream, by the copy engines: one H2D copy per run of consecutive source
+// rows, issued behind everything already on the engine stream (the readers of dst's previous batch).  No SM takes part:
+// the persistent encoder-pair and option-LSTM kernels of the step it overlaps count on their CTAs being co-resident.
+static void copy_img_rows(Corpus* c, const int64_t* inds, int n, float* dst) {
+  VD_CUDA_CHECK(cudaEventRecord(c->ev_main, c->eng->main_stream));
+  VD_CUDA_CHECK(cudaStreamWaitEvent(c->copy_stream, c->ev_main, 0));
+  const size_t row = (size_t)c->img_elems * 4;
+  for (int b = 0; b < n;) {
+    const int64_t p0 = c->h_img_pos[inds[b]];
+    int e = b + 1;
+    while (e < n && c->h_img_pos[inds[e]] == p0 + (e - b)) ++e;
+    VD_CUDA_CHECK(cudaMemcpyAsync((char*)dst + (size_t)b * row, (const char*)c->img_host + (size_t)p0 * row,
+                                  (size_t)(e - b) * row, cudaMemcpyHostToDevice, c->copy_stream));
+    b = e;
+  }
+}
+
+void corpus_prefetch(Corpus* c, const int64_t* inds, int n) {
+  VD_REQUIRE(inds != nullptr, VD_E_BADARG, "inds is null");
+  VD_REQUIRE(n > 0, VD_E_SHAPE, "a prefetch must hold at least one dialog");
+  for (int b = 0; b < n; ++b) VD_REQUIRE(inds[b] >= 0 && inds[b] < c->n, VD_E_SHAPE, "dialog index out of range");
+  if (!c->img_host) return;
+  VD_CUDA_CHECK(cudaSetDevice(c->gpuid));
+  copy_img_rows(c, inds, n, (float*)c->landing.ensure((size_t)n * c->img_elems * 4));
+  VD_CUDA_CHECK(cudaEventRecord(c->ev_prefetched, c->copy_stream));
+  c->pf_inds.assign(inds, inds + n);
+  c->pf_live = true;
+}
 
 void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd_batch* out) {
   VD_REQUIRE(inds != nullptr && out != nullptr, VD_E_BADARG, "inds / out is null");
@@ -443,16 +518,25 @@ void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd
   if (decoder_gen == 0) To = La;                                                   // raw opt_list rows, never trimmed (:452-459)
 
   // dialog indices -> device (the only per-batch PCIe traffic)
-  if (c->h_ind_cap[s] < n) {
+  // (a host-placed region corpus stages the batch's region counts behind the indices: its counts live on the host)
+  const bool host_counts = c->img_host && c->img_count;
+  const int staged = host_counts ? 2 * n : n;
+  if (c->h_ind_cap[s] < staged) {
     if (c->h_ind[s]) { VD_CUDA_CHECK(cudaEventSynchronize(c->ind_free[s])); cudaFreeHost(c->h_ind[s]); c->h_ind[s] = nullptr; }
-    VD_CUDA_CHECK(cudaMallocHost(&c->h_ind[s], (size_t)n * 4));
-    c->h_ind_cap[s] = n;
+    VD_CUDA_CHECK(cudaMallocHost(&c->h_ind[s], (size_t)staged * 4));
+    c->h_ind_cap[s] = staged;
   } else {
     VD_CUDA_CHECK(cudaEventSynchronize(c->ind_free[s]));                           // previous copy out of this slot is done
   }
   for (int b = 0; b < n; ++b) c->h_ind[s][b] = (int32_t)inds[b];
   int32_t* ind = (int32_t*)o.ind.ensure((size_t)n * 4);
   VD_CUDA_CHECK(cudaMemcpyAsync(ind, c->h_ind[s], (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  int32_t* host_cnt = nullptr;
+  if (host_counts) {
+    for (int b = 0; b < n; ++b) c->h_ind[s][n + b] = c->h_counts[c->h_img_pos[inds[b]]];
+    host_cnt = (int32_t*)o.cnt.ensure((size_t)n * 4);
+    VD_CUDA_CHECK(cudaMemcpyAsync(host_cnt, c->h_ind[s] + n, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  }
   VD_CUDA_CHECK(cudaEventRecord(c->ind_free[s], st));
 
   GatherJobs jobs; jobs.n = 0;
@@ -489,7 +573,21 @@ void corpus_get_batch(Corpus* c, const int64_t* inds, int n, int decoder_gen, vd
     k_gather_tokens<<<dim3(std::max(gx, 1), jobs.n), 256, 0, st>>>(jobs, ind);
     check_launch(cx, "k_gather_tokens");
     ++launches;
-    if (c->useIm) {
+    if (c->useIm && c->img_host) {
+      const bool hit = c->pf_live && c->pf_inds.size() == (size_t)n && std::equal(inds, inds + n, c->pf_inds.begin());
+      c->pf_live = false;
+      if (hit) {                                 // the prefetched rows become this slot's image buffer
+        std::swap(o.img, c->landing);
+        VD_CUDA_CHECK(cudaStreamWaitEvent(st, c->ev_prefetched, 0));
+      } else {
+        copy_img_rows(c, inds, n, (float*)o.img.ensure((size_t)n * c->img_elems * 4));
+        VD_CUDA_CHECK(cudaEventRecord(c->ev_copied, c->copy_stream));
+        VD_CUDA_CHECK(cudaStreamWaitEvent(st, c->ev_copied, 0));
+      }
+      out->img_feat = (float*)o.img.p;
+      out->img_count = host_cnt;
+      bytes += (int64_t)n * c->img_elems * 4 + (host_cnt ? (int64_t)n * 4 : 0);
+    } else if (c->useIm) {
       float* img = (float*)o.img.ensure((size_t)n * c->img_elems * 4);
       const int64_t e4 = c->img_elems / 4;
       int32_t* cnt = c->img_count ? (int32_t*)o.cnt.ensure((size_t)n * 4) : nullptr;
@@ -521,6 +619,11 @@ void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems) {
   else if (k == "img_fv") { p = c->img_fv; cnt = (int64_t)c->nimg * c->img_elems; }
   else if (k == "opt_list") { p = c->opt_list; cnt = (int64_t)c->m * c->La; }       // the split's answer pool (DESIGN §18)
   else VD_REQUIRE(false, VD_E_BADARG, "unknown prepared tensor name");
+  if (k == "img_fv" && c->img_host) {
+    *elems = cnt;
+    if (host_dst) memcpy(host_dst, c->img_host, (size_t)cnt * 4);
+    return;
+  }
   VD_REQUIRE(p != nullptr, VD_E_STATE, "this corpus does not hold that tensor (useHistory / useIm off)");
   *elems = cnt;
   if (host_dst) {
@@ -531,7 +634,7 @@ void corpus_read(Corpus* c, const char* name, void* host_dst, int64_t* elems) {
 }
 
 void corpus_region_counts(Corpus* c, const int32_t* counts_host, int64_t numImages) {
-  VD_REQUIRE(c->regions > 0 && c->img_fv, VD_E_STATE, "region counts need a corpus of region features (imgAtt = 2)");
+  VD_REQUIRE(c->regions > 0 && (c->img_fv || c->img_host), VD_E_STATE, "region counts need a corpus of region features (imgAtt = 2)");
   // the pad rows are zeroed in place: counts set once could not be raised later without the rows they zeroed
   VD_REQUIRE(c->img_count == nullptr, VD_E_STATE, "region counts are set once per corpus");
   VD_REQUIRE(counts_host != nullptr, VD_E_BADARG, "counts is null");
@@ -546,10 +649,24 @@ void corpus_region_counts(Corpus* c, const int32_t* counts_host, int64_t numImag
   cudaStream_t st = c->eng->main_stream;
   c->img_count = c->dalloc<int32_t>(c->nimg);
   VD_CUDA_CHECK(cudaMemcpyAsync(c->img_count, counts_host, (size_t)c->nimg * 4, cudaMemcpyHostToDevice, st));
+  if (c->img_host) {                 // +0.0f in every pad value, as k_zero_pad_regions writes on the device
+    VD_CUDA_CHECK(cudaStreamSynchronize(c->copy_stream));
+    c->h_counts.assign(counts_host, counts_host + numImages);
+    const int64_t row = c->img_elems / c->regions;
+    for (int64_t i = 0; i < numImages; ++i)
+      memset(c->img_host + i * c->img_elems + counts_host[i] * row, 0, (size_t)(c->regions - counts_host[i]) * row * 4);
+    VD_CUDA_CHECK(cudaStreamSynchronize(st));
+    return;
+  }
   const int64_t C4 = c->img_elems / c->regions / 4, total4 = (int64_t)c->nimg * c->img_elems / 4;
   k_zero_pad_regions<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>((float4*)c->img_fv, c->img_count, total4, c->regions, C4);
   check_launch(c->eng->cx, "k_zero_pad_regions");
   VD_CUDA_CHECK(cudaStreamSynchronize(st));
+}
+
+void corpus_image_memory(Corpus* c, int32_t* on_host, int64_t* bytes) {
+  if (on_host) *on_host = c->img_host != nullptr;
+  if (bytes) *bytes = (int64_t)c->nimg * c->img_elems * 4;
 }
 
 void corpus_batch_bytes(Corpus* c, int64_t* bytes, int32_t* launches) {

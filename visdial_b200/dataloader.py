@@ -13,12 +13,54 @@ There is no CPU path: without libvisdial_b200.so and a GPU every call raises.
 from __future__ import annotations
 
 import ctypes as C
+import os
+import sys
 from typing import Dict, Optional, Tuple
 
 import numpy as np
 
 from ._lib import check, vd_batch, vd_corpus_desc
 from .engine import Batch, Engine
+
+# Where a split's image features live (DESIGN §29): on the device while they fit beside the engine's working set, else in
+# pinned host memory.  The reserve is the working set of DESIGN §4 (about 15 GB at B = 32, 60 GB at B = 128: half a GiB per
+# dialog) plus a fixed 4 GiB for the context, the library's workspaces and the batch ring, and at most half the device, so
+# that features taking less than half of it never leave the device.
+RESERVE_FIXED = 4 << 30
+RESERVE_PER_DIALOG = 1 << 29
+
+
+def device_memory(gpuid: int) -> int:
+    """Total memory of GPU `gpuid` in bytes."""
+    import torch
+    return int(torch.cuda.get_device_properties(gpuid).total_memory)
+
+
+def host_memory() -> int:
+    """Physical memory of this host in bytes."""
+    return os.sysconf("SC_PAGE_SIZE") * os.sysconf("SC_PHYS_PAGES")
+
+
+def image_placement(image_bytes, batch_size: int, device_bytes: int):
+    """For each split's prepared image features (bytes, in load order), (on_host, imgDeviceBytes): the budget is
+    `device_bytes` minus min(RESERVE_FIXED + batch_size * RESERVE_PER_DIALOG, device_bytes / 2) minus the features of the
+    splits placed on the device before it; features over the budget stay in pinned host memory."""
+    budget = device_bytes - min(RESERVE_FIXED + int(batch_size) * RESERVE_PER_DIALOG, device_bytes // 2)
+    out = []
+    for b in image_bytes:
+        on_host = b > budget
+        out.append((on_host, max(budget, 1)))
+        if not on_host:
+            budget -= b
+    return out
+
+
+def split_image_bytes(path: str, subsets) -> list:
+    """The prepared feature bytes of each split of an image features file (fp32; from the datasets' headers only)."""
+    from . import h5lite
+    shapes = h5lite.shapes(path, ["images_" + s for s in subsets])
+    return [4 * int(np.prod(shapes["images_" + s], dtype=np.int64)) for s in subsets]
+
 
 _I32_KEYS = ("ques", "ques_length", "ans", "ans_length", "cap", "cap_length", "opt", "opt_list", "opt_length",
              "ans_index", "img_pos", "num_rounds")
@@ -97,7 +139,7 @@ def image_regions(path: str, dtype: str) -> Tuple[int, int]:
 class Corpus:
     """One split resident in HBM (vd_corpus handle)."""
 
-    def __init__(self, eng: Engine, raw: Dict[str, np.ndarray], opt: dict, start: int, end: int):
+    def __init__(self, eng: Engine, raw: Dict[str, np.ndarray], opt: dict, start: int, end: int, img_device_bytes: int = 0):
         self.eng = eng
         self.raw = {}
         for k in _I32_KEYS:
@@ -145,7 +187,7 @@ class Corpus:
                 setattr(d, field, a.ctypes.data)
         self.desc = d
         h = C.c_void_p()
-        check(eng.lib.vd_corpus_create(eng.h, C.byref(d), C.byref(h)))
+        check(eng.lib.vd_corpus_create_limited(eng.h, C.byref(d), int(img_device_bytes), C.byref(h)))
         self.h = h
         if region and raw.get("num_boxes") is not None:
             counts = np.ascontiguousarray(raw["num_boxes"], dtype=np.int32).reshape(-1)
@@ -154,6 +196,9 @@ class Corpus:
             except Exception:
                 eng.lib.vd_corpus_destroy(h)
                 raise
+        on_host, by = C.c_int32(), C.c_int64()
+        check(eng.lib.vd_corpus_image_memory(h, C.byref(on_host), C.byref(by)))
+        self.images_on_host, self.image_bytes = bool(on_host.value), int(by.value)
         self.numThreads = int(d.numThreads)
         self.R, self.K = int(d.numRounds), int(d.numOptions)
         self.ans_len1 = r["ans_length"].astype(np.int64) + 1                        # :196
@@ -175,6 +220,12 @@ class Corpus:
         nr = self.num_rounds[inds0].astype(np.int64) if (with_num_rounds and self.num_rounds is not None) else None
         return DeviceBatch(self.eng, b, self.R, self.K, self.img_shape, int(self.ans_len1[inds0].sum()), nr,
                            h2d_bytes=4 * len(inds0))
+
+    def prefetch(self, inds0: np.ndarray):
+        """Start copying these dialogs' image rows to the device for the get_batch that will ask for them (a no-op unless
+        the features are in host memory)."""
+        inds0 = np.ascontiguousarray(inds0, dtype=np.int64)
+        check(self.eng.lib.vd_corpus_prefetch(self.h, inds0.ctypes.data, len(inds0)))
 
     def read(self, name: str) -> np.ndarray:
         n = C.c_int64()
@@ -231,6 +282,7 @@ class Dataloader:
         self.numThreads: Dict[str, int] = {}
         self.part: Dict[str, tuple] = {}             # dtype -> (first dialog, one past the last) of this rank
         self.corpus: Dict[str, Corpus] = {}
+        self._ahead = None                           # (what, generator state before the draw, the draw) of a look-ahead
 
     def initialize(self, opt: dict, subsets, data: Dict[str, Dict[str, np.ndarray]], vocab_size_no_specials: int = None):
         """dataloader:initialize(opt, subsets), dataloader.lua:10-137.  `opt` carries encoder / useHistory /
@@ -246,9 +298,18 @@ class Dataloader:
         self.ind2word = {v: k for k, v in w2i.items()}                              # :24-29
         self.useHistory, self.concatHistory, self.useIm = bool(opt.get("useHistory")), bool(opt.get("concatHistory")), bool(opt.get("useIm"))
         self.maxHistoryLen = int(opt.get("maxHistoryLen") or 60)                    # :142
-        for dtype in subsets:
-            c = Corpus(self.eng, data[dtype], opt, self.word2ind["<START>"], self.word2ind["<END>"])
+        budgets = [0] * len(subsets)
+        if self.useIm:
+            sizes = [4 * int(np.prod(np.shape(data[s]["images"]), dtype=np.int64)) for s in subsets]
+            place = image_placement(sizes, int(opt.get("batchSize", 40)), device_memory(int(self.eng.params["gpuid"])))
+            budgets = [b for _, b in place]
+        for dtype, budget in zip(subsets, budgets):
+            c = Corpus(self.eng, data[dtype], opt, self.word2ind["<START>"], self.word2ind["<END>"], budget)
             self.corpus[dtype] = c
+            if self.useIm and self.rank == 0:
+                print("%s image features: %.2f GB in %s" % (dtype, c.image_bytes / 1e9,
+                                                            "pinned host memory" if c.images_on_host else "device memory"),
+                      file=sys.stderr, flush=True)
             self.part[dtype] = eval_partition(c.numThreads, self.rank, self.world) if dtype != "train" else (0, c.numThreads)
             self.numThreads[dtype] = self.part[dtype][1] - self.part[dtype][0]      # :94-105 (this rank's share)
             if c.num_rounds is not None:                                            # :110, read by Model.retrieve / predict
@@ -306,18 +367,45 @@ class Dataloader:
             setattr(self, "num%sThreads" % dtype.capitalize(), hi - lo)
         return self
 
+    def _draw(self, what, n: int, size: int) -> np.ndarray:
+        """self.rng.integers(0, n, size=size), drawn for `what`.  A look-ahead draw made for the same `what` is returned
+        instead; one made for anything else is undone first (the generator goes back to its state before it), so that a
+        run draws exactly what it draws without look-ahead, whatever it mixes."""
+        ahead, self._ahead = self._ahead, None
+        if ahead is not None and ahead[0] == what:
+            return ahead[2]
+        if ahead is not None:
+            self.rng.bit_generator.state = ahead[1]
+        return self.rng.integers(0, n, size=size)
+
+    def _draw_ahead(self, what, n: int, size: int, prefetch):
+        """Make the next draw for `what` now and hand it to `prefetch`, keeping the generator's state from before it."""
+        state = self.rng.bit_generator.state
+        nxt = self.rng.integers(0, n, size=size)
+        self._ahead = (what, state, nxt)
+        prefetch(nxt)
+
     def getTrainBatch(self, params: dict, batchSize: int = None) -> DeviceBatch:
         size = int(batchSize or params["batchSize"])                                # :325
-        inds = self.rng.integers(0, self.numThreads["train"], size=size)            # :326 (uniform with replacement)
-        return self.corpus["train"].get_batch(inds, 0 if params["decoder"] == "disc" else 1)   # :329-337
+        c = self.corpus["train"]
+        inds = self._draw(("train", size), self.numThreads["train"], size)         # :326 (uniform with replacement)
+        batch = c.get_batch(inds, 0 if params["decoder"] == "disc" else 1)          # :329-337
+        if c.images_on_host:                   # draw the next batch now and copy its rows while this one trains
+            self._draw_ahead(("train", size), self.numThreads["train"], size, c.prefetch)
+        return batch
 
     def getDenseTrainBatch(self, params: dict, dense):
         """A training batch of `batchSize` annotated entries of `dense` (visdial_b200.dense.read against the train
         split), drawn uniformly with replacement with this rank's generator: a disc batch for disc models, a batch with
         option_in / option_out (getTestBatch's gen layout) for gen models.  Returns (batch, the 0-based annotated round of
         each dialog (B,), their relevance rows (B, numOptions))."""
-        pick = self.rng.integers(0, len(dense), size=int(params["batchSize"]))
-        batch = self.corpus["train"].get_batch(dense.dialog[pick], 0 if params["decoder"] == "disc" else 2)
+        size = int(params["batchSize"])
+        c = self.corpus["train"]
+        what = ("dense", id(dense), size)
+        pick = self._draw(what, len(dense), size)
+        batch = c.get_batch(dense.dialog[pick], 0 if params["decoder"] == "disc" else 2)
+        if c.images_on_host:
+            self._draw_ahead(what, len(dense), size, lambda nxt: c.prefetch(dense.dialog[nxt]))
         return batch, (dense.round_id[pick] - 1).astype(np.int32), dense.relevance[pick]
 
     def getIndexData(self, inds0, params: dict, dtype: str) -> DeviceBatch:
@@ -333,9 +421,14 @@ class Dataloader:
 
     def getTestBatch(self, startId: int, params: dict, dtype: str = "val"):
         """`startId` is 0-based here (Lua's startId - 1); returns (batch, nextStartId) like :344-375."""
-        inds, nxt = test_batch_indices(startId, int(params["batchSize"]), *self.part[dtype])   # :347-357
+        B = int(params["batchSize"])
+        inds, nxt = test_batch_indices(startId, B, *self.part[dtype])               # :347-357
         mode = 0 if params["decoder"] == "disc" else 2                              # :362-371
-        return self.corpus[dtype].get_batch(inds, mode, with_num_rounds=True), nxt
+        c = self.corpus[dtype]
+        batch = c.get_batch(inds, mode, with_num_rounds=True)
+        if c.images_on_host and nxt < self.numThreads[dtype]:                       # the next batch's rows, while this one runs
+            c.prefetch(test_batch_indices(nxt, B, *self.part[dtype])[0])
+        return batch, nxt
 
     def close(self):
         for c in self.corpus.values():
